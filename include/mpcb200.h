@@ -1,5 +1,5 @@
 /*
- * mpcb200.h - C ABI of the B200-native batched box-constrained LQR step.
+ * mpcb200.h - C ABI of the H100-native batched box-constrained LQR step.
  *
  * This is the drop-in boundary for ONE path of locuslab/mpc.pytorch: the body of
  * LQRStepFn.forward / LQRStepFn.backward (reference mpc/lqr_step.py:277-309 and
@@ -39,7 +39,7 @@ enum {
   MPCB200_ERR_UNSUPPORTED_DIMS = 3,  /* (n,m) has no compiled kernel instance               */
   MPCB200_ERR_SMEM = 4,              /* problem does not fit shared memory and no workspace */
   MPCB200_ERR_LAUNCH = 5,            /* cudaGetLastError() after launch != cudaSuccess      */
-  MPCB200_ERR_NO_DEVICE = 6          /* no usable sm_100 device / wrong architecture        */
+  MPCB200_ERR_NO_DEVICE = 6          /* no usable sm_90 device / wrong architecture         */
 };
 
 /* Problem sizes and options.  Mirrors the closure arguments of

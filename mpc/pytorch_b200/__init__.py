@@ -1,4 +1,4 @@
-"""mpc.pytorch_b200 - B200-native (sm_100a) batched box-constrained LQR step.
+"""mpc.pytorch_b200 - H100-native (sm_90a) batched box-constrained LQR step.
 
 Host-side mirror of the reference's operator interface for ONE path
 (LQRStep / MPC with QuadCost + LinDx, reference mpc/lqr_step.py, mpc/mpc.py),

@@ -64,7 +64,7 @@ static int max_smem_optin() {
     int v = 0, major = 0;
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) return -1;
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return -1;
-    if (major != 10) return -1;   // sm_100a cubin only
+    if (major != 9) return -1;    // sm_90a cubin only
     cache[dev].store(v, std::memory_order_release);
   }
   return cache[dev].load(std::memory_order_acquire);
@@ -466,7 +466,7 @@ int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size) 
   const Entry* e = find(dims->n, dims->m);
   if (e == nullptr) return 0;
   int ms = max_smem_optin();
-  if (ms <= 0) ms = 227 * 1024;       // no device visible (CPU-side query): assume B200's opt-in limit
+  if (ms <= 0) ms = 227 * 1024;       // no device visible (CPU-side query): assume H100's opt-in limit
   return elem_size == 8 ? e->pws64(dims->T, ms) : e->pws32(dims->T, ms);
 }
 
@@ -480,7 +480,7 @@ const char* mpcb200_strerror(int code) {
     case MPCB200_ERR_UNSUPPORTED_DIMS: return "no kernel instance compiled for this (n_state, n_ctrl)";
     case MPCB200_ERR_SMEM: return "problem does not fit shared memory (pass Ks/ks buffers for long horizons)";
     case MPCB200_ERR_LAUNCH: return "CUDA launch failed";
-    case MPCB200_ERR_NO_DEVICE: return "no usable sm_100 device";
+    case MPCB200_ERR_NO_DEVICE: return "no usable sm_90 device";
     default: return "unknown error";
   }
 }

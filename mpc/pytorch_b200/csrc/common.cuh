@@ -1,5 +1,5 @@
 // common.cuh - PTX helpers (mbarrier, 1-D bulk TMA) and tiny per-lane linear algebra.
-// sm_100a only.  No reference code: the algorithms these serve are cited in lqr_step.cuh.
+// sm_90a only.  No reference code: the algorithms these serve are cited in lqr_step.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -48,7 +48,7 @@ MPCB_DEV bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t ns) {
   return ok != 0;
 }
 // non-blocking probe (mbarrier.test_wait).  Probing the NEXT stage at the end of a step (to take the
-// try_wait latency off the per-step path) was measured: 38.8 us vs 38.1 us at config 3 - not used.
+// try_wait latency off the per-step path) gained nothing at config 3 - not used.
 MPCB_DEV bool mbar_test(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -62,7 +62,7 @@ MPCB_DEV bool mbar_test(uint64_t* bar, uint32_t parity) {
 }
 MPCB_DEV void mbar_wait(uint64_t* bar, uint32_t parity) {
   // plain try_wait blocks in hardware for a bounded time; the suspend-hint form compiles to a
-  // NANOSLEEP polling loop (measured) whose wake-up granularity hurts a latency-bound consumer
+  // NANOSLEEP polling loop whose wake-up granularity hurts a latency-bound consumer
   while (!mbar_try_wait(bar, parity)) {
   }
 }
@@ -136,34 +136,18 @@ MPCB_DEV void load_vec(const R* p, R (&out)[CNT]) {
 template <typename R>
 MPCB_DEV R shfl(R v, int src) { return __shfl_sync(0xffffffffu, v, src); }
 
-// ------------------------------------------------------------------ packed pairs (FFMA2 on sm_100)
-// Blackwell issues two fp32 FMAs per lane with one instruction (PTX fma.rn.f32x2, SASS FFMA2,
-// including a scalar-broadcast operand form).  Every lane-op is still an IEEE fma, so results are
-// those of scalar fmaf; the issue-slot count of the small dense products halves.
+// ------------------------------------------------------------------ pairs
+// Two independent lanes of arithmetic.  Hopper has no packed fp32 FMA, so a pair is two scalar FFMAs;
+// the pair layout still matters: every operand a lane loads from shared memory feeds both of them.
+// fmaf / __fmul_rn keep each lane-op a single IEEE-rounded operation (no contraction across ops).
 template <typename R>
 struct P2 {
   R x, y;
 };
-MPCB_DEV unsigned long long pack2(float x, float y) {
-  unsigned long long u;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(u) : "f"(x), "f"(y));
-  return u;
-}
-MPCB_DEV P2<float> unpack2(unsigned long long u) {
-  P2<float> r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(u));
-  return r;
-}
 MPCB_DEV P2<float> fma2(P2<float> a, P2<float> b, P2<float> c) {   // a*b + c
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(pack2(a.x, a.y)), "l"(pack2(b.x, b.y)), "l"(pack2(c.x, c.y)));
-  return unpack2(d);
+  return {fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)};
 }
-MPCB_DEV P2<float> mul2(P2<float> a, P2<float> b) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pack2(a.x, a.y)), "l"(pack2(b.x, b.y)));
-  return unpack2(d);
-}
+MPCB_DEV P2<float> mul2(P2<float> a, P2<float> b) { return {__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
 MPCB_DEV P2<double> fma2(P2<double> a, P2<double> b, P2<double> c) {
   return {a.x * b.x + c.x, a.y * b.y + c.y};
 }

@@ -1,4 +1,4 @@
-// lqr_grad.cuh - gradient assembly of the KKT adjoint (sm_100a).
+// lqr_grad.cuh - gradient assembly of the KKT adjoint (sm_90a).
 //
 // Replaces the second half of LQRStepFn.backward (reference mpc/lqr_step.py:342-404):
 // costates lambda_t / dlambda_t (backward in t), then

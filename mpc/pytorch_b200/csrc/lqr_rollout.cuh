@@ -1,4 +1,4 @@
-// lqr_rollout.cuh - nominal trajectory x[t+1] = F[t] [x[t]; u[t]] + f[t] for LinDx dynamics (sm_100a).
+// lqr_rollout.cuh - nominal trajectory x[t+1] = F[t] [x[t]; u[t]] + f[t] for LinDx dynamics (sm_90a).
 //
 // Replaces util.get_traj for LinDx (reference mpc/util.py:102-126: T-1 bmm/cat/add launches per iLQR
 // iteration) with ONE launch.  N lanes per problem (lane r owns state component r and row r of F),

@@ -1,15 +1,15 @@
-// lqr_step.cuh - one box-constrained LQR step as ONE persistent-per-CTA kernel (sm_100a).
+// lqr_step.cuh - one box-constrained LQR step as ONE persistent-per-CTA kernel (sm_90a).
 //
 // Replaces the body of LQRStepFn.forward (reference mpc/lqr_step.py:277-309):
 //   c_back (:289-295), lqr_backward (:52-160) with pnqp (mpc/pnqp.py:5-82) or the
 //   u_zero_I masked solve (:100-127), and lqr_forward's rollout + line search (:164-261).
 //
-// Mapping (designed for B200, not translated from the reference's per-op loop):
+// Mapping (designed for the GPU, not translated from the reference's per-op loop):
 //  * P = n+m lanes own one problem; lane j owns COLUMN j of every p-wide matrix of that
 //    problem (Q_t, F_t, C_t) and, for j < n, column j of the value matrix V and of K_t.
 //    32/P problems share a warp; NW consumer warps (the smallest count whose spans stay 16-byte
 //    aligned: small CTAs = fine load-balance granularity, the batch is < 1 wave) + 1 producer warp
-//    form a CTA.  The dense products use packed FFMA2 (two fp32 FMAs per lane per instruction).
+//    form a CTA.  The dense products run as pairs of independent FMA chains (common.cuh P2).
 //  * the producer warp streams the per-time-step tiles C[t],F[t],c[t],f[t],x_bar[t],u_bar[t]
 //    (+ tensor bounds) of the CTA's W consecutive problems - contiguous in the reference's
 //    time-major layout - into a 3-stage shared-memory ring with 1-D bulk TMA
@@ -27,7 +27,7 @@
 // This is the GENERIC kernel (any n, m <= 32 lanes, unaligned spans): shapes with even n, m and 16-byte
 // aligned tensors run the column-pair kernel in lqr_step2.cuh.  The round-1 experiments that lived here as
 // compile-time knobs (two columns per lane, V in registers, padded tiles, mma.sync products, phase timers)
-// are described with their measurements in DESIGN.md section 7; their code was removed.
+// are listed in DESIGN.md section 7; their code was removed.
 #pragma once
 #include <atomic>
 #include <cstdio>

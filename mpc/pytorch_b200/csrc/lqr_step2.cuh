@@ -1,13 +1,13 @@
-// lqr_step2.cuh - the box-constrained LQR step, column-PAIR mapping with self-feeding warps (sm_100a).
+// lqr_step2.cuh - the box-constrained LQR step, column-PAIR mapping with self-feeding warps (sm_90a).
 //
 // Same contract as lqr_step.cuh (reference LQRStepFn.forward, mpc/lqr_step.py:277-309: c_back :289-295,
 // lqr_backward :52-160 incl. pnqp mpc/pnqp.py:5-82 and the u_zero_I solve :100-127, lqr_forward :164-261),
 // different machine mapping.  Why a second mapping: the round-1 kernel (one column per lane) issues one
-// shared-memory operand per FMA - 79 LSU wavefronts per problem-step at config 3 - and spends 20 % of its
-// instructions polling mbarriers between a producer warp and its consumers.  Here
+// shared-memory operand per FMA and spends part of its instructions polling mbarriers between a producer warp
+// and its consumers.  Here
 //  * L = (n+m)/2 lanes own one problem; a lane owns the column PAIR (c0, c0+1) of Q_t, F_t, C_t (x lanes also
-//    the pair of V and K_t columns).  Every value a lane loads from shared memory feeds two FMAs of ONE packed
-//    FFMA2 (pair x broadcast scalar), so operands per FMA halve and 32/L problems share a warp
+//    the pair of V and K_t columns).  Every value a lane loads from shared memory feeds two FMAs (pair x
+//    broadcast scalar), so operands per FMA halve and 32/L problems share a warp
 //    (n=8, m=2: 6 problems / warp instead of 3).
 //  * no producer warp and no empty barriers: every warp streams its OWN tiles.  After a warp has consumed
 //    stage s, up to 8 of its lanes each issue one 1-D bulk TMA copy (C, F, c, x_bar, u_bar, f, bounds) of tile
@@ -110,16 +110,15 @@ struct Step2Cfg {
   // n, m) and per-problem vectors that the lanes read straight from global memory with vector loads
   static constexpr bool OK = (N % 2 == 0) && (M % 2 == 0) && L <= 16 && N >= 2 && M >= 2 && (PPW * M * SZ) % 16 == 0 &&
                              (PPW * N * SZ) % 16 == 0 && (PPW * P * SZ) % 16 == 0;
-  // default choice between this mapping and the generic kernel, from measurements on B200 (profiles/
-  // r02_shapes_generic_vs_pair.log): the pair mapping wins where the dense products dominate (n+m >= 18:
-  // 1.5-1.8x at n=16, m=4) and for narrow problems (n+m <= 6, where 10+ problems share a warp); in between
-  // (n=8, m=2: 39 vs 37 us at config 3) the step is latency bound either way and the generic kernel stays.
+  // default choice between this mapping and the generic kernel, from tools/exp_shapes.py on an H100 SXM (400 W
+  // power limit), fp32, us per launch generic / pair: the pair mapping wins where the dense products dominate
+  // (n=16, m=4, T=50, B=4096: 935 / 653; n=8, m=4: 107 / 89) and is no slower for narrow problems (n+m <= 6);
+  // in between the generic kernel stays (n=8, m=2, B=16384: 196 / 206; n=12, m=4: 230 / 240).
   static constexpr bool PAIR_DEFAULT = OK && (P >= 18 || P <= 6 || (N == 8 && M == 4));
   // stage layout (elements): dense spans of the warp's PPW problems, in the tensors' own layouts
-  // Per-problem tiles are dense (stride p*p / n*p).  Padding them per problem to dodge the bank conflicts of the
-  // broadcast loads (n=16, m=4: F tiles 320 floats apart, 38 % of the shared wavefronts are conflicts) was
-  // measured: 449 vs 447 us at B=4096, 1504 vs 1457 us at B=16384 - the extra per-problem bulk copies cost what
-  // the conflicts did (profiles/r02_config5_padded_tiles_experiment.log); removed.
+  // Per-problem tiles are dense (stride p*p / n*p).  Padding them per problem dodges the bank conflicts of the
+  // broadcast loads (n=16, m=4: F tiles 320 floats apart) but costs one bulk copy per problem instead of one per
+  // warp span; it did not pay off in an earlier measurement and was removed.
   static constexpr int CS = P * P, FS = N * P;
   static constexpr int OFF_C = 0;
   static constexpr int OFF_F = OFF_C + PPW * CS;
@@ -132,9 +131,8 @@ struct Step2Cfg {
   static constexpr int OFF_c2 = OFF_hi + PPW * M;        // fused adjoint: the true cost's c (the c slot carries -r)
   static constexpr int OFF_END = OFF_c2 + PPW * P;
   static constexpr int STAGE_BYTES = round_up(OFF_END * SZ, 128);
-  // ring depth: 4 stages for small tiles, 3 for big ones.  Measured for n=16, m=4 (9.4 KB tiles, B=4096 / 16384,
-  // profiles/r02_config5_stages_experiment.log): 4 stages (5 warps / SM) 447 / 1457 us, 3 stages (6 warps / SM)
-  // 398 / 1399 us, 2 stages (8 warps / SM) 462 / 1422 us, 2 stages + a 200-register cap (spills) 688 / 1953 us.
+  // ring depth: 4 stages for small tiles, 3 for big ones (n=16, m=4: 9.4 KB tiles).  Fewer stages let more warps
+  // reside per SM but hide less of the copy latency; 3 was the best trade-off for the big tiles.
 #ifndef MPCB2_BIG_STAGES
 #define MPCB2_BIG_STAGES 3
 #endif
@@ -322,7 +320,7 @@ lqr_step2_kernel(const StepArgs a) {
   };
   // "done with the stage of tile g": refill it with tile g + S of the global sequence.  (A variant with a
   // dedicated producer warp per two consumer warps - the consumer only arrives on an `empty` mbarrier - was
-  // measured SLOWER: 43.1 vs 39.0 us at config 3, profiles/r02_step2_producer_variant.log; removed.)
+  // slower at config 3 and was removed.)
   auto release = [&](int g) {
     const int gn = g + S;
     if (gn < G) {

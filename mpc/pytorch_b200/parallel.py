@@ -76,7 +76,7 @@ def gpu_local_cpus(device):
 class numa_local:
     """``with numa_local(device): buf = t.pin_memory()`` - allocate (first-touch) host staging buffers while the
     thread runs on the GPU's local cores, so the pinned pages live on the socket the GPU hangs off.  A copy from
-    the far socket crosses the inter-socket link and measured 35-43 GB/s here instead of 55 GB/s."""
+    the far socket crosses the inter-socket link, which is slower than the GPU's own PCIe link."""
 
     def __init__(self, device):
         self.cpus = gpu_local_cpus(device)

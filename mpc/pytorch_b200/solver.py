@@ -1,4 +1,4 @@
-"""MPC: the outer iLQR loop around the B200 LQR step (host side, device-resident state).
+"""MPC: the outer iLQR loop around the CUDA LQR step (host side, device-resident state).
 
 Mirrors the reference module ``mpc.MPC`` (mpc/mpc.py:58-337): identical constructor
 keywords and defaults (:123-144), ``forward(x_init, cost, dx) -> (x, u, costs)`` (:184, :337),

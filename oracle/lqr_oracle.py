@@ -3,7 +3,7 @@
 This file is a from-scratch CPU restatement (torch CPU tensors, dtype generic)
 of the reference algorithm in locuslab/mpc.pytorch for ONE path:
 ``LQRStep`` = ``lqr_backward`` + ``pnqp`` + ``lqr_forward`` + KKT adjoint.
-Citations are relative to /root/reference.
+Citations are relative to the root of a locuslab/mpc.pytorch checkout.
 
 It is the *checker* for the CUDA path.  Only ``tests/``,
 ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / ``--impl
@@ -11,10 +11,10 @@ reference`` legs may import it.  Nothing under ``mpc/`` may: the product path
 fails loudly when the CUDA library is missing, it never routes here.
 
 Parity pin: ``oracle/make_golden.py`` runs the real reference (imported from
-/root/reference in the build container) and this oracle on identical seeded
+the checkout named by $MPC_REFERENCE) and this oracle on identical seeded
 inputs, asserts agreement, and stores the reference's outputs under
 ``tests/golden/``; ``tests/test_oracle_golden.py`` replays those fixtures
-anywhere (the GPU box has no /root/reference).
+anywhere, without the reference.
 
 Two pnqp semantics are provided (see SURVEY.md section 8(a) row P):
 

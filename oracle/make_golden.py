@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
-"""Generate tests/golden/*.npz from the REAL reference (build container only).
+"""Generate tests/golden/*.npz from the REAL reference.
 
-Run here (where /root/reference exists):   python oracle/make_golden.py
+Run with a checkout of locuslab/mpc.pytorch:   MPC_REFERENCE=<checkout> python oracle/make_golden.py
 It imports the unmodified reference package under the alias ``ref_mpc`` (so it
 cannot collide with this repo's drop-in ``mpc`` package), runs it on seeded
 inputs on CPU, checks that oracle/lqr_oracle.py (coupled=True) reproduces it,
-and stores inputs + the reference's outputs as small .npz fixtures.  The GPU box
-has no /root/reference; tests only ever read the fixtures.
+and stores inputs + the reference's outputs as small .npz fixtures.  Tests only
+ever read the fixtures; they never need the reference.
 
 No reference source is copied: only its numerical outputs are stored.
 """
@@ -24,12 +24,14 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 GOLD = os.path.join(ROOT, "tests", "golden")
-REF = os.environ.get("MPC_REFERENCE", "/root/reference")
+REF = os.environ.get("MPC_REFERENCE")
 sys.path.insert(0, ROOT)
 warnings.filterwarnings("ignore")
 
 
 def load_reference():
+    if not REF:
+        raise SystemExit("set MPC_REFERENCE to a checkout of locuslab/mpc.pytorch")
     spec = importlib.util.spec_from_file_location(
         "ref_mpc", os.path.join(REF, "mpc", "__init__.py"),
         submodule_search_locations=[os.path.join(REF, "mpc")])

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Fixtures for the learned / affine dynamics modules (SURVEY.md section 8(f) rank 2), from the REAL reference.
 
-Run in the build container (where /root/reference exists):   python oracle/make_golden_nn.py
+Run with a checkout of locuslab/mpc.pytorch:   MPC_REFERENCE=<checkout> python oracle/make_golden_nn.py
 Imports the unmodified reference under the alias ``ref_mpc`` (oracle/make_golden.py: load_reference), builds its
 ``NNDynamics`` / ``AffineDynamics`` (reference mpc/dynamics.py:15-131, :159-205) with seeded weights, and stores the
 weights, one batched step, the analytic Jacobians ``grad_input`` and a short box-constrained iLQR solve with

@@ -11,7 +11,7 @@ warnings.filterwarnings("ignore", category=UserWarning)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -20,7 +20,7 @@ def pytest_collection_modifyitems(config, items):
     import torch
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

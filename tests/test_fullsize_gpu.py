@@ -54,11 +54,14 @@ def _check_all(r, o, u, ul, uu, tol, bounded):
         assert torch.equal(r["new_u"] == lo, o.new_u == lo)
         assert torch.equal(r["new_u"] == hi, o.new_u == hi)
         assert bool(((r["new_u"] >= lo) & (r["new_u"] <= hi)).all())
-        # the status word flags only problems with a QP at the iteration cap (the reference prints
-        # "pnqp warning: Did not converge" for these), a vanishing fraction of the batch
+        # the status word flags only problems with a QP at the iteration cap, and only problems the reference
+        # itself leaves at the cap on the same inputs (it prints "pnqp warning: Did not converge" for them), up
+        # to the iteration counts that fp32 round-off decides differently (nbad above)
         capped = (r["qp_iters"] == 19).any(0)
         flagged = (r["status"] & 1) != 0
-        assert bool((flagged <= capped).all()) and float(flagged.float().mean()) < 1e-2
+        ref_capped = (o.qp_iters == 19).any(0)
+        assert bool((flagged <= capped).all())
+        assert int((flagged & ~ref_capped).sum()) <= nbad, (int(flagged.sum()), int(ref_capped.sum()), nbad)
     assert int((r["status"] & ~1).max()) == 0
 
 

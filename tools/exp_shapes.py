@@ -27,6 +27,6 @@ for (n, m, T, B, bounds) in CASES:
     d = max(float((outs["1"][k] - outs["2"][k]).abs().max()) for k in ("new_x", "new_u")) if len(outs) == 2 else float("nan")
     fl = bench.flops_per_solve(T, n, m) * B
     print(f"n={n} m={m} T={T} B={B} bounds={bounds}: generic {res['1']:.1f} us  pair {res['2']:.1f} us  "
-          f"(pair: {bps * B / (res['2'] * 1e-6) / 1e9 / 6577.4:.3f} of HBM, {fl / (res['2'] * 1e-6) / 1e12 / bench.FP32_FMA_PEAK_TFLOPS:.3f} of fp32 FMA)  max|d|={d:.1e}", flush=True)
+          f"(pair: {bps * B / (res['2'] * 1e-6) / 1e9 / bench.HBM_PEAK_GBS:.3f} of HBM, {fl / (res['2'] * 1e-6) / 1e12 / bench.FP32_FMA_PEAK_TFLOPS:.3f} of fp32 FMA)  max|d|={d:.1e}", flush=True)
     del sets, sts
     torch.cuda.empty_cache()

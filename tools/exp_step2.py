@@ -45,4 +45,4 @@ for B in Bs:
         d = max(float((outs["1"][k] - outs["2"][k]).abs().max()) for k in ("new_x", "new_u", "costs"))
         bps = bench.bytes_per_solve(T, n, m)
         print(f"B={B} box={box}: generic {res['1'][0]:.1f}/{res['1'][1]:.1f} us  pair {res['2'][0]:.1f}/{res['2'][1]:.1f} us (min/median)  "
-              f"pair frac of 6577 GB/s = {bps * B / (res['2'][0] * 1e-6) / 1e9 / 6577.4:.3f}  max|generic-pair| = {d:.2e}", flush=True)
+              f"pair frac of HBM = {bps * B / (res['2'][0] * 1e-6) / 1e9 / bench.HBM_PEAK_GBS:.3f}  max|generic-pair| = {d:.2e}", flush=True)

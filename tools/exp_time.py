@@ -25,4 +25,4 @@ for i in range(reps):
     st[i % nsets](sh)
 e1.record(); torch.cuda.synchronize()
 us = e0.elapsed_time(e1) / reps * 1e3
-print(f"lib={os.environ.get('MPCB200_LIB','default')[-20:]} dbg={os.environ.get('MPCB200_DEBUG','0')} B={B} bounded={bounded}: {us:.1f} us  {B/us:.2f} Msolves/s  {17128*B/us/1e3:.0f} GB/s ({17128*B/us/1e3/6577.4*100:.1f}% of 6577)")
+print(f"lib={os.environ.get('MPCB200_LIB','default')[-20:]} dbg={os.environ.get('MPCB200_DEBUG','0')} B={B} bounded={bounded}: {us:.1f} us  {B/us:.2f} Msolves/s  {17128*B/us/1e3:.0f} GB/s ({17128*B/us/1e3/bench.HBM_PEAK_GBS*100:.1f}% of the HBM data-sheet peak)")

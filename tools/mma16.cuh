@@ -1,4 +1,4 @@
-// mma16.cuh - the two dense products of one Riccati step for n_state = 16 on the tensor cores (sm_100a).
+// mma16.cuh - the two dense products of one Riccati step for n_state = 16 on the tensor cores (sm_90a).
 //
 //   Q' = F' V F   (p x p, p = 16 + m <= 22)      q' = F' v   (p)
 // (reference mpc/lqr_step.py:66-70: Q_t = C_t + F_t' V_{t+1} F_t, q_t = c_t + F_t' v_{t+1}; the caller adds C, c.)

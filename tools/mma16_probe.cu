@@ -1,6 +1,6 @@
 // mma16_probe.cu - checks tools/mma16.cuh (F'VF and F'v of an n=16 problem by mma.sync 3xTF32 with the permuted
 // contraction slots) against a double-precision host loop, and times it.  Not part of the product.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I mpc/pytorch_b200/csrc -I tools -o tools/mma16_probe tools/mma16_probe.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I mpc/pytorch_b200/csrc -I tools -o tools/mma16_probe tools/mma16_probe.cu
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdio>

@@ -3,7 +3,7 @@
 // passes (3xTF32: hi*hi + hi*lo + lo*hi, fp32 accumulate), ONE problem per warp, operands loaded once
 // per warp into fragments.  Checks accuracy against a double-precision host result and times the
 // steady-state cost per problem-step.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/mma_probe tools/mma_probe.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/mma_probe tools/mma_probe.cu
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdio>

@@ -1,16 +1,14 @@
 #!/usr/bin/env python3
 """Per-config measurements (BASELINE.json configs 1-5) of the step kernel, device resident, + the
-adjoint path and the cartpole MPC loop.  Prints a markdown table (-> profiles/r02_results_per_config.md)."""
-import ctypes, json, os, sys, time
+adjoint path and the cartpole MPC loop.  Prints a markdown table."""
+import ctypes, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bench
 from mpc.pytorch_b200.step import lqr_step_raw, lqr_grad_raw
 
 dev = torch.device("cuda:0")
-PEAK = 6577.4
-if os.path.exists("MEASURED_PEAKS.json"):
-    PEAK = float(json.load(open("MEASURED_PEAKS.json"))["hbm_gbs"])
+PEAK = bench.HBM_PEAK_GBS
 
 
 def time_step(B, T, n, m, bounds=None, reps=None):
