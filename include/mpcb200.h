@@ -16,7 +16,8 @@
  *      x_init[B,n] cur_x[T,B,n] cur_u[T,B,m]  (p = n+m)
  *  - the caller owns every buffer; the library allocates nothing, frees nothing
  *    and never writes an input.  Calls are asynchronous on `stream`, re-entrant,
- *    and keep no global state besides a launch counter.
+ *    and keep no global state besides a launch counter and, per host thread, the
+ *    plan of the last step launch (mpcb200_last_step_plan).
  *  - return value: 0 on success, MPCB200_ERR_* otherwise (mpcb200_strerror()).
  *  - optional outputs may be NULL.
  */
@@ -241,6 +242,16 @@ size_t mpcb200_step_smem_bytes(const mpcb200_dims* dims, int32_t elem_size);
  * T steps does not fit shared memory, or (one-problem-per-warp shapes such as n=16) moving it out of shared
  * memory is what lets enough warps be resident.  Pass Ks[T,B,m,n], ks[T,B,m] then. */
 int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size);
+
+/* Plan of the last step-kernel launch made by the calling thread (mpcb200_lqr_step_*, or the nested solve of
+ * mpcb200_lqr_adjoint_*), as MPCB200_PLAN_* bits; 0 if that thread's last step call launched no step kernel.
+ * The launchers record what they actually launched: the kernel, where the gains K_t, k_t of the T steps lived
+ * between the Riccati sweep and the rollout, and whether the rollout read them column per lane. */
+#define MPCB200_PLAN_GENERIC 1u    /* the generic kernel ran (one column per lane)                           */
+#define MPCB200_PLAN_PAIR 2u       /* the column-pair kernel ran                                              */
+#define MPCB200_PLAN_GAINS_SMEM 4u /* gains kept in shared memory; otherwise they went through Ks/ks          */
+#define MPCB200_PLAN_KREDUCE 8u    /* generic kernel, gains in Ks/ks: lane i reads column i, butterfly K dx   */
+int32_t mpcb200_last_step_plan(void);
 
 int mpcb200_version(void);
 const char* mpcb200_strerror(int code);

@@ -38,8 +38,12 @@ EXPORTED_SYMBOLS = (
     "mpcb200_lqr_adjoint_f32", "mpcb200_lqr_adjoint_f64", "mpcb200_adjoint_workspace_bytes",
     "mpcb200_dyn_rollout_f32", "mpcb200_dyn_rollout_f64", "mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64",
     "mpcb200_supported", "mpcb200_supported_list", "mpcb200_launch_count",
-    "mpcb200_step_smem_bytes", "mpcb200_step_prefers_workspace", "mpcb200_version", "mpcb200_strerror",
+    "mpcb200_step_smem_bytes", "mpcb200_step_prefers_workspace", "mpcb200_last_step_plan", "mpcb200_version",
+    "mpcb200_strerror",
 )
+
+# mpcb200_last_step_plan() bits (include/mpcb200.h)
+PLAN_GENERIC, PLAN_PAIR, PLAN_GAINS_SMEM, PLAN_KREDUCE = 1, 2, 4, 8
 
 
 def lib():
@@ -95,6 +99,8 @@ def lib():
     L.mpcb200_step_smem_bytes.restype = ctypes.c_size_t
     L.mpcb200_step_prefers_workspace.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32]
     L.mpcb200_step_prefers_workspace.restype = ctypes.c_int
+    L.mpcb200_last_step_plan.argtypes = []
+    L.mpcb200_last_step_plan.restype = ctypes.c_int32
     L.mpcb200_version.argtypes = []
     L.mpcb200_version.restype = ctypes.c_int
     L.mpcb200_strerror.argtypes = [ctypes.c_int]
@@ -118,6 +124,11 @@ def supported_pairs():
 
 def launch_count():
     return int(lib().mpcb200_launch_count())
+
+
+def last_step_plan():
+    """PLAN_* bits of the step kernel this thread launched last (0: its last step call launched none)."""
+    return int(lib().mpcb200_last_step_plan())
 
 
 def ptr(t):

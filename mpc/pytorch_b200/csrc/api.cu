@@ -53,6 +53,9 @@ static const Entry* find(int n, int m) {
 }
 
 static std::atomic<uint64_t> g_launches{0};
+static thread_local int t_step_plan = 0;      // MPCB200_PLAN_* bits of this thread's last step launch
+
+void record_step_plan(int plan) { t_step_plan = plan; }
 
 // per-device opt-in shared memory limit (cached for up to 64 devices)
 static int max_smem_optin() {
@@ -164,7 +167,8 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
     a.adj_dC = adj->dC; a.adj_dc = adj->dc; a.adj_dF = adj->dF; a.adj_df = adj->df; a.adj_dx_init = adj->dx_init;
     a.adj_c_ts = adj->c_ts;
   }   // developer A/B knob: 1 generic, 2 pair
-  rc = (sizeof(R) == 4 ? e->step32 : e->step64)(a, smem, (cudaStream_t)stream);
+  t_step_plan = 0;             // the launcher that launches records its plan
+  rc =(sizeof(R) == 4 ? e->step32 : e->step64)(a, smem, (cudaStream_t)stream);
   if (rc == 0) g_launches.fetch_add(1);
   return rc;
 }
@@ -469,6 +473,8 @@ int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size) 
   if (ms <= 0) ms = 227 * 1024;       // no device visible (CPU-side query): assume H100's opt-in limit
   return elem_size == 8 ? e->pws64(dims->T, ms) : e->pws32(dims->T, ms);
 }
+
+int32_t mpcb200_last_step_plan(void) { return t_step_plan; }
 
 int mpcb200_version(void) { return MPCB200_VERSION; }
 

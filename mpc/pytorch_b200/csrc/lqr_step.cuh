@@ -31,6 +31,7 @@
 #pragma once
 #include <atomic>
 #include <cstdio>
+#include "../../../include/mpcb200.h"
 #include "common.cuh"
 #include "dynamics.cuh"
 
@@ -64,6 +65,9 @@ struct StepArgs {
   int dyn_kind;   // true dynamics of the rollout: DYN_LINEAR (F,f) or a known system evaluated in the kernel
   DynParams dp;
 };
+
+// the plan (MPCB200_PLAN_* bits) of the step kernel this thread has just launched; read by mpcb200_last_step_plan
+void record_step_plan(int plan);
 
 template <typename R, int N, int M>
 struct StepCfg {
@@ -903,7 +907,10 @@ int launch_step_mode(const StepArgs& args, int max_smem_optin, cudaStream_t stre
   }
   const int grid = (a.B + K::W - 1) / K::W;
   kern<<<grid, K::THREADS, smem, stream>>>(a);
-  return cudaGetLastError() == cudaSuccess ? 0 : 5;
+  if (cudaGetLastError() != cudaSuccess) return 5;
+  record_step_plan((int)(MPCB200_PLAN_GENERIC | (a.k_in_smem ? MPCB200_PLAN_GAINS_SMEM : 0u) |
+                         (K::KREDUCE && !a.k_in_smem && a.do_rollout ? MPCB200_PLAN_KREDUCE : 0u)));
+  return 0;
 }
 
 template <typename R, int N, int M>

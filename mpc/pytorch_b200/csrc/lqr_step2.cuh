@@ -954,7 +954,9 @@ int launch_step2_mode(const StepArgs& args, int max_smem_optin, cudaStream_t str
   auto go = [&](auto kern) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin) != cudaSuccess) return 5;
     kern<<<grid, K::NW * 32, smem, stream>>>(a);
-    return cudaGetLastError() == cudaSuccess ? 0 : 5;
+    if (cudaGetLastError() != cudaSuccess) return 5;
+    record_step_plan((int)(MPCB200_PLAN_PAIR | (a.k_in_smem ? MPCB200_PLAN_GAINS_SMEM : 0u)));
+    return 0;
   };
   if constexpr (MODE == MODE_MASK) {
     if (adj)                     // fused KKT adjoint (+ the d tau store)

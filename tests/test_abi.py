@@ -59,6 +59,20 @@ def test_argument_errors_are_status_codes_not_crashes():
     assert L.mpcb200_step_smem_bytes(ctypes.byref(d), 4) == 0
 
 
+def test_last_step_plan_is_per_thread_and_starts_empty():
+    import threading
+    from mpc.pytorch_b200 import _lib
+    seen = []
+    th = threading.Thread(target=lambda: seen.append(_lib.last_step_plan()))
+    th.start()
+    th.join()
+    assert seen == [0]
+    assert (_lib.PLAN_GENERIC, _lib.PLAN_PAIR, _lib.PLAN_GAINS_SMEM, _lib.PLAN_KREDUCE) == (1, 2, 4, 8)
+    hdr = open(os.path.join(ROOT, "include", "mpcb200.h")).read()
+    for name, v in (("GENERIC", 1), ("PAIR", 2), ("GAINS_SMEM", 4), ("KREDUCE", 8)):
+        assert re.search(rf"#define MPCB200_PLAN_{name} {v}u\b", hdr), name
+
+
 def test_cpu_tensors_are_rejected_loudly():
     from mpc.pytorch_b200 import LQRStep, QuadCost, LinDx
     from mpc.pytorch_b200._lib import MpcB200Error

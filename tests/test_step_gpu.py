@@ -188,25 +188,6 @@ def test_line_search_alphas_on_notebook_problem():
     assert seen_backtrack
 
 
-def test_gains_spill_to_global_for_long_horizons():
-    """T too long for the shared-memory gain store: the kernel round-trips K,k through the caller's buffer."""
-    B, T, n, m = 20, 700, 8, 2
-    C, c, F, f, x0 = gen_problem(40, B, T, n, m, torch.float64)
-    F = F * 0.9
-    u, ul, uu = nominal_controls(40, B, T, m, torch.float64, 0.25)
-    x = orc.get_traj(T, u, x0, F, f)
-    o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, x, u, u_lower=ul, u_upper=uu, coupled=False)
-    from mpc.pytorch_b200 import _lib
-    from mpc.pytorch_b200._lib import Dims
-    import ctypes
-    d = Dims(B=B, T=T, n=n, m=m, F_T=T - 1, has_f=1, bounds_kind=1, has_zero_mask=0, has_delta_u=0,
-             max_ls_iter=10, pnqp_max_iter=20, do_rollout=1)
-    assert _lib.lib().mpcb200_step_smem_bytes(ctypes.byref(d), 8) > 227 * 1024
-    r = raw(n, m, T, x0, C, c, F, f, x, u, u_lower=ul, u_upper=uu)
-    assert maxdiff(r["new_x"], o.new_x) < 1e-8 and maxdiff(r["new_u"], o.new_u) < 1e-8
-    assert torch.equal(r["free_mask"].bool(), o.free_masks)
-
-
 def test_riccati_only_and_split_rollout_equal_fused():
     """do_rollout=0 exports the gains; LQRStep with a Module as true dynamics (split mode) must
     reproduce the fused kernel when the Module is the same affine map."""
