@@ -110,8 +110,7 @@ struct StepCfg {
   static constexpr int SC_K = SC_v + VS;         // M x VS (+ M) K_t,k_t exchange when gains are not smem resident
   static constexpr int KT = M * VS + round_up(M, 4);  // elements per (problem, t) of the gain store
   static constexpr int SC_Q = SC_K + KT;         // M x VS  Q_xu exchange (row a = Q[:n, n+a])
-  static constexpr int SC_X = SC_Q + M * VS;     // 2 x VS  rollout state exchange
-  static constexpr int SC_R = SC_X + 2 * VS;     // cost reduction
+  static constexpr int SC_R = SC_Q + M * VS;     // cost reduction
   static constexpr int SC_RAW = SC_R + round_up(P, 4);
   static constexpr int SCR = (SC_RAW % 32 == 0 || SC_RAW % 32 == 16) ? SC_RAW + 4 : SC_RAW;
   // KREDUCE: when the gains live in the caller's Ks/ks buffer (long horizons / large n), lane i reads only
@@ -392,7 +391,6 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
   R* Vs = scr + K::SC_V;
   R* vs = scr + K::SC_v;
   R* Qx = scr + K::SC_Q;
-  R* xs = scr + K::SC_X;
   R* red = scr + K::SC_R;
   R* kst = a.k_in_smem ? kstore_all + (size_t)pw * T * KT : scr + K::SC_K;
   R* gKs = (R*)a.Ks;
@@ -806,16 +804,11 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
           }
         }
       }
-      if (t < T - 1) {
-        R* xsb = xs + (t & 1) * VS;
+      if (t < T - 1) {                           // x_{t+1} to every lane of the problem: element i from its column's lane
 #pragma unroll
-        for (int sl = 0; sl < CPL; ++sl) {
-          if (wsl[sl] && isx[sl]) xsb[cc[sl]] = xn[sl];
-          xown[sl] = xn[sl];
-        }
-        __syncwarp();
-        xr.template load<EA>(xsb);
-        if constexpr (N & 1) xr.p[Vec<R, N>::NP - 1].y = R(0);
+        for (int i = 0; i < N; ++i) xr.set(i, shfl(xn[i / LP], base + i % LP));
+#pragma unroll
+        for (int sl = 0; sl < CPL; ++sl) xown[sl] = xn[sl];
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[stg]);

@@ -1,0 +1,74 @@
+"""Is config 3 (T=20, n=8, m=2, fp32, unbounded) latency bound or throughput bound?  (developer tool)
+
+Runs the step over a sweep of batch sizes and reports us per launch and us per busiest-SM problem slot: the
+launch time over the number of problems the most loaded SM holds (ceil(CTAs / SMs) * problems per CTA).  At
+B=4096 an SM holds about 6 CTAs of the generic kernel; at B=65536 it keeps as many resident as registers allow
+and runs waves of them.  If one warp's dependent chain set the time, the extra resident warps would hide it and the
+per-slot time would fall; if an SM resource saturates already at B=4096, the per-slot time stays flat.
+
+  python tools/exp_cfg3_bound.py [--riccati] [--batches 1024,4096,...]
+
+--riccati times the Riccati sweep alone (do_rollout = 0, gains written to Ks/ks).  The card's name, power limit
+and median SM clock under the load are printed with the numbers.
+"""
+import argparse
+import ctypes
+import math
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch  # noqa: E402
+
+import bench  # noqa: E402
+
+T, N, M = 20, 8, 2
+PROBLEMS_PER_CTA = 6        # the generic kernel at (8, 2) f32: 2 consumer warps x 3 problems
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--riccati", action="store_true")
+    ap.add_argument("--batches", default="1024,2048,4096,8192,16384,65536")
+    ap.add_argument("--reps", type=int, default=0, help="launches per timed block (0: ~0.2 s of work)")
+    args = ap.parse_args()
+    from mpc.pytorch_b200 import _lib
+    dev = torch.device("cuda:0")
+    stream = torch.cuda.current_stream(dev)
+    sh = ctypes.c_void_p(stream.cuda_stream)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    info = bench.device_info(0)
+    clk = bench.ClockSampler(0)
+    clk.start()
+    rows = []
+    for B in [int(b) for b in args.batches.split(",")]:
+        nsets = max(2, min(4, int(300e6 // (bench.bytes_per_solve(T, N, M) * B)) + 1))
+        sts = [bench.RawStepper(bench.gen_inputs(100 + s, B, T, N, M, dev), B, T, N, M) for s in range(nsets)]
+        if args.riccati:
+            for st in sts:
+                st.dims.do_rollout = 0
+                st.Ks = torch.empty(T, B, M, N, device=dev)
+                st.ks = torch.empty(T, B, M, device=dev)
+                st.args[-3], st.args[-2] = _lib.ptr(st.Ks), _lib.ptr(st.ks)
+        reps = args.reps or max(20, int(2e5 / max(1.0, 15.0 * B / 1024)))
+        us = bench.time_launches(sts, reps, stream, sh, blocks=5)
+        plan = _lib.last_step_plan()
+        if not plan & _lib.PLAN_GENERIC:
+            raise SystemExit(f"expected the generic kernel at (8, 2) f32, the plan was {plan}")
+        busiest = math.ceil(math.ceil(B / PROBLEMS_PER_CTA) / sms) * PROBLEMS_PER_CTA
+        rows.append((B, us / busiest))
+        print(f"B={B:6d}  {us:9.1f} us/launch  busiest SM {busiest:4d} problems  {us / busiest:6.3f} us/slot",
+              flush=True)
+        del sts
+        torch.cuda.empty_cache()
+    c = clk.stop()
+    print(f"card: {info['name']}, power limit {info['power_limit_w']} W, median SM clock {c['sm_mhz']} MHz "
+          f"(max {c['sm_max_mhz']}), throttle reasons {c['reasons']}; {sms} SMs; "
+          f"{'Riccati only' if args.riccati else 'sweep + rollout'}")
+    per_slot = dict(rows)
+    if 4096 in per_slot and 65536 in per_slot:
+        print(f"per-slot time at B=4096 / B=65536: {per_slot[4096] / per_slot[65536]:.3f}")
+
+
+if __name__ == "__main__":
+    main()
