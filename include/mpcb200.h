@@ -212,12 +212,16 @@ int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_
                               const double* u, double* F, double* f, void* stream);
 
 /*
- * Standalone projected-Newton box QP, n <= 8: replaces pnqp(H,q,lower,upper,x_init,n_iter) of the
- * reference (mpc/pnqp.py:5-82) for batches of small QPs  min 0.5 x'Hx + q'x, lower <= x <= upper.
+ * Standalone projected-Newton box QP, n <= mpcb200_pnqp_max_n(elem_size): replaces
+ * pnqp(H,q,lower,upper,x_init,n_iter) of the reference (mpc/pnqp.py:5-82) for batches of QPs
+ * min 0.5 x'Hx + q'x, lower <= x <= upper.
  * H[B,n,n] q,lower,upper[B,n]; x_init[B,n] or NULL (cold start -H^{-1}q).  Outputs x[B,n],
  * H_free[B,n,n] (the masked matrix H_ of the returning iteration, whose LU the reference returns),
  * If[B,n] uint8 free set, iters[B] (the reference's `i`), status[B] optional (MPCB200_ST_* bits).
- * Per-problem control flow (what the reference computes for n_batch = 1).
+ * Per-problem control flow (what the reference computes for n_batch = 1).  H must be symmetric: the
+ * Newton systems are solved by LDL^T of the lower triangle of H_.  n <= 8 runs one thread per QP,
+ * larger n one thread block per QP with the QP in shared memory; n > mpcb200_pnqp_max_n returns
+ * MPCB200_ERR_SMEM.
  */
 int mpcb200_pnqp_f32(int32_t B, int32_t n, const float* H, const float* q, const float* lower,
                      const float* upper, const float* x_init, int32_t n_iter, float* x, float* H_free,
@@ -225,6 +229,10 @@ int mpcb200_pnqp_f32(int32_t B, int32_t n, const float* H, const float* q, const
 int mpcb200_pnqp_f64(int32_t B, int32_t n, const double* H, const double* q, const double* lower,
                      const double* upper, const double* x_init, int32_t n_iter, double* x, double* H_free,
                      uint8_t* If, int32_t* iters, int32_t* status, void* stream);
+
+/* Largest n mpcb200_pnqp_* solves for elem_size 4 (f32) or 8 (f64), from the current device's opt-in shared
+ * memory per block (227 KB, the H100's, when no device is visible); 0 for any other elem_size. */
+int32_t mpcb200_pnqp_max_n(int32_t elem_size);
 
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);

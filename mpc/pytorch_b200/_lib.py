@@ -34,7 +34,7 @@ _lib = None
 # every symbol include/mpcb200.h declares
 EXPORTED_SYMBOLS = (
     "mpcb200_lqr_step_f32", "mpcb200_lqr_step_f64", "mpcb200_lqr_grad_f32", "mpcb200_lqr_grad_f64",
-    "mpcb200_rollout_f32", "mpcb200_rollout_f64", "mpcb200_pnqp_f32", "mpcb200_pnqp_f64",
+    "mpcb200_rollout_f32", "mpcb200_rollout_f64", "mpcb200_pnqp_f32", "mpcb200_pnqp_f64", "mpcb200_pnqp_max_n",
     "mpcb200_lqr_adjoint_f32", "mpcb200_lqr_adjoint_f64", "mpcb200_adjoint_workspace_bytes",
     "mpcb200_dyn_rollout_f32", "mpcb200_dyn_rollout_f64", "mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64",
     "mpcb200_supported", "mpcb200_supported_list", "mpcb200_launch_count",
@@ -75,6 +75,8 @@ def lib():
         fn = getattr(L, name)
         fn.argtypes = [ctypes.c_int32, ctypes.c_int32] + [vp] * 5 + [ctypes.c_int32] + [vp] * 6
         fn.restype = ctypes.c_int
+    L.mpcb200_pnqp_max_n.argtypes = [ctypes.c_int32]
+    L.mpcb200_pnqp_max_n.restype = ctypes.c_int32
     for name in ("mpcb200_lqr_adjoint_f32", "mpcb200_lqr_adjoint_f64"):
         fn = getattr(L, name)
         fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params)] + [vp] * 15 + [ctypes.c_size_t, vp]

@@ -1,10 +1,15 @@
-"""pnqp: batched projected-Newton box QP on the GPU (drop-in for reference mpc/pnqp.py:5, n <= 8).
+"""pnqp: batched projected-Newton box QP on the GPU (drop-in for reference mpc/pnqp.py:5).
 
 Same signature and return tuple as the reference: ``(x, H_free, If, i)``.  ``H_free`` is the masked
 matrix ``H_`` of the returning iteration (the reference returns its LU factorisation, or ``H_`` itself
 for n == 1); ``If`` is a 0/1 tensor of H's dtype; ``i`` is the iteration count of the slowest problem
 (the reference's batch-coupled loop returns when the slowest element converges).  Control flow is per
 problem (what the reference computes for n_batch == 1).
+
+QPs with n <= 8 run one per thread; larger ones run one per thread block, with the QP in shared memory, up to
+``mpcb200_pnqp_max_n`` (at least 128 in float32 and float64 on an H100); larger n raises ``MpcB200Error``.
+``H`` must be symmetric: the Newton systems are solved by an LDL^T factorisation of its lower triangle (the
+reference uses an LU, which also accepts a non-symmetric ``H``).
 """
 
 import torch
@@ -25,9 +30,13 @@ def pnqp(H, q, lower, upper, x_init=None, n_iter=20):
                 raise MpcB200Error(f"{nm}: expected a tensor on {H.device}, got {t_.device}")
             if tuple(t_.shape) not in ((B, n), (n,), (1, n)):
                 raise MpcB200Error(f"{nm}: expected shape {(B, n)}, got {tuple(t_.shape)}")
-    if n > 8:
-        raise MpcB200Error(f"pnqp kernels are compiled for n <= 8 (got {n}); inside LQRStep the QP size is n_ctrl")
     dtype, dev = H.dtype, H.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        max_n = L.mpcb200_pnqp_max_n(4 if dtype == torch.float32 else 8)
+    if n > max_n:
+        raise MpcB200Error(f"pnqp solves QPs with n <= {max_n} in {dtype} on {dev} (got n = {n}): the QP of one "
+                           "thread block must fit its shared memory")
     d = lambda t: t.detach().to(dtype).expand(B, n).contiguous() if torch.is_tensor(t) else \
         torch.full((B, n), float(t), dtype=dtype, device=dev)
     Hc, qc, lo, hi = H.detach().contiguous(), d(q), d(lower), d(upper)
@@ -37,7 +46,6 @@ def pnqp(H, q, lower, upper, x_init=None, n_iter=20):
     If = torch.empty(B, n, dtype=torch.uint8, device=dev)
     iters = torch.empty(B, dtype=torch.int32, device=dev)
     status = torch.empty(B, dtype=torch.int32, device=dev)
-    L = _lib.lib()
     fn = L.mpcb200_pnqp_f32 if dtype == torch.float32 else L.mpcb200_pnqp_f64
     with torch.cuda.device(dev):
         rc = fn(B, n, ptr(Hc), ptr(qc), ptr(lo), ptr(hi), ptr(x0), int(n_iter), ptr(x), ptr(Hf), ptr(If),

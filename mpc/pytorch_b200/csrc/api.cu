@@ -7,6 +7,7 @@
 #include "lqr_grad.cuh"
 #include "lqr_rollout.cuh"
 #include "lqr_step.cuh"
+#include "pnqp.cuh"
 
 namespace mpcb200 {
 #define MPCB200_INST(n, m)                                                  \
@@ -58,7 +59,7 @@ static thread_local int t_step_plan = 0;      // MPCB200_PLAN_* bits of this thr
 void record_step_plan(int plan) { t_step_plan = plan; }
 
 // per-device opt-in shared memory limit (cached for up to 64 devices)
-static int max_smem_optin() {
+int max_smem_optin() {
   static std::atomic<int> cache[64];         // written once per device with the same value: safe from any thread
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;

@@ -1,19 +1,12 @@
-// pnqp.cu - standalone projected-Newton box QP (reference mpc/pnqp.py:5-82) for small n.
-// One thread per QP; same per-problem control flow and arithmetic as inside the step kernel
-// (pnqp_lane in lqr_step.cuh).  min 0.5 x'Hx + q'x  s.t. lower <= x <= upper.
+// pnqp.cu - standalone projected-Newton box QP (reference mpc/pnqp.py:5-82), C entry points and dispatch.
+// n <= 8: one thread per QP; same per-problem control flow and arithmetic as inside the step kernel
+// (pnqp_lane in lqr_step.cuh).  8 < n <= pnqp_max_n: one CTA per QP (pnqp_large.cu).
+// min 0.5 x'Hx + q'x  s.t. lower <= x <= upper.
 #include "../../../include/mpcb200.h"
 #include "lqr_step.cuh"
+#include "pnqp.cuh"
 
 namespace mpcb200 {
-
-struct PnqpArgs {
-  int B, n_iter, has_init;
-  const void *H, *q, *lo, *hi, *x_init;
-  void *x, *Hfree;
-  unsigned char* If;
-  int* iters;
-  int* status;
-};
 
 template <typename R, int M>
 __global__ void __launch_bounds__(128) pnqp_kernel(const PnqpArgs a) {
@@ -63,7 +56,12 @@ static int pnqp_dispatch(const PnqpArgs& a, int n, cudaStream_t stream) {
     MPCB_PNQP_CASE(1) MPCB_PNQP_CASE(2) MPCB_PNQP_CASE(3) MPCB_PNQP_CASE(4)
     MPCB_PNQP_CASE(5) MPCB_PNQP_CASE(6) MPCB_PNQP_CASE(7) MPCB_PNQP_CASE(8)
 #undef MPCB_PNQP_CASE
-    default: return MPCB200_ERR_UNSUPPORTED_DIMS;
+    default: {
+      const int ms = max_smem_optin();
+      if (ms <= 0) return MPCB200_ERR_NO_DEVICE;
+      if (n > pnqp_max_n((int)sizeof(R), ms)) return MPCB200_ERR_SMEM;
+      return pnqp_cta_launch<R>(a, ms, stream);
+    }
   }
   return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH;
 }
@@ -75,7 +73,7 @@ static int pnqp_impl(int32_t B, int32_t n, const R* H, const R* q, const R* lowe
   if (B <= 0 || n <= 0 || n_iter < 1) return MPCB200_ERR_BAD_DIMS;
   if (!H || !q || !lower || !upper || !x || !H_free || !If || !iters) return MPCB200_ERR_NULL_POINTER;
   PnqpArgs a;
-  a.B = B; a.n_iter = n_iter; a.has_init = x_init != nullptr;
+  a.B = B; a.n = n; a.n_iter = n_iter; a.has_init = x_init != nullptr;
   a.H = H; a.q = q; a.lo = lower; a.hi = upper; a.x_init = x_init;
   a.x = x; a.Hfree = H_free; a.If = If; a.iters = iters; a.status = status;
   return pnqp_dispatch<R>(a, n, (cudaStream_t)stream);
@@ -92,5 +90,11 @@ int mpcb200_pnqp_f64(int32_t B, int32_t n, const double* H, const double* q, con
                      const double* upper, const double* x_init, int32_t n_iter, double* x, double* H_free,
                      uint8_t* If, int32_t* iters, int32_t* status, void* stream) {
   return mpcb200::pnqp_impl<double>(B, n, H, q, lower, upper, x_init, n_iter, x, H_free, If, iters, status, stream);
+}
+int32_t mpcb200_pnqp_max_n(int32_t elem_size) {
+  if (elem_size != 4 && elem_size != 8) return 0;
+  int ms = mpcb200::max_smem_optin();
+  if (ms <= 0) ms = 227 * 1024;       // no device visible (CPU-side query): assume H100's opt-in limit
+  return mpcb200::pnqp_max_n(elem_size, ms);
 }
 }

@@ -163,8 +163,43 @@ static int run_dyn(int kind, int B, int T) {
   return bad != 0;
 }
 
+// standalone pnqp above n = 8 (one thread block per QP): f64 box QPs H = L L' / n + I
+static int run_pnqp_large(int B, int n) {
+  const int max_n = mpcb200_pnqp_max_n(8);
+  if (max_n < n) return printf("pnqp max_n(8) = %d < %d\n", max_n, n), 1;
+  std::vector<double> L((size_t)n * n), H((size_t)B * n * n), q((size_t)B * n), lo((size_t)B * n, -0.5),
+      hi((size_t)B * n, 0.5);
+  for (int b = 0; b < B; ++b) {
+    for (auto& v : L) v = rnd();
+    for (int i = 0; i < n; ++i)
+      for (int j = 0; j < n; ++j) {
+        double s = i == j ? 1.0 : 0.0;
+        for (int k = 0; k < n; ++k) s += L[(size_t)i * n + k] * L[(size_t)j * n + k] / n;
+        H[((size_t)b * n + i) * n + j] = s;
+      }
+  }
+  for (auto& v : q) v = 2.0 * rnd();
+  Dev<double> dH(H.size()), dq(q.size()), dl(lo.size()), dh(hi.size()), ox(q.size()), oH(H.size());
+  Dev<unsigned char> oI(q.size());
+  Dev<int> oit(B), ost(B);
+  dH.up(H); dq.up(q); dl.up(lo); dh.up(hi);
+  int rc = mpcb200_pnqp_f64(B, n, dH.p, dq.p, dl.p, dh.p, nullptr, 20, ox.p, oH.p, oI.p, oit.p, ost.p, nullptr);
+  if (rc) return printf("pnqp n=%d rc=%d (%s)\n", n, rc, mpcb200_strerror(rc)), 1;
+  rc = mpcb200_pnqp_f64(B, max_n + 1, dH.p, dq.p, dl.p, dh.p, nullptr, 20, ox.p, oH.p, oI.p, oit.p, ost.p, nullptr);
+  if (rc != MPCB200_ERR_SMEM) return printf("pnqp n=max_n+1 rc=%d\n", rc), 1;
+  if (cudaDeviceSynchronize() != cudaSuccess) return printf("CUDA error: %s\n", cudaGetErrorString(cudaGetLastError())), 1;
+  double s = 0;
+  int bad = 0;
+  for (double v : ox.down()) { s += v; bad += !std::isfinite(v); }
+  std::vector<int> st = ost.down();
+  for (int v : st) bad += v != 0;
+  printf("pnqp B=%d n=%d (max_n f32 %d, f64 %d): checksum %.6f bad %d\n", B, n, mpcb200_pnqp_max_n(4), max_n, s, bad);
+  return bad != 0;
+}
+
 int main() {
   int fails = 0;
+  fails += run_pnqp_large(3, 100);
   fails += run_dyn(MPCB200_DYN_CARTPOLE, 37, 9);
   fails += run_dyn(MPCB200_DYN_PENDULUM, 20, 7);
   const int cases[][6] = {{13, 6, 8, 2, 0, 0}, {13, 6, 8, 2, 1, 0}, {12, 5, 8, 2, 2, 1}, {7, 4, 3, 1, 1, 0},

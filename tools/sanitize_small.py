@@ -17,4 +17,12 @@ for (B, T, n, m, dt) in [(13, 6, 8, 2, torch.float32), (7, 5, 3, 1, torch.float6
     a = lqr_step_raw(n, m, T, torch.zeros_like(x0), C, -torch.cat((x, u), 2), F, None, torch.zeros_like(x), torch.zeros_like(u), u_zero_I=I)
     g = lqr_grad_raw(n, m, T, C, c, F, o["new_x"], o["new_u"], a["new_x"], a["new_u"], x, True)
     torch.cuda.synchronize()
+from mpc.pnqp import pnqp
+for (B, n, dt) in [(2, 100, torch.float64), (3, 128, torch.float32)]:    # one thread block per QP
+    g = torch.Generator().manual_seed(n)
+    L = torch.randn(B, n, n, generator=g, dtype=torch.float64)
+    H = (L @ L.transpose(1, 2) + 0.5 * torch.eye(n, dtype=torch.float64)).to(dt).to(dev)
+    q = (2.0 * torch.randn(B, n, generator=g, dtype=torch.float64)).to(dt).to(dev)
+    pnqp(H, q, -torch.rand(B, n, generator=g).to(dt).to(dev), torch.rand(B, n, generator=g).to(dt).to(dev))
+    torch.cuda.synchronize()
 print("sanitize workload done")
