@@ -11,7 +11,10 @@ CUDA tensors, replaces
   * the Module rollout of ``lqr_forward`` (reference mpc/lqr_step.py:224-225)          -> inside the step kernel
 so that one iLQR iteration is three kernel launches plus the best-iterate bookkeeping.
 """
+import contextlib
 import ctypes
+import itertools
+import threading
 
 import torch
 from torch.nn import Module
@@ -20,17 +23,40 @@ from . import _lib
 from ._lib import MpcB200Error, check, ptr, stream_handle
 
 DYN_LINEAR, DYN_CARTPOLE, DYN_PENDULUM = 0, 1, 2
+DYN_DIMS = {DYN_CARTPOLE: (5, 1), DYN_PENDULUM: (3, 1)}       # (n_state, n_ctrl) of each known system
+
+_scope = threading.local()      # depth and epoch of the enclosing params_scope() on this thread
+_epochs = itertools.count(1)    # process-wide: two threads' scopes never share an epoch (the cache is per module)
+
+
+@contextlib.contextmanager
+def params_scope():
+    """One solve (``MPC.forward``): inside it, CUDA parameter tensors of known systems are read back to the host
+    once, not once per kernel launch (a device->host read per launch would serialise every iLQR iteration).
+    Nested scopes share the outermost one's values.  Outside any scope every read is fresh, so a direct
+    ``LQRStep`` call reads them once (its forward asks once)."""
+    depth = getattr(_scope, "depth", 0)
+    if depth == 0:
+        _scope.epoch = next(_epochs)
+    _scope.depth = depth + 1
+    try:
+        yield
+    finally:
+        _scope.depth = depth
 
 
 def _host_values(owner, params):
-    """Python floats of a (possibly CUDA, possibly learnable) parameter tensor, read back only when it changed:
-    the kernels take the parameters by value, and a device->host read per kernel call would serialise the GPU."""
-    key = (params.data_ptr(), params._version, params.device)
+    """Python floats of a (possibly CUDA, possibly learnable) parameter tensor, as ``forward`` would use them now.
+    The kernels take the parameters by value.  CPU tensors are read on every call (free); CUDA tensors once per
+    params_scope().  Tensor versions cannot tell whether the values changed: an edit through ``.data`` does not
+    bump ``_version``, and a reassigned tensor may reuse the old one's storage."""
+    if not params.is_cuda or getattr(_scope, "depth", 0) == 0:
+        return tuple(float(v) for v in params.detach().cpu())
     hit = getattr(owner, "_mpcb200_host_cache", None)
-    if hit is None or hit[0] != key:
-        hit = (key, tuple(float(v) for v in params.detach().cpu()))
+    if hit is None or hit[0] != _scope.epoch or hit[1] is not params:
+        hit = (_scope.epoch, params, tuple(float(v) for v in params.detach().cpu()))
         owner._mpcb200_host_cache = hit
-    return hit[1]
+    return hit[2]
 
 
 class CartpoleDx(Module):
@@ -140,15 +166,32 @@ def _dyn_array(params):
     return (ctypes.c_double * 8)(*params)
 
 
+def _check_dyn_shapes(kind, T, what, x, x_shape, u):
+    """The kernels index x and u by the system's own (n_state, 1): check the shapes before anything launches."""
+    if kind not in DYN_DIMS:
+        raise MpcB200Error(f"unknown dynamics kind {kind}")
+    n, m = DYN_DIMS[kind]
+    if int(T) < 1:
+        raise MpcB200Error(f"T must be at least 1, got {T}")
+    B = x.shape[-2] if x.dim() >= 2 else -1
+    want_x = (B, n) if x_shape == "BN" else (T, B, n)
+    if tuple(x.shape) != want_x or B < 1:
+        raise MpcB200Error(f"{what}: expected shape {want_x} (n_state = {n}), got {tuple(x.shape)}")
+    if tuple(u.shape) != (T, B, m):
+        raise MpcB200Error(f"u: expected shape {(T, B, m)} (n_ctrl = {m}), got {tuple(u.shape)}")
+    if x.dtype not in (torch.float32, torch.float64):
+        raise MpcB200Error(f"unsupported dtype {x.dtype}")
+    if not x.is_cuda:
+        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
+    if u.device != x.device:
+        raise MpcB200Error(f"u is on {u.device}, {what} on {x.device}")
+    return B, n, m
+
+
 def dyn_rollout_raw(kind, params, T, x_init, u):
     """x = get_traj(T, u, x_init, dynamics) for a known system, ONE kernel (reference mpc/util.py:102-126)."""
-    if not x_init.is_cuda:
-        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
+    B, n, m = _check_dyn_shapes(kind, T, "x_init", x_init, "BN", u)
     dtype, dev = x_init.dtype, x_init.device
-    B, n = x_init.shape
-    m = u.shape[2]
-    if tuple(u.shape) != (T, B, m) or u.device != dev:
-        raise MpcB200Error(f"u: expected shape {(T, B, m)} on {dev}, got {tuple(u.shape)} on {u.device}")
     x0 = x_init.detach().to(dtype).contiguous()
     u_ = u.detach().to(dtype).contiguous()
     x = torch.empty(T, B, n, dtype=dtype, device=dev)
@@ -163,9 +206,8 @@ def dyn_rollout_raw(kind, params, T, x_init, u):
 def dyn_linearize_raw(kind, params, T, x, u):
     """(F[T-1,B,n,n+m], f[T-1,B,n]) = linearisation of a known system along (x, u), ONE kernel
     (reference MPC.linearize_dynamics, mpc/mpc.py:490-601)."""
+    B, n, m = _check_dyn_shapes(kind, T, "x", x, "TBN", u)
     dtype, dev = x.dtype, x.device
-    _, B, n = x.shape
-    m = u.shape[2]
     x_ = x.detach().to(dtype).contiguous()
     u_ = u.detach().to(dtype).contiguous()
     F = torch.empty(T - 1, B, n, n + m, dtype=dtype, device=dev)

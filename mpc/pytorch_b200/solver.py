@@ -170,6 +170,11 @@ class MPC(Module):
 
     # ------------------------------------------------------------------------------------
     def forward(self, x_init, cost, dx):
+        from .dynamics import params_scope
+        with params_scope():            # a known system's CUDA parameters are read back once per solve
+            return self._forward(x_init, cost, dx)
+
+    def _forward(self, x_init, cost, dx):
         assert isinstance(cost, (QuadCost, Module, Function))
         assert isinstance(dx, (LinDx, Module, Function))
         T, n, m = self.T, self.n_state, self.n_ctrl

@@ -207,11 +207,17 @@ def _bound(v, t):
 def lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, current_x, current_u,
                      u_lower=None, u_upper=None, u_zero_I=None, delta_u=None,
                      linesearch_decay=0.2, max_linesearch_iter=10,
-                     coupled=True, exact_pinv=True):
-    """One box-constrained LQR step in delta space (true model = QuadCost/LinDx).
+                     coupled=True, exact_pinv=True, dynamics=None, ls_trace=None):
+    """One box-constrained LQR step in delta space (true cost = QuadCost).
 
     ``exact_pinv``: use the SVD pseudo-inverse for the unbounded m>1 branch like
     the reference (mpc/lqr_step.py:88-94); False uses an LU solve.
+    ``dynamics``: the true dynamics of the line-search rollout, a callable
+    ``x_{t+1} = dynamics(x_t, u_t)`` on [B, n] / [B, m] (mpc/lqr_step.py:224-225);
+    None rolls out ``F[t] [x; u] + f[t]`` (LinDx, :217-222).  The Riccati sweep
+    uses F (and delta space, so not f) either way.
+    ``ls_trace``: a list that receives ``current_cost - old_cost`` [B] of every
+    line-search pass, the comparison that decides each alpha (:247).
     """
     n, m = n_state, n_ctrl
     B = C.shape[1]
@@ -317,7 +323,9 @@ def lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, current_x, current_
                 nu = _clamp_assign(nu, lb, ub)
             new_u.append(nu)
             xut = torch.cat((new_x[t], nu), 1)
-            if t < T - 1:
+            if t < T - 1 and dynamics is not None:
+                new_x.append(dynamics(new_x[t], nu))
+            elif t < T - 1:
                 nx = _mv(F[t], xut)
                 if has_f:
                     nx = nx + f[t]
@@ -329,6 +337,8 @@ def lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, current_x, current_
         if full_du_norm is None:                                      # :243-245
             full_du_norm = (u - new_u).transpose(1, 2).reshape(B, -1).norm(2, 1)
         worse = current_cost > old_cost
+        if ls_trace is not None:
+            ls_trace.append(current_cost - old_cost)
         alphas = torch.where(worse, alphas * linesearch_decay, alphas)
         i += 1
     worse = current_cost > old_cost

@@ -168,3 +168,127 @@ def pendulum_case():
 
 if __name__ == "__main__" and os.environ.get("GOLDEN_PENDULUM", "1") == "1":
     pendulum_case()
+
+
+def _known_states(name, B, g):
+    """States of a known system with the angle pair (r cos th, r sin th) at radii 0.3, 1 and 3, not only 1."""
+    th = (torch.rand(B, generator=g) * 2 - 1) * 3.0
+    r = torch.tensor((0.3, 1.0, 3.0)).repeat(B)[:B]
+    rest = lambda s: (torch.rand(B, generator=g) - 0.5) * s
+    if name == "cartpole":
+        return torch.stack((rest(1.0), rest(1.0), r * torch.cos(th), r * torch.sin(th), rest(2.0)), 1)
+    return torch.stack((r * torch.cos(th), r * torch.sin(th), rest(2.0)), 1)
+
+
+def _jacobians(module, xs, us):
+    """R = dx'/dx, S = dx'/du of module(xs, us) by autograd (what the reference's AUTO_DIFF linearisation does)."""
+    xs = xs.clone().requires_grad_(True)
+    us = us.clone().requires_grad_(True)
+    nx = module(xs, us)
+    rows = [torch.autograd.grad(nx[:, j].sum(), [xs, us], retain_graph=True) for j in range(nx.shape[1])]
+    return nx.detach(), torch.stack([r[0] for r in rows], 1), torch.stack([r[1] for r in rows], 1)
+
+
+# non-default physics of each known system: parameters, dt, control clamp, step options
+KNOWN_SYSTEMS = {
+    "cartpole": dict(params=(9.81, 1.3, 0.25, 0.8), dt=0.04, clamp=("force_mag", 7.5), decay=0.3, ls_iter=4,
+                     u_weight=0.03),
+    "pendulum": dict(params=(9.1, 1.7, 0.6), dt=0.15, clamp=("max_torque", 1.5), decay=0.35, ls_iter=6,
+                     u_weight=1.0),
+}
+
+
+def known_step_cases():
+    """One LQR step whose line search rolls out a known nonlinear system (reference
+    LQRStep(..., true_dynamics=<env module>, true_cost=QuadCost), mpc/lqr_step.py:217-225) at non-default physics,
+    linearised along a rollout of nominal controls, with one x_init off the unit circle.  Two bound regimes: scalar
+    bounds inside the system's control clamp, and bounds twice as wide, so that the clamp inside the dynamics
+    engages.  Asserts that oracle.lqr_step_forward(dynamics=<our module>) equals the reference to 1e-10 with the
+    same saturated controls, and stores inputs, outputs, next states and autograd Jacobians of the reference module
+    as tests/golden/known_step_{cartpole,pendulum}_f64.npz."""
+    from oracle import lqr_oracle as orc
+    from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
+    rmpc, rstep, _, _ = load_reference()
+    torch.set_default_dtype(torch.float64)
+    ours_cls = {"cartpole": CartpoleDx, "pendulum": PendulumDx}
+    for name, spec in KNOWN_SYSTEMS.items():
+        renv = load_ref_env(name)
+        ref_cls = renv.CartpoleDx if name == "cartpole" else renv.PendulumDx
+        ref = ref_cls(params=torch.tensor(spec["params"]))
+        ours = ours_cls[name](params=torch.tensor(spec["params"]))
+        for mod in (ref, ours):
+            mod.dt = spec["dt"]
+            setattr(mod, spec["clamp"][0], spec["clamp"][1])
+        clamp = spec["clamp"][1]
+        n, m, B, T = ref.n_state, 1, 7, 12
+        p = n + m
+        g = torch.Generator().manual_seed(31 if name == "cartpole" else 32)
+        # one-step fixture: states at three radii, theta at +-pi with both signs of sin = 0 and near 0, controls
+        # at, one ulp inside and one ulp outside the clamp, and well inside / outside it
+        xs = _known_states(name, 24, g)
+        ic, is_ = (2, 3) if name == "cartpole" else (0, 1)
+        edge = ((-1.0, 0.0), (-1.0, -0.0), (1.0, 0.0), (1.0, 1e-9), (1.0, -1e-9), (-2.5, 0.0))
+        for k, (cv, sv) in enumerate(edge):
+            xs[k, ic], xs[k, is_] = cv, sv
+        ulp_in, ulp_out = np.nextafter(clamp, 0.0), np.nextafter(clamp, np.inf)
+        us = torch.tensor((clamp, -clamp, ulp_in, -ulp_in, ulp_out, -ulp_out, 0.5 * clamp, -3.0 * clamp)).repeat(3)
+        us = us.view(-1, 1)
+        step_next, R, S = _jacobians(ref, xs, us)
+        o_next, oR, oS = _jacobians(ours, xs, us)
+        assert maxdiff(o_next, step_next) <= 1e-13 and maxdiff(oR, R) <= 1e-12 and maxdiff(oS, S) <= 1e-12, name
+        # the LQR step: nominal controls (some beyond the clamp), their rollout and its linearisation
+        x0 = _known_states(name, B, g)
+        u = (torch.rand(T, B, 1, generator=g) * 2 - 1) * 1.2 * clamp
+        xs_ = [x0]
+        for t in range(T - 1):
+            xs_.append(ref(xs_[t], u[t]).detach())
+        x = torch.stack(xs_)
+        nx, Rl, Sl = _jacobians(ref, x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1))
+        F = torch.cat((Rl, Sl), 2).view(T - 1, B, n, p)
+        f = (nx - torch.einsum("bij,bj->bi", Rl, x[:-1].reshape(-1, n))
+             - torch.einsum("bij,bj->bi", Sl, u[:-1].reshape(-1, 1))).view(T - 1, B, n)
+        Lc = torch.randn(T, B, p, p, generator=g) / p ** 0.5
+        C = Lc @ Lc.transpose(-1, -2) + 0.5 * torch.eye(p)
+        c = torch.randn(T, B, p, generator=g)
+        # large requested state moves: controls on the bounds and first line-search passes that are worse than the
+        # nominal trajectory, so the nonlinear rollout is pinned over several passes (alpha decays)
+        c[..., :n] *= 20.0
+        c[..., n:] = 0.0
+        C[..., n:, :] *= spec["u_weight"]
+        C[..., :, n:] *= spec["u_weight"]
+        out = dict(params=torch.tensor(spec["params"]), dt=np.float64(spec["dt"]), clamp=np.float64(clamp),
+                   decay=np.float64(spec["decay"]), ls_iter=np.int64(spec["ls_iter"]), step_x=xs, step_u=us,
+                   step_next=step_next, R=R, S=S, x_init=x0, C=C, c=c, F=F, f=f, x=x, u=u)
+        for tag, bound in (("in", 0.8 * clamp), ("wide", 2.0 * clamp)):
+            with contextlib.redirect_stdout(io.StringIO()):
+                rx, ru, nqp, rcost, rfdn, ralpha = rstep.LQRStep(
+                    n, m, T, u_lower=-bound, u_upper=bound, linesearch_decay=spec["decay"],
+                    max_linesearch_iter=spec["ls_iter"], true_cost=rmpc.QuadCost(C, c), true_dynamics=ref,
+                    current_x=x, current_u=u)(x0, C, c, F, f)
+            o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, x, u, u_lower=-bound, u_upper=bound,
+                                     linesearch_decay=spec["decay"], max_linesearch_iter=spec["ls_iter"],
+                                     coupled=True, dynamics=ours)
+            for a, b in ((o.new_x, rx), (o.new_u, ru), (o.costs, rcost), (o.full_du_norm, rfdn),
+                         (o.mean_alphas, ralpha)):
+                assert maxdiff(a, b) <= 1e-10 * max(1.0, float(b.abs().max())), (name, tag, maxdiff(a, b))
+            assert float(o.n_total_qp_iter) == float(nqp), (name, tag)
+            for side in (-bound, bound):
+                assert torch.equal(o.new_u == side, ru == side), (name, tag, "active set")
+            beyond = float((ru.abs() > clamp).double().mean())
+            print(f"known step {name} bounds {tag}: saturated {float((ru.abs() == bound).double().mean()):.2f}, "
+                  f"beyond the clamp {beyond:.2f}, mean alpha {float(ralpha):.3f}")
+            if tag == "wide":
+                assert beyond > 0, "the in-dynamics clamp must engage"
+            assert float(ralpha) < 1.0, "the line search must decay some alphas"
+            out.update({f"bound_{tag}": np.float64(bound), f"new_x_{tag}": rx, f"new_u_{tag}": ru,
+                        f"costs_{tag}": rcost, f"full_du_norm_{tag}": rfdn, f"mean_alpha_{tag}": ralpha,
+                        f"n_qp_{tag}": float(nqp)})
+        npz(f"known_step_{name}_f64", **out)
+
+
+def maxdiff(a, b):
+    return float((torch.as_tensor(a).double() - torch.as_tensor(b).double()).abs().max())
+
+
+if __name__ == "__main__" and os.environ.get("GOLDEN_KNOWN_STEP", "1") == "1":
+    known_step_cases()

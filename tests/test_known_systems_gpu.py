@@ -1,0 +1,465 @@
+"""GPU: the known-system kernels against float64 references - the rollout and exact-Jacobian kernels against the
+plain-torch modules (tests/test_known_systems_cpu.py pins those to the reference), the fused LQR step's in-kernel
+line-search rollout against oracle.lqr_step_forward(dynamics=<module>), and MPC.forward against the same physics
+run as an opaque nn.Module.
+
+Every case uses non-default physics (parameters, dt and control clamp), states whose angle pair (r cos th, r sin th)
+is off the unit circle (radius 0.3 or 3 for the pendulum; 0.3 or 2 for the cartpole, whose th_acc denominator
+l (4/3 - mp c^2 / (mp + mc)) vanishes near |c| = 2.9 at these parameters), theta at +-pi with both signs of
+sin = 0 and near 0, and controls at, one ulp inside and one ulp outside the clamp.
+
+Tolerances.  float64: next states to 1e-12 x scale, Jacobians to 1e-11 x scale; the fused step to 1e-9 x scale with
+alphas, free sets and pnqp iteration counts bit exact.  float32: the kernel's error against the float64 truth must
+stay within K32 = 4 times the error of the same computation run in float32 on the CPU, plus 1e-6 x scale.
+
+Batch layouts of the generic step kernel (StepCfg in csrc/lqr_step.cuh, bulk_ok in csrc/api.cu).  A CTA holds
+W problems, PPW per warp: (5,1) has PPW = 5 and W = 10 (f64) / 20 (f32); (3,1) has PPW = 8 and W = 8.  The bulk
+(TMA) load path needs B*n*size and B*m*size to be multiples of 16 bytes (B even in f64, B a multiple of 4 in f32);
+the last CTA's count is then aligned too, since W is a multiple of 2 (f64) / 4 (f32).  Otherwise every tile is
+copied by the producer warp's lanes."""
+import functools
+import math
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import lqr_oracle as orc
+from tests.helpers import maxdiff
+
+pytestmark = pytest.mark.gpu
+DEV = torch.device("cuda:0")
+F32, F64 = torch.float32, torch.float64
+DT = {F32: "f32", F64: "f64"}
+K32 = 4
+
+# non-default physics of each system: parameters, dt, control clamp
+PHYS = {
+    "cartpole": dict(params=(9.81, 1.3, 0.25, 0.8), dt=0.1, clamp_attr="force_mag", clamp=7.5, n=5),
+    "pendulum": dict(params=(9.1, 1.7, 0.6), dt=0.15, clamp_attr="max_torque", clamp=1.5, n=3),
+}
+RADII = {"cartpole": (0.3, 1.0, 2.0), "pendulum": (0.3, 1.0, 3.0)}
+SYSTEMS = tuple(PHYS)
+
+
+def _module(name, params=None, device="cpu"):
+    from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
+    ph = PHYS[name]
+    p = torch.tensor(ph["params"], dtype=F64) if params is None else params
+    dx = (CartpoleDx if name == "cartpole" else PendulumDx)(params=p.to(device))
+    dx.dt = ph["dt"]
+    setattr(dx, ph["clamp_attr"], ph["clamp"])
+    return dx
+
+
+def _angle_cols(name):
+    return (2, 3) if name == "cartpole" else (0, 1)
+
+
+def _states(name, B, seed):
+    """float64 [B, n]: random states, angle pair at the RADII; the first rows hold the theta edge cases."""
+    g = torch.Generator().manual_seed(seed)
+    n = PHYS[name]["n"]
+    x = (torch.rand(B, n, generator=g, dtype=F64) - 0.5) * 2.0
+    th = (torch.rand(B, generator=g, dtype=F64) * 2 - 1) * 3.0
+    r0, _, r1 = RADII[name]
+    r = torch.tensor(RADII[name], dtype=F64).repeat(B)[:B]
+    ic, is_ = _angle_cols(name)
+    x[:, ic], x[:, is_] = r * torch.cos(th), r * torch.sin(th)
+    edge = ((-1.0, 0.0), (-1.0, -0.0), (-r0, 0.0), (-r1, -0.0), (1.0, 1e-9), (1.0, -1e-9), (r1, 0.0))
+    for k, (cv, sv) in enumerate(edge[:B]):
+        x[k, ic], x[k, is_] = cv, sv
+    return x
+
+
+def _clamp_edges(clamp, dtype):
+    """u at the clamp, one ulp (of dtype) inside and outside it, both signs."""
+    npd = np.float64 if dtype == F64 else np.float32
+    c = npd(clamp)
+    inn, out = float(np.nextafter(c, npd(0))), float(np.nextafter(c, npd(np.inf)))
+    return (clamp, -clamp, inn, -inn, out, -out)
+
+
+def _controls(name, T, B, dtype, seed):
+    """float64 [T, B, 1] in +-1.5 clamp; the edge values are spread over the first rows of every time step."""
+    g = torch.Generator().manual_seed(seed + 1)
+    clamp = PHYS[name]["clamp"]
+    u = (torch.rand(T, B, 1, generator=g, dtype=F64) * 2 - 1) * 1.5 * clamp
+    e = torch.tensor(_clamp_edges(clamp, dtype), dtype=F64)
+    k = min(B, len(e))
+    u[:, -k:, 0] = e[:k]                  # the last rows: the first rows hold the theta edges
+    return u
+
+
+def _jac(module, xs, us):
+    """(next, R, S) of module(xs, us) by autograd."""
+    xs = xs.clone().requires_grad_(True)
+    us = us.clone().requires_grad_(True)
+    nx = module(xs, us)
+    rows = [torch.autograd.grad(nx[:, j].sum(), [xs, us], retain_graph=True) for j in range(nx.shape[1])]
+    return nx.detach(), torch.stack([r[0] for r in rows], 1), torch.stack([r[1] for r in rows], 1)
+
+
+def _within(tag, got, w64, w32, dtype, tol64):
+    """float64: |got - w64| <= tol64 x scale; float32: <= K32 |w32 - w64| + 1e-6 x scale."""
+    scale = max(1.0, float(w64.abs().max())) if w64.numel() else 1.0
+    err = maxdiff(got, w64)
+    bound = tol64 * scale if dtype == F64 else K32 * maxdiff(w32, w64) + 1e-6 * scale
+    assert err <= bound, f"{tag}: |kernel - reference| = {err:.3e} > {bound:.3e}"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# rollout and exact Jacobians
+# ------------------------------------------------------------------------------------------------------------------
+BT = [(1, 1), (1, 200), (127, 11), (128, 2), (129, 11), (300, 200), (4097, 11), (4097, 2)]
+
+
+@pytest.mark.parametrize("B,T", BT, ids=[f"B{b}_T{t}" for b, t in BT])
+@pytest.mark.parametrize("dtype", [F64, F32], ids=["f64", "f32"])
+@pytest.mark.parametrize("name", SYSTEMS)
+def test_rollout_matches_module(name, dtype, B, T):
+    """Every step of the kernel rollout against the module's step from the kernel's own state (float64 CPU); the
+    first state is the caller's x_init, copied exactly; several CTAs of 128 threads and a partial last one."""
+    from mpc.pytorch_b200.dynamics import dyn_rollout_raw
+    dx = _module(name)
+    x0 = _states(name, B, 10 + B + T).to(dtype)
+    u = _controls(name, T, B, dtype, 20 + B + T).to(dtype)
+    x = dyn_rollout_raw(dx.mpcb200_kind, dx.mpcb200_params(), T, x0.to(DEV), u.to(DEV)).cpu()
+    assert x.shape == (T, B, dx.n_state) and x.dtype == dtype
+    assert torch.equal(x[0], x0)
+    if T == 1:
+        return
+    xs, us = x[:-1].reshape(-1, dx.n_state).double(), u[:-1].reshape(-1, 1).double()
+    w64 = dx(xs, us).view(T - 1, B, -1)
+    w32 = dx(xs.float(), us.float()).view(T - 1, B, -1) if dtype == F32 else None
+    _within(f"{name} {DT[dtype]} B={B} T={T} rollout", x[1:], w64, w32, dtype, 1e-12)
+
+
+@pytest.mark.parametrize("B,T", BT, ids=[f"B{b}_T{t}" for b, t in BT])
+@pytest.mark.parametrize("dtype", [F64, F32], ids=["f64", "f32"])
+@pytest.mark.parametrize("name", SYSTEMS)
+def test_jacobians_match_autograd(name, dtype, B, T):
+    """F = [R S] and f = x' - R x - S u of the linearisation kernel against float64 autograd of the module, at
+    states off the unit circle, theta edges and controls at / one ulp either side of the clamp."""
+    from mpc.pytorch_b200.dynamics import dyn_linearize_raw
+    dx = _module(name)
+    n = dx.n_state
+    x = torch.stack([_states(name, B, 30 + t) for t in range(T)]).to(dtype)
+    u = _controls(name, T, B, dtype, 40 + B + T).to(dtype)
+    F, f = dyn_linearize_raw(dx.mpcb200_kind, dx.mpcb200_params(), T, x.to(DEV), u.to(DEV))
+    F, f = F.cpu(), f.cpu()
+    assert F.shape == (T - 1, B, n, n + 1) and f.shape == (T - 1, B, n)
+    if T == 1:
+        assert F.numel() == 0 and f.numel() == 0
+        return
+    xs, us = x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1)
+
+    def lin(dt):
+        nx, R, S = _jac(dx, xs.to(dt), us.to(dt))
+        fw = nx - torch.einsum("bij,bj->bi", R, xs.to(dt)) - torch.einsum("bij,bj->bi", S, us.to(dt))
+        return torch.cat((R, S), 2).view(T - 1, B, n, n + 1), fw.view(T - 1, B, n)
+
+    F64w, f64w = lin(F64)
+    F32w, f32w = lin(F32) if dtype == F32 else (None, None)
+    tag = f"{name} {DT[dtype]} B={B} T={T}"
+    _within(tag + " F", F, F64w, F32w, dtype, 1e-11)
+    _within(tag + " f", f, f64w, f32w, dtype, 1e-11)
+    clamp = PHYS[name]["clamp"]
+    out = u[:-1, :, 0].double().abs() > clamp
+    assert bool((F[..., n][out] == 0).all()), f"{tag}: S must be exactly 0 beyond the clamp"
+    assert bool((F[..., n][~out].abs().sum(-1) > 0).all()), f"{tag}: S vanished inside / at the clamp"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the fused LQR step: line-search rollout of the known system inside the step kernel
+# ------------------------------------------------------------------------------------------------------------------
+def _round(t, dtype):
+    return t.to(dtype).double() if torch.is_tensor(t) and t.is_floating_point() and dtype == F32 else t
+
+
+# (scale of the linear state cost, scale of the control row / column of C) of the step cases: the step asks for
+# large state moves, so that the first line-search pass of the nonlinear rollout is often worse than the nominal
+# trajectory and alpha decays.  The cartpole's control authority dt / (mc + mp) is small: its control weight is
+# lowered too, or every step stays where the linearisation is accurate.
+PUSH = {"cartpole": (20.0, 0.03), "pendulum": (20.0, 1.0)}
+
+
+@functools.lru_cache(maxsize=8)
+def step_case(name, B, T, dtype, bounds, ls_iter, decay, seed, calm=False):
+    """Inputs (float64, rounded through dtype), the float64 oracle and its line-search trace, the float32 oracle.
+    The nominal controls are random; x is their nonlinear rollout and F, f its float64 linearisation.
+    calm: hanging start (theta near pi), small nominal controls and linear cost - for long horizons, where the
+    upright-pendulum rollout of random controls amplifies round-off past any fixed tolerance."""
+    dx = _module(name)
+    n, p, clamp = dx.n_state, dx.n_state + 1, PHYS[name]["clamp"]
+    g = torch.Generator().manual_seed(seed)
+    x0 = _states(name, B, seed)
+    if calm:
+        th = torch.pi + 0.4 * (torch.rand(B, generator=g, dtype=F64) - 0.5)
+        ic, is_ = _angle_cols(name)
+        x0[:, ic], x0[:, is_] = torch.cos(th), torch.sin(th)
+    x0 = _round(x0, dtype)
+    u = _round((torch.rand(T, B, 1, generator=g, dtype=F64) * 2 - 1) * (0.1 if calm else 0.8) * clamp, dtype)
+    xs = [x0]
+    for t in range(T - 1):
+        xs.append(dx(xs[t], u[t]))
+    x = _round(torch.stack(xs), dtype)
+    nx, R, S = _jac(dx, x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1))
+    F = torch.cat((R, S), 2).view(T - 1, B, n, p)
+    f = (nx - torch.einsum("bij,bj->bi", R, x[:-1].reshape(-1, n))
+         - torch.einsum("bij,bj->bi", S, u[:-1].reshape(-1, 1))).view(T - 1, B, n)
+    L = torch.randn(T, B, p, p, generator=g, dtype=F64) / p ** 0.5
+    C = L @ L.transpose(-1, -2) + 0.5 * torch.eye(p, dtype=F64)
+    c = torch.randn(T, B, p, generator=g, dtype=F64)
+    if calm:
+        c[..., n:] *= 0.2 * clamp
+    else:
+        x_lin, u_weight = PUSH[name]
+        c[..., :n] *= x_lin
+        c[..., n:] = 0.0
+        C[..., n:, :] *= u_weight
+        C[..., :, n:] *= u_weight
+    F, f, C, c = (_round(v, dtype) for v in (F, f, C, c))
+    kw = dict(linesearch_decay=decay, max_linesearch_iter=ls_iter)
+    if bounds == "scalar":
+        kw.update(u_lower=-0.8 * clamp, u_upper=0.8 * clamp)
+    elif bounds == "wide":                        # wider than the clamp inside the dynamics
+        kw.update(u_lower=-2.0 * clamp, u_upper=2.0 * clamp)
+    elif bounds in ("tensor", "delta"):
+        lo = -clamp * (0.3 + 1.7 * torch.rand(T, B, 1, generator=g, dtype=F64))
+        hi = clamp * (0.3 + 1.7 * torch.rand(T, B, 1, generator=g, dtype=F64))
+        kw.update(u_lower=_round(lo, dtype), u_upper=_round(hi, dtype))
+        u = torch.maximum(torch.minimum(u, kw["u_upper"]), kw["u_lower"])
+        if bounds == "delta":
+            kw["delta_u"] = 0.4 * clamp
+    P = dict(x0=x0, C=C, c=c, F=F, f=f, x=x, u=u)
+    trace = []
+    o64 = orc.lqr_step_forward(n, 1, T, x0, C, c, F, f, x, u, coupled=False, dynamics=dx, ls_trace=trace, **kw)
+    o32 = None
+    if dtype == F32:
+        lo32 = lambda v: v.float() if torch.is_tensor(v) and v.is_floating_point() else v
+        dx32 = _module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32))
+        o32 = orc.lqr_step_forward(n, 1, T, *[lo32(P[k]) for k in ("x0", "C", "c", "F", "f", "x", "u")],
+                                   coupled=False, dynamics=dx32, **{k: lo32(v) for k, v in kw.items()})
+    return P, kw, o64, torch.stack(trace), o32
+
+
+def _run_step(name, T, P, kw, dtype):
+    from mpc.pytorch_b200 import _lib
+    from mpc.pytorch_b200.step import lqr_step_raw
+    dx = _module(name)
+    d = lambda t: t.to(DEV, dtype) if torch.is_tensor(t) else t
+    o = lqr_step_raw(dx.n_state, 1, T, d(P["x0"]), d(P["C"]), d(P["c"]), d(P["F"]), d(P["f"]), d(P["x"]),
+                     d(P["u"]), want_gains=True, dyn=(dx.mpcb200_kind, dx.mpcb200_params()),
+                     **{k: d(v) for k, v in kw.items()})
+    plan = _lib.last_step_plan()
+    torch.cuda.synchronize()
+    return {k: v.cpu() for k, v in o.items() if v is not None}, plan
+
+
+def _passes(alphas, decay):
+    """Number of decays behind each alpha (alpha = decay ** passes): the line-search decisions, free of the
+    dtype's rounding of decay ** passes."""
+    return torch.round(torch.log(alphas.double()) / math.log(decay)).long()
+
+
+def _f32_compared(case):
+    """float32 cases: the problems whose line-search decisions the comparison may demand.  Left out are near-ties
+    (|cost - oldcost| within 1e-5 relative in any pass of the float64 oracle: round-off may decide that
+    comparison either way) and problems where the float32 oracle, the yardstick, decides differently."""
+    P, kw, o64, trace, o32 = case
+    old = o64.costs - trace[-1]
+    tie = (trace.abs() <= 1e-5 * old.abs().clamp_min(1.0)).any(0)
+    decay = kw["linesearch_decay"]
+    return ~tie & (_passes(o32.alphas, decay) == _passes(o64.alphas, decay))
+
+
+def check_step(tag, r, case, dtype):
+    """float64: 1e-9 x scale, alphas / free sets / pnqp iterations bit exact.  float32: the same line-search
+    decisions (number of decays) as the float64 oracle and alphas to 1e-6, except at near-ties; those problems
+    leave the trajectory comparison."""
+    P, kw, o64, trace, o32 = case
+    B = P["x0"].shape[0]
+    bounded = "u_lower" in kw
+    keep = torch.ones(B, dtype=torch.bool)
+    if dtype == F32:
+        keep = _f32_compared(case)
+        assert int((~keep).sum()) <= max(1, B // 8), f"{tag}: {int((~keep).sum())} of {B} problems left out"
+        decay = kw["linesearch_decay"]
+        assert torch.equal(_passes(r["alphas"], decay)[keep], _passes(o64.alphas, decay)[keep]), \
+            f"{tag}: line-search decisions {r['alphas']} vs {o64.alphas}"
+        assert maxdiff(r["alphas"][keep], o64.alphas[keep]) <= 1e-6, f"{tag}: alphas"
+    else:
+        assert torch.equal(r["alphas"], o64.alphas), f"{tag}: alphas {r['alphas']} vs {o64.alphas}"
+    sc = max(1.0, float(o64.new_x.abs().max()), float(o64.new_u.abs().max()))
+    for k in ("new_x", "new_u", "Ks", "ks"):
+        got, w64 = r[k][:, keep], getattr(o64, k)[:, keep]
+        w32 = getattr(o32, k)[:, keep] if o32 is not None else None
+        err = maxdiff(got, w64)
+        bound = 1e-9 * sc if dtype == F64 else K32 * maxdiff(w32, w64) + 1e-6 * sc
+        assert err <= bound, f"{tag}: {k} |kernel - oracle| = {err:.3e} > {bound:.3e}"
+    csc = max(1.0, float(o64.costs.abs().max()))
+    err = maxdiff(r["costs"][keep], o64.costs[keep])
+    bound = 1e-9 * csc if dtype == F64 else K32 * maxdiff(o32.costs[keep], o64.costs[keep]) + 1e-6 * csc
+    assert err <= bound, f"{tag}: costs {err:.3e} > {bound:.3e}"
+    assert int((r["status"] & ~1).max()) == 0, tag
+    if dtype == F64:
+        assert torch.equal(r["free_mask"].bool(), o64.free_masks), f"{tag}: free sets"
+        if bounded:
+            assert torch.equal(r["qp_iters"].long(), o64.qp_iters), f"{tag}: pnqp iterations"
+
+
+def _layout(name, B, dtype):
+    """(problems per CTA, bulk load path) of the generic step kernel, from the rules in the module docstring."""
+    n = PHYS[name]["n"]
+    W = {("cartpole", F64): 10, ("cartpole", F32): 20, ("pendulum", F64): 8, ("pendulum", F32): 8}[(name, dtype)]
+    sz = 8 if dtype == F64 else 4
+    return W, (B * sz) % 16 == 0 and (B * n * sz) % 16 == 0
+
+
+# (system, dtype, B, bulk path): every B leaves a partial last warp and a partial last CTA
+STEP_BATCHES = [("cartpole", F64, 22, True), ("cartpole", F64, 13, False), ("cartpole", F32, 44, True),
+                ("cartpole", F32, 43, False), ("pendulum", F64, 20, True), ("pendulum", F64, 21, False),
+                ("pendulum", F32, 20, True), ("pendulum", F32, 21, False)]
+# (bounds, max_linesearch_iter, decay)
+STEP_OPTS = [(None, 10, 0.2), ("scalar", 1, 0.2), ("wide", 2, 0.35), ("tensor", 10, 0.35), ("delta", 2, 0.2)]
+
+
+@pytest.mark.parametrize("bounds,ls_iter,decay", STEP_OPTS, ids=[f"{b}_ls{i}_d{d}" for b, i, d in STEP_OPTS])
+@pytest.mark.parametrize("name,dtype,B,bulk", STEP_BATCHES,
+                         ids=[f"{s}_{DT[d]}_B{b}" for s, d, b, _ in STEP_BATCHES])
+def test_fused_step_matches_oracle(name, dtype, B, bulk, bounds, ls_iter, decay):
+    from mpc.pytorch_b200 import _lib
+    W, is_bulk = _layout(name, B, dtype)
+    ppw = 5 if name == "cartpole" else 8
+    assert is_bulk == bulk and B % W != 0 and (B % W) % ppw != 0
+    T = 15
+    case = step_case(name, B, T, dtype, bounds, ls_iter, decay, 500 + B)
+    r, plan = _run_step(name, T, case[0], case[1], dtype)
+    tag = f"{name} {DT[dtype]} B={B} T={T} {bounds} ls={ls_iter} decay={decay}"
+    assert plan & _lib.PLAN_GENERIC, f"{tag}: plan {plan}"
+    check_step(tag, r, case, dtype)
+
+
+@pytest.mark.parametrize("dtype", [F64, F32], ids=["f64", "f32"])
+@pytest.mark.parametrize("name", SYSTEMS)
+def test_fused_step_cases_exercise_the_line_search_and_the_clamp(name, dtype):
+    """The step cases above are not vacuous, for each system and dtype, over the batches they use: in every bound
+    regime with more than one line-search pass some compared problems end with a decayed alpha; with one pass
+    (where alpha is restored at the end) some first passes are worse than the nominal; with bounds wider than the
+    clamp some controls go beyond it, where the dynamics see the clamped value."""
+    for bounds, ls_iter, decay in STEP_OPTS:
+        decayed = worse_first = beyond = 0
+        for s, d, B, _ in STEP_BATCHES:
+            if (s, d) != (name, dtype):
+                continue
+            case = step_case(name, B, 15, dtype, bounds, ls_iter, decay, 500 + B)
+            _, _, o64, trace, _ = case
+            keep = _f32_compared(case) if dtype == F32 else torch.ones(B, dtype=torch.bool)
+            decayed += int((o64.alphas[keep] < 1).sum())
+            worse_first += int((trace[0][keep] > 0).sum())
+            beyond += int((o64.new_u.abs() > PHYS[name]["clamp"]).sum())
+        tag = f"{name} {DT[dtype]} {bounds}"
+        assert (decayed if ls_iter > 1 else worse_first) > 0, f"{tag}: the line search never engages"
+        if bounds == "wide":
+            assert beyond > 0, f"{tag}: no control beyond the clamp"
+
+
+@functools.lru_cache(maxsize=None)
+def _gain_switch(n, dtype):
+    """First horizon at which the generic kernel (known-system instance (n, 1)) keeps its gains in Ks/ks."""
+    from mpc.pytorch_b200 import _lib
+    from tests.test_horizon_paths_gpu import _first_true, _probe_step
+    return _first_true(lambda T: not _probe_step(n, 1, dtype, T, 1, True) & _lib.PLAN_GAINS_SMEM)
+
+
+@pytest.mark.parametrize("name", SYSTEMS)
+def test_fused_step_on_both_sides_of_the_gain_store_switch(name):
+    """float64, one horizon below and one at the switch where the gains leave shared memory for the caller's
+    Ks/ks buffer (found on the device): the plan says so, and both match the oracle."""
+    from mpc.pytorch_b200 import _lib
+    n, B = PHYS[name]["n"], 13
+    Ts = _gain_switch(n, F64)
+    assert Ts is not None and 2 < Ts <= 1024, Ts
+    for T in (Ts - 1, Ts):
+        case = step_case(name, B, T, F64, "scalar", 4, 0.3, 700 + T, calm=True)
+        r, plan = _run_step(name, T, case[0], case[1], F64)
+        tag = f"{name} f64 B={B} T={T} (switch {Ts})"
+        assert plan & _lib.PLAN_GENERIC, tag
+        assert bool(plan & _lib.PLAN_GAINS_SMEM) == (T < Ts), f"{tag}: plan {plan}"
+        check_step(tag, r, case, F64)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# MPC.forward: the known system (three kernels per iteration) against the same physics as an opaque Module
+# ------------------------------------------------------------------------------------------------------------------
+def _mpc_pair(dx, x0, B, T, bounds, lqr_iter=6):
+    from mpc.pytorch_b200 import MPC, QuadCost, GradMethods
+
+    class Opaque(torch.nn.Module):                      # hides mpcb200_kind: the generic Module path
+        def forward(self, x, u):
+            return dx(x, u)
+
+    n = dx.n_state
+    q, p = dx.get_true_obj()
+    Q = torch.diag(q).double().expand(T, B, n + 1, n + 1).contiguous().to(DEV)
+    pp = p.double().expand(T, B, n + 1).contiguous().to(DEV)
+    kw = dict(u_lower=-bounds, u_upper=bounds, lqr_iter=lqr_iter, verbose=-1, exit_unconverged=False,
+              detach_unconverged=False, linesearch_decay=0.3, max_linesearch_iter=4,
+              grad_method=GradMethods.AUTO_DIFF, eps=1e-9)
+    a = MPC(n, 1, T, **kw)(x0.to(DEV), QuadCost(Q, pp), dx)
+    b = MPC(n, 1, T, **kw)(x0.to(DEV), QuadCost(Q, pp), Opaque())
+    return a, b
+
+
+def _assert_mpc_equal(tag, a, b):
+    (xa, ua, ca), (xb, ub, cb) = a, b
+    assert maxdiff(ua, ub) < 1e-7 * max(1.0, float(ub.abs().max())), f"{tag}: u {maxdiff(ua, ub):.3e}"
+    assert maxdiff(xa, xb) < 1e-7 * max(1.0, float(xb.abs().max())), f"{tag}: x {maxdiff(xa, xb):.3e}"
+    assert maxdiff(ca, cb) < 1e-8 * max(1.0, float(cb.abs().max())), f"{tag}: costs {maxdiff(ca, cb):.3e}"
+
+
+MPC_CASES = [(1, 100), (13, 25), (300, 2), (300, 25)]
+
+
+@pytest.mark.parametrize("bounds", ["in", "wide"])
+@pytest.mark.parametrize("B,T", MPC_CASES, ids=[f"B{b}_T{t}" for b, t in MPC_CASES])
+@pytest.mark.parametrize("name", SYSTEMS)
+def test_mpc_known_system_equals_module_path(name, B, T, bounds):
+    dx = _module(name)
+    clamp = PHYS[name]["clamp"]
+    x0 = _states(name, B, 900 + B + T)
+    a, b = _mpc_pair(dx, x0, B, T, (0.8 if bounds == "in" else 2.0) * clamp)
+    _assert_mpc_equal(f"{name} B={B} T={T} bounds {bounds}", a, b)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# parameters changed in place between solves
+# ------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("name", SYSTEMS)
+def test_kernels_follow_parameter_edits_between_solves(name):
+    """CUDA parameters edited between solves by an optimizer step, a no_grad copy_, .data[i] = and reassignment:
+    after each edit the kernel rollout and Jacobians equal the module's own forward and autograd, and MPC.forward
+    with the known system equals the same physics run as an opaque Module."""
+    from mpc.pytorch_b200.dynamics import dyn_linearize_raw, dyn_rollout_raw
+    from tests.test_known_systems_cpu import EDIT_ROUTES
+    dx = _module(name, params=torch.tensor(PHYS[name]["params"], dtype=F64, device=DEV).requires_grad_(True),
+                 device=DEV)
+    B, T = 9, 12
+    x0 = _states(name, B, 77)
+    u = _controls(name, T, B, F64, 78)
+    base = torch.tensor(PHYS[name]["params"], dtype=F64)
+    for k, (route, edit) in enumerate(EDIT_ROUTES):
+        _mpc_pair(dx, x0, B, T, 2.0 * PHYS[name]["clamp"], lqr_iter=2)      # a solve before the edit
+        edit(dx, (base * (1.0 + 0.15 * (k + 1))).to(DEV))
+        prm = dx.mpcb200_params()
+        assert prm[:len(base)] == tuple(float(v) for v in dx.params.detach().cpu()), route
+        x = dyn_rollout_raw(dx.mpcb200_kind, prm, T, x0.to(DEV), u.to(DEV))
+        want = dx(x[:-1].reshape(-1, dx.n_state), u[:-1].reshape(-1, 1).to(DEV)).view(T - 1, B, -1)
+        assert maxdiff(x[1:], want) <= 1e-12 * max(1.0, float(want.abs().max())), f"{route}: rollout"
+        F, f = dyn_linearize_raw(dx.mpcb200_kind, prm, T, x, u.to(DEV))
+        _, R, S = _jac(dx, x[:-1].reshape(-1, dx.n_state).detach(), u[:-1].reshape(-1, 1).to(DEV))
+        Fw = torch.cat((R, S), 2).view(T - 1, B, dx.n_state, -1)
+        assert maxdiff(F, Fw) <= 1e-11 * max(1.0, float(Fw.abs().max())), f"{route}: Jacobians"
+        a, b = _mpc_pair(dx, x0, B, T, 2.0 * PHYS[name]["clamp"], lqr_iter=3)
+        _assert_mpc_equal(f"{name} after {route}", a, b)
