@@ -4,7 +4,9 @@ The product path has NO CPU fallback: if the library is missing, or a tensor is
 not a CUDA tensor, the calls here raise.  torch is used only for device memory
 and the current stream.
 """
+import contextlib
 import ctypes
+import functools
 import os
 
 import torch
@@ -111,6 +113,19 @@ def lib():
     return L
 
 
+_DTYPE_SUFFIX = {torch.float32: "_f32", torch.float64: "_f64"}
+
+
+@functools.cache                # the library is loaded once per process: a symbol never changes
+def entry(name, dtype):
+    """The `name`_f32 or `name`_f64 symbol for tensors of `dtype`.  The outputs are allocated in the inputs' dtype, so
+    any other dtype would hand a kernel buffers of the wrong element size: refuse it."""
+    suffix = _DTYPE_SUFFIX.get(dtype)
+    if suffix is None:
+        raise MpcB200Error(f"unsupported dtype {dtype}")
+    return getattr(lib(), name + suffix)
+
+
 def check(rc, what):
     if rc != 0:
         raise MpcB200Error(f"{what} failed: [{rc}] {lib().mpcb200_strerror(rc).decode()}")
@@ -156,3 +171,10 @@ def ptr_view(t):
 
 def stream_handle(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def _on_device(dev):
+    """`torch.cuda.device(dev)` only when `dev` is not already current (the guard costs microseconds)."""
+    if dev.index is None or dev.index == torch.cuda.current_device():
+        return contextlib.nullcontext()
+    return torch.cuda.device(dev)

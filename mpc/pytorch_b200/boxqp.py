@@ -15,12 +15,11 @@ reference uses an LU, which also accepts a non-symmetric ``H``).
 import torch
 
 from . import _lib
-from ._lib import MpcB200Error, check, ptr, stream_handle
+from ._lib import MpcB200Error, _on_device, check, ptr, stream_handle
 
 
 def pnqp(H, q, lower, upper, x_init=None, n_iter=20):
-    if not H.is_cuda:
-        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
+    fn = _lib.entry("mpcb200_pnqp", H.dtype)
     if H.dim() != 3 or H.shape[1] != H.shape[2]:
         raise MpcB200Error(f"H: expected [B,n,n], got {tuple(H.shape)}")
     B, n, _ = H.size()
@@ -30,10 +29,11 @@ def pnqp(H, q, lower, upper, x_init=None, n_iter=20):
                 raise MpcB200Error(f"{nm}: expected a tensor on {H.device}, got {t_.device}")
             if tuple(t_.shape) not in ((B, n), (n,), (1, n)):
                 raise MpcB200Error(f"{nm}: expected shape {(B, n)}, got {tuple(t_.shape)}")
+    if not H.is_cuda:
+        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
     dtype, dev = H.dtype, H.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        max_n = L.mpcb200_pnqp_max_n(4 if dtype == torch.float32 else 8)
+    with _on_device(dev):
+        max_n = _lib.lib().mpcb200_pnqp_max_n(H.element_size())
     if n > max_n:
         raise MpcB200Error(f"pnqp solves QPs with n <= {max_n} in {dtype} on {dev} (got n = {n}): the QP of one "
                            "thread block must fit its shared memory")
@@ -46,8 +46,7 @@ def pnqp(H, q, lower, upper, x_init=None, n_iter=20):
     If = torch.empty(B, n, dtype=torch.uint8, device=dev)
     iters = torch.empty(B, dtype=torch.int32, device=dev)
     status = torch.empty(B, dtype=torch.int32, device=dev)
-    fn = L.mpcb200_pnqp_f32 if dtype == torch.float32 else L.mpcb200_pnqp_f64
-    with torch.cuda.device(dev):
+    with _on_device(dev):
         rc = fn(B, n, ptr(Hc), ptr(qc), ptr(lo), ptr(hi), ptr(x0), int(n_iter), ptr(x), ptr(Hf), ptr(If),
                 ptr(iters), ptr(status), stream_handle(dev))
     check(rc, "mpcb200_pnqp")

@@ -20,7 +20,7 @@ import torch
 from torch.nn import Module
 
 from . import _lib
-from ._lib import MpcB200Error, check, ptr, stream_handle
+from ._lib import MpcB200Error, _on_device, check, ptr, stream_handle
 
 DYN_LINEAR, DYN_CARTPOLE, DYN_PENDULUM = 0, 1, 2
 DYN_DIMS = {DYN_CARTPOLE: (5, 1), DYN_PENDULUM: (3, 1)}       # (n_state, n_ctrl) of each known system
@@ -181,10 +181,10 @@ def _check_dyn_shapes(kind, T, what, x, x_shape, u):
         raise MpcB200Error(f"u: expected shape {(T, B, m)} (n_ctrl = {m}), got {tuple(u.shape)}")
     if x.dtype not in (torch.float32, torch.float64):
         raise MpcB200Error(f"unsupported dtype {x.dtype}")
-    if not x.is_cuda:
-        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
     if u.device != x.device:
         raise MpcB200Error(f"u is on {u.device}, {what} on {x.device}")
+    if not x.is_cuda:
+        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
     return B, n, m
 
 
@@ -195,9 +195,8 @@ def dyn_rollout_raw(kind, params, T, x_init, u):
     x0 = x_init.detach().to(dtype).contiguous()
     u_ = u.detach().to(dtype).contiguous()
     x = torch.empty(T, B, n, dtype=dtype, device=dev)
-    L = _lib.lib()
-    fn = L.mpcb200_dyn_rollout_f32 if dtype == torch.float32 else L.mpcb200_dyn_rollout_f64
-    with torch.cuda.device(dev):
+    fn = _lib.entry("mpcb200_dyn_rollout", dtype)
+    with _on_device(dev):
         rc = fn(kind, _dyn_array(params), B, T, ptr(x0), ptr(u_), ptr(x), stream_handle(dev))
     check(rc, "mpcb200_dyn_rollout")
     return x
@@ -212,9 +211,8 @@ def dyn_linearize_raw(kind, params, T, x, u):
     u_ = u.detach().to(dtype).contiguous()
     F = torch.empty(T - 1, B, n, n + m, dtype=dtype, device=dev)
     f = torch.empty(T - 1, B, n, dtype=dtype, device=dev)
-    L = _lib.lib()
-    fn = L.mpcb200_dyn_linearize_f32 if dtype == torch.float32 else L.mpcb200_dyn_linearize_f64
-    with torch.cuda.device(dev):
+    fn = _lib.entry("mpcb200_dyn_linearize", dtype)
+    with _on_device(dev):
         rc = fn(kind, _dyn_array(params), B, T, ptr(x_), ptr(u_), ptr(F), ptr(f), stream_handle(dev))
     check(rc, "mpcb200_dyn_linearize")
     return F, f

@@ -13,7 +13,7 @@ from torch.autograd import Function
 from torch.nn import Module
 
 from . import _lib
-from ._lib import Dims, Params, MpcB200Error, check, ptr, ptr_view, stream_handle
+from ._lib import Dims, Params, MpcB200Error, _on_device, check, ptr, ptr_view, stream_handle
 
 PNQP_MAX_ITER = 20  # reference passes n_iter=20 (mpc/lqr_step.py:137)
 
@@ -38,15 +38,64 @@ def _dense(t, dtype=None):
     return t if t.is_contiguous() else t.contiguous()
 
 
-def _expect(name, t, shape, dev):
-    """The kernels read raw device pointers: a wrong shape or a tensor on another GPU would be an
-    out-of-bounds read, so fail here like the reference's indexing / eclamp size asserts would."""
-    if t is None:
-        return
-    if tuple(t.shape) != tuple(shape):
-        raise MpcB200Error(f"{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
-    if t.device != dev:
-        raise MpcB200Error(f"{name}: expected a tensor on {dev}, got {t.device}")
+def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=None, exact=False):
+    """Check, on tensor metadata alone, the tensors a raw call hands to the kernels; returns the batch size B.
+    The kernels read raw device pointers: a wrong dtype, shape or device would be an out-of-bounds access, so fail
+    here like the reference's indexing / eclamp size asserts would.  `named`: (name, tensor or None, layout), the
+    layout one of "TBpp", "TBp", "TBn", "TBm", "Bn" (p = n+m).  The first tensor leads: the outputs are allocated in
+    its dtype, and it fixes B and the device.  F [T-1|T,B,n,p] and f [T-1|T,B,n] may be absent or empty (F only for
+    T = 1); tensor bounds and u_zero_I are [T,B,m].  `exact`: the call runs in-kernel dynamics, which need an exact
+    (n, m) kernel instance."""
+    lead_name, lead, lead_layout = named[0]
+    if lead.dtype not in (torch.float32, torch.float64):
+        raise MpcB200Error(f"unsupported dtype {lead.dtype}")
+    if lead.dim() != len(lead_layout):
+        raise MpcB200Error(f"{lead_name}: expected shape [{','.join(lead_layout)}], got {tuple(lead.shape)}")
+    B, p = lead.shape[lead_layout.index("B")], n + m
+    shape_of = {"TBpp": (T, B, p, p), "TBp": (T, B, p), "TBn": (T, B, n), "TBm": (T, B, m), "Bn": (B, n)}
+    checked = []
+    for name, t, layout in named:
+        if t is not None:
+            if t.shape != shape_of[layout]:
+                raise MpcB200Error(f"{name}: expected shape {shape_of[layout]}, got {tuple(t.shape)}")
+            checked.append((name, t))
+    for name, t, shape in (("F", F, (B, n, p)), ("f", f, (B, n))):
+        if not _is_empty(t):
+            if t.shape[1:] != shape or t.shape[0] not in (T - 1, T):
+                raise MpcB200Error(f"{name}: expected shape (T-1 or T, {', '.join(map(str, shape))}), "
+                                   f"got {tuple(t.shape)}")
+            checked.append((name, t))
+    if _is_empty(F) and T > 1:
+        raise MpcB200Error("F is required for T > 1")
+    u_lower, u_upper = bounds
+    if (u_lower is None) != (u_upper is None):
+        raise MpcB200Error("u_lower and u_upper must be given together")
+    for name, t in (("u_lower", u_lower), ("u_upper", u_upper), ("u_zero_I", u_zero_I)):
+        if isinstance(t, torch.Tensor):
+            if t.shape != shape_of["TBm"]:
+                raise MpcB200Error(f"{name}: expected shape {shape_of['TBm']}, got {tuple(t.shape)}")
+            checked.append((name, t))
+    if exact and _pick_instance(n, m) != (n, m):
+        raise MpcB200Error("in-kernel dynamics need an exact (n_state, n_ctrl) kernel instance")
+    dev = lead.device
+    for name, t in checked:
+        if t.device != dev:
+            raise MpcB200Error(f"{name}: expected a tensor on {dev}, got {t.device}")
+    if not lead.is_cuda:
+        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
+    return B
+
+
+def _bounds(u_lower, u_upper, shape, dtype, dev, padded=False):
+    """(kind, s_lo, s_hi, lo_t, hi_t) of the kernels' control box: none (0), two scalars (1) or two `shape` tensors
+    (2).  A padded problem always takes tensors, which the caller widens: its padded controls get their own box."""
+    if u_lower is None:
+        return 0, 0.0, 0.0, None, None
+    if isinstance(u_lower, float) and isinstance(u_upper, float) and not padded:
+        return 1, u_lower, u_upper, None, None
+    lo_t, hi_t = [torch.full(shape, b, dtype=dtype, device=dev) if isinstance(b, float) else _dense(b, dtype)
+                  for b in (u_lower, u_upper)]
+    return 2, 0.0, 0.0, lo_t, hi_t
 
 
 def _time_strided(t, dtype):
@@ -54,8 +103,6 @@ def _time_strided(t, dtype):
     [B, ...] slices are contiguous: dense -> 0; stride-0 over time (`x.unsqueeze(0).expand(T, ...)`, an LTI
     `F`, reference mpc/mpc.py:205-226) -> MPCB200_TIME_INVARIANT; any other 16-byte aligned time stride -> it.
     Everything else (batch-expanded, transposed, ...) is copied to a dense tensor, as before."""
-    if t is None:
-        return None, 0
     if t.dtype != dtype:
         t = t.to(dtype)
     if t.requires_grad:
@@ -142,20 +189,33 @@ class _Pad:
         out[..., : self.m] = u
         return out
 
+    def stage(self, t, dtype, widen):
+        """(tensor, mpcb200_dims time-stride field) of a [T, B, ...] input (C, c, F, f); (None, 0) when it is absent
+        or empty.  An exact instance keeps the time stride (_time_strided); a padded one reads a dense `widen` copy."""
+        if t is None or t.nelement() == 0:
+            return None, 0
+        if not self.active:
+            return _time_strided(t, dtype)
+        return widen(_dense(t, dtype)), 0
 
-class _on_device:
-    """`torch.cuda.device(dev)` only when `dev` is not already current (the guard costs microseconds)."""
+    # the inverse of the widening, for outputs (None stays None)
+    def crop_n(self, x):          # [..., N] -> [..., n]
+        return x[..., : self.n] if self.active and x is not None else x
 
-    def __init__(self, dev):
-        self.guard = None if dev.index is None or dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
+    def crop_m(self, u):          # [..., M] -> [..., m]
+        return u[..., : self.m] if self.active and u is not None else u
 
-    def __enter__(self):
-        if self.guard is not None:
-            self.guard.__enter__()
+    def crop_mn(self, K):         # [..., M, N] -> [..., m, n]
+        return K[..., : self.m, : self.n] if self.active and K is not None else K
 
-    def __exit__(self, *exc):
-        if self.guard is not None:
-            self.guard.__exit__(*exc)
+    def crop_p(self, c):          # [..., P] -> [..., p]
+        return c[..., self.idx] if self.active else c
+
+    def crop_pp(self, C):         # [..., P, P] -> [..., p, p]
+        return C[..., self.idx[:, None], self.idx[None, :]] if self.active else C
+
+    def crop_np(self, F):         # [..., N, P] -> [..., n, p]
+        return F[..., : self.n, self.idx] if self.active and F is not None else F
 
 
 # ----------------------------------------------------------------------------------------------
@@ -168,80 +228,26 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
     """Run the step kernel.  Returns a dict of device tensors:
     new_x,new_u,costs,full_du_norm,alphas (do_rollout) and, on request, Ks,ks,qp_iters,
     free_mask,status."""
-    if not C.is_cuda:
-        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
-    dtype, dev = C.dtype, C.device
-    if dtype not in (torch.float32, torch.float64):
-        raise MpcB200Error(f"unsupported dtype {dtype}")
     n, m = n_state, n_ctrl
-    if C.dim() != 4:
-        raise MpcB200Error(f"C: expected [T,B,n+m,n+m], got {tuple(C.shape)}")
-    B = C.shape[1]
-    p = n + m
-    _expect("C", C, (T, B, p, p), dev)
-    _expect("c", c, (T, B, p), dev)
-    if not _is_empty(F):
-        if F.dim() != 4 or F.shape[0] not in (T - 1, T):
-            raise MpcB200Error(f"F: expected [T-1|T,B,n,n+m], got {tuple(F.shape)}")
-        _expect("F", F, (F.shape[0], B, n, p), dev)
-    elif T > 1:
-        raise MpcB200Error("F is required for T > 1")
-    if not _is_empty(f):
-        if f.dim() != 3 or f.shape[0] not in (T - 1, T):     # util.get_traj wants f.shape == F.shape[:3]
-            raise MpcB200Error(f"f: expected [T-1|T,B,n], got {tuple(f.shape)}")
-        _expect("f", f, (f.shape[0], B, n), dev)
-    _expect("x_init", x_init, (B, n), dev)
-    _expect("current_x", cur_x, (T, B, n), dev)
-    _expect("current_u", cur_u, (T, B, m), dev)
-    if (u_lower is None) != (u_upper is None):
-        raise MpcB200Error("u_lower and u_upper must be given together")
-    for nm, bnd in (("u_lower", u_lower), ("u_upper", u_upper)):
-        if torch.is_tensor(bnd):
-            _expect(nm, bnd, (T, B, m), dev)
-    if u_zero_I is not None:
-        _expect("u_zero_I", u_zero_I, (T, B, m), dev)
+    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("current_x", cur_x, "TBn"),
+                  ("current_u", cur_u, "TBm"), F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
+                  exact=dyn is not None)
+    dtype, dev = C.dtype, C.device
     N, M = _pick_instance(n, m)
     pad = _Pad(n, m, N, M, dev)
-
-    ts = dict(C=0, c=0, F=0, f=0)
+    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
+    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
+    x0_, cx_, cu_ = _dense(x_init, dtype), _dense(cur_x, dtype), _dense(cur_u, dtype)
+    bounds_kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev, pad.active)
+    zmask = (u_zero_I != 0).to(torch.uint8).contiguous() if u_zero_I is not None else None
     if pad.active:
-        C_, c_ = _dense(C, dtype), _dense(c, dtype)
-        F_ = _dense(F, dtype) if not _is_empty(F) else None
-        f_ = _dense(f, dtype) if not _is_empty(f) else None
-    else:       # honour time strides (time-invariant cost / LTI dynamics are read once, not T times)
-        C_, ts["C"] = _time_strided(C, dtype)
-        c_, ts["c"] = _time_strided(c, dtype)
-        F_, ts["F"] = _time_strided(F, dtype) if not _is_empty(F) else (None, 0)
-        f_, ts["f"] = _time_strided(f, dtype) if not _is_empty(f) else (None, 0)
-    x0_ = _dense(x_init, dtype) if x_init is not None else None
-    cx_, cu_ = _dense(cur_x, dtype), _dense(cur_u, dtype)
-    F_T = F_.shape[0] if F_ is not None else T - 1
-    bounds_kind = 0
-    lo_t = hi_t = None
-    s_lo = s_hi = 0.0
-    if u_lower is not None:
-        if isinstance(u_lower, float) and isinstance(u_upper, float) and not pad.active:
-            bounds_kind, s_lo, s_hi = 1, u_lower, u_upper
-        else:
-            bounds_kind = 2
-            lo_t = (torch.full((T, B, m), u_lower, dtype=dtype, device=dev)
-                    if isinstance(u_lower, float) else _dense(u_lower, dtype))
-            hi_t = (torch.full((T, B, m), u_upper, dtype=dtype, device=dev)
-                    if isinstance(u_upper, float) else _dense(u_upper, dtype))
-    zmask = None
-    if u_zero_I is not None:
-        zmask = (u_zero_I != 0).to(torch.uint8).contiguous()
-
-    if pad.active:
-        C_, c_ = pad.mat_pp(C_), pad.vec_p(c_)
-        F_ = pad.mat_np(F_) if F_ is not None else None
-        f_ = pad.vec_n(f_) if f_ is not None else None
         x0_ = pad.vec_n(x0_) if x0_ is not None else None
         cx_, cu_ = pad.vec_n(cx_), pad.vec_m(cu_)
         if lo_t is not None:
             lo_t, hi_t = pad.vec_m(lo_t, -1.0), pad.vec_m(hi_t, 1.0)
         if zmask is not None:
             zmask = pad.vec_m(zmask, 0)
+    F_T = F_.shape[0] if F_ is not None else T - 1
 
     out = {}
     new_x = new_u = costs = fdn = alphas = None
@@ -264,17 +270,14 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
                 has_zero_mask=int(zmask is not None), has_delta_u=int(delta_u is not None),
                 max_ls_iter=int(max_linesearch_iter), pnqp_max_iter=PNQP_MAX_ITER,
                 do_rollout=int(bool(do_rollout)), dynamics_kind=int(dyn[0]) if dyn is not None else 0,
-                C_tstride=ts["C"], c_tstride=ts["c"], F_tstride=ts["F"], f_tstride=ts["f"])
-    if dyn is not None and pad.active:
-        raise MpcB200Error("in-kernel dynamics need an exact (n_state, n_ctrl) kernel instance")
-    L = _lib.lib()
+                C_tstride=tsC, c_tstride=tsc, F_tstride=tsF, f_tstride=tsf)
     need_gains = want_gains or not do_rollout
     if not need_gains:
         # long horizons do not fit shared memory: the kernel then keeps gains in a caller buffer
-        key = (N, M, T, C_.element_size())
+        key = (N, M, T, C.element_size())
         fits = _smem_fits_cache.get(key)
         if fits is None:
-            fits = not L.mpcb200_step_prefers_workspace(ctypes.byref(dims), C_.element_size())
+            fits = not _lib.lib().mpcb200_step_prefers_workspace(ctypes.byref(dims), C.element_size())
             _smem_fits_cache[key] = fits
         need_gains = not fits
     if need_gains:
@@ -286,7 +289,7 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
     if dyn is not None:
         for i, v in enumerate(dyn[1]):
             params.dyn[i] = float(v)
-    fn = L.mpcb200_lqr_step_f32 if dtype == torch.float32 else L.mpcb200_lqr_step_f64
+    fn = _lib.entry("mpcb200_lqr_step", dtype)
     with _on_device(dev):
         rc = fn(ctypes.byref(dims), ctypes.byref(params), ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr_view(f_),
                 ptr(x0_), ptr(cx_), ptr(cu_), ptr(lo_t), ptr(hi_t), ptr(zmask), ptr(new_x), ptr(new_u),
@@ -294,45 +297,31 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
                 ptr(Ks), ptr(ks), stream_handle(dev))
     check(rc, "mpcb200_lqr_step")
     if do_rollout:
-        out.update(new_x=new_x[..., :n] if pad.active else new_x,
-                   new_u=new_u[..., :m] if pad.active else new_u,
-                   costs=costs, full_du_norm=fdn, alphas=alphas)
+        out.update(new_x=pad.crop_n(new_x), new_u=pad.crop_m(new_u), costs=costs, full_du_norm=fdn, alphas=alphas)
         if du_first is not None:
-            out["du_first"] = du_first[..., :m] if pad.active else du_first
+            out["du_first"] = pad.crop_m(du_first)
     if Ks is not None:
-        out.update(Ks=Ks[..., :m, :n] if pad.active else Ks, ks=ks[..., :m] if pad.active else ks)
+        out.update(Ks=pad.crop_mn(Ks), ks=pad.crop_m(ks))
     if want_stats:
-        out.update(qp_iters=qp_iters, free_mask=free_mask[..., :m] if pad.active else free_mask,
-                   status=status)
+        out.update(qp_iters=qp_iters, free_mask=pad.crop_m(free_mask), status=status)
     return out
 
 
 def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_df, f_T=None):
     """Run the gradient-assembly kernel; returns (dx_init, dC, dc, dF, df|None)."""
-    dtype, dev = C.dtype, C.device
     n, m = n_state, n_ctrl
-    B = C.shape[1]
-    p = n + m
-    _expect("C", C, (T, B, p, p), dev)
-    _expect("c", c, (T, B, p), dev)
-    if not _is_empty(F):
-        _expect("F", F, (F.shape[0], B, n, p), dev)
-        if F.shape[0] not in (T - 1, T):
-            raise MpcB200Error(f"F: expected T-1 or T time slices, got {F.shape[0]}")
-    for nm, t_, sh in (("new_x", new_x, (T, B, n)), ("new_u", new_u, (T, B, m)), ("dx", dx, (T, B, n)),
-                       ("du", du, (T, B, m)), ("dl_dx", dl_dx, (T, B, n))):
-        _expect(nm, t_, sh, dev)
+    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("new_x", new_x, "TBn"), ("new_u", new_u, "TBm"),
+                  ("dx", dx, "TBn"), ("du", du, "TBm"), ("dl_dx", dl_dx, "TBn"), F=F)
+    dtype, dev = C.dtype, C.device
     N, M = _pick_instance(n, m)
     pad = _Pad(n, m, N, M, dev)
-    C_, c_ = _dense(C, dtype), _dense(c, dtype)
-    F_ = _dense(F, dtype) if not _is_empty(F) else None
+    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
+    F_, tsF = pad.stage(F, dtype, pad.mat_np)
     nx_, nu_ = _dense(new_x, dtype), _dense(new_u, dtype)
     dx_, du_, r_ = _dense(dx, dtype), _dense(du, dtype), _dense(dl_dx, dtype)
-    F_T = F_.shape[0] if F_ is not None else 0
     if pad.active:
-        C_, c_ = pad.mat_pp(C_), pad.vec_p(c_)
-        F_ = pad.mat_np(F_) if F_ is not None else None
         nx_, nu_, dx_, du_, r_ = pad.vec_n(nx_), pad.vec_m(nu_), pad.vec_n(dx_), pad.vec_m(du_), pad.vec_n(r_)
+    F_T = F_.shape[0] if F_ is not None else 0
     P = N + M
     dx_init = torch.empty(B, N, dtype=dtype, device=dev)
     dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
@@ -345,22 +334,14 @@ def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_
         df[T - 1].zero_()
     dims = Dims(B=B, T=T, n=N, m=M, F_T=F_T if F_ is not None else T - 1, has_f=int(want_df),
                 bounds_kind=0, has_zero_mask=0, has_delta_u=0, max_ls_iter=1, pnqp_max_iter=1,
-                do_rollout=0)
-    L = _lib.lib()
-    fn = L.mpcb200_lqr_grad_f32 if dtype == torch.float32 else L.mpcb200_lqr_grad_f64
+                do_rollout=0, C_tstride=tsC, c_tstride=tsc, F_tstride=tsF)
+    fn = _lib.entry("mpcb200_lqr_grad", dtype)
     ws = torch.empty(2 * T * B * N, dtype=dtype, device=dev)     # costates: enables the two-kernel path
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ptr(C_), ptr(c_), ptr(F_), ptr(nx_), ptr(nu_), ptr(dx_), ptr(du_),
-                ptr(r_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(ws), stream_handle(dev))
+        rc = fn(ctypes.byref(dims), ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr(nx_), ptr(nu_), ptr(dx_),
+                ptr(du_), ptr(r_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(ws), stream_handle(dev))
     check(rc, "mpcb200_lqr_grad")
-    if pad.active:
-        i = pad.idx
-        dx_init = dx_init[:, :n]
-        dC = dC[:, :, i[:, None], i[None, :]]
-        dc = dc[:, :, i]
-        dF = dF[:, :, :n][..., i] if dF is not None else None
-        df = df[..., :n] if df is not None else None
-    return dx_init, dC, dc, dF, df
+    return pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df)
 
 
 _ws_cache = threading.local()
@@ -388,40 +369,27 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
     returns (dx_init, dC, dc, dF, df|None), or None when this shape needs the general multi-call path
     (zero-padded instance, horizon too long for the shared-memory gain store).  `validated`: the tensors are the
     ones LQRStepFn.forward checked and saved plus autograd's gradients of its outputs (shapes follow), so the
-    shape / device checks are not repeated on the backward path."""
-    dtype, dev = C.dtype, C.device
+    checks are not repeated on the backward path."""
     n, m = n_state, n_ctrl
+    if not validated:
+        _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("new_x", new_x, "TBn"), ("new_u", new_u, "TBm"),
+                  ("dl_dx", dl_dx, "TBn"), ("dl_du", dl_du, "TBm"), F=F, bounds=(u_lower, u_upper))
     if _pick_instance(n, m) != (n, m) or _is_empty(F):
         return None
+    dtype, dev = C.dtype, C.device
     B = C.shape[1]
     p = n + m
     F_T = F.shape[0]
-    if not validated:
-        _expect("C", C, (T, B, p, p), dev)
-        _expect("c", c, (T, B, p), dev)
-        _expect("F", F, (F_T, B, n, p), dev)
-        for nm, t_, sh in (("new_x", new_x, (T, B, n)), ("new_u", new_u, (T, B, m)), ("dl_dx", dl_dx, (T, B, n)),
-                           ("dl_du", dl_du, (T, B, m))):
-            _expect(nm, t_, sh, dev)
-    kind, s_lo, s_hi, lo_t, hi_t = 0, 0.0, 0.0, None, None
-    if u_lower is not None:
-        if isinstance(u_lower, float) and isinstance(u_upper, float):
-            kind, s_lo, s_hi = 1, u_lower, u_upper
-        else:
-            kind = 2
-            lo_t = (torch.full((T, B, m), u_lower, dtype=dtype, device=dev) if isinstance(u_lower, float)
-                    else _dense(u_lower, dtype))
-            hi_t = (torch.full((T, B, m), u_upper, dtype=dtype, device=dev) if isinstance(u_upper, float)
-                    else _dense(u_upper, dtype))
-            _expect("u_lower", lo_t, (T, B, m), dev)
-            _expect("u_upper", hi_t, (T, B, m), dev)
+    kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev)
     (C_, tsC), (c_, tsc), (F_, tsF) = _time_strided(C, dtype), _time_strided(c, dtype), _time_strided(F, dtype)
-    L = _lib.lib()
     esz = C.element_size()
-    # the ctypes structs, the shared-memory fit and the workspace size depend only on this key: build them once
+    # the entry point, the ctypes structs, the shared-memory fit and the workspace size depend only on this key:
+    # build them once
     key = (n, m, T, B, F_T, esz, kind, s_lo, s_hi, bool(want_df), tsC, tsc, tsF)
     plan = _adj_plans.get(key)
     if plan is None:
+        fn = _lib.entry("mpcb200_lqr_adjoint", dtype)
+        L = _lib.lib()
         dims = Dims(B=B, T=T, n=n, m=m, F_T=F_T, has_f=int(want_df), bounds_kind=kind, has_zero_mask=0,
                     has_delta_u=0, max_ls_iter=10, pnqp_max_iter=PNQP_MAX_ITER, do_rollout=1,
                     C_tstride=tsC, c_tstride=tsc, F_tstride=tsF)
@@ -430,8 +398,8 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
         nbytes = L.mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), esz) if fits else 0
         if len(_adj_plans) > 256:
             _adj_plans.clear()
-        plan = _adj_plans[key] = (fits, dims, params, ctypes.byref(dims), ctypes.byref(params), nbytes)
-    fits, dims, params, dims_ref, params_ref, nbytes = plan
+        plan = _adj_plans[key] = (fits, fn, dims, params, ctypes.byref(dims), ctypes.byref(params), nbytes)
+    fits, fn, dims, params, dims_ref, params_ref, nbytes = plan
     if not fits:
         return None
     nx_, nu_, gx_, gu_ = _dense(new_x, dtype), _dense(new_u, dtype), _dense(dl_dx, dtype), _dense(dl_du, dtype)
@@ -444,7 +412,6 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
     if want_df and f_T == T:
         df[T - 1].zero_()
     ws = _workspace(nbytes, dev)
-    fn = L.mpcb200_lqr_adjoint_f32 if dtype == torch.float32 else L.mpcb200_lqr_adjoint_f64
     with _on_device(dev):
         rc = fn(dims_ref, params_ref, ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr(nx_), ptr(nu_), ptr(gx_),
                 ptr(gu_), ptr(lo_t), ptr(hi_t), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(ws),
@@ -455,47 +422,24 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
 
 def rollout_raw(n_state, n_ctrl, T, x_init, u, F, f=None):
     """x = get_traj(T, u, x_init, LinDx(F, f)) in ONE kernel (reference mpc/util.py:102-126)."""
-    dtype, dev = x_init.dtype, x_init.device
-    if not x_init.is_cuda:
-        raise MpcB200Error("mpc.pytorch_b200 runs on CUDA tensors only (no CPU fallback)")
     n, m = n_state, n_ctrl
-    B = x_init.shape[0]
-    _expect("x_init", x_init, (B, n), dev)
-    _expect("u", u, (T, B, m), dev)
-    if not _is_empty(F):
-        if F.dim() != 4 or F.shape[0] not in (T - 1, T):
-            raise MpcB200Error(f"F: expected [T-1|T,B,n,n+m], got {tuple(F.shape)}")
-        _expect("F", F, (F.shape[0], B, n, n + m), dev)
-    elif T > 1:
-        raise MpcB200Error("F is required for T > 1")
-    if not _is_empty(f):
-        if f.shape[0] not in (T - 1, T):
-            raise MpcB200Error(f"f: expected [T-1|T,B,n], got {tuple(f.shape)}")
-        _expect("f", f, (f.shape[0], B, n), dev)
+    B = _validate(n, m, T, ("x_init", x_init, "Bn"), ("u", u, "TBm"), F=F, f=f)
+    dtype, dev = x_init.dtype, x_init.device
     N, M = _pick_instance(n, m)
     pad = _Pad(n, m, N, M, dev)
+    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
     x0_, u_ = _dense(x_init, dtype), _dense(u, dtype)
-    tsF = tsf = 0
-    if pad.active:
-        F_ = _dense(F, dtype) if not _is_empty(F) else None
-        f_ = _dense(f, dtype) if not _is_empty(f) else None
-    else:
-        F_, tsF = _time_strided(F, dtype) if not _is_empty(F) else (None, 0)
-        f_, tsf = _time_strided(f, dtype) if not _is_empty(f) else (None, 0)
     if pad.active:
         x0_, u_ = pad.vec_n(x0_), pad.vec_m(u_)
-        F_ = pad.mat_np(F_) if F_ is not None else None
-        f_ = pad.vec_n(f_) if f_ is not None else None
     x = torch.empty(T, B, N, dtype=dtype, device=dev)
     dims = Dims(B=B, T=T, n=N, m=M, F_T=F_.shape[0] if F_ is not None else T - 1, has_f=int(f_ is not None),
                 bounds_kind=0, has_zero_mask=0, has_delta_u=0, max_ls_iter=1, pnqp_max_iter=1, do_rollout=1,
                 F_tstride=tsF, f_tstride=tsf)
-    L = _lib.lib()
-    fn = L.mpcb200_rollout_f32 if dtype == torch.float32 else L.mpcb200_rollout_f64
+    fn = _lib.entry("mpcb200_rollout", dtype)
     with _on_device(dev):
         rc = fn(ctypes.byref(dims), ptr_view(F_), ptr_view(f_), ptr(x0_), ptr(u_), ptr(x), stream_handle(dev))
     check(rc, "mpcb200_rollout")
-    return x[..., :n] if pad.active else x
+    return pad.crop_n(x)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -602,22 +546,10 @@ class LQRStepFn(Function):
         ctx.o = o
         if o.no_op_forward:                                   # reference :278-282
             # nothing is computed here, but backward hands these tensors to the kernels as raw pointers:
-            # check shapes / devices now, at the call site, once
-            n, m, T = o.n_state, o.n_ctrl, o.T
-            dev, B = C.device, C.shape[1] if C.dim() == 4 else -1
-            _expect("C", C, (T, B, n + m, n + m), dev)
-            _expect("c", c, (T, B, n + m), dev)
-            _expect("x_init", x_init, (B, n), dev)
-            if not _is_empty(F):
-                if F.dim() != 4 or F.shape[0] not in (T - 1, T):
-                    raise MpcB200Error(f"F: expected [T-1|T,B,n,n+m], got {tuple(F.shape)}")
-                _expect("F", F, (F.shape[0], B, n, n + m), dev)
-            if not _is_empty(f):
-                if f.shape[0] not in (T - 1, T):
-                    raise MpcB200Error(f"f: expected [T-1|T,B,n], got {tuple(f.shape)}")
-                _expect("f", f, (f.shape[0], B, n), dev)
-            _expect("current_x", o.current_x, (T, B, n), dev)
-            _expect("current_u", o.current_u, (T, B, m), dev)
+            # check them now, at the call site, once
+            _validate(o.n_state, o.n_ctrl, o.T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"),
+                      ("current_x", o.current_x, "TBn"), ("current_u", o.current_u, "TBm"), F=F, f=f,
+                      bounds=(o.u_lower, o.u_upper))
             ctx.save_for_backward(x_init, C, c, F, f, o.current_x, o.current_u)
             return o.current_x, o.current_u
         assert o.delta_space                                  # reference :284,298

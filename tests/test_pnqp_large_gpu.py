@@ -20,8 +20,8 @@ N_ITER = 20
 
 def max_n(dtype):
     from mpc.pytorch_b200 import _lib
-    with torch.cuda.device(DEV):
-        return _lib.lib().mpcb200_pnqp_max_n(4 if dtype == torch.float32 else 8)
+    with _lib._on_device(DEV):
+        return _lib.lib().mpcb200_pnqp_max_n(torch.empty(0, dtype=dtype).element_size())
 
 
 def gen_qp(seed, B, n):
@@ -50,8 +50,8 @@ def raw(H, q, lo, hi, x0=None, n_iter=N_ITER):
     iters = torch.empty(B, dtype=torch.int32, device=DEV)
     status = torch.empty(B, dtype=torch.int32, device=DEV)
     L = _lib.lib()
-    fn = L.mpcb200_pnqp_f32 if dt == torch.float32 else L.mpcb200_pnqp_f64
-    with torch.cuda.device(DEV):
+    fn = _lib.entry("mpcb200_pnqp", dt)
+    with _lib._on_device(DEV):
         rc = fn(B, n, *[ptr(t) for t in ins], ptr(x0d), n_iter, ptr(x), ptr(Hf), ptr(If), ptr(iters), ptr(status),
                 stream_handle(DEV))
     assert rc == 0, L.mpcb200_strerror(rc)
@@ -213,9 +213,8 @@ def test_above_max_n_is_refused():
         out = [torch.empty(1, n, dtype=dtype, device=DEV), torch.empty(1, n, n, dtype=dtype, device=DEV),
                torch.empty(1, n, dtype=torch.uint8, device=DEV), torch.empty(1, dtype=torch.int32, device=DEV),
                torch.empty(1, dtype=torch.int32, device=DEV)]
-        L = _lib.lib()
-        fn = L.mpcb200_pnqp_f32 if dtype == torch.float32 else L.mpcb200_pnqp_f64
-        with torch.cuda.device(DEV):
+        fn = _lib.entry("mpcb200_pnqp", dtype)
+        with _lib._on_device(DEV):
             rc = fn(1, n, _lib.ptr(H), _lib.ptr(q), _lib.ptr(q), _lib.ptr(q), None, N_ITER,
                     *[_lib.ptr(t) for t in out], _lib.stream_handle(DEV))
         assert rc == 4   # MPCB200_ERR_SMEM

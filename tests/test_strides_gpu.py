@@ -13,7 +13,7 @@ DEV = torch.device("cuda:0")
 @pytest.mark.parametrize("n,m,B,T", [(8, 2, 48, 12), (16, 4, 24, 9), (4, 2, 40, 7), (5, 1, 18, 8)])
 @pytest.mark.parametrize("bounds", [None, 0.3])
 def test_time_invariant_and_strided_inputs_equal_dense(n, m, B, T, bounds):
-    from mpc.pytorch_b200.step import lqr_step_raw, rollout_raw, _time_strided
+    from mpc.pytorch_b200.step import lqr_grad_raw, lqr_step_raw, rollout_raw, _time_strided
     C, c, F, f, x0 = [t.to(DEV) for t in gen_problem(60 + n, B, T, n, m, torch.float32)]
     u, ul, uu = nominal_controls(60, B, T, m, torch.float32, bounds)
     u = u.to(DEV)
@@ -32,6 +32,14 @@ def test_time_invariant_and_strided_inputs_equal_dense(n, m, B, T, bounds):
     for k in ("new_x", "new_u", "costs", "alphas", "full_du_norm", "status", "free_mask"):
         assert torch.equal(a[k], b[k]), k
     assert int((a["status"] & ~1).max()) == 0        # (bit 0: an fp32 pnqp instance at the iteration cap, same in both)
+    # the gradient kernels read the same strided inputs
+    dx, du = a["new_x"] - x, a["new_u"] - u
+    ga = lqr_grad_raw(n, m, T, C_ti, c_str, F_lti, a["new_x"], a["new_u"], dx, du, x, True)
+    gb = lqr_grad_raw(n, m, T, C_ti.contiguous(), c_str.contiguous(), F_lti.contiguous(), a["new_x"], a["new_u"],
+                      dx, du, x, True)
+    torch.cuda.synchronize()
+    for k, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
+        assert torch.equal(ga[k], gb[k]), name
 
 
 def test_gradient_of_an_lti_system_sums_over_time():
