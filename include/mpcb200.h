@@ -234,6 +234,18 @@ int mpcb200_pnqp_f64(int32_t B, int32_t n, const double* H, const double* q, con
  * memory per block (227 KB, the H100's, when no device is visible); 0 for any other elem_size. */
 int32_t mpcb200_pnqp_max_n(int32_t elem_size);
 
+/*
+ * Shapes without a compiled instance.  The step, the gradient assembly, the rollout and the adjoint's nested solve
+ * of an (n_state, n_ctrl) pair that no instance covers run the large-shape kernels: one thread block per problem,
+ * runtime sizes, the per-time-step tiles of one problem in shared memory.  Their step needs Ks/ks (it returns
+ * MPCB200_ERR_SMEM without them, or when the shape does not fit shared memory).  The one-call adjoint works too; its
+ * workspace then includes the nested solve's gains.
+ * mpcb200_step_large_fits: 1 if the large-shape step runs (n, m) with elem_size 4 (f32) or 8 (f64), assuming the
+ * H100's 227 KB of opt-in shared memory per block (no device needed); 0 otherwise.  It does not look at whether an
+ * instance exists.
+ */
+int mpcb200_step_large_fits(const mpcb200_dims* dims, int32_t elem_size);
+
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);
 
@@ -248,7 +260,8 @@ size_t mpcb200_step_smem_bytes(const mpcb200_dims* dims, int32_t elem_size);
 
 /* 1 if the step kernel wants caller-provided Ks/ks buffers for these dims: either the gain store of all
  * T steps does not fit shared memory, or (one-problem-per-warp shapes such as n=16) moving it out of shared
- * memory is what lets enough warps be resident.  Pass Ks[T,B,m,n], ks[T,B,m] then. */
+ * memory is what lets enough warps be resident, or the shape runs the large-shape kernel.  Pass Ks[T,B,m,n],
+ * ks[T,B,m] then. */
 int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size);
 
 /* Plan of the last step-kernel launch made by the calling thread (mpcb200_lqr_step_*, or the nested solve of
@@ -259,6 +272,7 @@ int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size);
 #define MPCB200_PLAN_PAIR 2u       /* the column-pair kernel ran                                              */
 #define MPCB200_PLAN_GAINS_SMEM 4u /* gains kept in shared memory; otherwise they went through Ks/ks          */
 #define MPCB200_PLAN_KREDUCE 8u    /* generic kernel, gains in Ks/ks: lane i reads column i, butterfly K dx   */
+#define MPCB200_PLAN_LARGE 16u     /* the large-shape kernel ran (one thread block per problem, gains in Ks/ks) */
 int32_t mpcb200_last_step_plan(void);
 
 int mpcb200_version(void);

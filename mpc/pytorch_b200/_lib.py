@@ -41,11 +41,11 @@ EXPORTED_SYMBOLS = (
     "mpcb200_dyn_rollout_f32", "mpcb200_dyn_rollout_f64", "mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64",
     "mpcb200_supported", "mpcb200_supported_list", "mpcb200_launch_count",
     "mpcb200_step_smem_bytes", "mpcb200_step_prefers_workspace", "mpcb200_last_step_plan", "mpcb200_version",
-    "mpcb200_strerror",
+    "mpcb200_strerror", "mpcb200_step_large_fits",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
-PLAN_GENERIC, PLAN_PAIR, PLAN_GAINS_SMEM, PLAN_KREDUCE = 1, 2, 4, 8
+PLAN_GENERIC, PLAN_PAIR, PLAN_GAINS_SMEM, PLAN_KREDUCE, PLAN_LARGE = 1, 2, 4, 8, 16
 
 
 def lib():
@@ -103,6 +103,8 @@ def lib():
     L.mpcb200_step_smem_bytes.restype = ctypes.c_size_t
     L.mpcb200_step_prefers_workspace.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32]
     L.mpcb200_step_prefers_workspace.restype = ctypes.c_int
+    L.mpcb200_step_large_fits.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32]
+    L.mpcb200_step_large_fits.restype = ctypes.c_int
     L.mpcb200_last_step_plan.argtypes = []
     L.mpcb200_last_step_plan.restype = ctypes.c_int32
     L.mpcb200_version.argtypes = []

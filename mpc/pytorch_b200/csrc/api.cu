@@ -5,6 +5,7 @@
 
 #include "../../../include/mpcb200.h"
 #include "lqr_grad.cuh"
+#include "lqr_large.cuh"
 #include "lqr_rollout.cuh"
 #include "lqr_step.cuh"
 #include "pnqp.cuh"
@@ -52,6 +53,15 @@ static const Entry* find(int n, int m) {
     if (kTable[i].n == n && kTable[i].m == m) return &kTable[i];
   return nullptr;
 }
+
+// developer A/B knob MPCB200_KERNEL=3: the large-shape kernels (lqr_large.cu) also for shapes with an instance
+static bool large_forced() {
+  const char* k = std::getenv("MPCB200_KERNEL");
+  return k != nullptr && std::atoi(k) == 3;
+}
+// the step, gradient and rollout of (n, m) run the large-shape kernels
+static bool runs_large(int n, int m) { return find(n, m) == nullptr || large_forced(); }
+static constexpr int kOptinAssumed = 227 * 1024;   // H100 opt-in shared memory per block, for device-free queries
 
 static std::atomic<uint64_t> g_launches{0};
 static thread_local int t_step_plan = 0;      // MPCB200_PLAN_* bits of this thread's last step launch
@@ -120,7 +130,8 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
   }
   if ((Ks == nullptr) != (ks == nullptr)) return MPCB200_ERR_NULL_POINTER;
   const Entry* e = find(d->n, d->m);
-  if (e == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
+  const bool large = d->dynamics_kind == DYN_LINEAR && runs_large(d->n, d->m);
+  if (e == nullptr && !large) return MPCB200_ERR_UNSUPPORTED_DIMS;
   const int smem = max_smem_optin();
   if (smem <= 0) return MPCB200_ERR_NO_DEVICE;
 
@@ -160,6 +171,28 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
     if (!shape_ok) return MPCB200_ERR_BAD_DIMS;
     for (int i = 0; i < 8; ++i) a.dp.p[i] = p->dyn[i];
   }
+  if (large) {
+    // the fused adjoint has no large-shape kernel: adjoint_impl then takes its three-launch route
+    if (adj != nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
+    if (Ks == nullptr) return MPCB200_ERR_SMEM;      // the gains always go through the caller's Ks/ks
+    const int n = d->n, m = d->m, p = n + m;
+    auto spans = [&](const void* base, long long ts, long long span) {
+      return base != nullptr && aligned16(base) && (ts * (long long)sz) % 16 == 0 && (span * (long long)sz) % 16 == 0;
+    };
+    unsigned bulk = 0u;
+    if (spans(C, a.C_ts, (long long)p * p)) bulk |= LB_C;
+    if (spans(F, a.F_ts, (long long)n * p)) bulk |= LB_F;
+    if (spans(c, a.c_ts, p)) bulk |= LB_c;
+    if (d->has_f && spans(f, a.f_ts, n)) bulk |= LB_f;
+    if (spans(cur_x, (long long)d->B * n, n)) bulk |= LB_x;
+    if (spans(cur_u, (long long)d->B * m, m)) bulk |= LB_u;
+    if (d->bounds_kind == 2 && spans(u_lower, (long long)d->B * m, m) && spans(u_upper, (long long)d->B * m, m))
+      bulk |= LB_BOX;
+    t_step_plan = 0;
+    rc = large_step_launch<R>(a, n, m, bulk, smem, (cudaStream_t)stream);
+    if (rc == 0) g_launches.fetch_add(1);
+    return rc;
+  }
   if (const char* k = std::getenv("MPCB200_KERNEL")) a.impl = std::atoi(k);
   if (adj != nullptr) {          // fused KKT adjoint: column-pair kernel only
     if (!adj->ok || !a.bulk_ok || a.impl == 1) return MPCB200_ERR_UNSUPPORTED_DIMS;
@@ -185,7 +218,7 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
     return MPCB200_ERR_NULL_POINTER;
   if (d->F_T > 0 && (F == nullptr || dF == nullptr)) return MPCB200_ERR_NULL_POINTER;
   const Entry* e = find(d->n, d->m);
-  if (e == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
+  const bool large = runs_large(d->n, d->m);
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   GradArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -195,7 +228,8 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
   a.C_ts = tstride(d->C_tstride, (long long)d->B * (d->n + d->m) * (d->n + d->m));
   a.c_ts = tstride(d->c_tstride, (long long)d->B * (d->n + d->m));
   a.F_ts = tstride(d->F_tstride, (long long)d->B * d->n * (d->n + d->m));
-  rc = (sizeof(R) == 4 ? e->grad32 : e->grad64)(a, (cudaStream_t)stream);
+  rc = large ? large_grad_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
+             : (sizeof(R) == 4 ? e->grad32 : e->grad64)(a, (cudaStream_t)stream);
   if (rc == 0) g_launches.fetch_add(workspace != nullptr ? 2 : 1);
   return rc;
 }
@@ -203,7 +237,8 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
 // KKT adjoint in one call (reference LQRStepFn.backward, mpc/lqr_step.py:312-407)
 // ---------------------------------------------------------------------------------------------
 struct AdjLayout {                    // workspace carve-up (byte offsets, every piece 256-byte aligned)
-  size_t negr, zeros, dx, du, costate, scal, mask, maskf, total;
+  size_t negr, zeros, dx, du, costate, scal, mask, maskf, Ks, ks, total;
+  bool gains;                         // Ks/ks of the nested solve (the large-shape step keeps its gains there)
 };
 static size_t up256(size_t v) { return (v + 255) / 256 * 256; }
 static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz) {
@@ -218,6 +253,12 @@ static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz) {
   l.scal = o;    o += up256((size_t)3 * B * sz);
   l.mask = o;    o += up256(TB * m);
   l.maskf = o;   o += up256(TB * m * sz);                               // the same mask as element-typed 0/1 (rides on the TMA tile)
+  l.gains = runs_large(n, m);
+  l.Ks = l.ks = 0;
+  if (l.gains) {
+    l.Ks = o;    o += up256(TB * m * n * sz);
+    l.ks = o;    o += up256(TB * m * sz);
+  }
   l.total = o;
   return l;
 }
@@ -306,9 +347,11 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
   }
   // 3-launch path: the nested solve really reads its (zero) nominal trajectory
   if (cudaMemsetAsync(zeros, 0, TB * (d->n + d->m) * sizeof(R), st) != cudaSuccess) return MPCB200_ERR_LAUNCH;
+  R* Ks = l.gains ? (R*)(ws + l.Ks) : nullptr;
+  R* ks = l.gains ? (R*)(ws + l.ks) : nullptr;
   rc = step_impl<R>(&ds, &ps, C, negr, F, (const R*)nullptr, z0, zx, zu, (const R*)nullptr, (const R*)nullptr, mask,
                     dxs, dus, scal, scal + d->B, scal + 2 * d->B, (R*)nullptr, (int32_t*)nullptr,
-                    (uint8_t*)nullptr, (int32_t*)nullptr, (R*)nullptr, (R*)nullptr, stream);
+                    (uint8_t*)nullptr, (int32_t*)nullptr, Ks, ks, stream);
   if (rc == MPCB200_ERR_SMEM) return rc;     // long horizons: use the two-call path with Ks/ks buffers
   if (rc) return rc;
   mpcb200_dims dg = *d;
@@ -325,7 +368,7 @@ static int rollout_impl(const mpcb200_dims* d, const R* F, const R* f, const R* 
   if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
   if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
   const Entry* e = find(d->n, d->m);
-  if (e == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
+  const bool large = runs_large(d->n, d->m);
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   RolloutArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -333,7 +376,8 @@ static int rollout_impl(const mpcb200_dims* d, const R* F, const R* f, const R* 
   a.F = F; a.f = f; a.x_init = x_init; a.u = u; a.x = x;
   a.F_ts = tstride(d->F_tstride, (long long)d->B * d->n * (d->n + d->m));
   a.f_ts = tstride(d->f_tstride, (long long)d->B * d->n);
-  rc = (sizeof(R) == 4 ? e->roll32 : e->roll64)(a, (cudaStream_t)stream);
+  rc = large ? large_rollout_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
+             : (sizeof(R) == 4 ? e->roll32 : e->roll64)(a, (cudaStream_t)stream);
   if (rc == 0) g_launches.fetch_add(1);
   return rc;
 }
@@ -468,11 +512,16 @@ size_t mpcb200_step_smem_bytes(const mpcb200_dims* dims, int32_t elem_size) {
 
 int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr) return 0;
+  if (runs_large(dims->n, dims->m)) return 1;   // the large-shape step keeps its gains in Ks/ks
   const Entry* e = find(dims->n, dims->m);
-  if (e == nullptr) return 0;
   int ms = max_smem_optin();
-  if (ms <= 0) ms = 227 * 1024;       // no device visible (CPU-side query): assume H100's opt-in limit
+  if (ms <= 0) ms = kOptinAssumed;    // no device visible (CPU-side query): assume H100's opt-in limit
   return elem_size == 8 ? e->pws64(dims->T, ms) : e->pws32(dims->T, ms);
+}
+
+int mpcb200_step_large_fits(const mpcb200_dims* dims, int32_t elem_size) {
+  if (dims == nullptr || (elem_size != 4 && elem_size != 8)) return 0;
+  return large_step_fits(dims->n, dims->m, elem_size, kOptinAssumed) ? 1 : 0;
 }
 
 int32_t mpcb200_last_step_plan(void) { return t_step_plan; }

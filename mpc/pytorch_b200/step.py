@@ -6,6 +6,7 @@ shapes, and the same gradient tuple ``(dx_init, dC, dc, dF, df)`` (:407).  The
 arithmetic runs in csrc/lqr_step.cuh and csrc/lqr_grad.cuh.
 """
 import ctypes
+import os
 import threading
 
 import torch
@@ -75,7 +76,7 @@ def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=Non
             if t.shape != shape_of["TBm"]:
                 raise MpcB200Error(f"{name}: expected shape {shape_of['TBm']}, got {tuple(t.shape)}")
             checked.append((name, t))
-    if exact and _pick_instance(n, m) != (n, m):
+    if exact and _pick_instance(n, m, lead.element_size()) != (n, m):
         raise MpcB200Error("in-kernel dynamics need an exact (n_state, n_ctrl) kernel instance")
     dev = lead.device
     for name, t in checked:
@@ -126,28 +127,49 @@ _pick_cache = {}
 _smem_fits_cache = {}
 
 
-def _pick_instance(n, m):
-    hit = _pick_cache.get((n, m))
+def _pick_instance(n, m, elem_size=4):
+    """The (N, M) kernel shape an (n, m) problem runs at: the smallest compiled instance that covers it (zero padded),
+    else (n, m) itself on the large-shape kernels if they fit it in `elem_size`-byte elements."""
+    key = (n, m, elem_size)
+    hit = _pick_cache.get(key)
     if hit is not None:
         return hit
-    hit = _pick_instance_uncached(n, m)
-    _pick_cache[(n, m)] = hit
+    hit = _pick_instance_uncached(n, m, elem_size)
+    _pick_cache[key] = hit
     return hit
 
 
-def _pick_instance_uncached(n, m):
+def _large_fits(n, m, elem_size):
+    dims = Dims(B=1, T=1, n=n, m=m, F_T=0)
+    return bool(_lib.lib().mpcb200_step_large_fits(ctypes.byref(dims), elem_size))
+
+
+def large_limit(m, elem_size):
+    """The largest n_state the large-shape kernels take with n_ctrl = m (0: none)."""
+    n = 0
+    while _large_fits(n + 1, m, elem_size):
+        n += 1
+    return n
+
+
+def _pick_instance_uncached(n, m, elem_size=4):
     global _pairs_cache
     if _pairs_cache is None:
         _pairs_cache = _lib.supported_pairs()
     if (n, m) in _pairs_cache:
         return n, m
     cands = [(N + M, N, M) for (N, M) in _pairs_cache if N >= n and M >= m]
-    if not cands:
-        raise MpcB200Error(
-            f"(n_state={n}, n_ctrl={m}) exceeds every compiled kernel instance {_pairs_cache}; "
-            "add it to mpc/pytorch_b200/csrc/instances.def and rebuild")
-    _, N, M = min(cands)
-    return N, M
+    if cands:
+        _, N, M = min(cands)
+        return N, M
+    if _large_fits(n, m, elem_size):
+        return n, m
+    dtype = {4: "float32", 8: "float64"}.get(elem_size, f"{elem_size}-byte elements")
+    nmax = large_limit(m, elem_size)
+    limit = f"n_state <= {nmax} for n_ctrl={m}" if nmax else f"no n_state for n_ctrl={m}"
+    raise MpcB200Error(
+        f"(n_state={n}, n_ctrl={m}) exceeds every compiled kernel instance {_pairs_cache} and the shared-memory "
+        f"limit of the large-shape kernel in {dtype} ({limit}, 227 KB per problem)")
 
 
 class _Pad:
@@ -233,7 +255,7 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
                   ("current_u", cur_u, "TBm"), F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
                   exact=dyn is not None)
     dtype, dev = C.dtype, C.device
-    N, M = _pick_instance(n, m)
+    N, M = _pick_instance(n, m, C.element_size())
     pad = _Pad(n, m, N, M, dev)
     (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
     (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
@@ -274,7 +296,8 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
     need_gains = want_gains or not do_rollout
     if not need_gains:
         # long horizons do not fit shared memory: the kernel then keeps gains in a caller buffer
-        key = (N, M, T, C.element_size())
+        # the library's answer also depends on the MPCB200_KERNEL developer knob (3: the large kernels everywhere)
+        key = (N, M, T, C.element_size(), os.environ.get("MPCB200_KERNEL"))
         fits = _smem_fits_cache.get(key)
         if fits is None:
             fits = not _lib.lib().mpcb200_step_prefers_workspace(ctypes.byref(dims), C.element_size())
@@ -313,7 +336,7 @@ def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_
     B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("new_x", new_x, "TBn"), ("new_u", new_u, "TBm"),
                   ("dx", dx, "TBn"), ("du", du, "TBm"), ("dl_dx", dl_dx, "TBn"), F=F)
     dtype, dev = C.dtype, C.device
-    N, M = _pick_instance(n, m)
+    N, M = _pick_instance(n, m, C.element_size())
     pad = _Pad(n, m, N, M, dev)
     (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
     F_, tsF = pad.stage(F, dtype, pad.mat_np)
@@ -374,7 +397,7 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
     if not validated:
         _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("new_x", new_x, "TBn"), ("new_u", new_u, "TBm"),
                   ("dl_dx", dl_dx, "TBn"), ("dl_du", dl_du, "TBm"), F=F, bounds=(u_lower, u_upper))
-    if _pick_instance(n, m) != (n, m) or _is_empty(F):
+    if _pick_instance(n, m, C.element_size()) != (n, m) or _is_empty(F):
         return None
     dtype, dev = C.dtype, C.device
     B = C.shape[1]
@@ -425,7 +448,7 @@ def rollout_raw(n_state, n_ctrl, T, x_init, u, F, f=None):
     n, m = n_state, n_ctrl
     B = _validate(n, m, T, ("x_init", x_init, "Bn"), ("u", u, "TBm"), F=F, f=f)
     dtype, dev = x_init.dtype, x_init.device
-    N, M = _pick_instance(n, m)
+    N, M = _pick_instance(n, m, x_init.element_size())
     pad = _Pad(n, m, N, M, dev)
     (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
     x0_, u_ = _dense(x_init, dtype), _dense(u, dtype)

@@ -17,6 +17,30 @@ for (B, T, n, m, dt) in [(13, 6, 8, 2, torch.float32), (7, 5, 3, 1, torch.float6
     a = lqr_step_raw(n, m, T, torch.zeros_like(x0), C, -torch.cat((x, u), 2), F, None, torch.zeros_like(x), torch.zeros_like(u), u_zero_I=I)
     g = lqr_grad_raw(n, m, T, C, c, F, o["new_x"], o["new_u"], a["new_x"], a["new_u"], x, True)
     torch.cuda.synchronize()
+# a shape without a compiled instance: the large-shape step (bounded, gains in Ks/ks) and, through autograd, the
+# multi-call backward (masked large step + costate and outer-product kernels); then mpcb200_lqr_adjoint_* at the same
+# shape, whose nested solve keeps its gains in the workspace
+import ctypes
+from mpc.pytorch_b200 import LQRStep, QuadCost, LinDx
+from mpc.pytorch_b200._lib import Dims, Params, check, entry, lib, ptr
+B, T, n, m, dt = 3, 4, 20, 5, torch.float64
+C, c, F, f, x0 = [t.to(dev) for t in gen_problem(2, B, T, n, m, dt)]
+u, ul, uu = nominal_controls(2, B, T, m, dt, 0.25)
+u = u.to(dev)
+x = get_traj(T, u, x0, LinDx(F, f))
+lv = [t.clone().requires_grad_(True) for t in (x0, C, c, F, f)]
+nx, nu = LQRStep(n, m, T, u_lower=ul, u_upper=uu, current_x=x, current_u=u, true_cost=QuadCost(lv[1], lv[2]),
+                 true_dynamics=LinDx(lv[3], lv[4]))(*lv)[:2]
+(nx.sum() + nu.sum()).backward()
+dims = Dims(B=B, T=T, n=n, m=m, F_T=T - 1, has_f=1, bounds_kind=1, max_ls_iter=10, pnqp_max_iter=20, do_rollout=1)
+nbytes = lib().mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), 8)
+ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+outs = [torch.empty_like(t) for t in (x0, C, c, F, f)]
+ins = [C, c, F, nx.detach().contiguous(), nu.detach().contiguous(), torch.ones_like(x), torch.ones_like(u)]
+check(entry("mpcb200_lqr_adjoint", dt)(ctypes.byref(dims), ctypes.byref(Params(u_lo=ul, u_hi=uu, ls_decay=0.2)),
+                                       *[ptr(t) for t in ins], None, None, *[ptr(t) for t in outs], ptr(ws), nbytes,
+                                       None), "adjoint")
+torch.cuda.synchronize()
 from mpc.pnqp import pnqp
 for (B, n, dt) in [(2, 100, torch.float64), (3, 128, torch.float32)]:    # one thread block per QP
     g = torch.Generator().manual_seed(n)
