@@ -1,8 +1,11 @@
-// common.cuh - PTX helpers (mbarrier, 1-D bulk TMA) and tiny per-lane linear algebra.
+// common.cuh - PTX helpers (mbarrier, 1-D bulk TMA), the launchers' shared-memory opt-in and tiny per-lane
+// linear algebra.
 // sm_90a only.  No reference code: the algorithms these serve are cited in lqr_step.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <atomic>
+#include "../../../include/mpcb200.h"
 
 namespace mpcb200 {
 
@@ -34,32 +37,6 @@ MPCB_DEV bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// try_wait with a suspend-time hint: the warp sleeps in hardware until the phase completes (or the
-// hint expires) instead of burning issue slots in a polling loop.
-MPCB_DEV bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t ns) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(ns)
-      : "memory");
-  return ok != 0;
-}
-// non-blocking probe (mbarrier.test_wait).  Probing the NEXT stage at the end of a step (to take the
-// try_wait latency off the per-step path) gained nothing at config 3 - not used.
-MPCB_DEV bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 MPCB_DEV void mbar_wait(uint64_t* bar, uint32_t parity) {
   // plain try_wait blocks in hardware for a bounded time; the suspend-hint form compiles to a
   // NANOSLEEP polling loop whose wake-up granularity hurts a latency-bound consumer
@@ -83,16 +60,25 @@ MPCB_DEV void named_bar_sync(int id, int nthreads) {
   asm volatile("barrier.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ------------------------------------------------------------------ compile-time helpers
-__host__ __device__ constexpr int round_up(int v, int a) { return (v + a - 1) / a * a; }
-template <typename R>
-__host__ __device__ constexpr int vec_elems(int count) {
-  // widest vector (in elements) that divides `count` elements and keeps 16/8-byte alignment
-  return (count * (int)sizeof(R)) % 16 == 0 ? 16 / (int)sizeof(R)
-         : (count * (int)sizeof(R)) % 8 == 0 ? 8 / (int)sizeof(R)
-                                             : 1;
+// Raise Kern's opt-in dynamic shared-memory limit to max_smem_optin, once per device (the attribute is per
+// context).  Keyed on the kernel itself: instances of one template have the same type.  Atomic flags:
+// concurrent callers (one host thread per GPU is the expected pattern) may both set the attribute, which is
+// idempotent, but never read a torn value.
+template <auto Kern>
+int allow_smem_optin(int max_smem_optin) {
+  static std::atomic<int> configured[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return MPCB200_ERR_NO_DEVICE;
+  if (configured[dev].load(std::memory_order_acquire) < max_smem_optin) {
+    if (cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin) != cudaSuccess)
+      return MPCB200_ERR_LAUNCH;
+    configured[dev].store(max_smem_optin, std::memory_order_release);
+  }
+  return MPCB200_OK;
 }
 
+// ------------------------------------------------------------------ compile-time helpers
+__host__ __device__ constexpr int round_up(int v, int a) { return (v + a - 1) / a * a; }
 template <typename R, int V>
 struct VecLoad;
 template <>

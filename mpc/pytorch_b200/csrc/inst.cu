@@ -19,8 +19,8 @@ template <typename R>
 static int step_dispatch(const StepArgs& a, int max_smem, cudaStream_t s) {
   if (a.impl == 2 || (a.impl == 0 && Step2Cfg<R, INST_N, INST_M>::PAIR_DEFAULT)) {
     const int rc = launch_step2<R, INST_N, INST_M>(a, max_smem, s);
-    if (rc >= 0 && !(rc == 4 && a.impl == 0)) return rc;      // rc < 0: shape not supported by the pair mapping
-    if (a.impl == 2 && rc < 0) return 3;   // MPCB200_ERR_UNSUPPORTED_DIMS
+    if (rc != STEP2_DECLINED && !(rc == MPCB200_ERR_SMEM && a.impl == 0)) return rc;
+    if (a.impl == 2 && rc == STEP2_DECLINED) return MPCB200_ERR_UNSUPPORTED_DIMS;
   }
   return launch_step<R, INST_N, INST_M>(a, max_smem, s);
 }

@@ -337,14 +337,14 @@ int launch_grad(const GradArgs& a, cudaStream_t stream) {
   const int grid = (a.B + K::W - 1) / K::W;
   if (a.workspace == nullptr) {
     lqr_grad_kernel<R, N, M><<<grid, K::THREADS, 0, stream>>>(a);
-    return cudaGetLastError() == cudaSuccess ? 0 : 5;
+    return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH;
   }
   lqr_costate_kernel<R, N, M><<<grid, K::THREADS, 0, stream>>>(a);
-  if (cudaGetLastError() != cudaSuccess) return 5;
+  if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
   const long long items = (long long)((a.B + K::PPW - 1) / K::PPW) * ((a.T + K::TCHUNK - 1) / K::TCHUNK);
   const int grid2 = (int)((items + K::NW - 1) / K::NW);
   lqr_outer_kernel<R, N, M><<<grid2, K::THREADS, 0, stream>>>(a);
-  return cudaGetLastError() == cudaSuccess ? 0 : 5;
+  return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH;
 }
 
 }  // namespace mpcb200

@@ -21,7 +21,6 @@
 //   PLAIN / MASK  LDL^T of Q_uu (masked: u_zero_I rows and columns zeroed, +1e-8 on their diagonal),
 // and V = Q_xx + Q_xu K + K'Q_ux + K'(Q_uu K), v = q_x + Q_xu k + K'(q_u + Q_uu k) with the true Q_xu.
 // Rollout + line search (:164-261): per-problem alpha, passes repeat while the cost is worse than the nominal one.
-#include <atomic>
 #include "../../../include/mpcb200.h"
 #include "common.cuh"
 #include "lqr_large.cuh"
@@ -497,16 +496,9 @@ int large_step_launch(const StepArgs& a, int n, int m, unsigned bulk, int max_sm
   la.bulk = bulk;
   la.stages = large_step_smem_bytes(n, m, es, 2) <= (size_t)max_smem ? 2 : 1;
   const size_t smem = large_step_smem_bytes(n, m, es, la.stages);
-  auto kern = lqr_large_step_kernel<R>;
-  static std::atomic<int> configured[64];
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return MPCB200_ERR_NO_DEVICE;
-  if (configured[dev].load(std::memory_order_acquire) == 0) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem) != cudaSuccess)
-      return MPCB200_ERR_LAUNCH;
-    configured[dev].store(1, std::memory_order_release);
-  }
-  kern<<<a.B, LNT, smem, stream>>>(la);
+  const int rc = allow_smem_optin<lqr_large_step_kernel<R>>(max_smem);
+  if (rc != MPCB200_OK) return rc;
+  lqr_large_step_kernel<R><<<a.B, LNT, smem, stream>>>(la);
   if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
   record_step_plan((int)MPCB200_PLAN_LARGE);
   return MPCB200_OK;

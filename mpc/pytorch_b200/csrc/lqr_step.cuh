@@ -29,15 +29,9 @@
 // compile-time knobs (two columns per lane, V in registers, padded tiles, mma.sync products, phase timers)
 // are listed in DESIGN.md section 7; their code was removed.
 #pragma once
-#include <atomic>
-#include <cstdio>
 #include "../../../include/mpcb200.h"
 #include "common.cuh"
 #include "dynamics.cuh"
-
-#ifndef MPCB_STAGES
-#define MPCB_STAGES 3
-#endif
 
 namespace mpcb200 {
 
@@ -80,17 +74,14 @@ struct StepCfg {
   // consumer warps per CTA: the smallest count whose per-time-step spans stay 16-byte aligned for every
   // tensor (so the bulk-TMA path applies).  Small CTAs matter: 4096 problems are < 1 wave, and the
   // kernel time is set by the most loaded SM, so the CTA granularity is the load-balance granularity.
-#ifndef MPCB_MAXNW
-#define MPCB_MAXNW 4
-#endif
   static constexpr bool span_ok(int nw) {
     return (nw * PPW * M * (int)sizeof(R)) % 16 == 0 && (nw * PPW * N * (int)sizeof(R)) % 16 == 0;
   }
-  static constexpr int NW = (span_ok(1) && MPCB_MAXNW >= 1) ? 1 : (span_ok(2) && MPCB_MAXNW >= 2) ? 2 : 4;
+  static constexpr int NW = span_ok(1) ? 1 : span_ok(2) ? 2 : 4;
   static constexpr int W = NW * PPW;      // problems per CTA
   static_assert(span_ok(NW), "CTA problem count must keep spans 16-byte aligned");
   static constexpr int THREADS = (NW + 1) * 32;
-  static constexpr int S = MPCB_STAGES;   // ring stages
+  static constexpr int S = 3;             // ring stages
   static constexpr int VS = round_up(N, 4);
   static constexpr int CS = P * P, FS = N * P;     // per-problem strides of the C and F tiles inside a stage
   // stage tile offsets (elements); every sub-tile starts 16-byte aligned (span_ok / padded strides)
@@ -244,6 +235,28 @@ MPCB_DEV void pnqp_lane(const R (&H)[M][M], const R (&q)[M], const R (&lo)[M], c
 }
 
 // ---------------------------------------------------------------------------------------------
+// Shared by the step kernels (this file, lqr_step2.cuh, lqr_large.cu).
+// ---------------------------------------------------------------------------------------------
+enum { MODE_PLAIN = 0, MODE_BOX = 1, MODE_MASK = 2 };
+
+// Where the gains K_t, k_t of all T steps live between the Riccati sweep and the rollout: shared memory when
+// they fit, unless the kernel's own criterion `prefers_ws` moves them to the caller's Ks/ks.  Sets a.k_in_smem
+// and smem to the kernel's dynamic shared memory; MPCB200_ERR_SMEM when neither placement works.
+template <typename SmemFn>
+int plan_gain_store(StepArgs& a, bool prefers_ws, int max_smem_optin, SmemFn smem_bytes, size_t& smem) {
+  const bool have_ws = a.Ks != nullptr && a.ks != nullptr;
+  a.k_in_smem = 1;
+  smem = smem_bytes(true);
+  if (smem > (size_t)max_smem_optin || (prefers_ws && have_ws && a.do_rollout)) {
+    a.k_in_smem = 0;
+    smem = smem_bytes(false);
+    if (smem > (size_t)max_smem_optin) return MPCB200_ERR_SMEM;
+    if (a.do_rollout && !have_ws) return MPCB200_ERR_SMEM;
+  }
+  return MPCB200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // producer warp: stream one (t) tile set of the CTA's problems into ring stage `tile % S`
 // ---------------------------------------------------------------------------------------------
 template <typename R, int N, int M>
@@ -346,7 +359,6 @@ MPCB_DEV void step_producer(const StepArgs& a, unsigned char* stage_base, uint64
 // consumer warps.  MODE (compile time): 0 plain (no bounds, no mask), 1 box (pnqp; optional
 // u_zero_I), 2 mask (u_zero_I only - the adjoint solve).
 // ---------------------------------------------------------------------------------------------
-enum { MODE_PLAIN = 0, MODE_BOX = 1, MODE_MASK = 2 };
 
 template <typename R, int N, int M, int MODE>
 MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64_t* full,
@@ -473,8 +485,6 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     R Quu[M][M], qu[M];
 #pragma unroll
     for (int p2 = 0; p2 < M; ++p2) {
-      constexpr int dummy = 0;
-      (void)dummy;
       const int src = base + (N + p2) % LP;
 #pragma unroll
       for (int p1 = 0; p1 < M; ++p1) Quu[p1][p2] = shfl(Qc[(N + p2) / LP].get(N + p1), src);
@@ -513,8 +523,8 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
       }
       bool conv, badpiv;
       pnqp_lane<R, M>(Quu, qu, lb, ub, t < T - 1, kk, fac, fm, it, conv, badpiv, a.pnqp_iters);
-      if (!conv) status |= 1u;
-      if (badpiv) status |= 4u;
+      if (!conv) status |= MPCB200_ST_PNQP_UNCONVERGED;
+      if (badpiv) status |= MPCB200_ST_BAD_PIVOT;
 #pragma unroll
       for (int q = 0; q < M; ++q) kprev[q] = kk[q];
     } else {                                     // unconstrained (:84-94) or u_zero_I masked (:100-127)
@@ -534,7 +544,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
         if (!f1) A[p1][p1] += R(1e-8);
       }
       fac.factor(A);
-      if (fac.bad) status |= 4u;
+      if (fac.bad) status |= MPCB200_ST_BAD_PIVOT;
       fac.solve(rhs, sol);
 #pragma unroll
       for (int q = 0; q < M; ++q) kk[q] = -sol[q];
@@ -835,7 +845,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     ((R*)a.costs)[b] = cost;
     ((R*)a.full_du_norm)[b] = fdn;
     ((R*)a.alphas)[b] = alpha;
-    if (!(cost - cost == R(0))) status |= 2u;
+    if (!(cost - cost == R(0))) status |= MPCB200_ST_NONFINITE;
     if (a.status != nullptr) a.status[b] = (int)status;
   }
 }
@@ -868,7 +878,6 @@ lqr_step_kernel(const StepArgs a) {
   if (warp == K::NW) {
     step_producer<R, N, M>(a, stage_base, full, empty, votes, b0, cnt, lane);
   } else {
-
     step_consumer<R, N, M, MODE>(a, stage_base, full, empty, votes, scratch, kstore, b0, warp, lane);
   }
 }
@@ -877,33 +886,17 @@ template <typename R, int N, int M, int MODE>
 int launch_step_mode(const StepArgs& args, int max_smem_optin, cudaStream_t stream) {
   using K = StepCfg<R, N, M>;
   StepArgs a = args;
-  size_t smem = K::smem_bytes(a.T, true);
-  a.k_in_smem = 1;
-  const bool have_ws = a.Ks != nullptr && a.ks != nullptr;
-  if (smem > (size_t)max_smem_optin || (K::prefers_workspace(a.T, max_smem_optin) && have_ws && a.do_rollout)) {
-    a.k_in_smem = 0;
-    smem = K::smem_bytes(a.T, false);
-    if (smem > (size_t)max_smem_optin) return 4;
-    if (a.do_rollout && !have_ws) return 4;
-  }
-  auto kern = lqr_step_kernel<R, N, M, MODE>;
-  // per device: the opt-in shared-memory attribute is per context.  Atomic flags: concurrent callers (one host
-  // thread per GPU is the expected pattern) may both set the attribute - idempotent - but never read a torn value.
-  static std::atomic<int> configured[64];
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 6;
-  if (configured[dev].load(std::memory_order_acquire) < (int)smem) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin) !=
-        cudaSuccess)
-      return 5;
-    configured[dev].store(max_smem_optin, std::memory_order_release);
-  }
+  size_t smem;
+  int rc = plan_gain_store(a, K::prefers_workspace(a.T, max_smem_optin), max_smem_optin,
+                           [&](bool k_in_smem) { return K::smem_bytes(a.T, k_in_smem); }, smem);
+  if (rc == MPCB200_OK) rc = allow_smem_optin<lqr_step_kernel<R, N, M, MODE>>(max_smem_optin);
+  if (rc != MPCB200_OK) return rc;
   const int grid = (a.B + K::W - 1) / K::W;
-  kern<<<grid, K::THREADS, smem, stream>>>(a);
-  if (cudaGetLastError() != cudaSuccess) return 5;
+  lqr_step_kernel<R, N, M, MODE><<<grid, K::THREADS, smem, stream>>>(a);
+  if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
   record_step_plan((int)(MPCB200_PLAN_GENERIC | (a.k_in_smem ? MPCB200_PLAN_GAINS_SMEM : 0u) |
                          (K::KREDUCE && !a.k_in_smem && a.do_rollout ? MPCB200_PLAN_KREDUCE : 0u)));
-  return 0;
+  return MPCB200_OK;
 }
 
 template <typename R, int N, int M>

@@ -12,7 +12,7 @@
 //  * no producer warp and no empty barriers: every warp streams its OWN tiles.  After a warp has consumed
 //    stage s, up to 8 of its lanes each issue one 1-D bulk TMA copy (C, F, c, x_bar, u_bar, f, bounds) of tile
 //    seq+S into that stage in ONE instruction; completion is an mbarrier transaction count.  Warps are
-//    independent (a CTA is just NW of them), so the CTA size is only a scheduling granularity.
+//    independent, so a CTA is one warp.
 //  * V is exchanged through a per-problem row-major buffer (a lane stores its column pair of every row with
 //    8-byte stores, readers take whole rows as broadcast 128-bit loads) - exact V, no symmetry assumption.
 //  * gains K_t, k_t of all T steps stay in shared memory (or the caller's Ks/ks for long horizons); the
@@ -21,13 +21,6 @@
 // generic kernel in lqr_step.cuh.
 #pragma once
 #include "lqr_step.cuh"
-
-#ifndef MPCB2_STAGES
-#define MPCB2_STAGES 4
-#endif
-#ifndef MPCB2_NW
-#define MPCB2_NW 1
-#endif
 
 namespace mpcb200 {
 
@@ -102,8 +95,7 @@ struct Step2Cfg {
   static constexpr int P = N + M;
   static constexpr int L = P / 2;            // lanes per problem
   static constexpr int NXL = N / 2;          // x lanes (own two state columns each)
-  static constexpr int PPW = L > 0 ? 32 / (L > 0 ? L : 1) : 1;   // problems per warp
-  static constexpr int NW = MPCB2_NW;        // independent (self-feeding) warps per CTA
+  static constexpr int PPW = 32 / L;         // problems per warp
   static constexpr int EA = 16 / (int)sizeof(R);
   static constexpr int SZ = (int)sizeof(R);
   // shapes this mapping supports: even n, m; per-warp spans of C and F 16-byte multiples (always true for even
@@ -133,10 +125,7 @@ struct Step2Cfg {
   static constexpr int STAGE_BYTES = round_up(OFF_END * SZ, 128);
   // ring depth: 4 stages for small tiles, 3 for big ones (n=16, m=4: 9.4 KB tiles).  Fewer stages let more warps
   // reside per SM but hide less of the copy latency; 3 was the best trade-off for the big tiles.
-#ifndef MPCB2_BIG_STAGES
-#define MPCB2_BIG_STAGES 3
-#endif
-  static constexpr int S = STAGE_BYTES > 6144 ? MPCB2_BIG_STAGES : MPCB2_STAGES;
+  static constexpr int S = STAGE_BYTES > 6144 ? 3 : 4;
   static constexpr int MAX_REGS = 255;
   // per-problem scratch (elements)
   static constexpr int NV = round_up(N, 4);             // row stride of V / K rows (16-byte aligned rows)
@@ -160,20 +149,13 @@ struct Step2Cfg {
   }
   static constexpr int SCRS = pick_scr();
   static constexpr int HDR_BYTES = 128;                  // S mbarriers (per warp)
-  __host__ __device__ static size_t warp_smem_bytes(int T, bool k_in_smem, bool adj = false) {
+  __host__ __device__ static size_t smem_bytes(int T, bool k_in_smem, bool adj = false) {
     size_t b = HDR_BYTES + (size_t)S * STAGE_BYTES + (size_t)PPW * SCRS * SZ;
     if (k_in_smem) b += (size_t)PPW * T * KT * SZ;
     if (adj) b += (size_t)PPW * T * P * SZ;              // d tau of every step, kept for the costate sweep
     return round_up((int)b, 128);
   }
-  static size_t smem_bytes(int T, bool k_in_smem) { return (size_t)NW * warp_smem_bytes(T, k_in_smem); }
 };
-
-#ifdef MPCB2_TIMING
-#define TICK2(arr, i) { ck1 = clock64(); arr[i] += ck1 - ck0; ck0 = ck1; }
-#else
-#define TICK2(arr, i)
-#endif
 
 // One warp's tile stream: where its spans start in global memory and where its ring lives in shared memory.
 struct TileSrc {
@@ -260,28 +242,25 @@ MPCB_DEV TileSrc tile_src(const StepArgs& a, int b0, int cnt, unsigned char* wba
 }
 
 template <typename R, int N, int M, int MODE, bool KSM, bool ADJ = false>
-__global__ void __launch_bounds__(Step2Cfg<R, N, M>::NW * 32) __maxnreg__((Step2Cfg<R, N, M>::MAX_REGS))
+__global__ void __launch_bounds__(32) __maxnreg__((Step2Cfg<R, N, M>::MAX_REGS))
 lqr_step2_kernel(const StepArgs a) {
   using K = Step2Cfg<R, N, M>;
   constexpr int P = K::P, L = K::L, NXL = K::NXL, PPW = K::PPW, S = K::S, SZ = K::SZ, KT = K::KT, VSTR = K::VSTR, NV = K::NV;
   constexpr int EA = K::EA, A_N = K::A_N, A_M = K::A_M;
-  constexpr int NWC = K::NW;                                // independent warps per CTA
   constexpr unsigned FULLM = (1u << M) - 1u;
   constexpr bool BOX = MODE == MODE_BOX;
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int warp = NWC == 1 ? 0 : __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;                        // one warp per CTA
   const int T = a.T, B = a.B;
   // tensor bounds ride in the lo/hi slots; the fused adjoint uses the lo slot for its active-set mask (as R values)
   const int has_tb = (ADJ || (BOX && a.bounds_kind == 2)) ? 1 : 0;
   // global tile sequence of the sweep + first rollout pass: g < T -> t = T-1-g (backward), else t = g-T (forward)
   const int G = T + (a.do_rollout ? T : 0);
-  const size_t wsm = K::warp_smem_bytes(T, KSM, ADJ);
 
-  const int gw = blockIdx.x * NWC + warp;                   // global warp index
-  const int b0 = gw * PPW;
+  const int b0 = blockIdx.x * PPW;
   if (b0 >= B) return;                                      // warps are independent: no CTA-wide barrier below
   const int cnt = min(PPW, B - b0);
-  unsigned char* wbase = smem_raw + (size_t)warp * wsm;
+  unsigned char* wbase = smem_raw;
   uint64_t* full = reinterpret_cast<uint64_t*>(wbase);
   unsigned char* stage_base = wbase + K::HDR_BYTES;
   R* scratch = reinterpret_cast<R*>(stage_base + (size_t)S * K::STAGE_BYTES);
@@ -374,10 +353,6 @@ lqr_step2_kernel(const StepArgs a) {
   R kprev[M];
 #pragma unroll
   for (int q = 0; q < M; ++q) kprev[q] = R(0);
-#ifdef MPCB2_TIMING
-  long long tk[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tf[6] = {0, 0, 0, 0, 0, 0};
-  long long ck0, ck1;
-#endif
 
   // ======================= backward Riccati sweep (lqr_step.py:61-158) =======================
   // Software pipelined by hand: everything of step t-1 that does not depend on the value matrix (tile probe,
@@ -428,9 +403,6 @@ lqr_step2_kernel(const StepArgs a) {
   const R* st = acquire(0u);
   pre(T - 1, st);
   for (int t = T - 1; t >= 0; --t) {
-#ifdef MPCB2_TIMING
-    ck0 = clock64();
-#endif
     uint32_t ok_next = 0u;
     if (t > 0) ok_next = probe();                  // tile t-1: checked after the products
     if (t < T - 1) {                               // Q = C + F'VF, q = c_back + F'v  (:66-70)
@@ -460,7 +432,6 @@ lqr_step2_kernel(const StepArgs a) {
 #pragma unroll
       for (int k = 0; k < N; ++k) qp = fma2s(Fp[k], vv[k], qp);
     }
-    TICK2(tk, 2)
     // tile t is consumed (its C pair / rows / vectors were read by pre(t)): refill the stage with tile g + S
     __syncwarp();
     release(T - 1 - t);
@@ -470,7 +441,6 @@ lqr_step2_kernel(const StepArgs a) {
 #pragma unroll
       for (int k = 0; k < N; ++k) Fp[k] = ld_pair<R>(st_next + oF + k * P + c0);
     }
-    TICK2(tk, 7)
     // replicate Q_uu, q_u: control column a lives in lane base + NXL + a/2, component a%2
     R Quu[M][M], qu[M];
 #pragma unroll
@@ -480,7 +450,6 @@ lqr_step2_kernel(const StepArgs a) {
       for (int p1 = 0; p1 < M; ++p1) Quu[p1][a2] = shfl((a2 & 1) ? Qp[N + p1].y : Qp[N + p1].x, src);
       qu[a2] = shfl((a2 & 1) ? qp.y : qp.x, src);
     }
-    TICK2(tk, 3)
     R kk[M];
     unsigned fm = FULLM;
     int it = 0;
@@ -513,8 +482,8 @@ lqr_step2_kernel(const StepArgs a) {
       }
       bool conv, badpiv;
       pnqp_lane<R, M>(Quu, qu, lb, ub, t < T - 1, kk, fac, fm, it, conv, badpiv, a.pnqp_iters);
-      if (!conv) status |= 1u;
-      if (badpiv) status |= 4u;
+      if (!conv) status |= MPCB200_ST_PNQP_UNCONVERGED;
+      if (badpiv) status |= MPCB200_ST_BAD_PIVOT;
 #pragma unroll
       for (int q = 0; q < M; ++q) kprev[q] = kk[q];
     } else {                                       // unconstrained (:84-94) or u_zero_I masked (:100-127)
@@ -529,12 +498,11 @@ lqr_step2_kernel(const StepArgs a) {
         if (!f1) A[p1][p1] += R(1e-8);
       }
       fac.factor(A);
-      if (fac.bad) status |= 4u;
+      if (fac.bad) status |= MPCB200_ST_BAD_PIVOT;
       fac.solve(rhs, sol);
 #pragma unroll
       for (int q = 0; q < M; ++q) kk[q] = -sol[q];
     }
-    TICK2(tk, 4)
     // K[:, pair] = -Hff^{-1} Qux_f[:, pair] (rows of clamped / masked controls are zero)
     P2<R> Kp[M];
     R* Kt = KSM ? kst + (size_t)t * KT : kst;
@@ -588,7 +556,6 @@ lqr_step2_kernel(const StepArgs a) {
       }
     }
     __syncwarp();
-    TICK2(tk, 5)
     // V = Qxx + Qxu K + K'Qux + K'Quu K ; v = qx + Qxu k + K'qu + K'Quu k   (:155-158)
     {
       P2<R> Gp[M];                                 // (Qux + Quu K)[a][pair]
@@ -633,14 +600,12 @@ lqr_step2_kernel(const StepArgs a) {
         st_pair(vs + c0, vp);
       }
     }
-    TICK2(tk, 6)
     // V-independent part of step t-1, in the shadow of the V round trip through shared memory
     if (t > 0) {
       pre(t - 1, st_next);
       st = st_next;
     }
     __syncwarp();
-    TICK2(tk, 1)
   }
 
   // nominal cost (sum of the lanes' partial sums, fixed order)
@@ -727,9 +692,6 @@ lqr_step2_kernel(const StepArgs a) {
     R cpart = R(0), dun2 = R(0);
     size_t orow = (size_t)bsafe;                   // t*B + b
     for (int t = 0; t < T; ++t, orow += (size_t)B) {
-#ifdef MPCB2_TIMING
-      ck0 = clock64();
-#endif
       uint32_t ok_next = 0u;
       if (t + 1 < T) ok_next = probe();            // tile t+1
       R dxv[N];
@@ -759,7 +721,6 @@ lqr_step2_kernel(const StepArgs a) {
         const R d = tbu[q] - u[q];
         dun2 += d * d;
       }
-      TICK2(tf, 1)
       R tau[P];
 #pragma unroll
       for (int i = 0; i < N; ++i) tau[i] = xr[i];
@@ -796,7 +757,6 @@ lqr_step2_kernel(const StepArgs a) {
       if constexpr (ADJ) {                          // d tau_t of this pass, for the costate sweep
         if (writer_lane) st_pair(dts_all + ((size_t)pi * T + t) * P + c0, tj);
       }
-      TICK2(tf, 2)
       // operands of step t+1 into the (now dead) registers of step t
       const R* st_next = st;
       if (t + 1 < T) {
@@ -806,12 +766,10 @@ lqr_step2_kernel(const StepArgs a) {
       xown = xn;
       __syncwarp();
       if (t < T - 1) load_span<R, N, EA>(xs + (t & 1) * NV, xr);
-      TICK2(tf, 3)
       // tile t is consumed (its operands were loaded one step ago): refill its stage
       if (pass == 0) release(T + t);
       else if (t + S < T) issue(t + S, true);
       st = st_next;
-      TICK2(tf, 4)
     }
     if (writer_lane) red[lq] = cpart;
     __syncwarp();
@@ -826,12 +784,6 @@ lqr_step2_kernel(const StepArgs a) {
     const bool again = __any_sync(0xffffffffu, wr && worse) && more;          // per problem == the reference's batch loop
     if (!again) break;
   }
-#ifdef MPCB2_TIMING
-  if (lane == 0 && (gw % 97) == 0)
-    printf("warp %d T=%d bwd/step: WQ %lld issue+Fp %lld shfl %lld solve %lld Kexch %lld Vupd %lld pre %lld | fwd/step: u %lld dyn+cost %lld next+xchg %lld issue %lld\n",
-           gw, T, tk[2] / T, tk[7] / T, tk[3] / T, tk[4] / T, tk[5] / T, tk[6] / T, tk[1] / T,
-           tf[1] / T, tf[2] / T, tf[3] / T, tf[4] / T);
-#endif
   if constexpr (ADJ) {
     // ======================= costates and outer products (lqr_step.py:342-404) =======================
     // Third sweep, t = T-1 .. 0, over the same tiles (C, F, -r in the c slot, the true c, tau* in the x_bar/u_bar
@@ -927,9 +879,23 @@ lqr_step2_kernel(const StepArgs a) {
     ((R*)a.costs)[b] = cost;
     ((R*)a.full_du_norm)[b] = fdn;
     ((R*)a.alphas)[b] = alpha;
-    if (!(cost - cost == R(0))) status |= 2u;
+    if (!(cost - cost == R(0))) status |= MPCB200_ST_NONFINITE;
     if (a.status != nullptr) a.status[b] = (int)status;
   }
+}
+
+// launch_step2's answer when the column-pair mapping does not take the shape or the tensors' layout (or the fused
+// adjoint is asked of a mode other than MASK): the caller runs the generic kernel instead
+constexpr int STEP2_DECLINED = -1;
+
+template <auto Kern>
+int launch_step2_kernel(const StepArgs& a, int grid, size_t smem, int max_smem_optin, cudaStream_t stream) {
+  const int rc = allow_smem_optin<Kern>(max_smem_optin);
+  if (rc != MPCB200_OK) return rc;
+  Kern<<<grid, 32, smem, stream>>>(a);
+  if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
+  record_step_plan((int)(MPCB200_PLAN_PAIR | (a.k_in_smem ? MPCB200_PLAN_GAINS_SMEM : 0u)));
+  return MPCB200_OK;
 }
 
 template <typename R, int N, int M, int MODE>
@@ -937,43 +903,32 @@ int launch_step2_mode(const StepArgs& args, int max_smem_optin, cudaStream_t str
   using K = Step2Cfg<R, N, M>;
   StepArgs a = args;
   const bool adj = a.adj != 0;
-  if (adj && MODE != MODE_MASK) return -1;
-  a.k_in_smem = 1;
-  size_t smem = (size_t)K::NW * K::warp_smem_bytes(a.T, true, adj);
-  const bool have_ws = a.Ks != nullptr && a.ks != nullptr;
+  if (adj && MODE != MODE_MASK) return STEP2_DECLINED;
   // keep a few warps per SM resident: move the gain store to the caller's buffer when it is what limits them
-  const bool crowded = K::warp_smem_bytes(a.T, true, adj) > (size_t)max_smem_optin / 6;
-  if (smem > (size_t)max_smem_optin || (crowded && have_ws && a.do_rollout)) {
-    a.k_in_smem = 0;
-    smem = (size_t)K::NW * K::warp_smem_bytes(a.T, false, adj);
-    if (smem > (size_t)max_smem_optin) return 4;
-    if (a.do_rollout && !have_ws) return 4;
-  }
-  const int warps = (a.B + K::PPW - 1) / K::PPW;
-  const int grid = (warps + K::NW - 1) / K::NW;
-  auto go = [&](auto kern) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin) != cudaSuccess) return 5;
-    kern<<<grid, K::NW * 32, smem, stream>>>(a);
-    if (cudaGetLastError() != cudaSuccess) return 5;
-    record_step_plan((int)(MPCB200_PLAN_PAIR | (a.k_in_smem ? MPCB200_PLAN_GAINS_SMEM : 0u)));
-    return 0;
-  };
+  const bool crowded = K::smem_bytes(a.T, true, adj) > (size_t)max_smem_optin / 6;
+  size_t smem;
+  const int rc = plan_gain_store(a, crowded, max_smem_optin,
+                                 [&](bool k_in_smem) { return K::smem_bytes(a.T, k_in_smem, adj); }, smem);
+  if (rc != MPCB200_OK) return rc;
+  const int grid = (a.B + K::PPW - 1) / K::PPW;   // one warp per CTA
   if constexpr (MODE == MODE_MASK) {
     if (adj)                     // fused KKT adjoint (+ the d tau store)
-      return a.k_in_smem ? go(lqr_step2_kernel<R, N, M, MODE, true, true>) : go(lqr_step2_kernel<R, N, M, MODE, false, true>);
+      return a.k_in_smem ? launch_step2_kernel<lqr_step2_kernel<R, N, M, MODE, true, true>>(a, grid, smem, max_smem_optin, stream)
+                         : launch_step2_kernel<lqr_step2_kernel<R, N, M, MODE, false, true>>(a, grid, smem, max_smem_optin, stream);
   }
-  return a.k_in_smem ? go(lqr_step2_kernel<R, N, M, MODE, true>) : go(lqr_step2_kernel<R, N, M, MODE, false>);
+  return a.k_in_smem ? launch_step2_kernel<lqr_step2_kernel<R, N, M, MODE, true>>(a, grid, smem, max_smem_optin, stream)
+                     : launch_step2_kernel<lqr_step2_kernel<R, N, M, MODE, false>>(a, grid, smem, max_smem_optin, stream);
 }
 
 template <typename R, int N, int M>
 int launch_step2(const StepArgs& a, int max_smem_optin, cudaStream_t stream) {
   if constexpr (Step2Cfg<R, N, M>::OK) {
-    if (!a.bulk_ok) return -1;     // spans / bases not 16-byte aligned (odd batch sizes, sliced views): generic kernel
+    if (!a.bulk_ok) return STEP2_DECLINED;   // spans / bases not 16-byte aligned (odd batch sizes, sliced views)
     if (a.bounds_kind != 0) return launch_step2_mode<R, N, M, MODE_BOX>(a, max_smem_optin, stream);
     if (a.has_mask) return launch_step2_mode<R, N, M, MODE_MASK>(a, max_smem_optin, stream);
     return launch_step2_mode<R, N, M, MODE_PLAIN>(a, max_smem_optin, stream);
   } else {
-    return -1;
+    return STEP2_DECLINED;
   }
 }
 

@@ -2,7 +2,6 @@
 // One CTA per QP, runtime n.  The control flow and arithmetic per problem are those of pnqp_lane
 // (lqr_step.cuh), which keeps a whole QP in one thread's registers and therefore stops at n = 8.  Here the
 // threads of a block share one QP in shared memory; the iteration and its layout are in pnqp_cta.cuh.
-#include <atomic>
 #include "../../../include/mpcb200.h"
 #include "common.cuh"
 #include "pnqp.cuh"
@@ -61,17 +60,9 @@ __global__ void __launch_bounds__(NT) pnqp_cta_kernel(const PnqpArgs a) {
 
 template <typename R, int NT>
 static int launch(const PnqpArgs& a, int max_smem, cudaStream_t stream) {
-  auto kern = pnqp_cta_kernel<R, NT>;
-  // the opt-in shared-memory attribute is per device context; setting it twice is harmless
-  static std::atomic<int> configured[64];
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return MPCB200_ERR_NO_DEVICE;
-  if (configured[dev].load(std::memory_order_acquire) == 0) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem) != cudaSuccess)
-      return MPCB200_ERR_LAUNCH;
-    configured[dev].store(1, std::memory_order_release);
-  }
-  kern<<<a.B, NT, pnqp_cta_smem_bytes(a.n, (int)sizeof(R)), stream>>>(a);
+  const int rc = allow_smem_optin<pnqp_cta_kernel<R, NT>>(max_smem);
+  if (rc != MPCB200_OK) return rc;
+  pnqp_cta_kernel<R, NT><<<a.B, NT, pnqp_cta_smem_bytes(a.n, (int)sizeof(R)), stream>>>(a);
   return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH;
 }
 
