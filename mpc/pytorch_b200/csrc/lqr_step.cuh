@@ -5,11 +5,13 @@
 //   u_zero_I masked solve (:100-127), and lqr_forward's rollout + line search (:164-261).
 //
 // Mapping (designed for the GPU, not translated from the reference's per-op loop):
-//  * P = n+m lanes own one problem; lane j owns COLUMN j of every p-wide matrix of that
-//    problem (Q_t, F_t, C_t) and, for j < n, column j of the value matrix V and of K_t.
-//    32/P problems share a warp; NW consumer warps (the smallest count whose spans stay 16-byte
-//    aligned: small CTAs = fine load-balance granularity, the batch is < 1 wave) + 1 producer warp
-//    form a CTA.  The dense products run as pairs of independent FMA chains (common.cuh P2).
+//  * LP lanes own one problem, and slot s of lane j owns COLUMN j + s*LP of every p-wide matrix of
+//    that problem (Q_t, F_t, C_t) and, for a state column, that column of the value matrix V and of K_t.
+//    Most instances have LP = P = n+m and one slot; (8, 2) fp32 has LP = 8 and a second slot on lanes 0, 1
+//    for the control columns (StepCfg).  32/LP problems share a warp; NW consumer warps (the smallest
+//    count whose spans stay 16-byte aligned: small CTAs = fine load-balance granularity, the batch is
+//    < 1 wave; 2 for the (8, 2) layout) + 1 producer warp form a CTA.  The dense products run as pairs
+//    of independent FMA chains (common.cuh P2).
 //  * the producer warp streams the per-time-step tiles C[t],F[t],c[t],f[t],x_bar[t],u_bar[t]
 //    (+ tensor bounds) of the CTA's W consecutive problems - contiguous in the reference's
 //    time-major layout - into a 3-stage shared-memory ring with 1-D bulk TMA
@@ -68,19 +70,31 @@ struct StepCfg {
   static constexpr int P = N + M;
   static constexpr int EA = 16 / (int)sizeof(R);
   static_assert(P <= 32, "one problem must fit a warp");
-  static constexpr int CPL = 1;                     // columns per lane
-  static constexpr int LP = (P + CPL - 1) / CPL;   // lanes per problem
+  // Lane layout.  By default P lanes own one problem, one column each.  (8, 2) in fp32 uses n lanes: lane j
+  // keeps state column j, and lanes 0, 1 also keep control columns 8, 9 in a second slot.  A warp then holds
+  // 4 problems instead of 3 for about the same broadcast loads of V and F, and shared memory charges for the
+  // bytes delivered to lanes, which bound that kernel (DESIGN.md section 7).  fp64 keeps one column per lane:
+  // with the second slot it spilled under the 128-register cap of one-warp CTAs (92 B in PLAIN, 184 B in BOX).
+  static constexpr bool STATE_LANES = N == 8 && M == 2 && sizeof(R) == 4;
+  static constexpr int LP = STATE_LANES ? N : P;    // lanes per problem
+  static constexpr int CPL = (P + LP - 1) / LP;     // column slots per lane; slot s of lane j is column j + s*LP
   static constexpr int PPW = 32 / LP;               // problems per warp
+  // slot sl can hold a state column (compile time: the later slots of the (8, 2) layout hold controls only)
+  static constexpr bool x_slot(int sl) { return sl * LP < N; }
   // consumer warps per CTA: the smallest count whose per-time-step spans stay 16-byte aligned for every
   // tensor (so the bulk-TMA path applies).  Small CTAs matter: 4096 problems are < 1 wave, and the
   // kernel time is set by the most loaded SM, so the CTA granularity is the load-balance granularity.
   static constexpr bool span_ok(int nw) {
     return (nw * PPW * M * (int)sizeof(R)) % 16 == 0 && (nw * PPW * N * (int)sizeof(R)) % 16 == 0;
   }
-  static constexpr int NW = span_ok(1) ? 1 : span_ok(2) ? 2 : 4;
+  // The (8, 2) layout takes 2 (8 problems): one-warp CTAs measured slower on the H100 (DESIGN.md section 7).
+  static constexpr int NW = STATE_LANES ? 2 : span_ok(1) ? 1 : span_ok(2) ? 2 : 4;
   static constexpr int W = NW * PPW;      // problems per CTA
   static_assert(span_ok(NW), "CTA problem count must keep spans 16-byte aligned");
   static constexpr int THREADS = (NW + 1) * 32;
+  // resident CTAs per SM that the register budget must allow: config 3 (B = 4096) puts 32 problems on the
+  // busiest of 132 SMs, 4 CTAs of the (8, 2) layout
+  static constexpr int MIN_CTAS = STATE_LANES ? 32 / W : 0;
   static constexpr int S = 3;             // ring stages
   static constexpr int VS = round_up(N, 4);
   static constexpr int CS = P * P, FS = N * P;     // per-problem strides of the C and F tiles inside a stage
@@ -389,7 +403,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     const int col = j + sl * LP;
     wsl[sl] = writer_lane && col < P;
     cc[sl] = col < P ? col : P - 1;
-    isx[sl] = cc[sl] < N;
+    isx[sl] = K::x_slot(sl) && cc[sl] < N;
     ua[sl] = isx[sl] ? 0 : cc[sl] - N;       // control index of a u column
     fr[sl] = isx[sl] ? cc[sl] : N - 1;       // a valid row of F / V for every slot
   }
@@ -415,7 +429,9 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
   int stg = 0;
   uint32_t ph = 0;
   unsigned status = 0u;
-  R oldcost_part = R(0);
+  // cost partials of the nominal trajectory, one per owned column, summed in column order below.  One column per
+  // lane keeps the scalar: an array there changes the code of every single-column instance.
+  R oldcost_part = R(0), oldcost_slot[CPL] = {};
   R kprev[M];
 #pragma unroll
   for (int q = 0; q < M; ++q) kprev[q] = R(0);
@@ -450,7 +466,11 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
       const R Ct = Crow.dot(tb);
       const R cj = st[oc + cc[sl]];
       const R tbj = st[(isx[sl] ? ox : ou - N) + cc[sl]];
-      if (wsl[sl]) oldcost_part += tbj * (R(0.5) * Ct + cj);   // util.get_cost of the nominal trajectory (:169)
+      if constexpr (CPL == 1) {
+        if (wsl[sl]) oldcost_part += tbj * (R(0.5) * Ct + cj);       // util.get_cost of the nominal trajectory (:169)
+      } else {
+        if (wsl[sl]) oldcost_slot[sl] += tbj * (R(0.5) * Ct + cj);
+      }
       qj[sl] = Ct + cj;
     }
     if (t < T - 1) {                            // Q = C + F'VF, q = c_back + F'v  (:66-70)
@@ -644,12 +664,18 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     if (++stg == K::S) { stg = 0; ph ^= 1u; }
   }
 
-  // nominal cost  (sum of the lanes' partial sums, fixed order)
-  if (writer_lane) red[j] = oldcost_part;
+  // nominal cost  (sum of the columns' partial sums, in column order)
+  if constexpr (CPL == 1) {
+    if (writer_lane) red[j] = oldcost_part;
+  } else {
+#pragma unroll
+    for (int sl = 0; sl < CPL; ++sl)
+      if (wsl[sl]) red[cc[sl]] = oldcost_slot[sl];
+  }
   __syncwarp();
   R oldcost = R(0);
 #pragma unroll
-  for (int i = 0; i < LP; ++i) oldcost += red[i];
+  for (int i = 0; i < P; ++i) oldcost += red[i];
   __syncwarp();
 
   if (!a.do_rollout) {
@@ -672,8 +698,8 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     R xown[CPL];
 #pragma unroll
     for (int sl = 0; sl < CPL; ++sl) xown[sl] = valid ? gx0[(size_t)b * N + fr[sl]] : R(0);
-    R cpart = R(0), dun2 = R(0);
-    R kcol[M], kff[M];                           // KREDUCE with gains in global memory: column of K_t, k_t
+    R cpart = R(0), cpart_slot[CPL] = {}, dun2 = R(0);   // cost partials, as oldcost_part / oldcost_slot
+    R kcol[M], kff[M];                        // KREDUCE with gains in global memory: column of K_t, k_t
 #pragma unroll
     for (int q = 0; q < M; ++q) {
       kcol[q] = R(0);
@@ -781,7 +807,11 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
         Vec<R, P> Crow;
         Crow.template load<A_ROW>(st + oC + cc[sl] * P);
         const R Ct = Crow.dot(tau);
-        if (wsl[sl]) cpart += tj * (R(0.5) * Ct + st[oc + cc[sl]]);           // (:232)
+        if constexpr (CPL == 1) {
+          if (wsl[sl]) cpart += tj * (R(0.5) * Ct + st[oc + cc[sl]]);           // (:232)
+        } else {
+          if (wsl[sl]) cpart_slot[sl] += tj * (R(0.5) * Ct + st[oc + cc[sl]]);
+        }
         if (wr && wsl[sl]) {
           if (isx[sl]) {
             gnx[orow * N + cc[sl]] = tj;
@@ -791,7 +821,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
           }
         }
         xn[sl] = R(0);
-        if (t < T - 1) {                                          // (:217-222), or true_dynamics(x, u) (:224-225)
+        if (K::x_slot(sl) && t < T - 1) {                         // (:217-222), or true_dynamics(x, u) (:224-225)
           bool known = false;
           if constexpr (M == 1 && (N == DynDims<DYN_CARTPOLE>::N || N == DynDims<DYN_PENDULUM>::N)) {
             if (a.dyn_kind != DYN_LINEAR) {       // every lane evaluates the step function and keeps its row
@@ -824,11 +854,17 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
       if (lane == 0) mbar_arrive(&empty[stg]);
       if (++stg == K::S) { stg = 0; ph ^= 1u; }
     }
-    if (writer_lane) red[j] = cpart;
+    if constexpr (CPL == 1) {
+      if (writer_lane) red[j] = cpart;
+    } else {
+#pragma unroll
+      for (int sl = 0; sl < CPL; ++sl)
+        if (wsl[sl]) red[cc[sl]] = cpart_slot[sl];
+    }
     __syncwarp();
     cost = R(0);
 #pragma unroll
-    for (int i = 0; i < LP; ++i) cost += red[i];
+    for (int i = 0; i < P; ++i) cost += red[i];
     __syncwarp();
     if (pass == 0) fdn = sqrt(dun2);                              // (:243-245)
     worse = cost > oldcost;
@@ -851,7 +887,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
 }
 
 template <typename R, int N, int M, int MODE>
-__global__ void __launch_bounds__(StepCfg<R, N, M>::THREADS)
+__global__ void __launch_bounds__(StepCfg<R, N, M>::THREADS, StepCfg<R, N, M>::MIN_CTAS)
 lqr_step_kernel(const StepArgs a) {
   using K = StepCfg<R, N, M>;
   extern __shared__ __align__(128) unsigned char smem_raw[];

@@ -1,15 +1,17 @@
 """Is config 3 (T=20, n=8, m=2, fp32, unbounded) latency bound or throughput bound?  (developer tool)
 
 Runs the step over a sweep of batch sizes and reports us per launch and us per busiest-SM problem slot: the
-launch time over the number of problems the most loaded SM holds (ceil(CTAs / SMs) * problems per CTA).  At
-B=4096 an SM holds about 6 CTAs of the generic kernel; at B=65536 it keeps as many resident as registers allow
-and runs waves of them.  If one warp's dependent chain set the time, the extra resident warps would hide it and the
+launch time over the number of problems the most loaded SM holds (ceil(CTAs / SMs) * problems per CTA).  The
+generic kernel at (8, 2) fp32 puts 8 problems in a CTA (two consumer warps of 4 8-lane problems), so at B=4096 the
+busiest SM holds 4 CTAs; at B=65536 an SM keeps as many resident as registers and shared memory allow and runs
+waves of them.  If one warp's dependent chain set the time, the extra resident warps would hide it and the
 per-slot time would fall; if an SM resource saturates already at B=4096, the per-slot time stays flat.
 
-  python tools/exp_cfg3_bound.py [--riccati] [--batches 1024,4096,...]
+  python tools/exp_cfg3_bound.py [--riccati] [--batches 1024,4096,...] [--problems-per-cta 8]
 
 --riccati times the Riccati sweep alone (do_rollout = 0, gains written to Ks/ks).  The card's name, power limit
-and median SM clock under the load are printed with the numbers.
+and median SM clock under the load are printed with the numbers.  --problems-per-cta gives the CTA size of another
+build of the library (MPCB200_LIB), e.g. 6 for the earlier layout of 3 problems per warp and 2 consumer warps.
 """
 import argparse
 import ctypes
@@ -23,7 +25,7 @@ import torch  # noqa: E402
 import bench  # noqa: E402
 
 T, N, M = 20, 8, 2
-PROBLEMS_PER_CTA = 6        # the generic kernel at (8, 2) f32: 2 consumer warps x 3 problems
+PROBLEMS_PER_CTA = 8        # the generic kernel at (8, 2) f32: 2 consumer warps x 4 problems
 
 
 def main():
@@ -31,6 +33,7 @@ def main():
     ap.add_argument("--riccati", action="store_true")
     ap.add_argument("--batches", default="1024,2048,4096,8192,16384,65536")
     ap.add_argument("--reps", type=int, default=0, help="launches per timed block (0: ~0.2 s of work)")
+    ap.add_argument("--problems-per-cta", type=int, default=PROBLEMS_PER_CTA)
     args = ap.parse_args()
     from mpc.pytorch_b200 import _lib
     dev = torch.device("cuda:0")
@@ -55,7 +58,8 @@ def main():
         plan = _lib.last_step_plan()
         if not plan & _lib.PLAN_GENERIC:
             raise SystemExit(f"expected the generic kernel at (8, 2) f32, the plan was {plan}")
-        busiest = math.ceil(math.ceil(B / PROBLEMS_PER_CTA) / sms) * PROBLEMS_PER_CTA
+        w = args.problems_per_cta
+        busiest = math.ceil(math.ceil(B / w) / sms) * w
         rows.append((B, us / busiest))
         print(f"B={B:6d}  {us:9.1f} us/launch  busiest SM {busiest:4d} problems  {us / busiest:6.3f} us/slot",
               flush=True)
