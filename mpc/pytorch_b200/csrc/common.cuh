@@ -52,6 +52,19 @@ MPCB_DEV void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uin
       "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// The same copy with an L2 cache policy (createpolicy) for the lines it reads.
+MPCB_DEV void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+MPCB_DEV uint64_t l2_evict_first_policy() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
 // CTA-wide named barrier.  `bar.sync` is the .aligned form (the whole warp must execute it
 // convergently); callers reach it right after lane-divergent code, so reconverge first and use the
 // non-aligned `barrier.sync` (compute-sanitizer synccheck flagged the aligned form here).

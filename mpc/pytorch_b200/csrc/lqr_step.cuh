@@ -21,7 +21,7 @@
 //    broadcast vector loads; the m x m solve / pnqp runs redundantly on every lane of the
 //    problem from shuffled copies of Q_uu, q_u (registers only, no divergence inside a problem).
 //  * K_t,k_t for all t stay in shared memory between the backward sweep and the rollout;
-//    the rollout re-streams the tiles (L2 hits) and never round-trips gains through HBM
+//    the rollout re-streams the tiles (L2 hits, read evict-first) and never round-trips gains through HBM
 //    (unless T is too long for shared memory, then a caller-provided Ks/ks buffer is used).
 //  * line search: per-problem alpha; a CTA repeats the rollout while any of its problems is
 //    worse and iterations remain - per problem this is exactly the reference's batch loop.
@@ -292,6 +292,14 @@ MPCB_DEV void step_producer(const StepArgs& a, unsigned char* stage_base, uint64
   const int T = a.T;
   int s = 0;
   uint32_t ph = 0;
+  // The rollout reads each tile for the last time (a line-search repeat re-reads them, rarely).  Marking those
+  // reads evict-first keeps the tiles the rollout has not reached yet in L2: at config 3 the tiles of one launch
+  // (59 MB) exceed L2, and plain LRU replacement evicts exactly the lines the rollout reads next.
+  const uint64_t last_use = l2_evict_first_policy();
+  auto g2s = [&](void* dst, const void* src, uint32_t bytes, uint64_t* bar, bool fwd) {
+    if (fwd) bulk_g2s(dst, src, bytes, bar, last_use);
+    else bulk_g2s(dst, src, bytes, bar);
+  };
 
   auto issue = [&](int t, bool fwd) {
     mbar_wait(&empty[s], ph ^ 1u);
@@ -314,26 +322,26 @@ MPCB_DEV void step_producer(const StepArgs& a, unsigned char* stage_base, uint64
         if (a.bounds_kind == 2) bytes += 2u * cnt * M * SZ;
         mbar_arrive_expect_tx(&full[s], bytes);
         if constexpr (K::CS == P * P) {
-          bulk_g2s(st + K::OFF_C, gC + tC, (uint32_t)cnt * P * P * SZ, &full[s]);
+          g2s(st + K::OFF_C, gC + tC, (uint32_t)cnt * P * P * SZ, &full[s], fwd);
         } else {
           for (int q = 0; q < cnt; ++q)
-            bulk_g2s(st + K::OFF_C + q * K::CS, gC + tC + (size_t)q * P * P, (uint32_t)P * P * SZ, &full[s]);
+            g2s(st + K::OFF_C + q * K::CS, gC + tC + (size_t)q * P * P, (uint32_t)P * P * SZ, &full[s], fwd);
         }
         if (needF) {
           if constexpr (K::FS == N * P) {
-            bulk_g2s(st + K::OFF_F, gF + tF, (uint32_t)cnt * N * P * SZ, &full[s]);
+            g2s(st + K::OFF_F, gF + tF, (uint32_t)cnt * N * P * SZ, &full[s], fwd);
           } else {
             for (int q = 0; q < cnt; ++q)
-              bulk_g2s(st + K::OFF_F + q * K::FS, gF + tF + (size_t)q * N * P, (uint32_t)N * P * SZ, &full[s]);
+              g2s(st + K::OFF_F + q * K::FS, gF + tF + (size_t)q * N * P, (uint32_t)N * P * SZ, &full[s], fwd);
           }
         }
-        bulk_g2s(st + K::OFF_c, gc + tc, (uint32_t)cnt * P * SZ, &full[s]);
-        if (needf) bulk_g2s(st + K::OFF_f, gf + tf_, (uint32_t)cnt * N * SZ, &full[s]);
-        bulk_g2s(st + K::OFF_x, gx + tb * N, (uint32_t)cnt * N * SZ, &full[s]);
-        bulk_g2s(st + K::OFF_u, gu + tb * M, (uint32_t)cnt * M * SZ, &full[s]);
+        g2s(st + K::OFF_c, gc + tc, (uint32_t)cnt * P * SZ, &full[s], fwd);
+        if (needf) g2s(st + K::OFF_f, gf + tf_, (uint32_t)cnt * N * SZ, &full[s], fwd);
+        g2s(st + K::OFF_x, gx + tb * N, (uint32_t)cnt * N * SZ, &full[s], fwd);
+        g2s(st + K::OFF_u, gu + tb * M, (uint32_t)cnt * M * SZ, &full[s], fwd);
         if (a.bounds_kind == 2) {
-          bulk_g2s(st + K::OFF_lo, glo + tb * M, (uint32_t)cnt * M * SZ, &full[s]);
-          bulk_g2s(st + K::OFF_hi, ghi + tb * M, (uint32_t)cnt * M * SZ, &full[s]);
+          g2s(st + K::OFF_lo, glo + tb * M, (uint32_t)cnt * M * SZ, &full[s], fwd);
+          g2s(st + K::OFF_hi, ghi + tb * M, (uint32_t)cnt * M * SZ, &full[s], fwd);
         }
       }
     } else {
