@@ -279,15 +279,7 @@ __global__ void __launch_bounds__(LNT) lqr_large_step_kernel(const __grid_consta
       }
       for (int i = tid; i < m; i += LNT) {
         qq[i] = qv[n + i];
-        const R lo_abs = box2 ? lo_t[i] : s_lo;
-        const R hi_abs = box2 ? hi_t[i] : s_hi;
-        R lb = lo_abs - us[i], ub = hi_abs - us[i];
-        if (a.has_delta) {
-          if (lb < -s_du) lb = -s_du;
-          if (ub > s_du) ub = s_du;
-        }
-        plo[i] = lb;
-        phi[i] = ub;
+        qp_box<R>(box2 ? lo_t[i] : s_lo, box2 ? hi_t[i] : s_hi, us[i], a.has_delta, s_du, plo[i], phi[i]);
       }
       __syncthreads();
       bool conv, badpiv;
@@ -378,7 +370,7 @@ __global__ void __launch_bounds__(LNT) lqr_large_step_kernel(const __grid_consta
   block_sum2<R, LNT>(oldcost, dummy, red);
 
   if (!a.do_rollout) {
-    if (tid == 0 && a.status != nullptr) a.status[b] = (int)status;
+    if (tid == 0) write_step_status(a, b, status);
     return;
   }
 
@@ -422,19 +414,8 @@ __global__ void __launch_bounds__(LNT) lqr_large_step_kernel(const __grid_consta
         const R* dx = W + m * n;
         R s = R(0);
         for (int i = 0; i < n; ++i) s += Kq[i] * dx[i];
-        R u = (s + us[q]) + alpha * gq[q];
-        if (has_mask && mk[q]) u = R(0);
-        if (mode == MODE_BOX) {
-          R lo = box2 ? lo_t[q] : s_lo;
-          R hi = box2 ? hi_t[q] : s_hi;
-          if (a.has_delta) {
-            const R l2 = us[q] - s_du, h2 = us[q] + s_du;
-            lo = l2 < lo ? lo : l2;
-            hi = h2 > hi ? hi : h2;
-          }
-          u = u < lo ? lo : u;
-          u = u > hi ? hi : u;
-        }
+        const R u = rollout_control<R>((s + us[q]) + alpha * gq[q], us[q], has_mask && mk[q], mode == MODE_BOX,
+                                       box2 ? lo_t[q] : s_lo, box2 ? hi_t[q] : s_hi, a.has_delta, s_du);
         const R d = us[q] - u;
         du2 += d * d;
         tau[n + q] = u;
@@ -469,20 +450,12 @@ __global__ void __launch_bounds__(LNT) lqr_large_step_kernel(const __grid_consta
     }
     block_sum2<R, LNT>(cpart, du2, red);
     cost = cpart;
-    if (pass == 0) fdn = sqrt(du2);                          // (:243-245)
-    worse = cost > oldcost;
+    worse = line_search_update<R>(pass, cost, oldcost, du2, decay, fdn, alpha);
     const bool more = pass + 1 < a.max_ls;
-    if (worse) alpha *= decay;                               // (:247)
     if (!worse || !more) break;
   }
   if (worse) alpha /= decay;                                 // (:252)
-  if (tid == 0) {
-    ((R*)a.costs)[b] = cost;
-    ((R*)a.full_du_norm)[b] = fdn;
-    ((R*)a.alphas)[b] = alpha;
-    if (!(cost - cost == R(0))) status |= MPCB200_ST_NONFINITE;
-    if (a.status != nullptr) a.status[b] = (int)status;
-  }
+  if (tid == 0) write_step_result<R>(a, b, alpha, cost, fdn, status);
 }
 
 template <typename R>

@@ -270,6 +270,120 @@ int plan_gain_store(StepArgs& a, bool prefers_ws, int max_smem_optin, SmemFn sme
   return MPCB200_OK;
 }
 
+// The QP box of one control relative to the nominal u_bar (lqr_step.py:129-148): [lo - u_bar, hi - u_bar],
+// clipped to +-delta_u when a slew limit is set.
+template <typename R>
+MPCB_DEV void qp_box(R lo_abs, R hi_abs, R ubar, bool has_delta, R du, R& lb, R& ub) {
+  lb = lo_abs - ubar;
+  ub = hi_abs - ubar;
+  if (has_delta) {
+    if (lb < -du) lb = -du;
+    if (ub > du) ub = du;
+  }
+}
+
+// The control solve of one time step, run redundantly by every lane of a problem (registers only), in two forms.
+// Both give the feedforward kk and the factor of the free block of Q_uu that the gains are solved with, and OR
+// MPCB200_ST_* bits into status.
+//
+// BOX (:129-148): pnqp on the box, warm started from kprev (which it updates).  Gives the free set fm and the pnqp
+// iterations it.  The tensor bounds and u_bar come as callables q -> R, so each kernel reads them where it keeps them.
+template <typename R, int M, typename Lo, typename Hi, typename Ubar>
+MPCB_DEV void box_control_solve(const StepArgs& a, R (&Quu)[M][M], R (&qu)[M], R (&kprev)[M], bool valid, bool warm,
+                                Lo lo_t, Hi hi_t, Ubar ubar, R (&kk)[M], unsigned& fm, int& it, Ldl<R, M>& fac,
+                                unsigned& status) {
+  const R s_lo = (R)a.u_lo, s_hi = (R)a.u_hi, s_du = (R)a.delta_u;
+  R lb[M], ub[M];
+#pragma unroll
+  for (int q = 0; q < M; ++q) {
+    qp_box<R>(a.bounds_kind == 2 ? lo_t(q) : s_lo, a.bounds_kind == 2 ? hi_t(q) : s_hi, ubar(q), a.has_delta, s_du,
+              lb[q], ub[q]);
+    kk[q] = kprev[q];
+  }
+  if (!valid) {   // padding problems of a tail CTA or warp compute on stale shared memory: give their
+                  // (data dependent) pnqp loop a trivial QP so they never become the slowest problem
+#pragma unroll
+    for (int p1 = 0; p1 < M; ++p1) {
+#pragma unroll
+      for (int p2 = 0; p2 < M; ++p2) Quu[p1][p2] = p1 == p2 ? R(1) : R(0);
+      qu[p1] = R(0);
+      lb[p1] = R(-1);
+      ub[p1] = R(1);
+      kk[p1] = R(0);
+    }
+  }
+  bool conv, badpiv;
+  pnqp_lane<R, M>(Quu, qu, lb, ub, warm, kk, fac, fm, it, conv, badpiv, a.pnqp_iters);
+  if (!conv) status |= MPCB200_ST_PNQP_UNCONVERGED;
+  if (badpiv) status |= MPCB200_ST_BAD_PIVOT;
+#pragma unroll
+  for (int q = 0; q < M; ++q) kprev[q] = kk[q];
+}
+
+// PLAIN (:84-94) and MASK (:100-127): the LDL^T solve on the free set fm (all controls, or those u_zero_I leaves free);
+// the rows and columns of the other controls are zeroed, with 1e-8 on their diagonal.
+template <typename R, int M>
+MPCB_DEV void ldl_control_solve(const R (&Quu)[M][M], const R (&qu)[M], unsigned fm, R (&kk)[M], Ldl<R, M>& fac,
+                                unsigned& status) {
+  R A[M][M], rhs[M], sol[M];
+#pragma unroll
+  for (int p1 = 0; p1 < M; ++p1) {
+    const bool f1 = (fm >> p1) & 1u;
+    rhs[p1] = f1 ? qu[p1] : R(0);
+#pragma unroll
+    for (int p2 = 0; p2 < M; ++p2) A[p1][p2] = (f1 && ((fm >> p2) & 1u)) ? Quu[p1][p2] : R(0);
+    if (!f1) A[p1][p1] += R(1e-8);
+  }
+  fac.factor(A);
+  if (fac.bad) status |= MPCB200_ST_BAD_PIVOT;
+  fac.solve(rhs, sol);
+#pragma unroll
+  for (int q = 0; q < M; ++q) kk[q] = -sol[q];
+}
+
+// One control of a rollout (lqr_step.py:197-213), given u = K dx + u_bar + alpha k: zeroed where u_zero_I is set,
+// then (box) clamped to [lo, hi] intersected with u_bar +- delta_u, lower bound first like util.eclamp.
+template <typename R>
+MPCB_DEV R rollout_control(R u, R ubar, bool masked, bool box, R lo, R hi, bool has_delta, R du) {
+  if (masked) u = R(0);
+  if (box) {
+    if (has_delta) {
+      const R l2 = ubar - du, h2 = ubar + du;
+      lo = l2 < lo ? lo : l2;
+      hi = h2 > hi ? hi : h2;
+    }
+    u = u < lo ? lo : u;
+    u = u > hi ? hi : u;
+  }
+  return u;
+}
+
+// The line search after a rollout pass (lqr_step.py:243-247): the first pass gives ||du||, a cost worse than the
+// nominal one shrinks alpha.  Returns whether the pass was worse; the kernel decides whether another pass runs.
+template <typename R>
+MPCB_DEV bool line_search_update(int pass, R cost, R oldcost, R du2, R decay, R& fdn, R& alpha) {
+  if (pass == 0) fdn = sqrt(du2);
+  const bool worse = cost > oldcost;
+  if (worse) alpha *= decay;
+  return worse;
+}
+
+MPCB_DEV void write_step_status(const StepArgs& a, int b, unsigned status) {
+  if (a.status != nullptr) a.status[b] = (int)status;
+}
+
+// The per-problem results of a step with a rollout.  The kernels undo the last shrink of a worse final pass
+// (alpha /= decay, :252) themselves: done in here, ptxas schedules the PLAIN kernels differently (DESIGN.md
+// section 7).
+template <typename R>
+MPCB_DEV void write_step_result(const StepArgs& a, int b, R alpha, R cost, R fdn, unsigned status) {
+  ((R*)a.costs)[b] = cost;
+  ((R*)a.full_du_norm)[b] = fdn;
+  ((R*)a.alphas)[b] = alpha;
+  if (!(cost - cost == R(0))) status |= MPCB200_ST_NONFINITE;
+  write_step_status(a, b, status);
+}
+
 // ---------------------------------------------------------------------------------------------
 // producer warp: stream one (t) tile set of the CTA's problems into ring stage `tile % S`
 // ---------------------------------------------------------------------------------------------
@@ -518,6 +632,9 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
       for (int p1 = 0; p1 < M; ++p1) Quu[p1][p2] = shfl(Qc[(N + p2) / LP].get(N + p1), src);
       qu[p2] = shfl(qj[(N + p2) / LP], src);
     }
+    // This kernel keeps its own copy of box_control_solve and ldl_control_solve: with the shared ones, ptxas contracts
+    // the f64 (8, 2) BOX kernel's multiplies and adds differently, so its outputs are no longer bitwise the same, and
+    // it compiles the PLAIN kernels, config 3's among them, differently (DESIGN.md section 7).
     R kk[M];
     unsigned fm = FULLM;
     int it = 0;
@@ -687,7 +804,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
   __syncwarp();
 
   if (!a.do_rollout) {
-    if (wr && j == 0 && a.status != nullptr) a.status[b] = (int)status;
+    if (wr && j == 0) write_step_status(a, b, status);
     return;
   }
 
@@ -778,7 +895,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
         }
       }
 #pragma unroll
-      for (int q = 0; q < M; ++q) {
+      for (int q = 0; q < M; ++q) {               // own copy of rollout_control, for the same reason
         if constexpr (MODE != MODE_PLAIN) {
           if (has_mask && mk[q]) u[q] = R(0);                     // (:197-198)
         }
@@ -874,10 +991,8 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
 #pragma unroll
     for (int i = 0; i < P; ++i) cost += red[i];
     __syncwarp();
-    if (pass == 0) fdn = sqrt(dun2);                              // (:243-245)
-    worse = cost > oldcost;
+    worse = line_search_update<R>(pass, cost, oldcost, dun2, decay, fdn, alpha);
     const bool more = pass + 1 < a.max_ls;
-    if (worse) alpha *= decay;                                    // (:247)
     if (wr && j == 0 && worse && more) votes[pass & 31] = 1;
     if (warp == 0 && lane == 0) votes[(pass + 16) & 31] = 0;
     named_bar_sync(1, K::THREADS);
@@ -885,13 +1000,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     if (!cont || !more) break;
   }
   if (worse) alpha /= decay;                                      // (:252)
-  if (wr && j == 0) {
-    ((R*)a.costs)[b] = cost;
-    ((R*)a.full_du_norm)[b] = fdn;
-    ((R*)a.alphas)[b] = alpha;
-    if (!(cost - cost == R(0))) status |= MPCB200_ST_NONFINITE;
-    if (a.status != nullptr) a.status[b] = (int)status;
-  }
+  if (wr && j == 0) write_step_result<R>(a, b, alpha, cost, fdn, status);
 }
 
 template <typename R, int N, int M, int MODE>

@@ -454,54 +454,12 @@ lqr_step2_kernel(const StepArgs a) {
     unsigned fm = FULLM;
     int it = 0;
     Ldl<R, M> fac;
-    if constexpr (BOX) {                           // (:129-148)
-      R lb[M], ub[M];
-#pragma unroll
-      for (int q = 0; q < M; ++q) {
-        const R lo_abs = a.bounds_kind == 2 ? blo[q] : s_lo;
-        const R hi_abs = a.bounds_kind == 2 ? bhi[q] : s_hi;
-        lb[q] = lo_abs - ubar[q];
-        ub[q] = hi_abs - ubar[q];
-        if (a.has_delta) {
-          if (lb[q] < -s_du) lb[q] = -s_du;
-          if (ub[q] > s_du) ub[q] = s_du;
-        }
-        kk[q] = kprev[q];
-      }
-      if (!valid) {   // padding problems of a tail warp compute on stale shared memory: give their
-                      // (data dependent) pnqp loop a trivial QP so they never become the slowest problem
-#pragma unroll
-        for (int p1 = 0; p1 < M; ++p1) {
-#pragma unroll
-          for (int p2 = 0; p2 < M; ++p2) Quu[p1][p2] = p1 == p2 ? R(1) : R(0);
-          qu[p1] = R(0);
-          lb[p1] = R(-1);
-          ub[p1] = R(1);
-          kk[p1] = R(0);
-        }
-      }
-      bool conv, badpiv;
-      pnqp_lane<R, M>(Quu, qu, lb, ub, t < T - 1, kk, fac, fm, it, conv, badpiv, a.pnqp_iters);
-      if (!conv) status |= MPCB200_ST_PNQP_UNCONVERGED;
-      if (badpiv) status |= MPCB200_ST_BAD_PIVOT;
-#pragma unroll
-      for (int q = 0; q < M; ++q) kprev[q] = kk[q];
-    } else {                                       // unconstrained (:84-94) or u_zero_I masked (:100-127)
+    if constexpr (BOX) {
+      box_control_solve<R, M>(a, Quu, qu, kprev, valid, t < T - 1, [&](int q) { return blo[q]; },
+                              [&](int q) { return bhi[q]; }, [&](int q) { return ubar[q]; }, kk, fm, it, fac, status);
+    } else {
       if constexpr (MODE == MODE_MASK) fm = FULLM & ~zmk;
-      R A[M][M], rhs[M], sol[M];
-#pragma unroll
-      for (int p1 = 0; p1 < M; ++p1) {
-        const bool f1 = (fm >> p1) & 1u;
-        rhs[p1] = f1 ? qu[p1] : R(0);
-#pragma unroll
-        for (int p2 = 0; p2 < M; ++p2) A[p1][p2] = (f1 && ((fm >> p2) & 1u)) ? Quu[p1][p2] : R(0);
-        if (!f1) A[p1][p1] += R(1e-8);
-      }
-      fac.factor(A);
-      if (fac.bad) status |= MPCB200_ST_BAD_PIVOT;
-      fac.solve(rhs, sol);
-#pragma unroll
-      for (int q = 0; q < M; ++q) kk[q] = -sol[q];
+      ldl_control_solve<R, M>(Quu, qu, fm, kk, fac, status);
     }
     // K[:, pair] = -Hff^{-1} Qux_f[:, pair] (rows of clamped / masked controls are zero)
     P2<R> Kp[M];
@@ -617,7 +575,7 @@ lqr_step2_kernel(const StepArgs a) {
   __syncwarp();
 
   if (!a.do_rollout) {
-    if (wr && lq == 0 && a.status != nullptr) a.status[b] = (int)status;
+    if (wr && lq == 0) write_step_status(a, b, status);
     return;
   }
 
@@ -704,20 +662,9 @@ lqr_step2_kernel(const StepArgs a) {
       P2<R> ubj = {tbu[0], tbu[1]};
 #pragma unroll
       for (int q = 0; q < M; ++q) {
-        if constexpr (MODE != MODE_PLAIN) {
-          if (has_mask && ((zm >> q) & 1u)) u[q] = R(0);                    // (:197-198)
-        }
-        if constexpr (BOX) {                                                // (:200-213)
-          R lo = a.bounds_kind == 2 ? lo_t[q] : s_lo;
-          R hi = a.bounds_kind == 2 ? hi_t[q] : s_hi;
-          if (a.has_delta) {
-            const R l2 = tbu[q] - s_du, h2 = tbu[q] + s_du;
-            lo = l2 < lo ? lo : l2;
-            hi = h2 > hi ? hi : h2;
-          }
-          u[q] = u[q] < lo ? lo : u[q];                                       // util.eclamp: lower, then upper
-          u[q] = u[q] > hi ? hi : u[q];
-        }
+        u[q] = rollout_control<R>(u[q], tbu[q], MODE != MODE_PLAIN && has_mask && ((zm >> q) & 1u), BOX,
+                                  a.bounds_kind == 2 ? lo_t[q] : s_lo, a.bounds_kind == 2 ? hi_t[q] : s_hi,
+                                  a.has_delta, s_du);
         const R d = tbu[q] - u[q];
         dun2 += d * d;
       }
@@ -777,10 +724,8 @@ lqr_step2_kernel(const StepArgs a) {
 #pragma unroll
     for (int i = 0; i < L; ++i) cost += red[i];
     __syncwarp();
-    if (pass == 0) fdn = sqrt(dun2);                                          // (:243-245)
-    worse = cost > oldcost;
+    worse = line_search_update<R>(pass, cost, oldcost, dun2, decay, fdn, alpha);
     const bool more = pass + 1 < a.max_ls;
-    if (worse) alpha *= decay;                                                // (:247)
     const bool again = __any_sync(0xffffffffu, wr && worse) && more;          // per problem == the reference's batch loop
     if (!again) break;
   }
@@ -875,13 +820,7 @@ lqr_step2_kernel(const StepArgs a) {
     if (wr && isx) st_pair((R*)a.adj_dx_init + (size_t)b * N + c0, P2<R>{-dl_own.x, -dl_own.y});
   }
   if (worse) alpha /= decay;                                                  // (:252)
-  if (wr && lq == 0) {
-    ((R*)a.costs)[b] = cost;
-    ((R*)a.full_du_norm)[b] = fdn;
-    ((R*)a.alphas)[b] = alpha;
-    if (!(cost - cost == R(0))) status |= MPCB200_ST_NONFINITE;
-    if (a.status != nullptr) a.status[b] = (int)status;
-  }
+  if (wr && lq == 0) write_step_result<R>(a, b, alpha, cost, fdn, status);
 }
 
 // launch_step2's answer when the column-pair mapping does not take the shape or the tensors' layout (or the fused
