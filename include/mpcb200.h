@@ -40,7 +40,8 @@ enum {
   MPCB200_ERR_UNSUPPORTED_DIMS = 3,  /* (n,m) has no compiled kernel instance               */
   MPCB200_ERR_SMEM = 4,              /* problem does not fit shared memory and no workspace */
   MPCB200_ERR_LAUNCH = 5,            /* cudaGetLastError() after launch != cudaSuccess      */
-  MPCB200_ERR_NO_DEVICE = 6          /* no usable sm_90 device / wrong architecture         */
+  MPCB200_ERR_NO_DEVICE = 6,         /* no usable sm_90 device / wrong architecture         */
+  MPCB200_ERR_NO_GRAPH_COND = 7      /* conditional graph nodes unavailable (driver < 12.3)  */
 };
 
 /* Problem sizes and options.  Mirrors the closure arguments of
@@ -245,6 +246,53 @@ int32_t mpcb200_pnqp_max_n(int32_t elem_size);
  * instance exists.
  */
 int mpcb200_step_large_fits(const mpcb200_dims* dims, int32_t elem_size);
+
+/*
+ * The whole iLQR loop of MPC.forward (reference mpc/mpc.py:244-301) on the device, with a QuadCost(C, c) and either
+ * LinDx(F, f) dynamics or a known system (dims->dynamics_kind, params->dyn; F and f are then NULL and the
+ * linearisation is recomputed on the device every iteration).  One CUDA graph: an init kernel, then a conditional
+ * `while` node whose body is
+ *   LinDx:        rollout -> step -> track -> stop
+ *   known system: rollout -> linearisation (F, f into the workspace) -> step with in-kernel dynamics -> track -> stop
+ * The step runs with dims/params exactly as mpcb200_lqr_step_* (do_rollout = 1; du_first and status are requested,
+ * qp_iters and free_mask are not; Ks/ks go into the workspace when mpcb200_step_prefers_workspace asks for them), so
+ * mpcb200_last_step_plan reports its plan.  The track kernel keeps, per problem, the iterate of the lowest cost so far
+ * (`costs <= best_costs + best_cost_eps`, evaluated in the element type), carries the latest controls forward and forms
+ * the reference's batch-mixing full_du_norm over the caller's m_ref controls; the stop kernel ends the loop when
+ * max_b full_du_norm < eps (a NaN never does), when more than not_improved_lim iterations in a row improved no problem,
+ * or after lqr_iter iterations.
+ *
+ * u_init[T,B,m] or NULL (zeros).  Outputs best_x[T,B,n] best_u[T,B,m] best_costs[B] best_full_du_norm[B] and
+ * info[2] (int32, device): iterations run, iterations in which some problem's pnqp did not converge.
+ * workspace: device buffer of mpcb200_ilqr_workspace_bytes() bytes, 256-byte aligned, contents undefined on return.
+ * If `stream` is capturing (cudaStreamIsCapturing), nothing is launched: the init kernel and the conditional node
+ * join the caller's capture graph, which makes the whole solve capturable.  Otherwise the graph is instantiated,
+ * launched on `stream` and its executable destroyed; the call does not synchronise the host.
+ * mpcb200_launch_count counts each kernel node of the graph once, when the node is added; the number of iterations
+ * the loop ran is info[0].  Returns MPCB200_ERR_NO_GRAPH_COND (before launching anything) when the driver has no
+ * conditional nodes.
+ */
+typedef struct mpcb200_ilqr_opts {
+  int32_t lqr_iter;          /* >= 1                                                                          */
+  int32_t not_improved_lim;
+  int32_t m_ref;             /* the caller's n_ctrl (<= dims->m when zero padded): full_du_norm mixes over these */
+  int32_t reserved0;
+  double eps, best_cost_eps;
+} mpcb200_ilqr_opts;
+
+size_t mpcb200_ilqr_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size);
+int mpcb200_ilqr_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                     const float* C, const float* c, const float* F, const float* f,
+                     const float* x_init, const float* u_init,
+                     const float* u_lower, const float* u_upper, const uint8_t* u_zero_I,
+                     float* best_x, float* best_u, float* best_costs, float* best_full_du_norm,
+                     int32_t* info, void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                     const double* C, const double* c, const double* F, const double* f,
+                     const double* x_init, const double* u_init,
+                     const double* u_lower, const double* u_upper, const uint8_t* u_zero_I,
+                     double* best_x, double* best_u, double* best_costs, double* best_full_du_norm,
+                     int32_t* info, void* workspace, size_t workspace_bytes, void* stream);
 
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);

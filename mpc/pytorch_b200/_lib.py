@@ -27,8 +27,16 @@ class Params(ctypes.Structure):
     _fields_ = [(k, ctypes.c_double) for k in ("u_lo", "u_hi", "delta_u", "ls_decay")] + [("dyn", ctypes.c_double * 8)]
 
 
+class IlqrOpts(ctypes.Structure):
+    _fields_ = [(k, ctypes.c_int32) for k in ("lqr_iter", "not_improved_lim", "m_ref", "reserved0")] + \
+        [(k, ctypes.c_double) for k in ("eps", "best_cost_eps")]
+
+
 class MpcB200Error(RuntimeError):
     pass
+
+
+ERR_NO_GRAPH_COND = 7   # MPCB200_ERR_NO_GRAPH_COND: the driver has no conditional graph nodes (before CUDA 12.3)
 
 
 _lib = None
@@ -41,7 +49,8 @@ EXPORTED_SYMBOLS = (
     "mpcb200_dyn_rollout_f32", "mpcb200_dyn_rollout_f64", "mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64",
     "mpcb200_supported", "mpcb200_supported_list", "mpcb200_launch_count",
     "mpcb200_step_smem_bytes", "mpcb200_step_prefers_workspace", "mpcb200_last_step_plan", "mpcb200_version",
-    "mpcb200_strerror", "mpcb200_step_large_fits",
+    "mpcb200_strerror", "mpcb200_step_large_fits", "mpcb200_ilqr_f32", "mpcb200_ilqr_f64",
+    "mpcb200_ilqr_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -93,6 +102,13 @@ def lib():
         fn = getattr(L, name)
         fn.argtypes = [ctypes.c_int32, ctypes.POINTER(ctypes.c_double), ctypes.c_int32, ctypes.c_int32] + [vp] * 5
         fn.restype = ctypes.c_int
+    for name in ("mpcb200_ilqr_f32", "mpcb200_ilqr_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(IlqrOpts)] + [vp] * 15 + \
+            [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_ilqr_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(IlqrOpts), ctypes.c_int32]
+    L.mpcb200_ilqr_workspace_bytes.restype = ctypes.c_size_t
     L.mpcb200_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_supported.restype = ctypes.c_int
     L.mpcb200_supported_list.argtypes = [ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]

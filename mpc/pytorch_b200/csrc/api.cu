@@ -4,6 +4,7 @@
 #include <cstring>
 
 #include "../../../include/mpcb200.h"
+#include "ilqr.cuh"
 #include "lqr_grad.cuh"
 #include "lqr_large.cuh"
 #include "lqr_rollout.cuh"
@@ -405,6 +406,236 @@ static int dyn_impl(bool linearize, int kind, const double* dyn, int B, int T, c
   if (rc == 0 && !(linearize && T == 1)) g_launches.fetch_add(1);
   return rc;
 }
+
+// ---------------------------------------------------------------------------------------------
+// the iLQR loop of MPC.forward as one CUDA graph (reference mpc/mpc.py:244-301)
+// ---------------------------------------------------------------------------------------------
+// dims of the step inside the loop: the caller's, with the rollout on and, for a known system, the workspace F, f
+static mpcb200_dims ilqr_step_dims(const mpcb200_dims* d) {
+  mpcb200_dims ds = *d;
+  ds.do_rollout = 1;
+  if (d->dynamics_kind != DYN_LINEAR) {
+    ds.F_T = d->T - 1; ds.has_f = d->T > 1 ? 1 : 0; ds.F_tstride = 0; ds.f_tstride = 0;
+  }
+  return ds;
+}
+
+struct IlqrLayout {                   // workspace carve-up (byte offsets, every piece 256-byte aligned)
+  size_t u, x, new_x, new_u, costs, fdn_step, alphas, du_first, status, fdn, flags, state, F, f, Ks, ks, total;
+  bool gains;
+};
+static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz) {
+  IlqrLayout l;
+  const size_t TB = (size_t)d->T * d->B, B = d->B;
+  const size_t n = d->n, m = d->m;
+  size_t o = 0;
+  l.u = o;        o += up256(TB * m * sz);
+  l.x = o;        o += up256(TB * n * sz);
+  l.new_x = o;    o += up256(TB * n * sz);
+  l.new_u = o;    o += up256(TB * m * sz);
+  l.costs = o;    o += up256(B * sz);
+  l.fdn_step = o; o += up256(B * sz);
+  l.alphas = o;   o += up256(B * sz);
+  l.du_first = o; o += up256(TB * m * sz);
+  l.status = o;   o += up256(B * sizeof(int32_t));
+  l.fdn = o;      o += up256(B * sz);
+  l.flags = o;    o += up256(B);
+  l.state = o;    o += up256(sizeof(IlqrState));
+  l.F = l.f = 0;
+  if (d->dynamics_kind != DYN_LINEAR) {         // the linearisation of a known system, rewritten every iteration
+    const size_t TB1 = (size_t)(d->T > 1 ? d->T - 1 : 0) * B;
+    l.F = o;      o += up256(TB1 * n * (n + m) * sz);
+    l.f = o;      o += up256(TB1 * n * sz);
+  }
+  const mpcb200_dims ds = ilqr_step_dims(d);
+  l.gains = mpcb200_step_prefers_workspace(&ds, (int32_t)sz) != 0;
+  l.Ks = l.ks = 0;
+  if (l.gains) {
+    l.Ks = o;     o += up256(TB * m * n * sz);
+    l.ks = o;     o += up256(TB * m * sz);
+  }
+  l.total = o;
+  return l;
+}
+
+static bool ilqr_known_shape_ok(const mpcb200_dims* d) {
+  return (d->dynamics_kind == DYN_CARTPOLE && d->n == 5 && d->m == 1) ||
+         (d->dynamics_kind == DYN_PENDULUM && d->n == 3 && d->m == 1);
+}
+
+// argument checks that need no device: every error is reported before anything is captured or launched
+template <typename R>
+static int ilqr_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_ilqr_opts* o, const R* C,
+                      const R* c, const R* F, const R* f, const R* x_init, const R* u_lower, const R* u_upper,
+                      const uint8_t* u_zero_I, const R* best_x, const R* best_u, const R* best_costs,
+                      const R* best_fdn, const int32_t* info, const void* workspace, size_t workspace_bytes) {
+  int rc = check_dims(d);
+  if (rc) return rc;
+  if (p == nullptr || o == nullptr || C == nullptr || c == nullptr || x_init == nullptr || best_x == nullptr ||
+      best_u == nullptr || best_costs == nullptr || best_fdn == nullptr || info == nullptr || workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (o->lqr_iter < 1 || o->m_ref < 1 || o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
+  if (d->dynamics_kind != DYN_LINEAR) {
+    if (!ilqr_known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
+  } else {
+    if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
+    if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
+  }
+  if (d->bounds_kind < 0 || d->bounds_kind > 2) return MPCB200_ERR_BAD_DIMS;
+  if (d->bounds_kind == 2 && (u_lower == nullptr || u_upper == nullptr)) return MPCB200_ERR_NULL_POINTER;
+  if (d->has_zero_mask && u_zero_I == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (d->has_delta_u && d->bounds_kind == 0) return MPCB200_ERR_BAD_DIMS;
+  if (d->max_ls_iter < 1 || d->pnqp_max_iter < 1) return MPCB200_ERR_BAD_DIMS;
+  if (d->dynamics_kind == DYN_LINEAR && find(d->n, d->m) == nullptr && !runs_large(d->n, d->m))
+    return MPCB200_ERR_UNSUPPORTED_DIMS;
+  if (d->dynamics_kind != DYN_LINEAR && find(d->n, d->m) == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
+  const IlqrLayout l = ilqr_layout(d, sizeof(R));
+  if (workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+// Library-owned streams of this thread on the current device: [0] records a graph the caller does not capture,
+// [1] records the loop body.  Capture only records work on them; nothing ever executes on them.
+static cudaStream_t ilqr_stream(int which) {
+  static thread_local cudaStream_t streams[64][2] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
+  cudaStream_t& s = streams[dev][which];
+  if (s == nullptr && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) s = nullptr;
+  return s;
+}
+
+// Adds the init kernel and the `while` node (body recorded on `bs`) to the graph `os` is capturing.
+template <typename R>
+static int ilqr_record(cudaStream_t os, cudaStream_t bs, const mpcb200_dims* d, const mpcb200_params* p,
+                       const mpcb200_ilqr_opts* o, const R* C, const R* c, const R* F, const R* f, const R* x_init,
+                       const R* u_init, const R* u_lower, const R* u_upper, const uint8_t* u_zero_I, R* best_x,
+                       R* best_u, R* best_costs, R* best_fdn, int32_t* info, void* workspace) {
+  const IlqrLayout l = ilqr_layout(d, sizeof(R));
+  char* ws = (char*)workspace;
+  R* u = (R*)(ws + l.u);
+  R* x = (R*)(ws + l.x);
+  R* new_x = (R*)(ws + l.new_x);
+  R* new_u = (R*)(ws + l.new_u);
+  R* costs = (R*)(ws + l.costs);
+  R* du_first = (R*)(ws + l.du_first);
+  int32_t* status = (int32_t*)(ws + l.status);
+  R* fdn = (R*)(ws + l.fdn);
+  uint8_t* flags = (uint8_t*)(ws + l.flags);
+  IlqrState* st = (IlqrState*)(ws + l.state);
+  const int B = d->B, T = d->T, N = d->n, M = d->m;
+  const size_t TB = (size_t)T * B;
+  if (ilqr_launch_init<R>(TB * M, u_init, u, st, info, os) != 0) return MPCB200_ERR_LAUNCH;
+  g_launches.fetch_add(1);
+
+  cudaStreamCaptureStatus cst = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t ndeps = 0;
+  if (cudaStreamGetCaptureInfo(os, &cst, nullptr, &g, &deps, &ndeps) != cudaSuccess ||
+      cst != cudaStreamCaptureStatusActive)
+    return MPCB200_ERR_LAUNCH;
+  cudaGraphConditionalHandle handle;
+  if (cudaGraphConditionalHandleCreate(&handle, g, 1, cudaGraphCondAssignDefault) != cudaSuccess) {
+    cudaGetLastError();
+    return MPCB200_ERR_NO_GRAPH_COND;
+  }
+  cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
+  np.conditional.handle = handle;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  cudaGraphNode_t loop;
+  if (cudaGraphAddNode(&loop, g, deps, ndeps, &np) != cudaSuccess) {
+    cudaGetLastError();
+    return MPCB200_ERR_NO_GRAPH_COND;
+  }
+  if (cudaStreamUpdateCaptureDependencies(os, &loop, 1, cudaStreamSetCaptureDependencies) != cudaSuccess)
+    return MPCB200_ERR_LAUNCH;
+
+  // the body: the library's own launchers, recorded on bs (same plan selection as a direct call)
+  if (cudaStreamBeginCaptureToGraph(bs, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                    cudaStreamCaptureModeRelaxed) != cudaSuccess)
+    return MPCB200_ERR_LAUNCH;
+  const mpcb200_dims ds = ilqr_step_dims(d);
+  const R* Fs = F;
+  const R* fs = f;
+  int rc;
+  if (d->dynamics_kind == DYN_LINEAR) {
+    rc = rollout_impl<R>(d, F, f, x_init, u, x, bs);
+  } else {
+    R* Fw = (R*)(ws + l.F);
+    R* fw = (R*)(ws + l.f);
+    rc = dyn_impl<R>(false, d->dynamics_kind, p->dyn, B, T, x_init, u, x, nullptr, nullptr, bs);
+    if (rc == 0) rc = dyn_impl<R>(true, d->dynamics_kind, p->dyn, B, T, x, u, nullptr, Fw, fw, bs);
+    Fs = T > 1 ? Fw : nullptr;
+    fs = T > 1 ? fw : nullptr;
+  }
+  if (rc == 0)
+    rc = step_impl<R>(&ds, p, C, c, Fs, fs, x_init, x, u, u_lower, u_upper, u_zero_I, new_x, new_u, costs,
+                      (R*)(ws + l.fdn_step), (R*)(ws + l.alphas), du_first, (int32_t*)nullptr, (uint8_t*)nullptr,
+                      status, l.gains ? (R*)(ws + l.Ks) : (R*)nullptr, l.gains ? (R*)(ws + l.ks) : (R*)nullptr, bs);
+  if (rc == 0)
+    rc = ilqr_launch_track<R>(B, T, N, M, o->m_ref, (R)o->best_cost_eps, new_x, new_u, costs, du_first, status,
+                              best_costs, best_x, best_u, u, fdn, flags, st, bs);
+  if (rc == 0) {
+    g_launches.fetch_add(1);
+    rc = ilqr_launch_stop<R>(B, o->lqr_iter, o->not_improved_lim, o->eps, costs, fdn, flags, best_costs, best_fdn, st,
+                             info, handle, bs);
+    if (rc == 0) g_launches.fetch_add(1);
+  }
+  cudaGraph_t body = nullptr;
+  if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+  return rc;
+}
+
+template <typename R>
+static int ilqr_impl(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_ilqr_opts* o, const R* C,
+                     const R* c, const R* F, const R* f, const R* x_init, const R* u_init, const R* u_lower,
+                     const R* u_upper, const uint8_t* u_zero_I, R* best_x, R* best_u, R* best_costs, R* best_fdn,
+                     int32_t* info, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = ilqr_check<R>(d, p, o, C, c, F, f, x_init, u_lower, u_upper, u_zero_I, best_x, best_u, best_costs,
+                         best_fdn, info, workspace, workspace_bytes);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  int driver = 0;
+  if (cudaDriverGetVersion(&driver) != cudaSuccess || driver < 12030) return MPCB200_ERR_NO_GRAPH_COND;
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap == cudaStreamCaptureStatusInvalidated)
+    return MPCB200_ERR_LAUNCH;
+  const bool caller_captures = cap == cudaStreamCaptureStatusActive;
+  // the library's own graph and stream calls must not invalidate a capture the caller runs in global mode
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  cudaStream_t os = caller_captures ? st : ilqr_stream(0);
+  cudaStream_t bs = ilqr_stream(1);
+  if (os == nullptr || bs == nullptr) {
+    rc = MPCB200_ERR_LAUNCH;
+  } else if (caller_captures) {
+    rc = ilqr_record<R>(os, bs, d, p, o, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
+                        best_costs, best_fdn, info, workspace);
+  } else if (cudaStreamBeginCapture(os, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
+    rc = MPCB200_ERR_LAUNCH;
+  } else {
+    rc = ilqr_record<R>(os, bs, d, p, o, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
+                        best_costs, best_fdn, info, workspace);
+    cudaGraph_t g = nullptr;
+    if (cudaStreamEndCapture(os, &g) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+    if (rc == 0) {
+      cudaGraphExec_t exec = nullptr;
+      if (cudaGraphInstantiate(&exec, g, 0) != cudaSuccess) {
+        rc = MPCB200_ERR_LAUNCH;
+      } else {
+        if (cudaGraphLaunch(exec, st) != cudaSuccess) rc = MPCB200_ERR_LAUNCH;
+        cudaGraphExecDestroy(exec);        // released once the launch completes
+      }
+    }
+    if (g != nullptr) cudaGraphDestroy(g);
+  }
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (rc) cudaGetLastError();              // a failed build leaves no sticky launch error behind
+  return rc;
+}
 }  // namespace mpcb200
 
 using namespace mpcb200;
@@ -491,6 +722,30 @@ int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_
   return dyn_impl<double>(true, kind, dyn, B, T, x, u, nullptr, F, f, stream);
 }
 
+size_t mpcb200_ilqr_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
+  if (dims == nullptr || opts == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
+  if (dims->dynamics_kind == DYN_LINEAR ? (find(dims->n, dims->m) == nullptr && !runs_large(dims->n, dims->m))
+                                        : !ilqr_known_shape_ok(dims))
+    return 0;
+  return ilqr_layout(dims, (size_t)elem_size).total;
+}
+int mpcb200_ilqr_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                     const float* C, const float* c, const float* F, const float* f, const float* x_init,
+                     const float* u_init, const float* u_lower, const float* u_upper, const uint8_t* u_zero_I,
+                     float* best_x, float* best_u, float* best_costs, float* best_full_du_norm, int32_t* info,
+                     void* workspace, size_t workspace_bytes, void* stream) {
+  return ilqr_impl<float>(dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
+                          best_costs, best_full_du_norm, info, workspace, workspace_bytes, stream);
+}
+int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                     const double* C, const double* c, const double* F, const double* f, const double* x_init,
+                     const double* u_init, const double* u_lower, const double* u_upper, const uint8_t* u_zero_I,
+                     double* best_x, double* best_u, double* best_costs, double* best_full_du_norm, int32_t* info,
+                     void* workspace, size_t workspace_bytes, void* stream) {
+  return ilqr_impl<double>(dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
+                           best_costs, best_full_du_norm, info, workspace, workspace_bytes, stream);
+}
+
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }
 
 int mpcb200_supported_list(int32_t* out, int32_t cap) {
@@ -537,6 +792,7 @@ const char* mpcb200_strerror(int code) {
     case MPCB200_ERR_SMEM: return "problem does not fit shared memory (pass Ks/ks buffers for long horizons)";
     case MPCB200_ERR_LAUNCH: return "CUDA launch failed";
     case MPCB200_ERR_NO_DEVICE: return "no usable sm_90 device";
+    case MPCB200_ERR_NO_GRAPH_COND: return "conditional CUDA graph nodes are unavailable (driver older than 12.3)";
     default: return "unknown error";
   }
 }

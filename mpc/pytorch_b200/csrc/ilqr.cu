@@ -1,0 +1,49 @@
+// ilqr.cu - launchers of the device-side iLQR loop's bookkeeping kernels (ilqr.cuh), in a module of their own.
+#include "ilqr.cuh"
+
+namespace mpcb200 {
+
+static unsigned ilqr_grid(size_t items) {   // grid-stride kernels: enough blocks to cover `items`, at most 4096
+  const size_t g = (items + 255) / 256;
+  return (unsigned)(g < 1 ? 1 : (g > 4096 ? 4096 : g));
+}
+
+static int launched() { return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH; }
+
+template <typename R>
+int ilqr_launch_init(size_t n_u, const R* u_init, R* u, IlqrState* st, int32_t* info, cudaStream_t stream) {
+  ilqr_init_kernel<R><<<ilqr_grid(n_u), 256, 0, stream>>>(n_u, u_init, u, st, info);
+  return launched();
+}
+
+template <typename R>
+int ilqr_launch_track(int B, int T, int N, int M, int m_ref, R best_cost_eps, const R* new_x, const R* new_u,
+                      const R* costs, const R* du_first, const int32_t* status, const R* best_costs, R* best_x,
+                      R* best_u, R* u, R* fdn, uint8_t* flags, const IlqrState* st, cudaStream_t stream) {
+  ilqr_track_kernel<R><<<ilqr_grid((size_t)T * B * (N > M ? N : M)), 256, 0, stream>>>(
+      B, T, N, M, m_ref, best_cost_eps, new_x, new_u, costs, du_first, status, best_costs, best_x, best_u, u, fdn,
+      flags, st);
+  return launched();
+}
+
+template <typename R>
+int ilqr_launch_stop(int B, int lqr_iter, int not_improved_lim, double eps, const R* costs, const R* fdn,
+                     const uint8_t* flags, R* best_costs, R* best_fdn, IlqrState* st, int32_t* info,
+                     cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  ilqr_stop_kernel<R><<<1, ILQR_STOP_THREADS, 0, stream>>>(B, lqr_iter, not_improved_lim, eps, costs, fdn, flags,
+                                                           best_costs, best_fdn, st, info, handle);
+  return launched();
+}
+
+#define MPCB200_ILQR_INST(R)                                                                                       \
+  template int ilqr_launch_init<R>(size_t, const R*, R*, IlqrState*, int32_t*, cudaStream_t);                     \
+  template int ilqr_launch_track<R>(int, int, int, int, int, R, const R*, const R*, const R*, const R*,            \
+                                    const int32_t*, const R*, R*, R*, R*, R*, uint8_t*, const IlqrState*,          \
+                                    cudaStream_t);                                                                 \
+  template int ilqr_launch_stop<R>(int, int, int, double, const R*, const R*, const uint8_t*, R*, R*, IlqrState*, \
+                                   int32_t*, cudaGraphConditionalHandle, cudaStream_t);
+MPCB200_ILQR_INST(float)
+MPCB200_ILQR_INST(double)
+#undef MPCB200_ILQR_INST
+
+}  // namespace mpcb200

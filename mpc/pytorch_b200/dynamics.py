@@ -87,7 +87,8 @@ class CartpoleDx(Module):
         single = state.dim() == 1
         if single:
             state, u = state.unsqueeze(0), u.unsqueeze(0)
-        g, mc, mp, l = self.params.to(state).unbind()
+        # pinned parameters are copied without a host synchronisation, which also lets torch.cuda.graph capture it
+        g, mc, mp, l = self.params.to(state, non_blocking=self.params.is_pinned()).unbind()
         total, pml = mp + mc, mp * l
         force = u[:, 0].clamp(-self.force_mag, self.force_mag)
         pos, vel, c, s, om = state.unbind(1)
@@ -137,7 +138,7 @@ class PendulumDx(Module):
         single = x.dim() == 1
         if single:
             x, u = x.unsqueeze(0), u.unsqueeze(0)
-        g, m, l = self.params.to(x).unbind()
+        g, m, l = self.params.to(x, non_blocking=self.params.is_pinned()).unbind()
         tq = u.clamp(-self.max_torque, self.max_torque)[:, 0]
         c, s, om = x.unbind(1)
         th = torch.atan2(s, c)

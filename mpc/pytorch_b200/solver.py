@@ -8,7 +8,9 @@ keywords and defaults (:123-144), ``forward(x_init, cost, dx) -> (x, u, costs)``
 Differences are structural only: the best-iterate bookkeeping (reference :271-285, a Python
 loop over the batch with one host sync per element) is a ``torch.where`` on the device and the
 stop test costs ONE device->host read per iteration; every LQR step is a single CUDA kernel
-(``step.LQRStep``).
+(``step.LQRStep``).  Where the dynamics run in the kernels (``LinDx`` or a known system) and the cost
+is a ``QuadCost``, the whole loop, bookkeeping and stop test included, runs as one CUDA graph with no
+host read (``MPC._ilqr_device``, ``_use_device_loop``), computing bitwise what the host loop computes.
 """
 import sys
 from collections import namedtuple
@@ -216,6 +218,70 @@ class MPC(Module):
             print("Initial mean(cost): {:.4e}".format(
                 torch.mean(get_cost(T, u, cost, dx, x_init=x_init)).item()))
 
+        best = self._ilqr_device(x_init, cost, dx, u) if _use_device_loop(self, x_init, cost, dx, u) else None
+        if best is None:
+            best = self._ilqr_host(x_init, cost, dx, u)
+        x, u = best["x"], best["u"]
+        full_du_norm = best["full_du_norm"]
+
+        if isinstance(dx, LinDx):
+            F, f = dx.F, dx.f
+        else:
+            F, f = self.linearize_dynamics(x, u, dx, diff=True)
+        if isinstance(cost, QuadCost):
+            C, c = cost.C, cost.c
+        else:
+            C, c, _ = self.approximate_cost(x, u, cost, diff=True)
+
+        # the only differentiable call: identity forward, KKT-adjoint backward (reference :318-319)
+        x, u = self.solve_lqr_subproblem(x_init, C, c, F, f, cost, dx, x, u, no_op_forward=True)
+
+        if self.detach_unconverged:                         # reference :321-334
+            if float(full_du_norm.max()) > self.eps:
+                if self.exit_unconverged:
+                    assert False
+                if self.verbose >= 0:
+                    print("LQR Warning: All examples did not converge to a fixed point.")
+                    print("Detaching and *not* backpropping through the bad examples.")
+                keep = (full_du_norm < self.eps).view(1, -1, 1)
+                Ix = keep.expand_as(x).to(x.dtype)
+                Iu = keep.expand_as(u).to(u.dtype)
+                x = x * Ix + x.clone().detach() * (1. - Ix)
+                u = u * Iu + u.clone().detach() * (1. - Iu)
+
+        return (x, u, best["costs"])
+
+    # ------------------------------------------------------------------------------------
+    def _ilqr_device(self, x_init, cost, dx, u):
+        """The iLQR iterations as one library call (mpcb200_ilqr_*): a CUDA graph whose conditional `while` node runs
+        rollout, [linearisation,] step, best-iterate tracking and the stop test on the device, with the arithmetic of
+        _ilqr_host.  No host read unless pnqp warnings are to be printed.  None when the driver has no conditional
+        graph nodes (the caller then runs _ilqr_host)."""
+        global _graph_cond_unavailable
+        from . import step as _step
+        T, n, m = self.T, self.n_state, self.n_ctrl
+        if isinstance(dx, LinDx):
+            F, f, dyn = dx.F, dx.f, None
+        else:
+            from .dynamics import known_kind
+            F = f = None
+            dyn = known_kind(dx, n, m, x_init)
+        res = _step.ilqr_raw(n, m, T, x_init, cost.C, cost.c, F, f, u, u_lower=self.u_lower, u_upper=self.u_upper,
+                             u_zero_I=self.u_zero_I, delta_u=self.delta_u, linesearch_decay=self.linesearch_decay,
+                             max_linesearch_iter=self.max_linesearch_iter, lqr_iter=self.lqr_iter,
+                             not_improved_lim=self.not_improved_lim, eps=self.eps, best_cost_eps=self.best_cost_eps,
+                             dyn=dyn)
+        if res is None:
+            _graph_cond_unavailable = True
+            return None
+        if self.verbose >= 0 and self.u_lower is not None:
+            for _ in range(int(res["info"][1])):             # the one host read: iterations with a pnqp warning
+                print("[WARNING] pnqp warning: Did not converge")   # reference pnqp.py:81
+        return {"x": res["x"], "u": res["u"], "costs": res["costs"], "full_du_norm": res["full_du_norm"]}
+
+    def _ilqr_host(self, x_init, cost, dx, u):
+        """The iLQR iterations from Python: one host read per iteration for the stop test."""
+        T = self.T
         best = None
         n_not_improved = 0
         for i in range(self.lqr_iter):
@@ -269,35 +335,7 @@ class MPC(Module):
             if max_du < self.eps or n_not_improved > self.not_improved_lim:   # reference :299-301
                 break
 
-        x, u = best["x"], best["u"]
-        full_du_norm = best["full_du_norm"]
-
-        if isinstance(dx, LinDx):
-            F, f = dx.F, dx.f
-        else:
-            F, f = self.linearize_dynamics(x, u, dx, diff=True)
-        if isinstance(cost, QuadCost):
-            C, c = cost.C, cost.c
-        else:
-            C, c, _ = self.approximate_cost(x, u, cost, diff=True)
-
-        # the only differentiable call: identity forward, KKT-adjoint backward (reference :318-319)
-        x, u = self.solve_lqr_subproblem(x_init, C, c, F, f, cost, dx, x, u, no_op_forward=True)
-
-        if self.detach_unconverged:                         # reference :321-334
-            if float(full_du_norm.max()) > self.eps:
-                if self.exit_unconverged:
-                    assert False
-                if self.verbose >= 0:
-                    print("LQR Warning: All examples did not converge to a fixed point.")
-                    print("Detaching and *not* backpropping through the bad examples.")
-                keep = (full_du_norm < self.eps).view(1, -1, 1)
-                Ix = keep.expand_as(x).to(x.dtype)
-                Iu = keep.expand_as(u).to(u.dtype)
-                x = x * Ix + x.clone().detach() * (1. - Ix)
-                u = u * Iu + u.clone().detach() * (1. - Iu)
-
-        return (x, u, best["costs"])
+        return best
 
     # ------------------------------------------------------------------------------------
     def solve_lqr_subproblem(self, x_init, C, c, F, f, cost, dynamics, x, u, no_op_forward=False,
@@ -443,6 +481,54 @@ class MPC(Module):
         if not diff:
             F, f = F.detach(), f.detach()
         return F, f
+
+
+_graph_cond_unavailable = False     # set once a driver without conditional graph nodes refused the device loop
+
+
+def _use_device_loop(mpc, x_init, cost, dx, u):
+    """Whether MPC.forward runs its iLQR iterations as one device-side graph (MPC._ilqr_device) rather than from
+    Python (MPC._ilqr_host).  Decided on what the call shows without reading the device: the results are the same
+    either way, so there is no user option.  Taken for CUDA float32/float64 tensors of one dtype, a QuadCost, LinDx
+    dynamics or a known system linearised by ANALYTIC / AUTO_DIFF, no slew-rate penalty, verbose <= 0, lqr_iter >= 1,
+    T >= 2 and a shape the step kernels take (an exact or zero-padded instance, or the large-shape kernels for LinDx)."""
+    from .dynamics import DYN_LINEAR
+    from .step import _pick_instance
+    from ._lib import MpcB200Error
+    if _graph_cond_unavailable or mpc.slew_rate_penalty is not None or mpc.verbose > 0 or mpc.lqr_iter < 1:
+        return False
+    if not isinstance(cost, QuadCost) or mpc.T < 2:
+        return False
+    dtype, dev = x_init.dtype, x_init.device
+    if dtype not in (torch.float32, torch.float64) or not x_init.is_cuda:
+        return False
+    n, m = mpc.n_state, mpc.n_ctrl
+    same = [cost.C, cost.c, u]
+    if isinstance(dx, LinDx):
+        if dx.F is None:
+            return False
+        same.append(dx.F)
+        if dx.f is not None and dx.f.nelement() > 0:
+            same.append(dx.f)
+        known = False
+    elif isinstance(dx, Module) and getattr(dx, "mpcb200_kind", DYN_LINEAR) != DYN_LINEAR:
+        if mpc.grad_method not in (GradMethods.ANALYTIC, GradMethods.AUTO_DIFF):
+            return False
+        if (n, m) != (dx.n_state, dx.n_ctrl):
+            return False
+        known = True
+    else:
+        return False
+    same += [b for b in (mpc.u_lower, mpc.u_upper) if isinstance(b, torch.Tensor)]
+    if any(not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != dev for t in same):
+        return False
+    if isinstance(mpc.u_zero_I, torch.Tensor) and mpc.u_zero_I.device != dev:
+        return False
+    try:
+        N, M = _pick_instance(n, m, x_init.element_size())
+    except MpcB200Error:
+        return False
+    return not known or (N, M) == (n, m)
 
 
 _seen_tables = []

@@ -39,14 +39,14 @@ def _dense(t, dtype=None):
     return t if t.is_contiguous() else t.contiguous()
 
 
-def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=None, exact=False):
+def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=None, exact=False, need_F=True):
     """Check, on tensor metadata alone, the tensors a raw call hands to the kernels; returns the batch size B.
     The kernels read raw device pointers: a wrong dtype, shape or device would be an out-of-bounds access, so fail
     here like the reference's indexing / eclamp size asserts would.  `named`: (name, tensor or None, layout), the
     layout one of "TBpp", "TBp", "TBn", "TBm", "Bn" (p = n+m).  The first tensor leads: the outputs are allocated in
     its dtype, and it fixes B and the device.  F [T-1|T,B,n,p] and f [T-1|T,B,n] may be absent or empty (F only for
     T = 1); tensor bounds and u_zero_I are [T,B,m].  `exact`: the call runs in-kernel dynamics, which need an exact
-    (n, m) kernel instance."""
+    (n, m) kernel instance.  `need_F=False`: the call linearises a known system itself and takes no F."""
     lead_name, lead, lead_layout = named[0]
     if lead.dtype not in (torch.float32, torch.float64):
         raise MpcB200Error(f"unsupported dtype {lead.dtype}")
@@ -66,7 +66,7 @@ def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=Non
                 raise MpcB200Error(f"{name}: expected shape (T-1 or T, {', '.join(map(str, shape))}), "
                                    f"got {tuple(t.shape)}")
             checked.append((name, t))
-    if _is_empty(F) and T > 1:
+    if _is_empty(F) and T > 1 and need_F:
         raise MpcB200Error("F is required for T > 1")
     u_lower, u_upper = bounds
     if (u_lower is None) != (u_upper is None):
@@ -328,6 +328,64 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
     if want_stats:
         out.update(qp_iters=qp_iters, free_mask=pad.crop_m(free_mask), status=status)
     return out
+
+
+def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
+             delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
+             best_cost_eps=1e-4, dyn=None):
+    """The iLQR iterations of MPC.forward (reference mpc/mpc.py:244-301) in ONE library call: a CUDA graph that runs
+    rollout, [linearisation,] step, best-iterate tracking and the stop test until the stop test ends it, without a
+    host read.  The dynamics are LinDx(F, f), or the known system `dyn` = (kind, params) with F = f = None.  The
+    problem is zero padded once per solve to the kernel instance it runs at, which hands every kernel the values
+    lqr_step_raw and rollout_raw would hand it per call.  Returns a dict of device tensors x, u, costs, full_du_norm
+    (the best iterate) and info = int32 [iterations run, iterations with an unconverged pnqp]; None when the driver
+    has no conditional graph nodes (nothing was launched then)."""
+    n, m = n_state, n_ctrl
+    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
+                  F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I, exact=dyn is not None,
+                  need_F=dyn is None)
+    dtype, dev = C.dtype, C.device
+    N, M = _pick_instance(n, m, C.element_size())
+    pad = _Pad(n, m, N, M, dev)
+    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
+    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
+    x0_, u0_ = _dense(x_init, dtype), _dense(u_init, dtype)
+    bounds_kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev, pad.active)
+    zmask = (u_zero_I != 0).to(torch.uint8).contiguous() if u_zero_I is not None else None
+    if pad.active:
+        x0_, u0_ = pad.vec_n(x0_), pad.vec_m(u0_)
+        if lo_t is not None:
+            lo_t, hi_t = pad.vec_m(lo_t, -1.0), pad.vec_m(hi_t, 1.0)
+        if zmask is not None:
+            zmask = pad.vec_m(zmask, 0)
+    dims = Dims(B=B, T=T, n=N, m=M, F_T=F_.shape[0] if F_ is not None else T - 1, has_f=int(f_ is not None),
+                bounds_kind=bounds_kind, has_zero_mask=int(zmask is not None), has_delta_u=int(delta_u is not None),
+                max_ls_iter=int(max_linesearch_iter), pnqp_max_iter=PNQP_MAX_ITER, do_rollout=1,
+                dynamics_kind=int(dyn[0]) if dyn is not None else 0,
+                C_tstride=tsC, c_tstride=tsc, F_tstride=tsF, f_tstride=tsf)
+    params = Params(u_lo=float(s_lo), u_hi=float(s_hi), delta_u=float(delta_u) if delta_u is not None else 0.0,
+                    ls_decay=float(linesearch_decay))
+    if dyn is not None:
+        for i, v in enumerate(dyn[1]):
+            params.dyn[i] = float(v)
+    opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
+                         best_cost_eps=float(best_cost_eps))
+    nbytes = _lib.lib().mpcb200_ilqr_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    best_x = torch.empty(T, B, N, dtype=dtype, device=dev)
+    best_u = torch.empty(T, B, M, dtype=dtype, device=dev)
+    costs = torch.empty(B, dtype=dtype, device=dev)
+    fdn = torch.empty(B, dtype=dtype, device=dev)
+    info = torch.empty(2, dtype=torch.int32, device=dev)
+    fn = _lib.entry("mpcb200_ilqr", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(params), ctypes.byref(opts), ptr_view(C_), ptr_view(c_),
+                ptr_view(F_), ptr_view(f_), ptr(x0_), ptr(u0_), ptr(lo_t), ptr(hi_t), ptr(zmask), ptr(best_x),
+                ptr(best_u), ptr(costs), ptr(fdn), ptr(info), ptr(ws), nbytes, stream_handle(dev))
+    if rc == _lib.ERR_NO_GRAPH_COND:
+        return None
+    check(rc, "mpcb200_ilqr")
+    return {"x": pad.crop_n(best_x), "u": pad.crop_m(best_u), "costs": costs, "full_du_norm": fdn, "info": info}
 
 
 def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_df, f_T=None):
