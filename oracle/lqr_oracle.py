@@ -403,7 +403,8 @@ def lqr_step_backward(n_state, n_ctrl, T, x_init, C, c, F, f, new_x, new_u, dl_d
 def mpc_forward_lin(n_state, n_ctrl, T, x_init, C, c, F, f, u_lower=None, u_upper=None,
                     u_init=None, lqr_iter=10, delta_u=None, eps=1e-7,
                     linesearch_decay=0.2, max_linesearch_iter=10,
-                    not_improved_lim=5, best_cost_eps=1e-4, coupled=True, trace=None):
+                    not_improved_lim=5, best_cost_eps=1e-4, coupled=True, trace=None,
+                    u_zero_I=None):
     B = C.shape[1]
     dt = C.dtype
     u = torch.zeros(T, B, n_ctrl, dtype=dt) if u_init is None else u_init.clone()
@@ -412,7 +413,7 @@ def mpc_forward_lin(n_state, n_ctrl, T, x_init, C, c, F, f, u_lower=None, u_uppe
     for i in range(lqr_iter):
         x = get_traj(T, u, x_init, F, f)
         out = lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, x, u,
-                               u_lower=u_lower, u_upper=u_upper, delta_u=delta_u,
+                               u_lower=u_lower, u_upper=u_upper, u_zero_I=u_zero_I, delta_u=delta_u,
                                linesearch_decay=linesearch_decay,
                                max_linesearch_iter=max_linesearch_iter, coupled=coupled)
         x, u = out.new_x, out.new_u
