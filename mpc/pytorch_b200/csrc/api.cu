@@ -85,9 +85,14 @@ int max_smem_optin() {
   return cache[dev].load(std::memory_order_acquire);
 }
 
-// element stride between time slices: 0 = dense (what a zero-initialised mpcb200_dims means), < 0 = time
-// invariant (stride 0), > 0 = that many elements
-static long long tstride(long long given, long long dense) { return given == 0 ? dense : (given < 0 ? 0 : given); }
+// element strides between the time slices of C, c, F and f.  Each *_tstride field of mpcb200_dims: 0 = dense (what a
+// zero-initialised mpcb200_dims means), < 0 = time invariant (stride 0), > 0 = that many elements
+struct TimeStrides { long long C, c, F, f; };
+static TimeStrides time_strides(const mpcb200_dims* d) {
+  auto ts = [](long long given, long long dense) { return given == 0 ? dense : (given < 0 ? 0 : given); };
+  const long long B = d->B, n = d->n, p = d->n + d->m;
+  return {ts(d->C_tstride, B * p * p), ts(d->c_tstride, B * p), ts(d->F_tstride, B * n * p), ts(d->f_tstride, B * n)};
+}
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
@@ -96,6 +101,25 @@ static int check_dims(const mpcb200_dims* d) {
   if (d->B <= 0 || d->T <= 0 || d->n <= 0 || d->m <= 0) return MPCB200_ERR_BAD_DIMS;
   if (d->F_T != d->T - 1 && d->F_T != d->T) return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
+}
+
+// the step's option checks, one order for every entry point: an argument error gets the same code from each
+static int check_bounds(const mpcb200_dims* d, const void* lo, const void* hi) {
+  if (d->bounds_kind < 0 || d->bounds_kind > 2) return MPCB200_ERR_BAD_DIMS;
+  if (d->bounds_kind == 2 && (lo == nullptr || hi == nullptr)) return MPCB200_ERR_NULL_POINTER;
+  return MPCB200_OK;
+}
+static int check_step_options(const mpcb200_dims* d, const void* lo, const void* hi, const uint8_t* zero_mask) {
+  if (const int rc = check_bounds(d, lo, hi)) return rc;
+  if (d->has_zero_mask && zero_mask == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (d->has_delta_u && d->bounds_kind == 0) return MPCB200_ERR_BAD_DIMS;   // reference lqr_step.py:195
+  if (d->max_ls_iter < 1 || d->pnqp_max_iter < 1) return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+static bool known_shape_ok(const mpcb200_dims* d) {
+  return (d->dynamics_kind == DYN_CARTPOLE && d->n == 5 && d->m == 1) ||
+         (d->dynamics_kind == DYN_PENDULUM && d->n == 3 && d->m == 1);
 }
 
 struct AdjExtra {      // fused-adjoint request riding on a step launch (api-internal)
@@ -117,11 +141,8 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
     return MPCB200_ERR_NULL_POINTER;
   if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
   if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (d->bounds_kind < 0 || d->bounds_kind > 2) return MPCB200_ERR_BAD_DIMS;
-  if (d->bounds_kind == 2 && (u_lower == nullptr || u_upper == nullptr)) return MPCB200_ERR_NULL_POINTER;
-  if (d->has_zero_mask && u_zero_I == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (d->has_delta_u && d->bounds_kind == 0) return MPCB200_ERR_BAD_DIMS;   // reference lqr_step.py:195
-  if (d->max_ls_iter < 1 || d->pnqp_max_iter < 1) return MPCB200_ERR_BAD_DIMS;
+  rc = check_step_options(d, u_lower, u_upper, u_zero_I);
+  if (rc) return rc;
   if (d->do_rollout) {
     if (x_init == nullptr || new_x == nullptr || new_u == nullptr || costs == nullptr ||
         full_du_norm == nullptr || alphas == nullptr)
@@ -159,17 +180,13 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
   ok = ok && (x_init == nullptr || aligned16(x_init));
   ok = ok && ((size_t)d->B * d->m * sz) % 16 == 0 && ((size_t)d->B * d->n * sz) % 16 == 0;
   a.bulk_ok = ok ? 1 : 0;
-  a.C_ts = tstride(d->C_tstride, (long long)d->B * (d->n + d->m) * (d->n + d->m));
-  a.c_ts = tstride(d->c_tstride, (long long)d->B * (d->n + d->m));
-  a.F_ts = tstride(d->F_tstride, (long long)d->B * d->n * (d->n + d->m));
-  a.f_ts = tstride(d->f_tstride, (long long)d->B * d->n);
+  const TimeStrides ts = time_strides(d);
+  a.C_ts = ts.C; a.c_ts = ts.c; a.F_ts = ts.F; a.f_ts = ts.f;
   ok = ok && (a.C_ts * sz) % 16 == 0 && (a.c_ts * sz) % 16 == 0 && (a.F_ts * sz) % 16 == 0 && (a.f_ts * sz) % 16 == 0;
   a.bulk_ok = ok ? 1 : 0;
   a.dyn_kind = d->dynamics_kind;
   if (a.dyn_kind != DYN_LINEAR) {
-    const bool shape_ok = (a.dyn_kind == DYN_CARTPOLE && d->n == 5 && d->m == 1) ||
-                          (a.dyn_kind == DYN_PENDULUM && d->n == 3 && d->m == 1);
-    if (!shape_ok) return MPCB200_ERR_BAD_DIMS;
+    if (!known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
     for (int i = 0; i < 8; ++i) a.dp.p[i] = p->dyn[i];
   }
   if (large) {
@@ -226,9 +243,8 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
   a.B = d->B; a.T = d->T; a.F_T = d->F_T; a.has_df = df != nullptr;
   a.C = C; a.c = c; a.F = F; a.new_x = new_x; a.new_u = new_u; a.dx = dx; a.du = du; a.dl_dx = dl_dx;
   a.dx_init = dx_init; a.dC = dC; a.dc = dc; a.dF = dF; a.df = df; a.workspace = workspace;
-  a.C_ts = tstride(d->C_tstride, (long long)d->B * (d->n + d->m) * (d->n + d->m));
-  a.c_ts = tstride(d->c_tstride, (long long)d->B * (d->n + d->m));
-  a.F_ts = tstride(d->F_tstride, (long long)d->B * d->n * (d->n + d->m));
+  const TimeStrides ts = time_strides(d);
+  a.C_ts = ts.C; a.c_ts = ts.c; a.F_ts = ts.F;
   rc = large ? large_grad_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
              : (sizeof(R) == 4 ? e->grad32 : e->grad64)(a, (cudaStream_t)stream);
   if (rc == 0) g_launches.fetch_add(workspace != nullptr ? 2 : 1);
@@ -301,8 +317,8 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
       dl_du == nullptr || dx_init == nullptr || dC == nullptr || dc == nullptr || workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (d->T > 1 && (F == nullptr || dF == nullptr)) return MPCB200_ERR_NULL_POINTER;
-  if (d->bounds_kind < 0 || d->bounds_kind > 2) return MPCB200_ERR_BAD_DIMS;
-  if (d->bounds_kind == 2 && (u_lower == nullptr || u_upper == nullptr)) return MPCB200_ERR_NULL_POINTER;
+  rc = check_bounds(d, u_lower, u_upper);
+  if (rc) return rc;
   if (d->has_f && df == nullptr) return MPCB200_ERR_NULL_POINTER;
   const AdjLayout l = adj_layout(d->B, d->T, d->n, d->m, sizeof(R));
   if (workspace_bytes < l.total || !aligned16(workspace)) return MPCB200_ERR_BAD_DIMS;
@@ -337,7 +353,7 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
     AdjExtra ax;
     ax.c = c; ax.x = new_x; ax.u = new_u; ax.dC = dC; ax.dc = dc; ax.dF = dF; ax.df = d->has_f ? df : nullptr;
     ax.dx_init = dx_init; ax.has_df = d->has_f ? 1 : 0;
-    ax.c_ts = tstride(d->c_tstride, (long long)d->B * (d->n + d->m));
+    ax.c_ts = time_strides(d).c;
     ax.ok = aligned16(c) && aligned16(new_x) && aligned16(new_u) && (ax.c_ts * (long long)sizeof(R)) % 16 == 0;
     const R* maskf = (const R*)(ws + l.maskf);
     rc = step_impl<R>(&ds, &ps, C, negr, F, (const R*)nullptr, z0, zx, zu, maskf, maskf, mask,
@@ -375,8 +391,8 @@ static int rollout_impl(const mpcb200_dims* d, const R* F, const R* f, const R* 
   std::memset(&a, 0, sizeof(a));
   a.B = d->B; a.T = d->T; a.has_f = d->has_f ? 1 : 0;
   a.F = F; a.f = f; a.x_init = x_init; a.u = u; a.x = x;
-  a.F_ts = tstride(d->F_tstride, (long long)d->B * d->n * (d->n + d->m));
-  a.f_ts = tstride(d->f_tstride, (long long)d->B * d->n);
+  const TimeStrides ts = time_strides(d);
+  a.F_ts = ts.F; a.f_ts = ts.f;
   rc = large ? large_rollout_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
              : (sizeof(R) == 4 ? e->roll32 : e->roll64)(a, (cudaStream_t)stream);
   if (rc == 0) g_launches.fetch_add(1);
@@ -458,11 +474,6 @@ static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz) {
   return l;
 }
 
-static bool ilqr_known_shape_ok(const mpcb200_dims* d) {
-  return (d->dynamics_kind == DYN_CARTPOLE && d->n == 5 && d->m == 1) ||
-         (d->dynamics_kind == DYN_PENDULUM && d->n == 3 && d->m == 1);
-}
-
 // argument checks that need no device: every error is reported before anything is captured or launched
 template <typename R>
 static int ilqr_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_ilqr_opts* o, const R* C,
@@ -476,18 +487,13 @@ static int ilqr_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb
     return MPCB200_ERR_NULL_POINTER;
   if (o->lqr_iter < 1 || o->m_ref < 1 || o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
   if (d->dynamics_kind != DYN_LINEAR) {
-    if (!ilqr_known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
+    if (!known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
   } else {
     if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
     if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
   }
-  if (d->bounds_kind < 0 || d->bounds_kind > 2) return MPCB200_ERR_BAD_DIMS;
-  if (d->bounds_kind == 2 && (u_lower == nullptr || u_upper == nullptr)) return MPCB200_ERR_NULL_POINTER;
-  if (d->has_zero_mask && u_zero_I == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (d->has_delta_u && d->bounds_kind == 0) return MPCB200_ERR_BAD_DIMS;
-  if (d->max_ls_iter < 1 || d->pnqp_max_iter < 1) return MPCB200_ERR_BAD_DIMS;
-  if (d->dynamics_kind == DYN_LINEAR && find(d->n, d->m) == nullptr && !runs_large(d->n, d->m))
-    return MPCB200_ERR_UNSUPPORTED_DIMS;
+  rc = check_step_options(d, u_lower, u_upper, u_zero_I);
+  if (rc) return rc;
   if (d->dynamics_kind != DYN_LINEAR && find(d->n, d->m) == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
   const IlqrLayout l = ilqr_layout(d, sizeof(R));
   if (workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
@@ -724,9 +730,7 @@ int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_
 
 size_t mpcb200_ilqr_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
   if (dims == nullptr || opts == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
-  if (dims->dynamics_kind == DYN_LINEAR ? (find(dims->n, dims->m) == nullptr && !runs_large(dims->n, dims->m))
-                                        : !ilqr_known_shape_ok(dims))
-    return 0;
+  if (dims->dynamics_kind != DYN_LINEAR && !known_shape_ok(dims)) return 0;
   return ilqr_layout(dims, (size_t)elem_size).total;
 }
 int mpcb200_ilqr_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,

@@ -5,6 +5,7 @@ keyword names, defaults, call signature ``(x_init, C, c, F, f)``, return arity a
 shapes, and the same gradient tuple ``(dx_init, dC, dc, dF, df)`` (:407).  The
 arithmetic runs in csrc/lqr_step.cuh and csrc/lqr_grad.cuh.
 """
+import collections
 import ctypes
 import os
 import threading
@@ -201,12 +202,17 @@ class _Pad:
         out[..., : self.n, self.idx] = F
         return out
 
-    def vec_n(self, x):
+    # an exact instance (or None) passes through unchanged
+    def vec_n(self, x):           # [..., n] -> [..., N]
+        if not self.active or x is None:
+            return x
         out = x.new_zeros(*x.shape[:-1], self.N)
         out[..., : self.n] = x
         return out
 
-    def vec_m(self, u, fill=0.0):
+    def vec_m(self, u, fill=0.0):  # [..., m] -> [..., M], padded controls = fill
+        if not self.active or u is None:
+            return u
         out = u.new_full((*u.shape[:-1], self.M), fill)
         out[..., : self.m] = u
         return out
@@ -240,6 +246,52 @@ class _Pad:
         return F[..., : self.n, self.idx] if self.active and F is not None else F
 
 
+_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params")
+
+
+def _problem(n, m, T, B, dtype, dev, C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None,
+             delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, dyn=None):
+    """A raw call's (n, m) problem as the kernels take it, at the instance it runs at (_pick_instance): the _Pad;
+    C, c, F, f staged by _Pad.stage; the tensor bounds and u_zero_I (as a uint8 mask) widened for padded controls;
+    and the Dims / Params of a step with a rollout, time strides included.  lqr_step_raw and ilqr_raw make the same
+    call, so the iLQR graph hands each kernel what a host loop of raw calls hands it.  A call whose Dims differ sets
+    those fields on the returned `dims`; the caller densifies and widens its x / u (_dense, _Pad.vec_n / vec_m)."""
+    N, M = _pick_instance(n, m, dtype.itemsize)
+    pad = _Pad(n, m, N, M, dev)
+    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
+    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
+    kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev, pad.active)
+    zmask = (u_zero_I != 0).to(torch.uint8).contiguous() if u_zero_I is not None else None
+    dims = Dims(B=B, T=T, n=N, m=M, F_T=F_.shape[0] if F_ is not None else T - 1, has_f=int(f_ is not None),
+                bounds_kind=kind, has_zero_mask=int(zmask is not None), has_delta_u=int(delta_u is not None),
+                max_ls_iter=int(max_linesearch_iter), pnqp_max_iter=PNQP_MAX_ITER, do_rollout=1,
+                dynamics_kind=int(dyn[0]) if dyn is not None else 0,
+                C_tstride=tsC, c_tstride=tsc, F_tstride=tsF, f_tstride=tsf)
+    params = Params(u_lo=float(s_lo), u_hi=float(s_hi), delta_u=float(delta_u) if delta_u is not None else 0.0,
+                    ls_decay=float(linesearch_decay))
+    if dyn is not None:
+        for i, v in enumerate(dyn[1]):
+            params.dyn[i] = float(v)
+    return _Problem(pad, C_, c_, F_, f_, pad.vec_m(lo_t, -1.0), pad.vec_m(hi_t, 1.0), pad.vec_m(zmask, 0),
+                    dims, params)
+
+
+def _grad_outputs(T, B, N, M, F, f_T, want_df, dtype, dev):
+    """The (dx_init, dC, dc, dF, df) buffers the gradient kernels fill: dF like the staged F (None without one), df
+    only when `want_df`, with f's leading dimension `f_T` (default T-1); the kernels write its slices < T-1, so a T-th
+    slice (full-length f) is zeroed here."""
+    P = N + M
+    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
+    dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
+    dc = torch.empty(T, B, P, dtype=dtype, device=dev)
+    dF = torch.empty(F.shape[0], B, N, P, dtype=dtype, device=dev) if F is not None else None
+    f_T = T - 1 if f_T is None else f_T
+    df = torch.empty(f_T, B, N, dtype=dtype, device=dev) if want_df else None
+    if want_df and f_T == T:
+        df[T - 1].zero_()
+    return dx_init, dC, dc, dF, df
+
+
 # ----------------------------------------------------------------------------------------------
 # raw calls (dense CUDA tensors in, fresh CUDA tensors out)
 # ----------------------------------------------------------------------------------------------
@@ -255,21 +307,11 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
                   ("current_u", cur_u, "TBm"), F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
                   exact=dyn is not None)
     dtype, dev = C.dtype, C.device
-    N, M = _pick_instance(n, m, C.element_size())
-    pad = _Pad(n, m, N, M, dev)
-    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
-    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
-    x0_, cx_, cu_ = _dense(x_init, dtype), _dense(cur_x, dtype), _dense(cur_u, dtype)
-    bounds_kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev, pad.active)
-    zmask = (u_zero_I != 0).to(torch.uint8).contiguous() if u_zero_I is not None else None
-    if pad.active:
-        x0_ = pad.vec_n(x0_) if x0_ is not None else None
-        cx_, cu_ = pad.vec_n(cx_), pad.vec_m(cu_)
-        if lo_t is not None:
-            lo_t, hi_t = pad.vec_m(lo_t, -1.0), pad.vec_m(hi_t, 1.0)
-        if zmask is not None:
-            zmask = pad.vec_m(zmask, 0)
-    F_T = F_.shape[0] if F_ is not None else T - 1
+    s = _problem(n, m, T, B, dtype, dev, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+                 max_linesearch_iter, dyn)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    dims.do_rollout = int(bool(do_rollout))
+    x0_, cx_, cu_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_n(_dense(cur_x, dtype)), pad.vec_m(_dense(cur_u, dtype))
 
     out = {}
     new_x = new_u = costs = fdn = alphas = None
@@ -284,15 +326,10 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
         du_first = torch.empty(T, B, M, dtype=dtype, device=dev)
     qp_iters = free_mask = status = None
     if want_stats:
-        qp_iters = torch.zeros(T, B, dtype=torch.int32, device=dev) if bounds_kind else None
+        qp_iters = torch.zeros(T, B, dtype=torch.int32, device=dev) if dims.bounds_kind else None
         free_mask = torch.empty(T, B, M, dtype=torch.uint8, device=dev)
         status = torch.empty(B, dtype=torch.int32, device=dev)
     Ks = ks = None
-    dims = Dims(B=B, T=T, n=N, m=M, F_T=F_T, has_f=int(f_ is not None), bounds_kind=bounds_kind,
-                has_zero_mask=int(zmask is not None), has_delta_u=int(delta_u is not None),
-                max_ls_iter=int(max_linesearch_iter), pnqp_max_iter=PNQP_MAX_ITER,
-                do_rollout=int(bool(do_rollout)), dynamics_kind=int(dyn[0]) if dyn is not None else 0,
-                C_tstride=tsC, c_tstride=tsc, F_tstride=tsF, f_tstride=tsf)
     need_gains = want_gains or not do_rollout
     if not need_gains:
         # long horizons do not fit shared memory: the kernel then keeps gains in a caller buffer
@@ -306,18 +343,12 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
     if need_gains:
         Ks = torch.empty(T, B, M, N, dtype=dtype, device=dev)
         ks = torch.empty(T, B, M, dtype=dtype, device=dev)
-    params = Params(u_lo=float(s_lo), u_hi=float(s_hi),
-                    delta_u=float(delta_u) if delta_u is not None else 0.0,
-                    ls_decay=float(linesearch_decay))
-    if dyn is not None:
-        for i, v in enumerate(dyn[1]):
-            params.dyn[i] = float(v)
     fn = _lib.entry("mpcb200_lqr_step", dtype)
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(params), ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr_view(f_),
-                ptr(x0_), ptr(cx_), ptr(cu_), ptr(lo_t), ptr(hi_t), ptr(zmask), ptr(new_x), ptr(new_u),
-                ptr(costs), ptr(fdn), ptr(alphas), ptr(du_first), ptr(qp_iters), ptr(free_mask), ptr(status),
-                ptr(Ks), ptr(ks), stream_handle(dev))
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ptr_view(s.C), ptr_view(s.c), ptr_view(s.F),
+                ptr_view(s.f), ptr(x0_), ptr(cx_), ptr(cu_), ptr(s.u_lower), ptr(s.u_upper), ptr(s.u_zero_I),
+                ptr(new_x), ptr(new_u), ptr(costs), ptr(fdn), ptr(alphas), ptr(du_first), ptr(qp_iters),
+                ptr(free_mask), ptr(status), ptr(Ks), ptr(ks), stream_handle(dev))
     check(rc, "mpcb200_lqr_step")
     if do_rollout:
         out.update(new_x=pad.crop_n(new_x), new_u=pad.crop_m(new_u), costs=costs, full_du_norm=fdn, alphas=alphas)
@@ -336,7 +367,7 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
     """The iLQR iterations of MPC.forward (reference mpc/mpc.py:244-301) in ONE library call: a CUDA graph that runs
     rollout, [linearisation,] step, best-iterate tracking and the stop test until the stop test ends it, without a
     host read.  The dynamics are LinDx(F, f), or the known system `dyn` = (kind, params) with F = f = None.  The
-    problem is zero padded once per solve to the kernel instance it runs at, which hands every kernel the values
+    problem is staged once per solve, by the _problem call lqr_step_raw makes, so every kernel gets the values
     lqr_step_raw and rollout_raw would hand it per call.  Returns a dict of device tensors x, u, costs, full_du_norm
     (the best iterate) and info = int32 [iterations run, iterations with an unconverged pnqp]; None when the driver
     has no conditional graph nodes (nothing was launched then)."""
@@ -345,29 +376,10 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
                   F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I, exact=dyn is not None,
                   need_F=dyn is None)
     dtype, dev = C.dtype, C.device
-    N, M = _pick_instance(n, m, C.element_size())
-    pad = _Pad(n, m, N, M, dev)
-    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
-    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
-    x0_, u0_ = _dense(x_init, dtype), _dense(u_init, dtype)
-    bounds_kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev, pad.active)
-    zmask = (u_zero_I != 0).to(torch.uint8).contiguous() if u_zero_I is not None else None
-    if pad.active:
-        x0_, u0_ = pad.vec_n(x0_), pad.vec_m(u0_)
-        if lo_t is not None:
-            lo_t, hi_t = pad.vec_m(lo_t, -1.0), pad.vec_m(hi_t, 1.0)
-        if zmask is not None:
-            zmask = pad.vec_m(zmask, 0)
-    dims = Dims(B=B, T=T, n=N, m=M, F_T=F_.shape[0] if F_ is not None else T - 1, has_f=int(f_ is not None),
-                bounds_kind=bounds_kind, has_zero_mask=int(zmask is not None), has_delta_u=int(delta_u is not None),
-                max_ls_iter=int(max_linesearch_iter), pnqp_max_iter=PNQP_MAX_ITER, do_rollout=1,
-                dynamics_kind=int(dyn[0]) if dyn is not None else 0,
-                C_tstride=tsC, c_tstride=tsc, F_tstride=tsF, f_tstride=tsf)
-    params = Params(u_lo=float(s_lo), u_hi=float(s_hi), delta_u=float(delta_u) if delta_u is not None else 0.0,
-                    ls_decay=float(linesearch_decay))
-    if dyn is not None:
-        for i, v in enumerate(dyn[1]):
-            params.dyn[i] = float(v)
+    s = _problem(n, m, T, B, dtype, dev, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+                 max_linesearch_iter, dyn)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
     opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
                          best_cost_eps=float(best_cost_eps))
     nbytes = _lib.lib().mpcb200_ilqr_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
@@ -379,9 +391,9 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
     info = torch.empty(2, dtype=torch.int32, device=dev)
     fn = _lib.entry("mpcb200_ilqr", dtype)
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(params), ctypes.byref(opts), ptr_view(C_), ptr_view(c_),
-                ptr_view(F_), ptr_view(f_), ptr(x0_), ptr(u0_), ptr(lo_t), ptr(hi_t), ptr(zmask), ptr(best_x),
-                ptr(best_u), ptr(costs), ptr(fdn), ptr(info), ptr(ws), nbytes, stream_handle(dev))
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), ptr_view(s.C), ptr_view(s.c),
+                ptr_view(s.F), ptr_view(s.f), ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper), ptr(s.u_zero_I),
+                ptr(best_x), ptr(best_u), ptr(costs), ptr(fdn), ptr(info), ptr(ws), nbytes, stream_handle(dev))
     if rc == _lib.ERR_NO_GRAPH_COND:
         return None
     check(rc, "mpcb200_ilqr")
@@ -394,32 +406,16 @@ def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_
     B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("new_x", new_x, "TBn"), ("new_u", new_u, "TBm"),
                   ("dx", dx, "TBn"), ("du", du, "TBm"), ("dl_dx", dl_dx, "TBn"), F=F)
     dtype, dev = C.dtype, C.device
-    N, M = _pick_instance(n, m, C.element_size())
-    pad = _Pad(n, m, N, M, dev)
-    (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
-    F_, tsF = pad.stage(F, dtype, pad.mat_np)
-    nx_, nu_ = _dense(new_x, dtype), _dense(new_u, dtype)
-    dx_, du_, r_ = _dense(dx, dtype), _dense(du, dtype), _dense(dl_dx, dtype)
-    if pad.active:
-        nx_, nu_, dx_, du_, r_ = pad.vec_n(nx_), pad.vec_m(nu_), pad.vec_n(dx_), pad.vec_m(du_), pad.vec_n(r_)
-    F_T = F_.shape[0] if F_ is not None else 0
-    P = N + M
-    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
-    dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
-    dc = torch.empty(T, B, P, dtype=dtype, device=dev)
-    dF = torch.empty(F_T, B, N, P, dtype=dtype, device=dev) if F_ is not None else None
-    # df has f's leading dimension; the kernel writes slices < T-1, a T-th slice (full-length f) is zero
-    f_T = T - 1 if f_T is None else f_T
-    df = torch.empty(f_T, B, N, dtype=dtype, device=dev) if want_df else None
-    if want_df and f_T == T:
-        df[T - 1].zero_()
-    dims = Dims(B=B, T=T, n=N, m=M, F_T=F_T if F_ is not None else T - 1, has_f=int(want_df),
-                bounds_kind=0, has_zero_mask=0, has_delta_u=0, max_ls_iter=1, pnqp_max_iter=1,
-                do_rollout=0, C_tstride=tsC, c_tstride=tsc, F_tstride=tsF)
+    s = _problem(n, m, T, B, dtype, dev, C, c, F)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    dims.has_f, dims.max_ls_iter, dims.pnqp_max_iter, dims.do_rollout = int(want_df), 1, 1, 0
+    nx_, nu_ = pad.vec_n(_dense(new_x, dtype)), pad.vec_m(_dense(new_u, dtype))
+    dx_, du_, r_ = pad.vec_n(_dense(dx, dtype)), pad.vec_m(_dense(du, dtype)), pad.vec_n(_dense(dl_dx, dtype))
+    dx_init, dC, dc, dF, df = _grad_outputs(T, B, N, M, s.F, f_T, want_df, dtype, dev)
     fn = _lib.entry("mpcb200_lqr_grad", dtype)
     ws = torch.empty(2 * T * B * N, dtype=dtype, device=dev)     # costates: enables the two-kernel path
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr(nx_), ptr(nu_), ptr(dx_),
+        rc = fn(ctypes.byref(dims), ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr(nx_), ptr(nu_), ptr(dx_),
                 ptr(du_), ptr(r_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(ws), stream_handle(dev))
     check(rc, "mpcb200_lqr_grad")
     return pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df)
@@ -459,7 +455,6 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
         return None
     dtype, dev = C.dtype, C.device
     B = C.shape[1]
-    p = n + m
     F_T = F.shape[0]
     kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev)
     (C_, tsC), (c_, tsc), (F_, tsF) = _time_strided(C, dtype), _time_strided(c, dtype), _time_strided(F, dtype)
@@ -471,11 +466,10 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
     if plan is None:
         fn = _lib.entry("mpcb200_lqr_adjoint", dtype)
         L = _lib.lib()
-        dims = Dims(B=B, T=T, n=n, m=m, F_T=F_T, has_f=int(want_df), bounds_kind=kind, has_zero_mask=0,
-                    has_delta_u=0, max_ls_iter=10, pnqp_max_iter=PNQP_MAX_ITER, do_rollout=1,
-                    C_tstride=tsC, c_tstride=tsc, F_tstride=tsF)
+        s = _problem(n, m, T, B, dtype, dev, C, c, F, None, u_lower, u_upper)   # for its Dims / Params
+        dims, params = s.dims, s.params
+        dims.has_f = int(want_df)
         fits = not L.mpcb200_step_prefers_workspace(ctypes.byref(dims), esz)
-        params = Params(u_lo=float(s_lo), u_hi=float(s_hi), delta_u=0.0, ls_decay=0.2)
         nbytes = L.mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), esz) if fits else 0
         if len(_adj_plans) > 256:
             _adj_plans.clear()
@@ -484,14 +478,7 @@ def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_l
     if not fits:
         return None
     nx_, nu_, gx_, gu_ = _dense(new_x, dtype), _dense(new_u, dtype), _dense(dl_dx, dtype), _dense(dl_du, dtype)
-    dx_init = torch.empty(B, n, dtype=dtype, device=dev)
-    dC = torch.empty(T, B, p, p, dtype=dtype, device=dev)
-    dc = torch.empty(T, B, p, dtype=dtype, device=dev)
-    dF = torch.empty(F_T, B, n, p, dtype=dtype, device=dev)
-    f_T = T - 1 if f_T is None else f_T
-    df = torch.empty(f_T, B, n, dtype=dtype, device=dev) if want_df else None
-    if want_df and f_T == T:
-        df[T - 1].zero_()
+    dx_init, dC, dc, dF, df = _grad_outputs(T, B, n, m, F_, f_T, want_df, dtype, dev)
     ws = _workspace(nbytes, dev)
     with _on_device(dev):
         rc = fn(dims_ref, params_ref, ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr(nx_), ptr(nu_), ptr(gx_),
@@ -506,21 +493,15 @@ def rollout_raw(n_state, n_ctrl, T, x_init, u, F, f=None):
     n, m = n_state, n_ctrl
     B = _validate(n, m, T, ("x_init", x_init, "Bn"), ("u", u, "TBm"), F=F, f=f)
     dtype, dev = x_init.dtype, x_init.device
-    N, M = _pick_instance(n, m, x_init.element_size())
-    pad = _Pad(n, m, N, M, dev)
-    (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
-    x0_, u_ = _dense(x_init, dtype), _dense(u, dtype)
-    if pad.active:
-        x0_, u_ = pad.vec_n(x0_), pad.vec_m(u_)
-    x = torch.empty(T, B, N, dtype=dtype, device=dev)
-    dims = Dims(B=B, T=T, n=N, m=M, F_T=F_.shape[0] if F_ is not None else T - 1, has_f=int(f_ is not None),
-                bounds_kind=0, has_zero_mask=0, has_delta_u=0, max_ls_iter=1, pnqp_max_iter=1, do_rollout=1,
-                F_tstride=tsF, f_tstride=tsf)
+    s = _problem(n, m, T, B, dtype, dev, F=F, f=f)
+    s.dims.max_ls_iter = s.dims.pnqp_max_iter = 1
+    x0_, u_ = s.pad.vec_n(_dense(x_init, dtype)), s.pad.vec_m(_dense(u, dtype))
+    x = torch.empty(T, B, s.pad.N, dtype=dtype, device=dev)
     fn = _lib.entry("mpcb200_rollout", dtype)
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ptr_view(F_), ptr_view(f_), ptr(x0_), ptr(u_), ptr(x), stream_handle(dev))
+        rc = fn(ctypes.byref(s.dims), ptr_view(s.F), ptr_view(s.f), ptr(x0_), ptr(u_), ptr(x), stream_handle(dev))
     check(rc, "mpcb200_rollout")
-    return pad.crop_n(x)
+    return s.pad.crop_n(x)
 
 
 # ----------------------------------------------------------------------------------------------
