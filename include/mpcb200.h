@@ -63,7 +63,8 @@ typedef struct mpcb200_dims {
   int32_t dynamics_kind;  /* true dynamics of the rollout (reference lqr_step.py:217-225):
                              MPCB200_DYN_LINEAR = LinDx(F,f); MPCB200_DYN_CARTPOLE / _PENDULUM = the step
                              function of that system evaluated inside the kernel (params.dyn); F,f are
-                             then its linearisation and are used by the Riccati sweep only (ABI v2)  */
+                             then its linearisation and are used by the Riccati sweep only (ABI v2);
+                             OR'd with MPCB200_DYN_CTRL_PASSTHROUGH: that system under a slew-rate penalty */
   int32_t reserved0;      /* 0 (keeps the 64-bit fields below naturally aligned)              */
   /* Elements between consecutive TIME slices of C, c, F, f (ABI v2).  0: dense ([T,B,...] contiguous; what a
    * zero-initialised struct means).  > 0: that many elements.  MPCB200_TIME_INVARIANT (-1): one [B,...] slice
@@ -82,8 +83,13 @@ typedef struct mpcb200_params {
 
 /* Known nonlinear systems (reference mpc/env_dx/cartpole.py:63-96, mpc/env_dx/pendulum.py:49-84).
  * dyn[] = cartpole: gravity, masscart, masspole, length, force_mag, dt   (state x,dx,cos th,sin th,dth; n=5, m=1)
- *         pendulum: g, m, l, (unused), max_torque, dt                    (state cos th,sin th,dth; n=3, m=1) */
-enum { MPCB200_DYN_LINEAR = 0, MPCB200_DYN_CARTPOLE = 1, MPCB200_DYN_PENDULUM = 2 };
+ *         pendulum: g, m, l, (unused), max_torque, dt                    (state cos th,sin th,dth; n=3, m=1)
+ * MPCB200_DYN_CTRL_PASSTHROUGH, OR'd into CARTPOLE or PENDULUM: the slew-rate augmented system of the reference's
+ * CtrlPassthroughDynamics (mpc/dynamics.py:133-156).  State [u_{t-1}; x] (n = n_system + 1, m = 1), step
+ * [u; step(x, u)] with u the control before the system's own clamp; its linearisation is F = [[0, 0, I], [0, R, S]],
+ * f = [0; f_system].  Same dyn[] as the system.  Accepted by every call that takes a kind, at exactly that (n, m);
+ * the step runs a dynamics-only kernel instance, which mpcb200_supported / _supported_list do not list. */
+enum { MPCB200_DYN_LINEAR = 0, MPCB200_DYN_CARTPOLE = 1, MPCB200_DYN_PENDULUM = 2, MPCB200_DYN_CTRL_PASSTHROUGH = 16 };
 #define MPCB200_TIME_INVARIANT (-1)
 
 /* Per-problem status bits written to `status[B]`. */
@@ -200,8 +206,9 @@ int mpcb200_rollout_f64(const mpcb200_dims* dims, const double* F, const double*
  *   mpcb200_dyn_linearize_*: F[t,b] = [d step/dx, d step/du], f[t,b] = step(x,u) - F [x;u] at (x[t,b], u[t,b]),
  *                            t < T-1 - linearize_dynamics (reference mpc/mpc.py:490-601; its AUTO_DIFF mode does
  *                            (T-1)*n_state autograd passes).  Exact Jacobians by forward-mode dual numbers.
- * kind = MPCB200_DYN_CARTPOLE | MPCB200_DYN_PENDULUM; dyn = HOST pointer to 8 doubles (see mpcb200_params.dyn);
- * x_init[B,n] u[T,B,m] x[T,B,n] F[T-1,B,n,n+m] f[T-1,B,n]; n, m are those of the system.
+ * kind = MPCB200_DYN_CARTPOLE | MPCB200_DYN_PENDULUM, optionally | MPCB200_DYN_CTRL_PASSTHROUGH; dyn = HOST pointer
+ * to 8 doubles (see mpcb200_params.dyn); x_init[B,n] u[T,B,m] x[T,B,n] F[T-1,B,n,n+m] f[T-1,B,n]; n, m are those of
+ * the kind (n_system + 1 states with the passthrough).
  */
 int mpcb200_dyn_rollout_f32(int32_t kind, const double* dyn, int32_t B, int32_t T, const float* x_init,
                             const float* u, float* x, void* stream);

@@ -49,9 +49,39 @@ static const Entry kTable[] = {
 };
 static const int kTableLen = (int)(sizeof(kTable) / sizeof(kTable[0]));
 
+// dynamics-only step instances (inst_dyn.cu): no gradient or rollout kernels, and not listed by mpcb200_supported*
+#define MPCB200_DYN_INST(kind, n, m)                                        \
+  int dstep_f32__##kind(const StepArgs&, int, cudaStream_t);                \
+  int dstep_f64__##kind(const StepArgs&, int, cudaStream_t);                \
+  int dpws_f32__##kind(int, int);                                           \
+  int dpws_f64__##kind(int, int);                                           \
+  size_t dsmem_f32__##kind(int);                                            \
+  size_t dsmem_f64__##kind(int);
+#include "dyn_instances.def"
+#undef MPCB200_DYN_INST
+struct DynEntry {
+  int kind;
+  Entry e;
+};
+static const DynEntry kDynTable[] = {
+#define MPCB200_DYN_INST(kind, n, m)                                                                        \
+  {kind, {n, m, dstep_f32__##kind, dstep_f64__##kind, nullptr, nullptr, dsmem_f32__##kind, dsmem_f64__##kind, \
+          nullptr, nullptr, dpws_f32__##kind, dpws_f64__##kind}},
+#include "dyn_instances.def"
+#undef MPCB200_DYN_INST
+};
+
 static const Entry* find(int n, int m) {
   for (int i = 0; i < kTableLen; ++i)
     if (kTable[i].n == n && kTable[i].m == m) return &kTable[i];
+  return nullptr;
+}
+// the step instance of a call: the (n, m) instance, or for a passthrough kind its dynamics-only instance at exactly
+// that kind's (n, m)
+static const Entry* find_step(const mpcb200_dims* d) {
+  if ((d->dynamics_kind & DYN_CTRL_PASSTHROUGH) == 0) return find(d->n, d->m);
+  for (const DynEntry& de : kDynTable)
+    if (de.kind == d->dynamics_kind && de.e.n == d->n && de.e.m == d->m) return &de.e;
   return nullptr;
 }
 
@@ -118,8 +148,8 @@ static int check_step_options(const mpcb200_dims* d, const void* lo, const void*
 }
 
 static bool known_shape_ok(const mpcb200_dims* d) {
-  return (d->dynamics_kind == DYN_CARTPOLE && d->n == 5 && d->m == 1) ||
-         (d->dynamics_kind == DYN_PENDULUM && d->n == 3 && d->m == 1);
+  int n = 0, m = 0;
+  return dyn_kind_dims(d->dynamics_kind, n, m) && d->n == n && d->m == m;
 }
 
 struct AdjExtra {      // fused-adjoint request riding on a step launch (api-internal)
@@ -151,7 +181,7 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
     return MPCB200_ERR_NULL_POINTER;
   }
   if ((Ks == nullptr) != (ks == nullptr)) return MPCB200_ERR_NULL_POINTER;
-  const Entry* e = find(d->n, d->m);
+  const Entry* e = find_step(d);
   const bool large = d->dynamics_kind == DYN_LINEAR && runs_large(d->n, d->m);
   if (e == nullptr && !large) return MPCB200_ERR_UNSUPPORTED_DIMS;
   const int smem = max_smem_optin();
@@ -402,7 +432,8 @@ template <typename R>
 static int dyn_impl(bool linearize, int kind, const double* dyn, int B, int T, const R* x_or_init, const R* u,
                     R* x_out, R* F, R* f, void* stream) {
   if (dyn == nullptr || x_or_init == nullptr || u == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (B <= 0 || T <= 0 || (kind != DYN_CARTPOLE && kind != DYN_PENDULUM)) return MPCB200_ERR_BAD_DIMS;
+  int n = 0, m = 0;
+  if (B <= 0 || T <= 0 || !dyn_kind_dims(kind, n, m)) return MPCB200_ERR_BAD_DIMS;
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   DynArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -494,7 +525,7 @@ static int ilqr_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb
   }
   rc = check_step_options(d, u_lower, u_upper, u_zero_I);
   if (rc) return rc;
-  if (d->dynamics_kind != DYN_LINEAR && find(d->n, d->m) == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
+  if (d->dynamics_kind != DYN_LINEAR && find_step(d) == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
   const IlqrLayout l = ilqr_layout(d, sizeof(R));
   if (workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
@@ -764,15 +795,17 @@ uint64_t mpcb200_launch_count(void) { return g_launches.load(); }
 
 size_t mpcb200_step_smem_bytes(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr) return 0;
-  const Entry* e = find(dims->n, dims->m);
+  const Entry* e = find_step(dims);
   if (e == nullptr) return 0;
   return elem_size == 8 ? e->smem64(dims->T) : e->smem32(dims->T);
 }
 
 int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr) return 0;
-  if (runs_large(dims->n, dims->m)) return 1;   // the large-shape step keeps its gains in Ks/ks
-  const Entry* e = find(dims->n, dims->m);
+  const bool passthrough = (dims->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0;
+  if (!passthrough && runs_large(dims->n, dims->m)) return 1;   // the large-shape step keeps its gains in Ks/ks
+  const Entry* e = find_step(dims);
+  if (e == nullptr) return 1;                   // no instance: the step call itself reports it
   int ms = max_smem_optin();
   if (ms <= 0) ms = kOptinAssumed;    // no device visible (CPU-side query): assume H100's opt-in limit
   return elem_size == 8 ? e->pws64(dims->T, ms) : e->pws32(dims->T, ms);

@@ -11,7 +11,9 @@
 
 namespace mpcb200 {
 
-enum { DYN_LINEAR = 0, DYN_CARTPOLE = 1, DYN_PENDULUM = 2 };
+// DYN_CTRL_PASSTHROUGH is OR'd into a system's kind: the slew-rate augmented state [u_{t-1}; x] with dynamics
+// [u; f(x, u)] (reference CtrlPassthroughDynamics, mpc/dynamics.py:133-156), n_state + n_ctrl states
+enum { DYN_LINEAR = 0, DYN_CARTPOLE = 1, DYN_PENDULUM = 2, DYN_CTRL_PASSTHROUGH = 16 };
 
 struct DynParams {
   // cartpole: p[0..3] = gravity, masscart, masspole, length; p[4] = force_mag; p[5] = dt
@@ -149,16 +151,44 @@ MPCB_DEV void pendulum_step(const DynParams& dp, const T (&s)[3], const T& u_in,
 }
 
 template <int KIND>
-struct DynDims;
+struct DynDims {        // a passthrough kind: [u_{t-1}; x]
+  static_assert((KIND & DYN_CTRL_PASSTHROUGH) != 0, "unknown dynamics kind");
+  using Inner = DynDims<KIND & ~DYN_CTRL_PASSTHROUGH>;
+  static constexpr int N = Inner::N + Inner::M, M = Inner::M;
+};
 template <>
 struct DynDims<DYN_CARTPOLE> { static constexpr int N = 5, M = 1; };
 template <>
 struct DynDims<DYN_PENDULUM> { static constexpr int N = 3, M = 1; };
 
+// (n_state, n_ctrl) of a known kind, passthrough or not; false for DYN_LINEAR and anything unknown
+inline bool dyn_kind_dims(int kind, int& n, int& m) {
+  const int sys = kind & ~DYN_CTRL_PASSTHROUGH;
+  if (sys == DYN_CARTPOLE) n = DynDims<DYN_CARTPOLE>::N, m = DynDims<DYN_CARTPOLE>::M;
+  else if (sys == DYN_PENDULUM) n = DynDims<DYN_PENDULUM>::N, m = DynDims<DYN_PENDULUM>::M;
+  else return false;
+  if (kind & DYN_CTRL_PASSTHROUGH) n += m;
+  return true;
+}
+
+// one step of a known kind; a passthrough kind copies u (before the system's own clamp) into the first M states
 template <typename R, int KIND, typename T>
 MPCB_DEV void dyn_step(const DynParams& dp, const T (&s)[DynDims<KIND>::N], const T& u, T (&o)[DynDims<KIND>::N]) {
-  if constexpr (KIND == DYN_CARTPOLE) cartpole_step<R, T>(dp, s, u, o);
-  else pendulum_step<R, T>(dp, s, u, o);
+  if constexpr ((KIND & DYN_CTRL_PASSTHROUGH) != 0) {
+    constexpr int SYS = KIND & ~DYN_CTRL_PASSTHROUGH, NI = DynDims<SYS>::N;
+    static_assert(DynDims<SYS>::M == 1, "the known systems have one control");
+    T si[NI], oi[NI];
+#pragma unroll
+    for (int i = 0; i < NI; ++i) si[i] = s[1 + i];
+    dyn_step<R, SYS, T>(dp, si, u, oi);
+    o[0] = u;
+#pragma unroll
+    for (int i = 0; i < NI; ++i) o[1 + i] = oi[i];
+  } else if constexpr (KIND == DYN_CARTPOLE) {
+    cartpole_step<R, T>(dp, s, u, o);
+  } else {
+    pendulum_step<R, T>(dp, s, u, o);
+  }
 }
 
 // ------------------------------------------------------------------ kernels
@@ -169,7 +199,8 @@ struct DynArgs {
   void *x_out, *F, *f;
 };
 
-// x[0] = x_init, x[t+1] = dyn(x[t], u[t]): util.get_traj for a known Module (one thread per problem)
+// x[0] = x_init, x[t+1] = dyn(x[t], u[t]): util.get_traj for a known Module (one thread per problem); for a
+// passthrough kind x is [T, B, n+m] and x[t+1] = [u[t]; dyn(x[t][m:], u[t])]
 template <typename R, int KIND>
 __global__ void __launch_bounds__(128) dyn_rollout_kernel(const DynArgs a) {
   constexpr int N = DynDims<KIND>::N, M = DynDims<KIND>::M;
@@ -196,43 +227,84 @@ __global__ void __launch_bounds__(128) dyn_rollout_kernel(const DynArgs a) {
 }
 
 // F[t,b] = [dx'/dx  dx'/du], f[t,b] = x' - F [x;u] at (x[t,b], u[t,b]) for t < T-1 (one thread per (t, problem))
+// A passthrough kind differentiates only the system itself (n + m dual variables, the system's own F and f) and
+// writes F~ = [[0, 0, I], [0, R, S]], f~ = [0; f]: the blocks MPC assembles from the system's F and f.
 template <typename R, int KIND>
 __global__ void __launch_bounds__(128) dyn_linearize_kernel(const DynArgs a) {
   constexpr int N = DynDims<KIND>::N, M = DynDims<KIND>::M, P = N + M;
-  using D = Dual<R, P>;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)(a.T - 1) * a.B) return;
   const R* gx = (const R*)a.x + i * N;
   const R* gu = (const R*)a.u + i * M;
-  D s[N], o[N];
-  R xv[P];
+  if constexpr ((KIND & DYN_CTRL_PASSTHROUGH) != 0) {
+    constexpr int SYS = KIND & ~DYN_CTRL_PASSTHROUGH, NI = DynDims<SYS>::N, PI = NI + M;
+    using D = Dual<R, PI>;
+    D s[NI], o[NI];
+    R xv[PI];
 #pragma unroll
-  for (int k = 0; k < N; ++k) {
-    xv[k] = gx[k];
-    s[k] = dual_var<R, P>(xv[k], k);
-  }
-  xv[N] = gu[0];
-  const D u = dual_var<R, P>(xv[N], N);
-  dyn_step<R, KIND, D>(a.dp, s, u, o);
-  R* oF = (R*)a.F + i * N * P;
-  R* of = (R*)a.f + i * N;
-#pragma unroll
-  for (int r = 0; r < N; ++r) {
-    R acc = o[r].v;
-#pragma unroll
-    for (int k = 0; k < P; ++k) {
-      oF[r * P + k] = o[r].d[k];
-      acc -= o[r].d[k] * xv[k];
+    for (int k = 0; k < NI; ++k) {
+      xv[k] = gx[M + k];
+      s[k] = dual_var<R, PI>(xv[k], k);
     }
-    of[r] = acc;
+    xv[NI] = gu[0];
+    const D u = dual_var<R, PI>(xv[NI], NI);
+    dyn_step<R, SYS, D>(a.dp, s, u, o);
+    R* oF = (R*)a.F + i * N * P;
+    R* of = (R*)a.f + i * N;
+#pragma unroll
+    for (int r = 0; r < M; ++r) {              // u_{t} -> the first M states
+#pragma unroll
+      for (int k = 0; k < P; ++k) oF[r * P + k] = k == N + r ? R(1) : R(0);
+      of[r] = R(0);
+    }
+#pragma unroll
+    for (int r = 0; r < NI; ++r) {
+      R acc = o[r].v;
+      R* row = oF + (M + r) * P;
+#pragma unroll
+      for (int k = 0; k < M; ++k) row[k] = R(0);
+#pragma unroll
+      for (int k = 0; k < PI; ++k) {
+        row[M + k] = o[r].d[k];
+        acc -= o[r].d[k] * xv[k];
+      }
+      of[M + r] = acc;
+    }
+  } else {
+    using D = Dual<R, P>;
+    D s[N], o[N];
+    R xv[P];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      xv[k] = gx[k];
+      s[k] = dual_var<R, P>(xv[k], k);
+    }
+    xv[N] = gu[0];
+    const D u = dual_var<R, P>(xv[N], N);
+    dyn_step<R, KIND, D>(a.dp, s, u, o);
+    R* oF = (R*)a.F + i * N * P;
+    R* of = (R*)a.f + i * N;
+#pragma unroll
+    for (int r = 0; r < N; ++r) {
+      R acc = o[r].v;
+#pragma unroll
+      for (int k = 0; k < P; ++k) {
+        oF[r * P + k] = o[r].d[k];
+        acc -= o[r].d[k] * xv[k];
+      }
+      of[r] = acc;
+    }
   }
 }
 
 template <typename R>
 int launch_dyn_rollout(const DynArgs& a, cudaStream_t stream) {
   const int grid = (a.B + 127) / 128;
+  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH;
   if (a.kind == DYN_CARTPOLE) dyn_rollout_kernel<R, DYN_CARTPOLE><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == DYN_PENDULUM) dyn_rollout_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == CP) dyn_rollout_kernel<R, CP><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == PP) dyn_rollout_kernel<R, PP><<<grid, 128, 0, stream>>>(a);
   else return 2;
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }
@@ -241,8 +313,11 @@ int launch_dyn_linearize(const DynArgs& a, cudaStream_t stream) {
   const size_t items = (size_t)(a.T - 1) * a.B;
   if (items == 0) return 0;
   const int grid = (int)((items + 127) / 128);
+  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH;
   if (a.kind == DYN_CARTPOLE) dyn_linearize_kernel<R, DYN_CARTPOLE><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == DYN_PENDULUM) dyn_linearize_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == CP) dyn_linearize_kernel<R, CP><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == PP) dyn_linearize_kernel<R, PP><<<grid, 128, 0, stream>>>(a);
   else return 2;
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }

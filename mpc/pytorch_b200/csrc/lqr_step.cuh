@@ -494,9 +494,11 @@ MPCB_DEV void step_producer(const StepArgs& a, unsigned char* stage_base, uint64
 // ---------------------------------------------------------------------------------------------
 // consumer warps.  MODE (compile time): 0 plain (no bounds, no mask), 1 box (pnqp; optional
 // u_zero_I), 2 mask (u_zero_I only - the adjoint solve).
+// DYN: DYN_LINEAR for the (n, m) instances, whose rollout takes the true dynamics from a.dyn_kind; a passthrough kind
+// (DYN_CTRL_PASSTHROUGH | system) for the dynamics-only instances, whose rollout always runs that kind's dyn_step.
 // ---------------------------------------------------------------------------------------------
 
-template <typename R, int N, int M, int MODE>
+template <typename R, int N, int M, int MODE, int DYN = DYN_LINEAR>
 MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64_t* full,
                             uint64_t* empty, volatile int* votes, R* scratch_all, R* kstore_all,
                             int b0, int warp, int lane) {
@@ -948,7 +950,18 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
         xn[sl] = R(0);
         if (K::x_slot(sl) && t < T - 1) {                         // (:217-222), or true_dynamics(x, u) (:224-225)
           bool known = false;
-          if constexpr (M == 1 && (N == DynDims<DYN_CARTPOLE>::N || N == DynDims<DYN_PENDULUM>::N)) {
+          if constexpr (DYN != DYN_LINEAR) {      // [u; dyn_step(x[m:], u)], as the known system below
+            static_assert(N == DynDims<DYN>::N && M == DynDims<DYN>::M, "instance shape of the dynamics kind");
+            known = true;
+            R sv[N], ov[N];
+#pragma unroll
+            for (int i = 0; i < N; ++i) sv[i] = tau.get(i);
+            dyn_step<R, DYN, R>(a.dp, sv, tau.get(N), ov);
+            xn[sl] = ov[0];
+#pragma unroll
+            for (int i = 1; i < N; ++i)
+              if (fr[sl] == i) xn[sl] = ov[i];
+          } else if constexpr (M == 1 && (N == DynDims<DYN_CARTPOLE>::N || N == DynDims<DYN_PENDULUM>::N)) {
             if (a.dyn_kind != DYN_LINEAR) {       // every lane evaluates the step function and keeps its row
               known = true;
               R sv[N], ov[N];
@@ -1003,7 +1016,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
   if (wr && j == 0) write_step_result<R>(a, b, alpha, cost, fdn, status);
 }
 
-template <typename R, int N, int M, int MODE>
+template <typename R, int N, int M, int MODE, int DYN = DYN_LINEAR>
 __global__ void __launch_bounds__(StepCfg<R, N, M>::THREADS, StepCfg<R, N, M>::MIN_CTAS)
 lqr_step_kernel(const StepArgs a) {
   using K = StepCfg<R, N, M>;
@@ -1031,32 +1044,32 @@ lqr_step_kernel(const StepArgs a) {
   if (warp == K::NW) {
     step_producer<R, N, M>(a, stage_base, full, empty, votes, b0, cnt, lane);
   } else {
-    step_consumer<R, N, M, MODE>(a, stage_base, full, empty, votes, scratch, kstore, b0, warp, lane);
+    step_consumer<R, N, M, MODE, DYN>(a, stage_base, full, empty, votes, scratch, kstore, b0, warp, lane);
   }
 }
 
-template <typename R, int N, int M, int MODE>
+template <typename R, int N, int M, int MODE, int DYN = DYN_LINEAR>
 int launch_step_mode(const StepArgs& args, int max_smem_optin, cudaStream_t stream) {
   using K = StepCfg<R, N, M>;
   StepArgs a = args;
   size_t smem;
   int rc = plan_gain_store(a, K::prefers_workspace(a.T, max_smem_optin), max_smem_optin,
                            [&](bool k_in_smem) { return K::smem_bytes(a.T, k_in_smem); }, smem);
-  if (rc == MPCB200_OK) rc = allow_smem_optin<lqr_step_kernel<R, N, M, MODE>>(max_smem_optin);
+  if (rc == MPCB200_OK) rc = allow_smem_optin<lqr_step_kernel<R, N, M, MODE, DYN>>(max_smem_optin);
   if (rc != MPCB200_OK) return rc;
   const int grid = (a.B + K::W - 1) / K::W;
-  lqr_step_kernel<R, N, M, MODE><<<grid, K::THREADS, smem, stream>>>(a);
+  lqr_step_kernel<R, N, M, MODE, DYN><<<grid, K::THREADS, smem, stream>>>(a);
   if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
   record_step_plan((int)(MPCB200_PLAN_GENERIC | (a.k_in_smem ? MPCB200_PLAN_GAINS_SMEM : 0u) |
                          (K::KREDUCE && !a.k_in_smem && a.do_rollout ? MPCB200_PLAN_KREDUCE : 0u)));
   return MPCB200_OK;
 }
 
-template <typename R, int N, int M>
+template <typename R, int N, int M, int DYN = DYN_LINEAR>
 int launch_step(const StepArgs& a, int max_smem_optin, cudaStream_t stream) {
-  if (a.bounds_kind != 0) return launch_step_mode<R, N, M, MODE_BOX>(a, max_smem_optin, stream);
-  if (a.has_mask) return launch_step_mode<R, N, M, MODE_MASK>(a, max_smem_optin, stream);
-  return launch_step_mode<R, N, M, MODE_PLAIN>(a, max_smem_optin, stream);
+  if (a.bounds_kind != 0) return launch_step_mode<R, N, M, MODE_BOX, DYN>(a, max_smem_optin, stream);
+  if (a.has_mask) return launch_step_mode<R, N, M, MODE_MASK, DYN>(a, max_smem_optin, stream);
+  return launch_step_mode<R, N, M, MODE_PLAIN, DYN>(a, max_smem_optin, stream);
 }
 
 template <typename R, int N, int M>

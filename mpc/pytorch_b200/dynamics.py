@@ -23,7 +23,11 @@ from . import _lib
 from ._lib import MpcB200Error, _on_device, check, ptr, stream_handle
 
 DYN_LINEAR, DYN_CARTPOLE, DYN_PENDULUM = 0, 1, 2
+# OR'd into a known system's kind: that system under a slew-rate penalty, state [u_{t-1}; x]
+# (solver.CtrlPassthroughDynamics), which the step runs on a dynamics-only kernel instance
+DYN_CTRL_PASSTHROUGH = 16
 DYN_DIMS = {DYN_CARTPOLE: (5, 1), DYN_PENDULUM: (3, 1)}       # (n_state, n_ctrl) of each known system
+DYN_DIMS.update({k | DYN_CTRL_PASSTHROUGH: (n + m, m) for k, (n, m) in DYN_DIMS.items()})
 
 _scope = threading.local()      # depth and epoch of the enclosing params_scope() on this thread
 _epochs = itertools.count(1)    # process-wide: two threads' scopes never share an epoch (the cache is per module)

@@ -98,11 +98,19 @@ class SlewRateCost(Module):
 
 
 class CtrlPassthroughDynamics(Module):
-    """Dynamics of the slew-augmented state [u_{t-1}; x] (reference mpc/dynamics.py:133-156)."""
+    """Dynamics of the slew-augmented state [u_{t-1}; x] (reference mpc/dynamics.py:133-156).  Wrapping a known
+    system (dynamics.CartpoleDx / PendulumDx) it is one too, of kind inner | DYN_CTRL_PASSTHROUGH, so its rollout,
+    linearisation and line-search rollout run in the kernels; any other Module keeps the Module path."""
 
     def __init__(self, dynamics):
         super().__init__()
         self.dynamics = dynamics
+        from .dynamics import DYN_CARTPOLE, DYN_CTRL_PASSTHROUGH, DYN_PENDULUM
+        kind = getattr(dynamics, "mpcb200_kind", None)
+        if kind in (DYN_CARTPOLE, DYN_PENDULUM):
+            self.mpcb200_kind = kind | DYN_CTRL_PASSTHROUGH
+            self.n_state, self.n_ctrl = dynamics.n_state + dynamics.n_ctrl, dynamics.n_ctrl
+            self.mpcb200_params = dynamics.mpcb200_params      # the system's: its params_scope cache applies
 
     def forward(self, tilde_x, u):
         squeeze = tilde_x.dim() == 1
@@ -218,7 +226,8 @@ class MPC(Module):
             print("Initial mean(cost): {:.4e}".format(
                 torch.mean(get_cost(T, u, cost, dx, x_init=x_init)).item()))
 
-        best = self._ilqr_device(x_init, cost, dx, u) if _use_device_loop(self, x_init, cost, dx, u) else None
+        on_device = _use_device_loop(self, x_init, cost, dx, u) or _use_slew_device_loop(self, x_init, cost, dx, u)
+        best = self._ilqr_device(x_init, cost, dx, u) if on_device else None
         if best is None:
             best = self._ilqr_host(x_init, cost, dx, u)
         x, u = best["x"], best["u"]
@@ -260,13 +269,20 @@ class MPC(Module):
         global _graph_cond_unavailable
         from . import step as _step
         T, n, m = self.T, self.n_state, self.n_ctrl
+        C, c = cost.C, cost.c
+        F, f = (dx.F, dx.f) if isinstance(dx, LinDx) else (None, None)
+        if self.slew_rate_penalty is not None:       # the augmented problem, staged once for the whole solve
+            _, C, c, F, f, _, x_init = self._slew_augment(x_init, C, c, F, f)
+            if not isinstance(dx, LinDx):
+                dx = CtrlPassthroughDynamics(dx)
+            n = n + m
         if isinstance(dx, LinDx):
-            F, f, dyn = dx.F, dx.f, None
+            dyn = None
         else:
             from .dynamics import known_kind
             F = f = None
             dyn = known_kind(dx, n, m, x_init)
-        res = _step.ilqr_raw(n, m, T, x_init, cost.C, cost.c, F, f, u, u_lower=self.u_lower, u_upper=self.u_upper,
+        res = _step.ilqr_raw(n, m, T, x_init, C, c, F, f, u, u_lower=self.u_lower, u_upper=self.u_upper,
                              u_zero_I=self.u_zero_I, delta_u=self.delta_u, linesearch_decay=self.linesearch_decay,
                              max_linesearch_iter=self.max_linesearch_iter, lqr_iter=self.lqr_iter,
                              not_improved_lim=self.not_improved_lim, eps=self.eps, best_cost_eps=self.best_cost_eps,
@@ -277,7 +293,8 @@ class MPC(Module):
         if self.verbose >= 0 and self.u_lower is not None:
             for _ in range(int(res["info"][1])):             # the one host read: iterations with a pnqp warning
                 print("[WARNING] pnqp warning: Did not converge")   # reference pnqp.py:81
-        return {"x": res["x"], "u": res["u"], "costs": res["costs"], "full_du_norm": res["full_du_norm"]}
+        x = res["x"][:, :, m:] if self.slew_rate_penalty is not None else res["x"]
+        return {"x": x, "u": res["u"], "costs": res["costs"], "full_du_norm": res["full_du_norm"]}
 
     def _ilqr_host(self, x_init, cost, dx, u):
         """The iLQR iterations from Python: one host read per iteration for the stop test."""
@@ -361,6 +378,24 @@ class MPC(Module):
             return _lqr(x_init, C, c, F, f if f is not None else e)
 
         # ---- slew-rate penalty: augment the state with the previous control (reference :362-445)
+        n2 = n + m
+        slew_C, C2, c2, F2, f2, prev_u, x_init2 = self._slew_augment(x_init, C, c, F, f)
+        x2 = torch.cat((torch.cat((prev_u, _detach(u)[:-1])), x), 2)
+        dyn2 = None if isinstance(dynamics, LinDx) else CtrlPassthroughDynamics(dynamics)
+        if isinstance(dynamics, LinDx):
+            dyn2 = LinDx(F2, f2 if f2.nelement() > 0 else None)
+        true_cost2 = QuadCost(C2, c2) if isinstance(cost, QuadCost) else \
+            SlewRateCost(cost, slew_C, n, m)
+        _lqr = LQRStep(n_state=n2, n_ctrl=m, true_cost=true_cost2, true_dynamics=dyn2,
+                       current_x=x2, current_u=u, **common)
+        xo, *rest = _lqr(x_init2, C2, c2, F2, f2)
+        return [xo[:, :, m:]] + list(rest)
+
+    def _slew_augment(self, x_init, C, c, F, f):
+        """The slew-rate augmented problem over the state [u_{t-1}; x] (reference :362-445): (slew_C, C2, c2, F2, f2,
+        prev_u[1,B,m], x_init2).  F2 = [[0, 0, I], [0, F]] and f2 = [0; f] (empty without f); both None without F
+        (a known system, which the kernels linearise in augmented form).  Differentiable in C, c, F, f and x_init."""
+        n, m, T = self.n_state, self.n_ctrl, self.T
         B = C.size(1)
         n2, p2 = n + m, n + 2 * m
         kw = dict(dtype=C.dtype, device=C.device)
@@ -373,15 +408,16 @@ class MPC(Module):
         C2 = slew_C.clone()
         C2[:, :, m:, m:] += C
         c2 = torch.cat((torch.zeros(T, B, m, **kw), c), 2)
-        Fu = torch.zeros(F.shape[0], B, m, p2, **kw)
-        Fu[:, :, :, n2:] = torch.eye(m, **kw)
-        Fx = torch.cat((torch.zeros(F.shape[0], B, n, m, **kw), F), 3)
-        F2 = torch.cat((Fu, Fx), 2)
-        if f is not None and f.nelement() > 0:
-            f2 = torch.cat((torch.zeros(f.shape[0], B, m, **kw), f), 2)
-        else:
-            f2 = torch.empty(0, **kw)
-        u_data = _detach(u)
+        F2 = f2 = None
+        if F is not None:
+            Fu = torch.zeros(F.shape[0], B, m, p2, **kw)
+            Fu[:, :, :, n2:] = torch.eye(m, **kw)
+            Fx = torch.cat((torch.zeros(F.shape[0], B, n, m, **kw), F), 3)
+            F2 = torch.cat((Fu, Fx), 2)
+            if f is not None and f.nelement() > 0:
+                f2 = torch.cat((torch.zeros(f.shape[0], B, m, **kw), f), 2)
+            else:
+                f2 = torch.empty(0, **kw)
         if self.prev_ctrl is not None:
             prev_u = self.prev_ctrl
             while prev_u.ndimension() < 3:
@@ -391,17 +427,8 @@ class MPC(Module):
                 prev_u = prev_u.expand(1, B, m)
         else:
             prev_u = torch.zeros(1, B, m, **kw)
-        x2 = torch.cat((torch.cat((prev_u, u_data[:-1])), x), 2)
         x_init2 = torch.cat((prev_u[0], x_init), 1)
-        dyn2 = None if isinstance(dynamics, LinDx) else CtrlPassthroughDynamics(dynamics)
-        if isinstance(dynamics, LinDx):
-            dyn2 = LinDx(F2, f2 if f2.nelement() > 0 else None)
-        true_cost2 = QuadCost(C2, c2) if isinstance(cost, QuadCost) else \
-            SlewRateCost(cost, slew_C, n, m)
-        _lqr = LQRStep(n_state=n2, n_ctrl=m, true_cost=true_cost2, true_dynamics=dyn2,
-                       current_x=x2, current_u=u, **common)
-        xo, *rest = _lqr(x_init2, C2, c2, F2, f2)
-        return [xo[:, :, m:]] + list(rest)
+        return slew_C, C2, c2, F2, f2, prev_u, x_init2
 
     # ------------------------------------------------------------------------------------
     def approximate_cost(self, x, u, Cf, diff=True):
@@ -492,10 +519,28 @@ def _use_device_loop(mpc, x_init, cost, dx, u):
     either way, so there is no user option.  Taken for CUDA float32/float64 tensors of one dtype, a QuadCost, LinDx
     dynamics or a known system linearised by ANALYTIC / AUTO_DIFF, no slew-rate penalty, verbose <= 0, lqr_iter >= 1,
     T >= 2 and a shape the step kernels take (an exact or zero-padded instance, or the large-shape kernels for LinDx)."""
-    from .dynamics import DYN_LINEAR
+    return mpc.slew_rate_penalty is None and _device_loop_takes(mpc, x_init, cost, dx, u, slew=False)
+
+
+def _use_slew_device_loop(mpc, x_init, cost, dx, u):
+    """_use_device_loop for a solve with a slew-rate penalty: the same conditions on the augmented problem over
+    [u_{t-1}; x] (MPC._slew_augment).  LinDx runs it at the (n+m, m) instance _pick_instance gives (exact, padded or
+    large); a known system runs its passthrough kind's dynamics-only instance.  prev_ctrl must be absent or a tensor on
+    the solve's device."""
+    if mpc.slew_rate_penalty is None:
+        return False
+    prev = mpc.prev_ctrl
+    if prev is not None and (not isinstance(prev, torch.Tensor) or prev.device != x_init.device):
+        return False
+    return _device_loop_takes(mpc, x_init, cost, dx, u, slew=True)
+
+
+def _device_loop_takes(mpc, x_init, cost, dx, u, slew):
+    """The conditions the two device-loop predicates share; `slew`: on the augmented problem."""
+    from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR
     from .step import _pick_instance
     from ._lib import MpcB200Error
-    if _graph_cond_unavailable or mpc.slew_rate_penalty is not None or mpc.verbose > 0 or mpc.lqr_iter < 1:
+    if _graph_cond_unavailable or mpc.verbose > 0 or mpc.lqr_iter < 1:
         return False
     if not isinstance(cost, QuadCost) or mpc.T < 2:
         return False
@@ -503,6 +548,7 @@ def _use_device_loop(mpc, x_init, cost, dx, u):
     if dtype not in (torch.float32, torch.float64) or not x_init.is_cuda:
         return False
     n, m = mpc.n_state, mpc.n_ctrl
+    kind = DYN_LINEAR
     same = [cost.C, cost.c, u]
     if isinstance(dx, LinDx):
         if dx.F is None:
@@ -516,6 +562,7 @@ def _use_device_loop(mpc, x_init, cost, dx, u):
             return False
         if (n, m) != (dx.n_state, dx.n_ctrl):
             return False
+        kind = dx.mpcb200_kind | (DYN_CTRL_PASSTHROUGH if slew else 0)
         known = True
     else:
         return False
@@ -524,11 +571,12 @@ def _use_device_loop(mpc, x_init, cost, dx, u):
         return False
     if isinstance(mpc.u_zero_I, torch.Tensor) and mpc.u_zero_I.device != dev:
         return False
+    n_aug = n + m if slew else n
     try:
-        N, M = _pick_instance(n, m, x_init.element_size())
+        N, M = _pick_instance(n_aug, m, x_init.element_size(), kind)
     except MpcB200Error:
         return False
-    return not known or (N, M) == (n, m)
+    return not known or (N, M) == (n_aug, m)
 
 
 _seen_tables = []

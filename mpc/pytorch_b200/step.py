@@ -16,6 +16,7 @@ from torch.nn import Module
 
 from . import _lib
 from ._lib import Dims, Params, MpcB200Error, _on_device, check, ptr, ptr_view, stream_handle
+from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_DIMS, DYN_LINEAR
 
 PNQP_MAX_ITER = 20  # reference passes n_iter=20 (mpc/lqr_step.py:137)
 
@@ -40,14 +41,15 @@ def _dense(t, dtype=None):
     return t if t.is_contiguous() else t.contiguous()
 
 
-def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=None, exact=False, need_F=True):
+def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=None, dyn_kind=None, need_F=True):
     """Check, on tensor metadata alone, the tensors a raw call hands to the kernels; returns the batch size B.
     The kernels read raw device pointers: a wrong dtype, shape or device would be an out-of-bounds access, so fail
     here like the reference's indexing / eclamp size asserts would.  `named`: (name, tensor or None, layout), the
     layout one of "TBpp", "TBp", "TBn", "TBm", "Bn" (p = n+m).  The first tensor leads: the outputs are allocated in
     its dtype, and it fixes B and the device.  F [T-1|T,B,n,p] and f [T-1|T,B,n] may be absent or empty (F only for
-    T = 1); tensor bounds and u_zero_I are [T,B,m].  `exact`: the call runs in-kernel dynamics, which need an exact
-    (n, m) kernel instance.  `need_F=False`: the call linearises a known system itself and takes no F."""
+    T = 1); tensor bounds and u_zero_I are [T,B,m].  `dyn_kind`: the call runs that known system's dynamics in the
+    kernel, which needs the exact (n, m) instance _pick_instance gives that kind.  `need_F=False`: the call linearises
+    a known system itself and takes no F."""
     lead_name, lead, lead_layout = named[0]
     if lead.dtype not in (torch.float32, torch.float64):
         raise MpcB200Error(f"unsupported dtype {lead.dtype}")
@@ -77,7 +79,7 @@ def _validate(n, m, T, *named, F=None, f=None, bounds=(None, None), u_zero_I=Non
             if t.shape != shape_of["TBm"]:
                 raise MpcB200Error(f"{name}: expected shape {shape_of['TBm']}, got {tuple(t.shape)}")
             checked.append((name, t))
-    if exact and _pick_instance(n, m, lead.element_size()) != (n, m):
+    if dyn_kind is not None and _pick_instance(n, m, lead.element_size(), dyn_kind) != (n, m):
         raise MpcB200Error("in-kernel dynamics need an exact (n_state, n_ctrl) kernel instance")
     dev = lead.device
     for name, t in checked:
@@ -128,9 +130,14 @@ _pick_cache = {}
 _smem_fits_cache = {}
 
 
-def _pick_instance(n, m, elem_size=4):
+def _pick_instance(n, m, elem_size=4, kind=DYN_LINEAR):
     """The (N, M) kernel shape an (n, m) problem runs at: the smallest compiled instance that covers it (zero padded),
-    else (n, m) itself on the large-shape kernels if they fit it in `elem_size`-byte elements."""
+    else (n, m) itself on the large-shape kernels if they fit it in `elem_size`-byte elements.  A passthrough dynamics
+    `kind` runs its dynamics-only instance, which exists at exactly that kind's (n, m) only."""
+    if kind & DYN_CTRL_PASSTHROUGH:
+        if DYN_DIMS.get(kind) != (n, m):
+            raise MpcB200Error(f"dynamics kind {kind} has no kernel instance at (n_state={n}, n_ctrl={m})")
+        return n, m
     key = (n, m, elem_size)
     hit = _pick_cache.get(key)
     if hit is not None:
@@ -256,7 +263,7 @@ def _problem(n, m, T, B, dtype, dev, C=None, c=None, F=None, f=None, u_lower=Non
     and the Dims / Params of a step with a rollout, time strides included.  lqr_step_raw and ilqr_raw make the same
     call, so the iLQR graph hands each kernel what a host loop of raw calls hands it.  A call whose Dims differ sets
     those fields on the returned `dims`; the caller densifies and widens its x / u (_dense, _Pad.vec_n / vec_m)."""
-    N, M = _pick_instance(n, m, dtype.itemsize)
+    N, M = _pick_instance(n, m, dtype.itemsize, dyn[0] if dyn is not None else DYN_LINEAR)
     pad = _Pad(n, m, N, M, dev)
     (C_, tsC), (c_, tsc) = pad.stage(C, dtype, pad.mat_pp), pad.stage(c, dtype, pad.vec_p)
     (F_, tsF), (f_, tsf) = pad.stage(F, dtype, pad.mat_np), pad.stage(f, dtype, pad.vec_n)
@@ -305,7 +312,7 @@ def lqr_step_raw(n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u,
     n, m = n_state, n_ctrl
     B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("current_x", cur_x, "TBn"),
                   ("current_u", cur_u, "TBm"), F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
-                  exact=dyn is not None)
+                  dyn_kind=dyn[0] if dyn is not None else None)
     dtype, dev = C.dtype, C.device
     s = _problem(n, m, T, B, dtype, dev, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
                  max_linesearch_iter, dyn)
@@ -373,8 +380,8 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
     has no conditional graph nodes (nothing was launched then)."""
     n, m = n_state, n_ctrl
     B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
-                  F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I, exact=dyn is not None,
-                  need_F=dyn is None)
+                  F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
+                  dyn_kind=dyn[0] if dyn is not None else None, need_F=dyn is None)
     dtype, dev = C.dtype, C.device
     s = _problem(n, m, T, B, dtype, dev, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
                  max_linesearch_iter, dyn)
