@@ -1,0 +1,509 @@
+"""What the GPU test modules share: device plumbing, the two tolerance policies, case builders, the checks of a step
+against the oracle, the device probes of the kernels' switch horizons, and the runner that solves an MPC on the
+device loop or the host loop.
+
+Tolerance policies (DESIGN section 4):
+  * `within`: float64 within tol64 x scale of the float64 oracle; float32 within K32 = 4 times the error of the
+    oracle itself run in float32 on the same float32-rounded inputs (`round_through`), plus 1e-6 x scale;
+  * `tol_for`: the fixed SURVEY.md section 8c tolerances, for cases whose inputs are generated in their own dtype.
+
+Importing this module touches no device: the library is loaded when a function that needs it runs."""
+import contextlib
+import ctypes
+import functools
+import os
+from collections import namedtuple
+
+import numpy as np
+import torch
+
+from oracle import lqr_oracle as orc
+from tests.helpers import gen_problem, maxdiff, nominal_controls
+
+DEV = torch.device("cuda:0")
+F32, F64 = torch.float32, torch.float64
+DT = {F32: "f32", F64: "f64"}
+K32 = 4
+
+
+def _L():
+    from mpc.pytorch_b200 import _lib
+    return _lib
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# device plumbing
+# ------------------------------------------------------------------------------------------------------------------
+def to_dev(t, dtype=None):
+    """t on DEV, floating-point tensors cast to dtype when one is given; anything but a tensor is returned as is."""
+    if not torch.is_tensor(t):
+        return t
+    return t.to(DEV, dtype if dtype is not None and t.is_floating_point() else t.dtype)
+
+
+@contextlib.contextmanager
+def kernel_env(impl):
+    """MPCB200_KERNEL: None default dispatch, 1 generic, 2 column pair, 3 large-shape kernels."""
+    old = os.environ.pop("MPCB200_KERNEL", None)
+    if impl is not None:
+        os.environ["MPCB200_KERNEL"] = str(impl)
+    try:
+        yield
+    finally:
+        os.environ.pop("MPCB200_KERNEL", None)
+        if old is not None:
+            os.environ["MPCB200_KERNEL"] = old
+
+
+def run_step(n, m, T, P, kw=None, dtype=None, impl=None, want_gains=True, **opts):
+    """lqr_step_raw on the device for the problem P (x0, C, c, F, f, x, u), with the problem's options kw (bounds,
+    u_zero_I, delta_u, line search) and the call's opts (do_rollout, want_du_first, dyn); returns (outputs on the
+    CPU, step plan)."""
+    from mpc.pytorch_b200.step import lqr_step_raw
+    d = lambda t: to_dev(t, dtype)  # noqa: E731
+    with kernel_env(impl):
+        o = lqr_step_raw(n, m, T, *[d(P[k]) for k in ("x0", "C", "c", "F", "f", "x", "u")],
+                         want_gains=want_gains, **{k: d(v) for k, v in (kw or {}).items()}, **opts)
+        plan = _L().last_step_plan()
+    torch.cuda.synchronize()
+    return {k: v.cpu() for k, v in o.items() if v is not None}, plan
+
+
+def run_loop(n, m, T, P, kw, opts, dtype=None, impl=None):
+    """step.ilqr_raw on the device from P (x0, C, c, F, f, u0); returns (outputs on the CPU, the plan of the step
+    recorded in the loop body)."""
+    from mpc.pytorch_b200.step import ilqr_raw
+    d = lambda t: to_dev(t, dtype)  # noqa: E731
+    with kernel_env(impl):
+        res = ilqr_raw(n, m, T, *[d(P[k]) for k in ("x0", "C", "c", "F", "f", "u0")],
+                       **{k: d(v) for k, v in kw.items()}, **opts)
+        plan = _L().last_step_plan()
+    assert res is not None, "the driver has no conditional graph nodes"
+    torch.cuda.synchronize()
+    return {k: v.cpu() for k, v in res.items()}, plan
+
+
+def abi_adjoint(n, m, T, C, c, F, new_x, new_u, dl_dx, dl_du, lo=None, hi=None, with_f=True):
+    """mpcb200_lqr_adjoint_* through the C ABI on device tensors; lo, hi None, floats or tensors.  Returns
+    ([dx_init, dC, dc, dF, df or None] on the CPU, kernel launches)."""
+    L = _L()
+    dtype, B, p = C.dtype, C.shape[1], n + m
+    kind = 0 if lo is None else (1 if isinstance(lo, float) else 2)
+    dims = L.Dims(B=B, T=T, n=n, m=m, F_T=T - 1, has_f=int(with_f), bounds_kind=kind, max_ls_iter=10,
+                  pnqp_max_iter=20, do_rollout=1)
+    prm = L.Params(u_lo=lo if kind == 1 else 0.0, u_hi=hi if kind == 1 else 0.0, delta_u=0.0, ls_decay=0.2)
+    nbytes = L.lib().mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), C.element_size())
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
+    ins = [t.contiguous() for t in (C, c, F, new_x, new_u, dl_dx, dl_du)]         # alive until the sync
+    ins += [lo.contiguous() if kind == 2 else None, hi.contiguous() if kind == 2 else None]
+    out = [torch.empty(B, n, dtype=dtype, device=DEV), torch.empty(T, B, p, p, dtype=dtype, device=DEV),
+           torch.empty(T, B, p, dtype=dtype, device=DEV), torch.empty(T - 1, B, n, p, dtype=dtype, device=DEV),
+           torch.empty(T - 1, B, n, dtype=dtype, device=DEV) if with_f else None]
+    before = L.launch_count()
+    rc = L.entry("mpcb200_lqr_adjoint", dtype)(ctypes.byref(dims), ctypes.byref(prm), *[L.ptr(t) for t in ins + out],
+                                               L.ptr(ws), nbytes, L.stream_handle(DEV))
+    L.check(rc, "mpcb200_lqr_adjoint")
+    torch.cuda.synchronize()
+    return [t.cpu() if t is not None else None for t in out], L.launch_count() - before
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# tolerance policies
+# ------------------------------------------------------------------------------------------------------------------
+def round_through(t, dtype):
+    """float32 cases: every input is rounded to float32 once, so kernel and oracle see the same numbers."""
+    return t.to(dtype).double() if torch.is_tensor(t) and t.is_floating_point() and dtype == F32 else t
+
+
+def within(tag, what, got, w64, w32, dtype, tol64=1e-9, scale=None):
+    """float64: |got - w64| <= tol64 x scale; float32: <= K32 |w32 - w64| + 1e-6 x scale.  scale defaults to
+    max(1, |w64|)."""
+    if scale is None:
+        scale = max(1.0, float(w64.abs().max())) if w64.numel() else 1.0
+    err = maxdiff(got, w64)
+    bound = tol64 * scale if dtype == F64 else K32 * maxdiff(w32, w64) + 1e-6 * scale
+    assert err <= bound, f"{tag}: {what} |kernel - oracle| = {err:.3e} > {bound:.3e}"
+
+
+def tol_for(dtype, bounded):
+    """SURVEY.md section 8c: float64 1e-9 on x, u and costs; float32 4e-5 (unbounded) or 2e-4 (bounded: pnqp stops
+    at |dx| < 1e-4) on x, u and 3e-4 on costs."""
+    if dtype == F64:
+        return dict(xu=1e-9, cost=1e-9)
+    return dict(xu=2e-4 if bounded else 4e-5, cost=3e-4)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# case builders
+# ------------------------------------------------------------------------------------------------------------------
+@functools.lru_cache(maxsize=8)
+def linear_step_case(seed, B, T, n, m, dtype, mode, with_f=True, F_T=None):
+    """LinDx step inputs (float64, rounded through dtype) and the oracle's step: (P, kw, o64, o32|None).
+    mode: plain | mask (u_zero_I) | box (scalar bounds) | boxT (tensor bounds) | boxD (tensor bounds + delta_u).
+    F_T=T: F carries T time slices."""
+    C, c, F, f, x0 = gen_problem(seed, B, T, n, m, F64, with_f=with_f)
+    F = F * 0.9                         # trajectories stay O(1) over long horizons
+    if F_T == T:
+        F = torch.cat((F, F[-1:]), 0) if T > 1 else gen_problem(seed, B, 2, n, m, F64)[2] * 0.9
+    u, ul, uu = nominal_controls(seed, B, T, m, F64, {"box": 0.25, "boxT": "tensor", "boxD": "tensor"}.get(mode))
+    kw = {}
+    if mode.startswith("box"):
+        kw = dict(u_lower=round_through(ul, dtype), u_upper=round_through(uu, dtype))
+    if mode == "boxD":
+        kw["delta_u"] = 0.125
+    if mode == "mask":
+        kw["u_zero_I"] = torch.rand(T, B, m, generator=torch.Generator().manual_seed(seed)) < 0.3
+    C, c, F, f, x0, u = (round_through(t, dtype) for t in (C, c, F, f, x0, u))
+    x = round_through(orc.get_traj(T, u, x0, F, f), dtype)
+    P = dict(C=C, c=c, F=F, f=f, x0=x0, x=x, u=u)
+    return (P, kw) + oracle_steps(n, m, T, P, kw, dtype)
+
+
+def oracle_steps(n, m, T, P, kw, dtype, **opts):
+    """The oracle's step on P in float64 and, for float32 cases, in float32 (the yardstick): (o64, o32|None)."""
+    args = [P[k] for k in ("x0", "C", "c", "F", "f", "x", "u")]
+    o64 = orc.lqr_step_forward(n, m, T, *args, coupled=False, **kw, **opts)
+    if dtype != F32:
+        return o64, None
+    lo = lambda t: t.float() if torch.is_tensor(t) and t.is_floating_point() else t  # noqa: E731
+    return o64, orc.lqr_step_forward(n, m, T, *map(lo, args), coupled=False, **{k: lo(v) for k, v in kw.items()},
+                                     **opts)
+
+
+def rollout(module, x0, u):
+    """[T, B, n]: x0 rolled out through module under the controls u [T, B, m]."""
+    xs = [x0]
+    for t in range(u.shape[0] - 1):
+        xs.append(module(xs[t], u[t]))
+    return torch.stack(xs)
+
+
+def jacobians(module, xs, us):
+    """(next, R, S) of module(xs, us) by autograd."""
+    xs = xs.clone().requires_grad_(True)
+    us = us.clone().requires_grad_(True)
+    nx = module(xs, us)
+    rows = [torch.autograd.grad(nx[:, j].sum(), [xs, us], retain_graph=True) for j in range(nx.shape[1])]
+    return nx.detach(), torch.stack([r[0] for r in rows], 1), torch.stack([r[1] for r in rows], 1)
+
+
+def linearise(module, x, u):
+    """F = [R S] [T-1, B, n, n+m] and f = x' - R x - S u [T-1, B, n] of module at (x[:-1], u[:-1]), by autograd."""
+    T, B, n = x.shape
+    m = u.shape[2]
+    xs, us = x[:-1].reshape(-1, n), u[:-1].reshape(-1, m)
+    nx, R, S = jacobians(module, xs, us)
+    f = nx - torch.einsum("bij,bj->bi", R, xs) - torch.einsum("bij,bj->bi", S, us)
+    return torch.cat((R, S), 2).view(T - 1, B, n, n + m), f.view(T - 1, B, n)
+
+
+# known systems with non-default physics: parameters, dt, control clamp
+PHYS = {
+    "cartpole": dict(params=(9.81, 1.3, 0.25, 0.8), dt=0.1, clamp_attr="force_mag", clamp=7.5, n=5),
+    "pendulum": dict(params=(9.1, 1.7, 0.6), dt=0.15, clamp_attr="max_torque", clamp=1.5, n=3),
+}
+RADII = {"cartpole": (0.3, 1.0, 2.0), "pendulum": (0.3, 1.0, 3.0)}
+SYSTEMS = tuple(PHYS)
+BT = [(1, 1), (1, 200), (127, 11), (128, 2), (129, 11), (300, 200), (4097, 11), (4097, 2)]
+
+
+def known_module(name, params=None, device="cpu"):
+    from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
+    ph = PHYS[name]
+    p = torch.tensor(ph["params"], dtype=F64) if params is None else params
+    dx = (CartpoleDx if name == "cartpole" else PendulumDx)(params=p.to(device))
+    dx.dt = ph["dt"]
+    setattr(dx, ph["clamp_attr"], ph["clamp"])
+    return dx
+
+
+def angle_cols(name):
+    return (2, 3) if name == "cartpole" else (0, 1)
+
+
+def known_states(name, B, seed):
+    """float64 [B, n]: random states, angle pair at the RADII; the first rows hold the theta edge cases."""
+    g = torch.Generator().manual_seed(seed)
+    n = PHYS[name]["n"]
+    x = (torch.rand(B, n, generator=g, dtype=F64) - 0.5) * 2.0
+    th = (torch.rand(B, generator=g, dtype=F64) * 2 - 1) * 3.0
+    r0, _, r1 = RADII[name]
+    r = torch.tensor(RADII[name], dtype=F64).repeat(B)[:B]
+    ic, is_ = angle_cols(name)
+    x[:, ic], x[:, is_] = r * torch.cos(th), r * torch.sin(th)
+    edge = ((-1.0, 0.0), (-1.0, -0.0), (-r0, 0.0), (-r1, -0.0), (1.0, 1e-9), (1.0, -1e-9), (r1, 0.0))
+    for k, (cv, sv) in enumerate(edge[:B]):
+        x[k, ic], x[k, is_] = cv, sv
+    return x
+
+
+def _clamp_edges(clamp, dtype):
+    """u at the clamp, one ulp (of dtype) inside and outside it, both signs."""
+    npd = np.float64 if dtype == F64 else np.float32
+    c = npd(clamp)
+    inn, out = float(np.nextafter(c, npd(0))), float(np.nextafter(c, npd(np.inf)))
+    return (clamp, -clamp, inn, -inn, out, -out)
+
+
+def known_controls(name, T, B, dtype, seed):
+    """float64 [T, B, 1] in +-1.5 clamp; the edge values are spread over the first rows of every time step."""
+    g = torch.Generator().manual_seed(seed + 1)
+    clamp = PHYS[name]["clamp"]
+    u = (torch.rand(T, B, 1, generator=g, dtype=F64) * 2 - 1) * 1.5 * clamp
+    e = torch.tensor(_clamp_edges(clamp, dtype), dtype=F64)
+    k = min(B, len(e))
+    u[:, -k:, 0] = e[:k]                  # the last rows: the first rows hold the theta edges
+    return u
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# checks of one step against the oracle, over the problems `keep` (all by default)
+# ------------------------------------------------------------------------------------------------------------------
+def _cols(t, keep):
+    if t is None or keep is None:
+        return t
+    return t[:, keep] if t.dim() >= 2 else t[keep]
+
+
+def check_alphas(tag, r, o64, o32, keep=None):
+    """float64: alphas bit exact; float32: the float32 oracle's alphas wherever it makes the float64 oracle's
+    line-search decisions."""
+    got, w64 = _cols(r["alphas"], keep), _cols(o64.alphas, keep)
+    if o32 is None:
+        assert torch.equal(got, w64), f"{tag}: alphas {got} vs {w64}"
+    else:
+        w32 = _cols(o32.alphas, keep)
+        same = (w32.double() - w64).abs() <= 1e-6
+        assert torch.equal(got[same], w32[same]), f"{tag}: alphas"
+
+
+def check_trajectory(tag, r, u, o64, o32, dtype, keep=None):
+    """The outputs r holds, under `within`: new_x and new_u (on one scale), costs, Ks and ks; with du_first, the
+    first full step u - new_u and its per-problem norm full_du_norm (the line search takes the full step on these
+    problems).  A Riccati-only step holds the gains alone."""
+    g = lambda o, k: None if o is None else _cols(getattr(o, k), keep)  # noqa: E731
+    if "new_x" in r:
+        sc = max(1.0, float(g(o64, "new_x").abs().max()), float(g(o64, "new_u").abs().max()))
+        for k in ("new_x", "new_u"):
+            within(tag, k, _cols(r[k], keep), g(o64, k), g(o32, k), dtype, scale=sc)
+        within(tag, "costs", _cols(r["costs"], keep), g(o64, "costs"), g(o32, "costs"), dtype)
+    if "du_first" in r:
+        u = _cols(u, keep)
+        du = lambda o: None if o is None else u - g(o, "new_u")  # noqa: E731
+        norm = lambda d: None if d is None else d.pow(2).sum((0, 2)).sqrt()  # noqa: E731
+        within(tag, "du_first", _cols(r["du_first"], keep), du(o64), du(o32), dtype, scale=sc)
+        within(tag, "full_du_norm", _cols(r["full_du_norm"], keep), norm(du(o64)), norm(du(o32)), dtype, scale=sc)
+    if "Ks" in r:
+        within(tag, "Ks", _cols(r["Ks"], keep), g(o64, "Ks"), g(o32, "Ks"), dtype)
+        within(tag, "ks", _cols(r["ks"], keep), g(o64, "ks"), g(o32, "ks"), dtype)
+
+
+def check_pnqp(tag, r, o, kw, keep=None):
+    """pnqp against the oracle's o: no status bit but the cap flag, the cap flag only where the oracle's QP hits the
+    cap, free sets bit exact, with bounds the iteration counts, and masked controls exactly zero."""
+    assert int((r["status"] & ~1).max()) == 0, f"{tag}: status {r['status'].tolist()}"
+    assert torch.equal(_cols(r["free_mask"].bool(), keep), _cols(o.free_masks, keep)), f"{tag}: free sets"
+    bounded = kw.get("u_lower") is not None
+    if bounded:
+        capped = (o.qp_iters == 19).any(0)
+        flagged = _cols((r["status"] & 1).bool() & ~capped, keep)
+        assert not bool(flagged.any()), f"{tag}: pnqp flagged problems whose oracle QPs converged"
+        assert torch.equal(_cols(r["qp_iters"].long(), keep), _cols(o.qp_iters, keep)), f"{tag}: pnqp iterations"
+    if "new_u" in r and kw.get("u_zero_I") is not None:
+        assert bool((r["new_u"][kw["u_zero_I"]] == 0).all()), f"{tag}: masked controls"
+
+
+def check_clamps(tag, r, o, kw, keep=None):
+    """Bounded steps without delta_u: the controls on each bound bit exact."""
+    if "new_u" not in r or kw.get("u_lower") is None or kw.get("delta_u") is not None:
+        return
+    for side in ("u_lower", "u_upper"):
+        b = kw[side] if torch.is_tensor(kw[side]) else torch.full_like(o.new_u, kw[side])
+        assert torch.equal(_cols(r["new_u"].double() == b.double(), keep),
+                           _cols(o.new_u.double() == b.double(), keep)), f"{tag}: {side} clamp mask"
+
+
+def check_step_fixed(tag, r, o, kw, dtype):
+    """A step under the fixed tolerances of `tol_for` (on the scale of new_x), alphas bit exact.  float32 bounded
+    cases may flag one problem whose QP stopped at the cap because its |dx| < 1e-4 test is decided by round-off
+    (tests/test_step_gpu.py explains); that problem leaves the pnqp comparison."""
+    bounded = kw.get("u_lower") is not None
+    tol = tol_for(dtype, bounded)
+    scale = max(1.0, float(o.new_x.abs().max()))
+    for k in ("new_x", "new_u", "Ks", "ks"):
+        assert maxdiff(r[k], getattr(o, k)) <= tol["xu"] * scale, f"{tag}: {k}"
+    assert maxdiff(r["costs"], o.costs) <= tol["cost"] * max(1.0, float(o.costs.abs().max())), f"{tag}: costs"
+    assert maxdiff(r["alphas"], o.alphas) == 0.0, f"{tag}: alphas"
+    flagged = (r["status"] & 1) != 0
+    if dtype == F64 or not bounded:
+        assert not bool(flagged.any()), f"{tag}: pnqp flagged unconverged"
+    else:
+        assert int(flagged.sum()) <= 1 and bool((r["qp_iters"][:, flagged] == 19).any(0).all()), f"{tag}: cap flag"
+    check_pnqp(tag, r, o, kw, keep=~flagged)
+    check_clamps(tag, r, o, kw, keep=~flagged)
+    if bounded:
+        lo, hi = (kw[k] if torch.is_tensor(kw[k]) else torch.full_like(o.new_u, kw[k]) for k in ("u_lower", "u_upper"))
+        assert bool(((r["new_u"] >= lo) & (r["new_u"] <= hi)).all()), f"{tag}: controls outside the bounds"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the kernels' switch horizons, found on the device
+# ------------------------------------------------------------------------------------------------------------------
+INSTANCES = [(1, 1), (2, 1), (2, 2), (3, 1), (3, 2), (3, 4), (4, 1), (4, 2), (4, 4), (5, 1), (6, 2), (7, 4), (8, 1),
+             (8, 2), (8, 4), (12, 4), (16, 4)]
+PAIR_SHAPES = [s for s in INSTANCES if s[0] % 2 == 0 and s[1] % 2 == 0]
+KREDUCE_SHAPES = {(16, 4)}          # one problem per warp, n a power of two
+TMAX = 1024                         # switches are searched in [1, TMAX]
+ORACLE_TMAX = 900                   # oracle comparisons at switches up to this horizon
+PROBE_B = 8                         # one warp of every mapping; 16-byte aligned spans for every shape and dtype
+
+
+def plan_str(p):
+    L = _L()
+    if p == 0:
+        return "none"
+    s = "generic" if p & L.PLAN_GENERIC else "pair"
+    s += "/smem" if p & L.PLAN_GAINS_SMEM else "/Ks"
+    return s + ("+kreduce" if p & L.PLAN_KREDUCE else "")
+
+
+def plan(generic, smem, kreduce=False):
+    L = _L()
+    return ((L.PLAN_GENERIC if generic else L.PLAN_PAIR) | (L.PLAN_GAINS_SMEM if smem else 0)
+            | (L.PLAN_KREDUCE if kreduce else 0))
+
+
+@functools.lru_cache(maxsize=2)
+def _probe_inputs(n, m, dtype):
+    p = n + m
+    C = torch.eye(p, dtype=dtype, device=DEV).expand(TMAX, PROBE_B, p, p).contiguous()
+    c = torch.ones(TMAX, PROBE_B, p, dtype=dtype, device=DEV)
+    F = torch.cat((0.9 * torch.eye(n, dtype=dtype, device=DEV), torch.ones(n, m, dtype=dtype, device=DEV) / p), 1)
+    F = F.expand(TMAX, PROBE_B, n, p).contiguous()
+    x = torch.zeros(TMAX, PROBE_B, n, dtype=dtype, device=DEV)
+    u = torch.zeros(TMAX, PROBE_B, m, dtype=dtype, device=DEV)
+    return C, c, F, x, u
+
+
+def probe_step(n, m, dtype, T, impl, want_gains, do_rollout=True):
+    """Plan of one step launch at horizon T; 0 if the library refused it for lack of shared memory."""
+    from mpc.pytorch_b200.step import lqr_step_raw
+    C, c, F, x, u = _probe_inputs(n, m, dtype)
+    with kernel_env(impl):
+        try:
+            lqr_step_raw(n, m, T, x[0], C[:T], c[:T], F[:T - 1], None, x[:T], u[:T], do_rollout=do_rollout,
+                         want_gains=want_gains, want_stats=False)
+        except _L().MpcB200Error as e:
+            if "[4]" in str(e):
+                return 0
+            raise
+        return _L().last_step_plan()
+
+
+def probe_adjoint(n, m, dtype, T):
+    """Launches of one mpcb200_lqr_adjoint_* call at horizon T: 2 fused, 4 in-library 3-launch route, 0 if the
+    masked generic step does not fit shared memory either (callers then take the multi-call route)."""
+    C, c, F, x, u = _probe_inputs(n, m, dtype)
+    try:
+        _, launches = abi_adjoint(n, m, T, C[:T], c[:T], F[:T - 1], x[:T], u[:T], x[:T], u[:T], with_f=False)
+    except _L().MpcB200Error as e:
+        if "[4]" in str(e):
+            return 0
+        raise
+    return launches
+
+
+def first_true(pred, lo=0, hi=TMAX):
+    """Smallest T in (lo, hi] with pred(T), pred monotone and pred(lo) False; None if pred(hi) is False."""
+    if hi <= lo or not pred(hi):
+        return None
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        if pred(mid):
+            hi = mid
+        else:
+            lo = mid
+    return hi
+
+
+@functools.lru_cache(maxsize=None)
+def switches(n, m, dtype):
+    """First horizon of each non-default side (None: not below TMAX / not applicable to the shape).
+      generic          generic kernel with a Ks/ks buffer: gains leave shared memory
+      generic_riccati  generic kernel, Riccati sweep only: gains no longer fit shared memory
+      pair             pair kernel with a Ks/ks buffer: gains leave shared memory ("crowded" or not fitting)
+      pair_nofit       pair kernel, Riccati sweep only: gains no longer fit shared memory
+      adjoint          mpcb200_lqr_adjoint_*: fused kernel -> in-library 3-launch route"""
+    L = _L()
+    out = dict(
+        generic=first_true(lambda T: not probe_step(n, m, dtype, T, 1, True) & L.PLAN_GAINS_SMEM),
+        generic_riccati=first_true(lambda T: not probe_step(n, m, dtype, T, 1, True, False) & L.PLAN_GAINS_SMEM),
+        pair=None, pair_nofit=None, adjoint=None)
+    if (n, m) in PAIR_SHAPES:
+        out["pair"] = first_true(lambda T: not probe_step(n, m, dtype, T, 2, True) & L.PLAN_GAINS_SMEM)
+        out["pair_nofit"] = first_true(lambda T: not probe_step(n, m, dtype, T, 2, True, False) & L.PLAN_GAINS_SMEM)
+        out["adjoint"] = first_true(lambda T: probe_adjoint(n, m, dtype, T) != 2)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# MPC.forward on the device loop or on the host loop
+# ------------------------------------------------------------------------------------------------------------------
+Solve = namedtuple("Solve", "x u costs full_du_norm iters grads")
+
+
+def solve_on(monkeypatch, make, x0, cost, dx, device_loop, grads=()):
+    """make()(x0, cost, dx) on the device loop (asserting that its predicate, _use_device_loop or, for a slew-rate
+    penalty, _use_slew_device_loop, picks it) or on the host loop, asserting that the chosen loop ran.  The gradients
+    are those of x.sum() + u.sum() with respect to `grads`."""
+    from mpc.pytorch_b200 import solver, step
+    from mpc.pytorch_b200.solver import MPC
+    ctrl = make()
+    pred = "_use_device_loop" if ctrl.slew_rate_penalty is None else "_use_slew_device_loop"
+    seen = {"host_iters": 0}
+    with monkeypatch.context() as mp:
+        if device_loop:
+            u0 = torch.zeros(ctrl.T, x0.shape[0], ctrl.n_ctrl, dtype=x0.dtype, device=x0.device)
+            assert getattr(solver, pred)(ctrl, x0, cost, dx, u0)
+            real = step.ilqr_raw
+
+            def spy(*a, **k):
+                seen["res"] = real(*a, **k)
+                return seen["res"]
+            mp.setattr(step, "ilqr_raw", spy)
+        else:
+            mp.setattr(solver, pred, lambda *a: False)
+            real_sub = MPC.solve_lqr_subproblem
+
+            def count(self, *a, **k):
+                if not k.get("no_op_forward", False):
+                    seen["host_iters"] += 1
+                return real_sub(self, *a, **k)
+            mp.setattr(MPC, "solve_lqr_subproblem", count)
+        real_host = MPC._ilqr_host
+
+        def host(self, *a, **k):
+            seen["best"] = real_host(self, *a, **k)
+            return seen["best"]
+        mp.setattr(MPC, "_ilqr_host", host)
+        x, u, costs = make()(x0, cost, dx)
+    assert ("res" in seen) == device_loop and ("best" in seen) != device_loop
+    fdn = seen["res"]["full_du_norm"] if device_loop else seen["best"]["full_du_norm"]
+    iters = int(seen["res"]["info"][0]) if device_loop else seen["host_iters"]
+    gs = torch.autograd.grad(x.sum() + u.sum(), grads) if grads else ()
+    torch.cuda.synchronize()
+    return Solve(x, u, costs, fdn, iters, gs)
+
+
+def same_on_both_loops(monkeypatch, make, x0, cost, dx, grads=()):
+    """The host loop, then the device loop: x, u, costs, the iteration count and the gradients bit for bit.
+    Returns (device, host) solves."""
+    host = solve_on(monkeypatch, make, x0, cost, dx, False, grads)
+    dev = solve_on(monkeypatch, make, x0, cost, dx, True, grads)
+    for k, (a, b) in enumerate(zip(dev[:3], host[:3])):
+        assert a.shape == b.shape and a.dtype == b.dtype, f"output {k}"
+        assert torch.equal(a, b), f"output {k} {float((a - b).abs().max()):.3e}"
+    assert dev.iters == host.iters >= 1, (dev.iters, host.iters)
+    for k, (a, b) in enumerate(zip(dev.grads, host.grads)):
+        assert torch.equal(a, b), f"gradient {k} {float((a - b).abs().max()):.3e}"
+    return dev, host

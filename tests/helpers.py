@@ -1,4 +1,5 @@
-"""Shared test helpers: seeded problem generator (SURVEY.md section 8d) and fixture loading."""
+"""Shared test helpers that need no device: seeded problem generator (SURVEY.md section 8d), fixture loading, and
+references and edits that CPU and GPU tests both use."""
 import os
 
 import numpy as np
@@ -61,3 +62,71 @@ def maxdiff(a, b):
     a = torch.as_tensor(a)
     b = torch.as_tensor(b)
     return float((a.detach().cpu().double() - b.detach().cpu().double()).abs().max()) if a.numel() else 0.0
+
+
+def build_net(g, act):
+    """NNDynamics(3, 2) with the weights of a make_golden_nn fixture."""
+    from mpc.dynamics import NNDynamics
+    nl = int(g["n_layers"])
+    hidden = [g[f"W{i}"].shape[0] for i in range(nl - 1)]
+    net = NNDynamics(3, 2, hidden_sizes=hidden, activation=act).double()
+    with torch.no_grad():
+        for i, fc in enumerate(net.fcs):
+            fc.weight.copy_(g[f"W{i}"])
+            fc.bias.copy_(g[f"b{i}"])
+    return net
+
+
+def condensed_box_lqr_scipy(C, c, F, f, x0, lo, hi):
+    """Independent solution of one problem instance with scipy (stands in for cvxpy lqr_cp,
+    reference tests/test_mpc.py:35-62): minimise the rolled-out cost over u in the box."""
+    import numpy as np
+    from scipy.optimize import minimize
+    T, p = C.shape[0], C.shape[1]
+    n = x0.shape[0]
+    m = p - n
+    C, c, F, f, x0 = (a.numpy() for a in (C, c, F, f, x0))
+
+    def rollout(uflat):
+        u = uflat.reshape(T, m)
+        x = np.zeros((T, n))
+        x[0] = x0
+        for t in range(T - 1):
+            x[t + 1] = F[t] @ np.concatenate((x[t], u[t])) + f[t]
+        return x, u
+
+    def cost(uflat):
+        x, u = rollout(uflat)
+        tau = np.concatenate((x, u), 1)
+        return float(sum(0.5 * tau[t] @ C[t] @ tau[t] + c[t] @ tau[t] for t in range(T)))
+
+    res = minimize(cost, np.zeros(T * m), method="L-BFGS-B", bounds=[(lo, hi)] * (T * m),
+                   options=dict(maxiter=2000, ftol=1e-15, gtol=1e-10))
+    x, u = rollout(res.x)
+    return torch.from_numpy(x), torch.from_numpy(u)
+
+
+def _edit_routes():
+    """(label, edit(dx, new_values)) for every way a parameter tensor is commonly changed in place or replaced."""
+    def opt_step(dx, v):
+        opt = torch.optim.SGD([dx.params], lr=1.0)
+        opt.zero_grad()
+        dx.params.grad = (dx.params.detach() - v).clone()      # one SGD step lands exactly on v
+        opt.step()
+
+    def no_grad_copy(dx, v):
+        with torch.no_grad():
+            dx.params.copy_(v)
+
+    def data_item(dx, v):
+        for i in range(len(v)):
+            dx.params.data[i] = float(v[i])
+
+    def reassign(dx, v):
+        dx.params = v.clone().to(dx.params.device).requires_grad_(dx.params.requires_grad)
+
+    return [("optimizer step", opt_step), ("no_grad copy_", no_grad_copy), (".data[i] =", data_item),
+            ("reassign", reassign)]
+
+
+EDIT_ROUTES = _edit_routes()

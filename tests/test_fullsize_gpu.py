@@ -14,24 +14,10 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.helpers import gen_problem, load_golden, maxdiff, nominal_controls
+from tests.gpu_harness import DEV, run_step, to_dev
+from tests.helpers import gen_problem, load_golden, maxdiff
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
-
-
-def cu(t):
-    if t is None or isinstance(t, float):
-        return t
-    return t.to(DEV)
-
-
-def _run(n, m, T, x0, C, c, F, f, x, u, **kw):
-    from mpc.pytorch_b200.step import lqr_step_raw
-    o = lqr_step_raw(n, m, T, cu(x0), cu(C), cu(c), cu(F), cu(f), cu(x), cu(u), want_gains=False,
-                     **{k: cu(v) for k, v in kw.items()})
-    torch.cuda.synchronize()
-    return {k: v.cpu() for k, v in o.items() if torch.is_tensor(v)}
 
 
 def _check_all(r, o, u, ul, uu, tol, bounded):
@@ -73,7 +59,7 @@ def test_config3_all_problems_vs_oracle(bounds):
     x = orc.get_traj(T, u, x0, F, f)
     kw = {} if bounds is None else dict(u_lower=-bounds, u_upper=bounds)
     o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, x, u, coupled=False, **kw)
-    r = _run(n, m, T, x0, C, c, F, f, x, u, **kw)
+    r, _ = run_step(n, m, T, dict(x0=x0, C=C, c=c, F=F, f=f, x=x, u=u), kw, want_gains=False)
     _check_all(r, o, u, kw.get("u_lower"), kw.get("u_upper"), 2e-4 if bounds else 4e-5, bounds is not None)
     if bounds is not None:
         assert 0.5 < float((r["new_u"].abs() == bounds).float().mean()) < 0.95
@@ -92,7 +78,8 @@ def test_config4_all_problems_vs_oracle(kind):
         u = torch.zeros(T, B, m)
     x = orc.get_traj(T, u, x0, F, f)
     o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, x, u, u_lower=ul, u_upper=uu, coupled=False)
-    r = _run(n, m, T, x0, C, c, F, f, x, u, u_lower=ul, u_upper=uu)
+    r, _ = run_step(n, m, T, dict(x0=x0, C=C, c=c, F=F, f=f, x=x, u=u), dict(u_lower=ul, u_upper=uu),
+                    want_gains=False)
     _check_all(r, o, u, ul, uu, 2e-4, True)
 
 
@@ -100,7 +87,7 @@ def test_config5_shard_properties_and_sampled_oracle():
     """B=4096 is the per-GPU shard of BASELINE config 5 at 8 GPUs (32768 / 8)."""
     from mpc.pytorch_b200.step import lqr_step_raw
     B, T, n, m = 4096, 50, 16, 4
-    C, c, F, f, x0 = [cu(t) for t in gen_problem(5000, B, T, n, m, torch.float32)]
+    C, c, F, f, x0 = [to_dev(t) for t in gen_problem(5000, B, T, n, m, torch.float32)]
     u = torch.zeros(T, B, m, device=DEV)
     from mpc.pytorch_b200.solver import get_traj, LinDx
     x = get_traj(T, u, x0, LinDx(F, f))

@@ -5,56 +5,14 @@ solve makes no host read, so torch.cuda.graph captures it and its replays equal 
 import pytest
 import torch
 
-from mpc.pytorch_b200 import solver, step
+from mpc.pytorch_b200 import solver
 from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
 from mpc.pytorch_b200.solver import MPC, GradMethods, LinDx, QuadCost
 from tests.cartpole import initial_states
+from tests.gpu_harness import DEV, same_on_both_loops, solve_on
 from tests.helpers import gen_problem
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
-
-
-def _solve(monkeypatch, make, x0, cost, dx, device_loop):
-    """(x, u, costs, iterations) of make()(x0, cost, dx) on the device loop or on the host loop."""
-    seen = {"host_iters": 0, "info": None}
-    with monkeypatch.context() as mp:
-        if device_loop:
-            assert solver._use_device_loop(make(), x0, cost, dx, _u0(make(), x0))
-            real = step.ilqr_raw
-
-            def spy(*a, **k):
-                res = real(*a, **k)
-                seen["info"] = res["info"]
-                return res
-            mp.setattr(step, "ilqr_raw", spy)
-        else:
-            mp.setattr(solver, "_use_device_loop", lambda *a: False)
-            real = MPC.solve_lqr_subproblem
-
-            def count(self, *a, **k):
-                if not k.get("no_op_forward", False):
-                    seen["host_iters"] += 1
-                return real(self, *a, **k)
-            mp.setattr(MPC, "solve_lqr_subproblem", count)
-        x, u, costs = make()(x0, cost, dx)
-    torch.cuda.synchronize()
-    iters = int(seen["info"][0]) if device_loop else seen["host_iters"]
-    return x, u, costs, iters
-
-
-def _u0(ctrl, x0):
-    return torch.zeros(ctrl.T, x0.shape[0], ctrl.n_ctrl, dtype=x0.dtype, device=x0.device)
-
-
-def _same(monkeypatch, make, x0, cost, dx, min_iters=1):
-    hx, hu, hc, hi = _solve(monkeypatch, make, x0, cost, dx, False)
-    dxx, du, dc, di = _solve(monkeypatch, make, x0, cost, dx, True)
-    assert di == hi and hi >= min_iters
-    for a, b in ((hx, dxx), (hu, du), (hc, dc)):
-        assert a.shape == b.shape and a.dtype == b.dtype
-        assert torch.equal(a, b), float((a - b).abs().max())
-    return hi
 
 
 def _linear(B, T, n, m, dtype, seed=0):
@@ -85,7 +43,7 @@ def test_linear_8_2(monkeypatch, dtype, case):
         kw.update(u_init=(0.1 * torch.randn(T, m, generator=g, dtype=dtype)).to(DEV))
     if case == "u_init_3d":
         kw.update(u_init=(0.1 * torch.randn(T, B, m, generator=g, dtype=dtype)).to(DEV))
-    _same(monkeypatch, lambda: MPC(n, m, T, **kw), x0, QuadCost(C, c), LinDx(F, f))
+    same_on_both_loops(monkeypatch, lambda: MPC(n, m, T, **kw), x0, QuadCost(C, c), LinDx(F, f))
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
@@ -94,7 +52,7 @@ def test_linear_padded_and_large(monkeypatch, dtype, n, m):
     B, T = 32, 10
     C, c, F, f, x0 = _linear(B, T, n, m, dtype, seed=3)
     for bounds in ({}, dict(u_lower=-0.3, u_upper=0.3)):
-        _same(monkeypatch, lambda: MPC(n, m, T, lqr_iter=8, verbose=-1, exit_unconverged=False,
+        same_on_both_loops(monkeypatch, lambda: MPC(n, m, T, lqr_iter=8, verbose=-1, exit_unconverged=False,
                                        detach_unconverged=False, **bounds), x0, QuadCost(C, c), LinDx(F, f))
 
 
@@ -103,8 +61,8 @@ def test_linear_time_invariant_inputs(monkeypatch):
     C, c, F, f, x0 = _linear(B, T, n, m, torch.float32, seed=5)
     C2, c1 = C[0, 0], c[0, 0]                                   # expanded over time and batch by MPC
     F_lti = F[0].unsqueeze(0).expand(T - 1, B, n, n + m)         # stride 0 over time
-    _same(monkeypatch, lambda: MPC(n, m, T, u_lower=-0.2, u_upper=0.2, lqr_iter=6, verbose=-1, n_batch=B,
-                                   exit_unconverged=False, detach_unconverged=False),
+    same_on_both_loops(monkeypatch, lambda: MPC(n, m, T, u_lower=-0.2, u_upper=0.2, lqr_iter=6, verbose=-1,
+                                                n_batch=B, exit_unconverged=False, detach_unconverged=False),
           x0, QuadCost(C2, c1), LinDx(F_lti, None))
 
 
@@ -112,8 +70,9 @@ def test_linear_time_invariant_inputs(monkeypatch):
 def test_linear_batch_sizes(monkeypatch, B):
     T, n, m = 9, 8, 2
     C, c, F, f, x0 = _linear(B, T, n, m, torch.float32, seed=B)
-    _same(monkeypatch, lambda: MPC(n, m, T, u_lower=-0.25, u_upper=0.25, lqr_iter=10, verbose=-1,
-                                   exit_unconverged=False, detach_unconverged=False), x0, QuadCost(C, c), LinDx(F, f))
+    same_on_both_loops(monkeypatch, lambda: MPC(n, m, T, u_lower=-0.25, u_upper=0.25, lqr_iter=10, verbose=-1,
+                                                exit_unconverged=False, detach_unconverged=False),
+                       x0, QuadCost(C, c), LinDx(F, f))
 
 
 def test_stop_reasons(monkeypatch):
@@ -121,16 +80,17 @@ def test_stop_reasons(monkeypatch):
     C, c, F, f, x0 = _linear(B, T, n, m, torch.float64, seed=7)
     cost, dx = QuadCost(C, c), LinDx(F, f)
     base = dict(u_lower=-0.25, u_upper=0.25, verbose=-1, exit_unconverged=False, detach_unconverged=False)
+
+    def iters(**o):
+        return same_on_both_loops(monkeypatch, lambda: MPC(n, m, T, **base, **o), x0, cost, dx)[0].iters
+
     # by eps: a loose tolerance ends the loop before lqr_iter
-    it = _same(monkeypatch, lambda: MPC(n, m, T, lqr_iter=30, eps=1e-3, **base), x0, cost, dx)
-    assert it < 30
+    assert iters(lqr_iter=30, eps=1e-3) < 30
     # by not_improved_lim: no iteration ever counts as an improvement
-    it = _same(monkeypatch, lambda: MPC(n, m, T, lqr_iter=30, eps=0.0, best_cost_eps=-1e9, not_improved_lim=2,
-                                        **base), x0, cost, dx)
-    assert it == 3
+    assert iters(lqr_iter=30, eps=0.0, best_cost_eps=-1e9, not_improved_lim=2) == 3
     # at lqr_iter
-    assert _same(monkeypatch, lambda: MPC(n, m, T, lqr_iter=4, eps=0.0, **base), x0, cost, dx) == 4
-    assert _same(monkeypatch, lambda: MPC(n, m, T, lqr_iter=1, **base), x0, cost, dx) == 1
+    assert iters(lqr_iter=4, eps=0.0) == 4
+    assert iters(lqr_iter=1) == 1
 
 
 def _system_problem(sysdx, B, T, dtype):
@@ -159,7 +119,7 @@ def test_known_systems(monkeypatch, dtype, system):
     sysdx = CartpoleDx() if system == "cartpole" else PendulumDx()
     B, T = 32, 15
     x0, cost = _system_problem(sysdx, B, T, dtype)
-    _same(monkeypatch, _system_mpc(sysdx, T, 20), x0, cost, sysdx, min_iters=2)
+    assert same_on_both_loops(monkeypatch, _system_mpc(sysdx, T, 20), x0, cost, sysdx)[0].iters >= 2
 
 
 def test_config2_cartpole_full_size(monkeypatch):
@@ -170,7 +130,7 @@ def test_config2_cartpole_full_size(monkeypatch):
     make = lambda: MPC(5, 1, T, u_lower=sysdx.lower, u_upper=sysdx.upper, lqr_iter=50, verbose=-1,  # noqa: E731
                        exit_unconverged=False, detach_unconverged=False, linesearch_decay=sysdx.linesearch_decay,
                        max_linesearch_iter=sysdx.max_linesearch_iter, grad_method=GradMethods.AUTO_DIFF, eps=1e-2)
-    _same(monkeypatch, make, x0, cost, sysdx, min_iters=2)
+    assert same_on_both_loops(monkeypatch, make, x0, cost, sysdx)[0].iters >= 2
 
 
 def test_pnqp_warnings_match(monkeypatch, capsys):
@@ -178,18 +138,18 @@ def test_pnqp_warnings_match(monkeypatch, capsys):
     B, T = 64, 20
     x0, cost = _system_problem(sysdx, B, T, torch.float32)
     make = _system_mpc(sysdx, T, 30, verbose=0)
-    _solve(monkeypatch, make, x0, cost, sysdx, False)
+    solve_on(monkeypatch, make, x0, cost, sysdx, False)
     host_out = capsys.readouterr().out
-    _solve(monkeypatch, make, x0, cost, sysdx, True)
+    solve_on(monkeypatch, make, x0, cost, sysdx, True)
     dev_out = capsys.readouterr().out
     assert dev_out == host_out
     # and on a bounded LinDx problem whose QPs get the default 20 pnqp iterations
     C, c, F, f, x0 = _linear(64, 12, 8, 2, torch.float32, seed=11)
     make = lambda: MPC(8, 2, 12, u_lower=-0.05, u_upper=0.05, lqr_iter=10, verbose=0,  # noqa: E731
                        exit_unconverged=False, detach_unconverged=False)
-    _solve(monkeypatch, make, x0, QuadCost(C, c), LinDx(F, f), False)
+    solve_on(monkeypatch, make, x0, QuadCost(C, c), LinDx(F, f), False)
     host_out = capsys.readouterr().out
-    _solve(monkeypatch, make, x0, QuadCost(C, c), LinDx(F, f), True)
+    solve_on(monkeypatch, make, x0, QuadCost(C, c), LinDx(F, f), True)
     assert capsys.readouterr().out == host_out
 
 
@@ -236,7 +196,8 @@ def test_cuda_graph_capture_linear():
     C, c, F, f, x0 = _linear(B, T, n, m, torch.float32, seed=17)
     ctrl = MPC(n, m, T, u_lower=-0.25, u_upper=0.25, lqr_iter=10, verbose=-1, exit_unconverged=False,
                detach_unconverged=False)
-    assert solver._use_device_loop(ctrl, x0, QuadCost(C, c), LinDx(F, f), _u0(ctrl, x0))
+    u0 = torch.zeros(T, B, m, device=DEV)
+    assert solver._use_device_loop(ctrl, x0, QuadCost(C, c), LinDx(F, f), u0)
     _capture_matches_eager(ctrl, QuadCost(C, c), LinDx(F, f), [x0, 0.5 * x0, x0.flip(0)])
 
 

@@ -29,13 +29,12 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
+from tests.gpu_harness import (DEV, DT, F32, F64, INSTANCES, KREDUCE_SHAPES, ORACLE_TMAX, PAIR_SHAPES,
+                               plan as _plan, plan_str as _plan_str, probe_step, round_through, run_loop,
+                               same_on_both_loops, switches, within)
 from tests.helpers import gen_problem, maxdiff
-from tests.test_horizon_paths_gpu import (DT, INSTANCES, KREDUCE_SHAPES, ORACLE_TMAX, PAIR_SHAPES, _kernel, _plan,
-                                          _plan_str, _probe_step, switches)
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
-F32, F64 = torch.float32, torch.float64
 EPS = {F64: 1e-7, F32: 1e-4}        # the stop tolerance of each dtype's cases (MPC's default in float64)
 FDN_ERR = {}                        # (dtype, what) -> observed |full_du_norm - oracle| (or device - host), per run
 LOOP_SEEN = {}                      # dtype -> step plans run inside the loop
@@ -50,11 +49,6 @@ def _L():
 # ------------------------------------------------------------------------------------------------------------------
 # problems, the oracle's loop, the device loop
 # ------------------------------------------------------------------------------------------------------------------
-def _round(t, dtype):
-    """float32 cases: every input is rounded to float32 once, so kernel and oracle see the same numbers."""
-    return t.to(dtype).double() if torch.is_tensor(t) and t.is_floating_point() and dtype == F32 else t
-
-
 def _f32(t):
     return t.float() if torch.is_tensor(t) and t.is_floating_point() else t
 
@@ -84,9 +78,9 @@ def loop_case(seed, B, T, n, m, dtype, mode, lqr_iter, eps, not_improved_lim=5, 
         kw["delta_u"] = 0.125
     if mode in ("mask", "maskT"):
         kw["u_zero_I"] = torch.rand(T, B, m, generator=g) < 0.3
-    P = {k: _round(v, dtype) for k, v in dict(C=C, c=c, F=F, f=f, x0=x0).items()}
+    P = {k: round_through(v, dtype) for k, v in dict(C=C, c=c, F=F, f=f, x0=x0).items()}
     P["u0"] = torch.zeros(T, B, m, dtype=F64)
-    kw = {k: _round(v, dtype) for k, v in kw.items()}
+    kw = {k: round_through(v, dtype) for k, v in kw.items()}
     opts = dict(lqr_iter=lqr_iter, eps=eps, not_improved_lim=not_improved_lim, best_cost_eps=best_cost_eps)
     o64 = _oracle(n, m, T, P, kw, opts)
     o32 = None
@@ -95,29 +89,9 @@ def loop_case(seed, B, T, n, m, dtype, mode, lqr_iter, eps, not_improved_lim=5, 
     return P, kw, opts, o64, o32
 
 
-def run_loop(n, m, T, case, dtype, impl=None):
-    """step.ilqr_raw on the device; returns (outputs on the CPU, the plan of the step recorded in the loop body)."""
-    from mpc.pytorch_b200.step import ilqr_raw
-    P, kw, opts = case[:3]
-    d = lambda t: t.to(DEV, dtype if t.is_floating_point() else t.dtype) if torch.is_tensor(t) else t  # noqa: E731
-    with _kernel(impl):
-        res = ilqr_raw(n, m, T, d(P["x0"]), d(P["C"]), d(P["c"]), d(P["F"]), d(P["f"]), d(P["u0"]),
-                       **{k: d(v) for k, v in kw.items()}, **opts)
-        plan = _L().last_step_plan()
-    assert res is not None, "the driver has no conditional graph nodes"
-    torch.cuda.synchronize()
-    return {k: v.cpu() for k, v in res.items()}, plan
-
-
 # ------------------------------------------------------------------------------------------------------------------
 # comparisons
 # ------------------------------------------------------------------------------------------------------------------
-def _close(tag, what, got, w64, w32, dtype, scale):
-    err = maxdiff(got, w64)
-    bound = 1e-9 * scale if dtype == F64 else 4 * maxdiff(w32, w64) + 1e-6 * scale
-    assert err <= bound, f"{tag}: {what} |kernel - oracle| = {err:.3e} > {bound:.3e}"
-
-
 def _on_bounds(u, kw):
     """[2, T, B, m]: which controls sit on the lower / upper bound."""
     lo, hi = (kw[k] if torch.is_tensor(kw[k]) else torch.full_like(u, kw[k]) for k in ("u_lower", "u_upper"))
@@ -195,8 +169,7 @@ def check_loop(tag, r, case, dtype):
     keep = ~(out | dep)
     assert bool(keep.any()), f"{tag}: no comparable problem"
     sel = lambda o, k: None if o is None else (o[k][:, keep] if o[k].dim() == 3 else o[k][keep])  # noqa: E731
-    _close(tag, "costs", sel(r, "costs"), sel(o64, "costs"), sel(o32, "costs"), dtype,
-           max(1.0, float(sel(o64, "costs").abs().max())))
+    within(tag, "costs", sel(r, "costs"), sel(o64, "costs"), sel(o32, "costs"), dtype)
     rows = ~rows_holding(out | dep, T, m)
     if bool(rows.any()):
         g = lambda o: None if o is None else o["fdn"][rows]  # noqa: E731
@@ -214,7 +187,7 @@ def check_loop(tag, r, case, dtype):
 @functools.lru_cache(maxsize=None)
 def _pair_default(n, m, dtype):
     """Whether the default dispatch runs the column-pair kernel at this instance (asked of the device)."""
-    return bool(_probe_step(n, m, dtype, 2, None, False) & _L().PLAN_PAIR)
+    return bool(probe_step(n, m, dtype, 2, None, False) & _L().PLAN_PAIR)
 
 
 def loop_plan(n, m, dtype, T, impl):
@@ -305,7 +278,7 @@ def test_loop_plans_at_switch(group, dtype):
             if want is None:
                 continue
             tag = f"{group} n{n}m{m} {DT[dtype]} T={T} (T*={Ts}) {mode} MPCB200_KERNEL={impl}"
-            r, plan = run_loop(n, m, T, case, dtype, impl)
+            r, plan = run_loop(n, m, T, *case[:3], dtype, impl)
             assert plan == want, f"{tag}: plan {_plan_str(plan)}, expected {_plan_str(want)}"
             LOOP_SEEN.setdefault(dtype, set()).add(_plan_name(plan, impl, n, m, dtype))
             check_loop(tag, r, case, dtype)
@@ -320,7 +293,7 @@ def test_loop_large_shape_kernels(n, m, impl, mode, dtype):
     """The large-shape kernels inside the loop: a shape without an instance, and MPCB200_KERNEL=3 at instances."""
     T = 10
     case = loop_case(1200 + n + m, 8, T, n, m, dtype, mode, 3, EPS[dtype])
-    r, plan = run_loop(n, m, T, case, dtype, impl)
+    r, plan = run_loop(n, m, T, *case[:3], dtype, impl)
     assert plan == _L().PLAN_LARGE, _plan_str(plan)
     LOOP_SEEN.setdefault(dtype, set()).add("large")
     check_loop(f"large n{n}m{m} {DT[dtype]} {mode} MPCB200_KERNEL={impl}", r, case, dtype)
@@ -338,7 +311,7 @@ FULL = [("config3", 8, 2, 4096, 20, "plain", 4), ("config3_box", 8, 2, 4096, 20,
 def test_full_size_loop_vs_oracle(name, n, m, B, T, mode, lqr_iter):
     case = loop_case(3100 + FULL.index((name, n, m, B, T, mode, lqr_iter)), B, T, n, m, F32, mode, lqr_iter,
                      EPS[F32])
-    r, plan = run_loop(n, m, T, case, F32)
+    r, plan = run_loop(n, m, T, *case[:3], F32)
     tag = f"{name} B={B} T={T} {mode} plan {_plan_str(plan)}"
     print(tag, "iterations", int(r["info"][0]), "track-kernel passes", math.ceil(T * B * max(n, m) / (4096 * 256)))
     check_loop(tag, r, case, F32)
@@ -349,7 +322,7 @@ def test_full_size_config5_shard_runs_kreduce():
     n, m, B, T = 16, 4, 4096, 50
     assert T * B * max(n, m) > 4096 * 256
     case = loop_case(3103, B, T, n, m, F32, "box", 3, EPS[F32])
-    r, plan = run_loop(n, m, T, case, F32, impl=1)
+    r, plan = run_loop(n, m, T, *case[:3], F32, impl=1)
     assert plan == _plan(True, False, True), _plan_str(plan)
     LOOP_SEEN.setdefault(F32, set()).add("generic_kreduce")
     check_loop(f"config5 shard generic kernel B={B}", r, case, F32)
@@ -360,11 +333,11 @@ def test_device_loop_matches_host_loop_at_65536(monkeypatch):
     ten times.  The host loop keeps the best iterate with torch.where and reduces with torch: bitwise equal x, u,
     costs and iteration count, and full_du_norm equal up to its summation order."""
     from mpc.pytorch_b200.solver import MPC, LinDx, QuadCost
-    from tests.test_ilqr_graph_gpu import _same
     B, T, n, m = 65536, 20, 8, 2
     C, c, F, f, x0 = [t.to(DEV) for t in gen_problem(3200, B, T, n, m, F32)]
     kw = dict(u_lower=-0.25, u_upper=0.25, lqr_iter=5, verbose=-1, exit_unconverged=False, detach_unconverged=False)
-    assert _same(monkeypatch, lambda: MPC(n, m, T, **kw), x0, QuadCost(C, c), LinDx(F, f)) >= 2
+    dev, _ = same_on_both_loops(monkeypatch, lambda: MPC(n, m, T, **kw), x0, QuadCost(C, c), LinDx(F, f))
+    assert dev.iters >= 2
     ctrl = MPC(n, m, T, **kw)
     u0 = torch.zeros(T, B, m, device=DEV)
     host = ctrl._ilqr_host(x0, QuadCost(C, c), LinDx(F, f), u0)
@@ -398,7 +371,7 @@ def test_stop_by_eps():
     assert eps is not None, mx
     case = loop_case(3300, STOP_B, STOP_T, n, m, F64, "box", lqr_iter, eps)
     assert case[3]["iters"] == stop, (case[3]["iters"], stop, mx)
-    r, _ = run_loop(n, m, STOP_T, case, F64)
+    r, _ = run_loop(n, m, STOP_T, *case[:3], F64)
     check_loop(f"eps stop B={STOP_B} eps={eps:.2e}", r, case, F64)
 
 
@@ -408,7 +381,7 @@ def test_stop_by_not_improved_lim():
     n, m = 8, 2
     case = loop_case(3301, STOP_B, STOP_T, n, m, F64, "tensor", 10, 0.0, not_improved_lim=2, best_cost_eps=-1e9)
     assert case[3]["iters"] == 3
-    r, _ = run_loop(n, m, STOP_T, case, F64)
+    r, _ = run_loop(n, m, STOP_T, *case[:3], F64)
     check_loop(f"not_improved_lim stop B={STOP_B}", r, case, F64)
     first = loop_case(3301, STOP_B, STOP_T, n, m, F64, "tensor", 1, 0.0)[3]
     assert torch.equal(case[3]["fdn"], first["fdn"])          # the oracle's best iterate is its first one
@@ -418,7 +391,7 @@ def test_stop_at_lqr_iter():
     n, m = 8, 2
     case = loop_case(3302, STOP_B, STOP_T, n, m, F64, "boxT", 4, 0.0, not_improved_lim=4)
     assert case[3]["iters"] == 4
-    r, _ = run_loop(n, m, STOP_T, case, F64)
+    r, _ = run_loop(n, m, STOP_T, *case[:3], F64)
     check_loop(f"lqr_iter cap B={STOP_B}", r, case, F64)
 
 
@@ -463,11 +436,8 @@ def test_full_du_norm_decides_exit_and_detach(monkeypatch):
     assert 0 < int(keep.sum()) < B
 
     # the device loop's full_du_norm: the oracle's, and the host loop's up to summation order
-    from mpc.pytorch_b200.step import ilqr_raw
     d = [t.to(DEV) for t in (C, c, F, f, x0)]
-    r = ilqr_raw(n, m, T, d[4], d[0], d[1], d[2], d[3], P["u0"].to(DEV), lqr_iter=10, eps=eps, **box)
-    torch.cuda.synchronize()
-    rc = {k: v.cpu() for k, v in r.items()}
+    rc, _ = run_loop(n, m, T, P, box, dict(lqr_iter=10, eps=eps))
     check_loop(f"detach case eps={eps:.2e}", rc, (P, box, dict(lqr_iter=10, eps=eps), o, None), F64)
     # the keep / detach decision of every problem whose norm row holds no departing problem is the oracle's
     err = torch.maximum(_err_per_problem(rc["x"], o["x"]), _err_per_problem(rc["u"], o["u"]))
@@ -477,8 +447,8 @@ def test_full_du_norm_decides_exit_and_detach(monkeypatch):
     assert 0 < int(keep.sum()) < B
     ctrl = MPC(n, m, T, lqr_iter=10, eps=eps, **box)
     host = ctrl._ilqr_host(d[4], QuadCost(d[0], d[1]), LinDx(d[2], d[3]), P["u0"].to(DEV))
-    a, b = r["full_du_norm"], host["full_du_norm"]
-    assert torch.equal(r["x"], host["x"]) and torch.equal(r["u"], host["u"])
+    a, b = rc["full_du_norm"], host["full_du_norm"].cpu()
+    assert torch.equal(rc["x"], host["x"].cpu()) and torch.equal(rc["u"], host["u"].cpu())
     assert float(((a - b).abs() / b.abs().clamp_min(1e-300)).max()) <= 1e-12     # summation order only
 
     # exit_unconverged (default True): asserts with this eps, not with one above every problem's norm
@@ -518,7 +488,7 @@ MASK_CASES = [(8, 2, "mask", 5, 1, -1e9), (8, 2, "maskT", 4, 5, 1e-4), (3, 3, "m
 def test_masked_controls_vs_oracle(n, m, mode, lqr_iter, nil, bce, dtype):
     B, T = 16, 10
     case = loop_case(3400 + 10 * n + m, B, T, n, m, dtype, mode, lqr_iter, EPS[dtype], nil, bce)
-    r, _ = run_loop(n, m, T, case, dtype)
+    r, _ = run_loop(n, m, T, *case[:3], dtype)
     check_loop(f"n{n}m{m} {mode} {DT[dtype]}", r, case, dtype)
 
 

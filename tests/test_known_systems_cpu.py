@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.helpers import load_golden, maxdiff
+from tests.helpers import EDIT_ROUTES, load_golden, maxdiff
 
 SYSTEMS = ("cartpole", "pendulum")
 
@@ -78,32 +78,6 @@ def test_oracle_nonlinear_rollout_matches_reference(name, bounds):
 # ----------------------------------------------------------------------------------------------------------------
 # parameters the kernels see: what forward would use at that moment
 # ----------------------------------------------------------------------------------------------------------------
-def _edit_routes():
-    """(label, edit(dx, new_values)) for every way a parameter tensor is commonly changed in place or replaced."""
-    def opt_step(dx, v):
-        opt = torch.optim.SGD([dx.params], lr=1.0)
-        opt.zero_grad()
-        dx.params.grad = (dx.params.detach() - v).clone()      # one SGD step lands exactly on v
-        opt.step()
-
-    def no_grad_copy(dx, v):
-        with torch.no_grad():
-            dx.params.copy_(v)
-
-    def data_item(dx, v):
-        for i in range(len(v)):
-            dx.params.data[i] = float(v[i])
-
-    def reassign(dx, v):
-        dx.params = v.clone().to(dx.params.device).requires_grad_(dx.params.requires_grad)
-
-    return [("optimizer step", opt_step), ("no_grad copy_", no_grad_copy), (".data[i] =", data_item),
-            ("reassign", reassign)]
-
-
-EDIT_ROUTES = _edit_routes()
-
-
 @pytest.mark.parametrize("route", [r[0] for r in EDIT_ROUTES])
 @pytest.mark.parametrize("name", SYSTEMS)
 def test_kernel_parameters_follow_in_place_edits(name, route):

@@ -20,92 +20,16 @@ copied by the producer warp's lanes."""
 import functools
 import math
 
-import numpy as np
 import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.helpers import maxdiff
+from tests.gpu_harness import (BT, DEV, DT, F32, F64, PHYS, SYSTEMS, angle_cols, check_alphas, check_clamps, check_pnqp,
+                               check_trajectory, first_true, jacobians, known_controls, known_module, known_states,
+                               linearise, probe_step, round_through, rollout, run_step, within)
+from tests.helpers import EDIT_ROUTES, maxdiff
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
-F32, F64 = torch.float32, torch.float64
-DT = {F32: "f32", F64: "f64"}
-K32 = 4
-
-# non-default physics of each system: parameters, dt, control clamp
-PHYS = {
-    "cartpole": dict(params=(9.81, 1.3, 0.25, 0.8), dt=0.1, clamp_attr="force_mag", clamp=7.5, n=5),
-    "pendulum": dict(params=(9.1, 1.7, 0.6), dt=0.15, clamp_attr="max_torque", clamp=1.5, n=3),
-}
-RADII = {"cartpole": (0.3, 1.0, 2.0), "pendulum": (0.3, 1.0, 3.0)}
-SYSTEMS = tuple(PHYS)
-
-
-def _module(name, params=None, device="cpu"):
-    from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
-    ph = PHYS[name]
-    p = torch.tensor(ph["params"], dtype=F64) if params is None else params
-    dx = (CartpoleDx if name == "cartpole" else PendulumDx)(params=p.to(device))
-    dx.dt = ph["dt"]
-    setattr(dx, ph["clamp_attr"], ph["clamp"])
-    return dx
-
-
-def _angle_cols(name):
-    return (2, 3) if name == "cartpole" else (0, 1)
-
-
-def _states(name, B, seed):
-    """float64 [B, n]: random states, angle pair at the RADII; the first rows hold the theta edge cases."""
-    g = torch.Generator().manual_seed(seed)
-    n = PHYS[name]["n"]
-    x = (torch.rand(B, n, generator=g, dtype=F64) - 0.5) * 2.0
-    th = (torch.rand(B, generator=g, dtype=F64) * 2 - 1) * 3.0
-    r0, _, r1 = RADII[name]
-    r = torch.tensor(RADII[name], dtype=F64).repeat(B)[:B]
-    ic, is_ = _angle_cols(name)
-    x[:, ic], x[:, is_] = r * torch.cos(th), r * torch.sin(th)
-    edge = ((-1.0, 0.0), (-1.0, -0.0), (-r0, 0.0), (-r1, -0.0), (1.0, 1e-9), (1.0, -1e-9), (r1, 0.0))
-    for k, (cv, sv) in enumerate(edge[:B]):
-        x[k, ic], x[k, is_] = cv, sv
-    return x
-
-
-def _clamp_edges(clamp, dtype):
-    """u at the clamp, one ulp (of dtype) inside and outside it, both signs."""
-    npd = np.float64 if dtype == F64 else np.float32
-    c = npd(clamp)
-    inn, out = float(np.nextafter(c, npd(0))), float(np.nextafter(c, npd(np.inf)))
-    return (clamp, -clamp, inn, -inn, out, -out)
-
-
-def _controls(name, T, B, dtype, seed):
-    """float64 [T, B, 1] in +-1.5 clamp; the edge values are spread over the first rows of every time step."""
-    g = torch.Generator().manual_seed(seed + 1)
-    clamp = PHYS[name]["clamp"]
-    u = (torch.rand(T, B, 1, generator=g, dtype=F64) * 2 - 1) * 1.5 * clamp
-    e = torch.tensor(_clamp_edges(clamp, dtype), dtype=F64)
-    k = min(B, len(e))
-    u[:, -k:, 0] = e[:k]                  # the last rows: the first rows hold the theta edges
-    return u
-
-
-def _jac(module, xs, us):
-    """(next, R, S) of module(xs, us) by autograd."""
-    xs = xs.clone().requires_grad_(True)
-    us = us.clone().requires_grad_(True)
-    nx = module(xs, us)
-    rows = [torch.autograd.grad(nx[:, j].sum(), [xs, us], retain_graph=True) for j in range(nx.shape[1])]
-    return nx.detach(), torch.stack([r[0] for r in rows], 1), torch.stack([r[1] for r in rows], 1)
-
-
-def _within(tag, got, w64, w32, dtype, tol64):
-    """float64: |got - w64| <= tol64 x scale; float32: <= K32 |w32 - w64| + 1e-6 x scale."""
-    scale = max(1.0, float(w64.abs().max())) if w64.numel() else 1.0
-    err = maxdiff(got, w64)
-    bound = tol64 * scale if dtype == F64 else K32 * maxdiff(w32, w64) + 1e-6 * scale
-    assert err <= bound, f"{tag}: |kernel - reference| = {err:.3e} > {bound:.3e}"
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -121,9 +45,9 @@ def test_rollout_matches_module(name, dtype, B, T):
     """Every step of the kernel rollout against the module's step from the kernel's own state (float64 CPU); the
     first state is the caller's x_init, copied exactly; several CTAs of 128 threads and a partial last one."""
     from mpc.pytorch_b200.dynamics import dyn_rollout_raw
-    dx = _module(name)
-    x0 = _states(name, B, 10 + B + T).to(dtype)
-    u = _controls(name, T, B, dtype, 20 + B + T).to(dtype)
+    dx = known_module(name)
+    x0 = known_states(name, B, 10 + B + T).to(dtype)
+    u = known_controls(name, T, B, dtype, 20 + B + T).to(dtype)
     x = dyn_rollout_raw(dx.mpcb200_kind, dx.mpcb200_params(), T, x0.to(DEV), u.to(DEV)).cpu()
     assert x.shape == (T, B, dx.n_state) and x.dtype == dtype
     assert torch.equal(x[0], x0)
@@ -132,7 +56,7 @@ def test_rollout_matches_module(name, dtype, B, T):
     xs, us = x[:-1].reshape(-1, dx.n_state).double(), u[:-1].reshape(-1, 1).double()
     w64 = dx(xs, us).view(T - 1, B, -1)
     w32 = dx(xs.float(), us.float()).view(T - 1, B, -1) if dtype == F32 else None
-    _within(f"{name} {DT[dtype]} B={B} T={T} rollout", x[1:], w64, w32, dtype, 1e-12)
+    within(f"{name} {DT[dtype]} B={B} T={T}", "rollout", x[1:], w64, w32, dtype, 1e-12)
 
 
 @pytest.mark.parametrize("B,T", BT, ids=[f"B{b}_T{t}" for b, t in BT])
@@ -142,28 +66,21 @@ def test_jacobians_match_autograd(name, dtype, B, T):
     """F = [R S] and f = x' - R x - S u of the linearisation kernel against float64 autograd of the module, at
     states off the unit circle, theta edges and controls at / one ulp either side of the clamp."""
     from mpc.pytorch_b200.dynamics import dyn_linearize_raw
-    dx = _module(name)
+    dx = known_module(name)
     n = dx.n_state
-    x = torch.stack([_states(name, B, 30 + t) for t in range(T)]).to(dtype)
-    u = _controls(name, T, B, dtype, 40 + B + T).to(dtype)
+    x = torch.stack([known_states(name, B, 30 + t) for t in range(T)]).to(dtype)
+    u = known_controls(name, T, B, dtype, 40 + B + T).to(dtype)
     F, f = dyn_linearize_raw(dx.mpcb200_kind, dx.mpcb200_params(), T, x.to(DEV), u.to(DEV))
     F, f = F.cpu(), f.cpu()
     assert F.shape == (T - 1, B, n, n + 1) and f.shape == (T - 1, B, n)
     if T == 1:
         assert F.numel() == 0 and f.numel() == 0
         return
-    xs, us = x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1)
-
-    def lin(dt):
-        nx, R, S = _jac(dx, xs.to(dt), us.to(dt))
-        fw = nx - torch.einsum("bij,bj->bi", R, xs.to(dt)) - torch.einsum("bij,bj->bi", S, us.to(dt))
-        return torch.cat((R, S), 2).view(T - 1, B, n, n + 1), fw.view(T - 1, B, n)
-
-    F64w, f64w = lin(F64)
-    F32w, f32w = lin(F32) if dtype == F32 else (None, None)
+    F64w, f64w = linearise(dx, x.to(F64), u.to(F64))
+    F32w, f32w = linearise(dx, x.to(F32), u.to(F32)) if dtype == F32 else (None, None)
     tag = f"{name} {DT[dtype]} B={B} T={T}"
-    _within(tag + " F", F, F64w, F32w, dtype, 1e-11)
-    _within(tag + " f", f, f64w, f32w, dtype, 1e-11)
+    within(tag, "F", F, F64w, F32w, dtype, 1e-11)
+    within(tag, "f", f, f64w, f32w, dtype, 1e-11)
     clamp = PHYS[name]["clamp"]
     out = u[:-1, :, 0].double().abs() > clamp
     assert bool((F[..., n][out] == 0).all()), f"{tag}: S must be exactly 0 beyond the clamp"
@@ -173,10 +90,6 @@ def test_jacobians_match_autograd(name, dtype, B, T):
 # ------------------------------------------------------------------------------------------------------------------
 # the fused LQR step: line-search rollout of the known system inside the step kernel
 # ------------------------------------------------------------------------------------------------------------------
-def _round(t, dtype):
-    return t.to(dtype).double() if torch.is_tensor(t) and t.is_floating_point() and dtype == F32 else t
-
-
 # (scale of the linear state cost, scale of the control row / column of C) of the step cases: the step asks for
 # large state moves, so that the first line-search pass of the nonlinear rollout is often worse than the nominal
 # trajectory and alpha decays.  The cartpole's control authority dt / (mc + mp) is small: its control weight is
@@ -190,24 +103,18 @@ def step_case(name, B, T, dtype, bounds, ls_iter, decay, seed, calm=False):
     The nominal controls are random; x is their nonlinear rollout and F, f its float64 linearisation.
     calm: hanging start (theta near pi), small nominal controls and linear cost - for long horizons, where the
     upright-pendulum rollout of random controls amplifies round-off past any fixed tolerance."""
-    dx = _module(name)
+    dx = known_module(name)
     n, p, clamp = dx.n_state, dx.n_state + 1, PHYS[name]["clamp"]
     g = torch.Generator().manual_seed(seed)
-    x0 = _states(name, B, seed)
+    x0 = known_states(name, B, seed)
     if calm:
         th = torch.pi + 0.4 * (torch.rand(B, generator=g, dtype=F64) - 0.5)
-        ic, is_ = _angle_cols(name)
+        ic, is_ = angle_cols(name)
         x0[:, ic], x0[:, is_] = torch.cos(th), torch.sin(th)
-    x0 = _round(x0, dtype)
-    u = _round((torch.rand(T, B, 1, generator=g, dtype=F64) * 2 - 1) * (0.1 if calm else 0.8) * clamp, dtype)
-    xs = [x0]
-    for t in range(T - 1):
-        xs.append(dx(xs[t], u[t]))
-    x = _round(torch.stack(xs), dtype)
-    nx, R, S = _jac(dx, x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1))
-    F = torch.cat((R, S), 2).view(T - 1, B, n, p)
-    f = (nx - torch.einsum("bij,bj->bi", R, x[:-1].reshape(-1, n))
-         - torch.einsum("bij,bj->bi", S, u[:-1].reshape(-1, 1))).view(T - 1, B, n)
+    x0 = round_through(x0, dtype)
+    u = round_through((torch.rand(T, B, 1, generator=g, dtype=F64) * 2 - 1) * (0.1 if calm else 0.8) * clamp, dtype)
+    x = round_through(rollout(dx, x0, u), dtype)
+    F, f = linearise(dx, x, u)
     L = torch.randn(T, B, p, p, generator=g, dtype=F64) / p ** 0.5
     C = L @ L.transpose(-1, -2) + 0.5 * torch.eye(p, dtype=F64)
     c = torch.randn(T, B, p, generator=g, dtype=F64)
@@ -219,7 +126,7 @@ def step_case(name, B, T, dtype, bounds, ls_iter, decay, seed, calm=False):
         c[..., n:] = 0.0
         C[..., n:, :] *= u_weight
         C[..., :, n:] *= u_weight
-    F, f, C, c = (_round(v, dtype) for v in (F, f, C, c))
+    F, f, C, c = (round_through(v, dtype) for v in (F, f, C, c))
     kw = dict(linesearch_decay=decay, max_linesearch_iter=ls_iter)
     if bounds == "scalar":
         kw.update(u_lower=-0.8 * clamp, u_upper=0.8 * clamp)
@@ -228,7 +135,7 @@ def step_case(name, B, T, dtype, bounds, ls_iter, decay, seed, calm=False):
     elif bounds in ("tensor", "delta"):
         lo = -clamp * (0.3 + 1.7 * torch.rand(T, B, 1, generator=g, dtype=F64))
         hi = clamp * (0.3 + 1.7 * torch.rand(T, B, 1, generator=g, dtype=F64))
-        kw.update(u_lower=_round(lo, dtype), u_upper=_round(hi, dtype))
+        kw.update(u_lower=round_through(lo, dtype), u_upper=round_through(hi, dtype))
         u = torch.maximum(torch.minimum(u, kw["u_upper"]), kw["u_lower"])
         if bounds == "delta":
             kw["delta_u"] = 0.4 * clamp
@@ -237,24 +144,16 @@ def step_case(name, B, T, dtype, bounds, ls_iter, decay, seed, calm=False):
     o64 = orc.lqr_step_forward(n, 1, T, x0, C, c, F, f, x, u, coupled=False, dynamics=dx, ls_trace=trace, **kw)
     o32 = None
     if dtype == F32:
-        lo32 = lambda v: v.float() if torch.is_tensor(v) and v.is_floating_point() else v
-        dx32 = _module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32))
+        lo32 = lambda v: v.float() if torch.is_tensor(v) and v.is_floating_point() else v  # noqa: E731
+        dx32 = known_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32))
         o32 = orc.lqr_step_forward(n, 1, T, *[lo32(P[k]) for k in ("x0", "C", "c", "F", "f", "x", "u")],
                                    coupled=False, dynamics=dx32, **{k: lo32(v) for k, v in kw.items()})
     return P, kw, o64, torch.stack(trace), o32
 
 
-def _run_step(name, T, P, kw, dtype):
-    from mpc.pytorch_b200 import _lib
-    from mpc.pytorch_b200.step import lqr_step_raw
-    dx = _module(name)
-    d = lambda t: t.to(DEV, dtype) if torch.is_tensor(t) else t
-    o = lqr_step_raw(dx.n_state, 1, T, d(P["x0"]), d(P["C"]), d(P["c"]), d(P["F"]), d(P["f"]), d(P["x"]),
-                     d(P["u"]), want_gains=True, dyn=(dx.mpcb200_kind, dx.mpcb200_params()),
-                     **{k: d(v) for k, v in kw.items()})
-    plan = _lib.last_step_plan()
-    torch.cuda.synchronize()
-    return {k: v.cpu() for k, v in o.items() if v is not None}, plan
+def _run_step(name, T, case, dtype):
+    dx = known_module(name)
+    return run_step(dx.n_state, 1, T, case[0], case[1], dtype, dyn=(dx.mpcb200_kind, dx.mpcb200_params()))
 
 
 def _passes(alphas, decay):
@@ -279,34 +178,26 @@ def check_step(tag, r, case, dtype):
     decisions (number of decays) as the float64 oracle and alphas to 1e-6, except at near-ties; those problems
     leave the trajectory comparison."""
     P, kw, o64, trace, o32 = case
-    B = P["x0"].shape[0]
-    bounded = "u_lower" in kw
-    keep = torch.ones(B, dtype=torch.bool)
+    keep = torch.ones(P["x0"].shape[0], dtype=torch.bool)
     if dtype == F32:
         keep = _f32_compared(case)
-        assert int((~keep).sum()) <= max(1, B // 8), f"{tag}: {int((~keep).sum())} of {B} problems left out"
+        out = int((~keep).sum())
+        assert out <= max(1, len(keep) // 8), f"{tag}: {out} of {len(keep)} problems left out"
         decay = kw["linesearch_decay"]
         assert torch.equal(_passes(r["alphas"], decay)[keep], _passes(o64.alphas, decay)[keep]), \
             f"{tag}: line-search decisions {r['alphas']} vs {o64.alphas}"
         assert maxdiff(r["alphas"][keep], o64.alphas[keep]) <= 1e-6, f"{tag}: alphas"
+        assert int((r["status"] & ~1).max()) == 0, tag
     else:
-        assert torch.equal(r["alphas"], o64.alphas), f"{tag}: alphas {r['alphas']} vs {o64.alphas}"
+        check_alphas(tag, r, o64, None)
+        check_pnqp(tag, r, o64, kw)
+        check_clamps(tag, r, o64, kw)
+    check_trajectory(tag, r, P["u"], o64, o32, dtype, keep)
+    # the gains also on the scale of the trajectory: these systems' gains can be 14x larger than x and u
     sc = max(1.0, float(o64.new_x.abs().max()), float(o64.new_u.abs().max()))
-    for k in ("new_x", "new_u", "Ks", "ks"):
-        got, w64 = r[k][:, keep], getattr(o64, k)[:, keep]
-        w32 = getattr(o32, k)[:, keep] if o32 is not None else None
-        err = maxdiff(got, w64)
-        bound = 1e-9 * sc if dtype == F64 else K32 * maxdiff(w32, w64) + 1e-6 * sc
-        assert err <= bound, f"{tag}: {k} |kernel - oracle| = {err:.3e} > {bound:.3e}"
-    csc = max(1.0, float(o64.costs.abs().max()))
-    err = maxdiff(r["costs"][keep], o64.costs[keep])
-    bound = 1e-9 * csc if dtype == F64 else K32 * maxdiff(o32.costs[keep], o64.costs[keep]) + 1e-6 * csc
-    assert err <= bound, f"{tag}: costs {err:.3e} > {bound:.3e}"
-    assert int((r["status"] & ~1).max()) == 0, tag
-    if dtype == F64:
-        assert torch.equal(r["free_mask"].bool(), o64.free_masks), f"{tag}: free sets"
-        if bounded:
-            assert torch.equal(r["qp_iters"].long(), o64.qp_iters), f"{tag}: pnqp iterations"
+    for k in ("Ks", "ks"):
+        within(tag, k, r[k][:, keep], getattr(o64, k)[:, keep], None if o32 is None else getattr(o32, k)[:, keep],
+               dtype, scale=sc)
 
 
 def _layout(name, B, dtype):
@@ -335,7 +226,7 @@ def test_fused_step_matches_oracle(name, dtype, B, bulk, bounds, ls_iter, decay)
     assert is_bulk == bulk and B % W != 0 and (B % W) % ppw != 0
     T = 15
     case = step_case(name, B, T, dtype, bounds, ls_iter, decay, 500 + B)
-    r, plan = _run_step(name, T, case[0], case[1], dtype)
+    r, plan = _run_step(name, T, case, dtype)
     tag = f"{name} {DT[dtype]} B={B} T={T} {bounds} ls={ls_iter} decay={decay}"
     assert plan & _lib.PLAN_GENERIC, f"{tag}: plan {plan}"
     check_step(tag, r, case, dtype)
@@ -369,8 +260,7 @@ def test_fused_step_cases_exercise_the_line_search_and_the_clamp(name, dtype):
 def _gain_switch(n, dtype):
     """First horizon at which the generic kernel (known-system instance (n, 1)) keeps its gains in Ks/ks."""
     from mpc.pytorch_b200 import _lib
-    from tests.test_horizon_paths_gpu import _first_true, _probe_step
-    return _first_true(lambda T: not _probe_step(n, 1, dtype, T, 1, True) & _lib.PLAN_GAINS_SMEM)
+    return first_true(lambda T: not probe_step(n, 1, dtype, T, 1, True) & _lib.PLAN_GAINS_SMEM)
 
 
 @pytest.mark.parametrize("name", SYSTEMS)
@@ -383,7 +273,7 @@ def test_fused_step_on_both_sides_of_the_gain_store_switch(name):
     assert Ts is not None and 2 < Ts <= 1024, Ts
     for T in (Ts - 1, Ts):
         case = step_case(name, B, T, F64, "scalar", 4, 0.3, 700 + T, calm=True)
-        r, plan = _run_step(name, T, case[0], case[1], F64)
+        r, plan = _run_step(name, T, case, F64)
         tag = f"{name} f64 B={B} T={T} (switch {Ts})"
         assert plan & _lib.PLAN_GENERIC, tag
         assert bool(plan & _lib.PLAN_GAINS_SMEM) == (T < Ts), f"{tag}: plan {plan}"
@@ -426,9 +316,9 @@ MPC_CASES = [(1, 100), (13, 25), (300, 2), (300, 25)]
 @pytest.mark.parametrize("B,T", MPC_CASES, ids=[f"B{b}_T{t}" for b, t in MPC_CASES])
 @pytest.mark.parametrize("name", SYSTEMS)
 def test_mpc_known_system_equals_module_path(name, B, T, bounds):
-    dx = _module(name)
+    dx = known_module(name)
     clamp = PHYS[name]["clamp"]
-    x0 = _states(name, B, 900 + B + T)
+    x0 = known_states(name, B, 900 + B + T)
     a, b = _mpc_pair(dx, x0, B, T, (0.8 if bounds == "in" else 2.0) * clamp)
     _assert_mpc_equal(f"{name} B={B} T={T} bounds {bounds}", a, b)
 
@@ -442,12 +332,11 @@ def test_kernels_follow_parameter_edits_between_solves(name):
     after each edit the kernel rollout and Jacobians equal the module's own forward and autograd, and MPC.forward
     with the known system equals the same physics run as an opaque Module."""
     from mpc.pytorch_b200.dynamics import dyn_linearize_raw, dyn_rollout_raw
-    from tests.test_known_systems_cpu import EDIT_ROUTES
-    dx = _module(name, params=torch.tensor(PHYS[name]["params"], dtype=F64, device=DEV).requires_grad_(True),
+    dx = known_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F64, device=DEV).requires_grad_(True),
                  device=DEV)
     B, T = 9, 12
-    x0 = _states(name, B, 77)
-    u = _controls(name, T, B, F64, 78)
+    x0 = known_states(name, B, 77)
+    u = known_controls(name, T, B, F64, 78)
     base = torch.tensor(PHYS[name]["params"], dtype=F64)
     for k, (route, edit) in enumerate(EDIT_ROUTES):
         _mpc_pair(dx, x0, B, T, 2.0 * PHYS[name]["clamp"], lqr_iter=2)      # a solve before the edit
@@ -458,7 +347,7 @@ def test_kernels_follow_parameter_edits_between_solves(name):
         want = dx(x[:-1].reshape(-1, dx.n_state), u[:-1].reshape(-1, 1).to(DEV)).view(T - 1, B, -1)
         assert maxdiff(x[1:], want) <= 1e-12 * max(1.0, float(want.abs().max())), f"{route}: rollout"
         F, f = dyn_linearize_raw(dx.mpcb200_kind, prm, T, x, u.to(DEV))
-        _, R, S = _jac(dx, x[:-1].reshape(-1, dx.n_state).detach(), u[:-1].reshape(-1, 1).to(DEV))
+        _, R, S = jacobians(dx, x[:-1].reshape(-1, dx.n_state).detach(), u[:-1].reshape(-1, 1).to(DEV))
         Fw = torch.cat((R, S), 2).view(T - 1, B, dx.n_state, -1)
         assert maxdiff(F, Fw) <= 1e-11 * max(1.0, float(Fw.abs().max())), f"{route}: Jacobians"
         a, b = _mpc_pair(dx, x0, B, T, 2.0 * PHYS[name]["clamp"], lqr_iter=3)

@@ -3,19 +3,7 @@
 import pytest
 import torch
 
-from tests.helpers import load_golden
-
-
-def build_net(g, act):
-    from mpc.dynamics import NNDynamics
-    nl = int(g["n_layers"])
-    hidden = [g[f"W{i}"].shape[0] for i in range(nl - 1)]
-    net = NNDynamics(3, 2, hidden_sizes=hidden, activation=act).double()
-    with torch.no_grad():
-        for i, fc in enumerate(net.fcs):
-            fc.weight.copy_(g[f"W{i}"])
-            fc.bias.copy_(g[f"b{i}"])
-    return net
+from tests.helpers import build_net, load_golden
 
 
 @pytest.mark.parametrize("act", ["sigmoid", "relu"])

@@ -9,8 +9,7 @@ TOL_XU, TOL_COST = 2e-4, 1e-5
 import pytest
 import torch
 
-from tests.helpers import load_golden, maxdiff
-from tests.test_models_cpu import build_net
+from tests.helpers import build_net, load_golden, maxdiff
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")

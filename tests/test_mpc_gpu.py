@@ -5,7 +5,7 @@ import io
 import pytest
 import torch
 
-from tests.helpers import gen_problem, load_golden, maxdiff
+from tests.helpers import condensed_box_lqr_scipy, gen_problem, load_golden, maxdiff
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
@@ -186,7 +186,6 @@ def test_mpc_solution_is_the_box_qp_optimum(bound):
     """reference tests/test_mpc.py:91-194: the iLQR fixed point computed on the GPU equals the optimum of the
     box-constrained problem found by an independent solver (scipy L-BFGS-B on the condensed problem)."""
     from mpc import mpc
-    from tests.test_oracle_golden import _condensed_box_lqr_scipy
     B, T, n, m = 2, 5, 3, 2
     C, c, F, f, x0 = gen_problem(41, B, T, n, m, torch.float64, time_varying=True)
     lo, hi = (-1e4, 1e4) if bound is None else (-bound, bound)
@@ -194,7 +193,7 @@ def test_mpc_solution_is_the_box_qp_optimum(bound):
     x, u, _ = mpc.MPC(n, m, T, lqr_iter=30, eps=1e-10, verbose=-1, exit_unconverged=False, **kw)(
         x0.to(DEV), mpc.QuadCost(C.to(DEV), c.to(DEV)), mpc.LinDx(F.to(DEV), f.to(DEV)))
     for b in range(B):
-        xs, us = _condensed_box_lqr_scipy(C[:, b], c[:, b], F[:, b], f[:, b], x0[b], lo, hi)
+        xs, us = condensed_box_lqr_scipy(C[:, b], c[:, b], F[:, b], f[:, b], x0[b], lo, hi)
         assert maxdiff(u[:, b], us) < 2e-4 and maxdiff(x[:, b], xs) < 2e-4
 
 

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.helpers import GOLD, gen_problem, load_golden, maxdiff, nominal_controls
+from tests.helpers import GOLD, condensed_box_lqr_scipy, gen_problem, load_golden, maxdiff, nominal_controls
 
 
 def _names(prefix):
@@ -148,35 +148,6 @@ def test_unbounded_lqr_solves_the_kkt_system():
         assert maxdiff(tau[:, n:], o.new_u[:, b]) < 1e-9
 
 
-def _condensed_box_lqr_scipy(C, c, F, f, x0, lo, hi):
-    """Independent solution of one problem instance with scipy (stands in for cvxpy lqr_cp,
-    reference tests/test_mpc.py:35-62): minimise the rolled-out cost over u in the box."""
-    import numpy as np
-    from scipy.optimize import minimize
-    T, p = C.shape[0], C.shape[1]
-    n = x0.shape[0]
-    m = p - n
-    C, c, F, f, x0 = (a.numpy() for a in (C, c, F, f, x0))
-
-    def rollout(uflat):
-        u = uflat.reshape(T, m)
-        x = np.zeros((T, n))
-        x[0] = x0
-        for t in range(T - 1):
-            x[t + 1] = F[t] @ np.concatenate((x[t], u[t])) + f[t]
-        return x, u
-
-    def cost(uflat):
-        x, u = rollout(uflat)
-        tau = np.concatenate((x, u), 1)
-        return float(sum(0.5 * tau[t] @ C[t] @ tau[t] + c[t] @ tau[t] for t in range(T)))
-
-    res = minimize(cost, np.zeros(T * m), method="L-BFGS-B", bounds=[(lo, hi)] * (T * m),
-                   options=dict(maxiter=2000, ftol=1e-15, gtol=1e-10))
-    x, u = rollout(res.x)
-    return torch.from_numpy(x), torch.from_numpy(u)
-
-
 @pytest.mark.parametrize("bound", [None, 0.35])
 def test_ilqr_fixed_point_is_the_box_qp_optimum(bound):
     """reference tests/test_mpc.py:91-194 (LQR / box-LQR vs an independent convex solver, rtol 1e-3)."""
@@ -186,7 +157,7 @@ def test_ilqr_fixed_point_is_the_box_qp_optimum(bound):
     x, u, costs, fdn = orc.mpc_forward_lin(n, m, T, x0, C, c, F, f, u_lower=None if bound is None else lo,
                                            u_upper=None if bound is None else hi, lqr_iter=30, eps=1e-10)
     for b in range(B):
-        xs, us = _condensed_box_lqr_scipy(C[:, b], c[:, b], F[:, b], f[:, b], x0[b], lo, hi)
+        xs, us = condensed_box_lqr_scipy(C[:, b], c[:, b], F[:, b], f[:, b], x0[b], lo, hi)
         assert maxdiff(u[:, b], us) < 2e-4 and maxdiff(x[:, b], xs) < 2e-4
     if bound is not None:
         assert 0.05 < float(((u.abs() - bound).abs() < 1e-9).double().mean()) < 0.95

@@ -12,10 +12,10 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.helpers import gen_problem, maxdiff, nominal_controls
+from tests.gpu_harness import check_step_fixed, run_step
+from tests.helpers import gen_problem, nominal_controls
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
 SHAPES = [(1, 1), (2, 1), (2, 2), (3, 1), (3, 2), (3, 4), (4, 1), (4, 2), (4, 4), (5, 1), (6, 2), (7, 4), (8, 1), (8, 2),
           (8, 4), (12, 4), (16, 4), (3, 3), (6, 1), (5, 2), (10, 2)]          # the last four run zero-padded
 
@@ -42,27 +42,9 @@ def make_cases(count=42, seed=2024):
 CASES = make_cases()
 
 
-def _run(impl, monkeypatch, n, m, T, x0, C, c, F, f, x, u, **kw):
-    from mpc.pytorch_b200.step import lqr_step_raw
-    from mpc.pytorch_b200._lib import MpcB200Error
-    if impl is None:
-        monkeypatch.delenv("MPCB200_KERNEL", raising=False)
-    else:
-        monkeypatch.setenv("MPCB200_KERNEL", impl)
-    cu = lambda t: t.to(DEV) if torch.is_tensor(t) else t
-    try:
-        o = lqr_step_raw(n, m, T, cu(x0), cu(C), cu(c), cu(F), cu(f), cu(x), cu(u), want_gains=True,
-                         **{k: cu(v) for k, v in kw.items()})
-    except MpcB200Error as e:
-        if impl == "2" and "[3]" in str(e):
-            return None                       # the column-pair mapping does not take this shape / alignment
-        raise
-    torch.cuda.synchronize()
-    return {k: (v.cpu() if torch.is_tensor(v) else v) for k, v in o.items()}
-
-
 @pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
-def test_random_case_matches_oracle_under_every_kernel(case, monkeypatch):
+def test_random_case_matches_oracle_under_every_kernel(case):
+    from mpc.pytorch_b200._lib import MpcB200Error
     name, seed, B, T, n, m, dtype, bounds, delta, tv, wf, mask = case
     C, c, F, f, x0 = gen_problem(seed, B, T, n, m, dtype, tv, wf)
     if T == 1:
@@ -74,37 +56,15 @@ def test_random_case_matches_oracle_under_every_kernel(case, monkeypatch):
         g = torch.Generator().manual_seed(seed)
         kw["u_zero_I"] = torch.rand(T, B, m, generator=g) < 0.3
     o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, x, u, coupled=False, **kw)
-    f64 = dtype == torch.float64
-    tol = 1e-9 if f64 else (2e-4 if bounds is not None else 4e-5)
-    scale = max(1.0, float(o.new_x.abs().max()))
+    P = dict(x0=x0, C=C, c=c, F=F, f=f, x=x, u=u)
     ran = 0
     for impl in (None, "1", "2"):
-        r = _run(impl, monkeypatch, n, m, T, x0, C, c, F, f, x, u, **kw)
-        if r is None:
-            continue
+        try:
+            r, _ = run_step(n, m, T, P, kw, impl=impl)
+        except MpcB200Error as e:
+            if impl == "2" and "[3]" in str(e):
+                continue                      # the column-pair mapping does not take this shape / alignment
+            raise
         ran += 1
-        tag = f"{name} impl={impl}"
-        assert maxdiff(r["new_x"], o.new_x) <= tol * scale, tag
-        assert maxdiff(r["new_u"], o.new_u) <= tol * scale, tag
-        assert maxdiff(r["Ks"], o.Ks) <= tol * scale and maxdiff(r["ks"], o.ks) <= tol * scale, tag
-        assert maxdiff(r["costs"], o.costs) <= (1e-9 if f64 else 3e-4) * max(1.0, float(o.costs.abs().max())), tag
-        assert maxdiff(r["alphas"], o.alphas) == 0.0, tag
-        assert int((r["status"] & ~1).max()) == 0, tag
-        flagged = (r["status"] & 1) != 0
-        if f64 or bounds is None:
-            assert not bool(flagged.any()), tag
-        else:
-            assert int(flagged.sum()) <= 1 and bool((r["qp_iters"][:, flagged] == 19).any(0).all()), tag
-        ok = ~flagged
-        if bounds is not None:
-            assert torch.equal(r["free_mask"].bool()[:, ok], o.free_masks[:, ok]), tag
-            assert torch.equal(r["qp_iters"].long()[:, ok], o.qp_iters[:, ok]), tag
-            lo = ul if torch.is_tensor(ul) else torch.full_like(u, ul)
-            hi = uu if torch.is_tensor(uu) else torch.full_like(u, uu)
-            assert bool(((r["new_u"] >= lo) & (r["new_u"] <= hi)).all()), tag
-            if delta is None:
-                assert torch.equal((r["new_u"] == lo)[:, ok], (o.new_u == lo)[:, ok]), tag
-                assert torch.equal((r["new_u"] == hi)[:, ok], (o.new_u == hi)[:, ok]), tag
-        if mask:
-            assert bool((r["new_u"][kw["u_zero_I"]] == 0).all()), tag
+        check_step_fixed(f"{name} impl={impl}", r, o, kw, dtype)
     assert ran >= 2

@@ -7,23 +7,23 @@ import ctypes
 import pytest
 import torch
 
-from mpc.pytorch_b200 import _lib, solver, step
+from mpc.pytorch_b200 import _lib, step
 from mpc.pytorch_b200.dynamics import dyn_linearize_raw, dyn_rollout_raw
 from mpc.pytorch_b200.solver import MPC, CtrlPassthroughDynamics, GradMethods, LinDx, QuadCost
 from oracle import lqr_oracle as orc
+from tests.gpu_harness import (BT, DEV, F32, F64, PHYS, SYSTEMS, check_alphas, check_clamps, check_pnqp,
+                               check_trajectory, known_controls, known_module, known_states, linearise, rollout,
+                               run_step, same_on_both_loops, solve_on, within)
 from tests.helpers import gen_problem, load_golden, maxdiff
-from tests.test_known_systems_gpu import BT, PHYS, SYSTEMS, _controls, _jac, _module, _states, _within
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
-F64, F32 = torch.float64, torch.float32
 
 
-def _aug_states(name, B, T, dtype, seed):
+def _augknown_states(name, B, T, dtype, seed):
     """[B, n+1] passthrough states (previous control, then the system's edge states) and [T, B, 1] controls."""
-    u = _controls(name, T, B, dtype, seed)
-    prev = _controls(name, 1, B, dtype, seed + 5)[0]
-    return torch.cat((prev, _states(name, B, seed)), 1), u
+    u = known_controls(name, T, B, dtype, seed)
+    prev = known_controls(name, 1, B, dtype, seed + 5)[0]
+    return torch.cat((prev, known_states(name, B, seed)), 1), u
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -35,8 +35,8 @@ def _aug_states(name, B, T, dtype, seed):
 def test_passthrough_rollout_matches_module(name, dtype, B, T):
     """Every step of the passthrough rollout against CtrlPassthroughDynamics(module) from the kernel's own state;
     the first M states of each next state are the control exactly as given, before the system's clamp."""
-    pt = CtrlPassthroughDynamics(_module(name))
-    x0, u = _aug_states(name, B, T, dtype, 10 + B + T)
+    pt = CtrlPassthroughDynamics(known_module(name))
+    x0, u = _augknown_states(name, B, T, dtype, 10 + B + T)
     x0, u = x0.to(dtype), u.to(dtype)
     x = dyn_rollout_raw(pt.mpcb200_kind, pt.mpcb200_params(), T, x0.to(DEV), u.to(DEV)).cpu()
     assert x.shape == (T, B, pt.n_state) and x.dtype == dtype
@@ -44,11 +44,11 @@ def test_passthrough_rollout_matches_module(name, dtype, B, T):
     if T == 1:
         return
     assert torch.equal(x[1:, :, :1], u[:-1])
-    pt32 = CtrlPassthroughDynamics(_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32)))
+    pt32 = CtrlPassthroughDynamics(known_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32)))
     xs, us = x[:-1].reshape(-1, pt.n_state).double(), u[:-1].reshape(-1, 1).double()
     w64 = pt(xs, us).view(T - 1, B, -1)
     w32 = pt32(xs.float(), us.float()).view(T - 1, B, -1) if dtype == F32 else None
-    _within(f"{name} B={B} T={T} rollout", x[1:], w64, w32, dtype, 1e-12)
+    within(f"{name} B={B} T={T}", "rollout", x[1:], w64, w32, dtype, 1e-12)
 
 
 @pytest.mark.parametrize("B,T", BT, ids=[f"B{b}_T{t}" for b, t in BT])
@@ -58,29 +58,23 @@ def test_passthrough_linearisation_matches_autograd(name, dtype, B, T):
     """F~, f~ of the linearisation kernel against autograd of CtrlPassthroughDynamics(module) at states off the unit
     circle, theta edges, previous and current controls at / one ulp either side of the clamp; and bitwise the blocks
     MPC._slew_augment assembles from the system's own linearisation kernel."""
-    dx = _module(name)
+    dx = known_module(name)
     pt = CtrlPassthroughDynamics(dx)
     n = pt.n_state
     prm = pt.mpcb200_params()
-    x = torch.stack([_aug_states(name, B, 1, dtype, 30 + t)[0] for t in range(T)]).to(dtype)
-    u = _controls(name, T, B, dtype, 40 + B + T).to(dtype)
+    x = torch.stack([_augknown_states(name, B, 1, dtype, 30 + t)[0] for t in range(T)]).to(dtype)
+    u = known_controls(name, T, B, dtype, 40 + B + T).to(dtype)
     F, f = dyn_linearize_raw(pt.mpcb200_kind, prm, T, x.to(DEV), u.to(DEV))
     assert F.shape == (T - 1, B, n, n + 1) and f.shape == (T - 1, B, n)
     if T == 1:
         assert F.numel() == 0 and f.numel() == 0
         return
-    xs, us = x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1)
-    pt32 = CtrlPassthroughDynamics(_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32)))
-
-    def lin(mod, dt):
-        nx, R, S = _jac(mod, xs.to(dt), us.to(dt))
-        fw = nx - torch.einsum("bij,bj->bi", R, xs.to(dt)) - torch.einsum("bij,bj->bi", S, us.to(dt))
-        return torch.cat((R, S), 2).view(T - 1, B, n, n + 1), fw.view(T - 1, B, n)
-    Fw, fw = lin(pt, F64)
-    F32w, f32w = lin(pt32, F32) if dtype == F32 else (None, None)
+    pt32 = CtrlPassthroughDynamics(known_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F32)))
+    Fw, fw = linearise(pt, x.to(F64), u.to(F64))
+    F32w, f32w = linearise(pt32, x.to(F32), u.to(F32)) if dtype == F32 else (None, None)
     tag = f"{name} B={B} T={T}"
-    _within(f"{tag} F", F.cpu(), Fw, F32w, dtype, 1e-11)
-    _within(f"{tag} f", f.cpu(), fw, f32w, dtype, 1e-11)
+    within(tag, "F", F.cpu(), Fw, F32w, dtype, 1e-11)
+    within(tag, "f", f.cpu(), fw, f32w, dtype, 1e-11)
     Fi, fi = dyn_linearize_raw(dx.mpcb200_kind, prm, T, x[..., 1:].contiguous().to(DEV), u.to(DEV))
     ctrl = MPC(dx.n_state, 1, T, slew_rate_penalty=1.0)
     C = torch.zeros(T, B, n, n, dtype=dtype, device=DEV)          # the system's own (n_state + 1)^2
@@ -95,9 +89,9 @@ def _step_case(name, B, T, bounds, seed, calm=False):
     """A float64 passthrough LQR step around a module rollout, and the oracle's step with the module as dynamics.
     `calm`: the system starts near its resting angle with small controls, so that long horizons stay bounded."""
     g = torch.Generator().manual_seed(seed)
-    pt = CtrlPassthroughDynamics(_module(name))
+    pt = CtrlPassthroughDynamics(known_module(name))
     clamp = PHYS[name]["clamp"]
-    x0, u = _aug_states(name, B, T, F64, seed)
+    x0, u = _augknown_states(name, B, T, F64, seed)
     x0[:, 0] *= 0.2
     u = u * 0.2
     if calm:
@@ -105,16 +99,10 @@ def _step_case(name, B, T, bounds, seed, calm=False):
         ic, is_ = (3, 4) if name == "cartpole" else (1, 2)
         x0[:, ic], x0[:, is_] = torch.cos(th), torch.sin(th)
         u = u * 0.5
-    xs = [x0]
-    for t in range(T - 1):
-        xs.append(pt(xs[t], u[t]))
-    x = torch.stack(xs)
+    x = rollout(pt, x0, u)
     n = x.shape[2]
     p = n + 1
-    nx, R, S = _jac(pt, x[:-1].reshape(-1, n), u[:-1].reshape(-1, 1))
-    F = torch.cat((R, S), 2).view(T - 1, B, n, p)
-    f = (nx - torch.einsum("bij,bj->bi", R, x[:-1].reshape(-1, n))
-         - torch.einsum("bij,bj->bi", S, u[:-1].reshape(-1, 1))).view(T - 1, B, n)
+    F, f = linearise(pt, x, u)
     L = torch.randn(T, B, p, p, generator=g, dtype=F64) / p ** 0.5
     C = L @ L.transpose(-1, -2) + 0.5 * torch.eye(p, dtype=F64)
     c = torch.randn(T, B, p, generator=g, dtype=F64)
@@ -132,34 +120,27 @@ def _step_case(name, B, T, bounds, seed, calm=False):
 def _kernel_step(name, T, P, kw, monkeypatch):
     """lqr_step_raw with the passthrough kind (alphas, free sets, pnqp counts) and LQRStep with
     true_dynamics=CtrlPassthroughDynamics(known) (its outputs; split mode must not run)."""
-    pt = CtrlPassthroughDynamics(_module(name))
+    pt = CtrlPassthroughDynamics(known_module(name))
     n = pt.n_state
-    d = lambda t: t.to(DEV) if torch.is_tensor(t) else t
-    r = step.lqr_step_raw(n, 1, T, *[d(P[k]) for k in ("x0", "C", "c", "F", "f", "x", "u")],
-                          dyn=(pt.mpcb200_kind, pt.mpcb200_params()), **{k: d(v) for k, v in kw.items()})
-    plan = _lib.last_step_plan()
+    r, plan = run_step(n, 1, T, P, kw, want_gains=False, dyn=(pt.mpcb200_kind, pt.mpcb200_params()))
 
     def no_split(*a, **k):
         raise AssertionError("split-mode rollout ran")
     monkeypatch.setattr(step, "rollout_split", no_split)
-    C, c, F, f = (d(P[k]) for k in ("C", "c", "F", "f"))
+    C, c, F, f = (P[k].to(DEV) for k in ("C", "c", "F", "f"))
     nx, nu, _, costs, _, _ = step.LQRStep(n, 1, T, true_cost=QuadCost(C, c), true_dynamics=pt,
-                                          current_x=d(P["x"]), current_u=d(P["u"]), **kw)(d(P["x0"]), C, c, F, f)
-    assert torch.equal(nx, r["new_x"]) and torch.equal(nu, r["new_u"]) and torch.equal(costs, r["costs"])
-    torch.cuda.synchronize()
-    return {k: v.cpu() for k, v in r.items() if v is not None}, plan
+                                          current_x=P["x"].to(DEV), current_u=P["u"].to(DEV), **kw)(
+        P["x0"].to(DEV), C, c, F, f)
+    for k, v in (("new_x", nx), ("new_u", nu), ("costs", costs)):
+        assert torch.equal(v.cpu(), r[k]), k
+    return r, plan
 
 
-def _check_step(tag, r, o, bounded):
-    assert torch.equal(r["alphas"], o.alphas), f"{tag}: alphas {r['alphas']} vs {o.alphas}"
-    sc = max(1.0, float(o.new_x.abs().max()), float(o.new_u.abs().max()))
-    for k in ("new_x", "new_u"):
-        err = maxdiff(r[k], getattr(o, k))
-        assert err <= 1e-9 * sc, f"{tag}: {k} {err:.3e}"
-    assert maxdiff(r["costs"], o.costs) <= 1e-9 * max(1.0, float(o.costs.abs().max())), tag
-    assert torch.equal(r["free_mask"].bool(), o.free_masks), f"{tag}: free sets"
-    if bounded:
-        assert torch.equal(r["qp_iters"].long(), o.qp_iters), f"{tag}: pnqp iterations"
+def _check_step(tag, r, P, kw, o):
+    check_alphas(tag, r, o, None)
+    check_trajectory(tag, r, P["u"], o, None, F64)
+    check_pnqp(tag, r, o, kw)
+    check_clamps(tag, r, o, kw)
 
 
 # problems per CTA of the dynamics-only instances in float64: (6, 1) W = 4, (4, 1) W = 6; the bulk path needs B even
@@ -174,7 +155,7 @@ def test_passthrough_step_matches_oracle(name, B, bounds, monkeypatch):
     r, plan = _kernel_step(name, T, P, kw, monkeypatch)
     tag = f"{name} B={B} {bounds}"
     assert plan & _lib.PLAN_GENERIC, f"{tag}: plan {plan}"
-    _check_step(tag, r, o, bounds is not None)
+    _check_step(tag, r, P, kw, o)
 
 
 def _gain_switch(kind, n, esz):
@@ -189,7 +170,7 @@ def _gain_switch(kind, n, esz):
 
 @pytest.mark.parametrize("name", SYSTEMS)
 def test_passthrough_step_on_both_sides_of_the_gain_store_switch(name, monkeypatch):
-    pt = CtrlPassthroughDynamics(_module(name))
+    pt = CtrlPassthroughDynamics(known_module(name))
     Ts = _gain_switch(pt.mpcb200_kind, pt.n_state, 8)
     assert Ts is not None and 2 < Ts <= 1024, Ts
     for T in (Ts - 1, Ts):
@@ -198,63 +179,28 @@ def test_passthrough_step_on_both_sides_of_the_gain_store_switch(name, monkeypat
         tag = f"{name} T={T} (switch {Ts})"
         assert plan & _lib.PLAN_GENERIC, tag
         assert bool(plan & _lib.PLAN_GAINS_SMEM) == (T < Ts), f"{tag}: plan {plan}"
-        _check_step(tag, r, o, True)
+        _check_step(tag, r, P, kw, o)
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # MPC.forward with a slew-rate penalty: device loop vs host loop
 # ------------------------------------------------------------------------------------------------------------------
-def _run(monkeypatch, make, x0, cost, dx, device_loop, grads=()):
-    """(x, u, costs, full_du_norm, gradients of (x.sum() + u.sum()) w.r.t. `grads`) on the chosen loop."""
-    seen = {}
-    with monkeypatch.context() as mp:
-        if device_loop:
-            assert solver._use_slew_device_loop(make(), x0, cost, dx, _u0(make(), x0))
-            real = step.ilqr_raw
-
-            def spy(*a, **k):
-                seen["res"] = real(*a, **k)
-                return seen["res"]
-            mp.setattr(step, "ilqr_raw", spy)
-        else:
-            mp.setattr(solver, "_use_slew_device_loop", lambda *a: False)
-        real_host = MPC._ilqr_host
-
-        def host(self, *a, **k):
-            seen["best"] = real_host(self, *a, **k)
-            return seen["best"]
-        mp.setattr(MPC, "_ilqr_host", host)
-        x, u, costs = make()(x0, cost, dx)
-    assert ("res" in seen) == device_loop and ("best" in seen) != device_loop
-    fdn = seen["res"]["full_du_norm"] if device_loop else seen["best"]["full_du_norm"]
-    gs = torch.autograd.grad(x.sum() + u.sum(), grads) if grads else ()
-    torch.cuda.synchronize()
-    return x, u, costs, fdn, gs
-
-
-def _u0(ctrl, x0):
-    return torch.zeros(ctrl.T, x0.shape[0], ctrl.n_ctrl, dtype=x0.dtype, device=x0.device)
-
-
-def _bitwise(tag, a, b):
-    """x, u, costs and the gradients bit for bit; full_du_norm, which the device loop sums in another order (DESIGN
-    section 3.5), to 1e-12 (float64) / 1e-5 (float32) relative."""
-    for k, (p, q) in enumerate(zip(a[:3], b[:3])):
-        assert p.shape == q.shape and torch.equal(p, q), f"{tag}: output {k} {float((p - q).abs().max()):.3e}"
-    rtol = 1e-12 if a[3].dtype == F64 else 1e-5
-    assert torch.allclose(a[3], b[3], rtol=rtol, atol=0), f"{tag}: full_du_norm {float((a[3] - b[3]).abs().max())}"
-    for k, (p, q) in enumerate(zip(a[4], b[4])):
-        assert torch.equal(p, q), f"{tag}: gradient {k} {float((p - q).abs().max()):.3e}"
+def _same_full_du_norm(tag, dev, host):
+    """full_du_norm, which the device loop sums in another order (DESIGN section 3.5): 1e-12 (float64) / 1e-5
+    (float32) relative."""
+    a, b = dev.full_du_norm, host.full_du_norm
+    rtol = 1e-12 if a.dtype == F64 else 1e-5
+    assert torch.allclose(a, b, rtol=rtol, atol=0), f"{tag}: full_du_norm {float((a - b).abs().max())}"
 
 
 def _known_problem(name, B, T):
-    dx = _module(name, params=torch.tensor(PHYS[name]["params"], dtype=F64, device=DEV).requires_grad_(True),
+    dx = known_module(name, params=torch.tensor(PHYS[name]["params"], dtype=F64, device=DEV).requires_grad_(True),
                  device=DEV)
     n = dx.n_state
     q, p = dx.get_true_obj()
     Q = torch.diag(q).double().expand(T, B, n + 1, n + 1).contiguous().to(DEV).requires_grad_(True)
     pp = p.double().expand(T, B, n + 1).contiguous().to(DEV).requires_grad_(True)
-    return dx, Q, pp, _states(name, B, 40 + B).to(DEV)
+    return dx, Q, pp, known_states(name, B, 40 + B).to(DEV)
 
 
 KNOWN_CASES = [("in", None, None), ("wide", None, None), ("in", 0.3, None), ("in", None, "m"), ("wide", 0.5, "Bm")]
@@ -276,19 +222,18 @@ def test_known_system_slew_device_loop_equals_host_loop(name, bounds, delta, pre
               delta_u=None if delta is None else delta * clamp)
     make = lambda: MPC(dx.n_state, 1, T, **kw)
     cost = QuadCost(Q, pp)
-    dev = _run(monkeypatch, make, x0, cost, dx, True, grads=(Q, pp, dx.params))
-    host = _run(monkeypatch, make, x0, cost, dx, False, grads=(Q, pp, dx.params))
     tag = f"{name} {bounds} delta {delta} prev {prev}"
-    _bitwise(tag, dev, host)
-    assert float(dev[4][2].abs().max()) > 0, f"{tag}: no gradient reaches the system parameters"
+    dev, host = same_on_both_loops(monkeypatch, make, x0, cost, dx, grads=(Q, pp, dx.params))
+    _same_full_du_norm(tag, dev, host)
+    assert float(dev.grads[2].abs().max()) > 0, f"{tag}: no gradient reaches the system parameters"
 
     class Opaque(torch.nn.Module):                      # hides mpcb200_kind: today's Module path (split mode)
         def forward(self, xx, uu):
             return dx(xx, uu)
     x, u, costs = make()(x0, QuadCost(Q.detach(), pp.detach()), Opaque())
-    for k, (p, q) in enumerate(((x, dev[0]), (u, dev[1]))):
+    for k, (p, q) in enumerate(((x, dev.x), (u, dev.u))):
         assert maxdiff(p, q) < 1e-7 * max(1.0, float(p.abs().max())), f"{tag}: opaque module {k}"
-    assert maxdiff(costs, dev[2]) < 1e-8 * max(1.0, float(costs.abs().max())), f"{tag}: opaque costs"
+    assert maxdiff(costs, dev.costs) < 1e-8 * max(1.0, float(costs.abs().max())), f"{tag}: opaque costs"
 
 
 @pytest.mark.parametrize("name", SYSTEMS)
@@ -300,13 +245,12 @@ def test_known_system_slew_follows_parameter_edits(name, monkeypatch):
               grad_method=GradMethods.AUTO_DIFF)
     make = lambda: MPC(dx.n_state, 1, T, **kw)
     cost = QuadCost(Q.detach(), pp.detach())
-    first = _run(monkeypatch, make, x0, cost, dx, True)
+    first = solve_on(monkeypatch, make, x0, cost, dx, True)
     with torch.no_grad():
         dx.params.mul_(1.2)
-    dev = _run(monkeypatch, make, x0, cost, dx, True)
-    host = _run(monkeypatch, make, x0, cost, dx, False)
-    _bitwise(f"{name} after an edit", dev, host)
-    assert not torch.equal(first[0], dev[0])
+    dev, host = same_on_both_loops(monkeypatch, make, x0, cost, dx)
+    _same_full_du_norm(f"{name} after an edit", dev, host)
+    assert not torch.equal(first.x, dev.x)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -334,9 +278,8 @@ def test_lindx_slew_device_loop_equals_host_loop(n, m, dtype, case, monkeypatch)
         kw.update(u_zero_I=(torch.rand(T, B, m, generator=g) < 0.3).to(DEV))
     Cl, cl = C.requires_grad_(True), c.requires_grad_(True)
     make = lambda: MPC(n, m, T, **kw)
-    dev = _run(monkeypatch, make, x0, QuadCost(Cl, cl), LinDx(F, f), True, grads=(Cl, cl))
-    host = _run(monkeypatch, make, x0, QuadCost(Cl, cl), LinDx(F, f), False, grads=(Cl, cl))
-    _bitwise(f"({n},{m}) {dtype} {case}", dev, host)
+    dev, host = same_on_both_loops(monkeypatch, make, x0, QuadCost(Cl, cl), LinDx(F, f), grads=(Cl, cl))
+    _same_full_du_norm(f"({n},{m}) {dtype} {case}", dev, host)
 
 
 @pytest.mark.parametrize("name", ["slew_box_f64", "slew_unb_f64"])
@@ -353,8 +296,8 @@ def test_slew_fixtures_as_lindx_on_the_device_loop(name, monkeypatch):
     F = torch.cat((g["A"], g["Bm"]), 1).expand(T - 1, B, n, p).to(DEV)
     make = lambda: MPC(n, m, T, lqr_iter=15, verbose=-1, exit_unconverged=False, detach_unconverged=False,
                        slew_rate_penalty=float(g["penalty"]), prev_ctrl=prev, eps=1e-9, **kw)
-    x, u, costs, _, _ = _run(monkeypatch, make, g["x_init"].to(DEV), QuadCost(g["C"].to(DEV), g["c"].to(DEV)),
-                             LinDx(F), True)
+    x, u, costs = solve_on(monkeypatch, make, g["x_init"].to(DEV), QuadCost(g["C"].to(DEV), g["c"].to(DEV)),
+                           LinDx(F), True)[:3]
     tol = 2e-4 if bound is not None else 1e-8
     assert maxdiff(u, g["u"]) < tol and maxdiff(x, g["x"]) < tol
     assert maxdiff(costs, g["costs"]) < 10 * tol * max(1.0, float(g["costs"].abs().max()))
@@ -382,12 +325,7 @@ def test_known_system_slew_matches_reference_fixture(name, bounds, monkeypatch):
                prev_ctrl=g["prev_ctrl"].to(DEV))
     C, x0 = g["C"].to(DEV), g["x_init"].to(DEV)
     c = g["c"].to(DEV).requires_grad_(True)
-    assert solver._use_slew_device_loop(ctrl, x0, QuadCost(C, c), dx, _u0(ctrl, x0))
-    ran = []
-    real = step.ilqr_raw
-    monkeypatch.setattr(step, "ilqr_raw", lambda *a, **k: ran.append(1) or real(*a, **k))
-    x, u, costs = ctrl(x0, QuadCost(C, c), dx)
-    assert ran == [1]
+    x, u, costs = solve_on(monkeypatch, lambda: ctrl, x0, QuadCost(C, c), dx, True)[:3]
     wx, wu, wc = g[f"x_{bounds}"], g[f"u_{bounds}"], g[f"costs_{bounds}"]
     tag = f"{name} bounds {bounds}"
     rel = (costs.detach().cpu() - wc).abs() / wc.abs().clamp_min(1.0)
