@@ -1,103 +1,64 @@
-// api.cu - the C ABI declared in include/mpcb200.h: argument checks, (n,m) dispatch, launch.
+// api.cu - the C ABI declared in include/mpcb200.h: argument checks, the table of compiled instances, launch.
+// Every entry point gathers its tensor pointers into one record (StepCall, IlqrCall), reads the developer knob once
+// (kernel_knob) and checks its arguments in one fixed order, so a malformed call gets the same code from each.
 #include <atomic>
 #include <cstdlib>
 #include <cstring>
 
 #include "../../../include/mpcb200.h"
 #include "ilqr.cuh"
-#include "lqr_grad.cuh"
+#include "instance.cuh"
 #include "lqr_large.cuh"
-#include "lqr_rollout.cuh"
-#include "lqr_step.cuh"
 #include "pnqp.cuh"
 
 namespace mpcb200 {
-#define MPCB200_INST(n, m)                                                  \
-  int step_f32__##n##_##m(const StepArgs&, int, cudaStream_t);              \
-  int step_f64__##n##_##m(const StepArgs&, int, cudaStream_t);              \
-  int grad_f32__##n##_##m(const GradArgs&, cudaStream_t);                   \
-  int grad_f64__##n##_##m(const GradArgs&, cudaStream_t);                   \
-  int pws_f32__##n##_##m(int, int);                                         \
-  int pws_f64__##n##_##m(int, int);                                         \
-  int roll_f32__##n##_##m(const RolloutArgs&, cudaStream_t);                \
-  int roll_f64__##n##_##m(const RolloutArgs&, cudaStream_t);                \
-  size_t smem_f32__##n##_##m(int);                                          \
-  size_t smem_f64__##n##_##m(int);
+#define MPCB200_INST(n, m) extern const Instance inst__##n##_##m;
+#define MPCB200_DYN_INST(kind, n, m) extern const Instance inst_dyn__##kind;
 #include "instances.def"
-#undef MPCB200_INST
-
-struct Entry {
-  int n, m;
-  int (*step32)(const StepArgs&, int, cudaStream_t);
-  int (*step64)(const StepArgs&, int, cudaStream_t);
-  int (*grad32)(const GradArgs&, cudaStream_t);
-  int (*grad64)(const GradArgs&, cudaStream_t);
-  size_t (*smem32)(int);
-  size_t (*smem64)(int);
-  int (*roll32)(const RolloutArgs&, cudaStream_t);
-  int (*roll64)(const RolloutArgs&, cudaStream_t);
-  int (*pws32)(int, int);
-  int (*pws64)(int, int);
-};
-static const Entry kTable[] = {
-#define MPCB200_INST(n, m)                                                                  \
-  {n, m, step_f32__##n##_##m, step_f64__##n##_##m, grad_f32__##n##_##m, grad_f64__##n##_##m, \
-   smem_f32__##n##_##m, smem_f64__##n##_##m, roll_f32__##n##_##m, roll_f64__##n##_##m,   \
-   pws_f32__##n##_##m, pws_f64__##n##_##m},
-#include "instances.def"
-#undef MPCB200_INST
-};
-static const int kTableLen = (int)(sizeof(kTable) / sizeof(kTable[0]));
-
-// dynamics-only step instances (inst_dyn.cu): no gradient or rollout kernels, and not listed by mpcb200_supported*
-#define MPCB200_DYN_INST(kind, n, m)                                        \
-  int dstep_f32__##kind(const StepArgs&, int, cudaStream_t);                \
-  int dstep_f64__##kind(const StepArgs&, int, cudaStream_t);                \
-  int dpws_f32__##kind(int, int);                                           \
-  int dpws_f64__##kind(int, int);                                           \
-  size_t dsmem_f32__##kind(int);                                            \
-  size_t dsmem_f64__##kind(int);
 #include "dyn_instances.def"
+#undef MPCB200_INST
 #undef MPCB200_DYN_INST
-struct DynEntry {
-  int kind;
-  Entry e;
-};
-static const DynEntry kDynTable[] = {
-#define MPCB200_DYN_INST(kind, n, m)                                                                        \
-  {kind, {n, m, dstep_f32__##kind, dstep_f64__##kind, nullptr, nullptr, dsmem_f32__##kind, dsmem_f64__##kind, \
-          nullptr, nullptr, dpws_f32__##kind, dpws_f64__##kind}},
+// every compiled instance: the (n, m) instances of instances.def in file order, then the dynamics-only step
+// instances (no gradient or rollout kernels, and not listed by mpcb200_supported*)
+static constexpr const Instance* kInstances[] = {
+#define MPCB200_INST(n, m) &inst__##n##_##m,
+#define MPCB200_DYN_INST(kind, n, m) &inst_dyn__##kind,
+#include "instances.def"
 #include "dyn_instances.def"
+#undef MPCB200_INST
 #undef MPCB200_DYN_INST
 };
 
-static const Entry* find(int n, int m) {
-  for (int i = 0; i < kTableLen; ++i)
-    if (kTable[i].n == n && kTable[i].m == m) return &kTable[i];
+static const Instance* find(int n, int m, int kind = DYN_LINEAR) {
+  for (const Instance* e : kInstances)
+    if (e->kind == kind && e->n == n && e->m == m) return e;
   return nullptr;
 }
 // the step instance of a call: the (n, m) instance, or for a passthrough kind its dynamics-only instance at exactly
 // that kind's (n, m)
-static const Entry* find_step(const mpcb200_dims* d) {
-  if ((d->dynamics_kind & DYN_CTRL_PASSTHROUGH) == 0) return find(d->n, d->m);
-  for (const DynEntry& de : kDynTable)
-    if (de.kind == d->dynamics_kind && de.e.n == d->n && de.e.m == d->m) return &de.e;
-  return nullptr;
+static const Instance* find_step(const mpcb200_dims* d) {
+  return find(d->n, d->m, (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0 ? d->dynamics_kind : DYN_LINEAR);
 }
 
-// developer A/B knob MPCB200_KERNEL=3: the large-shape kernels (lqr_large.cu) also for shapes with an instance
-static bool large_forced() {
+// The developer A/B knob MPCB200_KERNEL, read once per entry-point call (the tests flip it inside one process):
+// 0 or unset = the measured dispatch, 1 = the generic step kernel, 2 = the column-pair step kernel (StepArgs::impl),
+// 3 = the large-shape kernels (lqr_large.cu) also for linear-dynamics shapes that have an instance.
+static int kernel_knob() {
   const char* k = std::getenv("MPCB200_KERNEL");
-  return k != nullptr && std::atoi(k) == 3;
+  return k != nullptr ? std::atoi(k) : 0;
 }
 // the step, gradient and rollout of (n, m) run the large-shape kernels
-static bool runs_large(int n, int m) { return find(n, m) == nullptr || large_forced(); }
-static constexpr int kOptinAssumed = 227 * 1024;   // H100 opt-in shared memory per block, for device-free queries
+static bool runs_large(int n, int m, int knob) { return find(n, m) == nullptr || knob == 3; }
 
 static std::atomic<uint64_t> g_launches{0};
 static thread_local int t_step_plan = 0;      // MPCB200_PLAN_* bits of this thread's last step launch
 
 void record_step_plan(int plan) { t_step_plan = plan; }
+// counts the kernels of a launcher that returned rc
+static int counted(int rc, int kernels = 1) {
+  if (rc == 0) g_launches.fetch_add(kernels);
+  return rc;
+}
 
 // per-device opt-in shared memory limit (cached for up to 64 devices)
 int max_smem_optin() {
@@ -114,6 +75,10 @@ int max_smem_optin() {
   }
   return cache[dev].load(std::memory_order_acquire);
 }
+int smem_optin_or_h100() {
+  const int ms = max_smem_optin();
+  return ms > 0 ? ms : kOptinAssumed;
+}
 
 // element strides between the time slices of C, c, F and f.  Each *_tstride field of mpcb200_dims: 0 = dense (what a
 // zero-initialised mpcb200_dims means), < 0 = time invariant (stride 0), > 0 = that many elements
@@ -125,6 +90,11 @@ static TimeStrides time_strides(const mpcb200_dims* d) {
 }
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+template <typename R>
+static bool span16(long long elems) { return (elems * (long long)sizeof(R)) % 16 == 0; }
+// base (NULL counts as aligned) and time stride of one tensor of a step call are 16-byte aligned
+template <typename R>
+static bool tile_aligned(const R* base, long long tstride) { return aligned16(base) && span16<R>(tstride); }
 
 static int check_dims(const mpcb200_dims* d) {
   if (d == nullptr) return MPCB200_ERR_NULL_POINTER;
@@ -159,30 +129,39 @@ struct AdjExtra {      // fused-adjoint request riding on a step launch (api-int
   long long c_ts;
 };
 
+// the tensor arguments of mpcb200_lqr_step_*, in the header's order
 template <typename R>
-static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C, const R* c, const R* F,
-                     const R* f, const R* x_init, const R* cur_x, const R* cur_u, const R* u_lower,
-                     const R* u_upper, const uint8_t* u_zero_I, R* new_x, R* new_u, R* costs,
-                     R* full_du_norm, R* alphas, R* du_first, int32_t* qp_iters, uint8_t* free_mask, int32_t* status,
-                     R* Ks, R* ks, void* stream, const AdjExtra* adj = nullptr) {
+struct StepCall {
+  const R *C, *c, *F, *f, *x_init, *cur_x, *cur_u, *u_lower, *u_upper;
+  const uint8_t* u_zero_I;
+  R *new_x, *new_u, *costs, *full_du_norm, *alphas, *du_first;
+  int32_t* qp_iters;
+  uint8_t* free_mask;
+  int32_t* status;
+  R *Ks, *ks;
+};
+
+template <typename R>
+static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const StepCall<R>& s, int knob, void* stream,
+                     const AdjExtra* adj = nullptr) {
   int rc = check_dims(d);
   if (rc) return rc;
-  if (p == nullptr || C == nullptr || c == nullptr || cur_x == nullptr || cur_u == nullptr)
+  if (p == nullptr || s.C == nullptr || s.c == nullptr || s.cur_x == nullptr || s.cur_u == nullptr)
     return MPCB200_ERR_NULL_POINTER;
-  if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
-  rc = check_step_options(d, u_lower, u_upper, u_zero_I);
+  if (d->T > 1 && s.F == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (d->has_f && s.f == nullptr) return MPCB200_ERR_NULL_POINTER;
+  rc = check_step_options(d, s.u_lower, s.u_upper, s.u_zero_I);
   if (rc) return rc;
   if (d->do_rollout) {
-    if (x_init == nullptr || new_x == nullptr || new_u == nullptr || costs == nullptr ||
-        full_du_norm == nullptr || alphas == nullptr)
+    if (s.x_init == nullptr || s.new_x == nullptr || s.new_u == nullptr || s.costs == nullptr ||
+        s.full_du_norm == nullptr || s.alphas == nullptr)
       return MPCB200_ERR_NULL_POINTER;
-  } else if (Ks == nullptr || ks == nullptr) {
+  } else if (s.Ks == nullptr || s.ks == nullptr) {
     return MPCB200_ERR_NULL_POINTER;
   }
-  if ((Ks == nullptr) != (ks == nullptr)) return MPCB200_ERR_NULL_POINTER;
-  const Entry* e = find_step(d);
-  const bool large = d->dynamics_kind == DYN_LINEAR && runs_large(d->n, d->m);
+  if ((s.Ks == nullptr) != (s.ks == nullptr)) return MPCB200_ERR_NULL_POINTER;
+  const Instance* e = find_step(d);
+  const bool large = d->dynamics_kind == DYN_LINEAR && runs_large(d->n, d->m, knob);
   if (e == nullptr && !large) return MPCB200_ERR_UNSUPPORTED_DIMS;
   const int smem = max_smem_optin();
   if (smem <= 0) return MPCB200_ERR_NO_DEVICE;
@@ -198,22 +177,23 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
   a.pnqp_iters = d->pnqp_max_iter;
   a.do_rollout = d->do_rollout ? 1 : 0;
   a.u_lo = p->u_lo; a.u_hi = p->u_hi; a.delta_u = p->delta_u; a.ls_decay = p->ls_decay;
-  a.C = C; a.c = c; a.F = F; a.f = f; a.x_init = x_init; a.cur_x = cur_x; a.cur_u = cur_u;
-  a.u_lower = u_lower; a.u_upper = u_upper; a.zero_mask = u_zero_I;
-  a.new_x = new_x; a.new_u = new_u; a.costs = costs; a.full_du_norm = full_du_norm; a.alphas = alphas;
-  a.du_first = du_first; a.qp_iters = qp_iters; a.free_mask = free_mask; a.status = status; a.Ks = Ks; a.ks = ks;
-  // bulk-TMA eligibility: every per-time-step span must start 16-byte aligned
-  const size_t sz = sizeof(R);
-  bool ok = aligned16(C) && aligned16(c) && aligned16(cur_x) && aligned16(cur_u) &&
-            (F == nullptr || aligned16(F)) && (!d->has_f || aligned16(f)) &&
-            (d->bounds_kind != 2 || (aligned16(u_lower) && aligned16(u_upper)));
-  ok = ok && (x_init == nullptr || aligned16(x_init));
-  ok = ok && ((size_t)d->B * d->m * sz) % 16 == 0 && ((size_t)d->B * d->n * sz) % 16 == 0;
-  a.bulk_ok = ok ? 1 : 0;
+  a.C = s.C; a.c = s.c; a.F = s.F; a.f = s.f; a.x_init = s.x_init; a.cur_x = s.cur_x; a.cur_u = s.cur_u;
+  a.u_lower = s.u_lower; a.u_upper = s.u_upper; a.zero_mask = s.u_zero_I;
+  a.new_x = s.new_x; a.new_u = s.new_u; a.costs = s.costs; a.full_du_norm = s.full_du_norm; a.alphas = s.alphas;
+  a.du_first = s.du_first; a.qp_iters = s.qp_iters; a.free_mask = s.free_mask; a.status = s.status;
+  a.Ks = s.Ks; a.ks = s.ks;
   const TimeStrides ts = time_strides(d);
   a.C_ts = ts.C; a.c_ts = ts.c; a.F_ts = ts.F; a.f_ts = ts.f;
-  ok = ok && (a.C_ts * sz) % 16 == 0 && (a.c_ts * sz) % 16 == 0 && (a.F_ts * sz) % 16 == 0 && (a.f_ts * sz) % 16 == 0;
-  a.bulk_ok = ok ? 1 : 0;
+  // Bulk-copy eligibility, per tensor: base and time stride 16-byte aligned (f, the tensor bounds: where the call
+  // has them).  The time stride of the batch-dense cur_x, cur_u and bounds is B*n, B*m elements.
+  const int n = d->n, m = d->m;
+  const long long Bn = (long long)d->B * n, Bm = (long long)d->B * m;
+  const bool al_C = tile_aligned(s.C, a.C_ts), al_c = tile_aligned(s.c, a.c_ts), al_F = tile_aligned(s.F, a.F_ts),
+             al_f = tile_aligned(d->has_f ? s.f : nullptr, a.f_ts), al_x = tile_aligned(s.cur_x, Bn),
+             al_u = tile_aligned(s.cur_u, Bm),
+             al_box = d->bounds_kind != 2 || (tile_aligned(s.u_lower, Bm) && tile_aligned(s.u_upper, Bm));
+  // the instance kernels copy batch-wide spans of every tensor, or none
+  a.bulk_ok = al_C && al_c && al_F && al_f && al_x && al_u && al_box && aligned16(s.x_init);
   a.dyn_kind = d->dynamics_kind;
   if (a.dyn_kind != DYN_LINEAR) {
     if (!known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
@@ -222,51 +202,44 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C,
   if (large) {
     // the fused adjoint has no large-shape kernel: adjoint_impl then takes its three-launch route
     if (adj != nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
-    if (Ks == nullptr) return MPCB200_ERR_SMEM;      // the gains always go through the caller's Ks/ks
-    const int n = d->n, m = d->m, p = n + m;
-    auto spans = [&](const void* base, long long ts, long long span) {
-      return base != nullptr && aligned16(base) && (ts * (long long)sz) % 16 == 0 && (span * (long long)sz) % 16 == 0;
-    };
+    if (s.Ks == nullptr) return MPCB200_ERR_SMEM;      // the gains always go through the caller's Ks/ks
+    // the large-shape kernel copies per-problem spans, tensor by tensor: their lengths must be 16-byte multiples too
+    const long long pp = n + m;
     unsigned bulk = 0u;
-    if (spans(C, a.C_ts, (long long)p * p)) bulk |= LB_C;
-    if (spans(F, a.F_ts, (long long)n * p)) bulk |= LB_F;
-    if (spans(c, a.c_ts, p)) bulk |= LB_c;
-    if (d->has_f && spans(f, a.f_ts, n)) bulk |= LB_f;
-    if (spans(cur_x, (long long)d->B * n, n)) bulk |= LB_x;
-    if (spans(cur_u, (long long)d->B * m, m)) bulk |= LB_u;
-    if (d->bounds_kind == 2 && spans(u_lower, (long long)d->B * m, m) && spans(u_upper, (long long)d->B * m, m))
-      bulk |= LB_BOX;
+    if (al_C && span16<R>(pp * pp)) bulk |= LB_C;
+    if (s.F != nullptr && al_F && span16<R>(n * pp)) bulk |= LB_F;
+    if (al_c && span16<R>(pp)) bulk |= LB_c;
+    if (d->has_f && al_f && span16<R>(n)) bulk |= LB_f;
+    if (al_x && span16<R>(n)) bulk |= LB_x;
+    if (al_u && span16<R>(m)) bulk |= LB_u;
+    if (d->bounds_kind == 2 && al_box && span16<R>(m)) bulk |= LB_BOX;
     t_step_plan = 0;
-    rc = large_step_launch<R>(a, n, m, bulk, smem, (cudaStream_t)stream);
-    if (rc == 0) g_launches.fetch_add(1);
-    return rc;
+    return counted(large_step_launch<R>(a, n, m, bulk, smem, (cudaStream_t)stream));
   }
-  if (const char* k = std::getenv("MPCB200_KERNEL")) a.impl = std::atoi(k);
+  a.impl = knob;
   if (adj != nullptr) {          // fused KKT adjoint: column-pair kernel only
     if (!adj->ok || !a.bulk_ok || a.impl == 1) return MPCB200_ERR_UNSUPPORTED_DIMS;
     a.impl = 2;
     a.adj = 1; a.adj_has_df = adj->has_df; a.adj_c = adj->c; a.adj_x = adj->x; a.adj_u = adj->u;
     a.adj_dC = adj->dC; a.adj_dc = adj->dc; a.adj_dF = adj->dF; a.adj_df = adj->df; a.adj_dx_init = adj->dx_init;
     a.adj_c_ts = adj->c_ts;
-  }   // developer A/B knob: 1 generic, 2 pair
+  }
   t_step_plan = 0;             // the launcher that launches records its plan
-  rc =(sizeof(R) == 4 ? e->step32 : e->step64)(a, smem, (cudaStream_t)stream);
-  if (rc == 0) g_launches.fetch_add(1);
-  return rc;
+  return counted(e->ops[sizeof(R) == 8].step(a, smem, (cudaStream_t)stream));
 }
 
 template <typename R>
 static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, const R* new_x,
                      const R* new_u, const R* dx, const R* du, const R* dl_dx, R* dx_init, R* dC, R* dc,
-                     R* dF, R* df, void* workspace, void* stream) {
+                     R* dF, R* df, void* workspace, int knob, void* stream) {
   int rc = check_dims(d);
   if (rc) return rc;
   if (C == nullptr || c == nullptr || new_x == nullptr || new_u == nullptr || dx == nullptr ||
       du == nullptr || dl_dx == nullptr || dx_init == nullptr || dC == nullptr || dc == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (d->F_T > 0 && (F == nullptr || dF == nullptr)) return MPCB200_ERR_NULL_POINTER;
-  const Entry* e = find(d->n, d->m);
-  const bool large = runs_large(d->n, d->m);
+  const Instance* e = find(d->n, d->m);
+  const bool large = runs_large(d->n, d->m, knob);
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   GradArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -275,10 +248,9 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
   a.dx_init = dx_init; a.dC = dC; a.dc = dc; a.dF = dF; a.df = df; a.workspace = workspace;
   const TimeStrides ts = time_strides(d);
   a.C_ts = ts.C; a.c_ts = ts.c; a.F_ts = ts.F;
-  rc = large ? large_grad_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
-             : (sizeof(R) == 4 ? e->grad32 : e->grad64)(a, (cudaStream_t)stream);
-  if (rc == 0) g_launches.fetch_add(workspace != nullptr ? 2 : 1);
-  return rc;
+  return counted(large ? large_grad_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
+                       : e->ops[sizeof(R) == 8].grad(a, (cudaStream_t)stream),
+                 workspace != nullptr ? 2 : 1);
 }
 // ---------------------------------------------------------------------------------------------
 // KKT adjoint in one call (reference LQRStepFn.backward, mpc/lqr_step.py:312-407)
@@ -288,7 +260,7 @@ struct AdjLayout {                    // workspace carve-up (byte offsets, every
   bool gains;                         // Ks/ks of the nested solve (the large-shape step keeps its gains there)
 };
 static size_t up256(size_t v) { return (v + 255) / 256 * 256; }
-static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz) {
+static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz, int knob) {
   AdjLayout l;
   const size_t TB = (size_t)T * B;
   size_t o = 0;
@@ -300,7 +272,7 @@ static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz) {
   l.scal = o;    o += up256((size_t)3 * B * sz);
   l.mask = o;    o += up256(TB * m);
   l.maskf = o;   o += up256(TB * m * sz);                               // the same mask as element-typed 0/1 (rides on the TMA tile)
-  l.gains = runs_large(n, m);
+  l.gains = runs_large(n, m, knob);
   l.Ks = l.ks = 0;
   if (l.gains) {
     l.Ks = o;    o += up256(TB * m * n * sz);
@@ -340,7 +312,7 @@ template <typename R>
 static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C, const R* c, const R* F,
                         const R* new_x, const R* new_u, const R* dl_dx, const R* dl_du, const R* u_lower,
                         const R* u_upper, R* dx_init, R* dC, R* dc, R* dF, R* df, void* workspace,
-                        size_t workspace_bytes, void* stream) {
+                        size_t workspace_bytes, int knob, void* stream) {
   int rc = check_dims(d);
   if (rc) return rc;
   if (p == nullptr || C == nullptr || c == nullptr || new_x == nullptr || new_u == nullptr || dl_dx == nullptr ||
@@ -350,7 +322,7 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
   rc = check_bounds(d, u_lower, u_upper);
   if (rc) return rc;
   if (d->has_f && df == nullptr) return MPCB200_ERR_NULL_POINTER;
-  const AdjLayout l = adj_layout(d->B, d->T, d->n, d->m, sizeof(R));
+  const AdjLayout l = adj_layout(d->B, d->T, d->n, d->m, sizeof(R), knob);
   if (workspace_bytes < l.total || !aligned16(workspace)) return MPCB200_ERR_BAD_DIMS;
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
@@ -377,6 +349,9 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
   mpcb200_params ps;
   std::memset(&ps, 0, sizeof(ps));
   ps.ls_decay = 0.2;
+  StepCall<R> sc = {};
+  sc.C = C; sc.c = negr; sc.F = F; sc.x_init = z0; sc.cur_x = zx; sc.cur_u = zu; sc.u_zero_I = mask;
+  sc.new_x = dxs; sc.new_u = dus; sc.costs = scal; sc.full_du_norm = scal + d->B; sc.alphas = scal + 2 * d->B;
   // Preferred: ONE launch of the column-pair kernel doing solve + costates + outer products (C, F read from HBM
   // once, d tau kept in shared memory).  Shapes / alignments it does not take fall through to the 3-launch path.
   {
@@ -384,38 +359,35 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
     ax.c = c; ax.x = new_x; ax.u = new_u; ax.dC = dC; ax.dc = dc; ax.dF = dF; ax.df = d->has_f ? df : nullptr;
     ax.dx_init = dx_init; ax.has_df = d->has_f ? 1 : 0;
     ax.c_ts = time_strides(d).c;
-    ax.ok = aligned16(c) && aligned16(new_x) && aligned16(new_u) && (ax.c_ts * (long long)sizeof(R)) % 16 == 0;
-    const R* maskf = (const R*)(ws + l.maskf);
-    rc = step_impl<R>(&ds, &ps, C, negr, F, (const R*)nullptr, z0, zx, zu, maskf, maskf, mask,
-                      dxs, dus, scal, scal + d->B, scal + 2 * d->B, (R*)nullptr, (int32_t*)nullptr,
-                      (uint8_t*)nullptr, (int32_t*)nullptr, (R*)nullptr, (R*)nullptr, stream, &ax);
+    ax.ok = tile_aligned(c, ax.c_ts) && aligned16(new_x) && aligned16(new_u);
+    sc.u_lower = sc.u_upper = (const R*)(ws + l.maskf);     // the mask rides in the bounds' tile slots
+    rc = step_impl<R>(&ds, &ps, sc, knob, stream, &ax);
     if (rc == 0) return 0;
     if (rc != MPCB200_ERR_UNSUPPORTED_DIMS && rc != MPCB200_ERR_SMEM) return rc;
   }
   // 3-launch path: the nested solve really reads its (zero) nominal trajectory
   if (cudaMemsetAsync(zeros, 0, TB * (d->n + d->m) * sizeof(R), st) != cudaSuccess) return MPCB200_ERR_LAUNCH;
-  R* Ks = l.gains ? (R*)(ws + l.Ks) : nullptr;
-  R* ks = l.gains ? (R*)(ws + l.ks) : nullptr;
-  rc = step_impl<R>(&ds, &ps, C, negr, F, (const R*)nullptr, z0, zx, zu, (const R*)nullptr, (const R*)nullptr, mask,
-                    dxs, dus, scal, scal + d->B, scal + 2 * d->B, (R*)nullptr, (int32_t*)nullptr,
-                    (uint8_t*)nullptr, (int32_t*)nullptr, Ks, ks, stream);
-  if (rc == MPCB200_ERR_SMEM) return rc;     // long horizons: use the two-call path with Ks/ks buffers
-  if (rc) return rc;
-  mpcb200_dims dg = *d;
-  return grad_impl<R>(&dg, C, c, F, new_x, new_u, dxs, dus, dl_dx, dx_init, dC, dc, dF, d->has_f ? df : (R*)nullptr,
-                      ws + l.costate, stream);
+  sc.u_lower = sc.u_upper = nullptr;
+  if (l.gains) {
+    sc.Ks = (R*)(ws + l.Ks);
+    sc.ks = (R*)(ws + l.ks);
+  }
+  rc = step_impl<R>(&ds, &ps, sc, knob, stream);
+  if (rc) return rc;               // MPCB200_ERR_SMEM at long horizons: use the two-call path with Ks/ks buffers
+  return grad_impl<R>(d, C, c, F, new_x, new_u, dxs, dus, dl_dx, dx_init, dC, dc, dF, d->has_f ? df : (R*)nullptr,
+                      ws + l.costate, knob, stream);
 }
 
 template <typename R>
-static int rollout_impl(const mpcb200_dims* d, const R* F, const R* f, const R* x_init, const R* u, R* x,
+static int rollout_impl(const mpcb200_dims* d, const R* F, const R* f, const R* x_init, const R* u, R* x, int knob,
                         void* stream) {
   int rc = check_dims(d);
   if (rc) return rc;
   if (x_init == nullptr || u == nullptr || x == nullptr) return MPCB200_ERR_NULL_POINTER;
   if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
   if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
-  const Entry* e = find(d->n, d->m);
-  const bool large = runs_large(d->n, d->m);
+  const Instance* e = find(d->n, d->m);
+  const bool large = runs_large(d->n, d->m, knob);
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   RolloutArgs a;
   std::memset(&a, 0, sizeof(a));
@@ -423,10 +395,8 @@ static int rollout_impl(const mpcb200_dims* d, const R* F, const R* f, const R* 
   a.F = F; a.f = f; a.x_init = x_init; a.u = u; a.x = x;
   const TimeStrides ts = time_strides(d);
   a.F_ts = ts.F; a.f_ts = ts.f;
-  rc = large ? large_rollout_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
-             : (sizeof(R) == 4 ? e->roll32 : e->roll64)(a, (cudaStream_t)stream);
-  if (rc == 0) g_launches.fetch_add(1);
-  return rc;
+  return counted(large ? large_rollout_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
+                       : e->ops[sizeof(R) == 8].rollout(a, (cudaStream_t)stream));
 }
 template <typename R>
 static int dyn_impl(bool linearize, int kind, const double* dyn, int B, int T, const R* x_or_init, const R* u,
@@ -454,6 +424,15 @@ static int dyn_impl(bool linearize, int kind, const double* dyn, int B, int T, c
   return rc;
 }
 
+// whether the step of `d` keeps its gains in the caller's Ks/ks (mpcb200_step_prefers_workspace)
+static int gains_in_workspace(const mpcb200_dims* d, int elem_size, int knob) {
+  const bool passthrough = (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0;
+  if (!passthrough && runs_large(d->n, d->m, knob)) return 1;   // the large-shape step keeps its gains in Ks/ks
+  const Instance* e = find_step(d);
+  if (e == nullptr) return 1;                   // no instance: the step call itself reports it
+  return e->ops[elem_size == 8].prefers_workspace(d->T, smem_optin_or_h100());
+}
+
 // ---------------------------------------------------------------------------------------------
 // the iLQR loop of MPC.forward as one CUDA graph (reference mpc/mpc.py:244-301)
 // ---------------------------------------------------------------------------------------------
@@ -471,7 +450,7 @@ struct IlqrLayout {                   // workspace carve-up (byte offsets, every
   size_t u, x, new_x, new_u, costs, fdn_step, alphas, du_first, status, fdn, flags, state, F, f, Ks, ks, total;
   bool gains;
 };
-static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz) {
+static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz, int knob) {
   IlqrLayout l;
   const size_t TB = (size_t)d->T * d->B, B = d->B;
   const size_t n = d->n, m = d->m;
@@ -495,7 +474,7 @@ static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz) {
     l.f = o;      o += up256(TB1 * n * sz);
   }
   const mpcb200_dims ds = ilqr_step_dims(d);
-  l.gains = mpcb200_step_prefers_workspace(&ds, (int32_t)sz) != 0;
+  l.gains = gains_in_workspace(&ds, (int)sz, knob) != 0;
   l.Ks = l.ks = 0;
   if (l.gains) {
     l.Ks = o;     o += up256(TB * m * n * sz);
@@ -505,29 +484,43 @@ static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz) {
   return l;
 }
 
+// the arguments of mpcb200_ilqr_*, in the header's order
+template <typename R>
+struct IlqrCall {
+  const mpcb200_dims* d;
+  const mpcb200_params* p;
+  const mpcb200_ilqr_opts* o;
+  const R *C, *c, *F, *f, *x_init, *u_init, *u_lower, *u_upper;
+  const uint8_t* u_zero_I;
+  R *best_x, *best_u, *best_costs, *best_fdn;
+  int32_t* info;
+  void* workspace;
+  size_t workspace_bytes;
+};
+
 // argument checks that need no device: every error is reported before anything is captured or launched
 template <typename R>
-static int ilqr_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_ilqr_opts* o, const R* C,
-                      const R* c, const R* F, const R* f, const R* x_init, const R* u_lower, const R* u_upper,
-                      const uint8_t* u_zero_I, const R* best_x, const R* best_u, const R* best_costs,
-                      const R* best_fdn, const int32_t* info, const void* workspace, size_t workspace_bytes) {
+static int ilqr_check(const IlqrCall<R>& q, int knob) {
+  const mpcb200_dims* d = q.d;
   int rc = check_dims(d);
   if (rc) return rc;
-  if (p == nullptr || o == nullptr || C == nullptr || c == nullptr || x_init == nullptr || best_x == nullptr ||
-      best_u == nullptr || best_costs == nullptr || best_fdn == nullptr || info == nullptr || workspace == nullptr)
+  if (q.p == nullptr || q.o == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr ||
+      q.best_x == nullptr || q.best_u == nullptr || q.best_costs == nullptr || q.best_fdn == nullptr ||
+      q.info == nullptr || q.workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
-  if (o->lqr_iter < 1 || o->m_ref < 1 || o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
+  if (q.o->lqr_iter < 1 || q.o->m_ref < 1 || q.o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
   if (d->dynamics_kind != DYN_LINEAR) {
     if (!known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
   } else {
-    if (d->T > 1 && F == nullptr) return MPCB200_ERR_NULL_POINTER;
-    if (d->has_f && f == nullptr) return MPCB200_ERR_NULL_POINTER;
+    if (d->T > 1 && q.F == nullptr) return MPCB200_ERR_NULL_POINTER;
+    if (d->has_f && q.f == nullptr) return MPCB200_ERR_NULL_POINTER;
   }
-  rc = check_step_options(d, u_lower, u_upper, u_zero_I);
+  rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I);
   if (rc) return rc;
   if (d->dynamics_kind != DYN_LINEAR && find_step(d) == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
-  const IlqrLayout l = ilqr_layout(d, sizeof(R));
-  if (workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
+  const IlqrLayout l = ilqr_layout(d, sizeof(R), knob);
+  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
 }
 
@@ -544,26 +537,19 @@ static cudaStream_t ilqr_stream(int which) {
 
 // Adds the init kernel and the `while` node (body recorded on `bs`) to the graph `os` is capturing.
 template <typename R>
-static int ilqr_record(cudaStream_t os, cudaStream_t bs, const mpcb200_dims* d, const mpcb200_params* p,
-                       const mpcb200_ilqr_opts* o, const R* C, const R* c, const R* F, const R* f, const R* x_init,
-                       const R* u_init, const R* u_lower, const R* u_upper, const uint8_t* u_zero_I, R* best_x,
-                       R* best_u, R* best_costs, R* best_fdn, int32_t* info, void* workspace) {
-  const IlqrLayout l = ilqr_layout(d, sizeof(R));
-  char* ws = (char*)workspace;
+static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, int knob) {
+  const mpcb200_dims* d = q.d;
+  const mpcb200_ilqr_opts* o = q.o;
+  const IlqrLayout l = ilqr_layout(d, sizeof(R), knob);
+  char* ws = (char*)q.workspace;
   R* u = (R*)(ws + l.u);
   R* x = (R*)(ws + l.x);
-  R* new_x = (R*)(ws + l.new_x);
-  R* new_u = (R*)(ws + l.new_u);
-  R* costs = (R*)(ws + l.costs);
-  R* du_first = (R*)(ws + l.du_first);
-  int32_t* status = (int32_t*)(ws + l.status);
   R* fdn = (R*)(ws + l.fdn);
   uint8_t* flags = (uint8_t*)(ws + l.flags);
   IlqrState* st = (IlqrState*)(ws + l.state);
   const int B = d->B, T = d->T, N = d->n, M = d->m;
   const size_t TB = (size_t)T * B;
-  if (ilqr_launch_init<R>(TB * M, u_init, u, st, info, os) != 0) return MPCB200_ERR_LAUNCH;
-  g_launches.fetch_add(1);
+  if (counted(ilqr_launch_init<R>(TB * M, q.u_init, u, st, q.info, os)) != 0) return MPCB200_ERR_LAUNCH;
 
   cudaStreamCaptureStatus cst = cudaStreamCaptureStatusNone;
   cudaGraph_t g = nullptr;
@@ -594,44 +580,42 @@ static int ilqr_record(cudaStream_t os, cudaStream_t bs, const mpcb200_dims* d, 
                                     cudaStreamCaptureModeRelaxed) != cudaSuccess)
     return MPCB200_ERR_LAUNCH;
   const mpcb200_dims ds = ilqr_step_dims(d);
-  const R* Fs = F;
-  const R* fs = f;
+  StepCall<R> sc = {};
+  sc.C = q.C; sc.c = q.c; sc.F = q.F; sc.f = q.f; sc.x_init = q.x_init; sc.cur_x = x; sc.cur_u = u;
+  sc.u_lower = q.u_lower; sc.u_upper = q.u_upper; sc.u_zero_I = q.u_zero_I;
+  sc.new_x = (R*)(ws + l.new_x); sc.new_u = (R*)(ws + l.new_u); sc.costs = (R*)(ws + l.costs);
+  sc.full_du_norm = (R*)(ws + l.fdn_step); sc.alphas = (R*)(ws + l.alphas); sc.du_first = (R*)(ws + l.du_first);
+  sc.status = (int32_t*)(ws + l.status);
+  if (l.gains) {
+    sc.Ks = (R*)(ws + l.Ks);
+    sc.ks = (R*)(ws + l.ks);
+  }
   int rc;
   if (d->dynamics_kind == DYN_LINEAR) {
-    rc = rollout_impl<R>(d, F, f, x_init, u, x, bs);
-  } else {
-    R* Fw = (R*)(ws + l.F);
-    R* fw = (R*)(ws + l.f);
-    rc = dyn_impl<R>(false, d->dynamics_kind, p->dyn, B, T, x_init, u, x, nullptr, nullptr, bs);
-    if (rc == 0) rc = dyn_impl<R>(true, d->dynamics_kind, p->dyn, B, T, x, u, nullptr, Fw, fw, bs);
-    Fs = T > 1 ? Fw : nullptr;
-    fs = T > 1 ? fw : nullptr;
+    rc = rollout_impl<R>(d, q.F, q.f, q.x_init, u, x, knob, bs);
+  } else {                            // a known system: the step reads the workspace F, f, rewritten every iteration
+    sc.F = T > 1 ? (R*)(ws + l.F) : nullptr;
+    sc.f = T > 1 ? (R*)(ws + l.f) : nullptr;
+    rc = dyn_impl<R>(false, d->dynamics_kind, q.p->dyn, B, T, q.x_init, u, x, nullptr, nullptr, bs);
+    if (rc == 0)
+      rc = dyn_impl<R>(true, d->dynamics_kind, q.p->dyn, B, T, x, u, nullptr, (R*)(ws + l.F), (R*)(ws + l.f), bs);
   }
+  if (rc == 0) rc = step_impl<R>(&ds, q.p, sc, knob, bs);
   if (rc == 0)
-    rc = step_impl<R>(&ds, p, C, c, Fs, fs, x_init, x, u, u_lower, u_upper, u_zero_I, new_x, new_u, costs,
-                      (R*)(ws + l.fdn_step), (R*)(ws + l.alphas), du_first, (int32_t*)nullptr, (uint8_t*)nullptr,
-                      status, l.gains ? (R*)(ws + l.Ks) : (R*)nullptr, l.gains ? (R*)(ws + l.ks) : (R*)nullptr, bs);
+    rc = counted(ilqr_launch_track<R>(B, T, N, M, o->m_ref, (R)o->best_cost_eps, sc.new_x, sc.new_u, sc.costs,
+                                      sc.du_first, sc.status, q.best_costs, q.best_x, q.best_u, u, fdn, flags, st, bs));
   if (rc == 0)
-    rc = ilqr_launch_track<R>(B, T, N, M, o->m_ref, (R)o->best_cost_eps, new_x, new_u, costs, du_first, status,
-                              best_costs, best_x, best_u, u, fdn, flags, st, bs);
-  if (rc == 0) {
-    g_launches.fetch_add(1);
-    rc = ilqr_launch_stop<R>(B, o->lqr_iter, o->not_improved_lim, o->eps, costs, fdn, flags, best_costs, best_fdn, st,
-                             info, handle, bs);
-    if (rc == 0) g_launches.fetch_add(1);
-  }
+    rc = counted(ilqr_launch_stop<R>(B, o->lqr_iter, o->not_improved_lim, o->eps, sc.costs, fdn, flags, q.best_costs,
+                                     q.best_fdn, st, q.info, handle, bs));
   cudaGraph_t body = nullptr;
   if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
   return rc;
 }
 
 template <typename R>
-static int ilqr_impl(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_ilqr_opts* o, const R* C,
-                     const R* c, const R* F, const R* f, const R* x_init, const R* u_init, const R* u_lower,
-                     const R* u_upper, const uint8_t* u_zero_I, R* best_x, R* best_u, R* best_costs, R* best_fdn,
-                     int32_t* info, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = ilqr_check<R>(d, p, o, C, c, F, f, x_init, u_lower, u_upper, u_zero_I, best_x, best_u, best_costs,
-                         best_fdn, info, workspace, workspace_bytes);
+static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
+  const int knob = kernel_knob();
+  int rc = ilqr_check<R>(q, knob);
   if (rc) return rc;
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   int driver = 0;
@@ -644,30 +628,28 @@ static int ilqr_impl(const mpcb200_dims* d, const mpcb200_params* p, const mpcb2
   // the library's own graph and stream calls must not invalidate a capture the caller runs in global mode
   cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
   cudaThreadExchangeStreamCaptureMode(&mode);
+  // a caller that is not capturing gets a graph of the library's own: captured, instantiated and launched here
   cudaStream_t os = caller_captures ? st : ilqr_stream(0);
   cudaStream_t bs = ilqr_stream(1);
-  if (os == nullptr || bs == nullptr) {
-    rc = MPCB200_ERR_LAUNCH;
-  } else if (caller_captures) {
-    rc = ilqr_record<R>(os, bs, d, p, o, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
-                        best_costs, best_fdn, info, workspace);
-  } else if (cudaStreamBeginCapture(os, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
+  if (os == nullptr || bs == nullptr ||
+      (!caller_captures && cudaStreamBeginCapture(os, cudaStreamCaptureModeRelaxed) != cudaSuccess)) {
     rc = MPCB200_ERR_LAUNCH;
   } else {
-    rc = ilqr_record<R>(os, bs, d, p, o, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
-                        best_costs, best_fdn, info, workspace);
-    cudaGraph_t g = nullptr;
-    if (cudaStreamEndCapture(os, &g) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
-    if (rc == 0) {
-      cudaGraphExec_t exec = nullptr;
-      if (cudaGraphInstantiate(&exec, g, 0) != cudaSuccess) {
-        rc = MPCB200_ERR_LAUNCH;
-      } else {
-        if (cudaGraphLaunch(exec, st) != cudaSuccess) rc = MPCB200_ERR_LAUNCH;
-        cudaGraphExecDestroy(exec);        // released once the launch completes
+    rc = ilqr_record<R>(os, bs, q, knob);
+    if (!caller_captures) {
+      cudaGraph_t g = nullptr;
+      if (cudaStreamEndCapture(os, &g) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+      if (rc == 0) {
+        cudaGraphExec_t exec = nullptr;
+        if (cudaGraphInstantiate(&exec, g, 0) != cudaSuccess) {
+          rc = MPCB200_ERR_LAUNCH;
+        } else {
+          if (cudaGraphLaunch(exec, st) != cudaSuccess) rc = MPCB200_ERR_LAUNCH;
+          cudaGraphExecDestroy(exec);        // released once the launch completes
+        }
       }
+      if (g != nullptr) cudaGraphDestroy(g);
     }
-    if (g != nullptr) cudaGraphDestroy(g);
   }
   cudaThreadExchangeStreamCaptureMode(&mode);
   if (rc) cudaGetLastError();              // a failed build leaves no sticky launch error behind
@@ -685,9 +667,10 @@ int mpcb200_lqr_step_f32(const mpcb200_dims* dims, const mpcb200_params* params,
                          const float* u_upper, const uint8_t* u_zero_I, float* new_x, float* new_u,
                          float* costs, float* full_du_norm, float* alphas, float* du_first, int32_t* qp_iters,
                          uint8_t* free_mask, int32_t* status, float* Ks, float* ks, void* stream) {
-  return step_impl<float>(dims, params, C, c, F, f, x_init, cur_x, cur_u, u_lower, u_upper, u_zero_I,
-                          new_x, new_u, costs, full_du_norm, alphas, du_first, qp_iters, free_mask, status, Ks, ks,
-                          stream);
+  return step_impl<float>(dims, params,
+                          {C, c, F, f, x_init, cur_x, cur_u, u_lower, u_upper, u_zero_I, new_x, new_u, costs,
+                           full_du_norm, alphas, du_first, qp_iters, free_mask, status, Ks, ks},
+                          kernel_knob(), stream);
 }
 int mpcb200_lqr_step_f64(const mpcb200_dims* dims, const mpcb200_params* params, const double* C,
                          const double* c, const double* F, const double* f, const double* x_init,
@@ -695,26 +678,29 @@ int mpcb200_lqr_step_f64(const mpcb200_dims* dims, const mpcb200_params* params,
                          const double* u_upper, const uint8_t* u_zero_I, double* new_x, double* new_u,
                          double* costs, double* full_du_norm, double* alphas, double* du_first, int32_t* qp_iters,
                          uint8_t* free_mask, int32_t* status, double* Ks, double* ks, void* stream) {
-  return step_impl<double>(dims, params, C, c, F, f, x_init, cur_x, cur_u, u_lower, u_upper, u_zero_I,
-                           new_x, new_u, costs, full_du_norm, alphas, du_first, qp_iters, free_mask, status, Ks, ks,
-                           stream);
+  return step_impl<double>(dims, params,
+                           {C, c, F, f, x_init, cur_x, cur_u, u_lower, u_upper, u_zero_I, new_x, new_u, costs,
+                            full_du_norm, alphas, du_first, qp_iters, free_mask, status, Ks, ks},
+                           kernel_knob(), stream);
 }
 int mpcb200_lqr_grad_f32(const mpcb200_dims* dims, const float* C, const float* c, const float* F,
                          const float* new_x, const float* new_u, const float* dx, const float* du,
                          const float* dl_dx, float* dx_init, float* dC, float* dc, float* dF, float* df,
                          void* workspace, void* stream) {
-  return grad_impl<float>(dims, C, c, F, new_x, new_u, dx, du, dl_dx, dx_init, dC, dc, dF, df, workspace, stream);
+  return grad_impl<float>(dims, C, c, F, new_x, new_u, dx, du, dl_dx, dx_init, dC, dc, dF, df, workspace,
+                          kernel_knob(), stream);
 }
 int mpcb200_lqr_grad_f64(const mpcb200_dims* dims, const double* C, const double* c, const double* F,
                          const double* new_x, const double* new_u, const double* dx, const double* du,
                          const double* dl_dx, double* dx_init, double* dC, double* dc, double* dF,
                          double* df, void* workspace, void* stream) {
-  return grad_impl<double>(dims, C, c, F, new_x, new_u, dx, du, dl_dx, dx_init, dC, dc, dF, df, workspace, stream);
+  return grad_impl<double>(dims, C, c, F, new_x, new_u, dx, du, dl_dx, dx_init, dC, dc, dF, df, workspace,
+                           kernel_knob(), stream);
 }
 
 size_t mpcb200_adjoint_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
-  return adj_layout(dims->B, dims->T, dims->n, dims->m, (size_t)elem_size).total;
+  return adj_layout(dims->B, dims->T, dims->n, dims->m, (size_t)elem_size, kernel_knob()).total;
 }
 int mpcb200_lqr_adjoint_f32(const mpcb200_dims* dims, const mpcb200_params* params, const float* C, const float* c,
                             const float* F, const float* new_x, const float* new_u, const float* dl_dx,
@@ -722,7 +708,7 @@ int mpcb200_lqr_adjoint_f32(const mpcb200_dims* dims, const mpcb200_params* para
                             float* dC, float* dc, float* dF, float* df, void* workspace, size_t workspace_bytes,
                             void* stream) {
   return adjoint_impl<float>(dims, params, C, c, F, new_x, new_u, dl_dx, dl_du, u_lower, u_upper, dx_init, dC, dc,
-                             dF, df, workspace, workspace_bytes, stream);
+                             dF, df, workspace, workspace_bytes, kernel_knob(), stream);
 }
 int mpcb200_lqr_adjoint_f64(const mpcb200_dims* dims, const mpcb200_params* params, const double* C, const double* c,
                             const double* F, const double* new_x, const double* new_u, const double* dl_dx,
@@ -730,16 +716,16 @@ int mpcb200_lqr_adjoint_f64(const mpcb200_dims* dims, const mpcb200_params* para
                             double* dC, double* dc, double* dF, double* df, void* workspace, size_t workspace_bytes,
                             void* stream) {
   return adjoint_impl<double>(dims, params, C, c, F, new_x, new_u, dl_dx, dl_du, u_lower, u_upper, dx_init, dC, dc,
-                              dF, df, workspace, workspace_bytes, stream);
+                              dF, df, workspace, workspace_bytes, kernel_knob(), stream);
 }
 
 int mpcb200_rollout_f32(const mpcb200_dims* dims, const float* F, const float* f, const float* x_init,
                         const float* u, float* x, void* stream) {
-  return rollout_impl<float>(dims, F, f, x_init, u, x, stream);
+  return rollout_impl<float>(dims, F, f, x_init, u, x, kernel_knob(), stream);
 }
 int mpcb200_rollout_f64(const mpcb200_dims* dims, const double* F, const double* f, const double* x_init,
                         const double* u, double* x, void* stream) {
-  return rollout_impl<double>(dims, F, f, x_init, u, x, stream);
+  return rollout_impl<double>(dims, F, f, x_init, u, x, kernel_knob(), stream);
 }
 
 int mpcb200_dyn_rollout_f32(int32_t kind, const double* dyn, int32_t B, int32_t T, const float* x_init,
@@ -762,53 +748,52 @@ int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_
 size_t mpcb200_ilqr_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
   if (dims == nullptr || opts == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
   if (dims->dynamics_kind != DYN_LINEAR && !known_shape_ok(dims)) return 0;
-  return ilqr_layout(dims, (size_t)elem_size).total;
+  return ilqr_layout(dims, (size_t)elem_size, kernel_knob()).total;
 }
 int mpcb200_ilqr_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
                      const float* C, const float* c, const float* F, const float* f, const float* x_init,
                      const float* u_init, const float* u_lower, const float* u_upper, const uint8_t* u_zero_I,
                      float* best_x, float* best_u, float* best_costs, float* best_full_du_norm, int32_t* info,
                      void* workspace, size_t workspace_bytes, void* stream) {
-  return ilqr_impl<float>(dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
-                          best_costs, best_full_du_norm, info, workspace, workspace_bytes, stream);
+  return ilqr_impl<float>({dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
+                           best_costs, best_full_du_norm, info, workspace, workspace_bytes},
+                          stream);
 }
 int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
                      const double* C, const double* c, const double* F, const double* f, const double* x_init,
                      const double* u_init, const double* u_lower, const double* u_upper, const uint8_t* u_zero_I,
                      double* best_x, double* best_u, double* best_costs, double* best_full_du_norm, int32_t* info,
                      void* workspace, size_t workspace_bytes, void* stream) {
-  return ilqr_impl<double>(dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
-                           best_costs, best_full_du_norm, info, workspace, workspace_bytes, stream);
+  return ilqr_impl<double>({dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
+                            best_costs, best_full_du_norm, info, workspace, workspace_bytes},
+                           stream);
 }
 
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }
 
 int mpcb200_supported_list(int32_t* out, int32_t cap) {
-  for (int i = 0; i < kTableLen && i < cap; ++i) {
-    out[2 * i] = kTable[i].n;
-    out[2 * i + 1] = kTable[i].m;
+  int count = 0;
+  for (const Instance* e : kInstances) {
+    if (e->kind != DYN_LINEAR) continue;
+    if (count < cap) {
+      out[2 * count] = e->n;
+      out[2 * count + 1] = e->m;
+    }
+    ++count;
   }
-  return kTableLen;
+  return count;
 }
 
 uint64_t mpcb200_launch_count(void) { return g_launches.load(); }
 
 size_t mpcb200_step_smem_bytes(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr) return 0;
-  const Entry* e = find_step(dims);
-  if (e == nullptr) return 0;
-  return elem_size == 8 ? e->smem64(dims->T) : e->smem32(dims->T);
+  const Instance* e = find_step(dims);
+  return e == nullptr ? 0 : e->ops[elem_size == 8].smem_bytes(dims->T);
 }
 
 int mpcb200_step_prefers_workspace(const mpcb200_dims* dims, int32_t elem_size) {
-  if (dims == nullptr) return 0;
-  const bool passthrough = (dims->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0;
-  if (!passthrough && runs_large(dims->n, dims->m)) return 1;   // the large-shape step keeps its gains in Ks/ks
-  const Entry* e = find_step(dims);
-  if (e == nullptr) return 1;                   // no instance: the step call itself reports it
-  int ms = max_smem_optin();
-  if (ms <= 0) ms = kOptinAssumed;    // no device visible (CPU-side query): assume H100's opt-in limit
-  return elem_size == 8 ? e->pws64(dims->T, ms) : e->pws32(dims->T, ms);
+  return dims == nullptr ? 0 : gains_in_workspace(dims, elem_size, kernel_knob());
 }
 
 int mpcb200_step_large_fits(const mpcb200_dims* dims, int32_t elem_size) {

@@ -73,6 +73,9 @@ MPCB_DEV void named_bar_sync(int id, int nthreads) {
   asm volatile("barrier.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// H100 opt-in shared memory per block, what the device-free queries assume when no device is visible
+constexpr int kOptinAssumed = 227 * 1024;
+
 // Raise Kern's opt-in dynamic shared-memory limit to max_smem_optin, once per device (the attribute is per
 // context).  Keyed on the kernel itself: instances of one template have the same type.  Atomic flags:
 // concurrent callers (one host thread per GPU is the expected pattern) may both set the attribute, which is

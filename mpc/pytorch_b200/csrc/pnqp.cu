@@ -93,8 +93,6 @@ int mpcb200_pnqp_f64(int32_t B, int32_t n, const double* H, const double* q, con
 }
 int32_t mpcb200_pnqp_max_n(int32_t elem_size) {
   if (elem_size != 4 && elem_size != 8) return 0;
-  int ms = mpcb200::max_smem_optin();
-  if (ms <= 0) ms = 227 * 1024;       // no device visible (CPU-side query): assume H100's opt-in limit
-  return mpcb200::pnqp_max_n(elem_size, ms);
+  return mpcb200::pnqp_max_n(elem_size, mpcb200::smem_optin_or_h100());
 }
 }

@@ -17,6 +17,8 @@ struct PnqpArgs {
 
 // opt-in dynamic shared memory per block of the current device (bytes); <= 0 if no usable sm_90 device (api.cu)
 int max_smem_optin();
+// the same for a query that must answer without a device: the H100's limit (kOptinAssumed) when none is usable
+int smem_optin_or_h100();
 
 // dynamic shared memory (bytes) of the CTA-per-QP kernel for an n x n QP of elem_size-byte elements
 size_t pnqp_cta_smem_bytes(int n, int elem_size);
