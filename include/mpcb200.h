@@ -301,6 +301,39 @@ int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, con
                      double* best_x, double* best_u, double* best_costs, double* best_full_du_norm,
                      int32_t* info, void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * A receding-horizon MPC episode on the device: for k = 0 .. n_steps-1, solve the problem from state x_k with warm
+ * start w_k exactly as mpcb200_ilqr_* does (same dims, params, opts and inputs), apply u_k = best_u[0], step the
+ * model to x_{k+1}, and shift the warm start.
+ *   x_0 = x_init;  w_0 = u_init[T,B,m] or zeros;
+ *   x_{k+1} = the rollout of the problem's own dynamics over the two steps (x_k, best_u[0:2]), at t = 1: for LinDx
+ *             F[0] [x_k; u_k] + f[0] (exact for a time-invariant system), for a known system one step of it
+ *             (params->dyn).  For a slew-rate augmented problem the state is [u_{t-1}; x] and the passthrough makes
+ *             it [u_k; x_{k+1}];
+ *   w_{k+1} = cat(best_u[1:], 0) with then w_{k+1}[T-2] = w_{k+1}[T-3], controls past opts->m_ref at 0.
+ * Outputs xs[n_steps+1,B,n] (xs[0] = x_init), us[n_steps,B,m], costs[n_steps,B] (best_costs of each solve),
+ * info[n_steps,2] (int32, each solve's info) and u_next[T,B,m] = w_{n_steps}, which continues the episode as the
+ * u_init of a later call.  Needs T >= 3 and n_steps >= 1 (else MPCB200_ERR_BAD_DIMS).
+ * One CUDA graph: an init kernel, then a conditional `while` node over control steps whose body is the iLQR loop's
+ * init kernel and `while` node, the model step (mpcb200_rollout_* or mpcb200_dyn_rollout_* at T = 2) and an advance
+ * kernel that writes the outputs and ends the loop after n_steps steps.  Capture contract, launch counting and
+ * MPCB200_ERR_NO_GRAPH_COND (also for a driver that refuses a conditional node inside a conditional body) as for
+ * mpcb200_ilqr_*.  workspace: mpcb200_episode_workspace_bytes() bytes, 256-byte aligned, undefined on return.
+ */
+size_t mpcb200_episode_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size);
+int mpcb200_episode_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                        int32_t n_steps, const float* C, const float* c, const float* F, const float* f,
+                        const float* x_init, const float* u_init,
+                        const float* u_lower, const float* u_upper, const uint8_t* u_zero_I,
+                        float* xs, float* us, float* costs, int32_t* info, float* u_next,
+                        void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                        int32_t n_steps, const double* C, const double* c, const double* F, const double* f,
+                        const double* x_init, const double* u_init,
+                        const double* u_lower, const double* u_upper, const uint8_t* u_zero_I,
+                        double* xs, double* us, double* costs, int32_t* info, double* u_next,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);
 

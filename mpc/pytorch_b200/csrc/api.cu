@@ -525,14 +525,58 @@ static int ilqr_check(const IlqrCall<R>& q, int knob) {
 }
 
 // Library-owned streams of this thread on the current device: [0] records a graph the caller does not capture,
-// [1] records the loop body.  Capture only records work on them; nothing ever executes on them.
+// [1] records the iLQR loop body, [2] the body of an episode's loop over control steps.  Capture only records work
+// on them; nothing ever executes on them.
 static cudaStream_t ilqr_stream(int which) {
-  static thread_local cudaStream_t streams[64][2] = {};
+  static thread_local cudaStream_t streams[64][3] = {};
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
   cudaStream_t& s = streams[dev][which];
   if (s == nullptr && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) s = nullptr;
   return s;
+}
+
+// A conditional handle in the graph `os` is capturing: the graph of a top-level capture, or the body of an enclosing
+// loop.  MPCB200_ERR_NO_GRAPH_COND when the driver refuses it.
+static int while_handle(cudaStream_t os, cudaGraphConditionalHandle* handle) {
+  cudaStreamCaptureStatus cst = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  if (cudaStreamGetCaptureInfo(os, &cst, nullptr, &g, nullptr, nullptr) != cudaSuccess ||
+      cst != cudaStreamCaptureStatusActive)
+    return MPCB200_ERR_LAUNCH;
+  if (cudaGraphConditionalHandleCreate(handle, g, 1, cudaGraphCondAssignDefault) != cudaSuccess) {
+    cudaGetLastError();
+    return MPCB200_ERR_NO_GRAPH_COND;
+  }
+  return MPCB200_OK;
+}
+
+// Adds a `while` node on `handle` after the work captured on `os` so far and starts recording its body on `bs`
+// (which the caller ends with cudaStreamEndCapture).  MPCB200_ERR_NO_GRAPH_COND when the driver refuses the node,
+// e.g. a conditional node inside a conditional body.
+static int open_while(cudaStream_t os, cudaStream_t bs, cudaGraphConditionalHandle handle) {
+  cudaStreamCaptureStatus cst = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t ndeps = 0;
+  if (cudaStreamGetCaptureInfo(os, &cst, nullptr, &g, &deps, &ndeps) != cudaSuccess ||
+      cst != cudaStreamCaptureStatusActive)
+    return MPCB200_ERR_LAUNCH;
+  cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
+  np.conditional.handle = handle;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  cudaGraphNode_t loop;
+  if (cudaGraphAddNode(&loop, g, deps, ndeps, &np) != cudaSuccess) {
+    cudaGetLastError();
+    return MPCB200_ERR_NO_GRAPH_COND;
+  }
+  if (cudaStreamUpdateCaptureDependencies(os, &loop, 1, cudaStreamSetCaptureDependencies) != cudaSuccess)
+    return MPCB200_ERR_LAUNCH;
+  if (cudaStreamBeginCaptureToGraph(bs, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                    cudaStreamCaptureModeRelaxed) != cudaSuccess)
+    return MPCB200_ERR_LAUNCH;
+  return MPCB200_OK;
 }
 
 // Adds the init kernel and the `while` node (body recorded on `bs`) to the graph `os` is capturing.
@@ -549,36 +593,13 @@ static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, i
   IlqrState* st = (IlqrState*)(ws + l.state);
   const int B = d->B, T = d->T, N = d->n, M = d->m;
   const size_t TB = (size_t)T * B;
-  if (counted(ilqr_launch_init<R>(TB * M, q.u_init, u, st, q.info, os)) != 0) return MPCB200_ERR_LAUNCH;
-
-  cudaStreamCaptureStatus cst = cudaStreamCaptureStatusNone;
-  cudaGraph_t g = nullptr;
-  const cudaGraphNode_t* deps = nullptr;
-  size_t ndeps = 0;
-  if (cudaStreamGetCaptureInfo(os, &cst, nullptr, &g, &deps, &ndeps) != cudaSuccess ||
-      cst != cudaStreamCaptureStatusActive)
-    return MPCB200_ERR_LAUNCH;
   cudaGraphConditionalHandle handle;
-  if (cudaGraphConditionalHandleCreate(&handle, g, 1, cudaGraphCondAssignDefault) != cudaSuccess) {
-    cudaGetLastError();
-    return MPCB200_ERR_NO_GRAPH_COND;
-  }
-  cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
-  np.conditional.handle = handle;
-  np.conditional.type = cudaGraphCondTypeWhile;
-  np.conditional.size = 1;
-  cudaGraphNode_t loop;
-  if (cudaGraphAddNode(&loop, g, deps, ndeps, &np) != cudaSuccess) {
-    cudaGetLastError();
-    return MPCB200_ERR_NO_GRAPH_COND;
-  }
-  if (cudaStreamUpdateCaptureDependencies(os, &loop, 1, cudaStreamSetCaptureDependencies) != cudaSuccess)
-    return MPCB200_ERR_LAUNCH;
-
+  int rc = while_handle(os, &handle);
+  if (rc) return rc;
+  if (counted(ilqr_launch_init<R>(TB * M, q.u_init, u, st, q.info, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
   // the body: the library's own launchers, recorded on bs (same plan selection as a direct call)
-  if (cudaStreamBeginCaptureToGraph(bs, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
-                                    cudaStreamCaptureModeRelaxed) != cudaSuccess)
-    return MPCB200_ERR_LAUNCH;
+  rc = open_while(os, bs, handle);
+  if (rc) return rc;
   const mpcb200_dims ds = ilqr_step_dims(d);
   StepCall<R> sc = {};
   sc.C = q.C; sc.c = q.c; sc.F = q.F; sc.f = q.f; sc.x_init = q.x_init; sc.cur_x = x; sc.cur_u = u;
@@ -590,7 +611,6 @@ static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, i
     sc.Ks = (R*)(ws + l.Ks);
     sc.ks = (R*)(ws + l.ks);
   }
-  int rc;
   if (d->dynamics_kind == DYN_LINEAR) {
     rc = rollout_impl<R>(d, q.F, q.f, q.x_init, u, x, knob, bs);
   } else {                            // a known system: the step reads the workspace F, f, rewritten every iteration
@@ -612,12 +632,11 @@ static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, i
   return rc;
 }
 
-template <typename R>
-static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
-  const int knob = kernel_knob();
-  int rc = ilqr_check<R>(q, knob);
-  if (rc) return rc;
-  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+// Runs `record(os)`, which adds a solve's nodes to the graph `os` is capturing, with the capture contract of
+// mpcb200_ilqr_*: on a capturing `stream` the nodes join the caller's graph and nothing is launched; otherwise the
+// graph is captured on a library stream, instantiated, launched on `stream` and destroyed.
+template <typename Record>
+static int run_graph(void* stream, Record&& record) {
   int driver = 0;
   if (cudaDriverGetVersion(&driver) != cudaSuccess || driver < 12030) return MPCB200_ERR_NO_GRAPH_COND;
   cudaStream_t st = (cudaStream_t)stream;
@@ -630,12 +649,12 @@ static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
   cudaThreadExchangeStreamCaptureMode(&mode);
   // a caller that is not capturing gets a graph of the library's own: captured, instantiated and launched here
   cudaStream_t os = caller_captures ? st : ilqr_stream(0);
-  cudaStream_t bs = ilqr_stream(1);
-  if (os == nullptr || bs == nullptr ||
+  int rc;
+  if (os == nullptr ||
       (!caller_captures && cudaStreamBeginCapture(os, cudaStreamCaptureModeRelaxed) != cudaSuccess)) {
     rc = MPCB200_ERR_LAUNCH;
   } else {
-    rc = ilqr_record<R>(os, bs, q, knob);
+    rc = record(os);
     if (!caller_captures) {
       cudaGraph_t g = nullptr;
       if (cudaStreamEndCapture(os, &g) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
@@ -654,6 +673,143 @@ static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
   cudaThreadExchangeStreamCaptureMode(&mode);
   if (rc) cudaGetLastError();              // a failed build leaves no sticky launch error behind
   return rc;
+}
+
+template <typename R>
+static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
+  const int knob = kernel_knob();
+  int rc = ilqr_check<R>(q, knob);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t bs = ilqr_stream(1);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH : ilqr_record<R>(os, bs, q, knob);
+  });
+}
+
+// ---------------------------------------------------------------------------------------------
+// a receding-horizon episode as one CUDA graph: solve, apply, shift and re-solve, n_steps times
+// ---------------------------------------------------------------------------------------------
+struct EpisodeLayout {                // workspace carve-up: the iLQR loop's workspace, then the episode's buffers
+  IlqrLayout ilqr;
+  size_t best_x, best_u, best_costs, best_fdn, info, state, warm, traj, ep, total;
+};
+static EpisodeLayout episode_layout(const mpcb200_dims* d, size_t sz, int knob) {
+  EpisodeLayout l;
+  l.ilqr = ilqr_layout(d, sz, knob);
+  const size_t TB = (size_t)d->T * d->B, B = d->B;
+  const size_t n = d->n, m = d->m;
+  size_t o = l.ilqr.total;
+  l.best_x = o;     o += up256(TB * n * sz);
+  l.best_u = o;     o += up256(TB * m * sz);
+  l.best_costs = o; o += up256(B * sz);
+  l.best_fdn = o;   o += up256(B * sz);
+  l.info = o;       o += up256(2 * sizeof(int32_t));
+  l.state = o;      o += up256(B * n * sz);             // x_k: the x_init of the solve of control step k
+  l.warm = o;       o += up256(TB * m * sz);            // w_k: its u_init
+  l.traj = o;       o += up256(2 * B * n * sz);         // the model step [x_k, x_{k+1}]
+  l.ep = o;         o += up256(sizeof(EpisodeState));
+  l.total = o;
+  return l;
+}
+
+// the arguments of mpcb200_episode_*, in the header's order
+template <typename R>
+struct EpisodeCall {
+  const mpcb200_dims* d;
+  const mpcb200_params* p;
+  const mpcb200_ilqr_opts* o;
+  int n_steps;
+  const R *C, *c, *F, *f, *x_init, *u_init, *u_lower, *u_upper;
+  const uint8_t* u_zero_I;
+  R *xs, *us, *costs;
+  int32_t* info;
+  R* u_next;
+  void* workspace;
+  size_t workspace_bytes;
+};
+
+// the solve of every control step: the caller's problem from the state and warm-start buffers, its best iterate in
+// the workspace
+template <typename R>
+static IlqrCall<R> episode_solve(const EpisodeCall<R>& e, const EpisodeLayout& l) {
+  char* ws = (char*)e.workspace;
+  const bool have = ws != nullptr;
+  return {e.d, e.p, e.o, e.C, e.c, e.F, e.f,
+          have ? (const R*)(ws + l.state) : nullptr, have ? (const R*)(ws + l.warm) : nullptr,
+          e.u_lower, e.u_upper, e.u_zero_I,
+          have ? (R*)(ws + l.best_x) : nullptr, have ? (R*)(ws + l.best_u) : nullptr,
+          have ? (R*)(ws + l.best_costs) : nullptr, have ? (R*)(ws + l.best_fdn) : nullptr,
+          have ? (int32_t*)(ws + l.info) : nullptr, e.workspace, l.ilqr.total};
+}
+
+// ilqr_check of the solve, plus the episode's own: every error is reported before anything is captured or launched
+template <typename R>
+static int episode_check(const EpisodeCall<R>& e, int knob) {
+  int rc = check_dims(e.d);
+  if (rc) return rc;
+  if (e.x_init == nullptr || e.xs == nullptr || e.us == nullptr || e.costs == nullptr || e.info == nullptr ||
+      e.u_next == nullptr || e.workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (e.d->T < 3 || e.n_steps < 1) return MPCB200_ERR_BAD_DIMS;     // the warm-start shift reads u[T-3]
+  const EpisodeLayout l = episode_layout(e.d, sizeof(R), knob);
+  if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  return ilqr_check<R>(episode_solve(e, l), knob);
+}
+
+// Adds the episode's init kernel and its `while` node over control steps (body recorded on `es`) to the graph `os`
+// is capturing.  Body: the iLQR loop (its own `while` node, body on `bs`) -> model step -> episode_advance_kernel.
+template <typename R>
+static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, const EpisodeCall<R>& e, int knob) {
+  const mpcb200_dims* d = e.d;
+  const EpisodeLayout l = episode_layout(d, sizeof(R), knob);
+  const IlqrCall<R> q = episode_solve(e, l);
+  char* ws = (char*)e.workspace;
+  R* state = (R*)(ws + l.state);
+  R* warm = (R*)(ws + l.warm);
+  R* traj = (R*)(ws + l.traj);
+  EpisodeState* ep = (EpisodeState*)(ws + l.ep);
+  const int B = d->B, T = d->T, N = d->n, M = d->m;
+  cudaGraphConditionalHandle handle;
+  int rc = while_handle(os, &handle);
+  if (rc) return rc;
+  if (counted(episode_launch_init<R>((size_t)B * N, (size_t)T * B * M, e.x_init, e.u_init, state, e.xs, warm, ep,
+                                     handle, os)) != 0)
+    return MPCB200_ERR_LAUNCH;
+  rc = open_while(os, es, handle);
+  if (rc) return rc;
+  rc = ilqr_record<R>(es, bs, q, knob);
+  // the model step from the solve's best controls, by the launchers the solve's rollout uses, at T = 2
+  if (rc == 0 && d->dynamics_kind == DYN_LINEAR) {
+    mpcb200_dims d2 = *d;
+    d2.T = 2;
+    d2.F_T = 1;
+    rc = rollout_impl<R>(&d2, e.F, e.f, state, q.best_u, traj, knob, es);
+  } else if (rc == 0) {
+    rc = dyn_impl<R>(false, d->dynamics_kind, e.p->dyn, B, 2, state, q.best_u, traj, nullptr, nullptr, es);
+  }
+  if (rc == 0)
+    rc = counted(episode_launch_advance<R>(B, T, N, M, e.o->m_ref, e.n_steps, traj, q.best_u, q.best_costs, q.info,
+                                           state, warm, e.xs, e.us, e.costs, e.info, ep, handle, es));
+  cudaGraph_t body = nullptr;
+  if (cudaStreamEndCapture(es, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+  if (rc == 0 && cudaMemcpyAsync(e.u_next, warm, (size_t)T * B * M * sizeof(R), cudaMemcpyDeviceToDevice, os) !=
+                     cudaSuccess)
+    rc = MPCB200_ERR_LAUNCH;
+  return rc;
+}
+
+template <typename R>
+static int episode_impl(const EpisodeCall<R>& e, void* stream) {
+  const int knob = kernel_knob();
+  int rc = episode_check<R>(e, knob);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t es = ilqr_stream(2), bs = ilqr_stream(1);
+    return es == nullptr || bs == nullptr ? MPCB200_ERR_LAUNCH : episode_record<R>(os, es, bs, e, knob);
+  });
 }
 }  // namespace mpcb200
 
@@ -767,6 +923,29 @@ int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, con
   return ilqr_impl<double>({dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
                             best_costs, best_full_du_norm, info, workspace, workspace_bytes},
                            stream);
+}
+
+size_t mpcb200_episode_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
+  if (mpcb200_ilqr_workspace_bytes(dims, opts, elem_size) == 0) return 0;
+  return episode_layout(dims, (size_t)elem_size, kernel_knob()).total;
+}
+int mpcb200_episode_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                        int32_t n_steps, const float* C, const float* c, const float* F, const float* f,
+                        const float* x_init, const float* u_init, const float* u_lower, const float* u_upper,
+                        const uint8_t* u_zero_I, float* xs, float* us, float* costs, int32_t* info, float* u_next,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  return episode_impl<float>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs,
+                              us, costs, info, u_next, workspace, workspace_bytes},
+                             stream);
+}
+int mpcb200_episode_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                        int32_t n_steps, const double* C, const double* c, const double* F, const double* f,
+                        const double* x_init, const double* u_init, const double* u_lower, const double* u_upper,
+                        const uint8_t* u_zero_I, double* xs, double* us, double* costs, int32_t* info, double* u_next,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  return episode_impl<double>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I,
+                               xs, us, costs, info, u_next, workspace, workspace_bytes},
+                              stream);
 }
 
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }

@@ -25,16 +25,18 @@ struct IlqrState {        // device-resident loop state, reset by ilqr_init_kern
 
 enum : uint8_t { ILQR_BETTER = 1u, ILQR_UNCONVERGED = 2u };
 
-// u = u_init (or 0); loop state and info reset.
+// u = u_init (or 0); loop state and info reset; the loop's handle set to 1.  The handle's launch default would do
+// that only when the graph is launched: a loop nested in the body of another (mpcb200_episode_*) restarts here.
 template <typename R>
 __global__ void __launch_bounds__(256)
 ilqr_init_kernel(size_t n_u, const R* __restrict__ u_init, R* __restrict__ u, IlqrState* __restrict__ st,
-                 int32_t* __restrict__ info) {
+                 int32_t* __restrict__ info, cudaGraphConditionalHandle handle) {
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   for (size_t i = i0; i < n_u; i += (size_t)gridDim.x * blockDim.x) u[i] = u_init != nullptr ? u_init[i] : R(0);
   if (i0 == 0) {
     st->iter = 0; st->n_not_improved = 0; st->n_unconverged = 0; st->reserved = 0;
     info[0] = 0; info[1] = 0;
+    cudaGraphSetConditional(handle, 1);
   }
 }
 
@@ -135,9 +137,90 @@ ilqr_stop_kernel(int B, int lqr_iter, int not_improved_lim, double eps, const R*
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// the receding-horizon episode (mpcb200_episode_*): an outer `while` node whose body is the iLQR loop above, the
+// model step from its best controls, then episode_advance_kernel
+// ---------------------------------------------------------------------------------------------
+struct EpisodeState {     // device-resident episode state, reset by episode_init_kernel
+  int32_t step;           // control steps completed
+  uint32_t tickets;       // blocks of the current episode_advance_kernel that have finished
+  int32_t reserved[2];
+};
+
+// state = xs[0] = x_init; warm = u_init (or 0); counters reset; the episode's handle set to 1.
+template <typename R>
+__global__ void __launch_bounds__(256)
+episode_init_kernel(size_t n_x, size_t n_u, const R* __restrict__ x_init, const R* __restrict__ u_init,
+                    R* __restrict__ state, R* __restrict__ xs0, R* __restrict__ warm, EpisodeState* __restrict__ ep,
+                    cudaGraphConditionalHandle handle) {
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = i0; i < n_x; i += step) {
+    const R v = x_init[i];
+    state[i] = v;
+    xs0[i] = v;
+  }
+  for (size_t i = i0; i < n_u; i += step) warm[i] = u_init != nullptr ? u_init[i] : R(0);
+  if (i0 == 0) {
+    ep->step = 0; ep->tickets = 0u; ep->reserved[0] = ep->reserved[1] = 0;
+    cudaGraphSetConditional(handle, 1);
+  }
+}
+
+// After the model step of control step k = ep->step, grid-wide.  us[k] = best_u[0]; xs[k+1] and the next solve's
+// x_init (state) = traj[1]; the next warm start warm[t] = best_u[t+1] for t < T-2, best_u[T-2] at t = T-2, 0 at
+// t = T-1 (cat(u[1:], 0), then w[-2] = w[-3]), with controls past m_ref at 0 as a freshly padded u_init has them;
+// costs[k] = best_costs, info_out[k] = info.  The last block to finish advances ep->step and ends the episode's
+// loop after n_steps control steps: every block has read ep->step by then.
+template <typename R>
+__global__ void __launch_bounds__(256)
+episode_advance_kernel(int B, int T, int N, int M, int m_ref, int n_steps, const R* __restrict__ traj,
+                       const R* __restrict__ best_u, const R* __restrict__ best_costs, const int32_t* __restrict__ info,
+                       R* __restrict__ state, R* __restrict__ warm, R* __restrict__ xs, R* __restrict__ us,
+                       R* __restrict__ costs, int32_t* __restrict__ info_out, EpisodeState* __restrict__ ep,
+                       cudaGraphConditionalHandle handle) {
+  const int k = ep->step;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const size_t BM = (size_t)B * M, BN = (size_t)B * N;
+  for (size_t i = i0; i < (size_t)T * BM; i += step) {
+    const int t = (int)(i / BM), j = (int)(i % M);
+    R v = R(0);
+    if (j < m_ref && t < T - 1) v = best_u[t < T - 2 ? i + BM : i];
+    warm[i] = v;
+  }
+  for (size_t i = i0; i < BM; i += step) us[(size_t)k * BM + i] = best_u[i];
+  for (size_t i = i0; i < BN; i += step) {
+    const R v = traj[BN + i];
+    state[i] = v;
+    xs[(size_t)(k + 1) * BN + i] = v;
+  }
+  for (size_t b = i0; b < (size_t)B; b += step) costs[(size_t)k * B + b] = best_costs[b];
+  if (i0 == 0) {
+    info_out[2 * k] = info[0];
+    info_out[2 * k + 1] = info[1];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&ep->tickets, 1u) == gridDim.x - 1) {
+      ep->tickets = 0u;
+      ep->step = k + 1;
+      if (k + 1 >= n_steps) cudaGraphSetConditional(handle, 0);
+    }
+  }
+}
+
 // Launchers (ilqr.cu), instantiated for float and double; 0 or MPCB200_ERR_LAUNCH.
 template <typename R>
-int ilqr_launch_init(size_t n_u, const R* u_init, R* u, IlqrState* st, int32_t* info, cudaStream_t stream);
+int ilqr_launch_init(size_t n_u, const R* u_init, R* u, IlqrState* st, int32_t* info,
+                     cudaGraphConditionalHandle handle, cudaStream_t stream);
+template <typename R>
+int episode_launch_init(size_t n_x, size_t n_u, const R* x_init, const R* u_init, R* state, R* xs0, R* warm,
+                        EpisodeState* ep, cudaGraphConditionalHandle handle, cudaStream_t stream);
+template <typename R>
+int episode_launch_advance(int B, int T, int N, int M, int m_ref, int n_steps, const R* traj, const R* best_u,
+                           const R* best_costs, const int32_t* info, R* state, R* warm, R* xs, R* us, R* costs,
+                           int32_t* info_out, EpisodeState* ep, cudaGraphConditionalHandle handle,
+                           cudaStream_t stream);
 template <typename R>
 int ilqr_launch_track(int B, int T, int N, int M, int m_ref, R best_cost_eps, const R* new_x, const R* new_u,
                       const R* costs, const R* du_first, const int32_t* status, const R* best_costs, R* best_x,

@@ -43,6 +43,26 @@ def _mv(A, x):
     return torch.matmul(A, x.unsqueeze(-1)).squeeze(-1)
 
 
+def _expand_cost(cost, T, n_batch, p):
+    """A QuadCost with C [p,p] / [T,p,p] and c [p] / [T,p] expanded to [T,B,p,p] and [T,B,p] (reference
+    mpc/mpc.py:205-226); any other cost as it is."""
+    if not isinstance(cost, QuadCost):
+        return cost
+    C, c = cost
+    if C.ndimension() == 2:
+        C = C.unsqueeze(0).unsqueeze(0).expand(T, n_batch, p, -1)
+    elif C.ndimension() == 3:
+        C = C.unsqueeze(1).expand(T, n_batch, p, -1)
+    if c.ndimension() == 1:
+        c = c.unsqueeze(0).unsqueeze(0).expand(T, n_batch, -1)
+    elif c.ndimension() == 2:
+        c = c.unsqueeze(1).expand(T, n_batch, -1)
+    if C.ndimension() != 4 or c.ndimension() != 3:
+        print("MPC Error: Unexpected QuadCost shape.")
+        sys.exit(-1)
+    return QuadCost(C, c)
+
+
 def get_traj(T, u, x_init, dynamics):
     """Nominal rollout under the true dynamics (reference mpc/util.py:102-126), no graph."""
     with torch.no_grad():
@@ -197,20 +217,7 @@ class MPC(Module):
             print("MPC Error: Could not infer batch size, pass in as n_batch")
             sys.exit(-1)
 
-        if isinstance(cost, QuadCost):                     # shape expansion, reference :205-226
-            C, c = cost
-            if C.ndimension() == 2:
-                C = C.unsqueeze(0).unsqueeze(0).expand(T, n_batch, n + m, -1)
-            elif C.ndimension() == 3:
-                C = C.unsqueeze(1).expand(T, n_batch, n + m, -1)
-            if c.ndimension() == 1:
-                c = c.unsqueeze(0).unsqueeze(0).expand(T, n_batch, -1)
-            elif c.ndimension() == 2:
-                c = c.unsqueeze(1).expand(T, n_batch, -1)
-            if C.ndimension() != 4 or c.ndimension() != 3:
-                print("MPC Error: Unexpected QuadCost shape.")
-                sys.exit(-1)
-            cost = QuadCost(C, c)
+        cost = _expand_cost(cost, T, n_batch, n + m)
 
         assert x_init.ndimension() == 2 and x_init.size(0) == n_batch
 
@@ -232,6 +239,7 @@ class MPC(Module):
             best = self._ilqr_host(x_init, cost, dx, u)
         x, u = best["x"], best["u"]
         full_du_norm = best["full_du_norm"]
+        self._solve_info = best["info"]           # int32 [iterations, pnqp-unconverged iterations] (control.py)
 
         if isinstance(dx, LinDx):
             F, f = dx.F, dx.f
@@ -268,10 +276,24 @@ class MPC(Module):
         graph nodes (the caller then runs _ilqr_host)."""
         global _graph_cond_unavailable
         from . import step as _step
-        T, n, m = self.T, self.n_state, self.n_ctrl
+        T, m = self.T, self.n_ctrl
+        n, x_init, C, c, F, f, dyn = self._device_problem(x_init, cost, dx)
+        res = _step.ilqr_raw(n, m, T, x_init, C, c, F, f, u, dyn=dyn, **self._device_options())
+        if res is None:
+            _graph_cond_unavailable = True
+            return None
+        self._print_pnqp_warnings(res["info"][1])          # the one host read: iterations with a pnqp warning
+        x = res["x"][:, :, m:] if self.slew_rate_penalty is not None else res["x"]
+        return {"x": x, "u": res["u"], "costs": res["costs"], "full_du_norm": res["full_du_norm"], "info": res["info"]}
+
+    def _device_problem(self, x_init, cost, dx):
+        """The problem of the device loop, staged once per solve (or episode): (n, x_init, C, c, F, f, dyn).  With a
+        slew-rate penalty, the augmented problem over [u_{t-1}; x] (n = n_state + n_ctrl).  dyn = (kind, params) of a
+        known system, with F = f = None; None for LinDx."""
+        n, m = self.n_state, self.n_ctrl
         C, c = cost.C, cost.c
         F, f = (dx.F, dx.f) if isinstance(dx, LinDx) else (None, None)
-        if self.slew_rate_penalty is not None:       # the augmented problem, staged once for the whole solve
+        if self.slew_rate_penalty is not None:
             _, C, c, F, f, _, x_init = self._slew_augment(x_init, C, c, F, f)
             if not isinstance(dx, LinDx):
                 dx = CtrlPassthroughDynamics(dx)
@@ -282,25 +304,30 @@ class MPC(Module):
             from .dynamics import known_kind
             F = f = None
             dyn = known_kind(dx, n, m, x_init)
-        res = _step.ilqr_raw(n, m, T, x_init, C, c, F, f, u, u_lower=self.u_lower, u_upper=self.u_upper,
-                             u_zero_I=self.u_zero_I, delta_u=self.delta_u, linesearch_decay=self.linesearch_decay,
-                             max_linesearch_iter=self.max_linesearch_iter, lqr_iter=self.lqr_iter,
-                             not_improved_lim=self.not_improved_lim, eps=self.eps, best_cost_eps=self.best_cost_eps,
-                             dyn=dyn)
-        if res is None:
-            _graph_cond_unavailable = True
-            return None
+        return n, x_init, C, c, F, f, dyn
+
+    def _device_options(self):
+        """The solver options step.ilqr_raw / step.episode_raw take."""
+        return dict(u_lower=self.u_lower, u_upper=self.u_upper, u_zero_I=self.u_zero_I, delta_u=self.delta_u,
+                    linesearch_decay=self.linesearch_decay, max_linesearch_iter=self.max_linesearch_iter,
+                    lqr_iter=self.lqr_iter, not_improved_lim=self.not_improved_lim, eps=self.eps,
+                    best_cost_eps=self.best_cost_eps)
+
+    def _print_pnqp_warnings(self, n_unconverged):
+        """The pnqp warnings of a device-side solve: one per iteration counted in `n_unconverged` (a device scalar,
+        read only when they are printed)."""
         if self.verbose >= 0 and self.u_lower is not None:
-            for _ in range(int(res["info"][1])):             # the one host read: iterations with a pnqp warning
+            for _ in range(int(n_unconverged)):
                 print("[WARNING] pnqp warning: Did not converge")   # reference pnqp.py:81
-        x = res["x"][:, :, m:] if self.slew_rate_penalty is not None else res["x"]
-        return {"x": x, "u": res["u"], "costs": res["costs"], "full_du_norm": res["full_du_norm"]}
 
     def _ilqr_host(self, x_init, cost, dx, u):
         """The iLQR iterations from Python: one host read per iteration for the stop test."""
+        from .step import _host_reads
         T = self.T
         best = None
         n_not_improved = 0
+        n_iter = n_unconverged = 0
+        _host_reads.n_warned = 0                        # pnqp warnings LQRStep prints itself (verbose > 0)
         for i in range(self.lqr_iter):
             u = _detach(u)
             x = get_traj(T, u, x_init=x_init, dynamics=dx)
@@ -335,6 +362,8 @@ class MPC(Module):
                 flags.append(defer["unconverged"].to(full_du_norm.dtype))
             vals = torch.stack(flags).tolist()              # the one host sync of this iteration
             max_du, any_better = vals[0], vals[1]
+            n_iter += 1
+            n_unconverged += 1 if defer and vals[2] else 0
             if defer and vals[2] and self.verbose >= 0:
                 print("[WARNING] pnqp warning: Did not converge")   # reference pnqp.py:81
             if any_better:
@@ -352,6 +381,8 @@ class MPC(Module):
             if max_du < self.eps or n_not_improved > self.not_improved_lim:   # reference :299-301
                 break
 
+        if best is not None:
+            best["info"] = torch.tensor([n_iter, n_unconverged + _host_reads.n_warned], dtype=torch.int32)
         return best
 
     # ------------------------------------------------------------------------------------

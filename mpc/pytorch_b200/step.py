@@ -21,7 +21,8 @@ from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_DIMS, DYN_LINEAR
 PNQP_MAX_ITER = 20  # reference passes n_iter=20 (mpc/lqr_step.py:137)
 
 # MPC's loop sets `_host_reads.defer` to a dict around its LQRStep calls: the per-step pnqp counters then stay
-# on the device (no .item() per step) and MPC reads them with its own stop-test scalars.  Thread local; the
+# on the device (no .item() per step) and MPC reads them with its own stop-test scalars.  Without it, a step that
+# prints a pnqp warning counts it in `_host_reads.n_warned`, which MPC's loop resets per solve.  Thread local; the
 # LQRStep(...) signature itself stays the reference's.
 _host_reads = threading.local()
 
@@ -407,6 +408,48 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
     return {"x": pad.crop_n(best_x), "u": pad.crop_m(best_u), "costs": costs, "full_du_norm": fdn, "info": info}
 
 
+def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
+                delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
+                best_cost_eps=1e-4, dyn=None):
+    """A receding-horizon episode of n_steps control steps in ONE library call (mpcb200_episode_*): each step solves
+    the problem from the current state as ilqr_raw does (u_init = the warm start), applies the plan's first control,
+    steps the model (LinDx: F[0] [x; u] + f[0]; a known system `dyn`: one step of it) and shifts the warm start
+    (cat(u[1:], 0), then w[-2] = w[-3]).  The problem is staged once per episode by the _problem call ilqr_raw makes.
+    u_init None: zeros.  Returns a dict of device tensors x [n_steps+1, B, n], u [n_steps, B, m], costs
+    [n_steps, B], info int32 [n_steps, 2] and u_next [T, B, m]; None when the driver has no conditional graph nodes
+    or no conditional node inside another's body (nothing was launched then)."""
+    n, m = n_state, n_ctrl
+    if T < 3 or n_steps < 1:
+        raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
+    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
+                  F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
+                  dyn_kind=dyn[0] if dyn is not None else None, need_F=dyn is None)
+    dtype, dev = C.dtype, C.device
+    s = _problem(n, m, T, B, dtype, dev, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+                 max_linesearch_iter, dyn)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
+    opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
+                         best_cost_eps=float(best_cost_eps))
+    nbytes = _lib.lib().mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    xs = torch.empty(n_steps + 1, B, N, dtype=dtype, device=dev)
+    us = torch.empty(n_steps, B, M, dtype=dtype, device=dev)
+    costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
+    info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
+    u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
+    fn = _lib.entry("mpcb200_episode", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), ptr_view(s.C),
+                ptr_view(s.c), ptr_view(s.F), ptr_view(s.f), ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper),
+                ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info), ptr(u_next), ptr(ws), nbytes,
+                stream_handle(dev))
+    if rc == _lib.ERR_NO_GRAPH_COND:
+        return None
+    check(rc, "mpcb200_episode")
+    return {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
+
+
 def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_df, f_T=None):
     """Run the gradient-assembly kernel; returns (dx_init, dC, dc, dF, df|None)."""
     n, m = n_state, n_ctrl
@@ -669,6 +712,7 @@ class LQRStepFn(Function):
             n_qp = float(per_t.sum().item())
             if o.verbose >= 0 and bool((res["status"] & 1).any()):
                 print("[WARNING] pnqp warning: Did not converge")   # reference pnqp.py:81
+                _host_reads.n_warned = getattr(_host_reads, "n_warned", 0) + 1
         else:
             n_qp = 0.0
         ctx.save_for_backward(x_init, C, c, F, f, new_x, new_u)
