@@ -1,6 +1,6 @@
 """What the GPU test modules share: device plumbing, the two tolerance policies, case builders, the checks of a step
-against the oracle, the device probes of the kernels' switch horizons, and the runner that solves an MPC on the
-device loop or the host loop.
+against the oracle, the device probes of the kernels' switch horizons, the runner that solves an MPC on the
+device loop or the host loop, and the raw call and float64 check of the standalone pnqp.
 
 Tolerance policies (DESIGN section 4):
   * `within`: float64 within tol64 x scale of the float64 oracle; float32 within K32 = 4 times the error of the
@@ -507,3 +507,55 @@ def same_on_both_loops(monkeypatch, make, x0, cost, dx, grads=()):
     for k, (a, b) in enumerate(zip(dev.grads, host.grads)):
         assert torch.equal(a, b), f"gradient {k} {float((a - b).abs().max()):.3e}"
     return dev, host
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the standalone pnqp (csrc/pnqp.cu: one thread per QP for n <= 8, one thread block per QP above)
+# ------------------------------------------------------------------------------------------------------------------
+PNQP_ITER = 20
+
+
+def gen_qp(seed, B, n):
+    """The pnqp generator of oracle/make_golden.py: H = LL' + I/2, q ~ 2N(0,1), bounds in (-1,0) and (0,1),
+    x_init ~ 0.3N(0,1); float64."""
+    g = torch.Generator().manual_seed(seed)
+    L = torch.randn(B, n, n, generator=g, dtype=F64)
+    H = L @ L.transpose(1, 2) + 0.5 * torch.eye(n, dtype=F64)
+    q = 2.0 * torch.randn(B, n, generator=g, dtype=F64)
+    lo = -torch.rand(B, n, generator=g, dtype=F64)
+    hi = torch.rand(B, n, generator=g, dtype=F64)
+    x0 = 0.3 * torch.randn(B, n, generator=g, dtype=F64)
+    return H, q, lo, hi, x0
+
+
+def pnqp_raw(H, q, lo, hi, x0=None, n_iter=PNQP_ITER):
+    """mpcb200_pnqp_* on dense [B,n] inputs: (x, H_free, If, iters, status) per problem, on the CPU."""
+    B, n, _ = H.shape
+    dt = H.dtype
+    ins = [t.to(DEV).contiguous() for t in (H, q, lo.expand(B, n), hi.expand(B, n))]
+    x0d = x0.to(DEV).contiguous() if x0 is not None else None
+    x = torch.empty(B, n, dtype=dt, device=DEV)
+    Hf = torch.empty(B, n, n, dtype=dt, device=DEV)
+    If = torch.empty(B, n, dtype=torch.uint8, device=DEV)
+    iters = torch.empty(B, dtype=torch.int32, device=DEV)
+    status = torch.empty(B, dtype=torch.int32, device=DEV)
+    lib = _L()
+    fn = lib.entry("mpcb200_pnqp", dt)
+    with lib._on_device(DEV):
+        rc = fn(B, n, *[lib.ptr(t) for t in ins], lib.ptr(x0d), n_iter, lib.ptr(x), lib.ptr(Hf), lib.ptr(If),
+                lib.ptr(iters), lib.ptr(status), lib.stream_handle(DEV))
+    assert rc == 0, lib.lib().mpcb200_strerror(rc)
+    torch.cuda.synchronize()
+    return x.cpu(), Hf.cpu(), If.cpu(), iters.cpu().long(), status.cpu()
+
+
+def check_qp_f64(got, want, tag):
+    """float64 pnqp_raw outputs `got` against the oracle's (x, H_free, If, iters) `want`: x within
+    1e-9 * max(1, |x|_inf), H_free within 1e-12, free sets and iteration counts exact."""
+    x, Hf, If, iters, status = got
+    xo, Ho, Ifo, ito = want
+    scale = max(1.0, float(xo.abs().max()))
+    assert maxdiff(x, xo) <= 1e-9 * scale, f"{tag}: x differs by {maxdiff(x, xo):.3g}"
+    assert torch.equal(If.bool(), Ifo.bool()), f"{tag}: free set"
+    assert torch.equal(iters, ito), f"{tag}: iterations {iters.tolist()} vs {ito.tolist()}"
+    assert maxdiff(Hf, Ho) <= 1e-12, f"{tag}: H_free"

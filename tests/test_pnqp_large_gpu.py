@@ -10,63 +10,16 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
+from tests.gpu_harness import DEV, F64, PNQP_ITER as N_ITER, check_qp_f64 as check_f64, gen_qp, pnqp_raw as raw
 from tests.helpers import load_golden, maxdiff
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda:0")
-F64 = torch.float64
-N_ITER = 20
 
 
 def max_n(dtype):
     from mpc.pytorch_b200 import _lib
     with _lib._on_device(DEV):
         return _lib.lib().mpcb200_pnqp_max_n(torch.empty(0, dtype=dtype).element_size())
-
-
-def gen_qp(seed, B, n):
-    """The pnqp generator of oracle/make_golden.py: H = LL' + I/2, q ~ 2N(0,1), bounds in (-1,0) and (0,1)."""
-    g = torch.Generator().manual_seed(seed)
-    L = torch.randn(B, n, n, generator=g, dtype=F64)
-    H = L @ L.transpose(1, 2) + 0.5 * torch.eye(n, dtype=F64)
-    q = 2.0 * torch.randn(B, n, generator=g, dtype=F64)
-    lo = -torch.rand(B, n, generator=g, dtype=F64)
-    hi = torch.rand(B, n, generator=g, dtype=F64)
-    x0 = 0.3 * torch.randn(B, n, generator=g, dtype=F64)
-    return H, q, lo, hi, x0
-
-
-def raw(H, q, lo, hi, x0=None, n_iter=N_ITER):
-    """mpcb200_pnqp_* on dense [B,n] inputs: (x, H_free, If, iters, status) per problem, on the CPU."""
-    from mpc.pytorch_b200 import _lib
-    from mpc.pytorch_b200._lib import ptr, stream_handle
-    B, n, _ = H.shape
-    dt = H.dtype
-    ins = [t.to(DEV).contiguous() for t in (H, q, lo.expand(B, n), hi.expand(B, n))]
-    x0d = x0.to(DEV).contiguous() if x0 is not None else None
-    x = torch.empty(B, n, dtype=dt, device=DEV)
-    Hf = torch.empty(B, n, n, dtype=dt, device=DEV)
-    If = torch.empty(B, n, dtype=torch.uint8, device=DEV)
-    iters = torch.empty(B, dtype=torch.int32, device=DEV)
-    status = torch.empty(B, dtype=torch.int32, device=DEV)
-    L = _lib.lib()
-    fn = _lib.entry("mpcb200_pnqp", dt)
-    with _lib._on_device(DEV):
-        rc = fn(B, n, *[ptr(t) for t in ins], ptr(x0d), n_iter, ptr(x), ptr(Hf), ptr(If), ptr(iters), ptr(status),
-                stream_handle(DEV))
-    assert rc == 0, L.mpcb200_strerror(rc)
-    torch.cuda.synchronize()
-    return x.cpu(), Hf.cpu(), If.cpu(), iters.cpu().long(), status.cpu()
-
-
-def check_f64(got, want, tag):
-    x, Hf, If, iters, status = got
-    xo, Ho, Ifo, ito = want
-    scale = max(1.0, float(xo.abs().max()))
-    assert maxdiff(x, xo) <= 1e-9 * scale, f"{tag}: x differs by {maxdiff(x, xo):.3g}"
-    assert torch.equal(If.bool(), Ifo.bool()), f"{tag}: free set"
-    assert torch.equal(iters, ito), f"{tag}: iterations {iters.tolist()} vs {ito.tolist()}"
-    assert maxdiff(Hf, Ho) <= 1e-12, f"{tag}: H_free"
 
 
 def test_reference_fixture_n100():
