@@ -207,7 +207,7 @@ def _bound(v, t):
 def lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, current_x, current_u,
                      u_lower=None, u_upper=None, u_zero_I=None, delta_u=None,
                      linesearch_decay=0.2, max_linesearch_iter=10,
-                     coupled=True, exact_pinv=True, dynamics=None, ls_trace=None):
+                     coupled=True, exact_pinv=True, dynamics=None, ls_trace=None, first_u=None):
     """One box-constrained LQR step in delta space (true cost = QuadCost).
 
     ``exact_pinv``: use the SVD pseudo-inverse for the unbounded m>1 branch like
@@ -218,6 +218,8 @@ def lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, current_x, current_
     uses F (and delta space, so not f) either way.
     ``ls_trace``: a list that receives ``current_cost - old_cost`` [B] of every
     line-search pass, the comparison that decides each alpha (:247).
+    ``first_u``: a list that receives new_u [T, B, m] of the first line-search pass, the full step (alpha = 1) that
+    full_du_norm measures (:243-245), also when later passes backtrack.
     """
     n, m = n_state, n_ctrl
     B = C.shape[1]
@@ -336,6 +338,8 @@ def lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, current_x, current_
         new_x = torch.stack(new_x)
         if full_du_norm is None:                                      # :243-245
             full_du_norm = (u - new_u).transpose(1, 2).reshape(B, -1).norm(2, 1)
+            if first_u is not None:
+                first_u.append(new_u)
         worse = current_cost > old_cost
         if ls_trace is not None:
             ls_trace.append(current_cost - old_cost)

@@ -11,6 +11,7 @@ Importing this module touches no device: the library is loaded when a function t
 import contextlib
 import ctypes
 import functools
+import math
 import os
 from collections import namedtuple
 
@@ -170,6 +171,174 @@ def oracle_steps(n, m, T, P, kw, dtype, **opts):
                                      **opts)
 
 
+LS_MARGIN = 1e-4                    # least |cost - oldcost| / max(1, |oldcost|) of a kept problem in every pass
+ONE, MID, MAX = 0, 1, 2             # line-search classes: one pass; backtracked, then better; worse on every pass
+LsCase = namedtuple("LsCase", "P kw o64 trace o32 first64 first32 classes")
+
+
+def rollout_passes(trace):
+    """Rollout passes each problem ran, from the oracle's ls_trace [passes, B] (cost - oldcost of every pass): up to
+    its first pass that is not worse, else all of them (the batch loop ran to max_ls)."""
+    better = trace <= 0
+    return torch.where(better.any(0), better.to(torch.int64).argmax(0) + 1, trace.shape[0])
+
+
+def ls_classes(trace):
+    """ONE, MID or MAX per problem (a problem of class MAX ends worse than its nominal and restores alpha)."""
+    p = rollout_passes(trace)
+    worse_end = trace.gather(0, (p - 1).view(1, -1))[0] > 0
+    return torch.where(worse_end, MAX, torch.where(p == 1, ONE, MID))
+
+
+def _ls_oracle(n, m, T, P, kw, lo=None):
+    """The per-problem oracle's step with its line-search trace and first-pass controls: (o, trace, first_u)."""
+    lo = lo or (lambda t: t)
+    trace, first = [], []
+    o = orc.lqr_step_forward(n, m, T, *[lo(P[k]) for k in ("x0", "C", "c", "F", "f", "x", "u")], coupled=False,
+                             ls_trace=trace, first_u=first, **{k: lo(v) for k, v in kw.items()})
+    return o, torch.stack(trace), first[0]
+
+
+def ls_nominal(seed, K, T, n, m, mode, shifted=False):
+    """K float64 problems whose nominal (x, u) makes the line search backtrack, four families by index k % 4:
+    0 unstable dynamics (F x 1.5-2, its 4/T-th power beyond T = 4) with the nominal rolled out from x0; 1 nominal controls
+    perturbed at t >= 1 (0.3 N(0, 1), kept in the box) after the state was rolled out; 2, 3 a nominal state perturbed
+    at t >= 1 (N(0, 1)) and pulled down the gradient of its stage cost by up to 6, so that its cost lies between the
+    costs of the rollout's passes.  These nominals start at x0 (x[0] = x_init).  shifted: family 1 is instead a
+    consistent nominal rolled out from a shifted initial state x0 + N(0, 1), so x[0] != x_init (DESIGN.md section 4:
+    the step's feedback then acts on x_init - x[0] from t = 0).  mode: plain | box (+-0.1) | boxT (tensor box) | boxD
+    (tensor box + delta_u) | mask (u_zero_I) | boxM (+-0.1 and u_zero_I)."""
+    C, c, F, f, x0 = gen_problem(seed, K, T, n, m, F64)
+    g = torch.Generator().manual_seed(seed + 13)
+    fam = torch.arange(K) % 4
+    s = 1.5 + 0.5 * torch.rand(K, generator=g, dtype=F64)
+    scale = torch.where(fam == 0, s ** min(1.0, 4.0 / T), torch.full_like(s, 0.9))
+    F = F * scale.view(1, K, 1, 1)
+    u, ul, uu = nominal_controls(seed, K, T, m, F64, {"box": 0.1, "boxM": 0.1, "boxT": "tensor",
+                                                      "boxD": "tensor"}.get(mode))
+    x = orc.get_traj(T, u, x0, F, f)
+    later = (torch.arange(T) >= 1).view(T, 1, 1)
+    du = 0.3 * torch.randn(T, K, m, generator=g, dtype=F64)
+    if shifted:
+        delta = torch.randn(K, n, generator=torch.Generator().manual_seed(seed + 17), dtype=F64)
+        x = orc.get_traj(T, u, x0 + delta * (fam == 1).view(K, 1), F, f)
+    else:
+        u = torch.where((fam == 1).view(1, K, 1) & later, u + du, u)
+    if ul is not None:
+        lo, hi = (torch.as_tensor(v, dtype=F64).expand_as(u) for v in (ul, uu))
+        u = torch.minimum(torch.maximum(u, lo), hi)
+    noise = torch.randn(T, K, n, generator=g, dtype=F64)
+    pull = 6.0 * torch.rand(K, generator=g, dtype=F64)
+    pert = (fam >= 2).view(1, K, 1) & later
+    x = torch.where(pert, x + noise, x)
+    grad = torch.einsum("tbij,tbj->tbi", C[..., :n, :], torch.cat((x, u), 2)) + c[..., :n]
+    x = torch.where(pert, x - pull.view(1, K, 1) * grad / grad.norm(dim=2, keepdim=True).clamp_min(1e-12), x)
+    kw = {}
+    if mode.startswith("box"):
+        kw = dict(u_lower=ul, u_upper=uu)
+    if mode == "boxD":
+        kw["delta_u"] = 0.125
+    if mode in ("mask", "boxM"):
+        kw["u_zero_I"] = torch.rand(T, K, m, generator=g) < 0.3
+    return dict(C=C, c=c, F=F, f=f, x0=x0, x=x, u=u), kw
+
+
+def _take(v, idx, B):
+    """Batch elements idx of an input: [B, ...] (x0) or [T, B, ...]; scalars as they are."""
+    if not torch.is_tensor(v):
+        return v
+    return v.index_select(0 if v.dim() == 2 and v.shape[0] == B else 1, idx)
+
+
+@functools.lru_cache(maxsize=8)
+def _ls_pool(seed, K, T, n, m, dtype, mode, max_ls, decay, shifted=False):
+    """The candidates of line_search_case: inputs rounded through dtype, and per candidate its class, or -1 where it
+    is not kept (a comparison within LS_MARGIN, a MAX problem whose final pass equals its first, or a float32 oracle
+    that decides differently)."""
+    P, kw = ls_nominal(seed, K, T, n, m, mode, shifted)
+    P = {k: round_through(v, dtype) for k, v in P.items()}
+    kw = {k: round_through(v, dtype) for k, v in kw.items()}
+    kw.update(linesearch_decay=decay, max_linesearch_iter=max_ls)
+    o, trace, first = _ls_oracle(n, m, T, P, kw)
+    cls = ls_classes(trace)
+    old = o.costs - trace[-1]
+    counted = torch.arange(trace.shape[0]).view(-1, 1) < rollout_passes(trace).view(1, -1)
+    ok = ((trace.abs() >= LS_MARGIN * old.abs().clamp_min(1.0)) | ~counted).all(0)
+    if max_ls > 1:
+        ok &= (cls != MAX) | ((first - o.new_u).abs().amax((0, 2)) > 1e-6)
+    if dtype == F32:
+        _, t32, _ = _ls_oracle(n, m, T, P, kw, lambda t: t.float() if torch.is_tensor(t) and t.is_floating_point()
+                               else t)
+        ok &= (ls_classes(t32) == cls) & (rollout_passes(t32) == rollout_passes(trace))
+    return P, kw, torch.where(ok, cls, -1)
+
+
+def line_search_case(seed, T, n, m, dtype, mode, max_ls, decay, layout, K=192, shifted=False):
+    """A batch with a chosen line-search class at each position (`layout`: a sequence of ONE / MID / MAX), drawn from
+    K seeded candidates (ls_nominal, `shifted` as there) classified by the float64 oracle.  The kernels and the oracle solve every
+    problem on its own, so a candidate keeps its class wherever it is placed; the oracle is rerun on the batch and
+    must agree.  A class the candidates lack is replaced by the next of MID, MAX, ONE that they have.  Returns an
+    LsCase: inputs P, options kw, float64 oracle o64 with its line-search trace, float32 oracle o32|None, the
+    first-pass controls of both, and the classes."""
+    P, kw, pool = _ls_pool(seed, K, T, n, m, dtype, mode, max_ls, decay, shifted)
+    have = {c: (pool == c).nonzero()[:, 0].tolist() for c in (ONE, MID, MAX)}
+    order = {ONE: (ONE, MID, MAX), MID: (MID, MAX, ONE), MAX: (MAX, MID, ONE)}
+    seen = {ONE: 0, MID: 0, MAX: 0}
+    idx = []
+    for c in layout:
+        c = next(d for d in order[c] if have[d])
+        idx.append(have[c][seen[c] % len(have[c])])
+        seen[c] += 1
+    idx = torch.tensor(idx)
+    Bp = pool.shape[0]
+    P = {k: _take(v, idx, Bp) for k, v in P.items()}
+    kw = {k: _take(v, idx, Bp) for k, v in kw.items()}
+    o64, trace, first64 = _ls_oracle(n, m, T, P, kw)
+    classes = ls_classes(trace)
+    assert torch.equal(classes, pool[idx]), "the oracle classifies a batch element unlike its candidate"
+    o32 = first32 = None
+    if dtype == F32:
+        o32, _, first32 = _ls_oracle(n, m, T, P, kw, lambda t: t.float() if torch.is_tensor(t) and
+                                     t.is_floating_point() else t)
+    return LsCase(P, kw, o64, trace, o32, first64, first32, classes)
+
+
+def step_layout(kernel, n, m, dtype):
+    """(problems per warp, problems per CTA) of a step kernel at the (n, m) it runs: StepCfg (lqr_step.cuh) for
+    the generic kernel, Step2Cfg (lqr_step2.cuh) for the column-pair kernel, one problem per CTA for the large-shape
+    kernels."""
+    if kernel == "large":
+        return 1, 1
+    if kernel == "pair":
+        ppw = 32 // ((n + m) // 2)
+        return ppw, ppw
+    sz = 8 if dtype == F64 else 4
+    lanes = n if (n, m, dtype) == (8, 2, F32) else n + m
+    ppw = 32 // lanes
+    span_ok = lambda nw: (nw * ppw * m * sz) % 16 == 0 and (nw * ppw * n * sz) % 16 == 0  # noqa: E731
+    nw = 2 if lanes == n else 1 if span_ok(1) else 2 if span_ok(2) else 4
+    return ppw, nw * ppw
+
+
+def ls_layout(B, ppw, W):
+    """Classes by batch position.  The first problem of every warp takes one pass, and so does all of warp 0 in
+    even CTAs of several warps: a repeat decided by that problem or that warp alone would stop too early.  The other
+    positions cycle through MAX, MID, ONE; the tail CTA keeps its warp 0 in the cycle.  With one problem per CTA the
+    cycle is ONE, MAX, MID."""
+    out = []
+    for b in range(B):
+        q, w, cta = b % ppw, (b % W) // ppw, b // W
+        if W == 1:
+            out.append((ONE, MAX, MID)[b % 3])
+        elif q == 0 or (w == 0 and W > ppw and cta % 2 == 0 and (cta + 1) * W < B):
+            out.append(ONE)
+        else:
+            out.append((MAX, MID, ONE)[(q - 1 + cta) % 3])
+    if B > 1:
+        out[-1] = MAX                   # the tail CTA always holds a problem that backtracks
+    return tuple(out)
+
+
 def rollout(module, x0, u):
     """[T, B, n]: x0 rolled out through module under the controls u [T, B, m]."""
     xs = [x0]
@@ -265,6 +434,24 @@ def _cols(t, keep):
     return t[:, keep] if t.dim() >= 2 else t[keep]
 
 
+def decays(alphas, decay):
+    """Number of decays behind each alpha (alpha = decay ** decays): the line-search decisions, free of the
+    dtype's rounding of decay ** decays."""
+    return torch.round(torch.log(alphas.double()) / math.log(decay)).long()
+
+
+def f32_compared(case):
+    """float32 cases (P, kw, o64, trace, o32, ...): the problems whose line-search decisions the comparison may
+    demand.  Left out are near-ties (|cost - oldcost| within 1e-5 relative in any pass of the float64 oracle:
+    round-off may decide that comparison either way) and problems where the float32 oracle, the yardstick, decides
+    differently."""
+    P, kw, o64, trace, o32 = case[:5]
+    old = o64.costs - trace[-1]
+    tie = (trace.abs() <= 1e-5 * old.abs().clamp_min(1.0)).any(0)
+    decay = kw["linesearch_decay"]
+    return ~tie & (decays(o32.alphas, decay) == decays(o64.alphas, decay))
+
+
 def check_alphas(tag, r, o64, o32, keep=None):
     """float64: alphas bit exact; float32: the float32 oracle's alphas wherever it makes the float64 oracle's
     line-search decisions."""
@@ -277,10 +464,11 @@ def check_alphas(tag, r, o64, o32, keep=None):
         assert torch.equal(got[same], w32[same]), f"{tag}: alphas"
 
 
-def check_trajectory(tag, r, u, o64, o32, dtype, keep=None):
+def check_trajectory(tag, r, u, o64, o32, dtype, keep=None, first=None):
     """The outputs r holds, under `within`: new_x and new_u (on one scale), costs, Ks and ks; with du_first, the
-    first full step u - new_u and its per-problem norm full_du_norm (the line search takes the full step on these
-    problems).  A Riccati-only step holds the gains alone."""
+    first full step u - new_u and its per-problem norm full_du_norm.  `first`: the new_u of the oracles' first
+    line-search pass (float64, float32|None) where the line search backtracks; by default their final new_u.  A
+    Riccati-only step holds the gains alone."""
     g = lambda o, k: None if o is None else _cols(getattr(o, k), keep)  # noqa: E731
     if "new_x" in r:
         sc = max(1.0, float(g(o64, "new_x").abs().max()), float(g(o64, "new_u").abs().max()))
@@ -289,10 +477,11 @@ def check_trajectory(tag, r, u, o64, o32, dtype, keep=None):
         within(tag, "costs", _cols(r["costs"], keep), g(o64, "costs"), g(o32, "costs"), dtype)
     if "du_first" in r:
         u = _cols(u, keep)
-        du = lambda o: None if o is None else u - g(o, "new_u")  # noqa: E731
+        f64, f32 = first if first is not None else (o64.new_u, None if o32 is None else o32.new_u)
+        du = lambda f: None if f is None else u - _cols(f, keep)  # noqa: E731
         norm = lambda d: None if d is None else d.pow(2).sum((0, 2)).sqrt()  # noqa: E731
-        within(tag, "du_first", _cols(r["du_first"], keep), du(o64), du(o32), dtype, scale=sc)
-        within(tag, "full_du_norm", _cols(r["full_du_norm"], keep), norm(du(o64)), norm(du(o32)), dtype, scale=sc)
+        within(tag, "du_first", _cols(r["du_first"], keep), du(f64), du(f32), dtype, scale=sc)
+        within(tag, "full_du_norm", _cols(r["full_du_norm"], keep), norm(du(f64)), norm(du(f32)), dtype, scale=sc)
     if "Ks" in r:
         within(tag, "Ks", _cols(r["Ks"], keep), g(o64, "Ks"), g(o32, "Ks"), dtype)
         within(tag, "ks", _cols(r["ks"], keep), g(o64, "ks"), g(o32, "ks"), dtype)

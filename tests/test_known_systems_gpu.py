@@ -18,15 +18,15 @@ W problems, PPW per warp: (5,1) has PPW = 5 and W = 10 (f64) / 20 (f32); (3,1) h
 the last CTA's count is then aligned too, since W is a multiple of 2 (f64) / 4 (f32).  Otherwise every tile is
 copied by the producer warp's lanes."""
 import functools
-import math
 
 import pytest
 import torch
 
 from oracle import lqr_oracle as orc
 from tests.gpu_harness import (BT, DEV, DT, F32, F64, PHYS, SYSTEMS, angle_cols, check_alphas, check_clamps, check_pnqp,
-                               check_trajectory, first_true, jacobians, known_controls, known_module, known_states,
-                               linearise, probe_step, round_through, rollout, run_step, within)
+                               check_trajectory, decays, f32_compared, first_true, jacobians, known_controls,
+                               known_module, known_states, linearise, probe_step, round_through, rollout, run_step,
+                               within)
 from tests.helpers import EDIT_ROUTES, maxdiff
 
 pytestmark = pytest.mark.gpu
@@ -156,23 +156,6 @@ def _run_step(name, T, case, dtype):
     return run_step(dx.n_state, 1, T, case[0], case[1], dtype, dyn=(dx.mpcb200_kind, dx.mpcb200_params()))
 
 
-def _passes(alphas, decay):
-    """Number of decays behind each alpha (alpha = decay ** passes): the line-search decisions, free of the
-    dtype's rounding of decay ** passes."""
-    return torch.round(torch.log(alphas.double()) / math.log(decay)).long()
-
-
-def _f32_compared(case):
-    """float32 cases: the problems whose line-search decisions the comparison may demand.  Left out are near-ties
-    (|cost - oldcost| within 1e-5 relative in any pass of the float64 oracle: round-off may decide that
-    comparison either way) and problems where the float32 oracle, the yardstick, decides differently."""
-    P, kw, o64, trace, o32 = case
-    old = o64.costs - trace[-1]
-    tie = (trace.abs() <= 1e-5 * old.abs().clamp_min(1.0)).any(0)
-    decay = kw["linesearch_decay"]
-    return ~tie & (_passes(o32.alphas, decay) == _passes(o64.alphas, decay))
-
-
 def check_step(tag, r, case, dtype):
     """float64: 1e-9 x scale, alphas / free sets / pnqp iterations bit exact.  float32: the same line-search
     decisions (number of decays) as the float64 oracle and alphas to 1e-6, except at near-ties; those problems
@@ -180,11 +163,11 @@ def check_step(tag, r, case, dtype):
     P, kw, o64, trace, o32 = case
     keep = torch.ones(P["x0"].shape[0], dtype=torch.bool)
     if dtype == F32:
-        keep = _f32_compared(case)
+        keep = f32_compared(case)
         out = int((~keep).sum())
         assert out <= max(1, len(keep) // 8), f"{tag}: {out} of {len(keep)} problems left out"
         decay = kw["linesearch_decay"]
-        assert torch.equal(_passes(r["alphas"], decay)[keep], _passes(o64.alphas, decay)[keep]), \
+        assert torch.equal(decays(r["alphas"], decay)[keep], decays(o64.alphas, decay)[keep]), \
             f"{tag}: line-search decisions {r['alphas']} vs {o64.alphas}"
         assert maxdiff(r["alphas"][keep], o64.alphas[keep]) <= 1e-6, f"{tag}: alphas"
         assert int((r["status"] & ~1).max()) == 0, tag
@@ -246,7 +229,7 @@ def test_fused_step_cases_exercise_the_line_search_and_the_clamp(name, dtype):
                 continue
             case = step_case(name, B, 15, dtype, bounds, ls_iter, decay, 500 + B)
             _, _, o64, trace, _ = case
-            keep = _f32_compared(case) if dtype == F32 else torch.ones(B, dtype=torch.bool)
+            keep = f32_compared(case) if dtype == F32 else torch.ones(B, dtype=torch.bool)
             decayed += int((o64.alphas[keep] < 1).sum())
             worse_first += int((trace[0][keep] > 0).sum())
             beyond += int((o64.new_u.abs() > PHYS[name]["clamp"]).sum())
