@@ -220,6 +220,25 @@ int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_
                               const double* u, double* F, double* f, void* stream);
 
 /*
+ * Vector-Jacobian product of mpcb200_dyn_linearize_* in the system's learnable parameters theta: cartpole dyn[0..3]
+ * (gravity, masscart, masspole, length), pendulum dyn[0..2] (g, m, l); force_mag / max_torque and dt are constants.
+ * For t < T-1, with z = [x; u], J = [d step/dx, d step/du] and f = step(x, u) - J z at (x[t,b], u[t,b]):
+ *   first[t,b,k]  = sum_r df[t,b,r] d step_r/dtheta_k
+ *   second[t,b,k] = sum_{r,j} (dF[t,b,r,j] - df[t,b,r] z_j) dJ_rj/dtheta_k
+ * so first + second, summed over (t, b), is the gradient of <dF, F> + <df, f> in theta; `first` alone is that gradient
+ * with J held constant.  A control beyond the clamp contributes no u column (the clamp's derivative is 0 there).
+ * kind = MPCB200_DYN_CARTPOLE or MPCB200_DYN_PENDULUM (a passthrough kind is MPCB200_ERR_BAD_DIMS); dyn = HOST pointer
+ * to 8 doubles; x[T,B,n] u[T,B,1] dF[T-1,B,n,n+1] df[T-1,B,n]; first, second [T-1,B,NP] (NP = 4 cartpole, 3 pendulum),
+ * either may be NULL.  One kernel; nothing is launched when T = 1 or both outputs are NULL.
+ */
+int mpcb200_dyn_linearize_vjp_f32(int32_t kind, const double* dyn, int32_t B, int32_t T, const float* x,
+                                  const float* u, const float* dF, const float* df, float* first, float* second,
+                                  void* stream);
+int mpcb200_dyn_linearize_vjp_f64(int32_t kind, const double* dyn, int32_t B, int32_t T, const double* x,
+                                  const double* u, const double* dF, const double* df, double* first, double* second,
+                                  void* stream);
+
+/*
  * Standalone projected-Newton box QP, n <= mpcb200_pnqp_max_n(elem_size): replaces
  * pnqp(H,q,lower,upper,x_init,n_iter) of the reference (mpc/pnqp.py:5-82) for batches of QPs
  * min 0.5 x'Hx + q'x, lower <= x <= upper.

@@ -47,6 +47,7 @@ EXPORTED_SYMBOLS = (
     "mpcb200_rollout_f32", "mpcb200_rollout_f64", "mpcb200_pnqp_f32", "mpcb200_pnqp_f64", "mpcb200_pnqp_max_n",
     "mpcb200_lqr_adjoint_f32", "mpcb200_lqr_adjoint_f64", "mpcb200_adjoint_workspace_bytes",
     "mpcb200_dyn_rollout_f32", "mpcb200_dyn_rollout_f64", "mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64",
+    "mpcb200_dyn_linearize_vjp_f32", "mpcb200_dyn_linearize_vjp_f64",
     "mpcb200_supported", "mpcb200_supported_list", "mpcb200_launch_count",
     "mpcb200_step_smem_bytes", "mpcb200_step_prefers_workspace", "mpcb200_last_step_plan", "mpcb200_version",
     "mpcb200_strerror", "mpcb200_step_large_fits", "mpcb200_ilqr_f32", "mpcb200_ilqr_f64",
@@ -101,6 +102,10 @@ def lib():
     for name in ("mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64"):
         fn = getattr(L, name)
         fn.argtypes = [ctypes.c_int32, ctypes.POINTER(ctypes.c_double), ctypes.c_int32, ctypes.c_int32] + [vp] * 5
+        fn.restype = ctypes.c_int
+    for name in ("mpcb200_dyn_linearize_vjp_f32", "mpcb200_dyn_linearize_vjp_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.c_int32, ctypes.POINTER(ctypes.c_double), ctypes.c_int32, ctypes.c_int32] + [vp] * 7
         fn.restype = ctypes.c_int
     for name in ("mpcb200_ilqr_f32", "mpcb200_ilqr_f64"):
         fn = getattr(L, name)

@@ -423,6 +423,21 @@ static int dyn_impl(bool linearize, int kind, const double* dyn, int B, int T, c
   if (rc == 0 && !(linearize && T == 1)) g_launches.fetch_add(1);
   return rc;
 }
+template <typename R>
+static int dyn_vjp_impl(int kind, const double* dyn, int B, int T, const R* x, const R* u, const R* dF, const R* df,
+                        R* first, R* second, void* stream) {
+  if (dyn == nullptr || x == nullptr || u == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (B <= 0 || T <= 0 || (kind != DYN_CARTPOLE && kind != DYN_PENDULUM)) return MPCB200_ERR_BAD_DIMS;
+  if (T > 1 && (dF == nullptr || df == nullptr)) return MPCB200_ERR_NULL_POINTER;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  if (T == 1 || (first == nullptr && second == nullptr)) return 0;
+  DynVjpArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.B = B; a.T = T; a.kind = kind;
+  for (int i = 0; i < 8; ++i) a.dp.p[i] = dyn[i];
+  a.x = x; a.u = u; a.dF = dF; a.df = df; a.first = first; a.second = second;
+  return counted(launch_dyn_linearize_vjp<R>(a, (cudaStream_t)stream));
+}
 
 // whether the step of `d` keeps its gains in the caller's Ks/ks (mpcb200_step_prefers_workspace)
 static int gains_in_workspace(const mpcb200_dims* d, int elem_size, int knob) {
@@ -899,6 +914,16 @@ int mpcb200_dyn_linearize_f32(int32_t kind, const double* dyn, int32_t B, int32_
 int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_t T, const double* x,
                               const double* u, double* F, double* f, void* stream) {
   return dyn_impl<double>(true, kind, dyn, B, T, x, u, nullptr, F, f, stream);
+}
+int mpcb200_dyn_linearize_vjp_f32(int32_t kind, const double* dyn, int32_t B, int32_t T, const float* x,
+                                  const float* u, const float* dF, const float* df, float* first, float* second,
+                                  void* stream) {
+  return dyn_vjp_impl<float>(kind, dyn, B, T, x, u, dF, df, first, second, stream);
+}
+int mpcb200_dyn_linearize_vjp_f64(int32_t kind, const double* dyn, int32_t B, int32_t T, const double* x,
+                                  const double* u, const double* dF, const double* df, double* first, double* second,
+                                  void* stream) {
+  return dyn_vjp_impl<double>(kind, dyn, B, T, x, u, dF, df, first, second, stream);
 }
 
 size_t mpcb200_ilqr_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {

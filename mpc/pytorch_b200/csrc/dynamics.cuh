@@ -107,6 +107,97 @@ MPCB_DEV Dual<R, NV> dclamp(const Dual<R, NV>& a, R lo, R hi) {
   for (int i = 0; i < NV; ++i) o.d[i] = in ? a.d[i] : R(0);
   return o;
 }
+// ------------------------------------------------------------------ nested duals Dual<Dual<R, NV>, NW>
+// Forward mode over forward mode: the inner dual carries d/dz, the outer one d/dtheta of a system parameter, so the
+// outer derivative of an inner derivative is a mixed second derivative d2/(dtheta dz) (dyn_linearize_vjp_kernel).
+// The generic operators above cover nested-with-nested; these are the scalar-on-the-left forms and the elementary
+// functions, whose generic versions call cos / sin / atan2 on the value.
+template <typename R, int NV>
+MPCB_DEV Dual<R, NV> dual_const(R v) {
+  Dual<R, NV> o;
+  o.v = v;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) o.d[i] = R(0);
+  return o;
+}
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> operator*(R s, const Dual<Dual<R, NV>, NW>& a) {
+  Dual<Dual<R, NV>, NW> o;
+  o.v = s * a.v;
+#pragma unroll
+  for (int i = 0; i < NW; ++i) o.d[i] = s * a.d[i];
+  return o;
+}
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> operator-(R s, const Dual<Dual<R, NV>, NW>& a) {
+  Dual<Dual<R, NV>, NW> o;
+  o.v = s - a.v;
+#pragma unroll
+  for (int i = 0; i < NW; ++i) o.d[i] = R(0) - a.d[i];
+  return o;
+}
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> operator/(R s, const Dual<Dual<R, NV>, NW>& a) {
+  Dual<Dual<R, NV>, NW> c;
+  c.v = dual_const<R, NV>(s);
+#pragma unroll
+  for (int i = 0; i < NW; ++i) c.d[i] = dual_const<R, NV>(R(0));
+  return c / a;
+}
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> dsin(const Dual<Dual<R, NV>, NW>& a) {
+  Dual<Dual<R, NV>, NW> o;
+  const Dual<R, NV> c = dcos(a.v);
+  o.v = dsin(a.v);
+#pragma unroll
+  for (int i = 0; i < NW; ++i) o.d[i] = c * a.d[i];
+  return o;
+}
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> dcos(const Dual<Dual<R, NV>, NW>& a) {
+  Dual<Dual<R, NV>, NW> o;
+  const Dual<R, NV> s = R(0) - dsin(a.v);
+  o.v = dcos(a.v);
+#pragma unroll
+  for (int i = 0; i < NW; ++i) o.d[i] = s * a.d[i];
+  return o;
+}
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> datan2(const Dual<Dual<R, NV>, NW>& y, const Dual<Dual<R, NV>, NW>& x) {
+  Dual<Dual<R, NV>, NW> o;
+  const Dual<R, NV> den = x.v * x.v + y.v * y.v;
+  o.v = datan2(y.v, x.v);
+#pragma unroll
+  for (int i = 0; i < NW; ++i) o.d[i] = (x.v * y.d[i] - y.v * x.d[i]) / den;
+  return o;
+}
+// dclamp's rule at every order: inside [lo, hi] (inclusive) the clamp is the identity, outside a constant
+template <typename R, int NV, int NW>
+MPCB_DEV Dual<Dual<R, NV>, NW> dclamp(const Dual<Dual<R, NV>, NW>& a, R lo, R hi) {
+  Dual<Dual<R, NV>, NW> o;
+  const bool in = a.v.v >= lo && a.v.v <= hi;
+  o.v = dclamp(a.v, lo, hi);
+#pragma unroll
+  for (int i = 0; i < NW; ++i) o.d[i] = in ? a.d[i] : dual_const<R, NV>(R(0));
+  return o;
+}
+
+// A system parameter p[i] as a number of type P: a plain constant, or (P a nested dual) the variable of the outer
+// derivative when i == seed, else a constant.
+template <typename R, typename P>
+struct DynParam {
+  static MPCB_DEV P get(const DynParams& dp, int i, int) { return (P)dp.p[i]; }
+};
+template <typename R, int NV>
+struct DynParam<R, Dual<Dual<R, NV>, 1>> {
+  static MPCB_DEV Dual<Dual<R, NV>, 1> get(const DynParams& dp, int i, int seed) {
+    Dual<Dual<R, NV>, 1> o;
+    o.v = dual_const<R, NV>((R)dp.p[i]);
+    o.d[0] = dual_const<R, NV>(i == seed ? R(1) : R(0));
+    return o;
+  }
+};
+
 // the same vocabulary on plain numbers
 MPCB_DEV float dsin(float a) { return sinf(a); }
 MPCB_DEV double dsin(double a) { return sin(a); }
@@ -118,12 +209,16 @@ MPCB_DEV float dclamp(float a, float lo, float hi) { return a < lo ? lo : (a > h
 MPCB_DEV double dclamp(double a, double lo, double hi) { return a < lo ? lo : (a > hi ? hi : a); }
 
 // ------------------------------------------------------------------ the two systems
+// The parameter number type P is R by default; a nested dual P differentiates in the learnable parameter `seed`
+// (cartpole p[0..3], pendulum p[0..2]).  force_mag / max_torque and dt are constants of type R.
 // cartpole (mpc/env_dx/cartpole.py:63-96): state (x, dx, cos th, sin th, dth), one control (force)
-template <typename R, typename T>
-MPCB_DEV void cartpole_step(const DynParams& dp, const T (&s)[5], const T& u_in, T (&o)[5]) {
-  const R gravity = (R)dp.p[0], masscart = (R)dp.p[1], masspole = (R)dp.p[2], length = (R)dp.p[3];
+template <typename R, typename T, typename P = R>
+MPCB_DEV void cartpole_step(const DynParams& dp, const T (&s)[5], const T& u_in, T (&o)[5], int seed = -1) {
+  using DP = DynParam<R, P>;
+  const P gravity = DP::get(dp, 0, seed), masscart = DP::get(dp, 1, seed), masspole = DP::get(dp, 2, seed),
+          length = DP::get(dp, 3, seed);
   const R force_mag = (R)dp.p[4], dt = (R)dp.p[5];
-  const R total_mass = masspole + masscart, polemass_length = masspole * length;
+  const P total_mass = masspole + masscart, polemass_length = masspole * length;
   const T u = dclamp(u_in, -force_mag, force_mag);
   const T th = datan2(s[3], s[2]);
   const T cart_in = (R(1) / total_mass) * (u + polemass_length * (s[4] * s[4] * s[3]));
@@ -138,9 +233,11 @@ MPCB_DEV void cartpole_step(const DynParams& dp, const T (&s)[5], const T& u_in,
   o[4] = s[4] + dt * th_acc;
 }
 // pendulum, `simple` parametrisation (mpc/env_dx/pendulum.py:49-84): state (cos th, sin th, dth), one control (torque)
-template <typename R, typename T>
-MPCB_DEV void pendulum_step(const DynParams& dp, const T (&s)[3], const T& u_in, T (&o)[3]) {
-  const R g = (R)dp.p[0], m = (R)dp.p[1], l = (R)dp.p[2], max_torque = (R)dp.p[4], dt = (R)dp.p[5];
+template <typename R, typename T, typename P = R>
+MPCB_DEV void pendulum_step(const DynParams& dp, const T (&s)[3], const T& u_in, T (&o)[3], int seed = -1) {
+  using DP = DynParam<R, P>;
+  const P g = DP::get(dp, 0, seed), m = DP::get(dp, 1, seed), l = DP::get(dp, 2, seed);
+  const R max_torque = (R)dp.p[4], dt = (R)dp.p[5];
   const T u = dclamp(u_in, -max_torque, max_torque);
   const T th = datan2(s[1], s[0]);
   const T newdth = s[2] + dt * ((R(3.) * g / (R(2.) * l)) * s[1] + (R(3.) / (m * l * l)) * u);
@@ -172,22 +269,23 @@ inline bool dyn_kind_dims(int kind, int& n, int& m) {
 }
 
 // one step of a known kind; a passthrough kind copies u (before the system's own clamp) into the first M states
-template <typename R, int KIND, typename T>
-MPCB_DEV void dyn_step(const DynParams& dp, const T (&s)[DynDims<KIND>::N], const T& u, T (&o)[DynDims<KIND>::N]) {
+template <typename R, int KIND, typename T, typename P = R>
+MPCB_DEV void dyn_step(const DynParams& dp, const T (&s)[DynDims<KIND>::N], const T& u, T (&o)[DynDims<KIND>::N],
+                       int seed = -1) {
   if constexpr ((KIND & DYN_CTRL_PASSTHROUGH) != 0) {
     constexpr int SYS = KIND & ~DYN_CTRL_PASSTHROUGH, NI = DynDims<SYS>::N;
     static_assert(DynDims<SYS>::M == 1, "the known systems have one control");
     T si[NI], oi[NI];
 #pragma unroll
     for (int i = 0; i < NI; ++i) si[i] = s[1 + i];
-    dyn_step<R, SYS, T>(dp, si, u, oi);
+    dyn_step<R, SYS, T, P>(dp, si, u, oi, seed);
     o[0] = u;
 #pragma unroll
     for (int i = 0; i < NI; ++i) o[1 + i] = oi[i];
   } else if constexpr (KIND == DYN_CARTPOLE) {
-    cartpole_step<R, T>(dp, s, u, o);
+    cartpole_step<R, T, P>(dp, s, u, o, seed);
   } else {
-    pendulum_step<R, T>(dp, s, u, o);
+    pendulum_step<R, T, P>(dp, s, u, o, seed);
   }
 }
 
@@ -297,6 +395,66 @@ __global__ void __launch_bounds__(128) dyn_linearize_kernel(const DynArgs a) {
   }
 }
 
+// Learnable parameters theta of a system: its first NP entries of DynParams::p (cartpole gravity, masscart, masspole,
+// length; pendulum g, m, l).  force_mag / max_torque and dt are constants.
+template <int KIND>
+struct DynLearnable;
+template <>
+struct DynLearnable<DYN_CARTPOLE> { static constexpr int NP = 4; };
+template <>
+struct DynLearnable<DYN_PENDULUM> { static constexpr int NP = 3; };
+
+struct DynVjpArgs {
+  int B, T, kind;
+  DynParams dp;
+  const void *x, *u, *dF, *df;
+  void *first, *second;           // [T-1, B, NP] each; either may be NULL
+};
+
+// Vector-Jacobian product of dyn_linearize_kernel in theta, one thread per (t, problem), t < T-1.  With z = [x; u],
+// J = dx'/dz and f = x' - J z at (x[t,b], u[t,b]):
+//   first[t,b,k]  = sum_r df_r dx'_r/dtheta_k                        (J held constant: the reference's gradient)
+//   second[t,b,k] = sum_{r,j} (dF_rj - df_r z_j) dJ_rj/dtheta_k      (what J's own dependence on theta adds)
+// so first + second = d/dtheta_k (<dF, J> + <df, f>).  One pass per theta_k over the nested dual Dual<Dual<R, P>, 1>:
+// the inner dual is the Jacobian dyn_linearize_kernel forms, the outer one carries d/dtheta_k, so its derivative part
+// holds dx'/dtheta_k and dJ/dtheta_k.  The clamp follows dclamp: a saturated control has no u column at any order.
+template <typename R, int KIND>
+__global__ void __launch_bounds__(128) dyn_linearize_vjp_kernel(const DynVjpArgs a) {
+  constexpr int N = DynDims<KIND>::N, M = DynDims<KIND>::M, P = N + M, NP = DynLearnable<KIND>::NP;
+  static_assert(M == 1, "the known systems have one control");
+  using D2 = Dual<Dual<R, P>, 1>;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)(a.T - 1) * a.B) return;
+  const R* gdF = (const R*)a.dF + i * N * P;
+  const R* gdf = (const R*)a.df + i * N;
+  R z[P];
+#pragma unroll
+  for (int k = 0; k < N; ++k) z[k] = ((const R*)a.x)[i * N + k];
+  z[N] = ((const R*)a.u)[i * M];
+#pragma unroll 1
+  for (int k = 0; k < NP; ++k) {
+    D2 s[N], o[N], u;
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+      s[j].v = dual_var<R, P>(z[j], j);
+      s[j].d[0] = dual_const<R, P>(R(0));
+    }
+    u.v = dual_var<R, P>(z[N], N);
+    u.d[0] = dual_const<R, P>(R(0));
+    dyn_step<R, KIND, D2, D2>(a.dp, s, u, o, k);
+    R first = R(0), second = R(0);
+#pragma unroll
+    for (int r = 0; r < N; ++r) {
+      const R dfr = gdf[r];
+      first += dfr * o[r].d[0].v;
+#pragma unroll
+      for (int j = 0; j < P; ++j) second += (gdF[r * P + j] - dfr * z[j]) * o[r].d[0].d[j];
+    }
+    if (a.first != nullptr) ((R*)a.first)[i * NP + k] = first;
+    if (a.second != nullptr) ((R*)a.second)[i * NP + k] = second;
+  }
+}
+
 template <typename R>
 int launch_dyn_rollout(const DynArgs& a, cudaStream_t stream) {
   const int grid = (a.B + 127) / 128;
@@ -319,6 +477,17 @@ int launch_dyn_linearize(const DynArgs& a, cudaStream_t stream) {
   else if (a.kind == CP) dyn_linearize_kernel<R, CP><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == PP) dyn_linearize_kernel<R, PP><<<grid, 128, 0, stream>>>(a);
   else return 2;
+  return cudaGetLastError() == cudaSuccess ? 0 : 5;
+}
+// the VJP of the linearisation of a known system (no passthrough kinds: the slew-rate tail linearises the system)
+template <typename R>
+int launch_dyn_linearize_vjp(const DynVjpArgs& a, cudaStream_t stream) {
+  const size_t items = (size_t)(a.T - 1) * a.B;
+  if (a.kind != DYN_CARTPOLE && a.kind != DYN_PENDULUM) return 2;
+  if (items == 0) return 0;
+  const int grid = (int)((items + 127) / 128);
+  if (a.kind == DYN_CARTPOLE) dyn_linearize_vjp_kernel<R, DYN_CARTPOLE><<<grid, 128, 0, stream>>>(a);
+  else dyn_linearize_vjp_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }
 

@@ -8,6 +8,7 @@ does - but they also carry ``mpcb200_kind`` / ``mpcb200_params()``.  ``MPC.forwa
 CUDA tensors, replaces
   * ``util.get_traj``            (T-1 Python calls of the Module per iteration)        -> ``mpcb200_dyn_rollout``
   * ``MPC.linearize_dynamics``   ((T-1)*n_state autograd passes in AUTO_DIFF mode)     -> ``mpcb200_dyn_linearize``
+  * its differentiable form in the solve's backward (autograd of those passes)      -> ``mpcb200_dyn_linearize_vjp``
   * the Module rollout of ``lqr_forward`` (reference mpc/lqr_step.py:224-225)          -> inside the step kernel
 so that one iLQR iteration is three kernel launches plus the best-iterate bookkeeping.
 """
@@ -28,6 +29,8 @@ DYN_LINEAR, DYN_CARTPOLE, DYN_PENDULUM = 0, 1, 2
 DYN_CTRL_PASSTHROUGH = 16
 DYN_DIMS = {DYN_CARTPOLE: (5, 1), DYN_PENDULUM: (3, 1)}       # (n_state, n_ctrl) of each known system
 DYN_DIMS.update({k | DYN_CTRL_PASSTHROUGH: (n + m, m) for k, (n, m) in DYN_DIMS.items()})
+# number of learnable parameters of each system: the leading entries of its `params` tensor (mpcb200_params()[:NP])
+DYN_NPARAMS = {DYN_CARTPOLE: 4, DYN_PENDULUM: 3}
 
 _scope = threading.local()      # depth and epoch of the enclosing params_scope() on this thread
 _epochs = itertools.count(1)    # process-wide: two threads' scopes never share an epoch (the cache is per module)
@@ -221,3 +224,64 @@ def dyn_linearize_raw(kind, params, T, x, u):
         rc = fn(kind, _dyn_array(params), B, T, ptr(x_), ptr(u_), ptr(F), ptr(f), stream_handle(dev))
     check(rc, "mpcb200_dyn_linearize")
     return F, f
+
+
+def dyn_linearize_vjp_raw(kind, params, T, x, u, dF, df):
+    """(first, second) [T-1, B, NP]: the vector-Jacobian product of dyn_linearize_raw(kind, params, T, x, u) in the
+    system's learnable parameters theta = params[:NP] (DYN_NPARAMS), per (t, b), ONE kernel.  With z = [x; u],
+    J = dx'/dz and f = x' - J z: first = sum_r df_r dx'_r/dtheta (J held constant), second = sum_rj (dF_rj - df_r z_j)
+    dJ_rj/dtheta; their sum over (t, b) is the gradient of <dF, F> + <df, f>."""
+    if kind not in DYN_NPARAMS:
+        raise MpcB200Error(f"dyn_linearize_vjp_raw: kind {kind} is not a known system (passthrough kinds have no VJP)")
+    n, m = DYN_DIMS[kind]
+    B = x.shape[1] if x.dim() == 3 else -1
+    dtype, dev = x.dtype, x.device
+    for name, t, shape in (("dF", dF, (T - 1, B, n, n + m)), ("df", df, (T - 1, B, n))):
+        if tuple(t.shape) != shape:
+            raise MpcB200Error(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
+        if t.dtype != dtype or t.device != dev:
+            raise MpcB200Error(f"{name} is {t.dtype} on {t.device}, x is {dtype} on {dev}")
+    _check_dyn_shapes(kind, T, "x", x, "TBN", u)
+    NP = DYN_NPARAMS[kind]
+    x_, u_, dF_, df_ = (t.detach().contiguous() for t in (x, u.to(dtype), dF, df))
+    first = torch.empty(T - 1, B, NP, dtype=dtype, device=dev)
+    second = torch.empty(T - 1, B, NP, dtype=dtype, device=dev)
+    fn = _lib.entry("mpcb200_dyn_linearize_vjp", dtype)
+    with _on_device(dev):
+        rc = fn(kind, _dyn_array(params), B, T, ptr(x_), ptr(u_), ptr(dF_), ptr(df_), ptr(first), ptr(second),
+                stream_handle(dev))
+    check(rc, "mpcb200_dyn_linearize_vjp")
+    return first, second
+
+
+class DynLinearize(torch.autograd.Function):
+    """(F, f) = dyn_linearize_raw along detached (x, u), differentiable in the system's `params` tensor: the backward
+    is the VJP kernel, summed over (t, b).  One module-level Function (DESIGN.md section 3.2): a class made per call
+    would be a new Python type, and a new autograd node type, on every solve.  The forward reads nothing from the
+    device: the parameter values are the host numbers the caller took from mpcb200_params()."""
+
+    @staticmethod
+    def forward(ctx, params, kind, kparams, T, x, u):
+        F, f = dyn_linearize_raw(kind, kparams, T, x, u)
+        ctx.save_for_backward(x, u)
+        ctx.kind, ctx.kparams, ctx.T = kind, kparams, T
+        ctx.p_dtype, ctx.p_device = params.dtype, params.device
+        return F, f
+
+    @staticmethod
+    def backward(ctx, dF, df):
+        x, u = ctx.saved_tensors
+        first, second = dyn_linearize_vjp_raw(ctx.kind, ctx.kparams, ctx.T, x, u, dF, df)
+        grad = (first + second).sum((0, 1))
+        return grad.to(dtype=ctx.p_dtype, device=ctx.p_device), None, None, None, None, None
+
+
+def linearize_known(dynamics, kind, kparams, T, x, u):
+    """(F, f) of the known system `dynamics` (kind DYN_CARTPOLE or DYN_PENDULUM) along (x, u), as MPC's differentiable
+    tail needs it: through DynLinearize when autograd records and dynamics.params requires grad, otherwise one
+    dyn_linearize_raw launch and no graph.  x and u are detached either way (no gradient reaches the linearisation
+    point)."""
+    params = getattr(dynamics, "params", None)
+    if torch.is_grad_enabled() and isinstance(params, torch.Tensor) and params.requires_grad:
+        return DynLinearize.apply(params, kind, kparams, T, x.detach(), u.detach())
+    return dyn_linearize_raw(kind, kparams, T, x, u)

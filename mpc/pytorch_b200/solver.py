@@ -484,16 +484,29 @@ class MPC(Module):
             return H.detach(), lin.detach(), costs.detach()
         return H, lin, costs
 
+    def _kernel_linearization(self, dynamics, x, diff):
+        """(kind, params) when linearize_dynamics runs in the kernels, else (DYN_LINEAR, None): a known system under
+        ANALYTIC or AUTO_DIFF at its own (n, m) on CUDA float32 / float64 tensors (dynamics.known_kind).  With diff,
+        only a system itself, not a passthrough kind: the VJP kernel differentiates the systems' own parameters."""
+        from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, known_kind
+        if self.grad_method not in (GradMethods.ANALYTIC, GradMethods.AUTO_DIFF):
+            return DYN_LINEAR, None
+        kind, kparams = known_kind(dynamics, self.n_state, self.n_ctrl, x)
+        if diff and kind & DYN_CTRL_PASSTHROUGH:
+            return DYN_LINEAR, None
+        return kind, kparams
+
     def linearize_dynamics(self, x, u, dynamics, diff):
         """First-order expansion x' ~ F [x;u] + f of Module dynamics (reference :490-601),
         evaluated for all T-1 steps and the whole batch at once."""
         T, n, m = self.T, self.n_state, self.n_ctrl
         B = x.shape[1]
-        if not diff and self.grad_method in (GradMethods.ANALYTIC, GradMethods.AUTO_DIFF):
-            from .dynamics import known_kind, dyn_linearize_raw
-            kind, kparams = known_kind(dynamics, n, m, x)
-            if kind:           # exact Jacobians of a known system by forward-mode duals, one kernel
-                return dyn_linearize_raw(kind, kparams, T, x, u)
+        kind, kparams = self._kernel_linearization(dynamics, x, diff)
+        if kind:               # exact Jacobians of a known system by forward-mode duals, one kernel
+            from .dynamics import dyn_linearize_raw, linearize_known
+            if diff:           # differentiable in the system's parameters through the VJP kernel
+                return linearize_known(dynamics, kind, kparams, T, x, u)
+            return dyn_linearize_raw(kind, kparams, T, x, u)
         xs = x[:-1].detach().reshape(-1, n)
         us = u[:-1].detach().reshape(-1, m)
         if self.grad_method == GradMethods.ANALYTIC:

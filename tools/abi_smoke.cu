@@ -148,6 +148,22 @@ static int run_dyn(int kind, int B, int T) {
   if (rc) return printf("dyn rollout rc=%d\n", rc), 1;
   rc = mpcb200_dyn_linearize_f32(kind, dyn, B, T, dx.p, du.p, dF.p, df.p, nullptr);
   if (rc) return printf("dyn linearize rc=%d\n", rc), 1;
+  {  // parameter VJP of the linearisation with (dF, df) = (F, f); second output omitted once
+    const int np = n == 5 ? 4 : 3;
+    Dev<float> first((size_t)(T - 1) * B * np), second((size_t)(T - 1) * B * np);
+    rc = mpcb200_dyn_linearize_vjp_f32(kind, dyn, B, T, dx.p, du.p, dF.p, df.p, first.p, second.p, nullptr);
+    if (rc) return printf("dyn linearize vjp rc=%d\n", rc), 1;
+    rc = mpcb200_dyn_linearize_vjp_f32(kind, dyn, B, T, dx.p, du.p, dF.p, df.p, first.p, nullptr, nullptr);
+    if (rc) return printf("dyn linearize vjp (first only) rc=%d\n", rc), 1;
+    rc = mpcb200_dyn_linearize_vjp_f32(kind | MPCB200_DYN_CTRL_PASSTHROUGH, dyn, B, T, dx.p, du.p, dF.p, df.p, first.p,
+                                       second.p, nullptr);
+    if (rc != MPCB200_ERR_BAD_DIMS) return printf("dyn linearize vjp (passthrough) rc=%d\n", rc), 1;
+    if (cudaDeviceSynchronize() != cudaSuccess) return printf("CUDA error: %s\n", cudaGetErrorString(cudaGetLastError())), 1;
+    int bad = 0;
+    for (float v : first.down()) bad += !std::isfinite(v);
+    for (float v : second.down()) bad += !std::isfinite(v);
+    if (bad) return printf("dyn linearize vjp: nonfinite %d\n", bad), 1;
+  }
   mpcb200_dims d = {B, T, n, m, T - 1, 1, 1, 0, 0, 3, 20, 1, kind};
   mpcb200_params prm = {-2.0, 2.0, 0.0, 0.5, {0}};
   for (int i = 0; i < 8; ++i) prm.dyn[i] = dyn[i];
