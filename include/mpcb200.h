@@ -144,9 +144,8 @@ int mpcb200_lqr_step_f64(const mpcb200_dims* dims, const mpcb200_params* params,
  *   df = -dlam[1:], dx_init = -dlam[0].
  * r = [dl_dx; dl_du] enters only through r_x.  dF has F_T slices (slice T-1, if present, is zeroed).
  * df may be NULL (reference returns an empty tensor when f is empty).
- * workspace: optional device buffer of 2*T*B*n elements (lambda_t, dlambda_t).  With it the
- * call runs as two kernels (sequential costates, then fully parallel outer products - the fast
- * path); with NULL it runs as one fused kernel.  Results are identical.
+ * workspace: required device buffer of 2*T*B*n elements (lambda_t, dlambda_t; MPCB200_ERR_NULL_POINTER
+ * without it).  The call runs as two kernels: sequential costates, then fully parallel outer products.
  */
 int mpcb200_lqr_grad_f32(const mpcb200_dims* dims,
                          const float* C, const float* c, const float* F,
@@ -170,9 +169,15 @@ int mpcb200_lqr_grad_f64(const mpcb200_dims* dims,
  *   2. the masked LQR step from the zero trajectory (c = r, x_init = 0, u_zero_I = I, default line search),
  *      i.e. the nested MPC(lqr_iter=1) of :328-340, with the step kernel;
  *   3. costates and outer products (mpcb200_lqr_grad_*, :342-404).
- * Outputs dx_init[B,n] dC[T,B,p,p] dc[T,B,p] dF[F_T,B,n,p] df[T-1,B,n] (df only if dims->has_f).
+ * The library picks the kernels.  The nested step keeps its gains in the workspace at the horizons and shapes where
+ * mpcb200_step_prefers_workspace says a step does, so every horizon a step with Ks/ks takes works here too.  Where it
+ * does not, and the column-pair kernel takes the shape, alignment and horizon, steps 2 and 3 run as one fused kernel
+ * (2 launches in all); otherwise the masked step kernel and the two gradient kernels run (4 launches).
+ * Outputs dx_init[B,n] dC[T,B,p,p] dc[T,B,p] dF[F_T,B,n,p] df[T-1,B,n] (df only if dims->has_f; F and dF may be
+ * NULL when T = 1 and F_T = 0).
  * workspace: device buffer of mpcb200_adjoint_workspace_bytes(dims, elem_size) bytes (scratch; contents
- * undefined on return).  Only dims->{B,T,n,m,F_T,has_f,bounds_kind} and params->{u_lo,u_hi} are read.
+ * undefined on return).  The size includes the nested step's Ks/ks where that step keeps its gains in a buffer.
+ * Only dims->{B,T,n,m,F_T,has_f,bounds_kind}, the time strides of C, c and F, and params->{u_lo,u_hi} are read.
  */
 size_t mpcb200_adjoint_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size);
 int mpcb200_lqr_adjoint_f32(const mpcb200_dims* dims, const mpcb200_params* params,

@@ -228,6 +228,15 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const StepC
   return counted(e->ops[sizeof(R) == 8].step(a, smem, (cudaStream_t)stream));
 }
 
+// whether the step of `d` keeps its gains in the caller's Ks/ks (mpcb200_step_prefers_workspace)
+static int gains_in_workspace(const mpcb200_dims* d, int elem_size, int knob) {
+  const bool passthrough = (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0;
+  if (!passthrough && runs_large(d->n, d->m, knob)) return 1;   // the large-shape step keeps its gains in Ks/ks
+  const Instance* e = find_step(d);
+  if (e == nullptr) return 1;                   // no instance: the step call itself reports it
+  return e->ops[elem_size == 8].prefers_workspace(d->T, smem_optin_or_h100());
+}
+
 template <typename R>
 static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, const R* new_x,
                      const R* new_u, const R* dx, const R* du, const R* dl_dx, R* dx_init, R* dC, R* dc,
@@ -235,7 +244,8 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
   int rc = check_dims(d);
   if (rc) return rc;
   if (C == nullptr || c == nullptr || new_x == nullptr || new_u == nullptr || dx == nullptr ||
-      du == nullptr || dl_dx == nullptr || dx_init == nullptr || dC == nullptr || dc == nullptr)
+      du == nullptr || dl_dx == nullptr || dx_init == nullptr || dC == nullptr || dc == nullptr ||
+      workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (d->F_T > 0 && (F == nullptr || dF == nullptr)) return MPCB200_ERR_NULL_POINTER;
   const Instance* e = find(d->n, d->m);
@@ -249,20 +259,30 @@ static int grad_impl(const mpcb200_dims* d, const R* C, const R* c, const R* F, 
   const TimeStrides ts = time_strides(d);
   a.C_ts = ts.C; a.c_ts = ts.c; a.F_ts = ts.F;
   return counted(large ? large_grad_launch<R>(a, d->n, d->m, (cudaStream_t)stream)
-                       : e->ops[sizeof(R) == 8].grad(a, (cudaStream_t)stream),
-                 workspace != nullptr ? 2 : 1);
+                       : e->ops[sizeof(R) == 8].grad(a, (cudaStream_t)stream), 2);
 }
 // ---------------------------------------------------------------------------------------------
 // KKT adjoint in one call (reference LQRStepFn.backward, mpc/lqr_step.py:312-407)
 // ---------------------------------------------------------------------------------------------
+// dims of the nested masked step (reference :328-340: MPC(lqr_iter=1, u_zero_I=I) with its defaults): the caller's,
+// without f, bounds or delta_u; its c is the dense -r, C and F keep the caller's strides
+static mpcb200_dims adjoint_step_dims(const mpcb200_dims* d) {
+  mpcb200_dims ds = *d;
+  ds.has_f = 0; ds.bounds_kind = 0; ds.has_zero_mask = 1; ds.has_delta_u = 0;
+  ds.max_ls_iter = 10; ds.pnqp_max_iter = 20; ds.do_rollout = 1; ds.dynamics_kind = 0;
+  ds.c_tstride = 0; ds.f_tstride = 0;
+  return ds;
+}
+
 struct AdjLayout {                    // workspace carve-up (byte offsets, every piece 256-byte aligned)
   size_t negr, zeros, dx, du, costate, scal, mask, maskf, Ks, ks, total;
-  bool gains;                         // Ks/ks of the nested solve (the large-shape step keeps its gains there)
+  bool gains;                         // Ks/ks of the nested step, where that step keeps its gains in a caller buffer
 };
 static size_t up256(size_t v) { return (v + 255) / 256 * 256; }
-static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz, int knob) {
+static AdjLayout adj_layout(const mpcb200_dims* d, size_t sz, int knob) {
   AdjLayout l;
-  const size_t TB = (size_t)T * B;
+  const int B = d->B, n = d->n, m = d->m;
+  const size_t TB = (size_t)d->T * B;
   size_t o = 0;
   l.negr = o;    o += up256(TB * (n + m) * sz);
   l.zeros = o;   o += up256((TB * (n + m) + (size_t)B * n) * sz);     // cur_x, cur_u, x_init of the nested solve
@@ -272,7 +292,8 @@ static AdjLayout adj_layout(int B, int T, int n, int m, size_t sz, int knob) {
   l.scal = o;    o += up256((size_t)3 * B * sz);
   l.mask = o;    o += up256(TB * m);
   l.maskf = o;   o += up256(TB * m * sz);                               // the same mask as element-typed 0/1 (rides on the TMA tile)
-  l.gains = runs_large(n, m, knob);
+  const mpcb200_dims ds = adjoint_step_dims(d);
+  l.gains = gains_in_workspace(&ds, (int)sz, knob) != 0;
   l.Ks = l.ks = 0;
   if (l.gains) {
     l.Ks = o;    o += up256(TB * m * n * sz);
@@ -322,7 +343,7 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
   rc = check_bounds(d, u_lower, u_upper);
   if (rc) return rc;
   if (d->has_f && df == nullptr) return MPCB200_ERR_NULL_POINTER;
-  const AdjLayout l = adj_layout(d->B, d->T, d->n, d->m, sizeof(R), knob);
+  const AdjLayout l = adj_layout(d, sizeof(R), knob);
   if (workspace_bytes < l.total || !aligned16(workspace)) return MPCB200_ERR_BAD_DIMS;
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
@@ -341,11 +362,8 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
       (R*)(ws + l.maskf), z0);
   if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
   g_launches.fetch_add(1);
-  // nested masked LQR step from the zero trajectory (reference :328-340: MPC(lqr_iter=1, u_zero_I=I) with its defaults)
-  mpcb200_dims ds = *d;
-  ds.has_f = 0; ds.bounds_kind = 0; ds.has_zero_mask = 1; ds.has_delta_u = 0;
-  ds.max_ls_iter = 10; ds.pnqp_max_iter = 20; ds.do_rollout = 1; ds.dynamics_kind = 0;
-  ds.c_tstride = 0; ds.f_tstride = 0;         // c of the nested solve is the dense -r; C and F keep the caller's strides
+  // nested masked LQR step from the zero trajectory
+  const mpcb200_dims ds = adjoint_step_dims(d);
   mpcb200_params ps;
   std::memset(&ps, 0, sizeof(ps));
   ps.ls_decay = 0.2;
@@ -353,8 +371,12 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
   sc.C = C; sc.c = negr; sc.F = F; sc.x_init = z0; sc.cur_x = zx; sc.cur_u = zu; sc.u_zero_I = mask;
   sc.new_x = dxs; sc.new_u = dus; sc.costs = scal; sc.full_du_norm = scal + d->B; sc.alphas = scal + 2 * d->B;
   // Preferred: ONE launch of the column-pair kernel doing solve + costates + outer products (C, F read from HBM
-  // once, d tau kept in shared memory).  Shapes / alignments it does not take fall through to the 3-launch path.
-  {
+  // once, d tau kept in shared memory).  Shapes / alignments it does not take fall through to the 3-launch path, and
+  // so do horizons where the nested step keeps its gains in Ks/ks: there the masked step + gradient kernels are the
+  // faster ones.  Config 5 ((16,4) f32, B = 4096, T = 50, past the KREDUCE switch) through LQRStepFn.backward on an
+  // H100 80GB HBM3 at 700 W: fused kernel 1.49 ms best / 1.96 ms median, masked step + gradient kernels 1.32 / 1.62 ms
+  // (tools/exp_grad.py, DESIGN.md section 4).
+  if (!l.gains) {
     AdjExtra ax;
     ax.c = c; ax.x = new_x; ax.u = new_u; ax.dC = dC; ax.dc = dc; ax.dF = dF; ax.df = d->has_f ? df : nullptr;
     ax.dx_init = dx_init; ax.has_df = d->has_f ? 1 : 0;
@@ -365,7 +387,8 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
     if (rc == 0) return 0;
     if (rc != MPCB200_ERR_UNSUPPORTED_DIMS && rc != MPCB200_ERR_SMEM) return rc;
   }
-  // 3-launch path: the nested solve really reads its (zero) nominal trajectory
+  // 3-launch path: the nested solve really reads its (zero) nominal trajectory, and keeps its gains in the workspace
+  // where a step call with Ks/ks would (gains_in_workspace)
   if (cudaMemsetAsync(zeros, 0, TB * (d->n + d->m) * sizeof(R), st) != cudaSuccess) return MPCB200_ERR_LAUNCH;
   sc.u_lower = sc.u_upper = nullptr;
   if (l.gains) {
@@ -373,7 +396,7 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
     sc.ks = (R*)(ws + l.ks);
   }
   rc = step_impl<R>(&ds, &ps, sc, knob, stream);
-  if (rc) return rc;               // MPCB200_ERR_SMEM at long horizons: use the two-call path with Ks/ks buffers
+  if (rc) return rc;
   return grad_impl<R>(d, C, c, F, new_x, new_u, dxs, dus, dl_dx, dx_init, dC, dc, dF, d->has_f ? df : (R*)nullptr,
                       ws + l.costate, knob, stream);
 }
@@ -437,15 +460,6 @@ static int dyn_vjp_impl(int kind, const double* dyn, int B, int T, const R* x, c
   for (int i = 0; i < 8; ++i) a.dp.p[i] = dyn[i];
   a.x = x; a.u = u; a.dF = dF; a.df = df; a.first = first; a.second = second;
   return counted(launch_dyn_linearize_vjp<R>(a, (cudaStream_t)stream));
-}
-
-// whether the step of `d` keeps its gains in the caller's Ks/ks (mpcb200_step_prefers_workspace)
-static int gains_in_workspace(const mpcb200_dims* d, int elem_size, int knob) {
-  const bool passthrough = (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0;
-  if (!passthrough && runs_large(d->n, d->m, knob)) return 1;   // the large-shape step keeps its gains in Ks/ks
-  const Instance* e = find_step(d);
-  if (e == nullptr) return 1;                   // no instance: the step call itself reports it
-  return e->ops[elem_size == 8].prefers_workspace(d->T, smem_optin_or_h100());
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -871,7 +885,7 @@ int mpcb200_lqr_grad_f64(const mpcb200_dims* dims, const double* C, const double
 
 size_t mpcb200_adjoint_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
-  return adj_layout(dims->B, dims->T, dims->n, dims->m, (size_t)elem_size, kernel_knob()).total;
+  return adj_layout(dims, (size_t)elem_size, kernel_knob()).total;
 }
 int mpcb200_lqr_adjoint_f32(const mpcb200_dims* dims, const mpcb200_params* params, const float* C, const float* c,
                             const float* F, const float* new_x, const float* new_u, const float* dl_dx,

@@ -7,9 +7,9 @@
 // The adjoint solve that produces (dx,du) is the step kernel in masked mode (lqr_step.cuh).
 //
 // Mapping: P = n+m lanes per problem (lane j holds tau_j, dtau_j; lanes j<n hold lambda_j,
-// dlambda_j), 32/P problems per warp.  The kernel is store bound (dC,dF dominate), so the
-// outer products are written with a FLAT index over the warp's contiguous problems: every
-// store instruction covers one fully used 128-byte line; operands come from warp shuffles.
+// dlambda_j), 32/P problems per warp.  The outer products are store bound (dC,dF dominate), so
+// they are written with a FLAT index over the warp's contiguous problems: every store
+// instruction covers one fully used 128-byte line; operands come from warp shuffles.
 #pragma once
 #include "common.cuh"
 
@@ -19,7 +19,7 @@ struct GradArgs {
   int B, T, F_T, has_df;
   const void *C, *c, *F, *new_x, *new_u, *dx, *du, *dl_dx;
   void *dx_init, *dC, *dc, *dF, *df;
-  void* workspace;   // optional: 2*T*B*n elements (lambda, dlambda) -> two-kernel path
+  void* workspace;   // 2*T*B*n elements: lambda_t, dlambda_t
   long long C_ts, c_ts, F_ts;   // elements between consecutive time slices of C, c, F (0 = time invariant)
 };
 
@@ -34,128 +34,13 @@ struct GradCfg {
   static constexpr int TCHUNK = 4;        // time steps per warp in the outer-product kernel
 };
 
-template <typename R, int N, int M>
-__global__ void __launch_bounds__(GradCfg<R, N, M>::THREADS)
-lqr_grad_kernel(const GradArgs a) {
-  using K = GradCfg<R, N, M>;
-  constexpr int P = K::P, LP = K::LP, PPW = K::PPW;
-  const int T = a.T, B = a.B;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool writer_lane = lane < PPW * LP;
-  const int pi = writer_lane ? lane / LP : PPW - 1;
-  const int base = pi * LP;
-  const int j = writer_lane ? lane - base : LP - 1;
-  const int bw0 = (blockIdx.x * K::NW + warp) * PPW;   // first problem of this warp
-  const int b = bw0 + pi;
-  const bool valid = b < B;
-  const bool wr = writer_lane && valid;
-  const int bb = valid ? b : 0;                          // safe index for loads
-  const bool is_x = j < N;
-  const int jr = is_x ? j : N - 1;
-  const int nprob = min(PPW, B - bw0);                   // valid problems of this warp (may be <= 0)
-
-  const R* gC = (const R*)a.C;
-  const R* gc = (const R*)a.c;
-  const R* gF = (const R*)a.F;
-  const R* gx = (const R*)a.new_x;
-  const R* gu = (const R*)a.new_u;
-  const R* gdx = (const R*)a.dx;
-  const R* gdu = (const R*)a.du;
-  const R* grx = (const R*)a.dl_dx;
-  R* oC = (R*)a.dC;
-  R* oc = (R*)a.dc;
-  R* oF = (R*)a.dF;
-  R* of = (R*)a.df;
-
-  R lam = R(0), dlam = R(0);   // lambda_{t+1}[jr], dlambda_{t+1}[jr] held by x lanes
-  for (int t = T - 1; t >= 0; --t) {
-    const size_t tb = (size_t)t * B + bb;
-    // tau_t[j], dtau_t[j]
-    const R tj = is_x ? gx[tb * N + j] : gu[tb * M + (j - N)];
-    const R dj = is_x ? gdx[tb * N + j] : gdu[tb * M + (j - N)];
-
-    // ---- dF_t, df_t use lambda_{t+1} (reference :387-402)
-    if (t < T - 1) {
-      // flat over the warp's problems: element e -> (problem pe, row k, col cc); a uniform
-      // number of rounds keeps every lane in the shuffles
-      const size_t off = ((size_t)t * B + bw0) * N * P;
-      constexpr int TOT = PPW * N * P;
-      constexpr int ROUNDS = (TOT + 31) / 32;
-#pragma unroll 4
-      for (int rr = 0; rr < ROUNDS; ++rr) {
-        const int e = rr * 32 + lane;
-        const int ec = e < TOT ? e : TOT - 1;
-        const int pe = ec / (N * P), r = ec - pe * (N * P);
-        const int k = r / P, cc = r - k * P;
-        const R dl = shfl(dlam, pe * LP + k);
-        const R l = shfl(lam, pe * LP + k);
-        const R tc = shfl(tj, pe * LP + cc);
-        const R dc_ = shfl(dj, pe * LP + cc);
-        if (e < TOT && pe < nprob) oF[off + e] = -(dl * tc + l * dc_);
-      }
-    } else if (a.F_T == T) {
-      const size_t off = ((size_t)t * B + bw0) * N * P;
-      for (int e = lane; e < PPW * N * P; e += 32)
-        if (e / (N * P) < nprob) oF[off + e] = R(0);
-    }
-    if (t < T - 1 && a.has_df && wr && is_x) of[tb * N + j] = -dlam;
-
-    // ---- dC_t, dc_t (reference :346-353)
-    {
-      const size_t off = ((size_t)t * B + bw0) * P * P;
-      constexpr int TOT = PPW * P * P;
-      constexpr int ROUNDS = (TOT + 31) / 32;
-#pragma unroll 4
-      for (int rr = 0; rr < ROUNDS; ++rr) {
-        const int e = rr * 32 + lane;
-        const int ec = e < TOT ? e : TOT - 1;
-        const int pe = ec / (P * P), r = ec - pe * (P * P);
-        const int i = r / P, cc = r - i * P;
-        const R ti = shfl(tj, pe * LP + i);
-        const R di = shfl(dj, pe * LP + i);
-        const R tc = shfl(tj, pe * LP + cc);
-        const R dcc = shfl(dj, pe * LP + cc);
-        if (e < TOT && pe < nprob) oC[off + e] = R(-0.5) * (di * tc + ti * dcc);
-      }
-      if (wr) oc[tb * P + j] = -dj;
-    }
-
-    // ---- costates (reference :355-385): row jr of C_t[:n,:], column jr of F_t[:, :n]
-    R nl = R(0), ndl = R(0);
-    {
-      const R* Crow = gC + (size_t)t * a.C_ts + ((size_t)bb * P + jr) * P;
-#pragma unroll
-      for (int i = 0; i < P; ++i) {
-        const R cv = Crow[i];
-        nl += cv * shfl(tj, base + i);
-        ndl += cv * shfl(dj, base + i);
-      }
-      nl += gc[(size_t)t * a.c_ts + (size_t)bb * P + jr];
-      ndl -= grx[tb * N + jr];
-      if (t < T - 1) {
-        const R* Fc = gF + (size_t)t * a.F_ts + (size_t)bb * N * P + jr;
-#pragma unroll
-        for (int k = 0; k < N; ++k) {
-          const R fv = Fc[k * P];
-          nl += fv * shfl(lam, base + k);
-          ndl += fv * shfl(dlam, base + k);
-        }
-      }
-    }
-    lam = nl;
-    dlam = ndl;
-  }
-  if (wr && is_x) ((R*)a.dx_init)[(size_t)b * N + j] = -dlam;
-}
-
-
 // ---------------------------------------------------------------------------------------------
-// Two-kernel path (used when the caller provides a workspace of 2*T*B*n elements):
+// Two kernels, through the caller's workspace of 2*T*B*n elements:
 //   1. lqr_costate_kernel: the sequential part - lambda_t, dlambda_t backward in t (reference
 //      :355-385), next step's operands prefetched into registers; writes the costates to the
 //      workspace plus dx_init and df.
 //   2. lqr_outer_kernel: dC, dc, dF for every (t, b) independently (reference :346-353,387-395) -
-//      T x more parallelism than the fused loop, a pure streaming-store kernel.
+//      T x more parallelism than a loop over t, a pure streaming-store kernel.
 // ---------------------------------------------------------------------------------------------
 template <typename R, int N, int M>
 __global__ void __launch_bounds__(GradCfg<R, N, M>::THREADS)
@@ -335,10 +220,6 @@ template <typename R, int N, int M>
 int launch_grad(const GradArgs& a, cudaStream_t stream) {
   using K = GradCfg<R, N, M>;
   const int grid = (a.B + K::W - 1) / K::W;
-  if (a.workspace == nullptr) {
-    lqr_grad_kernel<R, N, M><<<grid, K::THREADS, 0, stream>>>(a);
-    return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH;
-  }
   lqr_costate_kernel<R, N, M><<<grid, K::THREADS, 0, stream>>>(a);
   if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
   const long long items = (long long)((a.B + K::PPW - 1) / K::PPW) * ((a.T + K::TCHUNK - 1) / K::TCHUNK);

@@ -511,8 +511,8 @@ MPCB_DEV void load_tau(const GradArgs& a, int n, int m, size_t tb, R* tau, R* dt
   }
 }
 
-// costates lambda_t, dlambda_t backward in t (:355-385), df, dx_init; with a workspace the costates go there for
-// large_outer_kernel, without one this kernel also writes the outer products of every t
+// costates lambda_t, dlambda_t backward in t (:355-385), df, dx_init; the costates go to the workspace for
+// large_outer_kernel
 template <typename R>
 __global__ void __launch_bounds__(LNT) lqr_large_costate_kernel(const GradArgs a, int n, int m) {
   extern __shared__ __align__(16) unsigned char sm[];
@@ -524,12 +524,11 @@ __global__ void __launch_bounds__(LNT) lqr_large_costate_kernel(const GradArgs a
   R* nlam = dlam + n;         // lambda_t, dlambda_t
   R* ndlam = nlam + n;
   R* wl = (R*)a.workspace;
-  R* wd = wl != nullptr ? wl + (size_t)T * B * n : nullptr;
+  R* wd = wl + (size_t)T * B * n;
   for (int t = T - 1; t >= 0; --t) {
     const size_t tb = (size_t)t * B + b;
     load_tau<R>(a, n, m, tb, tau, dtau);
     __syncthreads();
-    if (wl == nullptr) large_outer<R>(a, n, m, t, b, tau, dtau, lam, dlam);
     const R* Cb = (const R*)a.C + (size_t)t * a.C_ts + (size_t)b * p * p;
     const R* Fb = t < T - 1 ? (const R*)a.F + (size_t)t * a.F_ts + (size_t)b * n * p : nullptr;
     for (int j = tid; j < n; j += LNT) {
@@ -552,10 +551,8 @@ __global__ void __launch_bounds__(LNT) lqr_large_costate_kernel(const GradArgs a
       }
       nlam[j] = nl;
       ndlam[j] = ndl;
-      if (wl != nullptr) {
-        wl[tb * n + j] = nl;
-        wd[tb * n + j] = ndl;
-      }
+      wl[tb * n + j] = nl;
+      wd[tb * n + j] = ndl;
     }
     __syncthreads();
     for (int j = tid; j < n; j += LNT) {
@@ -596,7 +593,6 @@ int large_grad_launch(const GradArgs& a, int n, int m, cudaStream_t stream) {
   if (smem > 48 * 1024) return MPCB200_ERR_SMEM;
   lqr_large_costate_kernel<R><<<a.B, LNT, smem, stream>>>(a, n, m);
   if (cudaGetLastError() != cudaSuccess) return MPCB200_ERR_LAUNCH;
-  if (a.workspace == nullptr) return MPCB200_OK;
   lqr_large_outer_kernel<R><<<(unsigned)((size_t)a.T * a.B), LNT, smem, stream>>>(a, n, m);
   return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH;
 }

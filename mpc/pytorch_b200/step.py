@@ -492,50 +492,57 @@ _adj_plans = {}
 
 def lqr_adjoint_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dl_dx, dl_du, u_lower, u_upper, want_df, f_T=None,
                     validated=False):
-    """LQRStepFn.backward in ONE library call (prep + nested masked step + costates + outer products);
-    returns (dx_init, dC, dc, dF, df|None), or None when this shape needs the general multi-call path
-    (zero-padded instance, horizon too long for the shared-memory gain store).  `validated`: the tensors are the
-    ones LQRStepFn.forward checked and saved plus autograd's gradients of its outputs (shapes follow), so the
-    checks are not repeated on the backward path."""
+    """LQRStepFn.backward in ONE library call (mpcb200_lqr_adjoint_*: active set, nested masked step, costates and
+    outer products; the library picks the kernels for the shape and horizon); returns (dx_init, dC, dc, dF|None,
+    df|None).  The problem is staged as _problem stages it (a shape without an exact instance runs zero padded) and
+    the outputs are cropped as lqr_grad_raw crops them.  `validated`: the tensors are the ones LQRStepFn.forward
+    checked and saved plus autograd's gradients of its outputs (shapes follow), so the checks are not repeated on the
+    backward path."""
     n, m = n_state, n_ctrl
     if not validated:
         _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("new_x", new_x, "TBn"), ("new_u", new_u, "TBm"),
                   ("dl_dx", dl_dx, "TBn"), ("dl_du", dl_du, "TBm"), F=F, bounds=(u_lower, u_upper))
-    if _pick_instance(n, m, C.element_size()) != (n, m) or _is_empty(F):
-        return None
     dtype, dev = C.dtype, C.device
     B = C.shape[1]
-    F_T = F.shape[0]
-    kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev)
-    (C_, tsC), (c_, tsc), (F_, tsF) = _time_strided(C, dtype), _time_strided(c, dtype), _time_strided(F, dtype)
     esz = C.element_size()
-    # the entry point, the ctypes structs, the shared-memory fit and the workspace size depend only on this key:
-    # build them once
-    key = (n, m, T, B, F_T, esz, kind, s_lo, s_hi, bool(want_df), tsC, tsc, tsF)
-    plan = _adj_plans.get(key)
-    if plan is None:
-        fn = _lib.entry("mpcb200_lqr_adjoint", dtype)
-        L = _lib.lib()
-        s = _problem(n, m, T, B, dtype, dev, C, c, F, None, u_lower, u_upper)   # for its Dims / Params
-        dims, params = s.dims, s.params
-        dims.has_f = int(want_df)
-        fits = not L.mpcb200_step_prefers_workspace(ctypes.byref(dims), esz)
-        nbytes = L.mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), esz) if fits else 0
-        if len(_adj_plans) > 256:
-            _adj_plans.clear()
-        plan = _adj_plans[key] = (fits, fn, dims, params, ctypes.byref(dims), ctypes.byref(params), nbytes)
-    fits, fn, dims, params, dims_ref, params_ref, nbytes = plan
-    if not fits:
-        return None
-    nx_, nu_, gx_, gu_ = _dense(new_x, dtype), _dense(new_u, dtype), _dense(dl_dx, dtype), _dense(dl_du, dtype)
-    dx_init, dC, dc, dF, df = _grad_outputs(T, B, n, m, F_, f_T, want_df, dtype, dev)
+    if _pick_instance(n, m, esz) == (n, m) and not _is_empty(F):
+        # an exact instance, staged as _problem stages it, with the entry point, the ctypes structs and the workspace
+        # size built once per signature (they depend only on the key)
+        kind, s_lo, s_hi, lo_t, hi_t = _bounds(u_lower, u_upper, (T, B, m), dtype, dev)
+        (C_, tsC), (c_, tsc), (F_, tsF) = _time_strided(C, dtype), _time_strided(c, dtype), _time_strided(F, dtype)
+        key = (n, m, T, B, F.shape[0], esz, kind, s_lo, s_hi, bool(want_df), tsC, tsc, tsF,
+               os.environ.get("MPCB200_KERNEL"))
+        plan = _adj_plans.get(key)
+        if plan is None:
+            s = _problem(n, m, T, B, dtype, dev, C, c, F, None, u_lower, u_upper)   # for its Dims / Params
+            if len(_adj_plans) > 256:
+                _adj_plans.clear()
+            plan = _adj_plans[key] = _adj_plan(s, want_df, dtype)
+    else:
+        s = _problem(n, m, T, B, dtype, dev, C, c, F, None, u_lower, u_upper)
+        C_, c_, F_, lo_t, hi_t = s.C, s.c, s.F, s.u_lower, s.u_upper
+        plan = _adj_plan(s, want_df, dtype)
+    fn, pad, dims_ref, params_ref, nbytes = plan[:5]
+    nx_, nu_ = pad.vec_n(_dense(new_x, dtype)), pad.vec_m(_dense(new_u, dtype))
+    gx_, gu_ = pad.vec_n(_dense(dl_dx, dtype)), pad.vec_m(_dense(dl_du, dtype))
+    dx_init, dC, dc, dF, df = _grad_outputs(T, B, pad.N, pad.M, F_, f_T, want_df, dtype, dev)
     ws = _workspace(nbytes, dev)
     with _on_device(dev):
         rc = fn(dims_ref, params_ref, ptr_view(C_), ptr_view(c_), ptr_view(F_), ptr(nx_), ptr(nu_), ptr(gx_),
                 ptr(gu_), ptr(lo_t), ptr(hi_t), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(ws),
                 nbytes, stream_handle(dev))
     check(rc, "mpcb200_lqr_adjoint")
-    return dx_init, dC, dc, dF, df
+    return pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df)
+
+
+def _adj_plan(s, want_df, dtype):
+    """(entry point, _Pad, Dims ref, Params ref, workspace bytes, Dims, Params) of an adjoint call of the staged
+    problem `s`; the last two keep the structs the refs point to alive."""
+    dims, params = s.dims, s.params
+    dims.has_f = int(want_df)
+    nbytes = _lib.lib().mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), dtype.itemsize)
+    fn = _lib.entry("mpcb200_lqr_adjoint", dtype)
+    return fn, s.pad, ctypes.byref(dims), ctypes.byref(params), nbytes, dims, params
 
 
 def rollout_raw(n_state, n_ctrl, T, x_init, u, F, f=None):
@@ -722,37 +729,14 @@ class LQRStepFn(Function):
     def backward(ctx, dl_dx, dl_du, temp=None, temp2=None, temp3=None, temp4=None):
         o = ctx.o
         x_init, C, c, F, f, new_x, new_u = ctx.saved_tensors
-        B = C.size(1)
         if dl_dx is None:
             dl_dx = torch.zeros_like(new_x)
         if dl_du is None:
             dl_du = torch.zeros_like(new_u)
         want_df = not _is_empty(f)
-        fast = lqr_adjoint_raw(o.n_state, o.n_ctrl, o.T, C, c, F, new_x, new_u, dl_dx, dl_du, o.u_lower, o.u_upper,
-                               want_df, f_T=f.shape[0] if want_df else None, validated=True)
-        if fast is not None:                                # the whole backward in one library call
-            dx_init, dC, dc, dF, df = fast
-            if df is None:
-                df = torch.zeros_like(f) if f is not None else None
-            return None, dx_init, dC, dc, dF, df
-        r = torch.cat((dl_dx, dl_du), 2)                     # reference :316-320
-        if o.u_lower is None:
-            I = None
-        else:                                               # reference :325-326
-            I = (torch.abs(new_u - o.u_lower) <= 1e-8) | (torch.abs(new_u - o.u_upper) <= 1e-8)
-        zx = torch.zeros(o.T, B, o.n_state, dtype=C.dtype, device=C.device)
-        zu = torch.zeros(o.T, B, o.n_ctrl, dtype=C.dtype, device=C.device)
-        # nested MPC(lqr_iter=1, u_zero_I=I)(0, QuadCost(C,-r), LinDx(F,None)) (reference :328-340):
-        # one masked LQR step from the zero trajectory with the reference's default line search.
-        res = lqr_step_raw(o.n_state, o.n_ctrl, o.T, torch.zeros_like(x_init), C, -r, F, None, zx, zu,
-                           u_zero_I=I, linesearch_decay=0.2, max_linesearch_iter=10,
-                           do_rollout=True, want_stats=False)
-        want_df = not _is_empty(f)
-        dx_init, dC, dc, dF, df = lqr_grad_raw(o.n_state, o.n_ctrl, o.T, C, c, F, new_x, new_u,
-                                               res["new_x"], res["new_u"], dl_dx, want_df,
-                                               f_T=f.shape[0] if want_df else None)
-        if dF is None:
-            dF = torch.zeros_like(F)
+        dx_init, dC, dc, dF, df = lqr_adjoint_raw(o.n_state, o.n_ctrl, o.T, C, c, F, new_x, new_u, dl_dx, dl_du,
+                                                  o.u_lower, o.u_upper, want_df, f_T=f.shape[0] if want_df else None,
+                                                  validated=True)
         if df is None:                                       # reference :402 (empty tensor)
             df = torch.zeros_like(f) if f is not None else None
         return None, dx_init, dC, dc, dF, df

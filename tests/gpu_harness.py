@@ -591,7 +591,7 @@ def probe_step(n, m, dtype, T, impl, want_gains, do_rollout=True):
 
 def probe_adjoint(n, m, dtype, T):
     """Launches of one mpcb200_lqr_adjoint_* call at horizon T: 2 fused, 4 in-library 3-launch route, 0 if the
-    masked generic step does not fit shared memory either (callers then take the multi-call route)."""
+    library refused it for lack of shared memory."""
     C, c, F, x, u = _probe_inputs(n, m, dtype)
     try:
         _, launches = abi_adjoint(n, m, T, C[:T], c[:T], F[:T - 1], x[:T], u[:T], x[:T], u[:T], with_f=False)

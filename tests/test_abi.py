@@ -54,6 +54,9 @@ def test_argument_errors_are_status_codes_not_crashes():
     assert L.mpcb200_lqr_step_f64(ctypes.byref(d), ctypes.byref(p), *nul) == 2
     assert L.mpcb200_lqr_grad_f32(ctypes.byref(d), *([None] * 15)) == 2
     d.B, d.n, d.m = 4, 8, 2
+    fake = [ctypes.c_void_p(1 << 20)] * 13          # never dereferenced: the call fails on the missing workspace first
+    assert L.mpcb200_lqr_grad_f32(ctypes.byref(d), *fake, None, None) == 1       # the costate workspace is required
+    assert L.mpcb200_lqr_grad_f64(ctypes.byref(d), *fake, None, None) == 1
     assert L.mpcb200_step_smem_bytes(ctypes.byref(d), 4) > 0
     d.n = 31
     assert L.mpcb200_step_smem_bytes(ctypes.byref(d), 4) == 0

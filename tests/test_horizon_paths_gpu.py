@@ -6,9 +6,10 @@ Both step kernels change code path with the horizon T, chosen at launch from sha
     where lane i reads column i of K_t and K dx is summed by a butterfly);
   * column-pair kernel: the same choice, with the gains moved out early once the store is "crowded"; when the
     store does not fit and there is no buffer it refuses, and the default dispatch runs the generic kernel;
-  * KKT adjoint: the fused pair kernel (2 launches) while d tau of all T steps fits shared memory, else the
-    in-library masked step + costate + outer-product kernels (4 launches); LQRStepFn.backward takes the Python
-    multi-call route (3 launches) where lqr_adjoint_raw declines the shape.
+  * KKT adjoint: the fused pair kernel (2 launches) while d tau of all T steps fits shared memory and the masked
+    step would keep its gains there, else the in-library masked step + costate + outer-product kernels (4 launches),
+    whose masked step keeps its gains in the workspace where a step with Ks/ks would; LQRStepFn.backward is that one
+    library call for every shape.
 The switch horizons are found on the device by bisection (mpcb200_last_step_plan for step paths, launch counts for
 adjoint routes), never hard-coded, and every comparison asserts the plan that ran, so a retuned constant cannot
 silently drop a path: test_zz_coverage_table fails if any instance x dtype misses an applicable path.
@@ -278,9 +279,15 @@ def check_routes_agree(tag, a, b, case, dtype):
 ADJ_BOUNDS = (None, "box", "tensor")
 
 
-@pytest.mark.parametrize("n,m,dtype", PAIR_PARAMS, ids=PAIR_PIDS)
-def test_adjoint_fused_to_three_launch_switch(n, m, dtype):
-    """Fused just below the fit limit, in-library 3-launch route at it, both against the oracle's adjoint."""
+def _prefers_workspace(n, m, T, dtype):
+    from mpc.pytorch_b200._lib import Dims
+    d = Dims(B=1, T=T, n=n, m=m, F_T=T - 1)
+    return bool(_L().lib().mpcb200_step_prefers_workspace(ctypes.byref(d), dtype.itemsize))
+
+
+def _adjoint_switch(n, m, dtype, check_plan):
+    """Fused just below the adjoint's switch horizon, in-library 3-launch route at it, both against the oracle's
+    adjoint; check_plan(tag, T, launches, plan) checks the nested step's plan."""
     Ta = switches(n, m, dtype)["adjoint"]
     assert Ta is not None and Ta <= ORACLE_TMAX
     B = _B(n, m, dtype)
@@ -291,10 +298,37 @@ def test_adjoint_fused_to_three_launch_switch(n, m, dtype):
         got, launches = _run_abi_adjoint(n, m, T, case, dtype)
         tag = f"adjoint n{n}m{m} {DT[dtype]} T={T} B={B} bounds={bounds} f={with_f}"
         assert launches == (2 if T < Ta else 4), f"{tag}: {launches} launches"
-        # the nested masked step (fused or not) keeps its gains in shared memory: it has no Ks/ks buffer
-        assert _L().last_step_plan() & _L().PLAN_GAINS_SMEM, f"{tag}: {_plan_str(_L().last_step_plan())}"
+        check_plan(tag, T, launches, _L().last_step_plan())
         _seen(n, m, dtype, "adjoint_launches", launches)
         check_adjoint(tag, got, case, dtype)
+
+
+# the KREDUCE shape's adjoint switches at the horizon where its masked step starts to keep the gains in Ks/ks
+SWITCH_PARAMS = [p for p in PAIR_PARAMS if p[:2] not in KREDUCE_SHAPES]
+SWITCH_PIDS = [f"n{n}m{m}_{DT[d]}" for n, m, d in SWITCH_PARAMS]
+KREDUCE_PARAMS = [p for p in PAIR_PARAMS if p[:2] in KREDUCE_SHAPES]
+KREDUCE_PIDS = [f"n{n}m{m}_{DT[d]}" for n, m, d in KREDUCE_PARAMS]
+
+
+@pytest.mark.parametrize("n,m,dtype", SWITCH_PARAMS, ids=SWITCH_PIDS)
+def test_adjoint_fused_to_three_launch_switch(n, m, dtype):
+    """Fused just below the fit limit, in-library 3-launch route at it, both against the oracle's adjoint."""
+    def check_plan(tag, T, launches, plan):
+        # the nested masked step (fused or not) keeps its gains in shared memory: it has no Ks/ks buffer
+        assert plan & _L().PLAN_GAINS_SMEM, f"{tag}: {_plan_str(plan)}"
+    _adjoint_switch(n, m, dtype, check_plan)
+
+
+@pytest.mark.parametrize("n,m,dtype", KREDUCE_PARAMS, ids=KREDUCE_PIDS)
+def test_adjoint_switch_moves_gains_to_workspace(n, m, dtype):
+    """(16,4): the adjoint leaves the fused kernel where its masked step starts to prefer Ks/ks (the KREDUCE switch),
+    although the fused kernel would fit; there the 3-launch route's masked step keeps its gains in the workspace.
+    Both sides against the oracle's adjoint."""
+    def check_plan(tag, T, launches, plan):
+        gains_ws = _prefers_workspace(n, m, T, dtype)
+        assert gains_ws == (launches == 4), f"{tag}: prefers Ks/ks {gains_ws}, {launches} launches"
+        assert bool(plan & _L().PLAN_GAINS_SMEM) != gains_ws, f"{tag}: {_plan_str(plan)}, Ks/ks given: {gains_ws}"
+    _adjoint_switch(n, m, dtype, check_plan)
 
 
 ROUTE_SHAPES = [(2, 2), (4, 2), (8, 2), (8, 4), (12, 4), (16, 4), (5, 1), (3, 4)]
@@ -322,40 +356,96 @@ def test_adjoint_routes_agree_at_short_horizon(n, m, dtype):
         check_routes_agree(tag + " fused vs 3-launch", g2, g3, case, dtype)
 
 
-@pytest.mark.parametrize("dtype", [F32, F64], ids=["f32", "f64"])
-def test_config5_backward_takes_multicall_route(dtype):
-    """(16,4) T=50 (config 5): LQRStepFn.backward sends this shape to the Python multi-call route (the fit test asks
-    the generic kernel, whose KREDUCE preference says no), although the fused adjoint fits; all three routes agree."""
+def _autograd_backward(n, m, T, P, kw, dtype, keys=("x0", "C", "c", "F", "f")):
+    """LQRStepFn.backward through autograd (no_op_forward at the solution P["x"], P["u"]) with respect to P[keys]
+    (F and f are None when not in keys): ([dx_init, dC, dc, dF, df] on the CPU, None where not asked, library
+    launches)."""
     from mpc.pytorch_b200 import LQRStep, QuadCost, LinDx
-    n, m, T, B = 16, 4, 50, 5
-    case = adjoint_case(800, B, T, n, m, dtype, "box", True)
-    P, kw = case[:2]
-    lv = [P[k].to(DEV, dtype).requires_grad_(True) for k in ("x0", "C", "c", "F", "f")]
-    fn = LQRStep(n, m, T, true_cost=QuadCost(lv[1], lv[2]), true_dynamics=LinDx(lv[3], lv[4]),
-                 current_x=P["x"].to(DEV, dtype), current_u=P["u"].to(DEV, dtype), no_op_forward=True, **kw)
-    xo, uo = fn(*lv)
+    lv = [P[k].to(DEV, dtype).requires_grad_(True) for k in keys]
+    F, f = (dict(zip(keys, lv)).get(k) for k in ("F", "f"))
+    fn = LQRStep(n, m, T, true_cost=QuadCost(lv[1], lv[2]), true_dynamics=LinDx(F, f),
+                 current_x=P["x"].to(DEV, dtype), current_u=P["u"].to(DEV, dtype), no_op_forward=True,
+                 **{k: to_dev(v, dtype) for k, v in kw.items()})
+    xo, uo = fn(lv[0], lv[1], lv[2], F, f)
     before = _L().launch_count()
     grads = torch.autograd.grad((xo, uo), lv, (P["wx"].to(DEV, dtype), P["wu"].to(DEV, dtype)))
     torch.cuda.synchronize()
+    return [g.cpu() for g in grads] + [None] * (5 - len(grads)), _L().launch_count() - before
+
+
+@pytest.mark.parametrize("dtype", [F32, F64], ids=["f32", "f64"])
+def test_config5_backward_takes_three_launch_route(dtype):
+    """(16,4) T=50 (config 5), past the generic kernel's KREDUCE switch: LQRStepFn.backward is the one library call,
+    which takes the 3-launch route with the masked step's gains in the workspace (faster there than the fused kernel,
+    which would fit this horizon); it agrees with the route the generic kernel gives."""
+    n, m, T, B = 16, 4, 50, 5
+    case = adjoint_case(800, B, T, n, m, dtype, "box", True)
     tag = f"config5 backward {DT[dtype]}"
+    got, launches = _autograd_backward(n, m, T, *case[:2], dtype)
     # (the step plan is per host thread, and autograd runs this backward on its own device thread)
-    assert _L().launch_count() - before == 3, f"{tag}: not the multi-call route"
-    _seen(n, m, dtype, "adjoint_launches", 3)
-    multi = [t.cpu() for t in grads[:5]]
-    check_adjoint(tag + " multi-call", multi, case, dtype)
-    fused, l2 = _run_abi_adjoint(n, m, T, case, dtype)
+    assert launches == 4, f"{tag}: {launches} launches, not the 3-launch route"
+    _seen(n, m, dtype, "adjoint_launches", 4)
+    check_adjoint(tag + " autograd", got, case, dtype)
     three, l3 = _run_abi_adjoint(n, m, T, case, dtype, impl=1)
-    assert (l2, l3) == (2, 4), (l2, l3)
-    check_adjoint(tag + " fused", fused, case, dtype)
+    assert l3 == 4, l3
     check_adjoint(tag + " 3-launch", three, case, dtype)
-    check_routes_agree(tag + " multi-call vs fused", multi, fused, case, dtype)
-    check_routes_agree(tag + " multi-call vs 3-launch", multi, three, case, dtype)
+    check_routes_agree(tag + " default vs generic 3-launch", got, three, case, dtype)
+
+
+# (n, m, T, dtype, B, launches of the one library call): a padded shape that runs fused ((6,1) -> (6,2)), and two
+# horizons whose nested step keeps its gains in the workspace: past the gain store's size, and config 5 in float32
+BACKWARD_CASES = [(6, 1, 9, F64, 7, 2), (8, 2, 700, F64, 6, 4), (16, 4, 50, F32, 5, 4)]
+
+
+@pytest.mark.parametrize("n,m,T,dtype,B,launches", BACKWARD_CASES,
+                         ids=[f"n{n}m{m}_T{T}_{DT[d]}" for n, m, T, d, _, _ in BACKWARD_CASES])
+def test_backward_is_one_library_call(n, m, T, dtype, B, launches):
+    """LQRStepFn.backward against the oracle's adjoint, as one mpcb200_lqr_adjoint_* call of the expected launch
+    count; the same call made on this thread (lqr_adjoint_raw) gives the same gradients and shows the nested step's
+    gain store."""
+    from mpc.pytorch_b200.step import lqr_adjoint_raw
+    case = adjoint_case(1000 + n * 10 + m + T, B, T, n, m, dtype, "box", True)
+    P, kw = case[:2]
+    tag = f"backward n{n}m{m} T={T} {DT[dtype]}"
+    got, l_auto = _autograd_backward(n, m, T, P, kw, dtype)
+    assert l_auto == launches, f"{tag}: {l_auto} launches"
+    check_adjoint(tag, got, case, dtype)
+    d = lambda t: to_dev(t, dtype)  # noqa: E731
+    raw = lqr_adjoint_raw(n, m, T, d(P["C"]), d(P["c"]), d(P["F"]), d(P["x"]), d(P["u"]), d(P["wx"]), d(P["wu"]),
+                          kw["u_lower"], kw["u_upper"], True)
+    plan = _L().last_step_plan()
+    torch.cuda.synchronize()
+    for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
+        assert torch.equal(raw[i].cpu(), got[i]), f"{tag}: {name} autograd vs lqr_adjoint_raw"
+    if launches == 4:
+        assert _prefers_workspace(n, m, T, dtype) and not plan & _L().PLAN_GAINS_SMEM, f"{tag}: {_plan_str(plan)}"
+
+
+@pytest.mark.parametrize("with_F", [False, True], ids=["F_none", "F_given"])
+def test_backward_single_step(with_F):
+    """T = 1 with F = None (the forward pass takes it, so the backward must: no dF) and with F given (T slices, whose
+    dF slice is zero): LQRStepFn.backward against the oracle's adjoint, one fused library call."""
+    n, m, T, B, dtype = 8, 2, 1, 6, F64
+    C, c, F, _, x0 = gen_problem(1100, B, 2, n, m, F64)
+    g = torch.Generator().manual_seed(1100)
+    x, u = torch.randn(T, B, n, generator=g, dtype=F64), 0.1 * torch.randn(T, B, m, generator=g, dtype=F64)
+    P = dict(x0=x0, C=C[:1], c=c[:1], F=F[:1], x=x, u=u, wx=torch.randn(T, B, n, generator=g, dtype=F64),
+             wu=torch.randn(T, B, m, generator=g, dtype=F64))
+    F_orc = P["F"] if with_F else torch.zeros(0, B, n, n + m, dtype=F64)
+    ref = orc.lqr_step_backward(n, m, T, x0, P["C"], P["c"], F_orc, None, x, u, P["wx"], P["wu"], coupled=False)
+    got, launches = _autograd_backward(n, m, T, P, {}, dtype, keys=("x0", "C", "c", "F") if with_F else
+                                       ("x0", "C", "c"))
+    assert launches == 2, launches
+    for i, name in enumerate(("dx_init", "dC", "dc", "dF")):
+        if name == "dF" and not with_F:
+            continue
+        within("T=1", name, got[i], ref[i], None, dtype)
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# mpcb200_lqr_grad_* with and without a workspace
+# mpcb200_lqr_grad_* (the costate workspace is required)
 # ------------------------------------------------------------------------------------------------------------------
-def _abi_grad(n, m, T, P, dx, du, dtype, with_f, workspace):
+def _abi_grad(n, m, T, P, dx, du, dtype, with_f):
     L = _L()
     from mpc.pytorch_b200._lib import Dims, check, ptr, stream_handle
     ins = [P["C"], P["c"], P["F"], P["x"], P["u"], dx, du, P["wx"]]
@@ -365,7 +455,7 @@ def _abi_grad(n, m, T, P, dx, du, dtype, with_f, workspace):
     out = [torch.empty(B, n, dtype=dtype, device=DEV), torch.empty(T, B, p, p, dtype=dtype, device=DEV),
            torch.empty(T, B, p, dtype=dtype, device=DEV), torch.empty(T - 1, B, n, p, dtype=dtype, device=DEV),
            torch.empty(T - 1, B, n, dtype=dtype, device=DEV) if with_f else None]
-    ws = torch.empty(2 * T * B * n, dtype=dtype, device=DEV) if workspace else None
+    ws = torch.empty(2 * T * B * n, dtype=dtype, device=DEV)
     fn = L.lib().mpcb200_lqr_grad_f32 if dtype == F32 else L.lib().mpcb200_lqr_grad_f64
     before = L.launch_count()
     rc = fn(ctypes.byref(dims), *[ptr(t) for t in ins], *[ptr(t) for t in out], ptr(ws), stream_handle(DEV))
@@ -378,24 +468,18 @@ GRAD_CASES = [(8, 2, 9, F64), (8, 2, 300, F64), (5, 1, 9, F64), (5, 1, 300, F32)
 
 
 @pytest.mark.parametrize("n,m,T,dtype", GRAD_CASES, ids=[f"n{n}m{m}_T{T}_{DT[d]}" for n, m, T, d in GRAD_CASES])
-def test_grad_without_workspace_matches_two_kernel_path(n, m, T, dtype):
-    """The one-kernel gradient (workspace NULL) and the two-kernel one, fed the costate inputs of a solved problem
-    (the oracle's adjoint solution dx, du), against the oracle's outer products."""
+def test_grad_two_kernels_match_oracle(n, m, T, dtype):
+    """The two gradient kernels (costates through the workspace, then the outer products), fed the costate inputs of
+    a solved problem (the oracle's adjoint solution dx, du), against the oracle's outer products."""
     case = adjoint_case(900 + n + T, 12, T, n, m, dtype, "box", True)
     P, _, ref64, ref32 = case
     dx, du = ref64[5], ref64[6]
-    one, l1 = _abi_grad(n, m, T, P, dx, du, dtype, True, False)
-    two, l2 = _abi_grad(n, m, T, P, dx, du, dtype, True, True)
-    assert (l1, l2) == (1, 2), (l1, l2)
+    two, launches = _abi_grad(n, m, T, P, dx, du, dtype, True)
+    assert launches == 2, launches
     tag = f"grad n{n}m{m} T={T} {DT[dtype]}"
     for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
-        sc = max(1.0, float(ref64[i].abs().max()))
         # float32: the kernel is fed float32-rounded dx, du, so the yardstick is the float32 oracle's own adjoint
-        for got, nm in ((one, "one kernel"), (two, "two kernels")):
-            within(f"{tag} {nm}", name, got[i], ref64[i], ref32[i] if ref32 is not None else None, dtype)
-        d = maxdiff(one[i], two[i])
-        assert d <= (1e-12 if dtype == F64 else 1e-6) * sc, f"{tag}: one vs two kernels, {name}: {d:.3e}"
-        _seen(n, m, dtype, "grad one vs two kernels bit-identical", d == 0.0)
+        within(f"{tag} two kernels", name, two[i], ref64[i], ref32[i] if ref32 is not None else None, dtype)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -430,7 +514,4 @@ def test_zz_coverage_table():
     ident = {k: v for k, v in COVERAGE.items() if "pair smem vs Ks bit-identical" in v}
     print("pair kernel, gains in smem vs Ks bit-identical:",
           {f"n{n}m{m}_{DT[d]}": sorted(v["pair smem vs Ks bit-identical"]) for (n, m, d), v in ident.items()})
-    gid = {k: v for k, v in COVERAGE.items() if "grad one vs two kernels bit-identical" in v}
-    print("grad one vs two kernels bit-identical:",
-          {f"n{n}m{m}_{DT[d]}": sorted(v["grad one vs two kernels bit-identical"]) for (n, m, d), v in gid.items()})
     assert not missing, "\n".join(missing)

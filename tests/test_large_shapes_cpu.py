@@ -78,12 +78,15 @@ def test_adjoint_workspace_sizes(es):
     L = _lib().lib()
     size = lambda n, m, B, T: L.mpcb200_adjoint_workspace_bytes(ctypes.byref(_dims(n, m, B, T)), es)
     up = lambda v: (v + 255) // 256 * 256
-    for n, m in ((8, 2), (16, 4), (5, 1), (12, 4)):                           # instance shapes: unchanged
-        assert size(n, m, 7, 9) == _adj_bytes_without_gains(7, 9, n, m, es)
+    prefers = lambda n, m, T: L.mpcb200_step_prefers_workspace(ctypes.byref(_dims(n, m, 7, T)), es)
+    gains = lambda n, m, B, T: up(T * B * m * n * es) + up(T * B * m * es)
+    for n, m in ((8, 2), (16, 4), (5, 1), (12, 4)):                           # instance shapes, short horizon
+        assert not prefers(n, m, 9) and size(n, m, 7, 9) == _adj_bytes_without_gains(7, 9, n, m, es)
+    # (16, 4) past the horizon where its step keeps the gains in Ks/ks (KREDUCE): + the nested step's gains
+    assert prefers(16, 4, 50) and size(16, 4, 7, 50) == _adj_bytes_without_gains(7, 50, 16, 4, es) + gains(16, 4, 7, 50)
     for n, m in ((20, 4), (14, 7)):                                          # large shapes: + the nested gains
         B, T = 7, 9
-        assert size(n, m, B, T) == (_adj_bytes_without_gains(B, T, n, m, es) + up(T * B * m * n * es)
-                                    + up(T * B * m * es))
+        assert size(n, m, B, T) == _adj_bytes_without_gains(B, T, n, m, es) + gains(n, m, B, T)
 
 
 # ------------------------------------------------------------------------------------------------------------------

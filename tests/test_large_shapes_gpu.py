@@ -193,13 +193,16 @@ def test_adjoint_matches_oracle(mode, dtype):
     names = ("dx_init", "dC", "dc", "dF", "df")
     for i, k in enumerate(names):
         within(f"abi {mode}", k, got[i], want[i], want32[i] if want32 else None, dtype)
-    # through autograd: LQRStepFn.backward takes the multi-call route for these shapes
+    # through autograd: LQRStepFn.backward is the same library call (prep, masked large step, 2 gradient kernels)
     leaves = [to_dev(P[k], dtype).requires_grad_(True) for k in ("x0", "C", "c", "F", "f")]
     dk = {k: to_dev(v, dtype) for k, v in kw.items()}
     step = LQRStep(n, m, T, current_x=to_dev(P["x"], dtype), current_u=to_dev(P["u"], dtype),
                    true_cost=QuadCost(leaves[1], leaves[2]), true_dynamics=LinDx(leaves[3], leaves[4]), **dk)
     nx, nu = step(*leaves)[:2]
+    before = _L().launch_count()
     torch.autograd.backward((nx, nu), (to_dev(dl_dx, dtype), to_dev(dl_du, dtype)))
+    torch.cuda.synchronize()
+    assert _L().launch_count() - before == 4
     for i, k in enumerate(names):
         if dtype == F64:      # the forward solution is the kernel's, the same as the oracle's to 1e-9
             within(f"autograd {mode}", k, leaves[i].grad.cpu(), want[i], None, dtype,
@@ -360,9 +363,9 @@ def test_instance_and_padded_shapes_keep_their_plan(n, m):
 
 
 @pytest.mark.parametrize("dtype", [F64, F32], ids=["f64", "f32"])
-def test_grad_without_workspace(dtype):
-    """mpcb200_lqr_grad_* with workspace = NULL: the costate kernel writes the outer products itself.  It equals the
-    two-kernel path bit for bit and the oracle within the policy."""
+def test_grad_two_kernels_match_oracle(dtype):
+    """mpcb200_lqr_grad_* at a shape without an instance: the costate kernel writes the costates to the workspace,
+    the outer-product kernel reads them (2 launches); against the oracle within the policy."""
     from mpc.pytorch_b200._lib import Dims, check, entry, ptr
     n, m, B, T = 20, 4, 5, 10
     P, kw, o64, o32 = linear_step_case(41, B, T, n, m, dtype, "plain")
@@ -380,16 +383,15 @@ def test_grad_without_workspace(dtype):
                                                   dl_dx)]
     p = n + m
     dims = Dims(B=B, T=T, n=n, m=m, F_T=T - 1, has_f=1)
-    res = []
-    for ws in (torch.empty(2 * T * B * n, dtype=dtype, device=DEV), None):
-        out = [torch.empty(*s, dtype=dtype, device=DEV) for s in ((B, n), (T, B, p, p), (T, B, p), (T - 1, B, n, p),
-                                                                  (T - 1, B, n))]
-        check(entry("mpcb200_lqr_grad", dtype)(ctypes.byref(dims), *[ptr(t) for t in ins + out], ptr(ws), None), "grad")
-        torch.cuda.synchronize()
-        res.append([o.cpu() for o in out])
+    ws = torch.empty(2 * T * B * n, dtype=dtype, device=DEV)
+    out = [torch.empty(*s, dtype=dtype, device=DEV) for s in ((B, n), (T, B, p, p), (T, B, p), (T - 1, B, n, p),
+                                                              (T - 1, B, n))]
+    before = _L().launch_count()
+    check(entry("mpcb200_lqr_grad", dtype)(ctypes.byref(dims), *[ptr(t) for t in ins + out], ptr(ws), None), "grad")
+    torch.cuda.synchronize()
+    assert _L().launch_count() - before == 2
     for i, k in enumerate(("dx_init", "dC", "dc", "dF", "df")):
-        assert torch.equal(res[0][i], res[1][i]), k
-        within("grad", k, res[1][i], want[i], want32[i] if want32 else None, dtype)
+        within("grad", k, out[i].cpu(), want[i], want32[i] if want32 else None, dtype)
 
 
 # ------------------------------------------------------------------------------------------------------------------

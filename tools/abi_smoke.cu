@@ -63,7 +63,7 @@ static int run_case(int B, int T, int n, int m, int bounds_kind, int with_mask) 
                             with_mask ? dmask.p : nullptr, nx.p, nu.p, costs.p, fdn.p, al.p, du1.p, qp.p,
                             fmask.p, st.p, Ks.p, ks.p, nullptr);
   if (rc) return printf("step rc=%d (%s)\n", rc, mpcb200_strerror(rc)), 1;
-  // adjoint: masked step on (C, -r) from zeros, then the gradient assembly (both paths)
+  // adjoint: masked step on (C, -r) from zeros, then the gradient assembly
   Dev<float> r(c.size()), zx(cx.size()), zu(cu.size()), z0(x0.size()), ax(cx.size()), au(cu.size()), rx(cx.size()),
       gx0(x0.size()), gC(C.size()), gc(c.size()), gF(F.size()), gf(f.size()), ws((size_t)2 * T * B * n);
   std::vector<float> rr(c.size());
@@ -76,11 +76,9 @@ static int run_case(int B, int T, int n, int m, int bounds_kind, int with_mask) 
   rc = mpcb200_lqr_step_f32(&da, &prm, dC.p, r.p, dF.p, nullptr, z0.p, zx.p, zu.p, nullptr, nullptr, dmask.p, ax.p,
                             au.p, costs.p, fdn.p, al.p, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
   if (rc) return printf("adjoint step rc=%d\n", rc), 1;
-  for (int pass = 0; pass < 2; ++pass) {
-    rc = mpcb200_lqr_grad_f32(&d, dC.p, dc.p, dF.p, nx.p, nu.p, ax.p, au.p, rx.p, gx0.p, gC.p, gc.p, gF.p, gf.p,
-                              pass ? ws.p : nullptr, nullptr);
-    if (rc) return printf("grad rc=%d\n", rc), 1;
-  }
+  rc = mpcb200_lqr_grad_f32(&d, dC.p, dc.p, dF.p, nx.p, nu.p, ax.p, au.p, rx.p, gx0.p, gC.p, gc.p, gF.p, gf.p, ws.p,
+                            nullptr);
+  if (rc) return printf("grad rc=%d\n", rc), 1;
   {  // the whole KKT adjoint in one call (prep + nested masked step + costates + outer products)
     const size_t wsb = mpcb200_adjoint_workspace_bytes(&d, 4);
     Dev<unsigned char> aws(wsb);
@@ -91,7 +89,7 @@ static int run_case(int B, int T, int n, int m, int bounds_kind, int with_mask) 
     rc = mpcb200_lqr_adjoint_f32(&d, &prm, dC.p, dc.p, dF.p, nx.p, nu.p, r.p /* [T,B,p] >= [T,B,n] */, wu.p,
                                  bounds_kind == 2 ? dlo.p : nullptr, bounds_kind == 2 ? dhi.p : nullptr, gx0.p, gC.p,
                                  gc.p, gF.p, gf.p, aws.p, wsb, nullptr);
-    if (rc && rc != MPCB200_ERR_SMEM) return printf("one-call adjoint rc=%d (%s)\n", rc, mpcb200_strerror(rc)), 1;
+    if (rc) return printf("one-call adjoint rc=%d (%s)\n", rc, mpcb200_strerror(rc)), 1;
     // time-invariant dynamics / cost through the stride fields (one slice read for every t)
     mpcb200_dims ds = d;
     ds.F_tstride = MPCB200_TIME_INVARIANT;

@@ -17,9 +17,9 @@ for (B, T, n, m, dt) in [(13, 6, 8, 2, torch.float32), (7, 5, 3, 1, torch.float6
     a = lqr_step_raw(n, m, T, torch.zeros_like(x0), C, -torch.cat((x, u), 2), F, None, torch.zeros_like(x), torch.zeros_like(u), u_zero_I=I)
     g = lqr_grad_raw(n, m, T, C, c, F, o["new_x"], o["new_u"], a["new_x"], a["new_u"], x, True)
     torch.cuda.synchronize()
-# a shape without a compiled instance: the large-shape step (bounded, gains in Ks/ks) and, through autograd, the
-# multi-call backward (masked large step + costate and outer-product kernels); then mpcb200_lqr_adjoint_* at the same
-# shape, whose nested solve keeps its gains in the workspace
+# a shape without a compiled instance: the large-shape step (bounded, gains in Ks/ks) and, through autograd and then
+# directly, mpcb200_lqr_adjoint_* (masked large step with its gains in the workspace + costate and outer-product
+# kernels)
 import ctypes
 from mpc.pytorch_b200 import LQRStep, QuadCost, LinDx
 from mpc.pytorch_b200._lib import Dims, Params, check, entry, lib, ptr
