@@ -12,7 +12,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("MPCB200_LIB", os.path.join(_HERE, "libmpcb200.so"))   # override: developer experiments
+LIB_PATH = os.path.join(_HERE, "libmpcb200.so")
 
 
 class Dims(ctypes.Structure):

@@ -102,8 +102,8 @@ struct Step2Cfg {
   // n, m) and per-problem vectors that the lanes read straight from global memory with vector loads
   static constexpr bool OK = (N % 2 == 0) && (M % 2 == 0) && L <= 16 && N >= 2 && M >= 2 && (PPW * M * SZ) % 16 == 0 &&
                              (PPW * N * SZ) % 16 == 0 && (PPW * P * SZ) % 16 == 0;
-  // default choice between this mapping and the generic kernel, from tools/exp_shapes.py on an H100 SXM (400 W
-  // power limit), fp32, us per launch generic / pair: the pair mapping wins where the dense products dominate
+  // default choice between this mapping and the generic kernel, from tools/exp_step.py --preset shapes --kernel 1,2
+  // on an H100 SXM (400 W power limit), fp32, us per launch generic / pair: the pair mapping wins where the dense products dominate
   // (n=16, m=4, T=50, B=4096: 935 / 653; n=8, m=4: 107 / 89) and is no slower for narrow problems (n+m <= 6);
   // in between the generic kernel stays (n=8, m=2, B=16384: 196 / 206; n=12, m=4: 230 / 240).
   static constexpr bool PAIR_DEFAULT = OK && (P >= 18 || P <= 6 || (N == 8 && M == 4));

@@ -7,22 +7,21 @@ busiest SM holds 4 CTAs; at B=65536 an SM keeps as many resident as registers an
 waves of them.  If one warp's dependent chain set the time, the extra resident warps would hide it and the
 per-slot time would fall; if an SM resource saturates already at B=4096, the per-slot time stays flat.
 
-  python tools/exp_cfg3_bound.py [--riccati] [--batches 1024,4096,...] [--problems-per-cta 8]
+  python tools/exp_cfg3_bound.py [--riccati] [--batches 1024,4096,...] [--problems-per-cta 8] [--out DIR]
 
---riccati times the Riccati sweep alone (do_rollout = 0, gains written to Ks/ks).  The card's name, power limit
-and median SM clock under the load are printed with the numbers.  --problems-per-cta gives the CTA size of another
-build of the library (MPCB200_LIB), e.g. 6 for the earlier layout of 3 problems per warp and 2 consumer warps.
+--riccati times the Riccati sweep alone (do_rollout = 0, gains written to Ks/ks).  The card (measure.card) and the
+median SM clock under the load are printed with the numbers; with --out DIR they go to DIR/exp_cfg3_bound.json with
+the rows.  Another build of the library is measured by running this script in that build's tree;
+--problems-per-cta gives its CTA size, e.g. 6 for the earlier layout of 3 problems per warp and 2 consumer warps.
 """
 import argparse
 import ctypes
 import math
-import os
-import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch  # noqa: E402
+import torch
 
-import bench  # noqa: E402
+import measure
+import bench  # noqa: E402  (importable once measure has put the repository root on sys.path)
 
 T, N, M = 20, 8, 2
 PROBLEMS_PER_CTA = 8        # the generic kernel at (8, 2) f32: 2 consumer warps x 4 problems
@@ -34,13 +33,14 @@ def main():
     ap.add_argument("--batches", default="1024,2048,4096,8192,16384,65536")
     ap.add_argument("--reps", type=int, default=0, help="launches per timed block (0: ~0.2 s of work)")
     ap.add_argument("--problems-per-cta", type=int, default=PROBLEMS_PER_CTA)
+    ap.add_argument("--out", default=None, help="directory for exp_cfg3_bound.json (default: print only)")
     args = ap.parse_args()
     from mpc.pytorch_b200 import _lib
     dev = torch.device("cuda:0")
     stream = torch.cuda.current_stream(dev)
     sh = ctypes.c_void_p(stream.cuda_stream)
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
-    info = bench.device_info(0)
+    c = measure.card()
     clk = bench.ClockSampler(0)
     clk.start()
     rows = []
@@ -60,18 +60,19 @@ def main():
             raise SystemExit(f"expected the generic kernel at (8, 2) f32, the plan was {plan}")
         w = args.problems_per_cta
         busiest = math.ceil(math.ceil(B / w) / sms) * w
-        rows.append((B, us / busiest))
+        rows.append(dict(B=B, us=us, busiest_problems=busiest, us_per_slot=us / busiest))
         print(f"B={B:6d}  {us:9.1f} us/launch  busiest SM {busiest:4d} problems  {us / busiest:6.3f} us/slot",
               flush=True)
         del sts
         torch.cuda.empty_cache()
-    c = clk.stop()
-    print(f"card: {info['name']}, power limit {info['power_limit_w']} W, median SM clock {c['sm_mhz']} MHz "
-          f"(max {c['sm_max_mhz']}), throttle reasons {c['reasons']}; {sms} SMs; "
+    load = clk.stop()
+    print(f"median SM clock under load {load['sm_mhz']} MHz, throttle reasons {load['reasons']}; {sms} SMs; "
           f"{'Riccati only' if args.riccati else 'sweep + rollout'}")
-    per_slot = dict(rows)
+    per_slot = {r["B"]: r["us_per_slot"] for r in rows}
     if 4096 in per_slot and 65536 in per_slot:
         print(f"per-slot time at B=4096 / B=65536: {per_slot[4096] / per_slot[65536]:.3f}")
+    measure.report(args.out, __file__, c, rows, {r["B"]: [r["us"]] for r in rows}, clock=load, riccati=args.riccati,
+                   problems_per_cta=args.problems_per_cta)
 
 
 if __name__ == "__main__":

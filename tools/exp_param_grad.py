@@ -10,26 +10,21 @@ Workloads (learnable `params` on the device, requires_grad; the loss is a fixed 
   config2       cartpole B=128, T=25, bounds +-100, <=50 iterations, eps 1e-2, float32: MPC.forward + backward
   pendulum      the pendulum notebook's size, B=16, T=20, PendulumDx(params=(10, 1, 1)), bounds +-2, float32
   config2_f64   config2 in float64 (also gives d/dc and d/dx_init, to compare against TREE at rounding level)
-Each tree runs in worker processes of its own (the two builds share module names), alternated: this tree, TREE,
-this tree, ...  A worker warms up once, then times --reps calls (host clock around work that ends in a device
-synchronise) and saves its outputs; the parent compares x, u, costs (bitwise) and the gradients of the two trees.
-Prints one JSON line per workload and the card's name and power limit, read in the same run; with --out DIR, also
-writes DIR/exp_param_grad.json."""
+Each tree runs in worker processes of its own, alternated (measure.alternate): this tree, TREE, this tree, ...  A
+worker warms up once, then times --reps calls (measure.host_time); the first worker of each tree saves its outputs,
+and the parent compares them (measure.compare, and the relative change of each gradient).  Prints one JSON line per
+workload and the card (measure.card); with --out DIR, also writes DIR/exp_param_grad.json."""
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
-import tempfile
-import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import measure
+
 WORKLOADS = ("tail_known", "tail_opaque", "config2", "pendulum", "config2_f64")
 
 
-def _worker(tree, reps, out):
-    sys.path.insert(0, tree)
+def _worker(tree, out, save, reps):
+    measure.enter(tree)
     import torch
     from mpc.pytorch_b200 import MPC, GradMethods, QuadCost
     from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
@@ -68,12 +63,7 @@ def _worker(tree, reps, out):
             with torch.no_grad():
                 x, u, _ = ctrl(x0, QuadCost(Q, c), dx)
             if workload == "tail_opaque":
-                inner = dx
-
-                class Opaque(torch.nn.Module):
-                    def forward(self, x, u):
-                        return inner(x, u)
-                dx = Opaque()
+                dx = measure.Opaque(dx)
             wF = torch.randn(x.shape[0] - 1, x.shape[1], x.shape[2], x.shape[2] + 1, generator=torch.Generator()
                              .manual_seed(1), dtype=dtype).to(dev)
 
@@ -92,22 +82,12 @@ def _worker(tree, reps, out):
             return res
         return run
 
-    rows, saved = {}, {}
+    times, saved = {}, {}
     for w in WORKLOADS:
         run = make(w)
-        res = run()                                     # warm-up
-        torch.cuda.synchronize()
-        ts = []
-        for _ in range(reps):
-            t0 = time.perf_counter()
-            res = run()
-            torch.cuda.synchronize()
-            ts.append(time.perf_counter() - t0)
-        rows[w] = ts
-        saved.update({f"{w}/{k}": v.cpu() for k, v in res.items()})
-    torch.save(saved, out + ".pt")
-    with open(out + ".json", "w") as fh:
-        json.dump(rows, fh)
+        run()                                           # warm-up
+        times[w], saved[w] = measure.host_time(run, reps)
+    measure.save(out, times, outputs=saved if save else None)
 
 
 def _rel(a, b):
@@ -117,59 +97,34 @@ def _rel(a, b):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=7)
-    ap.add_argument("--rounds", type=int, default=3, help="alternated worker processes per tree")
-    ap.add_argument("--parent", default=None, help="another tree of the project, built, to compare against")
-    ap.add_argument("--out", default=None, help="directory for exp_param_grad.json (default: print only)")
-    ap.add_argument("--worker", nargs=2, metavar=("TREE", "OUT"), help=argparse.SUPPRESS)
+    measure.add_arguments(ap)
     a = ap.parse_args()
     if a.worker:
-        return _worker(a.worker[0], a.reps, a.worker[1])
+        return _worker(*a.worker[:2], a.worker[2] == "1", a.reps)
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: nothing to measure")
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip().splitlines()
-    card = smi[0] if smi else torch.cuda.get_device_name(0)
-    trees = {"this": ROOT}
-    if a.parent:
-        trees["parent"] = os.path.abspath(a.parent)
-    times = {k: {w: [] for w in WORKLOADS} for k in trees}
-    outs = {}
-    with tempfile.TemporaryDirectory() as tmp:
-        for r in range(a.rounds):
-            for k, tree in trees.items():
-                out = os.path.join(tmp, f"{k}{r}")
-                subprocess.run([sys.executable, os.path.abspath(__file__), "--reps", str(a.reps), "--worker", tree,
-                                out], check=True, cwd=tmp)
-                with open(out + ".json") as fh:
-                    for w, ts in json.load(fh).items():
-                        times[k][w] += ts
-                outs[k] = torch.load(out + ".pt")
+    c = measure.card()
+    arms = {k: (tree, {}) for k, tree in measure.trees(a.parent).items()}
+    times, _, outs = measure.alternate(__file__, arms, a.rounds, ["--reps", str(a.reps)])
     rows = []
     for w in WORKLOADS:
         row = dict(workload=w, this_ms=1e3 * statistics.median(times["this"][w]),
                    this_ms_all=[round(1e3 * t, 3) for t in times["this"][w]])
-        if "parent" in trees:
+        if "parent" in arms:
             row.update(parent_ms=1e3 * statistics.median(times["parent"][w]),
                        parent_ms_all=[round(1e3 * t, 3) for t in times["parent"][w]])
             row["speedup"] = row["parent_ms"] / row["this_ms"]
-            mine, theirs = outs["this"], outs["parent"]
-            for key in sorted(k for k in mine if k.startswith(w + "/")):
-                name = key.split("/", 1)[1]
-                if name in ("x", "u", "costs"):
-                    row[f"{name}_bitwise"] = bool(torch.equal(mine[key], theirs[key]))
-                else:
-                    row[f"{name}_rel_change"] = _rel(mine[key], theirs[key])
+            mine, theirs = outs["this"][w], outs["parent"][w]
+            row.update(measure.compare(mine, theirs))
+            row.update({f"{k}_rel_change": _rel(mine[k], theirs[k]) for k in mine
+                        if k not in ("x", "u", "costs")})
         rows.append(row)
         print(json.dumps(row), flush=True)
-    if "tail_known" in times["this"]:
-        print(f"tail: known system {rows[0]['this_ms']:.3f} ms, opaque Module {rows[1]['this_ms']:.3f} ms "
-              f"(x{rows[1]['this_ms'] / rows[0]['this_ms']:.1f})")
-    if a.out is not None:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "exp_param_grad.json"), "w") as fh:
-            json.dump(dict(card=card, torch=torch.__version__, rows=rows), fh, indent=1)
-    print("card:", card)
+    print(f"tail: known system {rows[0]['this_ms']:.3f} ms, opaque Module {rows[1]['this_ms']:.3f} ms "
+          f"(x{rows[1]['this_ms'] / rows[0]['this_ms']:.1f})")
+    runs = {k: {w: [round(1e3 * t, 3) for t in ts] for w, ts in v.items()} for k, v in times.items()}
+    measure.report(a.out, __file__, c, rows, runs, rounds=a.rounds, reps=a.reps)
 
 
 if __name__ == "__main__":

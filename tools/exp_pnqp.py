@@ -1,25 +1,23 @@
 """Cost of the standalone pnqp (mpc.pnqp.pnqp) over batch size, QP size and precision.  (developer tool)
 
-  python tools/exp_pnqp.py [--reps 7] [--batches 2,256,4096] [--sizes 8,9,16,32,64,100,128]
+  python tools/exp_pnqp.py [--reps 7] [--batches 2,256,4096] [--sizes 8,9,16,32,64,100,128] [--out DIR]
 
 Each row times the whole Python call (argument broadcast, output allocation, one kernel, the read of the
 iteration counts) with CUDA events: two warm-up calls, then the median of --reps calls.  n = 8 runs the
 thread-per-QP kernel, n > 8 the thread-block-per-QP kernel.  For the B = 2 rows the per-problem CPU oracle
 (oracle/lqr_oracle.py, coupled=False) is timed on the same inputs as a baseline.  Inputs follow the pnqp
-generator of oracle/make_golden.py.  The card's name and power limit are printed with the numbers.
+generator of oracle/make_golden.py.  The card (measure.card) is printed with the numbers; with --out DIR, the rows,
+every call's time and the card go to DIR/exp_pnqp.json.
 """
 import argparse
 import contextlib
 import io
-import os
 import statistics
-import sys
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch  # noqa: E402
+import torch
 
-import bench  # noqa: E402
+import measure
 
 
 def gen(B, n, dtype, dev):
@@ -37,12 +35,13 @@ def main():
     ap.add_argument("--reps", type=int, default=7)
     ap.add_argument("--batches", default="2,256,4096")
     ap.add_argument("--sizes", default="8,9,16,32,64,100,128")
+    ap.add_argument("--out", default=None, help="directory for exp_pnqp.json (default: print only)")
     args = ap.parse_args()
     from mpc.pnqp import pnqp
     from oracle import lqr_oracle as orc
     dev = torch.device("cuda:0")
-    info = bench.device_info(0)
-    print(f"card: {info['name']}, power limit {info['power_limit_w']} W")
+    c = measure.card()
+    rows, runs = [], {}
     print(f"{'dtype':>7} {'B':>5} {'n':>4} {'iters':>5} {'ms/call':>9} {'QPs/s':>10} {'CPU oracle ms':>14}")
     for dtype in (torch.float32, torch.float64):
         for B in [int(b) for b in args.batches.split(",")]:
@@ -72,8 +71,11 @@ def main():
                     cpu = f"{statistics.median(tc):.2f}"
                 name = str(dtype).replace("torch.", "")
                 print(f"{name:>7} {B:5d} {n:4d} {it:5d} {med:9.3f} {B / med * 1e3:10.3g} {cpu:>14}", flush=True)
+                rows.append(dict(dtype=name, B=B, n=n, iters=it, ms=med, cpu_oracle_ms=float(cpu) if cpu else None))
+                runs[f"{name},{B},{n}"] = ms
                 del H, q, lo, hi
     torch.cuda.empty_cache()
+    measure.report(args.out, __file__, c, rows, runs, reps=args.reps)
 
 
 if __name__ == "__main__":

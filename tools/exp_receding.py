@@ -10,23 +10,18 @@ Episodes (float32, the notebooks' solver options: lqr_iter=50, eps=1e-2, AUTO_DI
   config2   B=128, T=25  (cartpole at BASELINE config 2's size)
 The loop is control._episode_host: per control step MPC.forward, the model step by the rollout kernel and the shift
 of the warm start, as the notebooks do it.  Prints one JSON line per episode (ms per control step and per episode,
-median over --reps alternated repetitions, after one warm-up of each) and the card's name and power limit, read in
-the same run; with --out DIR, also writes them to DIR/exp_receding.json."""
+median over --reps alternated repetitions of measure.host_time, after one warm-up of each) and the card
+(measure.card); with --out DIR, also writes them to DIR/exp_receding.json."""
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
-import time
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-from mpc.pytorch_b200 import control  # noqa: E402
-from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx  # noqa: E402
-from mpc.pytorch_b200.solver import MPC, GradMethods, QuadCost  # noqa: E402
+import measure
+from mpc.pytorch_b200 import control
+from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
+from mpc.pytorch_b200.solver import MPC, GradMethods, QuadCost
 
 DEV = torch.device("cuda:0")
 
@@ -50,14 +45,6 @@ def _case(name, B, T):
     return ctrl, x0.to(DEV), QuadCost(Q, pp), sysdx
 
 
-def _timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return out, time.perf_counter() - t0
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -66,9 +53,7 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: nothing to measure")
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip().splitlines()
-    card = smi[0] if smi else torch.cuda.get_device_name(0)
+    c = measure.card()
     rows = []
     for name, B, T in (("cartpole", 8, 25), ("pendulum", 16, 20), ("config2", 128, 25)):
         ctrl, x0, cost, dx = _case(name, B, T)
@@ -80,13 +65,13 @@ def main():
 
         def graph():
             return control.receding_horizon(ctrl, x0, cost, dx, a.steps)
-        ref, _ = _timed(loop)                         # warm-up of both
-        got, _ = _timed(graph)
+        ref = measure.host_time(loop, 1)[1]            # warm-up of both
+        got = measure.host_time(graph, 1)[1]
         same = all(torch.equal(getattr(got, k), getattr(ref, k).to(DEV)) for k in control.Episode._fields)
         t_loop, t_graph = [], []
         for _ in range(a.reps):                       # alternated
-            t_loop.append(_timed(loop)[1])
-            t_graph.append(_timed(graph)[1])
+            t_loop += measure.host_time(loop, 1)[0]
+            t_graph += measure.host_time(graph, 1)[0]
         ml, mg = statistics.median(t_loop), statistics.median(t_graph)
         row = dict(episode=name, B=B, T=T, steps=a.steps, bitwise_equal=same,
                    iterations=int(got.info[:, 0].sum()),
@@ -95,11 +80,8 @@ def main():
                    loop_s_all=t_loop, graph_s_all=t_graph)
         rows.append(row)
         print(json.dumps(row), flush=True)
-    if a.out is not None:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "exp_receding.json"), "w") as fh:
-            json.dump(dict(card=card, torch=torch.__version__, rows=rows), fh, indent=1)
-    print("card:", card)
+    measure.report(a.out, __file__, c, rows, {r["episode"]: dict(loop_s=r["loop_s_all"], graph_s=r["graph_s_all"])
+                                              for r in rows}, steps=a.steps, reps=a.reps)
     if not all(r["bitwise_equal"] for r in rows):
         raise SystemExit("receding_horizon differs from the loop")
 
