@@ -84,28 +84,105 @@ def run_loop(n, m, T, P, kw, opts, dtype=None, impl=None):
     return {k: v.cpu() for k, v in res.items()}, plan
 
 
-def abi_adjoint(n, m, T, C, c, F, new_x, new_u, dl_dx, dl_du, lo=None, hi=None, with_f=True):
-    """mpcb200_lqr_adjoint_* through the C ABI on device tensors; lo, hi None, floats or tensors.  Returns
-    ([dx_init, dC, dc, dF, df or None] on the CPU, kernel launches)."""
+def staged(t, dtype):
+    """(tensor, mpcb200_dims time-stride field) of a [T, B, ...] input as the shim stages it (step._time_strided):
+    dense and misaligned contiguous views stay as they are, stride-0 and 16-byte time strides keep their stride.
+    None and empty tensors: (None, 0)."""
+    from mpc.pytorch_b200.step import _time_strided
+    if t is None or t.numel() == 0:
+        return None, 0
+    return _time_strided(t, dtype)
+
+
+def _grad_buffers(T, B, n, m, F_T, want_df, dtype, poison):
+    """dx_init, dC, dc, dF [F_T slices], df [T-1 slices] or None: empty, or all NaN when `poison`."""
+    p = n + m
+    make = (lambda *s: torch.full(s, float("nan"), dtype=dtype, device=DEV)) if poison else \
+        (lambda *s: torch.empty(s, dtype=dtype, device=DEV))
+    return [make(B, n), make(T, B, p, p), make(T, B, p), make(F_T, B, n, p), make(T - 1, B, n) if want_df else None]
+
+
+def abi_adjoint(n, m, T, C, c, F, new_x, new_u, dl_dx, dl_du, lo=None, hi=None, with_f=True, F_T=None, poison=False):
+    """mpcb200_lqr_adjoint_* through the C ABI on device tensors; lo, hi None, floats or tensors.  C, c and F keep
+    their time strides (stride 0, or a 16-byte multiple) and every tensor its storage offset, as the shim hands them
+    over.  F_T: time slices of F and dF (default T - 1).  poison: every output starts as NaN, so an element the call
+    does not write fails any comparison; with_f False then still hands over a NaN df buffer (has_f = 0), which must
+    come back untouched.  Returns ([dx_init, dC, dc, dF, df or None] on the CPU, kernel launches)."""
     L = _L()
-    dtype, B, p = C.dtype, C.shape[1], n + m
+    dtype, B = C.dtype, C.shape[1]
+    F_T = T - 1 if F_T is None else F_T
+    assert F is None and F_T == 0 or F.shape[0] == F_T, "F must hold F_T time slices"
     kind = 0 if lo is None else (1 if isinstance(lo, float) else 2)
-    dims = L.Dims(B=B, T=T, n=n, m=m, F_T=T - 1, has_f=int(with_f), bounds_kind=kind, max_ls_iter=10,
-                  pnqp_max_iter=20, do_rollout=1)
+    (C_, tsC), (c_, tsc), (F_, tsF) = staged(C, dtype), staged(c, dtype), staged(F, dtype)
+    dims = L.Dims(B=B, T=T, n=n, m=m, F_T=F_T, has_f=int(with_f), bounds_kind=kind, max_ls_iter=10,
+                  pnqp_max_iter=20, do_rollout=1, C_tstride=tsC, c_tstride=tsc, F_tstride=tsF)
     prm = L.Params(u_lo=lo if kind == 1 else 0.0, u_hi=hi if kind == 1 else 0.0, delta_u=0.0, ls_decay=0.2)
     nbytes = L.lib().mpcb200_adjoint_workspace_bytes(ctypes.byref(dims), C.element_size())
     ws = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
-    ins = [t.contiguous() for t in (C, c, F, new_x, new_u, dl_dx, dl_du)]         # alive until the sync
+    ins = [t.contiguous() for t in (new_x, new_u, dl_dx, dl_du)]         # alive until the sync
     ins += [lo.contiguous() if kind == 2 else None, hi.contiguous() if kind == 2 else None]
-    out = [torch.empty(B, n, dtype=dtype, device=DEV), torch.empty(T, B, p, p, dtype=dtype, device=DEV),
-           torch.empty(T, B, p, dtype=dtype, device=DEV), torch.empty(T - 1, B, n, p, dtype=dtype, device=DEV),
-           torch.empty(T - 1, B, n, dtype=dtype, device=DEV) if with_f else None]
+    out = _grad_buffers(T, B, n, m, F_T, with_f or poison, dtype, poison)
+    df = out[4]
+    if not with_f:
+        out[4] = None
     before = L.launch_count()
-    rc = L.entry("mpcb200_lqr_adjoint", dtype)(ctypes.byref(dims), ctypes.byref(prm), *[L.ptr(t) for t in ins + out],
+    rc = L.entry("mpcb200_lqr_adjoint", dtype)(ctypes.byref(dims), ctypes.byref(prm), L.ptr_view(C_), L.ptr_view(c_),
+                                               L.ptr_view(F_), *[L.ptr(t) for t in ins + out[:4]], L.ptr(df),
                                                L.ptr(ws), nbytes, L.stream_handle(DEV))
     L.check(rc, "mpcb200_lqr_adjoint")
     torch.cuda.synchronize()
+    if not with_f and df is not None:
+        assert bool(df.isnan().all()), "mpcb200_lqr_adjoint wrote df although has_f = 0"
     return [t.cpu() if t is not None else None for t in out], L.launch_count() - before
+
+
+def abi_grad(n, m, T, C, c, F, new_x, new_u, dx, du, dl_dx, with_df=True, F_T=None, poison=False):
+    """mpcb200_lqr_grad_* (costates through the workspace, then the outer products) through the C ABI on device
+    tensors, C, c and F staged as abi_adjoint stages them; F_T and poison as there (without df the df pointer is
+    NULL: the kernels take has_df from it).  Returns ([dx_init, dC, dc, dF, df or None] on the CPU, launches)."""
+    L = _L()
+    dtype, B = C.dtype, C.shape[1]
+    F_T = T - 1 if F_T is None else F_T
+    assert F is None and F_T == 0 or F.shape[0] == F_T, "F must hold F_T time slices"
+    (C_, tsC), (c_, tsc), (F_, tsF) = staged(C, dtype), staged(c, dtype), staged(F, dtype)
+    dims = L.Dims(B=B, T=T, n=n, m=m, F_T=F_T, has_f=int(with_df), max_ls_iter=1, pnqp_max_iter=1,
+                  C_tstride=tsC, c_tstride=tsc, F_tstride=tsF)
+    ins = [t.contiguous() for t in (new_x, new_u, dx, du, dl_dx)]
+    out = _grad_buffers(T, B, n, m, F_T, with_df, dtype, poison)
+    ws = torch.empty(2 * T * B * n, dtype=dtype, device=DEV)
+    before = L.launch_count()
+    rc = L.entry("mpcb200_lqr_grad", dtype)(ctypes.byref(dims), L.ptr_view(C_), L.ptr_view(c_), L.ptr_view(F_),
+                                            *[L.ptr(t) for t in ins + out], L.ptr(ws), L.stream_handle(DEV))
+    L.check(rc, "mpcb200_lqr_grad")
+    torch.cuda.synchronize()
+    return [t.cpu() if t is not None else None for t in out], L.launch_count() - before
+
+
+def abi_rollout(n, m, T, F, f, x0, u, poison=False):
+    """mpcb200_rollout_* through the C ABI on device tensors: x [T, B, n] on the CPU.  F [T-1 or T, B, n, n+m] (None
+    or empty at T = 1) and f [T-1, B, n] (None or empty: no f) are staged as abi_adjoint stages them; poison: x starts
+    as NaN."""
+    L = _L()
+    dtype, B = x0.dtype, x0.shape[0]
+    (F_, tsF), (f_, tsf) = staged(F, dtype), staged(f, dtype)
+    dims = L.Dims(B=B, T=T, n=n, m=m, F_T=F.shape[0] if F is not None else T - 1, has_f=int(f_ is not None),
+                  max_ls_iter=1, pnqp_max_iter=1, F_tstride=tsF, f_tstride=tsf)
+    x = torch.full((T, B, n), float("nan") if poison else 0.0, dtype=dtype, device=DEV)
+    ins = [x0.contiguous(), u.contiguous()]
+    rc = L.entry("mpcb200_rollout", dtype)(ctypes.byref(dims), L.ptr_view(F_), L.ptr_view(f_),
+                                           *[L.ptr(t) for t in ins], L.ptr(x), L.stream_handle(DEV))
+    L.check(rc, "mpcb200_rollout")
+    torch.cuda.synchronize()
+    return x.cpu()
+
+
+def misaligned(t):
+    """A contiguous copy of t that starts one element into its allocation, so data_ptr() % 16 != 0: the shim hands it
+    to the kernels unchanged (a contiguous tensor is never copied), and the library picks its copy path for it."""
+    buf = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)
+    v = buf[1:].view(t.shape)
+    v.copy_(t)
+    return v
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -320,6 +397,46 @@ def step_layout(kernel, n, m, dtype):
     return ppw, nw * ppw
 
 
+def grad_layout(n, m):
+    """(problems per warp, problems per CTA) of the gradient kernels (GradCfg, lqr_grad.cuh): n+m lanes per problem,
+    four warps per CTA.  The outer-product kernel masks its flat stores by the problems of its warp group."""
+    ppw = 32 // (n + m)
+    return ppw, 4 * ppw
+
+
+def rollout_layout(n):
+    """(problems per warp, problems per CTA) of the LinDx rollout kernel (RolloutCfg, lqr_rollout.cuh): n lanes per
+    problem, four warps per CTA."""
+    ppw = 32 // n
+    return ppw, 4 * ppw
+
+
+def pool_size(*layout):
+    """Smallest pool of at least 3 problems whose size is coprime to every given warp / CTA size: batch element b is
+    pool problem b % K, so neighbouring warps and CTAs hold different problems, and a kernel that reads another
+    batch element's operands reads another problem."""
+    return next(k for k in range(3, 64) if all(math.gcd(k, s) == 1 for s in layout))
+
+
+def layout_batches(ppw, W, K=None):
+    """Batch sizes that put problems at every warp and CTA position and end in every kind of tail: one problem, a
+    partial, full and just-overfull warp, a CTA short by one, full and overfull by one, two CTAs and a warp and one
+    more.  With a pool of K: also K CTAs and a warp and one more, so that every pool problem sits at every position
+    of a full CTA."""
+    out = {1, ppw - 1, ppw, ppw + 1, W - 1, W, W + 1, 2 * W + ppw + 1}
+    if K is not None:
+        out.add(K * W + ppw + 1)
+    return sorted(b for b in out if b >= 1)
+
+
+def batch_rows(v, idx):
+    """Batch elements idx of an input or an oracle output: [B, n] along dim 0, [T, B, ...] along dim 1; floats and
+    empty tensors as they are."""
+    if not torch.is_tensor(v) or v.numel() == 0:
+        return v
+    return v.index_select(0 if v.dim() == 2 else 1, idx)
+
+
 def ls_layout(B, ppw, W):
     """Classes by batch position.  The first problem of every warp takes one pass, and so does all of warp 0 in
     even CTAs of several warps: a repeat decided by that problem or that warp alone would stop too early.  The other
@@ -510,6 +627,86 @@ def check_clamps(tag, r, o, kw, keep=None):
         b = kw[side] if torch.is_tensor(kw[side]) else torch.full_like(o.new_u, kw[side])
         assert torch.equal(_cols(r["new_u"].double() == b.double(), keep),
                            _cols(o.new_u.double() == b.double(), keep)), f"{tag}: {side} clamp mask"
+
+
+@functools.lru_cache(maxsize=16)
+def adjoint_case(seed, B, T, n, m, dtype, bounds, with_f, F_T=None):
+    """A solved problem (one oracle step from u = 0, so box bounds leave an active set), upstream gradients,
+    and the oracle's adjoint in float64 (and float32): (P, kw, ref64, ref32|None).  F_T=T: F carries T time slices
+    (the oracle's dF then ends in a zero slice)."""
+    C, c, F, f, x0 = gen_problem(seed, B, T, n, m, F64, with_f=with_f)
+    F = F * 0.9
+    if F_T == T:
+        F = torch.cat((F, F[-1:]), 0) if T > 1 else gen_problem(seed, B, 2, n, m, F64)[2] * 0.9
+    g = torch.Generator().manual_seed(seed)
+    kw = {}
+    if bounds == "box":
+        kw = dict(u_lower=-0.25, u_upper=0.25)
+    elif bounds == "tensor":
+        kw = dict(u_lower=round_through(-0.5 * torch.rand(T, B, m, generator=g, dtype=F64) - 0.05, dtype),
+                  u_upper=round_through(0.5 * torch.rand(T, B, m, generator=g, dtype=F64) + 0.05, dtype))
+    C, c, F, f, x0 = (round_through(t, dtype) for t in (C, c, F, f, x0))
+    u = torch.zeros(T, B, m, dtype=F64)
+    o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, orc.get_traj(T, u, x0, F, f), u, coupled=False, **kw)
+    x, u = round_through(o.new_x, dtype), round_through(o.new_u, dtype)
+    wx = round_through(torch.randn(T, B, n, generator=g, dtype=F64), dtype)
+    wu = round_through(torch.randn(T, B, m, generator=g, dtype=F64), dtype)
+    P = dict(C=C, c=c, F=F, f=f, x0=x0, x=x, u=u, wx=wx, wu=wu)
+    ref64 = orc.lqr_step_backward(n, m, T, x0, C, c, F, f, x, u, wx, wu, coupled=False, **kw)
+    ref32 = None
+    if dtype == F32:
+        lo = lambda t: t.float() if torch.is_tensor(t) else t  # noqa: E731
+        ref32 = orc.lqr_step_backward(n, m, T, lo(x0), lo(C), lo(c), lo(F), lo(f), lo(x), lo(u), lo(wx), lo(wu),
+                                      coupled=False, **{k: lo(v) for k, v in kw.items()})
+    return P, kw, ref64, ref32
+
+
+def run_abi_adjoint(n, m, T, case, dtype, impl=None, F_T=None, poison=False):
+    """abi_adjoint on the problem of an adjoint_case (with df where it has f) under MPCB200_KERNEL=impl."""
+    P, kw, _, _ = case
+    d = lambda t: to_dev(t, dtype)  # noqa: E731
+    with kernel_env(impl):
+        return abi_adjoint(n, m, T, d(P["C"]), d(P["c"]), d(P["F"]), d(P["x"]), d(P["u"]), d(P["wx"]), d(P["wu"]),
+                           d(kw.get("u_lower")), d(kw.get("u_upper")), P["f"] is not None, F_T, poison)
+
+
+def check_adjoint(tag, got, case, dtype):
+    _, _, ref64, ref32 = case
+    for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
+        if got[i] is None:
+            assert ref64[i].numel() == 0, f"{tag}: {name} missing"
+            continue
+        within(tag, name, got[i], ref64[i], ref32[i] if ref32 is not None else None, dtype)
+
+
+def check_routes_agree(tag, a, b, case, dtype):
+    """Two adjoint routes on one input: float64 within 1e-9 x scale of each other; float32 within the sum of their
+    float32 yardsticks (each is checked against the oracle on its own)."""
+    _, _, ref64, ref32 = case
+    for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
+        if a[i] is None:
+            continue
+        sc = max(1.0, float(ref64[i].abs().max()))
+        err = maxdiff(a[i], b[i])
+        bound = 1e-9 * sc if dtype == F64 else 2 * (4 * maxdiff(ref32[i], ref64[i]) + 1e-6 * sc)
+        assert err <= bound, f"{tag}: {name} routes differ by {err:.3e} > {bound:.3e}"
+
+
+def autograd_backward(n, m, T, P, kw, dtype, keys=("x0", "C", "c", "F", "f")):
+    """LQRStepFn.backward through autograd (no_op_forward at the solution P["x"], P["u"]) with respect to P[keys]
+    (F and f are None when not in keys): ([dx_init, dC, dc, dF, df] on the CPU, None where not asked, library
+    launches)."""
+    from mpc.pytorch_b200 import LQRStep, QuadCost, LinDx
+    lv = [P[k].to(DEV, dtype).requires_grad_(True) for k in keys]
+    F, f = (dict(zip(keys, lv)).get(k) for k in ("F", "f"))
+    fn = LQRStep(n, m, T, true_cost=QuadCost(lv[1], lv[2]), true_dynamics=LinDx(F, f),
+                 current_x=P["x"].to(DEV, dtype), current_u=P["u"].to(DEV, dtype), no_op_forward=True,
+                 **{k: to_dev(v, dtype) for k, v in kw.items()})
+    xo, uo = fn(lv[0], lv[1], lv[2], F, f)
+    before = _L().launch_count()
+    grads = torch.autograd.grad((xo, uo), lv, (P["wx"].to(DEV, dtype), P["wu"].to(DEV, dtype)))
+    torch.cuda.synchronize()
+    return [g.cpu() for g in grads] + [None] * (5 - len(grads)), _L().launch_count() - before
 
 
 def check_step_fixed(tag, r, o, kw, dtype):

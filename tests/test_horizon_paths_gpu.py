@@ -19,15 +19,15 @@ horizons: the kernel's error against the float64 oracle must stay within 4x the 
 float32 (on the same float32-rounded inputs) plus 1e-6 x scale.  Inputs come from tests.helpers.gen_problem with
 F *= 0.9, so trajectories stay O(1) at T ~ 900."""
 import ctypes
-import functools
 
 import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.gpu_harness import (DEV, DT, F32, F64, INSTANCES, KREDUCE_SHAPES, ORACLE_TMAX, PAIR_SHAPES, abi_adjoint,
-                               check_alphas, check_clamps, check_pnqp, check_trajectory, kernel_env, linear_step_case,
-                               plan as _plan, plan_str as _plan_str, round_through, run_step, switches, to_dev, within)
+from tests.gpu_harness import (DT, F32, F64, INSTANCES, KREDUCE_SHAPES, ORACLE_TMAX, PAIR_SHAPES, abi_grad,
+                               adjoint_case, autograd_backward, check_adjoint, check_alphas, check_clamps, check_pnqp,
+                               check_routes_agree, check_trajectory, kernel_env, linear_step_case, plan as _plan,
+                               plan_str as _plan_str, run_abi_adjoint, run_step, switches, to_dev, within)
 from tests.helpers import gen_problem, maxdiff
 
 pytestmark = pytest.mark.gpu
@@ -217,65 +217,6 @@ def test_pair_long_horizon_and_no_fit(n, m, dtype):
 # ------------------------------------------------------------------------------------------------------------------
 # KKT adjoint routes
 # ------------------------------------------------------------------------------------------------------------------
-@functools.lru_cache(maxsize=4)
-def adjoint_case(seed, B, T, n, m, dtype, bounds, with_f):
-    """A solved problem (one oracle step from u = 0, so box bounds leave an active set), upstream gradients,
-    and the oracle's adjoint in float64 (and float32): (P, kw, ref64, ref32|None)."""
-    C, c, F, f, x0 = gen_problem(seed, B, T, n, m, F64, with_f=with_f)
-    F = F * 0.9
-    g = torch.Generator().manual_seed(seed)
-    kw = {}
-    if bounds == "box":
-        kw = dict(u_lower=-0.25, u_upper=0.25)
-    elif bounds == "tensor":
-        kw = dict(u_lower=round_through(-0.5 * torch.rand(T, B, m, generator=g, dtype=F64) - 0.05, dtype),
-                  u_upper=round_through(0.5 * torch.rand(T, B, m, generator=g, dtype=F64) + 0.05, dtype))
-    C, c, F, f, x0 = (round_through(t, dtype) for t in (C, c, F, f, x0))
-    u = torch.zeros(T, B, m, dtype=F64)
-    o = orc.lqr_step_forward(n, m, T, x0, C, c, F, f, orc.get_traj(T, u, x0, F, f), u, coupled=False, **kw)
-    x, u = round_through(o.new_x, dtype), round_through(o.new_u, dtype)
-    wx = round_through(torch.randn(T, B, n, generator=g, dtype=F64), dtype)
-    wu = round_through(torch.randn(T, B, m, generator=g, dtype=F64), dtype)
-    P = dict(C=C, c=c, F=F, f=f, x0=x0, x=x, u=u, wx=wx, wu=wu)
-    ref64 = orc.lqr_step_backward(n, m, T, x0, C, c, F, f, x, u, wx, wu, coupled=False, **kw)
-    ref32 = None
-    if dtype == F32:
-        lo = lambda t: t.float() if torch.is_tensor(t) else t
-        ref32 = orc.lqr_step_backward(n, m, T, lo(x0), lo(C), lo(c), lo(F), lo(f), lo(x), lo(u), lo(wx), lo(wu),
-                                      coupled=False, **{k: lo(v) for k, v in kw.items()})
-    return P, kw, ref64, ref32
-
-
-def _run_abi_adjoint(n, m, T, case, dtype, impl=None):
-    P, kw, _, _ = case
-    d = lambda t: to_dev(t, dtype)  # noqa: E731
-    with kernel_env(impl):
-        return abi_adjoint(n, m, T, d(P["C"]), d(P["c"]), d(P["F"]), d(P["x"]), d(P["u"]), d(P["wx"]), d(P["wu"]),
-                           d(kw.get("u_lower")), d(kw.get("u_upper")), P["f"] is not None)
-
-
-def check_adjoint(tag, got, case, dtype):
-    _, _, ref64, ref32 = case
-    for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
-        if got[i] is None:
-            assert ref64[i].numel() == 0, f"{tag}: {name} missing"
-            continue
-        within(tag, name, got[i], ref64[i], ref32[i] if ref32 is not None else None, dtype)
-
-
-def check_routes_agree(tag, a, b, case, dtype):
-    """Two adjoint routes on one input: float64 within 1e-9 x scale of each other; float32 within the sum of their
-    float32 yardsticks (each is checked against the oracle on its own)."""
-    _, _, ref64, ref32 = case
-    for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
-        if a[i] is None:
-            continue
-        sc = max(1.0, float(ref64[i].abs().max()))
-        err = maxdiff(a[i], b[i])
-        bound = 1e-9 * sc if dtype == F64 else 2 * (4 * maxdiff(ref32[i], ref64[i]) + 1e-6 * sc)
-        assert err <= bound, f"{tag}: {name} routes differ by {err:.3e} > {bound:.3e}"
-
-
 ADJ_BOUNDS = (None, "box", "tensor")
 
 
@@ -295,7 +236,7 @@ def _adjoint_switch(n, m, dtype, check_plan):
         bounds = ADJ_BOUNDS[(n + m + k) % 3]
         with_f = (n + k) % 3 != 0
         case = adjoint_case(600 + n * 10 + m, B, T, n, m, dtype, bounds, with_f)
-        got, launches = _run_abi_adjoint(n, m, T, case, dtype)
+        got, launches = run_abi_adjoint(n, m, T, case, dtype)
         tag = f"adjoint n{n}m{m} {DT[dtype]} T={T} B={B} bounds={bounds} f={with_f}"
         assert launches == (2 if T < Ta else 4), f"{tag}: {launches} launches"
         check_plan(tag, T, launches, _L().last_step_plan())
@@ -344,33 +285,16 @@ def test_adjoint_routes_agree_at_short_horizon(n, m, dtype):
     with_f = n % 2 == 0
     case = adjoint_case(700 + n * 10 + m, B, T, n, m, dtype, bounds, with_f)
     tag = f"routes n{n}m{m} {DT[dtype]} T={T} bounds={bounds} f={with_f}"
-    g3, l3 = _run_abi_adjoint(n, m, T, case, dtype, impl=1)
+    g3, l3 = run_abi_adjoint(n, m, T, case, dtype, impl=1)
     assert l3 == 4, f"{tag}: {l3} launches"
     check_adjoint(tag + " 3-launch", g3, case, dtype)
     _seen(n, m, dtype, "adjoint_launches", l3)
     if (n, m) in PAIR_SHAPES:
-        g2, l2 = _run_abi_adjoint(n, m, T, case, dtype)
+        g2, l2 = run_abi_adjoint(n, m, T, case, dtype)
         assert l2 == 2, f"{tag}: {l2} launches"
         check_adjoint(tag + " fused", g2, case, dtype)
         _seen(n, m, dtype, "adjoint_launches", l2)
         check_routes_agree(tag + " fused vs 3-launch", g2, g3, case, dtype)
-
-
-def _autograd_backward(n, m, T, P, kw, dtype, keys=("x0", "C", "c", "F", "f")):
-    """LQRStepFn.backward through autograd (no_op_forward at the solution P["x"], P["u"]) with respect to P[keys]
-    (F and f are None when not in keys): ([dx_init, dC, dc, dF, df] on the CPU, None where not asked, library
-    launches)."""
-    from mpc.pytorch_b200 import LQRStep, QuadCost, LinDx
-    lv = [P[k].to(DEV, dtype).requires_grad_(True) for k in keys]
-    F, f = (dict(zip(keys, lv)).get(k) for k in ("F", "f"))
-    fn = LQRStep(n, m, T, true_cost=QuadCost(lv[1], lv[2]), true_dynamics=LinDx(F, f),
-                 current_x=P["x"].to(DEV, dtype), current_u=P["u"].to(DEV, dtype), no_op_forward=True,
-                 **{k: to_dev(v, dtype) for k, v in kw.items()})
-    xo, uo = fn(lv[0], lv[1], lv[2], F, f)
-    before = _L().launch_count()
-    grads = torch.autograd.grad((xo, uo), lv, (P["wx"].to(DEV, dtype), P["wu"].to(DEV, dtype)))
-    torch.cuda.synchronize()
-    return [g.cpu() for g in grads] + [None] * (5 - len(grads)), _L().launch_count() - before
 
 
 @pytest.mark.parametrize("dtype", [F32, F64], ids=["f32", "f64"])
@@ -381,12 +305,12 @@ def test_config5_backward_takes_three_launch_route(dtype):
     n, m, T, B = 16, 4, 50, 5
     case = adjoint_case(800, B, T, n, m, dtype, "box", True)
     tag = f"config5 backward {DT[dtype]}"
-    got, launches = _autograd_backward(n, m, T, *case[:2], dtype)
+    got, launches = autograd_backward(n, m, T, *case[:2], dtype)
     # (the step plan is per host thread, and autograd runs this backward on its own device thread)
     assert launches == 4, f"{tag}: {launches} launches, not the 3-launch route"
     _seen(n, m, dtype, "adjoint_launches", 4)
     check_adjoint(tag + " autograd", got, case, dtype)
-    three, l3 = _run_abi_adjoint(n, m, T, case, dtype, impl=1)
+    three, l3 = run_abi_adjoint(n, m, T, case, dtype, impl=1)
     assert l3 == 4, l3
     check_adjoint(tag + " 3-launch", three, case, dtype)
     check_routes_agree(tag + " default vs generic 3-launch", got, three, case, dtype)
@@ -407,7 +331,7 @@ def test_backward_is_one_library_call(n, m, T, dtype, B, launches):
     case = adjoint_case(1000 + n * 10 + m + T, B, T, n, m, dtype, "box", True)
     P, kw = case[:2]
     tag = f"backward n{n}m{m} T={T} {DT[dtype]}"
-    got, l_auto = _autograd_backward(n, m, T, P, kw, dtype)
+    got, l_auto = autograd_backward(n, m, T, P, kw, dtype)
     assert l_auto == launches, f"{tag}: {l_auto} launches"
     check_adjoint(tag, got, case, dtype)
     d = lambda t: to_dev(t, dtype)  # noqa: E731
@@ -433,7 +357,7 @@ def test_backward_single_step(with_F):
              wu=torch.randn(T, B, m, generator=g, dtype=F64))
     F_orc = P["F"] if with_F else torch.zeros(0, B, n, n + m, dtype=F64)
     ref = orc.lqr_step_backward(n, m, T, x0, P["C"], P["c"], F_orc, None, x, u, P["wx"], P["wu"], coupled=False)
-    got, launches = _autograd_backward(n, m, T, P, {}, dtype, keys=("x0", "C", "c", "F") if with_F else
+    got, launches = autograd_backward(n, m, T, P, {}, dtype, keys=("x0", "C", "c", "F") if with_F else
                                        ("x0", "C", "c"))
     assert launches == 2, launches
     for i, name in enumerate(("dx_init", "dC", "dc", "dF")):
@@ -445,25 +369,6 @@ def test_backward_single_step(with_F):
 # ------------------------------------------------------------------------------------------------------------------
 # mpcb200_lqr_grad_* (the costate workspace is required)
 # ------------------------------------------------------------------------------------------------------------------
-def _abi_grad(n, m, T, P, dx, du, dtype, with_f):
-    L = _L()
-    from mpc.pytorch_b200._lib import Dims, check, ptr, stream_handle
-    ins = [P["C"], P["c"], P["F"], P["x"], P["u"], dx, du, P["wx"]]
-    ins = [t.to(DEV, dtype).contiguous() for t in ins]             # kept alive across the call
-    B, p = P["C"].shape[1], n + m
-    dims = Dims(B=B, T=T, n=n, m=m, F_T=T - 1, has_f=int(with_f), max_ls_iter=1, pnqp_max_iter=1)
-    out = [torch.empty(B, n, dtype=dtype, device=DEV), torch.empty(T, B, p, p, dtype=dtype, device=DEV),
-           torch.empty(T, B, p, dtype=dtype, device=DEV), torch.empty(T - 1, B, n, p, dtype=dtype, device=DEV),
-           torch.empty(T - 1, B, n, dtype=dtype, device=DEV) if with_f else None]
-    ws = torch.empty(2 * T * B * n, dtype=dtype, device=DEV)
-    fn = L.lib().mpcb200_lqr_grad_f32 if dtype == F32 else L.lib().mpcb200_lqr_grad_f64
-    before = L.launch_count()
-    rc = fn(ctypes.byref(dims), *[ptr(t) for t in ins], *[ptr(t) for t in out], ptr(ws), stream_handle(DEV))
-    check(rc, "mpcb200_lqr_grad")
-    torch.cuda.synchronize()
-    return [t.cpu() if t is not None else None for t in out], L.launch_count() - before
-
-
 GRAD_CASES = [(8, 2, 9, F64), (8, 2, 300, F64), (5, 1, 9, F64), (5, 1, 300, F32), (16, 4, 12, F32), (16, 4, 250, F64)]
 
 
@@ -474,7 +379,8 @@ def test_grad_two_kernels_match_oracle(n, m, T, dtype):
     case = adjoint_case(900 + n + T, 12, T, n, m, dtype, "box", True)
     P, _, ref64, ref32 = case
     dx, du = ref64[5], ref64[6]
-    two, launches = _abi_grad(n, m, T, P, dx, du, dtype, True)
+    d = lambda t: to_dev(t, dtype)  # noqa: E731
+    two, launches = abi_grad(n, m, T, *[d(P[k]) for k in ("C", "c", "F", "x", "u")], d(dx), d(du), d(P["wx"]))
     assert launches == 2, launches
     tag = f"grad n{n}m{m} T={T} {DT[dtype]}"
     for i, name in enumerate(("dx_init", "dC", "dc", "dF", "df")):
