@@ -61,7 +61,8 @@ typedef struct mpcb200_dims {
   int32_t do_rollout;     /* 1: Riccati sweep + line-search rollout (LinDx/QuadCost)
                              0: Riccati sweep only; Ks/ks must be given                */
   int32_t dynamics_kind;  /* true dynamics of the rollout (reference lqr_step.py:217-225):
-                             MPCB200_DYN_LINEAR = LinDx(F,f); MPCB200_DYN_CARTPOLE / _PENDULUM = the step
+                             MPCB200_DYN_LINEAR = LinDx(F,f); MPCB200_DYN_CARTPOLE / _PENDULUM /
+                             _PENDULUM_FULL = the step
                              function of that system evaluated inside the kernel (params.dyn); F,f are
                              then its linearisation and are used by the Riccati sweep only (ABI v2);
                              OR'd with MPCB200_DYN_CTRL_PASSTHROUGH: that system under a slew-rate penalty */
@@ -84,12 +85,19 @@ typedef struct mpcb200_params {
 /* Known nonlinear systems (reference mpc/env_dx/cartpole.py:63-96, mpc/env_dx/pendulum.py:49-84).
  * dyn[] = cartpole: gravity, masscart, masspole, length, force_mag, dt   (state x,dx,cos th,sin th,dth; n=5, m=1)
  *         pendulum: g, m, l, (unused), max_torque, dt                    (state cos th,sin th,dth; n=3, m=1)
- * MPCB200_DYN_CTRL_PASSTHROUGH, OR'd into CARTPOLE or PENDULUM: the slew-rate augmented system of the reference's
+ *         pendulum_full: g, m, l, d, b, max_torque, dt                   (state cos th,sin th,dth; n=3, m=1)
+ * PENDULUM is the reference's PendulumDx(simple=True); PENDULUM_FULL is PendulumDx(simple=False), with damping d on
+ * the wrapped angle atan2(sin th, cos th) and gravity bias b inside sin(th + b), as the reference writes them.  The
+ * step of PENDULUM_FULL runs on a dynamics-only kernel instance at (3, 1).
+ * MPCB200_DYN_CTRL_PASSTHROUGH, OR'd into any of the three: the slew-rate augmented system of the reference's
  * CtrlPassthroughDynamics (mpc/dynamics.py:133-156).  State [u_{t-1}; x] (n = n_system + 1, m = 1), step
  * [u; step(x, u)] with u the control before the system's own clamp; its linearisation is F = [[0, 0, I], [0, R, S]],
  * f = [0; f_system].  Same dyn[] as the system.  Accepted by every call that takes a kind, at exactly that (n, m);
  * the step runs a dynamics-only kernel instance, which mpcb200_supported / _supported_list do not list. */
-enum { MPCB200_DYN_LINEAR = 0, MPCB200_DYN_CARTPOLE = 1, MPCB200_DYN_PENDULUM = 2, MPCB200_DYN_CTRL_PASSTHROUGH = 16 };
+enum {
+  MPCB200_DYN_LINEAR = 0, MPCB200_DYN_CARTPOLE = 1, MPCB200_DYN_PENDULUM = 2, MPCB200_DYN_PENDULUM_FULL = 4,
+  MPCB200_DYN_CTRL_PASSTHROUGH = 16
+};
 #define MPCB200_TIME_INVARIANT (-1)
 
 /* Per-problem status bits written to `status[B]`. */
@@ -211,7 +219,8 @@ int mpcb200_rollout_f64(const mpcb200_dims* dims, const double* F, const double*
  *   mpcb200_dyn_linearize_*: F[t,b] = [d step/dx, d step/du], f[t,b] = step(x,u) - F [x;u] at (x[t,b], u[t,b]),
  *                            t < T-1 - linearize_dynamics (reference mpc/mpc.py:490-601; its AUTO_DIFF mode does
  *                            (T-1)*n_state autograd passes).  Exact Jacobians by forward-mode dual numbers.
- * kind = MPCB200_DYN_CARTPOLE | MPCB200_DYN_PENDULUM, optionally | MPCB200_DYN_CTRL_PASSTHROUGH; dyn = HOST pointer
+ * kind = MPCB200_DYN_CARTPOLE | MPCB200_DYN_PENDULUM | MPCB200_DYN_PENDULUM_FULL, optionally
+ * | MPCB200_DYN_CTRL_PASSTHROUGH; dyn = HOST pointer
  * to 8 doubles (see mpcb200_params.dyn); x_init[B,n] u[T,B,m] x[T,B,n] F[T-1,B,n,n+m] f[T-1,B,n]; n, m are those of
  * the kind (n_system + 1 states with the passthrough).
  */
@@ -226,15 +235,17 @@ int mpcb200_dyn_linearize_f64(int32_t kind, const double* dyn, int32_t B, int32_
 
 /*
  * Vector-Jacobian product of mpcb200_dyn_linearize_* in the system's learnable parameters theta: cartpole dyn[0..3]
- * (gravity, masscart, masspole, length), pendulum dyn[0..2] (g, m, l); force_mag / max_torque and dt are constants.
+ * (gravity, masscart, masspole, length), pendulum dyn[0..2] (g, m, l), pendulum_full dyn[0..4] (g, m, l, d, b);
+ * force_mag / max_torque and dt are constants.
  * For t < T-1, with z = [x; u], J = [d step/dx, d step/du] and f = step(x, u) - J z at (x[t,b], u[t,b]):
  *   first[t,b,k]  = sum_r df[t,b,r] d step_r/dtheta_k
  *   second[t,b,k] = sum_{r,j} (dF[t,b,r,j] - df[t,b,r] z_j) dJ_rj/dtheta_k
  * so first + second, summed over (t, b), is the gradient of <dF, F> + <df, f> in theta; `first` alone is that gradient
  * with J held constant.  A control beyond the clamp contributes no u column (the clamp's derivative is 0 there).
- * kind = MPCB200_DYN_CARTPOLE or MPCB200_DYN_PENDULUM (a passthrough kind is MPCB200_ERR_BAD_DIMS); dyn = HOST pointer
- * to 8 doubles; x[T,B,n] u[T,B,1] dF[T-1,B,n,n+1] df[T-1,B,n]; first, second [T-1,B,NP] (NP = 4 cartpole, 3 pendulum),
- * either may be NULL.  One kernel; nothing is launched when T = 1 or both outputs are NULL.
+ * kind = MPCB200_DYN_CARTPOLE, MPCB200_DYN_PENDULUM or MPCB200_DYN_PENDULUM_FULL (a passthrough kind is
+ * MPCB200_ERR_BAD_DIMS); dyn = HOST pointer to 8 doubles; x[T,B,n] u[T,B,1] dF[T-1,B,n,n+1] df[T-1,B,n]; first,
+ * second [T-1,B,NP] (NP = 4 cartpole, 3 pendulum, 5 pendulum_full), either may be NULL.  One kernel; nothing is
+ * launched when T = 1 or both outputs are NULL.
  */
 int mpcb200_dyn_linearize_vjp_f32(int32_t kind, const double* dyn, int32_t B, int32_t T, const float* x,
                                   const float* u, const float* dF, const float* df, float* first, float* second,

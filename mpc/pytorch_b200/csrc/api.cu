@@ -34,10 +34,19 @@ static const Instance* find(int n, int m, int kind = DYN_LINEAR) {
     if (e->kind == kind && e->n == n && e->m == m) return e;
   return nullptr;
 }
-// the step instance of a call: the (n, m) instance, or for a passthrough kind its dynamics-only instance at exactly
-// that kind's (n, m)
+// whether the step of `kind` runs on a dynamics-only instance (dyn_instances.def): every passthrough kind, and every
+// kind with a record there
+static bool own_instance(int kind) {
+  if ((kind & DYN_CTRL_PASSTHROUGH) != 0) return true;
+  for (const Instance* e : kInstances)
+    if (kind != DYN_LINEAR && e->kind == kind) return true;
+  return false;
+}
+// the step instance of a call: such a kind runs its dynamics-only instance, at exactly that kind's (n, m); every
+// other call runs the (n, m) instance.  (An (n, m) instance's line search has no branch for a kind that has its own
+// instance.)
 static const Instance* find_step(const mpcb200_dims* d) {
-  return find(d->n, d->m, (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0 ? d->dynamics_kind : DYN_LINEAR);
+  return find(d->n, d->m, own_instance(d->dynamics_kind) ? d->dynamics_kind : DYN_LINEAR);
 }
 
 // The developer A/B knob MPCB200_KERNEL, read once per entry-point call (the tests flip it inside one process):
@@ -230,8 +239,8 @@ static int step_impl(const mpcb200_dims* d, const mpcb200_params* p, const StepC
 
 // whether the step of `d` keeps its gains in the caller's Ks/ks (mpcb200_step_prefers_workspace)
 static int gains_in_workspace(const mpcb200_dims* d, int elem_size, int knob) {
-  const bool passthrough = (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0;
-  if (!passthrough && runs_large(d->n, d->m, knob)) return 1;   // the large-shape step keeps its gains in Ks/ks
+  // the large-shape step keeps its gains in Ks/ks
+  if (!own_instance(d->dynamics_kind) && runs_large(d->n, d->m, knob)) return 1;
   const Instance* e = find_step(d);
   if (e == nullptr) return 1;                   // no instance: the step call itself reports it
   return e->ops[elem_size == 8].prefers_workspace(d->T, smem_optin_or_h100());
@@ -450,7 +459,8 @@ template <typename R>
 static int dyn_vjp_impl(int kind, const double* dyn, int B, int T, const R* x, const R* u, const R* dF, const R* df,
                         R* first, R* second, void* stream) {
   if (dyn == nullptr || x == nullptr || u == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (B <= 0 || T <= 0 || (kind != DYN_CARTPOLE && kind != DYN_PENDULUM)) return MPCB200_ERR_BAD_DIMS;
+  if (B <= 0 || T <= 0 || (kind != DYN_CARTPOLE && kind != DYN_PENDULUM && kind != DYN_PENDULUM_FULL))
+    return MPCB200_ERR_BAD_DIMS;
   if (T > 1 && (dF == nullptr || df == nullptr)) return MPCB200_ERR_NULL_POINTER;
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   if (T == 1 || (first == nullptr && second == nullptr)) return 0;

@@ -3,9 +3,10 @@
 // The reference linearises Module dynamics with autograd - (T-1)*n_state backward passes per iLQR iteration
 // (mpc/mpc.py:490-601, AUTO_DIFF :538-550) - and rolls them out with one Python call per time step
 // (mpc/util.py:102-126, mpc/lqr_step.py:224-225).  For the two systems its examples ship, the step functions
-// are restated here (cartpole: mpc/env_dx/cartpole.py:63-96, pendulum: mpc/env_dx/pendulum.py:49-84) as ONE
-// generic device function each, evaluated on plain numbers (rollouts, line search) or on forward-mode dual
-// numbers (exact Jacobians R = dx'/dx, S = dx'/du in one pass; f = x' - R x - S u as the reference forms it).
+// are restated here (cartpole: mpc/env_dx/cartpole.py:63-96, pendulum: mpc/env_dx/pendulum.py:49-84, in its
+// `simple` (g, m, l) and its five-parameter (g, m, l, d, b) form) as ONE generic device function each, evaluated on
+// plain numbers (rollouts, line search) or on forward-mode dual numbers (exact Jacobians R = dx'/dx, S = dx'/du in
+// one pass; f = x' - R x - S u as the reference forms it).
 #pragma once
 #include "common.cuh"
 
@@ -13,11 +14,13 @@ namespace mpcb200 {
 
 // DYN_CTRL_PASSTHROUGH is OR'd into a system's kind: the slew-rate augmented state [u_{t-1}; x] with dynamics
 // [u; f(x, u)] (reference CtrlPassthroughDynamics, mpc/dynamics.py:133-156), n_state + n_ctrl states
-enum { DYN_LINEAR = 0, DYN_CARTPOLE = 1, DYN_PENDULUM = 2, DYN_CTRL_PASSTHROUGH = 16 };
+enum { DYN_LINEAR = 0, DYN_CARTPOLE = 1, DYN_PENDULUM = 2, DYN_PENDULUM_FULL = 4, DYN_CTRL_PASSTHROUGH = 16 };
 
 struct DynParams {
   // cartpole: p[0..3] = gravity, masscart, masspole, length; p[4] = force_mag; p[5] = dt
   // pendulum: p[0..2] = g, m, l;                              p[4] = max_torque; p[5] = dt
+  // pendulum_full: p[0..4] = g, m, l, d, b;                   p[5] = max_torque; p[6] = dt
+  // The learnable parameters lead (DynLearnable<KIND>::NP of them): the VJP kernel seeds p[0..NP).
   double p[8];
 };
 
@@ -210,7 +213,7 @@ MPCB_DEV double dclamp(double a, double lo, double hi) { return a < lo ? lo : (a
 
 // ------------------------------------------------------------------ the two systems
 // The parameter number type P is R by default; a nested dual P differentiates in the learnable parameter `seed`
-// (cartpole p[0..3], pendulum p[0..2]).  force_mag / max_torque and dt are constants of type R.
+// (cartpole p[0..3], pendulum p[0..2], pendulum_full p[0..4]).  force_mag / max_torque and dt are constants of type R.
 // cartpole (mpc/env_dx/cartpole.py:63-96): state (x, dx, cos th, sin th, dth), one control (force)
 template <typename R, typename T, typename P = R>
 MPCB_DEV void cartpole_step(const DynParams& dp, const T (&s)[5], const T& u_in, T (&o)[5], int seed = -1) {
@@ -246,6 +249,23 @@ MPCB_DEV void pendulum_step(const DynParams& dp, const T (&s)[3], const T& u_in,
   o[1] = dsin(newth);
   o[2] = newdth;
 }
+// pendulum, five-parameter form (mpc/env_dx/pendulum.py:68-80, simple=False): damping d and gravity bias b.  As the
+// reference writes it: the damping acts on the wrapped angle th = atan2(sin, cos), not on dth, and the gravity term
+// is sin(th + b), not the state's sin th.
+template <typename R, typename T, typename P = R>
+MPCB_DEV void pendulum_full_step(const DynParams& dp, const T (&s)[3], const T& u_in, T (&o)[3], int seed = -1) {
+  using DP = DynParam<R, P>;
+  const P g = DP::get(dp, 0, seed), m = DP::get(dp, 1, seed), l = DP::get(dp, 2, seed), d = DP::get(dp, 3, seed),
+          b = DP::get(dp, 4, seed);
+  const R max_torque = (R)dp.p[5], dt = (R)dp.p[6];
+  const T u = dclamp(u_in, -max_torque, max_torque);
+  const T th = datan2(s[1], s[0]);
+  const T newdth = s[2] + dt * ((R(3.) * g / (R(2.) * l)) * dsin(b + th) + (R(3.) / (m * l * l)) * u - d * th);
+  const T newth = th + dt * newdth;
+  o[0] = dcos(newth);
+  o[1] = dsin(newth);
+  o[2] = newdth;
+}
 
 template <int KIND>
 struct DynDims {        // a passthrough kind: [u_{t-1}; x]
@@ -257,12 +277,15 @@ template <>
 struct DynDims<DYN_CARTPOLE> { static constexpr int N = 5, M = 1; };
 template <>
 struct DynDims<DYN_PENDULUM> { static constexpr int N = 3, M = 1; };
+template <>
+struct DynDims<DYN_PENDULUM_FULL> { static constexpr int N = 3, M = 1; };
 
 // (n_state, n_ctrl) of a known kind, passthrough or not; false for DYN_LINEAR and anything unknown
 inline bool dyn_kind_dims(int kind, int& n, int& m) {
   const int sys = kind & ~DYN_CTRL_PASSTHROUGH;
   if (sys == DYN_CARTPOLE) n = DynDims<DYN_CARTPOLE>::N, m = DynDims<DYN_CARTPOLE>::M;
   else if (sys == DYN_PENDULUM) n = DynDims<DYN_PENDULUM>::N, m = DynDims<DYN_PENDULUM>::M;
+  else if (sys == DYN_PENDULUM_FULL) n = DynDims<DYN_PENDULUM_FULL>::N, m = DynDims<DYN_PENDULUM_FULL>::M;
   else return false;
   if (kind & DYN_CTRL_PASSTHROUGH) n += m;
   return true;
@@ -284,8 +307,11 @@ MPCB_DEV void dyn_step(const DynParams& dp, const T (&s)[DynDims<KIND>::N], cons
     for (int i = 0; i < NI; ++i) o[1 + i] = oi[i];
   } else if constexpr (KIND == DYN_CARTPOLE) {
     cartpole_step<R, T, P>(dp, s, u, o, seed);
-  } else {
+  } else if constexpr (KIND == DYN_PENDULUM) {
     pendulum_step<R, T, P>(dp, s, u, o, seed);
+  } else {
+    static_assert(KIND == DYN_PENDULUM_FULL, "unknown dynamics kind");
+    pendulum_full_step<R, T, P>(dp, s, u, o, seed);
   }
 }
 
@@ -396,13 +422,15 @@ __global__ void __launch_bounds__(128) dyn_linearize_kernel(const DynArgs a) {
 }
 
 // Learnable parameters theta of a system: its first NP entries of DynParams::p (cartpole gravity, masscart, masspole,
-// length; pendulum g, m, l).  force_mag / max_torque and dt are constants.
+// length; pendulum g, m, l; pendulum_full g, m, l, d, b).  force_mag / max_torque and dt are constants.
 template <int KIND>
 struct DynLearnable;
 template <>
 struct DynLearnable<DYN_CARTPOLE> { static constexpr int NP = 4; };
 template <>
 struct DynLearnable<DYN_PENDULUM> { static constexpr int NP = 3; };
+template <>
+struct DynLearnable<DYN_PENDULUM_FULL> { static constexpr int NP = 5; };
 
 struct DynVjpArgs {
   int B, T, kind;
@@ -458,11 +486,14 @@ __global__ void __launch_bounds__(128) dyn_linearize_vjp_kernel(const DynVjpArgs
 template <typename R>
 int launch_dyn_rollout(const DynArgs& a, cudaStream_t stream) {
   const int grid = (a.B + 127) / 128;
-  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH;
+  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH,
+                FP = DYN_PENDULUM_FULL | DYN_CTRL_PASSTHROUGH;
   if (a.kind == DYN_CARTPOLE) dyn_rollout_kernel<R, DYN_CARTPOLE><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == DYN_PENDULUM) dyn_rollout_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == DYN_PENDULUM_FULL) dyn_rollout_kernel<R, DYN_PENDULUM_FULL><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == CP) dyn_rollout_kernel<R, CP><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == PP) dyn_rollout_kernel<R, PP><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == FP) dyn_rollout_kernel<R, FP><<<grid, 128, 0, stream>>>(a);
   else return 2;
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }
@@ -471,11 +502,14 @@ int launch_dyn_linearize(const DynArgs& a, cudaStream_t stream) {
   const size_t items = (size_t)(a.T - 1) * a.B;
   if (items == 0) return 0;
   const int grid = (int)((items + 127) / 128);
-  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH;
+  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH,
+                FP = DYN_PENDULUM_FULL | DYN_CTRL_PASSTHROUGH;
   if (a.kind == DYN_CARTPOLE) dyn_linearize_kernel<R, DYN_CARTPOLE><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == DYN_PENDULUM) dyn_linearize_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == DYN_PENDULUM_FULL) dyn_linearize_kernel<R, DYN_PENDULUM_FULL><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == CP) dyn_linearize_kernel<R, CP><<<grid, 128, 0, stream>>>(a);
   else if (a.kind == PP) dyn_linearize_kernel<R, PP><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == FP) dyn_linearize_kernel<R, FP><<<grid, 128, 0, stream>>>(a);
   else return 2;
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }
@@ -483,11 +517,12 @@ int launch_dyn_linearize(const DynArgs& a, cudaStream_t stream) {
 template <typename R>
 int launch_dyn_linearize_vjp(const DynVjpArgs& a, cudaStream_t stream) {
   const size_t items = (size_t)(a.T - 1) * a.B;
-  if (a.kind != DYN_CARTPOLE && a.kind != DYN_PENDULUM) return 2;
+  if (a.kind != DYN_CARTPOLE && a.kind != DYN_PENDULUM && a.kind != DYN_PENDULUM_FULL) return 2;
   if (items == 0) return 0;
   const int grid = (int)((items + 127) / 128);
   if (a.kind == DYN_CARTPOLE) dyn_linearize_vjp_kernel<R, DYN_CARTPOLE><<<grid, 128, 0, stream>>>(a);
-  else dyn_linearize_vjp_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == DYN_PENDULUM) dyn_linearize_vjp_kernel<R, DYN_PENDULUM><<<grid, 128, 0, stream>>>(a);
+  else dyn_linearize_vjp_kernel<R, DYN_PENDULUM_FULL><<<grid, 128, 0, stream>>>(a);
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }
 

@@ -13,7 +13,7 @@ struct InstanceOps {                  // one element type of one compiled shape
   int (*prefers_workspace)(int T, int max_smem);
   size_t (*smem_bytes)(int T);
 };
-// kind: DYN_LINEAR for an (n, m) instance of instances.def, or the passthrough kind of a dynamics-only instance.
+// kind: DYN_LINEAR for an (n, m) instance of instances.def, or the dynamics kind of a dynamics-only instance.
 // Constant-initialised (addresses only), so the records and api.cu's table of them need no start-up code.
 struct Instance {
   int kind, n, m;

@@ -494,8 +494,8 @@ MPCB_DEV void step_producer(const StepArgs& a, unsigned char* stage_base, uint64
 // ---------------------------------------------------------------------------------------------
 // consumer warps.  MODE (compile time): 0 plain (no bounds, no mask), 1 box (pnqp; optional
 // u_zero_I), 2 mask (u_zero_I only - the adjoint solve).
-// DYN: DYN_LINEAR for the (n, m) instances, whose rollout takes the true dynamics from a.dyn_kind; a passthrough kind
-// (DYN_CTRL_PASSTHROUGH | system) for the dynamics-only instances, whose rollout always runs that kind's dyn_step.
+// DYN: DYN_LINEAR for the (n, m) instances, whose rollout takes the true dynamics from a.dyn_kind; the kind of a
+// dynamics-only instance (dyn_instances.def), whose rollout always runs that kind's dyn_step.
 // ---------------------------------------------------------------------------------------------
 
 template <typename R, int N, int M, int MODE, int DYN = DYN_LINEAR>
@@ -950,7 +950,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
         xn[sl] = R(0);
         if (K::x_slot(sl) && t < T - 1) {                         // (:217-222), or true_dynamics(x, u) (:224-225)
           bool known = false;
-          if constexpr (DYN != DYN_LINEAR) {      // [u; dyn_step(x[m:], u)], as the known system below
+          if constexpr (DYN != DYN_LINEAR) {      // dyn_step of the instance's kind ([u; ...] for a passthrough)
             static_assert(N == DynDims<DYN>::N && M == DynDims<DYN>::M, "instance shape of the dynamics kind");
             known = true;
             R sv[N], ov[N];

@@ -1,7 +1,7 @@
 """Known nonlinear systems whose step function and exact Jacobians run inside the CUDA kernels
 (SURVEY.md section 8(f) rank 2): drop-in stand-ins for the reference's example environments
 ``mpc.env_dx.cartpole.CartpoleDx`` (mpc/env_dx/cartpole.py:28-96) and ``mpc.env_dx.pendulum.PendulumDx``
-(mpc/env_dx/pendulum.py:17-84, ``simple`` parametrisation).
+(mpc/env_dx/pendulum.py:17-84, both the ``simple`` (g, m, l) and the five-parameter (g, m, l, d, b) form).
 
 They are ordinary ``nn.Module`` dynamics - ``forward(x, u)`` is plain torch, so they work anywhere a Module
 does - but they also carry ``mpcb200_kind`` / ``mpcb200_params()``.  ``MPC.forward`` recognises that and, on
@@ -23,14 +23,20 @@ from torch.nn import Module
 from . import _lib
 from ._lib import MpcB200Error, _on_device, check, ptr, stream_handle
 
-DYN_LINEAR, DYN_CARTPOLE, DYN_PENDULUM = 0, 1, 2
+# DYN_PENDULUM is PendulumDx(simple=True), DYN_PENDULUM_FULL PendulumDx(simple=False)
+DYN_LINEAR, DYN_CARTPOLE, DYN_PENDULUM, DYN_PENDULUM_FULL = 0, 1, 2, 4
 # OR'd into a known system's kind: that system under a slew-rate penalty, state [u_{t-1}; x]
 # (solver.CtrlPassthroughDynamics), which the step runs on a dynamics-only kernel instance
 DYN_CTRL_PASSTHROUGH = 16
-DYN_DIMS = {DYN_CARTPOLE: (5, 1), DYN_PENDULUM: (3, 1)}       # (n_state, n_ctrl) of each known system
+DYN_KNOWN = (DYN_CARTPOLE, DYN_PENDULUM, DYN_PENDULUM_FULL)
+# (n_state, n_ctrl) of each known system
+DYN_DIMS = {DYN_CARTPOLE: (5, 1), DYN_PENDULUM: (3, 1), DYN_PENDULUM_FULL: (3, 1)}
 DYN_DIMS.update({k | DYN_CTRL_PASSTHROUGH: (n + m, m) for k, (n, m) in DYN_DIMS.items()})
 # number of learnable parameters of each system: the leading entries of its `params` tensor (mpcb200_params()[:NP])
-DYN_NPARAMS = {DYN_CARTPOLE: 4, DYN_PENDULUM: 3}
+DYN_NPARAMS = {DYN_CARTPOLE: 4, DYN_PENDULUM: 3, DYN_PENDULUM_FULL: 5}
+# kinds whose step runs on a dynamics-only kernel instance of their own (csrc/dyn_instances.def), at exactly their
+# (n_state, n_ctrl): the passthrough kinds, and the systems the (n, m) instances' line search has no branch for
+DYN_OWN_INSTANCE = frozenset({DYN_PENDULUM_FULL} | {k | DYN_CTRL_PASSTHROUGH for k in DYN_KNOWN})
 
 _scope = threading.local()      # depth and epoch of the enclosing params_scope() on this thread
 _epochs = itertools.count(1)    # process-wide: two threads' scopes never share an epoch (the cache is per module)
@@ -115,20 +121,28 @@ class CartpoleDx(Module):
 
 
 class PendulumDx(Module):
-    """state = (cos th, sin th, dth), one control (torque, clamped to +-max_torque); the reference's
-    ``simple`` parametrisation (g, m, l)."""
+    """state = (cos th, sin th, dth), one control (torque, clamped to +-max_torque).  ``simple=True``: the
+    reference's (g, m, l) parametrisation (kind DYN_PENDULUM).  ``simple=False``: its five-parameter form
+    (g, m, l, d, b) with damping d and gravity bias b (kind DYN_PENDULUM_FULL), written as the reference writes it:
+    d multiplies the wrapped angle atan2(sin th, cos th), and gravity acts through sin(th + b), not the state's
+    sin th."""
     mpcb200_kind = DYN_PENDULUM
     n_state, n_ctrl = 3, 1
 
     def __init__(self, params=None, simple=True):
         super().__init__()
-        if not simple:
-            raise NotImplementedError("only the `simple` (g, m, l) pendulum runs inside the kernels")
-        self.simple = True
+        self.simple = bool(simple)
+        if not self.simple:
+            self.mpcb200_kind = DYN_PENDULUM_FULL
         self.max_torque = 2.0
         self.dt = 0.05
-        self.params = torch.tensor((10.0, 1.0, 1.0)) if params is None else params
-        assert len(self.params) == 3
+        if params is None:
+            params = torch.tensor((10.0, 1.0, 1.0) if self.simple else (10.0, 1.0, 1.0, 0.0, 0.0))
+        self.params = params
+        if self.simple:
+            assert len(self.params) == 3
+        elif len(self.params) != 5:
+            raise ValueError(f"PendulumDx(simple=False) takes 5 params (g, m, l, d, b), got {len(self.params)}")
         self.goal_state = torch.tensor([1.0, 0.0, 0.0])
         self.goal_weights = torch.tensor([1.0, 1.0, 0.1])
         self.ctrl_penalty = 0.001
@@ -138,6 +152,9 @@ class PendulumDx(Module):
         self.max_linesearch_iter = 5
 
     def mpcb200_params(self):
+        if not self.simple:
+            g, m, l, d, b = _host_values(self, self.params)
+            return (g, m, l, d, b, float(self.max_torque), float(self.dt), 0.0)
         g, m, l = _host_values(self, self.params)
         return (g, m, l, 0.0, float(self.max_torque), float(self.dt), 0.0, 0.0)
 
@@ -145,10 +162,16 @@ class PendulumDx(Module):
         single = x.dim() == 1
         if single:
             x, u = x.unsqueeze(0), u.unsqueeze(0)
-        g, m, l = self.params.to(x, non_blocking=self.params.is_pinned()).unbind()
         tq = u.clamp(-self.max_torque, self.max_torque)[:, 0]
         c, s, om = x.unbind(1)
         th = torch.atan2(s, c)
+        if not self.simple:
+            g, m, l, d, b = self.params.to(x, non_blocking=self.params.is_pinned()).unbind()
+            om2 = om + self.dt * (3.0 * g / (2.0 * l) * torch.sin(th + b) + 3.0 * tq / (m * l ** 2) - d * th)
+            th2 = th + om2 * self.dt
+            out = torch.stack((torch.cos(th2), torch.sin(th2), om2), 1)
+            return out.squeeze(0) if single else out
+        g, m, l = self.params.to(x, non_blocking=self.params.is_pinned()).unbind()
         om2 = om + self.dt * (3.0 * g / (2.0 * l) * s + 3.0 * tq / (m * l ** 2))
         th2 = th + om2 * self.dt
         out = torch.stack((torch.cos(th2), torch.sin(th2), om2), 1)
@@ -277,7 +300,7 @@ class DynLinearize(torch.autograd.Function):
 
 
 def linearize_known(dynamics, kind, kparams, T, x, u):
-    """(F, f) of the known system `dynamics` (kind DYN_CARTPOLE or DYN_PENDULUM) along (x, u), as MPC's differentiable
+    """(F, f) of the known system `dynamics` (a kind of DYN_KNOWN) along (x, u), as MPC's differentiable
     tail needs it: through DynLinearize when autograd records and dynamics.params requires grad, otherwise one
     dyn_linearize_raw launch and no graph.  x and u are detached either way (no gradient reaches the linearisation
     point)."""

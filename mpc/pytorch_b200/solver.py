@@ -119,15 +119,15 @@ class SlewRateCost(Module):
 
 class CtrlPassthroughDynamics(Module):
     """Dynamics of the slew-augmented state [u_{t-1}; x] (reference mpc/dynamics.py:133-156).  Wrapping a known
-    system (dynamics.CartpoleDx / PendulumDx) it is one too, of kind inner | DYN_CTRL_PASSTHROUGH, so its rollout,
-    linearisation and line-search rollout run in the kernels; any other Module keeps the Module path."""
+    system (dynamics.CartpoleDx / PendulumDx, either form) it is one too, of kind inner | DYN_CTRL_PASSTHROUGH, so its
+    rollout, linearisation and line-search rollout run in the kernels; any other Module keeps the Module path."""
 
     def __init__(self, dynamics):
         super().__init__()
         self.dynamics = dynamics
-        from .dynamics import DYN_CARTPOLE, DYN_CTRL_PASSTHROUGH, DYN_PENDULUM
+        from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_KNOWN
         kind = getattr(dynamics, "mpcb200_kind", None)
-        if kind in (DYN_CARTPOLE, DYN_PENDULUM):
+        if kind in DYN_KNOWN:
             self.mpcb200_kind = kind | DYN_CTRL_PASSTHROUGH
             self.n_state, self.n_ctrl = dynamics.n_state + dynamics.n_ctrl, dynamics.n_ctrl
             self.mpcb200_params = dynamics.mpcb200_params      # the system's: its params_scope cache applies

@@ -16,7 +16,7 @@ from torch.nn import Module
 
 from . import _lib
 from ._lib import Dims, Params, MpcB200Error, _on_device, check, ptr, ptr_view, stream_handle
-from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_DIMS, DYN_LINEAR
+from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_DIMS, DYN_LINEAR, DYN_OWN_INSTANCE
 
 PNQP_MAX_ITER = 20  # reference passes n_iter=20 (mpc/lqr_step.py:137)
 
@@ -133,9 +133,10 @@ _smem_fits_cache = {}
 
 def _pick_instance(n, m, elem_size=4, kind=DYN_LINEAR):
     """The (N, M) kernel shape an (n, m) problem runs at: the smallest compiled instance that covers it (zero padded),
-    else (n, m) itself on the large-shape kernels if they fit it in `elem_size`-byte elements.  A passthrough dynamics
-    `kind` runs its dynamics-only instance, which exists at exactly that kind's (n, m) only."""
-    if kind & DYN_CTRL_PASSTHROUGH:
+    else (n, m) itself on the large-shape kernels if they fit it in `elem_size`-byte elements.  A dynamics `kind` with
+    a dynamics-only instance (DYN_OWN_INSTANCE: every passthrough kind, and DYN_PENDULUM_FULL) runs that instance,
+    which exists at exactly that kind's (n, m) only."""
+    if kind in DYN_OWN_INSTANCE or kind & DYN_CTRL_PASSTHROUGH:
         if DYN_DIMS.get(kind) != (n, m):
             raise MpcB200Error(f"dynamics kind {kind} has no kernel instance at (n_state={n}, n_ctrl={m})")
         return n, m

@@ -126,8 +126,9 @@ static int run_case(int B, int T, int n, int m, int bounds_kind, int with_mask) 
 // known systems: rollout, exact Jacobians, and the step kernel with the system inside its line search
 static int run_dyn(int kind, int B, int T) {
   const int n = kind == MPCB200_DYN_CARTPOLE ? 5 : 3, m = 1, p = n + m;
-  const double prm_c[8] = {9.8, 1.0, 0.1, 0.5, 100.0, 0.05, 0, 0}, prm_p[8] = {10.0, 1.0, 1.0, 0.0, 2.0, 0.05, 0, 0};
-  const double* dyn = kind == MPCB200_DYN_CARTPOLE ? prm_c : prm_p;
+  const double prm_c[8] = {9.8, 1.0, 0.1, 0.5, 100.0, 0.05, 0, 0}, prm_p[8] = {10.0, 1.0, 1.0, 0.0, 2.0, 0.05, 0, 0},
+               prm_pf[8] = {10.0, 1.0, 1.0, 0.3, 0.2, 2.0, 0.05, 0};
+  const double* dyn = kind == MPCB200_DYN_CARTPOLE ? prm_c : (kind == MPCB200_DYN_PENDULUM ? prm_p : prm_pf);
   std::vector<float> x0((size_t)B * n), u((size_t)T * B * m), C((size_t)T * B * p * p, 0.f), c((size_t)T * B * p);
   for (int b = 0; b < B; ++b) {
     const float th = 3.f * rnd();
@@ -147,7 +148,7 @@ static int run_dyn(int kind, int B, int T) {
   rc = mpcb200_dyn_linearize_f32(kind, dyn, B, T, dx.p, du.p, dF.p, df.p, nullptr);
   if (rc) return printf("dyn linearize rc=%d\n", rc), 1;
   {  // parameter VJP of the linearisation with (dF, df) = (F, f); second output omitted once
-    const int np = n == 5 ? 4 : 3;
+    const int np = kind == MPCB200_DYN_CARTPOLE ? 4 : (kind == MPCB200_DYN_PENDULUM ? 3 : 5);
     Dev<float> first((size_t)(T - 1) * B * np), second((size_t)(T - 1) * B * np);
     rc = mpcb200_dyn_linearize_vjp_f32(kind, dyn, B, T, dx.p, du.p, dF.p, df.p, first.p, second.p, nullptr);
     if (rc) return printf("dyn linearize vjp rc=%d\n", rc), 1;
@@ -216,6 +217,7 @@ int main() {
   fails += run_pnqp_large(3, 100);
   fails += run_dyn(MPCB200_DYN_CARTPOLE, 37, 9);
   fails += run_dyn(MPCB200_DYN_PENDULUM, 20, 7);
+  fails += run_dyn(MPCB200_DYN_PENDULUM_FULL, 20, 7);
   const int cases[][6] = {{13, 6, 8, 2, 0, 0}, {13, 6, 8, 2, 1, 0}, {12, 5, 8, 2, 2, 1}, {7, 4, 3, 1, 1, 0},
                           {5, 4, 16, 4, 2, 0}, {1, 3, 2, 2, 0, 0}, {33, 7, 5, 1, 1, 1}, {9, 3, 3, 4, 2, 0},
                           {64, 40, 8, 2, 1, 0}, {16, 6, 4, 2, 1, 0}, {12, 5, 16, 4, 0, 0}, {24, 6, 8, 2, 2, 1},

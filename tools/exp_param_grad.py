@@ -10,9 +10,14 @@ Workloads (learnable `params` on the device, requires_grad; the loss is a fixed 
   config2       cartpole B=128, T=25, bounds +-100, <=50 iterations, eps 1e-2, float32: MPC.forward + backward
   pendulum      the pendulum notebook's size, B=16, T=20, PendulumDx(params=(10, 1, 1)), bounds +-2, float32
   config2_f64   config2 in float64 (also gives d/dc and d/dx_init, to compare against TREE at rounding level)
+  pendulum_full the pendulum notebook's size with the five-parameter PendulumDx(params=(10, 1, 1, 0.3, 0.2),
+                simple=False), bounds +-2, float32: MPC.forward + backward, d/dparams of all five entries
+  pendulum_full_opaque  the same with the physics wrapped as an opaque Module (torch rollout, AUTO_DIFF with
+                create_graph, split-mode line search: the only route before the kernels knew this system)
 Each tree runs in worker processes of its own, alternated (measure.alternate): this tree, TREE, this tree, ...  A
 worker warms up once, then times --reps calls (measure.host_time); the first worker of each tree saves its outputs,
-and the parent compares them (measure.compare, and the relative change of each gradient).  Prints one JSON line per
+and the parent compares them (measure.compare, and the relative change of each gradient).  A tree that cannot
+build a workload's system (PendulumDx(simple=False) raising NotImplementedError) leaves that workload out.  Prints one JSON line per
 workload and the card (measure.card); with --out DIR, also writes DIR/exp_param_grad.json."""
 import argparse
 import json
@@ -20,7 +25,8 @@ import statistics
 
 import measure
 
-WORKLOADS = ("tail_known", "tail_opaque", "config2", "pendulum", "config2_f64")
+WORKLOADS = ("tail_known", "tail_opaque", "config2", "pendulum", "config2_f64", "pendulum_full",
+             "pendulum_full_opaque")
 
 
 def _worker(tree, out, save, reps):
@@ -31,11 +37,13 @@ def _worker(tree, out, save, reps):
     dev = torch.device("cuda:0")
 
     def problem(name, dtype):
-        B, T = (16, 20) if name == "pendulum" else (128, 25)
+        B, T = (128, 25) if name == "cartpole" else (16, 20)
         g = torch.Generator().manual_seed(0)
-        if name == "pendulum":
-            params = torch.tensor((10.0, 1.0, 1.0), dtype=dtype, device=dev).requires_grad_(True)
-            dx = PendulumDx(params=params)
+        if name.startswith("pendulum"):
+            full = name == "pendulum_full"
+            params = torch.tensor((10.0, 1.0, 1.0, 0.3, 0.2) if full else (10.0, 1.0, 1.0), dtype=dtype,
+                                  device=dev).requires_grad_(True)
+            dx = PendulumDx(params=params, simple=not full)
             th = (torch.rand(B, generator=g, dtype=dtype) * 2 - 1) * 1.5708
             x0 = torch.stack((th.cos(), th.sin(), torch.rand(B, generator=g, dtype=dtype) * 2 - 1), 1)
         else:
@@ -58,7 +66,8 @@ def _worker(tree, out, save, reps):
 
     def make(workload):
         dtype = torch.float64 if workload == "config2_f64" else torch.float32
-        ctrl, dx, params, x0, Q, c, wx, wu = problem("pendulum" if workload == "pendulum" else "cartpole", dtype)
+        name = workload.replace("_opaque", "") if workload.startswith("pendulum") else "cartpole"
+        ctrl, dx, params, x0, Q, c, wx, wu = problem(name, dtype)
         if workload.startswith("tail"):
             with torch.no_grad():
                 x, u, _ = ctrl(x0, QuadCost(Q, c), dx)
@@ -72,6 +81,8 @@ def _worker(tree, out, save, reps):
                 g, = torch.autograd.grad((wF * F).sum() + (wx[:-1] * f).sum(), params)
                 return {"F": F.detach(), "f": f.detach(), "grad_params": g}
             return run
+        if workload == "pendulum_full_opaque":
+            dx = measure.Opaque(dx)
         leaves = [params, c, x0] if dtype == torch.float64 else [params]
 
         def run():
@@ -84,7 +95,10 @@ def _worker(tree, out, save, reps):
 
     times, saved = {}, {}
     for w in WORKLOADS:
-        run = make(w)
+        try:
+            run = make(w)
+        except NotImplementedError:
+            continue
         run()                                           # warm-up
         times[w], saved[w] = measure.host_time(run, reps)
     measure.save(out, times, outputs=saved if save else None)
@@ -109,9 +123,11 @@ def main():
     times, _, outs = measure.alternate(__file__, arms, a.rounds, ["--reps", str(a.reps)])
     rows = []
     for w in WORKLOADS:
+        if w not in times["this"]:
+            continue
         row = dict(workload=w, this_ms=1e3 * statistics.median(times["this"][w]),
                    this_ms_all=[round(1e3 * t, 3) for t in times["this"][w]])
-        if "parent" in arms:
+        if "parent" in arms and w in times["parent"]:
             row.update(parent_ms=1e3 * statistics.median(times["parent"][w]),
                        parent_ms_all=[round(1e3 * t, 3) for t in times["parent"][w]])
             row["speedup"] = row["parent_ms"] / row["this_ms"]
@@ -123,6 +139,9 @@ def main():
         print(json.dumps(row), flush=True)
     print(f"tail: known system {rows[0]['this_ms']:.3f} ms, opaque Module {rows[1]['this_ms']:.3f} ms "
           f"(x{rows[1]['this_ms'] / rows[0]['this_ms']:.1f})")
+    by = {r["workload"]: r["this_ms"] for r in rows}
+    print(f"pendulum_full: kernels {by['pendulum_full']:.3f} ms, opaque Module {by['pendulum_full_opaque']:.3f} ms "
+          f"(x{by['pendulum_full_opaque'] / by['pendulum_full']:.1f})")
     runs = {k: {w: [round(1e3 * t, 3) for t in ts] for w, ts in v.items()} for k, v in times.items()}
     measure.report(a.out, __file__, c, rows, runs, rounds=a.rounds, reps=a.reps)
 
