@@ -369,6 +369,59 @@ int mpcb200_episode_f64(const mpcb200_dims* dims, const mpcb200_params* params, 
                         double* xs, double* us, double* costs, int32_t* info, double* u_next,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * mpcb200_episode_* that also keeps each solve's best iterate: plan_x[n_steps,T,B,n] and plan_u[n_steps,T,B,m]
+ * (plan_u[k][0] = us[k]), the linearisation points of mpcb200_episode_backward_*.  Same arguments, outputs and graph
+ * as mpcb200_episode_*, plus one kernel node per control step (before the advance kernel) that copies the plan.
+ * NULL plan_x or plan_u: MPCB200_ERR_NULL_POINTER.  Workspace: mpcb200_episode_workspace_bytes().
+ */
+int mpcb200_episode_plans_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                              int32_t n_steps, const float* C, const float* c, const float* F, const float* f,
+                              const float* x_init, const float* u_init,
+                              const float* u_lower, const float* u_upper, const uint8_t* u_zero_I,
+                              float* xs, float* us, float* costs, int32_t* info, float* u_next,
+                              float* plan_x, float* plan_u, void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_plans_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                              int32_t n_steps, const double* C, const double* c, const double* F, const double* f,
+                              const double* x_init, const double* u_init,
+                              const double* u_lower, const double* u_upper, const uint8_t* u_zero_I,
+                              double* xs, double* us, double* costs, int32_t* info, double* u_next,
+                              double* plan_x, double* plan_u, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The reverse sweep of an episode of mpcb200_episode_plans_* (no slew-rate penalty): given dl_dxs[n_steps+1,B,n]
+ * and dl_dus[n_steps,B,m], the gradient of L(xs, us) for the closed loop
+ *   plan_k = the solve from x_k (its KKT adjoint at the best iterate, as mpcb200_lqr_adjoint_* with u_lower/u_upper;
+ *            a known system's F, f its linearisation along the plan, differentiable in theta),
+ *   u_k = plan_u[k][0],  x_{k+1} = the model step (LinDx F[0] [x_k; u_k] + f[0]; a known system one step of it),
+ * with the warm starts held constant.  dims, params, C, c, F, u_lower, u_upper: the staged problem of the forward
+ * (f does not enter the gradient); xs, us, plan_x, plan_u: its outputs.
+ * Outputs: dx_init[B,n], dC[T,B,p,p], dc[T,B,p] (dense, whatever C's and c's time strides); LinDx: dF[F_T,B,n,p]
+ * (dense) and, with has_f, df[T-1,B,n] (the model step's f[0] and the adjoints' f[t < T-1]); a known system
+ * (dims->dynamics_kind 1, 2 or 4): dtheta[B,NP], per problem b the gradient in the system's learnable parameters
+ * params->dyn[0..NP), summed in a fixed order (NP = 4, 3, 5); dF, df unused.
+ * One CUDA graph: an init kernel, then a conditional `while` node over k = n_steps-1 .. 0 whose body is a staging
+ * kernel (the plan of step k into fixed buffers and the model step's VJP), [the linearisation,] the adjoint, [the
+ * linearisation's VJP] and an accumulate kernel that counts k down.  Capture contract, launch counting and
+ * MPCB200_ERR_NO_GRAPH_COND as for mpcb200_ilqr_*.  T >= 3 and n_steps >= 1, else MPCB200_ERR_BAD_DIMS.
+ * workspace: mpcb200_episode_backward_workspace_bytes() bytes (0 for dims it does not take), 256-byte aligned.
+ */
+size_t mpcb200_episode_backward_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size);
+int mpcb200_episode_backward_f32(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                 const float* C, const float* c, const float* F,
+                                 const float* u_lower, const float* u_upper,
+                                 const float* xs, const float* us, const float* plan_x, const float* plan_u,
+                                 const float* dl_dxs, const float* dl_dus,
+                                 float* dx_init, float* dC, float* dc, float* dF, float* df, float* dtheta,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_backward_f64(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                 const double* C, const double* c, const double* F,
+                                 const double* u_lower, const double* u_upper,
+                                 const double* xs, const double* us, const double* plan_x, const double* plan_u,
+                                 const double* dl_dxs, const double* dl_dus,
+                                 double* dx_init, double* dC, double* dc, double* dF, double* df, double* dtheta,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);
 

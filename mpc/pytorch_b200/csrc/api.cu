@@ -6,6 +6,7 @@
 #include <cstring>
 
 #include "../../../include/mpcb200.h"
+#include "episode_grad.cuh"
 #include "ilqr.cuh"
 #include "instance.cuh"
 #include "lqr_large.cuh"
@@ -342,7 +343,7 @@ template <typename R>
 static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R* C, const R* c, const R* F,
                         const R* new_x, const R* new_u, const R* dl_dx, const R* dl_du, const R* u_lower,
                         const R* u_upper, R* dx_init, R* dC, R* dc, R* dF, R* df, void* workspace,
-                        size_t workspace_bytes, int knob, void* stream) {
+                        size_t workspace_bytes, int knob, void* stream, bool zero_by_kernel = false) {
   int rc = check_dims(d);
   if (rc) return rc;
   if (p == nullptr || C == nullptr || c == nullptr || new_x == nullptr || new_u == nullptr || dl_dx == nullptr ||
@@ -397,8 +398,13 @@ static int adjoint_impl(const mpcb200_dims* d, const mpcb200_params* p, const R*
     if (rc != MPCB200_ERR_UNSUPPORTED_DIMS && rc != MPCB200_ERR_SMEM) return rc;
   }
   // 3-launch path: the nested solve really reads its (zero) nominal trajectory, and keeps its gains in the workspace
-  // where a step call with Ks/ks would (gains_in_workspace)
-  if (cudaMemsetAsync(zeros, 0, TB * (d->n + d->m) * sizeof(R), st) != cudaSuccess) return MPCB200_ERR_LAUNCH;
+  // where a step call with Ks/ks would (gains_in_workspace).  `zero_by_kernel`: a kernel zeroes it, for a caller
+  // that records the adjoint into a conditional body, which holds kernel nodes only (mpcb200_episode_backward_*).
+  if (zero_by_kernel) {
+    if (counted(launch_fill_zero<R>(TB * (d->n + d->m), zeros, st)) != 0) return MPCB200_ERR_LAUNCH;
+  } else if (cudaMemsetAsync(zeros, 0, TB * (d->n + d->m) * sizeof(R), st) != cudaSuccess) {
+    return MPCB200_ERR_LAUNCH;
+  }
   sc.u_lower = sc.u_upper = nullptr;
   if (l.gains) {
     sc.Ks = (R*)(ws + l.Ks);
@@ -766,6 +772,7 @@ struct EpisodeCall {
   R* u_next;
   void* workspace;
   size_t workspace_bytes;
+  R *plan_x, *plan_u;          // mpcb200_episode_plans_*: each solve's best iterate; NULL for mpcb200_episode_*
 };
 
 // the solve of every control step: the caller's problem from the state and warm-start buffers, its best iterate in
@@ -791,6 +798,7 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
       e.u_next == nullptr || e.workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (e.d->T < 3 || e.n_steps < 1) return MPCB200_ERR_BAD_DIMS;     // the warm-start shift reads u[T-3]
+  if ((e.plan_x == nullptr) != (e.plan_u == nullptr)) return MPCB200_ERR_NULL_POINTER;
   const EpisodeLayout l = episode_layout(e.d, sizeof(R), knob);
   if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
@@ -798,7 +806,8 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
 }
 
 // Adds the episode's init kernel and its `while` node over control steps (body recorded on `es`) to the graph `os`
-// is capturing.  Body: the iLQR loop (its own `while` node, body on `bs`) -> model step -> episode_advance_kernel.
+// is capturing.  Body: the iLQR loop (its own `while` node, body on `bs`) -> model step -> [episode_plans_kernel,
+// with plan_x / plan_u] -> episode_advance_kernel.
 template <typename R>
 static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, const EpisodeCall<R>& e, int knob) {
   const mpcb200_dims* d = e.d;
@@ -828,6 +837,8 @@ static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, con
   } else if (rc == 0) {
     rc = dyn_impl<R>(false, d->dynamics_kind, e.p->dyn, B, 2, state, q.best_u, traj, nullptr, nullptr, es);
   }
+  if (rc == 0 && e.plan_x != nullptr)
+    rc = counted(episode_launch_plans<R>(B, T, N, M, q.best_x, q.best_u, e.plan_x, e.plan_u, ep, es));
   if (rc == 0)
     rc = counted(episode_launch_advance<R>(B, T, N, M, e.o->m_ref, e.n_steps, traj, q.best_u, q.best_costs, q.info,
                                            state, warm, e.xs, e.us, e.costs, e.info, ep, handle, es));
@@ -848,6 +859,170 @@ static int episode_impl(const EpisodeCall<R>& e, void* stream) {
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t es = ilqr_stream(2), bs = ilqr_stream(1);
     return es == nullptr || bs == nullptr ? MPCB200_ERR_LAUNCH : episode_record<R>(os, es, bs, e, knob);
+  });
+}
+
+// ---------------------------------------------------------------------------------------------
+// the reverse sweep of an episode (episode_grad.cuh): for k = n_steps-1 .. 0, the model step's VJP, each solve's KKT
+// adjoint at its best iterate (a known system: through its linearisation and that linearisation's VJP), summed
+// ---------------------------------------------------------------------------------------------
+// learnable parameters of a known system (DynLearnable), 0 for anything else
+static int dyn_nparams(int kind) {
+  return kind == DYN_CARTPOLE ? DynLearnable<DYN_CARTPOLE>::NP
+         : kind == DYN_PENDULUM ? DynLearnable<DYN_PENDULUM>::NP
+         : kind == DYN_PENDULUM_FULL ? DynLearnable<DYN_PENDULUM_FULL>::NP : 0;
+}
+// dims of each step's adjoint: the episode's; a known system's F, f are its dense linearisation [T-1, B, ...]
+static mpcb200_dims epgrad_adjoint_dims(const mpcb200_dims* d) {
+  mpcb200_dims da = *d;
+  if (d->dynamics_kind != DYN_LINEAR) {
+    da.F_T = d->T - 1; da.has_f = 1; da.F_tstride = 0; da.f_tstride = 0;
+  }
+  da.dynamics_kind = DYN_LINEAR;
+  return da;
+}
+
+struct EpGradLayout {                 // workspace carve-up (byte offsets, every piece 256-byte aligned)
+  mpcb200_dims da;
+  size_t adj, adj_bytes, stage_x, stage_u, dl_dx, dl_du, gx, theta, dxk, dCk, dck, dFk, dfk, Fk, fk, first, second,
+      state, total;
+};
+static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob) {
+  EpGradLayout l;
+  l.da = epgrad_adjoint_dims(d);
+  const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m, TB = T * B, T1B = (T - 1) * B;
+  const size_t NP = dyn_nparams(d->dynamics_kind);
+  const bool known = d->dynamics_kind != DYN_LINEAR;
+  size_t o = 0;
+  l.adj_bytes = adj_layout(&l.da, sz, knob).total;
+  l.adj = o;      o += up256(l.adj_bytes);
+  l.stage_x = o;  o += up256(TB * n * sz);
+  l.stage_u = o;  o += up256(TB * m * sz);
+  l.dl_dx = o;    o += up256(TB * n * sz);
+  l.dl_du = o;    o += up256(TB * m * sz);
+  l.gx = o;       o += up256(B * n * sz);
+  l.theta = o;    o += up256(B * NP * sz);
+  l.dxk = o;      o += up256(B * n * sz);
+  l.dCk = o;      o += up256(TB * p * p * sz);
+  l.dck = o;      o += up256(TB * p * sz);
+  l.dFk = o;      o += up256((size_t)l.da.F_T * B * n * p * sz);
+  l.dfk = o;      o += up256(l.da.has_f ? T1B * n * sz : 0);
+  l.Fk = l.fk = l.first = l.second = 0;
+  if (known) {                        // the linearisation along the staged plan, and its VJP
+    l.Fk = o;     o += up256(T1B * n * p * sz);
+    l.fk = o;     o += up256(T1B * n * sz);
+    l.first = o;  o += up256(T1B * NP * sz);
+    l.second = o; o += up256(T1B * NP * sz);
+  }
+  l.state = o;    o += up256(sizeof(EpGradState));
+  l.total = o;
+  return l;
+}
+
+// the arguments of mpcb200_episode_backward_*, in the header's order
+template <typename R>
+struct EpGradCall {
+  const mpcb200_dims* d;
+  const mpcb200_params* p;
+  int n_steps;
+  const R *C, *c, *F, *u_lower, *u_upper, *xs, *us, *plan_x, *plan_u, *dl_dxs, *dl_dus;
+  R *dx_init, *dC, *dc, *dF, *df, *dtheta;
+  void* workspace;
+  size_t workspace_bytes;
+};
+
+// argument checks that need no device: every error is reported before anything is captured or launched
+template <typename R>
+static int epgrad_check(const EpGradCall<R>& q, int knob) {
+  const mpcb200_dims* d = q.d;
+  int rc = check_dims(d);
+  if (rc) return rc;
+  if (q.p == nullptr || q.C == nullptr || q.c == nullptr || q.xs == nullptr || q.us == nullptr ||
+      q.plan_x == nullptr || q.plan_u == nullptr || q.dl_dxs == nullptr || q.dl_dus == nullptr ||
+      q.dx_init == nullptr || q.dC == nullptr || q.dc == nullptr || q.workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (d->T < 3 || q.n_steps < 1) return MPCB200_ERR_BAD_DIMS;
+  rc = check_bounds(d, q.u_lower, q.u_upper);
+  if (rc) return rc;
+  if (d->dynamics_kind != DYN_LINEAR) {
+    // a known system itself: a slew-rate (passthrough) episode has no device backward
+    if (dyn_nparams(d->dynamics_kind) == 0 || !known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
+    if (q.dtheta == nullptr) return MPCB200_ERR_NULL_POINTER;
+  } else {
+    if (q.F == nullptr || q.dF == nullptr) return MPCB200_ERR_NULL_POINTER;
+    if (d->has_f && q.df == nullptr) return MPCB200_ERR_NULL_POINTER;
+  }
+  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob);
+  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+// Adds the init kernel and the `while` node over k = n_steps-1 .. 0 (body recorded on `bs`) to the graph `os` is
+// capturing.  Body: stage -> [linearisation] -> adjoint -> [linearisation VJP] -> accumulate.
+template <typename R>
+static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, int knob) {
+  const mpcb200_dims* d = q.d;
+  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob);
+  char* ws = (char*)q.workspace;
+  const bool known = d->dynamics_kind != DYN_LINEAR;
+  const int B = d->B, T = d->T;
+  EpGradArgs<R> a;
+  std::memset(&a, 0, sizeof(a));
+  a.B = B; a.T = T; a.N = d->n; a.M = d->m; a.n_steps = q.n_steps; a.F_T = l.da.F_T; a.has_f = l.da.has_f;
+  a.kind = d->dynamics_kind; a.NP = dyn_nparams(d->dynamics_kind);
+  for (int i = 0; i < 8; ++i) a.dp.p[i] = q.p->dyn[i];
+  a.xs = q.xs; a.us = q.us; a.plan_x = q.plan_x; a.plan_u = q.plan_u; a.dl_dxs = q.dl_dxs; a.dl_dus = q.dl_dus;
+  a.F = known ? nullptr : q.F;
+  a.stage_x = (R*)(ws + l.stage_x); a.stage_u = (R*)(ws + l.stage_u);
+  a.dl_dx = (R*)(ws + l.dl_dx); a.dl_du = (R*)(ws + l.dl_du);
+  a.gx = (R*)(ws + l.gx); a.theta_step = known ? (R*)(ws + l.theta) : nullptr;
+  a.g = q.dx_init;
+  R* dxk = (R*)(ws + l.dxk);
+  R* dCk = (R*)(ws + l.dCk);
+  R* dck = (R*)(ws + l.dck);
+  R* dFk = (R*)(ws + l.dFk);
+  R* dfk = l.da.has_f ? (R*)(ws + l.dfk) : nullptr;
+  R* first = known ? (R*)(ws + l.first) : nullptr;
+  R* second = known ? (R*)(ws + l.second) : nullptr;
+  a.dx_k = dxk; a.dC_k = dCk; a.dc_k = dck; a.dF_k = dFk; a.df_k = dfk; a.first = first; a.second = second;
+  a.dC = q.dC; a.dc = q.dc;
+  a.dF = known ? nullptr : q.dF; a.df = known || !d->has_f ? nullptr : q.df;
+  a.dtheta = known ? q.dtheta : nullptr;
+  a.st = (EpGradState*)(ws + l.state);
+  cudaGraphConditionalHandle handle;
+  int rc = while_handle(os, &handle);
+  if (rc) return rc;
+  if (counted(epgrad_launch_init<R>(a, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
+  rc = open_while(os, bs, handle);
+  if (rc) return rc;
+  rc = counted(epgrad_launch_stage<R>(a, bs));
+  const R* F = q.F;
+  if (rc == 0 && known) {
+    F = (const R*)(ws + l.Fk);
+    rc = dyn_impl<R>(true, d->dynamics_kind, q.p->dyn, B, T, a.stage_x, a.stage_u, nullptr, (R*)(ws + l.Fk),
+                     (R*)(ws + l.fk), bs);
+  }
+  if (rc == 0)
+    rc = adjoint_impl<R>(&l.da, q.p, q.C, q.c, F, a.stage_x, a.stage_u, a.dl_dx, a.dl_du, q.u_lower, q.u_upper, dxk,
+                         dCk, dck, dFk, dfk, ws + l.adj, l.adj_bytes, knob, bs, true);
+  if (rc == 0 && known)
+    rc = dyn_vjp_impl<R>(d->dynamics_kind, q.p->dyn, B, T, a.stage_x, a.stage_u, dFk, dfk, first, second, bs);
+  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, handle, bs));
+  cudaGraph_t body = nullptr;
+  if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+  return rc;
+}
+
+template <typename R>
+static int epgrad_impl(const EpGradCall<R>& q, void* stream) {
+  const int knob = kernel_knob();
+  int rc = epgrad_check<R>(q, knob);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t bs = ilqr_stream(2);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_record<R>(os, bs, q, knob);
   });
 }
 }  // namespace mpcb200
@@ -995,6 +1170,55 @@ int mpcb200_episode_f64(const mpcb200_dims* dims, const mpcb200_params* params, 
   return episode_impl<double>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I,
                                xs, us, costs, info, u_next, workspace, workspace_bytes},
                               stream);
+}
+
+int mpcb200_episode_plans_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                              int32_t n_steps, const float* C, const float* c, const float* F, const float* f,
+                              const float* x_init, const float* u_init, const float* u_lower, const float* u_upper,
+                              const uint8_t* u_zero_I, float* xs, float* us, float* costs, int32_t* info,
+                              float* u_next, float* plan_x, float* plan_u, void* workspace, size_t workspace_bytes,
+                              void* stream) {
+  if (plan_x == nullptr || plan_u == nullptr) return MPCB200_ERR_NULL_POINTER;
+  return episode_impl<float>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs,
+                              us, costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u},
+                             stream);
+}
+int mpcb200_episode_plans_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                              int32_t n_steps, const double* C, const double* c, const double* F, const double* f,
+                              const double* x_init, const double* u_init, const double* u_lower,
+                              const double* u_upper, const uint8_t* u_zero_I, double* xs, double* us, double* costs,
+                              int32_t* info, double* u_next, double* plan_x, double* plan_u, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  if (plan_x == nullptr || plan_u == nullptr) return MPCB200_ERR_NULL_POINTER;
+  return episode_impl<double>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I,
+                               xs, us, costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u},
+                              stream);
+}
+
+size_t mpcb200_episode_backward_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size) {
+  if (dims == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8)) return 0;
+  if (dims->dynamics_kind != DYN_LINEAR && (dyn_nparams(dims->dynamics_kind) == 0 || !known_shape_ok(dims))) return 0;
+  return epgrad_layout(dims, (size_t)elem_size, kernel_knob()).total;
+}
+int mpcb200_episode_backward_f32(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                 const float* C, const float* c, const float* F, const float* u_lower,
+                                 const float* u_upper, const float* xs, const float* us, const float* plan_x,
+                                 const float* plan_u, const float* dl_dxs, const float* dl_dus, float* dx_init,
+                                 float* dC, float* dc, float* dF, float* df, float* dtheta, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  return epgrad_impl<float>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,
+                             dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes},
+                            stream);
+}
+int mpcb200_episode_backward_f64(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                 const double* C, const double* c, const double* F, const double* u_lower,
+                                 const double* u_upper, const double* xs, const double* us, const double* plan_x,
+                                 const double* plan_u, const double* dl_dxs, const double* dl_dus, double* dx_init,
+                                 double* dC, double* dc, double* dF, double* df, double* dtheta, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  return epgrad_impl<double>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,
+                              dl_dus, dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes},
+                             stream);
 }
 
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }

@@ -1,0 +1,235 @@
+// episode_grad.cu - the kernels of an episode's reverse sweep (episode_grad.cuh) and their launchers, in a module of
+// their own: the init and accumulate kernels call the device runtime's cudaGraphSetConditional.
+#include "episode_grad.cuh"
+
+namespace mpcb200 {
+
+static unsigned epgrad_grid(size_t items) {   // grid-stride kernels: enough blocks to cover `items`, at most 4096
+  const size_t g = (items + 255) / 256;
+  return (unsigned)(g < 1 ? 1 : (g > 4096 ? 4096 : g));
+}
+static int launched() { return cudaGetLastError() == cudaSuccess ? MPCB200_OK : MPCB200_ERR_LAUNCH; }
+
+// plan_x[k] = best_x, plan_u[k] = best_u for the control step k = ep->step (before episode_advance_kernel moves it)
+template <typename R>
+__global__ void __launch_bounds__(256)
+episode_plans_kernel(size_t n_x, size_t n_u, const R* __restrict__ best_x, const R* __restrict__ best_u,
+                     R* __restrict__ plan_x, R* __restrict__ plan_u, const EpisodeState* __restrict__ ep) {
+  const size_t k = (size_t)ep->step;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = i0; i < n_x; i += step) plan_x[k * n_x + i] = best_x[i];
+  for (size_t i = i0; i < n_u; i += step) plan_u[k * n_u + i] = best_u[i];
+}
+
+template <typename R>
+__global__ void __launch_bounds__(256) fill_zero_kernel(size_t n, R* __restrict__ p) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    p[i] = R(0);
+}
+
+// g = dl_dxs[n_steps]; the accumulators and the adjoint's incoming gradients zeroed; k = n_steps - 1; the loop's
+// handle set to 1
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_init_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
+  for (size_t i = i0; i < B * N; i += step) a.g[i] = a.dl_dxs[(size_t)a.n_steps * B * N + i];
+  for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] = R(0);
+  for (size_t i = i0; i < T * B * P; i += step) a.dc[i] = R(0);
+  for (size_t i = i0; i < T * B * N; i += step) a.dl_dx[i] = R(0);
+  for (size_t i = i0; i < T * B * M; i += step) a.dl_du[i] = R(0);
+  if (a.kind == DYN_LINEAR) {
+    for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) a.dF[i] = R(0);
+    if (a.has_f)
+      for (size_t i = i0; i < (T - 1) * B * N; i += step) a.df[i] = R(0);
+  } else {
+    for (size_t i = i0; i < B * a.NP; i += step) a.dtheta[i] = R(0);
+  }
+  if (i0 == 0) {
+    a.st->k = a.n_steps - 1; a.st->tickets = 0u; a.st->reserved[0] = a.st->reserved[1] = 0;
+    cudaGraphSetConditional(handle, 1);
+  }
+}
+
+// the plan of step k into the fixed buffers the body's launchers read
+template <typename R>
+__device__ __forceinline__ void epgrad_stage_plan(const EpGradArgs<R>& a, size_t k, size_t i0, size_t step) {
+  const size_t nx = (size_t)a.T * a.B * a.N, nu = (size_t)a.T * a.B * a.M;
+  for (size_t i = i0; i < nx; i += step) a.stage_x[i] = a.plan_x[k * nx + i];
+  for (size_t i = i0; i < nu; i += step) a.stage_u[i] = a.plan_u[k * nu + i];
+}
+
+// LinDx: x' = F[0] z + f[0] with z = [x_k; u_k].  One thread per (b, column j of F[0]): column j of F[0]^T g goes
+// to gx (j < N) or into dl_du[0] (j >= N), and column j of dF[0] takes g z_j.
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_stage_linear_kernel(const EpGradArgs<R> a) {
+  const size_t k = (size_t)a.st->k;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  epgrad_stage_plan(a, k, i0, step);
+  const int N = a.N, M = a.M, P = N + M;
+  const size_t B = a.B;
+  for (size_t idx = i0; idx < B * P; idx += step) {
+    const size_t b = idx / P;
+    const int j = (int)(idx % P);
+    const R* g = a.g + b * N;
+    const R* Fb = a.F + b * N * P;
+    R* dFb = a.dF + b * N * P;
+    const R zj = j < N ? a.xs[(k * B + b) * N + j] : a.us[(k * B + b) * M + (j - N)];
+    R v = R(0);
+    for (int i = 0; i < N; ++i) {
+      const R gi = g[i];
+      v += Fb[(size_t)i * P + j] * gi;
+      dFb[(size_t)i * P + j] += gi * zj;
+    }
+    if (j < N) a.gx[b * N + j] = v;
+    else a.dl_du[b * M + (j - N)] = a.dl_dus[(k * B + b) * M + (j - N)] + v;
+    if (a.has_f && j == 0)
+      for (int i = 0; i < N; ++i) a.df[b * N + i] += g[i];
+  }
+}
+
+// A known system: R, S by the forward-mode duals dyn_linearize_kernel uses, and theta_step = sum_r g_r dx'_r/dtheta
+// by the nested duals of dyn_linearize_vjp_kernel (its `first`, with df = g).  One thread per problem.
+template <typename R, int KIND>
+__global__ void __launch_bounds__(256) epgrad_stage_known_kernel(const EpGradArgs<R> a) {
+  constexpr int N = DynDims<KIND>::N, M = DynDims<KIND>::M, P = N + M, NP = DynLearnable<KIND>::NP;
+  static_assert(M == 1, "the known systems have one control");
+  const size_t k = (size_t)a.st->k;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  epgrad_stage_plan(a, k, i0, step);
+  for (size_t b = i0; b < (size_t)a.B; b += step) {
+    R z[P], g[N];
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+      z[j] = a.xs[(k * a.B + b) * N + j];
+      g[j] = a.g[b * N + j];
+    }
+    z[N] = a.us[k * a.B + b];
+    {
+      using D = Dual<R, P>;
+      D s[N], o[N];
+#pragma unroll
+      for (int j = 0; j < N; ++j) s[j] = dual_var<R, P>(z[j], j);
+      const D u = dual_var<R, P>(z[N], N);
+      dyn_step<R, KIND, D>(a.dp, s, u, o);
+#pragma unroll
+      for (int j = 0; j < P; ++j) {
+        R v = R(0);
+#pragma unroll
+        for (int r = 0; r < N; ++r) v += o[r].d[j] * g[r];
+        if (j < N) a.gx[b * N + j] = v;
+        else a.dl_du[b] = a.dl_dus[k * a.B + b] + v;
+      }
+    }
+    using D2 = Dual<Dual<R, P>, 1>;
+#pragma unroll 1
+    for (int p = 0; p < NP; ++p) {
+      D2 s[N], o[N], u;
+#pragma unroll
+      for (int j = 0; j < N; ++j) {
+        s[j].v = dual_var<R, P>(z[j], j);
+        s[j].d[0] = dual_const<R, P>(R(0));
+      }
+      u.v = dual_var<R, P>(z[N], N);
+      u.d[0] = dual_const<R, P>(R(0));
+      dyn_step<R, KIND, D2, D2>(a.dp, s, u, o, p);
+      R first = R(0);
+#pragma unroll
+      for (int r = 0; r < N; ++r) first += g[r] * o[r].d[0].v;
+      a.theta_step[b * NP + p] = first;
+    }
+  }
+}
+
+// g = dl_dxs[k] + R^T g + dx_init_k; dC, dc (LinDx: dF, df) += the adjoint's; a known system: dtheta[b] +=
+// theta_step[b] + sum_t (first + second)[t, b] in t order.  The last block to finish counts k down and ends the
+// loop after k = 0: every block has read st->k by then.
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_accum_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
+  const int k = a.st->k;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
+  for (size_t i = i0; i < B * N; i += step) a.g[i] = a.dl_dxs[(size_t)k * B * N + i] + a.gx[i] + a.dx_k[i];
+  for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] += a.dC_k[i];
+  for (size_t i = i0; i < T * B * P; i += step) a.dc[i] += a.dc_k[i];
+  if (a.kind == DYN_LINEAR) {
+    for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) a.dF[i] += a.dF_k[i];
+    if (a.has_f)
+      for (size_t i = i0; i < (T - 1) * B * N; i += step) a.df[i] += a.df_k[i];
+  } else {
+    const size_t NP = a.NP;
+    for (size_t i = i0; i < B * NP; i += step) {
+      const size_t b = i / NP, p = i % NP;
+      R acc = a.dtheta[i] + a.theta_step[i];
+      for (size_t t = 0; t + 1 < T; ++t) acc += a.first[(t * B + b) * NP + p] + a.second[(t * B + b) * NP + p];
+      a.dtheta[i] = acc;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&a.st->tickets, 1u) == gridDim.x - 1) {
+      a.st->tickets = 0u;
+      a.st->k = k - 1;
+      if (k == 0) cudaGraphSetConditional(handle, 0);
+    }
+  }
+}
+
+template <typename R>
+int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
+                         const EpisodeState* ep, cudaStream_t stream) {
+  const size_t nx = (size_t)T * B * N, nu = (size_t)T * B * M;
+  episode_plans_kernel<R><<<epgrad_grid(nx > nu ? nx : nu), 256, 0, stream>>>(nx, nu, best_x, best_u, plan_x, plan_u,
+                                                                              ep);
+  return launched();
+}
+
+template <typename R>
+int launch_fill_zero(size_t n, R* p, cudaStream_t stream) {
+  fill_zero_kernel<R><<<epgrad_grid(n), 256, 0, stream>>>(n, p);
+  return launched();
+}
+
+// the largest grid-stride range of the init and accumulate kernels: dC
+template <typename R>
+static size_t epgrad_items(const EpGradArgs<R>& a) {
+  const size_t P = (size_t)a.N + a.M;
+  return (size_t)a.T * a.B * P * P;
+}
+
+template <typename R>
+int epgrad_launch_init(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  epgrad_init_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_stage(const EpGradArgs<R>& a, cudaStream_t stream) {
+  const size_t items = (size_t)a.T * a.B * (a.N > a.M ? a.N : a.M);
+  const unsigned grid = epgrad_grid(items);
+  if (a.kind == DYN_LINEAR) epgrad_stage_linear_kernel<R><<<grid, 256, 0, stream>>>(a);
+  else if (a.kind == DYN_CARTPOLE) epgrad_stage_known_kernel<R, DYN_CARTPOLE><<<grid, 256, 0, stream>>>(a);
+  else if (a.kind == DYN_PENDULUM) epgrad_stage_known_kernel<R, DYN_PENDULUM><<<grid, 256, 0, stream>>>(a);
+  else if (a.kind == DYN_PENDULUM_FULL) epgrad_stage_known_kernel<R, DYN_PENDULUM_FULL><<<grid, 256, 0, stream>>>(a);
+  else return MPCB200_ERR_BAD_DIMS;
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_accum(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  epgrad_accum_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+  return launched();
+}
+
+#define MPCB200_EPGRAD_INST(R)                                                                                     \
+  template int episode_launch_plans<R>(int, int, int, int, const R*, const R*, R*, R*, const EpisodeState*,        \
+                                       cudaStream_t);                                                              \
+  template int launch_fill_zero<R>(size_t, R*, cudaStream_t);                                                      \
+  template int epgrad_launch_init<R>(const EpGradArgs<R>&, cudaGraphConditionalHandle, cudaStream_t);              \
+  template int epgrad_launch_stage<R>(const EpGradArgs<R>&, cudaStream_t);                                         \
+  template int epgrad_launch_accum<R>(const EpGradArgs<R>&, cudaGraphConditionalHandle, cudaStream_t);
+MPCB200_EPGRAD_INST(float)
+MPCB200_EPGRAD_INST(double)
+
+}  // namespace mpcb200

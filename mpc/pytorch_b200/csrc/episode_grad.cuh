@@ -1,0 +1,57 @@
+// episode_grad.cuh - the reverse sweep of a receding-horizon episode (mpcb200_episode_backward_*): the closed loop's
+// chain rule over control steps k = n_steps-1 .. 0, as one CUDA graph with a conditional `while` node.
+//
+// Forward (mpcb200_episode_plans_*): episode_plans_kernel keeps each solve's best iterate, plan_x[k], plan_u[k].
+// Backward, with g = dL/dx_{k+1} carried in dx_init:
+//   a. epgrad_stage_*_kernel: plan_x[k], plan_u[k] into fixed buffers; the model step's VJP at (x_k, u_k):
+//      gx = R^T g, dl_du[0] = dl_dus[k] + S^T g (rows t > 0 stay 0), and the parameter part (LinDx: dF[0] += g z^T,
+//      df[0] += g; a known system: theta_step = g . dx'/dtheta with the Jacobian held constant, the VJP's `first`);
+//   b. a known system's linearisation along the staged plan, c. the KKT adjoint on the staged plan, d. a known
+//      system's linearisation VJP (first + second) - the library's own launchers, recorded on the body stream;
+//   e. epgrad_accum_kernel: g = dl_dxs[k] + gx + dx_init_k, and the adjoint's dC, dc (dF, df; theta) summed in.
+// Every buffer a body kernel reads is written by an earlier kernel of the same iteration or by epgrad_init_kernel,
+// so the body holds kernel nodes only.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "dynamics.cuh"
+#include "ilqr.cuh"
+
+namespace mpcb200 {
+
+struct EpGradState {      // device-resident sweep state, reset by epgrad_init_kernel
+  int32_t k;              // the control step the body works on
+  uint32_t tickets;       // blocks of the current epgrad_accum_kernel that have finished
+  int32_t reserved[2];
+};
+
+template <typename R>
+struct EpGradArgs {
+  int B, T, N, M, n_steps, F_T, has_f, kind, NP;
+  DynParams dp;
+  const R *xs, *us, *plan_x, *plan_u, *dl_dxs, *dl_dus;
+  const R* F;             // LinDx: slice 0 of the staged F, [B, N, N+M]
+  R *stage_x, *stage_u;   // [T, B, N], [T, B, M]: the plan of step k
+  R *dl_dx, *dl_du;       // the adjoint's incoming gradients [T, B, N] (0), [T, B, M] (row 0 written per step)
+  R *gx, *theta_step;     // R^T g [B, N]; the model step's parameter part [B, NP]
+  R* g;                   // dL/dx_{k+1}; dL/dx_init after the loop (the caller's dx_init)
+  const R *dx_k, *dC_k, *dc_k, *dF_k, *df_k, *first, *second;     // the adjoint's (and VJP's) outputs of step k
+  R *dC, *dc, *dF, *df, *dtheta;
+  EpGradState* st;
+};
+
+// Launchers (episode_grad.cu), instantiated for float and double; 0 or MPCB200_ERR_LAUNCH.
+template <typename R>
+int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
+                         const EpisodeState* ep, cudaStream_t stream);
+template <typename R>
+int epgrad_launch_init(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream);
+template <typename R>
+int epgrad_launch_stage(const EpGradArgs<R>& a, cudaStream_t stream);
+template <typename R>
+int epgrad_launch_accum(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream);
+template <typename R>
+int launch_fill_zero(size_t n, R* p, cudaStream_t stream);
+
+}  // namespace mpcb200

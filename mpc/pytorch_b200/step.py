@@ -411,14 +411,16 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
 
 def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
-                best_cost_eps=1e-4, dyn=None):
+                best_cost_eps=1e-4, dyn=None, keep_plans=False):
     """A receding-horizon episode of n_steps control steps in ONE library call (mpcb200_episode_*): each step solves
     the problem from the current state as ilqr_raw does (u_init = the warm start), applies the plan's first control,
     steps the model (LinDx: F[0] [x; u] + f[0]; a known system `dyn`: one step of it) and shifts the warm start
     (cat(u[1:], 0), then w[-2] = w[-3]).  The problem is staged once per episode by the _problem call ilqr_raw makes.
     u_init None: zeros.  Returns a dict of device tensors x [n_steps+1, B, n], u [n_steps, B, m], costs
     [n_steps, B], info int32 [n_steps, 2] and u_next [T, B, m]; None when the driver has no conditional graph nodes
-    or no conditional node inside another's body (nothing was launched then)."""
+    or no conditional node inside another's body (nothing was launched then).  keep_plans: the call is
+    mpcb200_episode_plans_*, and the dict also holds "saved", what episode_backward_raw takes: the staged problem and
+    the padded xs, us and each solve's best iterate plan_x [n_steps, T, B, N], plan_u [n_steps, T, B, M]."""
     n, m = n_state, n_ctrl
     if T < 3 or n_steps < 1:
         raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
@@ -439,16 +441,63 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
     info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
     u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
-    fn = _lib.entry("mpcb200_episode", dtype)
+    args = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), ptr_view(s.C),
+            ptr_view(s.c), ptr_view(s.F), ptr_view(s.f), ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper),
+            ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info), ptr(u_next)]
+    name = "mpcb200_episode"
+    if keep_plans:
+        name = "mpcb200_episode_plans"
+        plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
+        plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
+        args += [ptr(plan_x), ptr(plan_u)]
+    fn = _lib.entry(name, dtype)
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), ptr_view(s.C),
-                ptr_view(s.c), ptr_view(s.F), ptr_view(s.f), ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper),
-                ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info), ptr(u_next), ptr(ws), nbytes,
-                stream_handle(dev))
+        rc = fn(*args, ptr(ws), nbytes, stream_handle(dev))
     if rc == _lib.ERR_NO_GRAPH_COND:
         return None
-    check(rc, "mpcb200_episode")
-    return {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
+    check(rc, name)
+    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
+    if keep_plans:
+        res["saved"] = (s, n_steps, xs, us, plan_x, plan_u)
+    return res
+
+
+def episode_backward_raw(saved, dl_dxs, dl_dus):
+    """The reverse sweep of an episode run by episode_raw(..., keep_plans=True) in ONE library call
+    (mpcb200_episode_backward_*): `saved` is that call's res["saved"], dl_dxs [n_steps+1, B, n] and dl_dus
+    [n_steps, B, m] the gradients of its x and u.  Returns (dx_init [B, n], dC [T, B, p, p], dc [T, B, p], dF, df,
+    dtheta): LinDx dF like the staged F's [F_T, B, n, p] and df like its f (None without f), dtheta None; a known
+    system dF = df = None and dtheta [B, NP], one row per problem (the caller sums over b, as DynLinearize does)."""
+    s, n_steps, xs, us, plan_x, plan_u = saved
+    pad, dims = s.pad, s.dims
+    T, B, N, M = dims.T, dims.B, pad.N, pad.M
+    dtype, dev = xs.dtype, xs.device
+    gx_, gu_ = pad.vec_n(_dense(dl_dxs, dtype)), pad.vec_m(_dense(dl_dus, dtype))
+    kind = dims.dynamics_kind
+    P = N + M
+    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
+    dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
+    dc = torch.empty(T, B, P, dtype=dtype, device=dev)
+    dF = df = dtheta = None
+    if kind == DYN_LINEAR:
+        dF = torch.empty(s.F.shape[0], B, N, P, dtype=dtype, device=dev)
+        if dims.has_f:
+            df = torch.empty(T - 1, B, N, dtype=dtype, device=dev)
+    else:
+        from .dynamics import DYN_NPARAMS
+        dtheta = torch.empty(B, DYN_NPARAMS[kind], dtype=dtype, device=dev)
+    nbytes = _lib.lib().mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), xs.element_size())
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    fn = _lib.entry("mpcb200_episode_backward", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), ptr_view(s.C), ptr_view(s.c),
+                ptr_view(s.F), ptr(s.u_lower), ptr(s.u_upper), ptr(xs), ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_),
+                ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(dtheta), ptr(ws), nbytes,
+                stream_handle(dev))
+    check(rc, "mpcb200_episode_backward")
+    if df is not None and s.f.shape[0] == T:          # a full-length f: its last slice never enters the episode
+        df = torch.cat((df, torch.zeros_like(df[:1])), 0)
+    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)
 
 
 def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_df, f_T=None):

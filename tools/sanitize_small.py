@@ -49,4 +49,20 @@ for (B, n, dt) in [(2, 100, torch.float64), (3, 128, torch.float32)]:    # one t
     q = (2.0 * torch.randn(B, n, generator=g, dtype=torch.float64)).to(dt).to(dev)
     pnqp(H, q, -torch.rand(B, n, generator=g).to(dt).to(dev), torch.rand(B, n, generator=g).to(dt).to(dev))
     torch.cuda.synchronize()
+# differentiable receding-horizon episodes: mpcb200_episode_plans_* and mpcb200_episode_backward_*, LinDx and pendulum
+from mpc.pytorch_b200 import MPC
+from mpc.pytorch_b200.dynamics import PendulumDx
+from mpc.pytorch_b200.control import receding_horizon
+B, T, n, m = 3, 4, 3, 2
+C, c, F, f, x0 = [t.to(dev).requires_grad_(True) for t in gen_problem(3, B, T, n, m, torch.float32)]
+ep = receding_horizon(MPC(n, m, T, u_lower=-0.3, u_upper=0.3, lqr_iter=3, verbose=-1), x0, QuadCost(C, c),
+                      LinDx(F, f), 2, differentiable=True)
+(ep.x.sum() + ep.u.sum()).backward()
+pend = PendulumDx(params=torch.tensor((10.0, 1.0, 1.0), device=dev, requires_grad=True))
+q, p = pend.get_true_obj()
+x0 = torch.tensor([[1.0, 0.0, 0.1], [0.0, 1.0, -0.2]], device=dev, dtype=torch.float64, requires_grad=True)
+ep = receding_horizon(MPC(3, 1, T, u_lower=-2.0, u_upper=2.0, lqr_iter=3, verbose=-1), x0,
+                      QuadCost(torch.diag(q).double().to(dev), p.double().to(dev)), pend, 2, differentiable=True)
+(ep.x.sum() + ep.u.sum()).backward()
+torch.cuda.synchronize()
 print("sanitize workload done")
