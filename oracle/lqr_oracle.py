@@ -441,3 +441,135 @@ def mpc_forward_lin(n_state, n_ctrl, T, x_init, C, c, F, f, u_lower=None, u_uppe
         if float(out.full_du_norm.max()) < eps or n_not_improved > not_improved_lim:
             break
     return best["x"], best["u"], best["costs"], best["full_du_norm"]
+
+
+# ----------------------------------------------------------------------------
+# receding-horizon episodes (the notebooks' loop, examples/*.ipynb) and their reverse sweep
+# ----------------------------------------------------------------------------
+Episode = namedtuple("Episode", "x u costs iters plan_x plan_u u_next")
+
+
+def shift_warm_start(plan_u):
+    """The next solve's u_init: cat(plan_u[1:], 0), then w[-2] = w[-3] (the notebooks' rule)."""
+    w = torch.cat((plan_u[1:], torch.zeros_like(plan_u[:1])), 0)
+    w[-2] = w[-3]
+    return w
+
+
+def lindx_step(F, f, x, u):
+    """The LinDx plant of an episode: F[0] [x; u] + f[0] (no f: None or empty)."""
+    nx = _mv(F[0], torch.cat((x, u), 1))
+    return nx + f[0] if f is not None and f.nelement() > 0 else nx
+
+
+def receding_horizon_lin(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init=None, **kw):
+    """n_steps control steps of the notebooks' loop on mpc_forward_lin: solve from x_k with u_init = w_k, apply
+    u_k = plan_u[0], step the plant F[0] [x_k; u_k] + f[0], w_{k+1} = shift_warm_start(plan_u).  kw: mpc_forward_lin's
+    options (bounds, delta_u, u_zero_I, lqr_iter, eps, coupled, ...).  Returns an Episode: x [n_steps+1, B, n],
+    u [n_steps, B, m], costs [n_steps, B], iters [n_steps] (each solve's iterations), each solve's best iterate
+    plan_x [n_steps, T, B, n], plan_u [n_steps, T, B, m], and u_next = w_{n_steps}."""
+    B = C.shape[1]
+    w = torch.zeros(T, B, n_ctrl, dtype=C.dtype) if u_init is None else u_init
+    x = x_init
+    xs, us, costs, iters, plan_x, plan_u = [x_init], [], [], [], [], []
+    for _ in range(n_steps):
+        trace = []
+        bx, bu, bc, _ = mpc_forward_lin(n_state, n_ctrl, T, x, C, c, F, f, u_init=w, trace=trace, **kw)
+        x = lindx_step(F, f, x, bu[0])
+        w = shift_warm_start(bu)
+        xs.append(x)
+        us.append(bu[0])
+        costs.append(bc)
+        iters.append(len(trace))
+        plan_x.append(bx)
+        plan_u.append(bu)
+    return Episode(torch.stack(xs), torch.stack(us), torch.stack(costs), iters, torch.stack(plan_x),
+                   torch.stack(plan_u), w)
+
+
+def known_linearisation(step, theta, x, u, full=True):
+    """F = [R S] [T-1, B, n, n+m] and f = x' - R x - S u of x' = step(x_t, u_t, theta) at the detached points
+    (x[:-1], u[:-1]), by autograd; theta [B, NP] (one row per problem) requires grad.  full: F keeps its graph in
+    theta (create_graph, this project's convention, INTEGRATION.md section 2); False: F is a constant, as in the
+    reference's AUTO_DIFF linearisation (mpc/mpc.py:538-592), so f differentiates as x' alone."""
+    T, B, n = x.shape
+    m = u.shape[2]
+    rows = []
+    for t in range(T - 1):
+        xt, ut = x[t].detach().requires_grad_(True), u[t].detach().requires_grad_(True)
+        nx = step(xt, ut, theta)
+        J = [torch.cat(torch.autograd.grad(nx[:, r].sum(), (xt, ut), retain_graph=True,
+                                                 create_graph=full), 1) for r in range(n)]
+        J = torch.stack(J, 1)
+        if not full:
+            J = J.detach()
+        rows.append((J, nx - _mv(J, torch.cat((xt, ut), 1).detach())))
+    return torch.stack([r[0] for r in rows]), torch.stack([r[1] for r in rows])
+
+
+def receding_horizon_backward(n_state, n_ctrl, T, C, c, F, f, xs, us, plan_x, plan_u, dl_dxs, dl_dus,
+                              u_lower=None, u_upper=None, step=None, theta=None, full_linearisation=True,
+                              coupled=False):
+    """The reverse sweep of an episode from GIVEN plans plan_x [n_steps, T, B, n], plan_u [n_steps, T, B, m], states
+    xs [n_steps+1, B, n] and controls us [n_steps, B, m]: autograd's gradient of sum(dl_dxs * xs) + sum(dl_dus * us)
+    for the loop `for k: plan = ctrl'(x_k); x_{k+1} = step(x_k, plan_u[k][0])`, each solve contributing MPC.forward's
+    differentiable tail (lqr_step_backward at its plan with the step's bounds), the warm starts held constant.
+
+    g = dl_dxs[n]; for k = n-1 .. 0: the model step's VJP at (x_k, u_k) splits g into an x_k part and a u_k part (LinDx:
+    F[0]^T g, dF[0] += g z^T, df[0] += g); the solve's adjoint takes dl_du[0] = dl_dus[k] + (u_k part); then
+    g = dl_dxs[k] + (x_k part) + dx_init_k, and dC, dc (dF, df) accumulate.
+
+    LinDx: step None, F [T-1|T, B, n, n+m], f [T-1|T, B, n] or None / empty.  A known system: step(x, u, theta) its
+    one-step model (a CPU torch forward) with per-problem parameters theta [B, NP], F = f = None; each solve
+    linearises it along its plan (known_linearisation, `full_linearisation` as `full` there) and the model step
+    contributes only the direct derivative of x' in theta.  Returns a dict of dx_init, dC, dc, and dF, df (LinDx; df
+    None without f) or dtheta [B, NP] (one row per problem)."""
+    n, m = n_state, n_ctrl
+    n_steps = us.shape[0]
+    known = step is not None
+    dt = C.dtype
+    has_f = f is not None and f.nelement() > 0
+    if known:
+        theta = theta.detach().clone().requires_grad_(True)
+    dC, dc = torch.zeros_like(C), torch.zeros_like(c)
+    dF = None if known else torch.zeros_like(F)
+    df = torch.zeros_like(f) if has_f and not known else None
+    dtheta = torch.zeros_like(theta) if known else None
+    g = dl_dxs[n_steps].clone()
+    B = g.shape[0]
+    for k in range(n_steps - 1, -1, -1):
+        xk, uk = xs[k], us[k]
+        if known:
+            xl, ul = xk.detach().requires_grad_(True), uk.detach().requires_grad_(True)
+            gx, gu, gth = torch.autograd.grad((step(xl, ul, theta) * g).sum(), (xl, ul, theta))
+            dtheta += gth
+            Fk, fk = known_linearisation(step, theta, plan_x[k], plan_u[k], full_linearisation)
+        else:
+            z = torch.cat((xk, uk), 1)
+            gz = _mv(F[0].transpose(1, 2), g)
+            gx, gu = gz[:, :n], gz[:, n:]
+            dF[0] += g.unsqueeze(2) * z.unsqueeze(1)
+            if has_f:
+                df[0] += g
+            Fk, fk = F, f
+        dl_dx = torch.zeros(T, B, n, dtype=dt)
+        dl_du = torch.zeros(T, B, m, dtype=dt)
+        dl_du[0] = dl_dus[k] + gu
+        dxk, dCk, dck, dFk, dfk, _, _ = lqr_step_backward(
+            n, m, T, plan_x[k][0], C, c, Fk.detach(), fk.detach() if fk is not None else None, plan_x[k], plan_u[k],
+            dl_dx, dl_du, u_lower=u_lower, u_upper=u_upper, coupled=coupled)
+        dC += dCk
+        dc += dck
+        if known:
+            dtheta += torch.autograd.grad((Fk * dFk).sum() + (fk * dfk).sum(), theta)[0]
+        else:
+            dF += dFk
+            if has_f:
+                df[:T - 1] += dfk
+        g = dl_dxs[k] + gx + dxk
+    out = dict(dx_init=g, dC=dC, dc=dc)
+    if known:
+        out["dtheta"] = dtheta
+    else:
+        out.update(dF=dF, df=df)
+    return out

@@ -832,6 +832,271 @@ def switches(n, m, dtype):
     return out
 
 
+@functools.lru_cache(maxsize=None)
+def _pair_default(n, m, dtype):
+    """Whether the default dispatch runs the column-pair kernel at this instance (asked of the device)."""
+    return bool(probe_step(n, m, dtype, 2, None, False) & _L().PLAN_PAIR)
+
+
+def loop_plan(n, m, dtype, T, impl):
+    """The plan the loop body's step records at horizon T under MPCB200_KERNEL=impl; None where the step refuses.
+    The loop hands the step a Ks/ks workspace from the generic kernel's switch horizon on (mpcb200_ilqr_workspace
+    asks mpcb200_step_prefers_workspace); below it the gains must fit shared memory."""
+    L = _L()
+    if impl == 3 or (n, m) not in INSTANCES:
+        return L.PLAN_LARGE
+    sw = switches(n, m, dtype)
+    ws = sw["generic"] is not None and T >= sw["generic"]
+    if impl == 2 or (impl is None and _pair_default(n, m, dtype)):
+        if ws:
+            return plan(False, sw["pair"] is None or T < sw["pair"])
+        if sw["pair_nofit"] is None or T < sw["pair_nofit"]:
+            return plan(False, True)
+        if impl == 2:
+            return None                 # the pair kernel refuses: no workspace and the gains do not fit
+    return plan(True, not ws, ws and (n, m) in KREDUCE_SHAPES)
+
+
+def plan_name(p, impl, n, m, dtype):
+    """The loop's step plan p by name: refused, large, pair_smem, pair_ks, pair_fallback (the generic kernel with
+    gains in shared memory where the default dispatch would run the pair kernel), generic_smem, generic_kreduce,
+    generic_ks."""
+    L = _L()
+    if p is None:
+        return "refused"
+    if p == L.PLAN_LARGE:
+        return "large"
+    if p & L.PLAN_PAIR:
+        return "pair_smem" if p & L.PLAN_GAINS_SMEM else "pair_ks"
+    if p & L.PLAN_GAINS_SMEM:
+        return "pair_fallback" if impl is None and _pair_default(n, m, dtype) else "generic_smem"
+    return "generic_kreduce" if p & L.PLAN_KREDUCE else "generic_ks"
+
+
+SWITCH_PLANS = {"generic": ("generic_smem", "generic_ks"), "kreduce": ("generic_smem", "generic_kreduce"),
+                "pair": ("pair_smem", "pair_ks"), "fallback": ("pair_smem", "pair_fallback")}
+
+
+@functools.lru_cache(maxsize=None)
+def pick_switch(group, dtype):
+    """(n, m, T*, impls) of the instance whose `group` switch of the loop's step plan comes first, None if no
+    instance has it within ORACLE_TMAX.  Below T* the loop runs SWITCH_PLANS[group][0], from T* on [1]."""
+    cands = []
+    for n, m in INSTANCES:
+        sw = switches(n, m, dtype)
+        pair = (n, m) in PAIR_SHAPES
+        impls = (None, 1, 2) if pair else (None, 1)
+        Ts, impl = None, 1
+        if group == "generic" and (n, m) not in KREDUCE_SHAPES:
+            Ts = sw["generic"]
+        elif group == "kreduce" and (n, m) in KREDUCE_SHAPES:
+            Ts = sw["generic"]
+        elif group == "pair" and pair and sw["generic"] is not None and sw["pair"] is not None:
+            Ts, impl = max(sw["generic"], sw["pair"]), 2
+        elif group == "fallback" and pair and sw["pair_nofit"] is not None and _pair_default(n, m, dtype):
+            if sw["generic"] is None or sw["pair_nofit"] < sw["generic"]:
+                Ts, impl, impls = sw["pair_nofit"], None, (None, 1)
+        if Ts is None or Ts < 3 or Ts > ORACLE_TMAX:
+            continue
+        below, at = (plan_name(loop_plan(n, m, dtype, T, impl), impl, n, m, dtype) for T in (Ts - 1, Ts))
+        if (below, at) == SWITCH_PLANS[group]:
+            cands.append((Ts, n + m, n, m, impls))
+    if not cands:
+        return None
+    Ts, _, n, m, impls = min(cands)
+    return n, m, Ts, impls
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# receding-horizon episodes through the C ABI (mpcb200_episode_plans_*, mpcb200_episode_backward_*)
+# ------------------------------------------------------------------------------------------------------------------
+def _owned(poison, *shape, dtype):
+    """A caller-owned buffer: every byte 0xFF when `poison` (NaN in float32 and float64, -1 in int32), else empty."""
+    t = torch.empty(shape, dtype=dtype, device=DEV)
+    if poison:
+        t.view(torch.uint8).fill_(255)
+    return t
+
+
+def abi_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
+                delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5,
+                eps=1e-7, best_cost_eps=1e-4, dyn=None, poison=False):
+    """The call step.episode_raw(..., keep_plans=True) makes (mpcb200_episode_plans_*, the problem staged by the same
+    step._problem), with caller-owned outputs and workspace.  poison: every workspace byte and every output starts at
+    0xFF, so a kernel that reads an element nothing wrote reads NaN (or info -1).  Returns (res, launches, plan): res
+    as episode_raw's dict, "saved" included, launches the library kernels the call recorded, plan
+    mpcb200_last_step_plan() after it (the step plan of the solve)."""
+    from mpc.pytorch_b200 import step as S
+    L = _L()
+    B = x_init.shape[0]
+    dtype = C.dtype
+    s = S._problem(n, m, T, B, dtype, DEV, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+                   max_linesearch_iter, dyn)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    x0_, u0_ = pad.vec_n(S._dense(x_init, dtype)), pad.vec_m(S._dense(u_init, dtype))
+    opts = L.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
+                      best_cost_eps=float(best_cost_eps))
+    nbytes = L.lib().mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
+    ws = _owned(poison, nbytes, dtype=torch.uint8)
+    xs, us = _owned(poison, n_steps + 1, B, N, dtype=dtype), _owned(poison, n_steps, B, M, dtype=dtype)
+    costs, info = _owned(poison, n_steps, B, dtype=dtype), _owned(poison, n_steps, 2, dtype=torch.int32)
+    u_next = _owned(poison, T, B, M, dtype=dtype)
+    plan_x, plan_u = _owned(poison, n_steps, T, B, N, dtype=dtype), _owned(poison, n_steps, T, B, M, dtype=dtype)
+    before = L.launch_count()
+    with L._on_device(DEV):
+        rc = L.entry("mpcb200_episode_plans", dtype)(
+            ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), L.ptr_view(s.C),
+            L.ptr_view(s.c), L.ptr_view(s.F), L.ptr_view(s.f), L.ptr(x0_), L.ptr(u0_), L.ptr(s.u_lower),
+            L.ptr(s.u_upper), L.ptr(s.u_zero_I), L.ptr(xs), L.ptr(us), L.ptr(costs), L.ptr(info), L.ptr(u_next),
+            L.ptr(plan_x), L.ptr(plan_u), L.ptr(ws), nbytes, L.stream_handle(DEV))
+    L.check(rc, "mpcb200_episode_plans")
+    launches, p = L.launch_count() - before, L.last_step_plan()
+    torch.cuda.synchronize()
+    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next),
+           "saved": (s, n_steps, xs, us, plan_x, plan_u)}
+    return res, launches, p
+
+
+def abi_episode_backward(saved, dl_dxs, dl_dus, poison=False):
+    """The call step.episode_backward_raw makes (mpcb200_episode_backward_*), with caller-owned outputs and
+    workspace, poison as in abi_episode.  Returns ((dx_init, dC, dc, dF, df, dtheta) cropped as episode_backward_raw
+    crops them, launches, plan): plan is the nested step's, recorded in the sweep's body."""
+    from mpc.pytorch_b200 import step as S
+    from mpc.pytorch_b200.dynamics import DYN_LINEAR, DYN_NPARAMS
+    L = _L()
+    s, n_steps, xs, us, plan_x, plan_u = saved
+    pad, dims = s.pad, s.dims
+    T, B, N, M = dims.T, dims.B, pad.N, pad.M
+    dtype, P = xs.dtype, pad.N + pad.M
+    gx_, gu_ = pad.vec_n(S._dense(dl_dxs, dtype)), pad.vec_m(S._dense(dl_dus, dtype))
+    dx_init, dC, dc = (_owned(poison, B, N, dtype=dtype), _owned(poison, T, B, P, P, dtype=dtype),
+                       _owned(poison, T, B, P, dtype=dtype))
+    dF = df = dtheta = None
+    if dims.dynamics_kind == DYN_LINEAR:
+        dF = _owned(poison, s.F.shape[0], B, N, P, dtype=dtype)
+        df = _owned(poison, T - 1, B, N, dtype=dtype) if dims.has_f else None
+    else:
+        dtheta = _owned(poison, B, DYN_NPARAMS[dims.dynamics_kind], dtype=dtype)
+    nbytes = L.lib().mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), xs.element_size())
+    ws = _owned(poison, nbytes, dtype=torch.uint8)
+    before = L.launch_count()
+    with L._on_device(DEV):
+        rc = L.entry("mpcb200_episode_backward", dtype)(
+            ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), L.ptr_view(s.C), L.ptr_view(s.c),
+            L.ptr_view(s.F), L.ptr(s.u_lower), L.ptr(s.u_upper), L.ptr(xs), L.ptr(us), L.ptr(plan_x), L.ptr(plan_u),
+            L.ptr(gx_), L.ptr(gu_), L.ptr(dx_init), L.ptr(dC), L.ptr(dc), L.ptr(dF), L.ptr(df), L.ptr(dtheta),
+            L.ptr(ws), nbytes, L.stream_handle(DEV))
+    L.check(rc, "mpcb200_episode_backward")
+    launches, p = L.launch_count() - before, L.last_step_plan()
+    torch.cuda.synchronize()
+    if df is not None and s.f.shape[0] == T:
+        df = torch.cat((df, torch.zeros_like(df[:1])), 0)
+    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta), \
+        launches, p
+
+
+def episode_linear_inputs(seed, B, T, n, m, dtype, mode, F_T=None, f_T="T-1", time_invariant=()):
+    """A LinDx episode's inputs, float64 rounded through dtype, and the solver's problem options: (P, kw).
+    mode: plain | box (+-0.25) | tensor (tensor box) | boxT (tensor box + delta_u) | mask (u_zero_I).  F_T = T: F has
+    T slices; f_T: "none", "T-1" or "T" slices of f.  time_invariant: names among "F", "C", "c" whose slices all
+    equal slice 0; P holds them dense (what the oracle takes), and P["time_invariant"] names them, so that
+    episode_device_inputs hands them over as stride-0 views over time made on the device."""
+    C, c, F, f, x0 = gen_problem(seed, B, T, n, m, F64)
+    F = 0.9 * F
+    g = torch.Generator().manual_seed(seed + 1)
+    if F_T == T:
+        F = torch.cat((F, F[-1:]), 0)
+    if f_T == "T":
+        f = torch.cat((f, f[-1:]), 0)
+    elif f_T == "none":
+        f = None
+    P = dict(C=C, c=c, F=F, f=f, x0=x0)
+    for k in time_invariant:
+        P[k] = P[k][:1].expand(P[k].shape).contiguous()
+    kw = {}
+    if mode == "box":
+        kw = dict(u_lower=-0.25, u_upper=0.25)
+    elif mode in ("tensor", "boxT"):
+        kw = dict(u_lower=-0.5 * torch.rand(T, B, m, generator=g, dtype=F64) - 0.05,
+                  u_upper=0.5 * torch.rand(T, B, m, generator=g, dtype=F64) + 0.05)
+        if mode == "boxT":
+            kw["delta_u"] = 0.125
+    elif mode == "mask":
+        kw["u_zero_I"] = torch.rand(T, B, m, generator=g) < 0.3
+    P = {k: round_through(v, dtype) for k, v in P.items()}
+    P["time_invariant"] = tuple(time_invariant)
+    kw = {k: round_through(v, dtype) for k, v in kw.items()}
+    return P, kw
+
+
+def episode_device_inputs(P, dtype):
+    """x0, C, c, F, f of an episode_linear_inputs problem on DEV in dtype.  A time-invariant input is slice 0 moved
+    to the device and expanded there (a copy of an expanded tensor, .to() included, is dense), so the shim stages it
+    with time stride 0 (MPCB200_TIME_INVARIANT)."""
+    out = []
+    for k in ("x0", "C", "c", "F", "f"):
+        t = P[k]
+        if t is not None and k in P.get("time_invariant", ()):
+            t = to_dev(t[:1], dtype).expand(t.shape)
+        else:
+            t = to_dev(t, dtype)
+        out.append(t)
+    return out
+
+
+def epgrad_launches(route, known):
+    """Library kernels an mpcb200_episode_backward_* call records (api.cu epgrad_record): the init, stage and
+    accumulate kernels; a known system's linearisation and its VJP; the adjoint: prep + fused column-pair kernel, or
+    prep, fill_zero, masked step and the two gradient kernels on every three-launch route."""
+    return 3 + (2 if known else 0) + (2 if route == "fused" else 5)
+
+
+def episode_known_module(name):
+    """(module, clamp) of the episodes' known systems: cartpole (params (9.81, 1.3, 0.25, 0.8), force_mag 6),
+    pendulum ((10, 1, 1)) and the five-parameter pendulum ((10, 1, 1, 0.1, 0.05)), max_torque 2; float64 params, as
+    oracle/make_golden_receding_grad.py builds the reference's."""
+    from mpc.pytorch_b200.dynamics import CartpoleDx, PendulumDx
+    if name == "cartpole":
+        mod = CartpoleDx(params=torch.tensor((9.81, 1.3, 0.25, 0.8), dtype=F64))
+        mod.force_mag = 6.0
+    elif name == "pendulum":
+        mod = PendulumDx(params=torch.tensor((10.0, 1.0, 1.0), dtype=F64))
+    else:
+        mod = PendulumDx(params=torch.tensor((10.0, 1.0, 1.0, 0.1, 0.05), dtype=F64), simple=False)
+    clamp = mod.force_mag if name == "cartpole" else mod.max_torque
+    return mod, float(clamp)
+
+
+def episode_known_step(mod):
+    """The oracle's step(x, u, theta): the module's CPU torch forward with per-problem parameters theta [B, NP]."""
+    def step(x, u, theta):
+        mod.params = theta.t()
+        return mod(x, u)
+    return step
+
+
+def episode_known_inputs(name, B, T, dtype, seed):
+    """A known system's episode: (module, n, m, P, bounds at the clamp, dyn = (kind, params), theta [NP]).  The
+    module's own cost; states with the angle pair on the unit circle."""
+    from mpc.pytorch_b200.dynamics import DYN_NPARAMS
+    mod, clamp = episode_known_module(name)
+    n, m = mod.n_state, mod.n_ctrl
+    q, p = mod.get_true_obj()
+    g = torch.Generator().manual_seed(seed)
+    th = (torch.rand(B, generator=g, dtype=F64) * 2 - 1) * (3.0 if name == "cartpole" else 1.0)
+    if name == "cartpole":
+        x0 = torch.stack((torch.rand(B, generator=g, dtype=F64) - 0.5, torch.rand(B, generator=g, dtype=F64) - 0.5,
+                          th.cos(), th.sin(), torch.rand(B, generator=g, dtype=F64) - 0.5), 1)
+    else:
+        x0 = torch.stack((th.cos(), th.sin(), torch.rand(B, generator=g, dtype=F64) - 0.5), 1)
+    P = dict(C=torch.diag(q.double()).expand(T, B, n + m, n + m).contiguous(),
+             c=p.double().expand(T, B, n + m).contiguous(), x0=x0, F=None, f=None)
+    P = {k: round_through(v, dtype) for k, v in P.items()}
+    dyn = (mod.mpcb200_kind, mod.mpcb200_params())
+    theta = torch.tensor(dyn[1][:DYN_NPARAMS[mod.mpcb200_kind]], dtype=F64)
+    return mod, n, m, P, dict(u_lower=-clamp, u_upper=clamp), dyn, theta
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # MPC.forward on the device loop or on the host loop
 # ------------------------------------------------------------------------------------------------------------------

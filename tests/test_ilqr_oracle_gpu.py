@@ -29,9 +29,9 @@ import pytest
 import torch
 
 from oracle import lqr_oracle as orc
-from tests.gpu_harness import (DEV, DT, F32, F64, INSTANCES, KREDUCE_SHAPES, ORACLE_TMAX, PAIR_SHAPES,
-                               plan as _plan, plan_str as _plan_str, probe_step, round_through, run_loop,
-                               same_on_both_loops, switches, within)
+from tests.gpu_harness import (DEV, DT, F32, F64, ORACLE_TMAX, SWITCH_PLANS, loop_plan, pick_switch, plan as _plan,
+                               plan_name as _plan_name, plan_str as _plan_str, round_through, run_loop,
+                               same_on_both_loops, within)
 from tests.helpers import gen_problem, maxdiff
 
 pytestmark = pytest.mark.gpu
@@ -184,78 +184,6 @@ def check_loop(tag, r, case, dtype):
 # ------------------------------------------------------------------------------------------------------------------
 # (a) every step plan the loop body can record, on both sides of its switch horizon
 # ------------------------------------------------------------------------------------------------------------------
-@functools.lru_cache(maxsize=None)
-def _pair_default(n, m, dtype):
-    """Whether the default dispatch runs the column-pair kernel at this instance (asked of the device)."""
-    return bool(probe_step(n, m, dtype, 2, None, False) & _L().PLAN_PAIR)
-
-
-def loop_plan(n, m, dtype, T, impl):
-    """The plan the loop body's step records at horizon T under MPCB200_KERNEL=impl; None where the step refuses.
-    The loop hands the step a Ks/ks workspace from the generic kernel's switch horizon on (mpcb200_ilqr_workspace
-    asks mpcb200_step_prefers_workspace); below it the gains must fit shared memory."""
-    L = _L()
-    if impl == 3 or (n, m) not in INSTANCES:
-        return L.PLAN_LARGE
-    sw = switches(n, m, dtype)
-    ws = sw["generic"] is not None and T >= sw["generic"]
-    if impl == 2 or (impl is None and _pair_default(n, m, dtype)):
-        if ws:
-            return _plan(False, sw["pair"] is None or T < sw["pair"])
-        if sw["pair_nofit"] is None or T < sw["pair_nofit"]:
-            return _plan(False, True)
-        if impl == 2:
-            return None                 # the pair kernel refuses: no workspace and the gains do not fit
-    return _plan(True, not ws, ws and (n, m) in KREDUCE_SHAPES)
-
-
-def _plan_name(plan, impl, n, m, dtype):
-    L = _L()
-    if plan is None:
-        return "refused"
-    if plan == L.PLAN_LARGE:
-        return "large"
-    if plan & L.PLAN_PAIR:
-        return "pair_smem" if plan & L.PLAN_GAINS_SMEM else "pair_ks"
-    if plan & L.PLAN_GAINS_SMEM:
-        return "pair_fallback" if impl is None and _pair_default(n, m, dtype) else "generic_smem"
-    return "generic_kreduce" if plan & L.PLAN_KREDUCE else "generic_ks"
-
-
-SWITCH_PLANS = {"generic": ("generic_smem", "generic_ks"), "kreduce": ("generic_smem", "generic_kreduce"),
-                "pair": ("pair_smem", "pair_ks"), "fallback": ("pair_smem", "pair_fallback")}
-
-
-@functools.lru_cache(maxsize=None)
-def pick_switch(group, dtype):
-    """(n, m, T*, impls) of the instance whose `group` switch of the loop's step plan comes first, None if no
-    instance has it within ORACLE_TMAX.  Below T* the loop runs SWITCH_PLANS[group][0], from T* on [1]."""
-    cands = []
-    for n, m in INSTANCES:
-        sw = switches(n, m, dtype)
-        pair = (n, m) in PAIR_SHAPES
-        impls = (None, 1, 2) if pair else (None, 1)
-        Ts, impl = None, 1
-        if group == "generic" and (n, m) not in KREDUCE_SHAPES:
-            Ts = sw["generic"]
-        elif group == "kreduce" and (n, m) in KREDUCE_SHAPES:
-            Ts = sw["generic"]
-        elif group == "pair" and pair and sw["generic"] is not None and sw["pair"] is not None:
-            Ts, impl = max(sw["generic"], sw["pair"]), 2
-        elif group == "fallback" and pair and sw["pair_nofit"] is not None and _pair_default(n, m, dtype):
-            if sw["generic"] is None or sw["pair_nofit"] < sw["generic"]:
-                Ts, impl, impls = sw["pair_nofit"], None, (None, 1)
-        if Ts is None or Ts < 3 or Ts > ORACLE_TMAX:
-            continue
-        below, at = (_plan_name(loop_plan(n, m, dtype, T, impl), impl, n, m, dtype) for T in (Ts - 1, Ts))
-        if (below, at) == SWITCH_PLANS[group]:
-            cands.append((Ts, n + m, n, m, impls))
-    if not cands:
-        return None
-    Ts, _, n, m, impls = min(cands)
-    return n, m, Ts, impls
-
-
 MODES = ("plain", "box", "boxT")
 GROUPS = list(SWITCH_PLANS)
 
