@@ -389,7 +389,8 @@ int mpcb200_episode_plans_f64(const mpcb200_dims* dims, const mpcb200_params* pa
                               double* plan_x, double* plan_u, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
- * The reverse sweep of an episode of mpcb200_episode_plans_* (no slew-rate penalty): given dl_dxs[n_steps+1,B,n]
+ * The reverse sweep of an episode of mpcb200_episode_plans_* (a slew-rate episode: mpcb200_episode_backward_slew_*,
+ * below): given dl_dxs[n_steps+1,B,n]
  * and dl_dus[n_steps,B,m], the gradient of L(xs, us) for the closed loop
  *   plan_k = the solve from x_k (its KKT adjoint at the best iterate, as mpcb200_lqr_adjoint_* with u_lower/u_upper;
  *            a known system's F, f its linearisation along the plan, differentiable in theta),
@@ -421,6 +422,40 @@ int mpcb200_episode_backward_f64(const mpcb200_dims* dims, const mpcb200_params*
                                  const double* dl_dxs, const double* dl_dus,
                                  double* dx_init, double* dC, double* dc, double* dF, double* df, double* dtheta,
                                  void* workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The reverse sweep of a slew-rate episode: mpcb200_episode_backward_* on the augmented problem over
+ * [u_{k-1}; x_k] that mpcb200_episode_plans_* staged and ran (C~ = slew_C + C, c~ = [0; c], LinDx F~ = [[0, 0, I],
+ * [0, F]], f~ = [0; f]; a known system's passthrough kind), with the previous control held constant, as the
+ * reference detaches prev_ctrl: the first n_prev entries of every augmented state get no gradient, so
+ * dl_dxs[k][:, :n_prev] is ignored, dx_init[:, :n_prev] is returned 0, and the model step's passthrough row carries
+ * nothing back.  Every argument after n_prev is that of mpcb200_episode_backward_*, in the augmented (padded) sizes;
+ * the caller crops the gradients (dC[.., n_prev:, n_prev:], dc[.., n_prev:], dF[.., n_prev:, n_prev:],
+ * df[.., n_prev:], dx_init[:, n_prev:]).  A known system's dtheta is its linearisation VJP applied to the
+ * [n_prev:, n_prev:] block of each adjoint's dF~ and to df~[n_prev:], plus the model step's direct part.
+ * n_prev: the system's n_ctrl, explicit because zero padding can make dims->m larger and an augmented LinDx
+ * problem looks like a plain one; 1 <= n_prev <= dims->m and n_prev < dims->n, else MPCB200_ERR_BAD_DIMS.  A known
+ * system: dims->dynamics_kind is its passthrough kind (17, 18, 20) at the dynamics-only shape (n_state + 1, 1) and
+ * n_prev = 1; kinds 1, 2 and 4 take mpcb200_episode_backward_* instead (MPCB200_ERR_BAD_DIMS here).  Errors, capture
+ * contract, launch counting and MPCB200_ERR_NO_GRAPH_COND as for mpcb200_episode_backward_*; every argument error
+ * is reported before anything is captured.  workspace: mpcb200_episode_backward_slew_workspace_bytes() bytes (0 for
+ * arguments it does not take), 256-byte aligned.
+ */
+size_t mpcb200_episode_backward_slew_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev, int32_t elem_size);
+int mpcb200_episode_backward_slew_f32(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                      int32_t n_prev, const float* C, const float* c, const float* F,
+                                      const float* u_lower, const float* u_upper,
+                                      const float* xs, const float* us, const float* plan_x, const float* plan_u,
+                                      const float* dl_dxs, const float* dl_dus,
+                                      float* dx_init, float* dC, float* dc, float* dF, float* df, float* dtheta,
+                                      void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                      int32_t n_prev, const double* C, const double* c, const double* F,
+                                      const double* u_lower, const double* u_upper,
+                                      const double* xs, const double* us, const double* plan_x, const double* plan_u,
+                                      const double* dl_dxs, const double* dl_dus,
+                                      double* dx_init, double* dC, double* dc, double* dF, double* df, double* dtheta,
+                                      void* workspace, size_t workspace_bytes, void* stream);
 
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);

@@ -54,6 +54,8 @@ EXPORTED_SYMBOLS = (
     "mpcb200_ilqr_workspace_bytes", "mpcb200_episode_f32", "mpcb200_episode_f64", "mpcb200_episode_workspace_bytes",
     "mpcb200_episode_plans_f32", "mpcb200_episode_plans_f64", "mpcb200_episode_backward_f32",
     "mpcb200_episode_backward_f64", "mpcb200_episode_backward_workspace_bytes",
+    "mpcb200_episode_backward_slew_f32", "mpcb200_episode_backward_slew_f64",
+    "mpcb200_episode_backward_slew_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -135,6 +137,13 @@ def lib():
         fn.restype = ctypes.c_int
     L.mpcb200_episode_backward_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32]
     L.mpcb200_episode_backward_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_episode_backward_slew_f32", "mpcb200_episode_backward_slew_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.c_int32, ctypes.c_int32] + [vp] * 18 + \
+            [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_episode_backward_slew_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32, ctypes.c_int32]
+    L.mpcb200_episode_backward_slew_workspace_bytes.restype = ctypes.c_size_t
     L.mpcb200_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_supported.restype = ctypes.c_int
     L.mpcb200_supported_list.argtypes = [ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]

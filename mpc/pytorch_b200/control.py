@@ -10,8 +10,8 @@ wherever both apply.
 
 With ``differentiable=True`` the episode's x and u carry gradients.  On the device path the forward also keeps each
 solve's best iterate (``step.episode_raw(..., keep_plans=True)``) and the backward is one more library call
-(``step.episode_backward_raw``), the closed loop's reverse sweep as one CUDA graph; the host path runs the same loop
-with autograd recording.
+(``step.episode_backward_raw``), the closed loop's reverse sweep as one CUDA graph, with or without a slew-rate
+penalty; the host path runs the same loop with autograd recording.
 """
 import copy
 from collections import namedtuple
@@ -61,8 +61,10 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False):
     ``u_upper`` as ``LQRStepFn.backward`` takes them; a known system's linearisation differentiated in its
     parameters, ``DynLinearize``), the model step its exact vector-Jacobian product in x_k, u_k and the parameters
     (``LinDx``: F[0], f[0]), and the warm starts w_k and ``prev_ctrl`` are held constant, as in the reference.
-    Where the episode runs as one graph and has no slew-rate penalty, the backward is one more graph
-    (``step.episode_backward_raw``); otherwise the host path's loop runs with autograd recording."""
+    Where the episode runs as one graph, with or without a slew-rate penalty, the backward is one more graph
+    (``step.episode_backward_raw``); otherwise the host path's loop runs with autograd recording.  Under a slew-rate
+    penalty each solve runs on the augmented state [u_{k-1}; x_k], and u_{k-1} is held constant there as the
+    reference holds ``prev_ctrl``: no gradient flows through the previous control into the solve."""
     T, n, m = ctrl.T, ctrl.n_state, ctrl.n_ctrl
     if T < 3:
         raise MpcB200Error(f"a receding-horizon episode needs a horizon T >= 3 (the warm-start shift), got T={T}")
@@ -74,7 +76,7 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False):
     from .dynamics import params_scope
     if differentiable and torch.is_grad_enabled() and _requires_grad(x_init, cost, dx):
         with params_scope():
-            if ctrl.slew_rate_penalty is None and _takes_device_path(ctrl, x_init, cost, dx, w0):
+            if _takes_device_path(ctrl, x_init, cost, dx, w0):
                 ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0)
                 if ep is not None:
                     return ep
@@ -147,7 +149,11 @@ class EpisodeFn(torch.autograd.Function):
     """(x, u, costs, info, u_next) of a differentiable device episode: the forward is step.episode_raw with
     keep_plans, the backward one step.episode_backward_raw call.  One module-level Function (DESIGN.md section 3.2).
     `o` = (ctrl, dx, n_steps, w0); the known system's parameter values are the host numbers the forward took
-    (params_scope) and the backward reuses them.  Every tensor the backward reads (xs, us, the plans, the staged C, c,
+    (params_scope) and the backward reuses them.  Under a slew-rate penalty the staged problem is the augmented one
+    over [u_{k-1}; x] (MPC._device_problem): x is returned without its first m states, the backward pads dl_dx with
+    m zeros in front, the sweep detaches those states (n_prev = m), and the gradients are cropped to the blocks of
+    x_init, C, c, F and f inside the augmented ones (prev_ctrl and the warm starts get none).  Every tensor the
+    backward reads (xs, us, the plans, the staged C, c,
     F, f and bounds) goes through save_for_backward, so an in-place edit of x or u before the backward raises, and the
     outputs do not keep themselves alive through ctx; ctx holds only the staged problem's metadata.  First order only:
     the backward is raw kernels."""
@@ -158,8 +164,9 @@ class EpisodeFn(torch.autograd.Function):
         ctrl, dx, n_steps, w0 = o
         T, m = ctrl.T, ctrl.n_ctrl
         n, x0, C_, c_, F_, f_, dyn = ctrl._device_problem(x_init, QuadCost(C, c), dx)
+        slew = ctrl.slew_rate_penalty is not None
         res = _step.episode_raw(n, m, T, n_steps, x0, C_, c_, F_, f_, w0, dyn=dyn, keep_plans=True,
-                                **ctrl._device_options())
+                                n_prev=m if slew else 0, **ctrl._device_options())
         if res is None:
             raise _NoGraph()
         ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
@@ -168,7 +175,8 @@ class EpisodeFn(torch.autograd.Function):
         ctx.problem = s._replace(C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None)
         ctx.p_meta = (params.dtype, params.device) if params is not None else None
         ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
-        return res["x"], res["u"], res["costs"], res["info"], res["u_next"]
+        x = res["x"][:, :, m:] if slew else res["x"]
+        return x, res["u"], res["costs"], res["info"], res["u_next"]
 
     @staticmethod
     @once_differentiable
@@ -176,13 +184,19 @@ class EpisodeFn(torch.autograd.Function):
         from . import step as _step
         xs, us, plan_x, plan_u, C, c, F, f, lo, hi = ctx.saved_tensors
         s = ctx.problem._replace(C=C, c=c, F=F, f=f, u_lower=lo, u_upper=hi)
-        n_steps = ctx.n_steps
+        n_steps, k = ctx.n_steps, s.n_prev
         if dl_dx is None:
             dl_dx = xs.new_zeros(n_steps + 1, s.dims.B, s.pad.n)
+        elif k:                                   # the previous control's states: no gradient of their own
+            dl_dx = torch.cat((dl_dx.new_zeros(n_steps + 1, s.dims.B, k), dl_dx), 2)
         if dl_du is None:
             dl_du = us.new_zeros(n_steps, s.dims.B, s.pad.m)
         dx_init, dC, dc, dF, df, dtheta = _step.episode_backward_raw((s, n_steps, xs, us, plan_x, plan_u), dl_dx,
                                                                      dl_du)
+        if k:                                     # the blocks of x_init, C, c, F, f inside the augmented problem
+            dx_init, dC, dc = dx_init[:, k:], dC[..., k:, k:], dc[..., k:]
+            dF = dF[..., k:, k:] if dF is not None else None
+            df = df[..., k:] if df is not None else None
         need = ctx.needs_input_grad
         dparams = None
         if dtheta is not None and need[6]:

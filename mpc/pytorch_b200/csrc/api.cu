@@ -872,6 +872,8 @@ static int dyn_nparams(int kind) {
          : kind == DYN_PENDULUM ? DynLearnable<DYN_PENDULUM>::NP
          : kind == DYN_PENDULUM_FULL ? DynLearnable<DYN_PENDULUM_FULL>::NP : 0;
 }
+// a sweep's parameter count: the system's, for its passthrough kind too
+static int epgrad_nparams(int kind) { return dyn_nparams(kind & ~DYN_CTRL_PASSTHROUGH); }
 // dims of each step's adjoint: the episode's; a known system's F, f are its dense linearisation [T-1, B, ...]
 static mpcb200_dims epgrad_adjoint_dims(const mpcb200_dims* d) {
   mpcb200_dims da = *d;
@@ -891,7 +893,7 @@ static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob) {
   EpGradLayout l;
   l.da = epgrad_adjoint_dims(d);
   const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m, TB = T * B, T1B = (T - 1) * B;
-  const size_t NP = dyn_nparams(d->dynamics_kind);
+  const size_t NP = epgrad_nparams(d->dynamics_kind);
   const bool known = d->dynamics_kind != DYN_LINEAR;
   size_t o = 0;
   l.adj_bytes = adj_layout(&l.da, sz, knob).total;
@@ -919,7 +921,7 @@ static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob) {
   return l;
 }
 
-// the arguments of mpcb200_episode_backward_*, in the header's order
+// the arguments of mpcb200_episode_backward_*, in the header's order; mpcb200_episode_backward_slew_* adds n_prev
 template <typename R>
 struct EpGradCall {
   const mpcb200_dims* d;
@@ -929,7 +931,19 @@ struct EpGradCall {
   R *dx_init, *dC, *dc, *dF, *df, *dtheta;
   void* workspace;
   size_t workspace_bytes;
+  bool slew = false;          // the slew entry: the augmented problem, with the first n_prev states detached
+  int n_prev = 0;
 };
+
+// the slew entry's own dims checks: 1 <= n_prev <= m and n_prev < n; a known system is its passthrough kind at its
+// dynamics-only shape, with n_prev its n_ctrl (the systems themselves belong to mpcb200_episode_backward_*)
+static bool slew_dims_ok(const mpcb200_dims* d, int n_prev) {
+  if (n_prev < 1 || n_prev > d->m || n_prev >= d->n) return false;
+  if (d->dynamics_kind == DYN_LINEAR) return true;
+  int n = 0, m = 0;
+  return (d->dynamics_kind & DYN_CTRL_PASSTHROUGH) != 0 && epgrad_nparams(d->dynamics_kind) != 0 &&
+         known_shape_ok(d) && dyn_kind_dims(d->dynamics_kind & ~DYN_CTRL_PASSTHROUGH, n, m) && n_prev == m;
+}
 
 // argument checks that need no device: every error is reported before anything is captured or launched
 template <typename R>
@@ -942,11 +956,12 @@ static int epgrad_check(const EpGradCall<R>& q, int knob) {
       q.dx_init == nullptr || q.dC == nullptr || q.dc == nullptr || q.workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (d->T < 3 || q.n_steps < 1) return MPCB200_ERR_BAD_DIMS;
+  if (q.slew && !slew_dims_ok(d, q.n_prev)) return MPCB200_ERR_BAD_DIMS;
   rc = check_bounds(d, q.u_lower, q.u_upper);
   if (rc) return rc;
   if (d->dynamics_kind != DYN_LINEAR) {
-    // a known system itself: a slew-rate (passthrough) episode has no device backward
-    if (dyn_nparams(d->dynamics_kind) == 0 || !known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
+    // mpcb200_episode_backward_* takes a known system itself, the slew entry its passthrough kind (slew_dims_ok)
+    if (!q.slew && (dyn_nparams(d->dynamics_kind) == 0 || !known_shape_ok(d))) return MPCB200_ERR_BAD_DIMS;
     if (q.dtheta == nullptr) return MPCB200_ERR_NULL_POINTER;
   } else {
     if (q.F == nullptr || q.dF == nullptr) return MPCB200_ERR_NULL_POINTER;
@@ -970,7 +985,7 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   EpGradArgs<R> a;
   std::memset(&a, 0, sizeof(a));
   a.B = B; a.T = T; a.N = d->n; a.M = d->m; a.n_steps = q.n_steps; a.F_T = l.da.F_T; a.has_f = l.da.has_f;
-  a.kind = d->dynamics_kind; a.NP = dyn_nparams(d->dynamics_kind);
+  a.kind = d->dynamics_kind; a.NP = epgrad_nparams(d->dynamics_kind);
   for (int i = 0; i < 8; ++i) a.dp.p[i] = q.p->dyn[i];
   a.xs = q.xs; a.us = q.us; a.plan_x = q.plan_x; a.plan_u = q.plan_u; a.dl_dxs = q.dl_dxs; a.dl_dus = q.dl_dus;
   a.F = known ? nullptr : q.F;
@@ -993,7 +1008,7 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   cudaGraphConditionalHandle handle;
   int rc = while_handle(os, &handle);
   if (rc) return rc;
-  if (counted(epgrad_launch_init<R>(a, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
+  if (counted(epgrad_launch_init<R>(a, q.n_prev, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
   rc = open_while(os, bs, handle);
   if (rc) return rc;
   rc = counted(epgrad_launch_stage<R>(a, bs));
@@ -1006,9 +1021,16 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   if (rc == 0)
     rc = adjoint_impl<R>(&l.da, q.p, q.C, q.c, F, a.stage_x, a.stage_u, a.dl_dx, a.dl_du, q.u_lower, q.u_upper, dxk,
                          dCk, dck, dFk, dfk, ws + l.adj, l.adj_bytes, knob, bs, true);
-  if (rc == 0 && known)
+  if (rc == 0 && known && !q.slew) {
     rc = dyn_vjp_impl<R>(d->dynamics_kind, q.p->dyn, B, T, a.stage_x, a.stage_u, dFk, dfk, first, second, bs);
-  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, handle, bs));
+  } else if (rc == 0 && known) {
+    DynVjpArgs v;
+    std::memset(&v, 0, sizeof(v));
+    v.B = B; v.T = T; v.kind = d->dynamics_kind; v.dp = a.dp;
+    v.x = a.stage_x; v.u = a.stage_u; v.dF = dFk; v.df = dfk; v.first = first; v.second = second;
+    rc = counted(epgrad_launch_vjp_passthrough<R>(v, bs));
+  }
+  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, q.n_prev, handle, bs));
   cudaGraph_t body = nullptr;
   if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
   return rc;
@@ -1218,6 +1240,33 @@ int mpcb200_episode_backward_f64(const mpcb200_dims* dims, const mpcb200_params*
                                  size_t workspace_bytes, void* stream) {
   return epgrad_impl<double>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,
                               dl_dus, dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes},
+                             stream);
+}
+
+size_t mpcb200_episode_backward_slew_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev, int32_t elem_size) {
+  if (dims == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8)) return 0;
+  if (!slew_dims_ok(dims, n_prev)) return 0;
+  return epgrad_layout(dims, (size_t)elem_size, kernel_knob()).total;
+}
+int mpcb200_episode_backward_slew_f32(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                      int32_t n_prev, const float* C, const float* c, const float* F,
+                                      const float* u_lower, const float* u_upper, const float* xs, const float* us,
+                                      const float* plan_x, const float* plan_u, const float* dl_dxs,
+                                      const float* dl_dus, float* dx_init, float* dC, float* dc, float* dF, float* df,
+                                      float* dtheta, void* workspace, size_t workspace_bytes, void* stream) {
+  return epgrad_impl<float>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,
+                             dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, true, n_prev},
+                            stream);
+}
+int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
+                                      int32_t n_prev, const double* C, const double* c, const double* F,
+                                      const double* u_lower, const double* u_upper, const double* xs,
+                                      const double* us, const double* plan_x, const double* plan_u,
+                                      const double* dl_dxs, const double* dl_dus, double* dx_init, double* dC,
+                                      double* dc, double* dF, double* df, double* dtheta, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  return epgrad_impl<double>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,
+                              dl_dus, dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, true, n_prev},
                              stream);
 }
 

@@ -424,7 +424,10 @@ __global__ void __launch_bounds__(128) dyn_linearize_kernel(const DynArgs a) {
 // Learnable parameters theta of a system: its first NP entries of DynParams::p (cartpole gravity, masscart, masspole,
 // length; pendulum g, m, l; pendulum_full g, m, l, d, b).  force_mag / max_torque and dt are constants.
 template <int KIND>
-struct DynLearnable;
+struct DynLearnable {   // a passthrough kind: the system's own (its passthrough row has no parameter)
+  static_assert((KIND & DYN_CTRL_PASSTHROUGH) != 0, "unknown dynamics kind");
+  static constexpr int NP = DynLearnable<KIND & ~DYN_CTRL_PASSTHROUGH>::NP;
+};
 template <>
 struct DynLearnable<DYN_CARTPOLE> { static constexpr int NP = 4; };
 template <>
@@ -513,7 +516,8 @@ int launch_dyn_linearize(const DynArgs& a, cudaStream_t stream) {
   else return 2;
   return cudaGetLastError() == cudaSuccess ? 0 : 5;
 }
-// the VJP of the linearisation of a known system (no passthrough kinds: the slew-rate tail linearises the system)
+// the VJP of the linearisation of a known system (no passthrough kinds: the slew-rate tail linearises the system;
+// the reverse sweep of a slew-rate episode instantiates the kernel at a passthrough kind itself, episode_grad.cu)
 template <typename R>
 int launch_dyn_linearize_vjp(const DynVjpArgs& a, cudaStream_t stream) {
   const size_t items = (size_t)(a.T - 1) * a.B;

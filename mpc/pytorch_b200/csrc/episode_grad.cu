@@ -28,12 +28,14 @@ __global__ void __launch_bounds__(256) fill_zero_kernel(size_t n, R* __restrict_
 }
 
 // g = dl_dxs[n_steps]; the accumulators and the adjoint's incoming gradients zeroed; k = n_steps - 1; the loop's
-// handle set to 1
-template <typename R>
-__global__ void __launch_bounds__(256) epgrad_init_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
+// handle set to 1.  DETACH (a slew-rate episode): g's first n_prev entries, the previous control, are 0
+template <typename R, bool DETACH>
+__device__ __forceinline__ void epgrad_init_body(const EpGradArgs<R>& a, int n_prev,
+                                                 cudaGraphConditionalHandle handle) {
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
-  for (size_t i = i0; i < B * N; i += step) a.g[i] = a.dl_dxs[(size_t)a.n_steps * B * N + i];
+  for (size_t i = i0; i < B * N; i += step)
+    a.g[i] = DETACH && i % N < (size_t)n_prev ? R(0) : a.dl_dxs[(size_t)a.n_steps * B * N + i];
   for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] = R(0);
   for (size_t i = i0; i < T * B * P; i += step) a.dc[i] = R(0);
   for (size_t i = i0; i < T * B * N; i += step) a.dl_dx[i] = R(0);
@@ -49,6 +51,15 @@ __global__ void __launch_bounds__(256) epgrad_init_kernel(const EpGradArgs<R> a,
     a.st->k = a.n_steps - 1; a.st->tickets = 0u; a.st->reserved[0] = a.st->reserved[1] = 0;
     cudaGraphSetConditional(handle, 1);
   }
+}
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_init_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
+  epgrad_init_body<R, false>(a, 0, handle);
+}
+template <typename R>
+__global__ void __launch_bounds__(256)
+epgrad_init_detach_kernel(const EpGradArgs<R> a, int n_prev, cudaGraphConditionalHandle handle) {
+  epgrad_init_body<R, true>(a, n_prev, handle);
 }
 
 // the plan of step k into the fixed buffers the body's launchers read
@@ -143,13 +154,15 @@ __global__ void __launch_bounds__(256) epgrad_stage_known_kernel(const EpGradArg
 
 // g = dl_dxs[k] + R^T g + dx_init_k; dC, dc (LinDx: dF, df) += the adjoint's; a known system: dtheta[b] +=
 // theta_step[b] + sum_t (first + second)[t, b] in t order.  The last block to finish counts k down and ends the
-// loop after k = 0: every block has read st->k by then.
-template <typename R>
-__global__ void __launch_bounds__(256) epgrad_accum_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
+// loop after k = 0: every block has read st->k by then.  DETACH: g's first n_prev entries are 0, as in init.
+template <typename R, bool DETACH>
+__device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_prev,
+                                                  cudaGraphConditionalHandle handle) {
   const int k = a.st->k;
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
-  for (size_t i = i0; i < B * N; i += step) a.g[i] = a.dl_dxs[(size_t)k * B * N + i] + a.gx[i] + a.dx_k[i];
+  for (size_t i = i0; i < B * N; i += step)
+    a.g[i] = DETACH && i % N < (size_t)n_prev ? R(0) : a.dl_dxs[(size_t)k * B * N + i] + a.gx[i] + a.dx_k[i];
   for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] += a.dC_k[i];
   for (size_t i = i0; i < T * B * P; i += step) a.dc[i] += a.dc_k[i];
   if (a.kind == DYN_LINEAR) {
@@ -175,6 +188,15 @@ __global__ void __launch_bounds__(256) epgrad_accum_kernel(const EpGradArgs<R> a
     }
   }
 }
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_accum_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
+  epgrad_accum_body<R, false>(a, 0, handle);
+}
+template <typename R>
+__global__ void __launch_bounds__(256)
+epgrad_accum_detach_kernel(const EpGradArgs<R> a, int n_prev, cudaGraphConditionalHandle handle) {
+  epgrad_accum_body<R, true>(a, n_prev, handle);
+}
 
 template <typename R>
 int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
@@ -199,26 +221,53 @@ static size_t epgrad_items(const EpGradArgs<R>& a) {
 }
 
 template <typename R>
-int epgrad_launch_init(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream) {
-  epgrad_init_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  if (n_prev == 0) epgrad_init_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+  else epgrad_init_detach_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, n_prev, handle);
   return launched();
 }
 
+// a passthrough kind runs the system's stage kernel code at its augmented shape: with g's first entry 0 (the detach
+// rule), gx = [0; R^T g[1:]], dl_du[0] = dl_dus[k] + S^T g[1:] and theta_step the VJP's `first` with df = g[1:]
 template <typename R>
 int epgrad_launch_stage(const EpGradArgs<R>& a, cudaStream_t stream) {
   const size_t items = (size_t)a.T * a.B * (a.N > a.M ? a.N : a.M);
   const unsigned grid = epgrad_grid(items);
+  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH,
+                FP = DYN_PENDULUM_FULL | DYN_CTRL_PASSTHROUGH;
   if (a.kind == DYN_LINEAR) epgrad_stage_linear_kernel<R><<<grid, 256, 0, stream>>>(a);
   else if (a.kind == DYN_CARTPOLE) epgrad_stage_known_kernel<R, DYN_CARTPOLE><<<grid, 256, 0, stream>>>(a);
   else if (a.kind == DYN_PENDULUM) epgrad_stage_known_kernel<R, DYN_PENDULUM><<<grid, 256, 0, stream>>>(a);
   else if (a.kind == DYN_PENDULUM_FULL) epgrad_stage_known_kernel<R, DYN_PENDULUM_FULL><<<grid, 256, 0, stream>>>(a);
+  else if (a.kind == CP) epgrad_stage_known_kernel<R, CP><<<grid, 256, 0, stream>>>(a);
+  else if (a.kind == PP) epgrad_stage_known_kernel<R, PP><<<grid, 256, 0, stream>>>(a);
+  else if (a.kind == FP) epgrad_stage_known_kernel<R, FP><<<grid, 256, 0, stream>>>(a);
   else return MPCB200_ERR_BAD_DIMS;
   return launched();
 }
 
 template <typename R>
-int epgrad_launch_accum(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream) {
-  epgrad_accum_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+int epgrad_launch_accum(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  if (n_prev == 0) epgrad_accum_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+  else epgrad_accum_detach_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, n_prev, handle);
+  return launched();
+}
+
+// The linearisation VJP of a passthrough kind, dyn_linearize_vjp_kernel at that kind: the augmented F~ = [[0, 0, I],
+// [0, R, S]] depends on theta only through its [1:, 1:] block and f~ only through f~[1:], so the kernel applies the
+// system's VJP to the [1:, 1:] block of dF~ and to df~[1:] at x~[1:] (the structural zeros add nothing).  The public
+// mpcb200_dyn_linearize_vjp_* keeps taking the systems themselves only (launch_dyn_linearize_vjp).
+template <typename R>
+int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream) {
+  constexpr int CP = DYN_CARTPOLE | DYN_CTRL_PASSTHROUGH, PP = DYN_PENDULUM | DYN_CTRL_PASSTHROUGH,
+                FP = DYN_PENDULUM_FULL | DYN_CTRL_PASSTHROUGH;
+  const size_t items = (size_t)(a.T - 1) * a.B;
+  if (items == 0) return MPCB200_OK;
+  const int grid = (int)((items + 127) / 128);
+  if (a.kind == CP) dyn_linearize_vjp_kernel<R, CP><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == PP) dyn_linearize_vjp_kernel<R, PP><<<grid, 128, 0, stream>>>(a);
+  else if (a.kind == FP) dyn_linearize_vjp_kernel<R, FP><<<grid, 128, 0, stream>>>(a);
+  else return MPCB200_ERR_BAD_DIMS;
   return launched();
 }
 
@@ -226,9 +275,10 @@ int epgrad_launch_accum(const EpGradArgs<R>& a, cudaGraphConditionalHandle handl
   template int episode_launch_plans<R>(int, int, int, int, const R*, const R*, R*, R*, const EpisodeState*,        \
                                        cudaStream_t);                                                              \
   template int launch_fill_zero<R>(size_t, R*, cudaStream_t);                                                      \
-  template int epgrad_launch_init<R>(const EpGradArgs<R>&, cudaGraphConditionalHandle, cudaStream_t);              \
+  template int epgrad_launch_init<R>(const EpGradArgs<R>&, int, cudaGraphConditionalHandle, cudaStream_t);         \
   template int epgrad_launch_stage<R>(const EpGradArgs<R>&, cudaStream_t);                                         \
-  template int epgrad_launch_accum<R>(const EpGradArgs<R>&, cudaGraphConditionalHandle, cudaStream_t);
+  template int epgrad_launch_accum<R>(const EpGradArgs<R>&, int, cudaGraphConditionalHandle, cudaStream_t);        \
+  template int epgrad_launch_vjp_passthrough<R>(const DynVjpArgs&, cudaStream_t);
 MPCB200_EPGRAD_INST(float)
 MPCB200_EPGRAD_INST(double)
 

@@ -11,6 +11,10 @@
 //   e. epgrad_accum_kernel: g = dl_dxs[k] + gx + dx_init_k, and the adjoint's dC, dc (dF, df; theta) summed in.
 // Every buffer a body kernel reads is written by an earlier kernel of the same iteration or by epgrad_init_kernel,
 // so the body holds kernel nodes only.
+// A slew-rate episode (mpcb200_episode_backward_slew_*) runs the same sweep on its augmented problem over
+// [u_{k-1}; x_k] (LinDx, or a known system's passthrough kind) with the previous control detached, as the reference
+// detaches prev_ctrl: the *_detach_kernel forms of init and accumulate set g's first n_prev entries to 0, so no
+// gradient flows into them and the passthrough row of the model step carries nothing back.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,12 +49,15 @@ struct EpGradArgs {
 template <typename R>
 int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
                          const EpisodeState* ep, cudaStream_t stream);
+// n_prev > 0 (a slew-rate episode, mpcb200_episode_backward_slew_*): the detach rule, g[:, :n_prev] = 0
 template <typename R>
-int epgrad_launch_init(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream);
+int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream);
 template <typename R>
 int epgrad_launch_stage(const EpGradArgs<R>& a, cudaStream_t stream);
 template <typename R>
-int epgrad_launch_accum(const EpGradArgs<R>& a, cudaGraphConditionalHandle handle, cudaStream_t stream);
+int epgrad_launch_accum(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream);
+template <typename R>
+int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream);
 template <typename R>
 int launch_fill_zero(size_t n, R* p, cudaStream_t stream);
 

@@ -255,7 +255,8 @@ class _Pad:
         return F[..., : self.n, self.idx] if self.active and F is not None else F
 
 
-_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params")
+# n_prev: an episode's slew-rate augmentation, the leading states that hold the previous control (0: none)
+_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev", defaults=(0,))
 
 
 def _problem(n, m, T, B, dtype, dev, C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None,
@@ -411,7 +412,7 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
 
 def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
-                best_cost_eps=1e-4, dyn=None, keep_plans=False):
+                best_cost_eps=1e-4, dyn=None, keep_plans=False, n_prev=0):
     """A receding-horizon episode of n_steps control steps in ONE library call (mpcb200_episode_*): each step solves
     the problem from the current state as ilqr_raw does (u_init = the warm start), applies the plan's first control,
     steps the model (LinDx: F[0] [x; u] + f[0]; a known system `dyn`: one step of it) and shifts the warm start
@@ -420,7 +421,9 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     [n_steps, B], info int32 [n_steps, 2] and u_next [T, B, m]; None when the driver has no conditional graph nodes
     or no conditional node inside another's body (nothing was launched then).  keep_plans: the call is
     mpcb200_episode_plans_*, and the dict also holds "saved", what episode_backward_raw takes: the staged problem and
-    the padded xs, us and each solve's best iterate plan_x [n_steps, T, B, N], plan_u [n_steps, T, B, M]."""
+    the padded xs, us and each solve's best iterate plan_x [n_steps, T, B, N], plan_u [n_steps, T, B, M].
+    n_prev > 0: the problem is a slew-rate penalty's augmented one over [u_{k-1}; x_k] and its first n_prev states
+    are the previous control; the staged problem records it, so episode_backward_raw detaches them."""
     n, m = n_state, n_ctrl
     if T < 3 or n_steps < 1:
         raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
@@ -458,7 +461,7 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     check(rc, name)
     res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
     if keep_plans:
-        res["saved"] = (s, n_steps, xs, us, plan_x, plan_u)
+        res["saved"] = (s._replace(n_prev=int(n_prev)), n_steps, xs, us, plan_x, plan_u)
     return res
 
 
@@ -467,7 +470,10 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
     (mpcb200_episode_backward_*): `saved` is that call's res["saved"], dl_dxs [n_steps+1, B, n] and dl_dus
     [n_steps, B, m] the gradients of its x and u.  Returns (dx_init [B, n], dC [T, B, p, p], dc [T, B, p], dF, df,
     dtheta): LinDx dF like the staged F's [F_T, B, n, p] and df like its f (None without f), dtheta None; a known
-    system dF = df = None and dtheta [B, NP], one row per problem (the caller sums over b, as DynLinearize does)."""
+    system dF = df = None and dtheta [B, NP], one row per problem (the caller sums over b, as DynLinearize does).
+    A slew-rate episode (the staged problem's n_prev > 0) runs mpcb200_episode_backward_slew_*: every size is the
+    augmented problem's, and the first n_prev states of each augmented state get no gradient (dx_init[:, :n_prev] = 0);
+    the caller crops the gradients to the system's own blocks."""
     s, n_steps, xs, us, plan_x, plan_u = saved
     pad, dims = s.pad, s.dims
     T, B, N, M = dims.T, dims.B, pad.N, pad.M
@@ -484,17 +490,24 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
         if dims.has_f:
             df = torch.empty(T - 1, B, N, dtype=dtype, device=dev)
     else:
-        from .dynamics import DYN_NPARAMS
-        dtheta = torch.empty(B, DYN_NPARAMS[kind], dtype=dtype, device=dev)
-    nbytes = _lib.lib().mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), xs.element_size())
+        from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_NPARAMS
+        dtheta = torch.empty(B, DYN_NPARAMS[kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
+    L = _lib.lib()
+    if s.n_prev:
+        name = "mpcb200_episode_backward_slew"
+        nbytes = L.mpcb200_episode_backward_slew_workspace_bytes(ctypes.byref(dims), int(s.n_prev), xs.element_size())
+        head = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), int(s.n_prev)]
+    else:
+        name = "mpcb200_episode_backward"
+        nbytes = L.mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), xs.element_size())
+        head = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps)]
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    fn = _lib.entry("mpcb200_episode_backward", dtype)
+    fn = _lib.entry(name, dtype)
     with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), ptr_view(s.C), ptr_view(s.c),
-                ptr_view(s.F), ptr(s.u_lower), ptr(s.u_upper), ptr(xs), ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_),
-                ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(dtheta), ptr(ws), nbytes,
-                stream_handle(dev))
-    check(rc, "mpcb200_episode_backward")
+        rc = fn(*head, ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr(s.u_lower), ptr(s.u_upper), ptr(xs), ptr(us),
+                ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df),
+                ptr(dtheta), ptr(ws), nbytes, stream_handle(dev))
+    check(rc, name)
     if df is not None and s.f.shape[0] == T:          # a full-length f: its last slice never enters the episode
         df = torch.cat((df, torch.zeros_like(df[:1])), 0)
     return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)

@@ -212,8 +212,26 @@ static int run_pnqp_large(int B, int n) {
   return bad != 0;
 }
 
+// the slew-rate episode backward's argument checks (they run before anything is launched): the pendulum's
+// passthrough kind at its dynamics-only shape (4, 1) takes n_prev = 1 only, and its workspace follows
+static int run_episode_backward_slew() {
+  mpcb200_dims d = {4, 5, 4, 1, 4, 1, 0, 0, 0, 10, 20, 1, MPCB200_DYN_PENDULUM | MPCB200_DYN_CTRL_PASSTHROUGH};
+  mpcb200_params prm = {0.0, 0.0, 0.0, 0.2, {10.0, 1.0, 1.0, 2.0, 0.05}};
+  const size_t need = mpcb200_episode_backward_slew_workspace_bytes(&d, 1, 4);
+  if (need == 0 || mpcb200_episode_backward_slew_workspace_bytes(&d, 2, 4) != 0)
+    return printf("episode backward slew workspace %zu\n", need), 1;
+  Dev<float> buf(1024), ws(need / sizeof(float) + 64);
+  float* p = buf.p;
+  const int rc = mpcb200_episode_backward_slew_f32(&d, &prm, 3, 0, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p,
+                                                   ws.p, need, nullptr);
+  if (rc != MPCB200_ERR_BAD_DIMS) return printf("episode backward slew n_prev=0 rc=%d\n", rc), 1;
+  printf("episode backward slew: workspace %zu bytes, n_prev=0 refused\n", need);
+  return 0;
+}
+
 int main() {
   int fails = 0;
+  fails += run_episode_backward_slew();
   fails += run_pnqp_large(3, 100);
   fails += run_dyn(MPCB200_DYN_CARTPOLE, 37, 9);
   fails += run_dyn(MPCB200_DYN_PENDULUM, 20, 7);
