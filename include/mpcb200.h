@@ -457,6 +457,81 @@ int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_pa
                                       double* dx_init, double* dC, double* dc, double* dF, double* df, double* dtheta,
                                       void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * An episode closed on a plant other than the model the solves plan with, with additive process disturbances:
+ *   x_{k+1} = plant(x_k, u_k) + w_k
+ * where each solve still plans with the problem's own dynamics (dims, params, F, f).  The plant is
+ *   kind MPCB200_DYN_LINEAR: F_plant[B,n,n+m] and, with has_f, f_plant[B,n] - the t = 0 slices of a LinDx, at the
+ *        problem's (padded) sizes: x' = F_plant [x; u] + f_plant;
+ *   a known kind (dyn[] as in mpcb200_params.dyn): its own step, with its own parameters.  Its (n, m) must be the
+ *        problem's exactly, else MPCB200_ERR_BAD_DIMS; under a slew-rate penalty that is its passthrough kind, which
+ *        steps [u_{k-1}; x_k] to [u_k; plant(x_k, u_k)].
+ * mpcb200_episode_plant_* takes no n_prev, so it cannot tell a slew-rate augmented problem from a plain one of the
+ * same (n, m): it accepts a passthrough plant wherever the shapes match, and a passthrough plant on a problem that is
+ * not augmented would read x[0] as the previous control.  The caller pairs them; mpcb200_episode_backward_plant_*,
+ * which takes n_prev, refuses the mismatch (MPCB200_ERR_BAD_DIMS).
+ */
+typedef struct mpcb200_plant {
+  int32_t kind;           /* MPCB200_DYN_LINEAR or a known kind (| MPCB200_DYN_CTRL_PASSTHROUGH) */
+  int32_t has_f;          /* LinDx: f_plant given                                                 */
+  double dyn[8];          /* known kind: its parameters                                           */
+} mpcb200_plant;
+
+/*
+ * mpcb200_episode_plans_* with the model step replaced by the plant's (mpcb200_plant above) plus w[n_steps,B,n]
+ * (NULL: none), added before xs[k+1] and the next solve's state are written.  Under a slew-rate penalty w's first
+ * n_ctrl entries (the previous control) are the caller's to keep at 0.  plan_x and plan_u may both be NULL (only one:
+ * MPCB200_ERR_NULL_POINTER), which records mpcb200_episode_*'s graph.  Checks, capture contract, launch counting and
+ * workspace (mpcb200_episode_workspace_bytes()) as for mpcb200_episode_*; every argument error is reported before
+ * anything is captured.
+ */
+int mpcb200_episode_plant_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                              const mpcb200_plant* plant, int32_t n_steps, const float* C, const float* c,
+                              const float* F, const float* f, const float* F_plant, const float* f_plant,
+                              const float* w, const float* x_init, const float* u_init, const float* u_lower,
+                              const float* u_upper, const uint8_t* u_zero_I, float* xs, float* us, float* costs,
+                              int32_t* info, float* u_next, float* plan_x, float* plan_u, void* workspace,
+                              size_t workspace_bytes, void* stream);
+int mpcb200_episode_plant_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                              const mpcb200_plant* plant, int32_t n_steps, const double* C, const double* c,
+                              const double* F, const double* f, const double* F_plant, const double* f_plant,
+                              const double* w, const double* x_init, const double* u_init, const double* u_lower,
+                              const double* u_upper, const uint8_t* u_zero_I, double* xs, double* us, double* costs,
+                              int32_t* info, double* u_next, double* plan_x, double* plan_u, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
+/*
+ * The reverse sweep of an episode of mpcb200_episode_plant_* (run with plan_x, plan_u): mpcb200_episode_backward_*
+ * (n_prev = 0) or mpcb200_episode_backward_slew_* (n_prev > 0, the same n_prev rules) with the model step's VJP taken
+ * at the plant.  The model's outputs dF, df (LinDx) or dtheta (a known system) get the solves' part only: the
+ * adjoints, and a known system's linearisation VJP.  The plant's own outputs get the plant steps' direct part:
+ *   LinDx plant: dF_plant[B,n,n+m] = sum_k g_k [x_k; u_k]^T and, with has_f, df_plant[B,n] = sum_k g_k;
+ *   a known plant: dtheta_plant[B,NP_plant] = sum_k the VJP's `first` (its Jacobian held constant);
+ * with g_k = dL/dx_{k+1}.  dw[n_steps,B,n] (NULL: not written) = dL/dw_k = g_k.  A known plant must be a passthrough
+ * kind exactly when n_prev > 0, with n_prev its n_ctrl, else MPCB200_ERR_BAD_DIMS.  Errors, capture contract and
+ * launch counting as for mpcb200_episode_backward_*; every argument error is reported before anything is captured.
+ * workspace: mpcb200_episode_backward_plant_workspace_bytes() bytes (0 for arguments it does not take).
+ */
+size_t mpcb200_episode_backward_plant_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev,
+                                                      const mpcb200_plant* plant, int32_t elem_size);
+int mpcb200_episode_backward_plant_f32(const mpcb200_dims* dims, const mpcb200_params* params,
+                                       const mpcb200_plant* plant, int32_t n_steps, int32_t n_prev, const float* C,
+                                       const float* c, const float* F, const float* F_plant, const float* u_lower,
+                                       const float* u_upper, const float* xs, const float* us, const float* plan_x,
+                                       const float* plan_u, const float* dl_dxs, const float* dl_dus, float* dx_init,
+                                       float* dC, float* dc, float* dF, float* df, float* dtheta, float* dF_plant,
+                                       float* df_plant, float* dtheta_plant, float* dw, void* workspace,
+                                       size_t workspace_bytes, void* stream);
+int mpcb200_episode_backward_plant_f64(const mpcb200_dims* dims, const mpcb200_params* params,
+                                       const mpcb200_plant* plant, int32_t n_steps, int32_t n_prev, const double* C,
+                                       const double* c, const double* F, const double* F_plant,
+                                       const double* u_lower, const double* u_upper, const double* xs,
+                                       const double* us, const double* plan_x, const double* plan_u,
+                                       const double* dl_dxs, const double* dl_dus, double* dx_init, double* dC,
+                                       double* dc, double* dF, double* df, double* dtheta, double* dF_plant,
+                                       double* df_plant, double* dtheta_plant, double* dw, void* workspace,
+                                       size_t workspace_bytes, void* stream);
+
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);
 

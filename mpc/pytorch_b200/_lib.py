@@ -32,6 +32,10 @@ class IlqrOpts(ctypes.Structure):
         [(k, ctypes.c_double) for k in ("eps", "best_cost_eps")]
 
 
+class Plant(ctypes.Structure):
+    _fields_ = [("kind", ctypes.c_int32), ("has_f", ctypes.c_int32), ("dyn", ctypes.c_double * 8)]
+
+
 class MpcB200Error(RuntimeError):
     pass
 
@@ -55,7 +59,9 @@ EXPORTED_SYMBOLS = (
     "mpcb200_episode_plans_f32", "mpcb200_episode_plans_f64", "mpcb200_episode_backward_f32",
     "mpcb200_episode_backward_f64", "mpcb200_episode_backward_workspace_bytes",
     "mpcb200_episode_backward_slew_f32", "mpcb200_episode_backward_slew_f64",
-    "mpcb200_episode_backward_slew_workspace_bytes",
+    "mpcb200_episode_backward_slew_workspace_bytes", "mpcb200_episode_plant_f32", "mpcb200_episode_plant_f64",
+    "mpcb200_episode_backward_plant_f32", "mpcb200_episode_backward_plant_f64",
+    "mpcb200_episode_backward_plant_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -144,6 +150,19 @@ def lib():
         fn.restype = ctypes.c_int
     L.mpcb200_episode_backward_slew_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_episode_backward_slew_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_episode_plant_f32", "mpcb200_episode_plant_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(IlqrOpts), ctypes.POINTER(Plant),
+                       ctypes.c_int32] + [vp] * 20 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    for name in ("mpcb200_episode_backward_plant_f32", "mpcb200_episode_backward_plant_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(Plant), ctypes.c_int32,
+                       ctypes.c_int32] + [vp] * 23 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_episode_backward_plant_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32,
+                                                                 ctypes.POINTER(Plant), ctypes.c_int32]
+    L.mpcb200_episode_backward_plant_workspace_bytes.restype = ctypes.c_size_t
     L.mpcb200_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_supported.restype = ctypes.c_int
     L.mpcb200_supported_list.argtypes = [ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]

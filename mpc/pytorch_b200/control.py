@@ -26,7 +26,7 @@ from .solver import CtrlPassthroughDynamics, LinDx, QuadCost, _mv
 Episode = namedtuple("Episode", "x u costs info u_next")
 
 
-def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False):
+def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plant=None, disturbance=None):
     """Run `n_steps` control steps of receding-horizon MPC from `x_init` [B, n] with the solver `ctrl` (an ``MPC``,
     which supplies every solver option).  For k = 0 .. n_steps-1:
 
@@ -64,48 +64,141 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False):
     Where the episode runs as one graph, with or without a slew-rate penalty, the backward is one more graph
     (``step.episode_backward_raw``); otherwise the host path's loop runs with autograd recording.  Under a slew-rate
     penalty each solve runs on the augmented state [u_{k-1}; x_k], and u_{k-1} is held constant there as the
-    reference holds ``prev_ctrl``: no gradient flows through the previous control into the solve."""
+    reference holds ``prev_ctrl``: no gradient flows through the previous control into the solve.
+
+    ``plant``: what steps the loop, while every solve still plans with ``dx``.  None (or ``dx`` itself) is the model.
+    Otherwise a ``LinDx`` (its t = 0 slice, as the model's LinDx step), a known system with its own ``params``,
+    ``force_mag`` / ``max_torque`` and ``dt`` (its kind may differ from the model's), or any other Module, called as
+    ``plant(x_k, u_k)``; it must map (n_state, n_ctrl) to n_state.  ``disturbance``: w [n_steps, B, n] in x_init's
+    dtype and on its device, or None.  The loop is then
+
+        for k: _, plan_u, _ = ctrl'(x_k, cost, dx);  x_{k+1} = plant(x_k, plan_u[0]) + w_k
+
+    and ``Episode.x[k+1]`` is the disturbed state (under a slew-rate penalty the plant steps x, and solve k still takes
+    ``prev_ctrl = u_{k-1}``).  Its gradient is autograd's for that loop: the model's parameters (``params``, or F and
+    f) get the solves' part only, the plant's the plant steps' exact VJP (a known system's ``params`` the VJP's
+    ``first``; a LinDx's F[0], f[0]: g z^T and g), ``disturbance`` gets dL/dx_{k+1} at step k, and a tensor that the
+    model and the plant share gets the sum.  The episode runs as one graph when the model's episode would and the
+    plant steps at the staged shape (a LinDx plant with F, f on the episode's device and dtype; a known plant whose
+    state width is the staged one); otherwise (an opaque Module plant, say) the host path runs, stepping the plant
+    with the kernels the graph uses and adding w_k, so the two agree bit for bit wherever both apply."""
     T, n, m = ctrl.T, ctrl.n_state, ctrl.n_ctrl
     if T < 3:
         raise MpcB200Error(f"a receding-horizon episode needs a horizon T >= 3 (the warm-start shift), got T={T}")
     if n_steps < 1:
         raise MpcB200Error(f"a receding-horizon episode needs n_steps >= 1, got {n_steps}")
     B = x_init.shape[0]
+    if plant is dx:
+        plant = None
+    _check_plant(plant, disturbance, x_init, n, m, n_steps)
+    if plant is None and disturbance is not None:
+        plant = dx                        # the model steps the disturbed loop
     cost = solver._expand_cost(cost, T, ctrl.n_batch if ctrl.n_batch is not None else B, n + m)
     w0 = _first_warm_start(ctrl, x_init)
     from .dynamics import params_scope
-    if differentiable and torch.is_grad_enabled() and _requires_grad(x_init, cost, dx):
+    if differentiable and torch.is_grad_enabled() and _requires_grad(x_init, cost, dx, plant, disturbance):
         with params_scope():
-            if _takes_device_path(ctrl, x_init, cost, dx, w0):
-                ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0)
+            if _takes_device_path(ctrl, x_init, cost, dx, w0, plant):
+                ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
                 if ep is not None:
                     return ep
-            return _episode_host(ctrl, x_init, cost, dx, n_steps, w0)
+            return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
     with torch.no_grad(), params_scope():     # a known system's CUDA parameters are read once per episode
-        if _takes_device_path(ctrl, x_init, cost, dx, w0):
-            ep = _episode_device(ctrl, x_init, cost, dx, n_steps, w0)
+        if _takes_device_path(ctrl, x_init, cost, dx, w0, plant):
+            ep = _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
             if ep is not None:
                 return ep
-        return _episode_host(ctrl, x_init, cost, dx, n_steps, w0)
+        return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
 
 
-def _requires_grad(x_init, cost, dx):
+def _check_plant(plant, w, x_init, n, m, n_steps):
+    """A plant's shapes against the model's (n_state, n_ctrl) and w's against the episode, before anything runs.  An
+    opaque Module without n_state / n_ctrl is checked on its output at every step (_plant_step)."""
+    if isinstance(plant, LinDx):
+        F, f = plant.F, plant.f
+        if not isinstance(F, torch.Tensor) or F.dim() < 3 or F.shape[0] < 1 or tuple(F.shape[-2:]) != (n, n + m):
+            raise MpcB200Error(f"plant: a LinDx plant needs F [T, B, {n}, {n + m}], got "
+                               f"{tuple(F.shape) if isinstance(F, torch.Tensor) else F}")
+        if f is not None and f.nelement() > 0 and (f.dim() < 2 or f.shape[0] < 1 or f.shape[-1] != n):
+            raise MpcB200Error(f"plant: a LinDx plant needs f [T, B, {n}], got {tuple(f.shape)}")
+    elif plant is not None:
+        dims = (getattr(plant, "n_state", n), getattr(plant, "n_ctrl", m))
+        if dims != (n, m):
+            raise MpcB200Error(f"plant: maps (n_state, n_ctrl) = {dims}, the model {(n, m)}")
+    if w is not None:
+        B = x_init.shape[0]
+        if tuple(w.shape) != (n_steps, B, n) or w.dtype != x_init.dtype or w.device != x_init.device:
+            raise MpcB200Error(f"disturbance: expected a {x_init.dtype} tensor of shape {(n_steps, B, n)} on "
+                               f"{x_init.device}, got a {w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
+
+
+def _requires_grad(x_init, cost, dx, plant=None, w=None):
     """Whether any input an episode differentiates in requires grad: x_init, a QuadCost's C and c (a Module cost's
-    parameters), LinDx's F and f, or a Module's parameters and ``params``."""
-    ts = [x_init]
+    parameters), LinDx's F and f, or a Module's parameters and ``params``, of the model and of the plant; and w."""
+    ts = [x_init, w]
     ts += [cost.C, cost.c] if isinstance(cost, QuadCost) else list(cost.parameters())
-    if isinstance(dx, LinDx):
-        ts += [dx.F, dx.f]
-    else:
-        ts += list(dx.parameters()) + [getattr(dx, "params", None)]
+    for d in (dx, plant):
+        if isinstance(d, LinDx):
+            ts += [d.F, d.f]
+        elif d is not None:
+            ts += list(d.parameters()) + [getattr(d, "params", None)]
     return any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts)
 
 
-def _takes_device_path(ctrl, x_init, cost, dx, w0):
+def _takes_device_path(ctrl, x_init, cost, dx, w0, plant=None):
     """Whether the episode runs as one graph: exactly when each of its solves would take the device loop (T >= 3 is
-    checked before).  Decided on tensor metadata alone."""
-    return solver._use_device_loop(ctrl, x_init, cost, dx, w0) or \
-        solver._use_slew_device_loop(ctrl, x_init, cost, dx, w0)
+    checked before) and the plant, if any, steps at the staged shape (_plant_on_device).  Decided on tensor metadata
+    alone."""
+    return (solver._use_device_loop(ctrl, x_init, cost, dx, w0) or
+            solver._use_slew_device_loop(ctrl, x_init, cost, dx, w0)) and \
+        (plant is None or _plant_on_device(ctrl, x_init, dx, plant))
+
+
+def _plant_on_device(ctrl, x_init, dx, plant):
+    """Whether the plant steps inside the episode's graph: a LinDx plant whose F (and f) are tensors of the episode's
+    dtype and device (staged like the model's, _Pad), or a known system whose state width, n or n + m under a
+    slew-rate penalty, is the staged one.  A known model always runs at its own width; a LinDx model where
+    _pick_instance gives the exact shape or the large-shape kernels."""
+    from .dynamics import DYN_LINEAR, known_kind
+    from .step import _pick_instance
+    n, m = ctrl.n_state, ctrl.n_ctrl
+    if isinstance(plant, LinDx):
+        ts = [plant.F] + ([plant.f] if plant.f is not None and plant.f.nelement() > 0 else [])
+        return all(t.dtype == x_init.dtype and t.device == x_init.device for t in ts)
+    if known_kind(plant, n, m, x_init)[0] == DYN_LINEAR:
+        return False
+    if not isinstance(dx, LinDx):
+        return True
+    n_aug = n + m if ctrl.slew_rate_penalty is not None else n
+    return _pick_instance(n_aug, m, x_init.element_size(), DYN_LINEAR) == (n_aug, m)
+
+
+def _plant_spec(ctrl, x_init, C, plant, F_p, f_p):
+    """The plant as step.episode_raw takes it, on the problem MPC._device_problem stages: (DYN_LINEAR, None, F, f) of
+    a LinDx plant (under a slew-rate penalty its slice 0 alone, the one that steps, augmented as MPC._slew_augment
+    augments F, f), or (kind, params, None, None) of a known system (its passthrough kind under a slew-rate
+    penalty)."""
+    from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, known_kind
+    slew = ctrl.slew_rate_penalty is not None
+    if isinstance(plant, LinDx):
+        if slew:                          # [[0, 0, I], [0, F_p]] and [0; f_p] of the slice that steps
+            m = ctrl.n_ctrl
+            F0 = F_p[:1]
+            Fu = F0.new_zeros(1, F0.shape[1], m, F0.shape[3] + m)
+            Fu[..., F0.shape[3]:] = torch.eye(m, dtype=F0.dtype, device=F0.device)
+            F_p = torch.cat((Fu, torch.cat((F0.new_zeros(*F0.shape[:3], m), F0), 3)), 2)
+            if f_p is not None and f_p.nelement() > 0:
+                f_p = torch.cat((f_p.new_zeros(1, f_p.shape[1], m), f_p[:1]), 2)
+        return DYN_LINEAR, None, F_p, f_p
+    kind, params = known_kind(plant, ctrl.n_state, ctrl.n_ctrl, x_init)
+    return (kind | DYN_CTRL_PASSTHROUGH if slew else kind), params, None, None
+
+
+def _staged_w(ctrl, w):
+    """w as the augmented problem takes it under a slew-rate penalty: m zeros in front (the previous control)."""
+    if w is None or ctrl.slew_rate_penalty is None:
+        return w
+    return torch.cat((w.new_zeros(*w.shape[:2], ctrl.n_ctrl), w), 2)
 
 
 def shift_warm_start(plan_u):
@@ -126,13 +219,17 @@ def _first_warm_start(ctrl, x_init):
     return u.to(dtype=x_init.dtype, device=x_init.device)
 
 
-def _episode_device(ctrl, x_init, cost, dx, n_steps, w0):
+def _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
     """The episode as one library call (step.episode_raw) on the problem MPC._ilqr_device stages, once; None when the
     driver refused the graph (nothing ran then)."""
     from . import step as _step
     T, m = ctrl.T, ctrl.n_ctrl
     n, x0, C, c, F, f, dyn = ctrl._device_problem(x_init, cost, dx)
-    res = _step.episode_raw(n, m, T, n_steps, x0, C, c, F, f, w0, dyn=dyn, **ctrl._device_options())
+    kw = {}
+    if plant is not None:
+        F_p, f_p = (plant.F, plant.f) if isinstance(plant, LinDx) else (None, None)
+        kw = dict(plant=_plant_spec(ctrl, x_init, cost.C, plant, F_p, f_p), w=_staged_w(ctrl, w))
+    res = _step.episode_raw(n, m, T, n_steps, x0, C, c, F, f, w0, dyn=dyn, **kw, **ctrl._device_options())
     if res is None:
         solver._graph_cond_unavailable = True
         return None
@@ -148,7 +245,7 @@ class _NoGraph(Exception):
 class EpisodeFn(torch.autograd.Function):
     """(x, u, costs, info, u_next) of a differentiable device episode: the forward is step.episode_raw with
     keep_plans, the backward one step.episode_backward_raw call.  One module-level Function (DESIGN.md section 3.2).
-    `o` = (ctrl, dx, n_steps, w0); the known system's parameter values are the host numbers the forward took
+    `o` = (ctrl, dx, n_steps, w0, plant); the known system's parameter values are the host numbers the forward took
     (params_scope) and the backward reuses them.  Under a slew-rate penalty the staged problem is the augmented one
     over [u_{k-1}; x] (MPC._device_problem): x is returned without its first m states, the backward pads dl_dx with
     m zeros in front, the sweep detaches those states (n_prev = m), and the gradients are cropped to the blocks of
@@ -156,24 +253,34 @@ class EpisodeFn(torch.autograd.Function):
     backward reads (xs, us, the plans, the staged C, c,
     F, f and bounds) goes through save_for_backward, so an in-place edit of x or u before the backward raises, and the
     outputs do not keep themselves alive through ctx; ctx holds only the staged problem's metadata.  First order only:
-    the backward is raw kernels."""
+    the backward is raw kernels.  `o[4]` a plant (receding_horizon's `plant`), or None: F_p, f_p (a LinDx plant's),
+    plant_params (a known plant's) and w are then inputs too, the staged plant's F, f go through save_for_backward,
+    and their gradients come from the plant sweep (step.episode_backward_raw), F_p's and f_p's in slice 0."""
 
     @staticmethod
-    def forward(ctx, o, x_init, C, c, F, f, params):
+    def forward(ctx, o, x_init, C, c, F, f, params, F_p=None, f_p=None, plant_params=None, w=None):
         from . import step as _step
-        ctrl, dx, n_steps, w0 = o
+        ctrl, dx, n_steps, w0, plant = o
         T, m = ctrl.T, ctrl.n_ctrl
         n, x0, C_, c_, F_, f_, dyn = ctrl._device_problem(x_init, QuadCost(C, c), dx)
         slew = ctrl.slew_rate_penalty is not None
+        kw = {}
+        if plant is not None:
+            kw = dict(plant=_plant_spec(ctrl, x_init, C, plant, F_p, f_p), w=_staged_w(ctrl, w))
         res = _step.episode_raw(n, m, T, n_steps, x0, C_, c_, F_, f_, w0, dyn=dyn, keep_plans=True,
-                                n_prev=m if slew else 0, **ctrl._device_options())
+                                n_prev=m if slew else 0, **kw, **ctrl._device_options())
         if res is None:
             raise _NoGraph()
         ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
         s, ctx.n_steps, xs, us, plan_x, plan_u = res["saved"]
-        ctx.save_for_backward(xs, us, plan_x, plan_u, s.C, s.c, s.F, s.f, s.u_lower, s.u_upper)
-        ctx.problem = s._replace(C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None)
+        sp = s.plant
+        ctx.save_for_backward(xs, us, plan_x, plan_u, s.C, s.c, s.F, s.f, s.u_lower, s.u_upper,
+                              sp.F if sp is not None else None, sp.f if sp is not None else None)
+        ctx.problem = s._replace(C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None,
+                                 plant=sp._replace(F=None, f=None) if sp is not None else None)
         ctx.p_meta = (params.dtype, params.device) if params is not None else None
+        ctx.plant_meta = (F_p.shape if F_p is not None else None, f_p.shape if f_p is not None else None,
+                          (plant_params.dtype, plant_params.device) if plant_params is not None else None)
         ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
         x = res["x"][:, :, m:] if slew else res["x"]
         return x, res["u"], res["costs"], res["info"], res["u_next"]
@@ -182,8 +289,10 @@ class EpisodeFn(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, dl_dx, dl_du, *_):
         from . import step as _step
-        xs, us, plan_x, plan_u, C, c, F, f, lo, hi = ctx.saved_tensors
+        xs, us, plan_x, plan_u, C, c, F, f, lo, hi, Fp, fp = ctx.saved_tensors
         s = ctx.problem._replace(C=C, c=c, F=F, f=f, u_lower=lo, u_upper=hi)
+        if s.plant is not None:
+            s = s._replace(plant=s.plant._replace(F=Fp, f=fp))
         n_steps, k = ctx.n_steps, s.n_prev
         if dl_dx is None:
             dl_dx = xs.new_zeros(n_steps + 1, s.dims.B, s.pad.n)
@@ -191,47 +300,74 @@ class EpisodeFn(torch.autograd.Function):
             dl_dx = torch.cat((dl_dx.new_zeros(n_steps + 1, s.dims.B, k), dl_dx), 2)
         if dl_du is None:
             dl_du = us.new_zeros(n_steps, s.dims.B, s.pad.m)
-        dx_init, dC, dc, dF, df, dtheta = _step.episode_backward_raw((s, n_steps, xs, us, plan_x, plan_u), dl_dx,
-                                                                     dl_du)
+        out = _step.episode_backward_raw((s, n_steps, xs, us, plan_x, plan_u), dl_dx, dl_du)
+        dx_init, dC, dc, dF, df, dtheta = out[:6]
+        dF_p, df_p, dth_p, dw = out[6:] if s.plant is not None else (None, None, None, None)
         if k:                                     # the blocks of x_init, C, c, F, f inside the augmented problem
             dx_init, dC, dc = dx_init[:, k:], dC[..., k:, k:], dc[..., k:]
             dF = dF[..., k:, k:] if dF is not None else None
             df = df[..., k:] if df is not None else None
+            dF_p = dF_p[..., k:, k:] if dF_p is not None else None
+            df_p = df_p[..., k:] if df_p is not None else None
+            dw = dw[..., k:] if dw is not None else None
         need = ctx.needs_input_grad
-        dparams = None
+        dparams = dFp = dfp = dpp = None
         if dtheta is not None and need[6]:
             dparams = dtheta.sum(0).to(dtype=ctx.p_meta[0], device=ctx.p_meta[1])
+        F_shape, f_shape, pp_meta = ctx.plant_meta
+        if dF_p is not None and need[7]:          # the plant steps with its slice 0
+            dFp = dF_p.new_zeros(F_shape)
+            dFp[0] = dF_p
+        if df_p is not None and need[8]:
+            dfp = df_p.new_zeros(f_shape)
+            dfp[0] = df_p
+        if dth_p is not None and need[9]:
+            dpp = dth_p.sum(0).to(dtype=pp_meta[0], device=pp_meta[1])
         return (None, dx_init if need[1] else None, dC if need[2] else None, dc if need[3] else None,
-                dF if need[4] else None, df if need[5] else None, dparams if need[6] else None)
+                dF if need[4] else None, df if need[5] else None, dparams if need[6] else None, dFp, dfp, dpp,
+                dw if dw is not None and need[10] else None)
 
 
-def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0):
+def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
     """The differentiable episode on the device path (EpisodeFn); None when the driver refused the graph."""
     F, f, params = None, None, None
     if isinstance(dx, LinDx):
         F, f = dx.F, dx.f
     else:
         params = getattr(dx, "params", None)
+    extra = ()
+    if plant is not None:
+        F_p = f_p = p_params = None
+        if isinstance(plant, LinDx):
+            F_p, f_p = plant.F, plant.f
+        else:
+            p_params = getattr(plant, "params", None)
+        extra = (F_p, f_p, p_params, w)
     try:
-        x, u, costs, info, u_next = EpisodeFn.apply((ctrl, dx, n_steps, w0), x_init, cost.C, cost.c, F, f, params)
+        x, u, costs, info, u_next = EpisodeFn.apply((ctrl, dx, n_steps, w0, plant), x_init, cost.C, cost.c, F, f,
+                                                    params, *extra)
     except _NoGraph:
         solver._graph_cond_unavailable = True
         return None
     return Episode(x, u, costs, info, u_next)
 
 
-def _episode_host(ctrl, x_init, cost, dx, n_steps, w):
+def _episode_host(ctrl, x_init, cost, dx, n_steps, w, plant=None, dist=None):
     """The episode as a Python loop over MPC.forward, on a shallow copy of ctrl that takes each step's warm start.
-    Differentiable where autograd records: the warm starts and prev_ctrl are held constant."""
+    Differentiable where autograd records: the warm starts and prev_ctrl are held constant.  A plant steps the loop
+    in the model's place (_model_step applied to it), and dist[k] is added to its step."""
     slew = ctrl.slew_rate_penalty is not None
     solve = copy.copy(ctrl)
     solve.exit_unconverged = solve.detach_unconverged = False
     xs, us, costs, infos = [x_init], [], [], []
     x, prev = x_init, ctrl.prev_ctrl
-    for _ in range(n_steps):
+    for k in range(n_steps):
         solve.u_init, solve.prev_ctrl = w, prev
         _, plan_u, plan_costs = solve(x, cost, dx)
-        x = _model_step(solve, x, plan_u, cost, dx)
+        if plant is None:
+            x = _model_step(solve, x, plan_u, cost, dx)
+        else:
+            x = _plant_step(solve, x, plan_u, cost, plant, dist[k] if dist is not None else None)
         w = shift_warm_start(plan_u.detach())
         if slew:
             prev = plan_u[0].detach()
@@ -240,6 +376,15 @@ def _episode_host(ctrl, x_init, cost, dx, n_steps, w):
         costs.append(plan_costs)
         infos.append(solve._solve_info.to(x_init.device))
     return Episode(torch.stack(xs), torch.stack(us), torch.stack(costs), torch.stack(infos), w)
+
+
+def _plant_step(solve, x, plan_u, cost, plant, w_k):
+    """x_{k+1} = plant(x_k, u_k) + w_k on the host path: the plant stepped as _model_step steps the model (the
+    kernels the device path runs, or a Module call), then w_k added."""
+    nx = _model_step(solve, x, plan_u, cost, plant)
+    if tuple(nx.shape) != tuple(x.shape):
+        raise MpcB200Error(f"plant: returned a state of shape {tuple(nx.shape)} for x_k of shape {tuple(x.shape)}")
+    return nx + w_k if w_k is not None else nx
 
 
 def _model_step(solve, x, plan_u, cost, dx):

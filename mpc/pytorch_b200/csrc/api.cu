@@ -773,7 +773,32 @@ struct EpisodeCall {
   void* workspace;
   size_t workspace_bytes;
   R *plan_x, *plan_u;          // mpcb200_episode_plans_*: each solve's best iterate; NULL for mpcb200_episode_*
+  // mpcb200_episode_plant_*: the plant that steps the loop and the disturbances; otherwise the model steps it
+  const mpcb200_plant* plant;
+  const R *F_plant, *f_plant, *w;
 };
+
+// the model step's kind, parameters, F, f and has_f: the plant's where the call names one, else the model's
+template <typename R>
+struct EpisodeStep {
+  int kind, has_f;
+  const double* dyn;
+  const R *F, *f;
+};
+template <typename R>
+static EpisodeStep<R> episode_step(const EpisodeCall<R>& e) {
+  if (e.plant == nullptr) return {e.d->dynamics_kind, e.d->has_f, e.p->dyn, e.F, e.f};
+  return {e.plant->kind, e.plant->has_f, e.plant->dyn, e.F_plant, e.f_plant};
+}
+
+// a plant record against the staged dims: LinDx at those dims, or a known kind (its passthrough kind too) whose own
+// (n, m) are exactly dims' (n, m)
+static int plant_check(const mpcb200_dims* d, const mpcb200_plant* pl) {
+  if (pl->kind == DYN_LINEAR) return MPCB200_OK;
+  int n = 0, m = 0;
+  if (!dyn_kind_dims(pl->kind, n, m) || n != d->n || m != d->m) return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
 
 // the solve of every control step: the caller's problem from the state and warm-start buffers, its best iterate in
 // the workspace
@@ -799,6 +824,12 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
     return MPCB200_ERR_NULL_POINTER;
   if (e.d->T < 3 || e.n_steps < 1) return MPCB200_ERR_BAD_DIMS;     // the warm-start shift reads u[T-3]
   if ((e.plan_x == nullptr) != (e.plan_u == nullptr)) return MPCB200_ERR_NULL_POINTER;
+  if (e.plant != nullptr) {
+    rc = plant_check(e.d, e.plant);
+    if (rc) return rc;
+    if (e.plant->kind == DYN_LINEAR && (e.F_plant == nullptr || (e.plant->has_f && e.f_plant == nullptr)))
+      return MPCB200_ERR_NULL_POINTER;
+  }
   const EpisodeLayout l = episode_layout(e.d, sizeof(R), knob);
   if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
@@ -828,20 +859,26 @@ static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, con
   rc = open_while(os, es, handle);
   if (rc) return rc;
   rc = ilqr_record<R>(es, bs, q, knob);
-  // the model step from the solve's best controls, by the launchers the solve's rollout uses, at T = 2
-  if (rc == 0 && d->dynamics_kind == DYN_LINEAR) {
+  // the model step (the plant's, where the call names one) from the solve's best controls, by the launchers the
+  // solve's rollout uses, at T = 2
+  const EpisodeStep<R> s = episode_step(e);
+  if (rc == 0 && s.kind == DYN_LINEAR) {
     mpcb200_dims d2 = *d;
     d2.T = 2;
     d2.F_T = 1;
-    rc = rollout_impl<R>(&d2, e.F, e.f, state, q.best_u, traj, knob, es);
+    if (e.plant != nullptr) {         // the plant's slice 0, dense
+      d2.has_f = s.has_f;
+      d2.F_tstride = d2.f_tstride = 0;
+    }
+    rc = rollout_impl<R>(&d2, s.F, s.f, state, q.best_u, traj, knob, es);
   } else if (rc == 0) {
-    rc = dyn_impl<R>(false, d->dynamics_kind, e.p->dyn, B, 2, state, q.best_u, traj, nullptr, nullptr, es);
+    rc = dyn_impl<R>(false, s.kind, s.dyn, B, 2, state, q.best_u, traj, nullptr, nullptr, es);
   }
   if (rc == 0 && e.plan_x != nullptr)
     rc = counted(episode_launch_plans<R>(B, T, N, M, q.best_x, q.best_u, e.plan_x, e.plan_u, ep, es));
   if (rc == 0)
     rc = counted(episode_launch_advance<R>(B, T, N, M, e.o->m_ref, e.n_steps, traj, q.best_u, q.best_costs, q.info,
-                                           state, warm, e.xs, e.us, e.costs, e.info, ep, handle, es));
+                                           e.w, state, warm, e.xs, e.us, e.costs, e.info, ep, handle, es));
   cudaGraph_t body = nullptr;
   if (cudaStreamEndCapture(es, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
   if (rc == 0 && cudaMemcpyAsync(e.u_next, warm, (size_t)T * B * M * sizeof(R), cudaMemcpyDeviceToDevice, os) !=
@@ -889,11 +926,13 @@ struct EpGradLayout {                 // workspace carve-up (byte offsets, every
   size_t adj, adj_bytes, stage_x, stage_u, dl_dx, dl_du, gx, theta, dxk, dCk, dck, dFk, dfk, Fk, fk, first, second,
       state, total;
 };
-static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob) {
+// step_kind: the kind of the step whose parameter part the stage writes (the plant's; -1: the model's)
+static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob, int step_kind = -1) {
   EpGradLayout l;
   l.da = epgrad_adjoint_dims(d);
   const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m, TB = T * B, T1B = (T - 1) * B;
   const size_t NP = epgrad_nparams(d->dynamics_kind);
+  const size_t NP_step = step_kind < 0 ? NP : (size_t)epgrad_nparams(step_kind);
   const bool known = d->dynamics_kind != DYN_LINEAR;
   size_t o = 0;
   l.adj_bytes = adj_layout(&l.da, sz, knob).total;
@@ -903,7 +942,7 @@ static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob) {
   l.dl_dx = o;    o += up256(TB * n * sz);
   l.dl_du = o;    o += up256(TB * m * sz);
   l.gx = o;       o += up256(B * n * sz);
-  l.theta = o;    o += up256(B * NP * sz);
+  l.theta = o;    o += up256(B * NP_step * sz);
   l.dxk = o;      o += up256(B * n * sz);
   l.dCk = o;      o += up256(TB * p * p * sz);
   l.dck = o;      o += up256(TB * p * sz);
@@ -933,7 +972,30 @@ struct EpGradCall {
   size_t workspace_bytes;
   bool slew = false;          // the slew entry: the augmented problem, with the first n_prev states detached
   int n_prev = 0;
+  // mpcb200_episode_backward_plant_*: the plant that stepped the loop, and its own outputs (EpPlantArgs)
+  const mpcb200_plant* plant = nullptr;
+  const R* F_plant = nullptr;
+  R *dF_plant = nullptr, *df_plant = nullptr, *dtheta_plant = nullptr, *dw = nullptr;
 };
+
+// the plant entry's own checks: plant_check, a passthrough kind exactly under a slew-rate penalty (n_prev its
+// n_ctrl), and the outputs its kind writes
+template <typename R>
+static int epgrad_plant_check(const EpGradCall<R>& q) {
+  const mpcb200_plant* pl = q.plant;
+  int rc = plant_check(q.d, pl);
+  if (rc) return rc;
+  if (pl->kind == DYN_LINEAR) {
+    if (q.F_plant == nullptr || q.dF_plant == nullptr || (pl->has_f && q.df_plant == nullptr))
+      return MPCB200_ERR_NULL_POINTER;
+    return MPCB200_OK;
+  }
+  int n = 0, m = 0;
+  dyn_kind_dims(pl->kind & ~DYN_CTRL_PASSTHROUGH, n, m);
+  const bool through = (pl->kind & DYN_CTRL_PASSTHROUGH) != 0;
+  if (through != (q.n_prev > 0) || (through && q.n_prev != m)) return MPCB200_ERR_BAD_DIMS;
+  return q.dtheta_plant == nullptr ? MPCB200_ERR_NULL_POINTER : MPCB200_OK;
+}
 
 // the slew entry's own dims checks: 1 <= n_prev <= m and n_prev < n; a known system is its passthrough kind at its
 // dynamics-only shape, with n_prev its n_ctrl (the systems themselves belong to mpcb200_episode_backward_*)
@@ -967,7 +1029,11 @@ static int epgrad_check(const EpGradCall<R>& q, int knob) {
     if (q.F == nullptr || q.dF == nullptr) return MPCB200_ERR_NULL_POINTER;
     if (d->has_f && q.df == nullptr) return MPCB200_ERR_NULL_POINTER;
   }
-  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob);
+  if (q.plant != nullptr) {
+    rc = epgrad_plant_check(q);
+    if (rc) return rc;
+  }
+  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
   if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
@@ -978,7 +1044,7 @@ static int epgrad_check(const EpGradCall<R>& q, int knob) {
 template <typename R>
 static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, int knob) {
   const mpcb200_dims* d = q.d;
-  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob);
+  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
   char* ws = (char*)q.workspace;
   const bool known = d->dynamics_kind != DYN_LINEAR;
   const int B = d->B, T = d->T;
@@ -1005,13 +1071,29 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   a.dF = known ? nullptr : q.dF; a.df = known || !d->has_f ? nullptr : q.df;
   a.dtheta = known ? q.dtheta : nullptr;
   a.st = (EpGradState*)(ws + l.state);
+  // the stage runs on the plant: a copy of `a` with its kind, parameters, F and parameter-part outputs
+  EpGradArgs<R> as = a;
+  EpPlantArgs<R> pl;
+  std::memset(&pl, 0, sizeof(pl));
+  if (q.plant != nullptr) {
+    const bool pknown = q.plant->kind != DYN_LINEAR;
+    as.kind = q.plant->kind; as.has_f = q.plant->has_f; as.NP = epgrad_nparams(q.plant->kind);
+    for (int i = 0; i < 8; ++i) as.dp.p[i] = q.plant->dyn[i];
+    as.F = pknown ? nullptr : q.F_plant;
+    as.dF = pknown ? nullptr : q.dF_plant;
+    as.df = pknown || !q.plant->has_f ? nullptr : q.df_plant;
+    as.theta_step = pknown ? (R*)(ws + l.theta) : nullptr;
+    pl.kind = as.kind; pl.has_f = as.has_f; pl.NP = as.NP; pl.theta_step = as.theta_step;
+    pl.dF = as.dF; pl.df = as.df; pl.dtheta = pknown ? q.dtheta_plant : nullptr; pl.dw = q.dw;
+  }
+  const EpPlantArgs<R>* plp = q.plant != nullptr ? &pl : nullptr;
   cudaGraphConditionalHandle handle;
   int rc = while_handle(os, &handle);
   if (rc) return rc;
-  if (counted(epgrad_launch_init<R>(a, q.n_prev, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
+  if (counted(epgrad_launch_init<R>(a, q.n_prev, plp, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
   rc = open_while(os, bs, handle);
   if (rc) return rc;
-  rc = counted(epgrad_launch_stage<R>(a, bs));
+  rc = counted(epgrad_launch_stage<R>(as, bs));
   const R* F = q.F;
   if (rc == 0 && known) {
     F = (const R*)(ws + l.Fk);
@@ -1030,7 +1112,7 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
     v.x = a.stage_x; v.u = a.stage_u; v.dF = dFk; v.df = dfk; v.first = first; v.second = second;
     rc = counted(epgrad_launch_vjp_passthrough<R>(v, bs));
   }
-  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, q.n_prev, handle, bs));
+  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, q.n_prev, plp, handle, bs));
   cudaGraph_t body = nullptr;
   if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
   return rc;
@@ -1269,6 +1351,51 @@ int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_pa
                               dl_dus, dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, true, n_prev},
                              stream);
 }
+
+#define MPCB200_EPISODE_PLANT(SUF, R)                                                                              \
+  int mpcb200_episode_plant_##SUF(const mpcb200_dims* dims, const mpcb200_params* params,                          \
+                                  const mpcb200_ilqr_opts* opts, const mpcb200_plant* plant, int32_t n_steps,      \
+                                  const R* C, const R* c, const R* F, const R* f, const R* F_plant,                \
+                                  const R* f_plant, const R* w, const R* x_init, const R* u_init, const R* u_lower, \
+                                  const R* u_upper, const uint8_t* u_zero_I, R* xs, R* us, R* costs,               \
+                                  int32_t* info, R* u_next, R* plan_x, R* plan_u, void* workspace,                 \
+                                  size_t workspace_bytes, void* stream) {                                          \
+    if (plant == nullptr) return MPCB200_ERR_NULL_POINTER;                                                         \
+    EpisodeCall<R> e = {dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs, us, \
+                        costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u, plant, F_plant, f_plant, w}; \
+    return episode_impl<R>(e, stream);                                                                             \
+  }
+MPCB200_EPISODE_PLANT(f32, float)
+MPCB200_EPISODE_PLANT(f64, double)
+#undef MPCB200_EPISODE_PLANT
+
+size_t mpcb200_episode_backward_plant_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev,
+                                                      const mpcb200_plant* plant, int32_t elem_size) {
+  if (dims == nullptr || plant == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8))
+    return 0;
+  if (n_prev != 0 ? !slew_dims_ok(dims, n_prev)
+                  : dims->dynamics_kind != DYN_LINEAR && (dyn_nparams(dims->dynamics_kind) == 0 || !known_shape_ok(dims)))
+    return 0;
+  if (plant_check(dims, plant) != 0) return 0;
+  return epgrad_layout(dims, (size_t)elem_size, kernel_knob(), plant->kind).total;
+}
+#define MPCB200_EPISODE_BACKWARD_PLANT(SUF, R)                                                                     \
+  int mpcb200_episode_backward_plant_##SUF(                                                                        \
+      const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_plant* plant, int32_t n_steps,         \
+      int32_t n_prev, const R* C, const R* c, const R* F, const R* F_plant, const R* u_lower, const R* u_upper,    \
+      const R* xs, const R* us, const R* plan_x, const R* plan_u, const R* dl_dxs, const R* dl_dus, R* dx_init,    \
+      R* dC, R* dc, R* dF, R* df, R* dtheta, R* dF_plant, R* df_plant, R* dtheta_plant, R* dw, void* workspace,    \
+      size_t workspace_bytes, void* stream) {                                                                      \
+    if (plant == nullptr) return MPCB200_ERR_NULL_POINTER;                                                         \
+    if (n_prev < 0) return MPCB200_ERR_BAD_DIMS;                                                                   \
+    EpGradCall<R> q = {dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,   \
+                       dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, n_prev > 0, n_prev, plant,     \
+                       F_plant, dF_plant, df_plant, dtheta_plant, dw};                                             \
+    return epgrad_impl<R>(q, stream);                                                                              \
+  }
+MPCB200_EPISODE_BACKWARD_PLANT(f32, float)
+MPCB200_EPISODE_BACKWARD_PLANT(f64, double)
+#undef MPCB200_EPISODE_BACKWARD_PLANT
 
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }
 

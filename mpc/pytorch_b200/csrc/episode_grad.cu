@@ -28,14 +28,27 @@ __global__ void __launch_bounds__(256) fill_zero_kernel(size_t n, R* __restrict_
 }
 
 // g = dl_dxs[n_steps]; the accumulators and the adjoint's incoming gradients zeroed; k = n_steps - 1; the loop's
-// handle set to 1.  DETACH (a slew-rate episode): g's first n_prev entries, the previous control, are 0
-template <typename R, bool DETACH>
-__device__ __forceinline__ void epgrad_init_body(const EpGradArgs<R>& a, int n_prev,
+// handle set to 1.  DETACH (a slew-rate episode): g's first n_prev entries, the previous control, are 0.  PLANT:
+// the plant's accumulators zeroed too, and dw[n_steps-1] = g
+template <typename R, bool DETACH, bool PLANT>
+__device__ __forceinline__ void epgrad_init_body(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>& pl,
                                                  cudaGraphConditionalHandle handle) {
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
-  for (size_t i = i0; i < B * N; i += step)
-    a.g[i] = DETACH && i % N < (size_t)n_prev ? R(0) : a.dl_dxs[(size_t)a.n_steps * B * N + i];
+  for (size_t i = i0; i < B * N; i += step) {
+    const R v = DETACH && i % N < (size_t)n_prev ? R(0) : a.dl_dxs[(size_t)a.n_steps * B * N + i];
+    a.g[i] = v;
+    if (PLANT && pl.dw != nullptr) pl.dw[(size_t)(a.n_steps - 1) * B * N + i] = v;
+  }
+  if (PLANT) {
+    if (pl.kind == DYN_LINEAR) {
+      for (size_t i = i0; i < B * N * P; i += step) pl.dF[i] = R(0);
+      if (pl.has_f)
+        for (size_t i = i0; i < B * N; i += step) pl.df[i] = R(0);
+    } else {
+      for (size_t i = i0; i < B * pl.NP; i += step) pl.dtheta[i] = R(0);
+    }
+  }
   for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] = R(0);
   for (size_t i = i0; i < T * B * P; i += step) a.dc[i] = R(0);
   for (size_t i = i0; i < T * B * N; i += step) a.dl_dx[i] = R(0);
@@ -54,12 +67,18 @@ __device__ __forceinline__ void epgrad_init_body(const EpGradArgs<R>& a, int n_p
 }
 template <typename R>
 __global__ void __launch_bounds__(256) epgrad_init_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
-  epgrad_init_body<R, false>(a, 0, handle);
+  epgrad_init_body<R, false, false>(a, 0, EpPlantArgs<R>{}, handle);
 }
 template <typename R>
 __global__ void __launch_bounds__(256)
 epgrad_init_detach_kernel(const EpGradArgs<R> a, int n_prev, cudaGraphConditionalHandle handle) {
-  epgrad_init_body<R, true>(a, n_prev, handle);
+  epgrad_init_body<R, true, false>(a, n_prev, EpPlantArgs<R>{}, handle);
+}
+template <typename R>
+__global__ void __launch_bounds__(256)
+epgrad_init_plant_kernel(const EpGradArgs<R> a, const EpPlantArgs<R> pl, int n_prev,
+                         cudaGraphConditionalHandle handle) {
+  epgrad_init_body<R, true, true>(a, n_prev, pl, handle);
 }
 
 // the plan of step k into the fixed buffers the body's launchers read
@@ -155,14 +174,20 @@ __global__ void __launch_bounds__(256) epgrad_stage_known_kernel(const EpGradArg
 // g = dl_dxs[k] + R^T g + dx_init_k; dC, dc (LinDx: dF, df) += the adjoint's; a known system: dtheta[b] +=
 // theta_step[b] + sum_t (first + second)[t, b] in t order.  The last block to finish counts k down and ends the
 // loop after k = 0: every block has read st->k by then.  DETACH: g's first n_prev entries are 0, as in init.
-template <typename R, bool DETACH>
-__device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_prev,
+// PLANT: theta_step is the plant's and goes into the plant's dtheta, not into the model's; dw[k-1] = g (k > 0).
+template <typename R, bool DETACH, bool PLANT>
+__device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>& pl,
                                                   cudaGraphConditionalHandle handle) {
   const int k = a.st->k;
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
-  for (size_t i = i0; i < B * N; i += step)
-    a.g[i] = DETACH && i % N < (size_t)n_prev ? R(0) : a.dl_dxs[(size_t)k * B * N + i] + a.gx[i] + a.dx_k[i];
+  for (size_t i = i0; i < B * N; i += step) {
+    const R v = DETACH && i % N < (size_t)n_prev ? R(0) : a.dl_dxs[(size_t)k * B * N + i] + a.gx[i] + a.dx_k[i];
+    a.g[i] = v;
+    if (PLANT && pl.dw != nullptr && k > 0) pl.dw[(size_t)(k - 1) * B * N + i] = v;
+  }
+  if (PLANT && pl.kind != DYN_LINEAR)
+    for (size_t i = i0; i < B * pl.NP; i += step) pl.dtheta[i] += pl.theta_step[i];
   for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] += a.dC_k[i];
   for (size_t i = i0; i < T * B * P; i += step) a.dc[i] += a.dc_k[i];
   if (a.kind == DYN_LINEAR) {
@@ -173,7 +198,7 @@ __device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_
     const size_t NP = a.NP;
     for (size_t i = i0; i < B * NP; i += step) {
       const size_t b = i / NP, p = i % NP;
-      R acc = a.dtheta[i] + a.theta_step[i];
+      R acc = PLANT ? a.dtheta[i] : a.dtheta[i] + a.theta_step[i];
       for (size_t t = 0; t + 1 < T; ++t) acc += a.first[(t * B + b) * NP + p] + a.second[(t * B + b) * NP + p];
       a.dtheta[i] = acc;
     }
@@ -190,12 +215,18 @@ __device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_
 }
 template <typename R>
 __global__ void __launch_bounds__(256) epgrad_accum_kernel(const EpGradArgs<R> a, cudaGraphConditionalHandle handle) {
-  epgrad_accum_body<R, false>(a, 0, handle);
+  epgrad_accum_body<R, false, false>(a, 0, EpPlantArgs<R>{}, handle);
 }
 template <typename R>
 __global__ void __launch_bounds__(256)
 epgrad_accum_detach_kernel(const EpGradArgs<R> a, int n_prev, cudaGraphConditionalHandle handle) {
-  epgrad_accum_body<R, true>(a, n_prev, handle);
+  epgrad_accum_body<R, true, false>(a, n_prev, EpPlantArgs<R>{}, handle);
+}
+template <typename R>
+__global__ void __launch_bounds__(256)
+epgrad_accum_plant_kernel(const EpGradArgs<R> a, const EpPlantArgs<R> pl, int n_prev,
+                          cudaGraphConditionalHandle handle) {
+  epgrad_accum_body<R, true, true>(a, n_prev, pl, handle);
 }
 
 template <typename R>
@@ -221,8 +252,11 @@ static size_t epgrad_items(const EpGradArgs<R>& a) {
 }
 
 template <typename R>
-int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream) {
-  if (n_prev == 0) epgrad_init_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl, cudaGraphConditionalHandle handle,
+                       cudaStream_t stream) {
+  if (pl != nullptr)
+    epgrad_init_plant_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, *pl, n_prev, handle);
+  else if (n_prev == 0) epgrad_init_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
   else epgrad_init_detach_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, n_prev, handle);
   return launched();
 }
@@ -247,8 +281,11 @@ int epgrad_launch_stage(const EpGradArgs<R>& a, cudaStream_t stream) {
 }
 
 template <typename R>
-int epgrad_launch_accum(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream) {
-  if (n_prev == 0) epgrad_accum_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
+int epgrad_launch_accum(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl,
+                        cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  if (pl != nullptr)
+    epgrad_accum_plant_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, *pl, n_prev, handle);
+  else if (n_prev == 0) epgrad_accum_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
   else epgrad_accum_detach_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, n_prev, handle);
   return launched();
 }
@@ -275,9 +312,11 @@ int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream) {
   template int episode_launch_plans<R>(int, int, int, int, const R*, const R*, R*, R*, const EpisodeState*,        \
                                        cudaStream_t);                                                              \
   template int launch_fill_zero<R>(size_t, R*, cudaStream_t);                                                      \
-  template int epgrad_launch_init<R>(const EpGradArgs<R>&, int, cudaGraphConditionalHandle, cudaStream_t);         \
+  template int epgrad_launch_init<R>(const EpGradArgs<R>&, int, const EpPlantArgs<R>*, cudaGraphConditionalHandle, \
+                                     cudaStream_t);                                                                \
   template int epgrad_launch_stage<R>(const EpGradArgs<R>&, cudaStream_t);                                         \
-  template int epgrad_launch_accum<R>(const EpGradArgs<R>&, int, cudaGraphConditionalHandle, cudaStream_t);        \
+  template int epgrad_launch_accum<R>(const EpGradArgs<R>&, int, const EpPlantArgs<R>*,                            \
+                                      cudaGraphConditionalHandle, cudaStream_t);                                   \
   template int epgrad_launch_vjp_passthrough<R>(const DynVjpArgs&, cudaStream_t);
 MPCB200_EPGRAD_INST(float)
 MPCB200_EPGRAD_INST(double)

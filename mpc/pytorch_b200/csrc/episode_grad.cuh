@@ -15,6 +15,10 @@
 // [u_{k-1}; x_k] (LinDx, or a known system's passthrough kind) with the previous control detached, as the reference
 // detaches prev_ctrl: the *_detach_kernel forms of init and accumulate set g's first n_prev entries to 0, so no
 // gradient flows into them and the passthrough row of the model step carries nothing back.
+// An episode closed on a plant other than the model, x_{k+1} = plant(x_k, u_k) + w_k
+// (mpcb200_episode_backward_plant_*): step a. runs on the plant (its kind, dp, F; its dF, df, theta_step), and the
+// *_plant_kernel forms of init and accumulate zero and sum the plant's own accumulators, keep theta_step out of the
+// model's dtheta, and write dw[k] = g.  They apply the detach rule too, with n_prev = 0 meaning none.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,17 +49,31 @@ struct EpGradArgs {
   EpGradState* st;
 };
 
+// The plant's side of a sweep (mpcb200_episode_backward_plant_*): the stage kernel runs on a copy of EpGradArgs with
+// the plant's kind, dp, F, dF, df and theta_step, and the *_plant_kernel forms of init and accumulate read this.
+template <typename R>
+struct EpPlantArgs {
+  int kind, has_f, NP;    // the plant's kind, whether its f is given, its parameter count (0 for LinDx)
+  const R* theta_step;    // the stage's parameter part [B, NP] (the plant's)
+  R *dF, *df;             // LinDx plant: slice 0 of its dF [B, N, N+M], df [B, N] (the stage adds g z^T, g)
+  R* dtheta;              // known plant: [B, NP], sum over k of theta_step
+  R* dw;                  // dL/dw [n_steps, B, N] (dw[k] = dL/dx_{k+1}), or NULL
+};
+
 // Launchers (episode_grad.cu), instantiated for float and double; 0 or MPCB200_ERR_LAUNCH.
 template <typename R>
 int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
                          const EpisodeState* ep, cudaStream_t stream);
-// n_prev > 0 (a slew-rate episode, mpcb200_episode_backward_slew_*): the detach rule, g[:, :n_prev] = 0
+// n_prev > 0 (a slew-rate episode, mpcb200_episode_backward_slew_*): the detach rule, g[:, :n_prev] = 0.
+// pl non-NULL (mpcb200_episode_backward_plant_*): the plant forms, which also take n_prev = 0
 template <typename R>
-int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream);
+int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl, cudaGraphConditionalHandle handle,
+                       cudaStream_t stream);
 template <typename R>
 int epgrad_launch_stage(const EpGradArgs<R>& a, cudaStream_t stream);
 template <typename R>
-int epgrad_launch_accum(const EpGradArgs<R>& a, int n_prev, cudaGraphConditionalHandle handle, cudaStream_t stream);
+int epgrad_launch_accum(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl,
+                        cudaGraphConditionalHandle handle, cudaStream_t stream);
 template <typename R>
 int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream);
 template <typename R>

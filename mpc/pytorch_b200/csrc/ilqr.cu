@@ -28,11 +28,17 @@ int episode_launch_init(size_t n_x, size_t n_u, const R* x_init, const R* u_init
 
 template <typename R>
 int episode_launch_advance(int B, int T, int N, int M, int m_ref, int n_steps, const R* traj, const R* best_u,
-                           const R* best_costs, const int32_t* info, R* state, R* warm, R* xs, R* us, R* costs,
-                           int32_t* info_out, EpisodeState* ep, cudaGraphConditionalHandle handle,
+                           const R* best_costs, const int32_t* info, const R* w, R* state, R* warm, R* xs, R* us,
+                           R* costs, int32_t* info_out, EpisodeState* ep, cudaGraphConditionalHandle handle,
                            cudaStream_t stream) {
-  episode_advance_kernel<R><<<ilqr_grid((size_t)T * B * (N > M ? N : M)), 256, 0, stream>>>(
-      B, T, N, M, m_ref, n_steps, traj, best_u, best_costs, info, state, warm, xs, us, costs, info_out, ep, handle);
+  const unsigned grid = ilqr_grid((size_t)T * B * (N > M ? N : M));
+  if (w == nullptr)
+    episode_advance_kernel<R><<<grid, 256, 0, stream>>>(B, T, N, M, m_ref, n_steps, traj, best_u, best_costs, info,
+                                                        state, warm, xs, us, costs, info_out, ep, handle);
+  else
+    episode_advance_disturbed_kernel<R><<<grid, 256, 0, stream>>>(B, T, N, M, m_ref, n_steps, traj, best_u,
+                                                                  best_costs, info, w, state, warm, xs, us, costs,
+                                                                  info_out, ep, handle);
   return launched();
 }
 
@@ -61,7 +67,7 @@ int ilqr_launch_stop(int B, int lqr_iter, int not_improved_lim, double eps, cons
   template int episode_launch_init<R>(size_t, size_t, const R*, const R*, R*, R*, R*, EpisodeState*,              \
                                       cudaGraphConditionalHandle, cudaStream_t);                                   \
   template int episode_launch_advance<R>(int, int, int, int, int, int, const R*, const R*, const R*,              \
-                                         const int32_t*, R*, R*, R*, R*, R*, int32_t*, EpisodeState*,              \
+                                         const int32_t*, const R*, R*, R*, R*, R*, R*, int32_t*, EpisodeState*,    \
                                          cudaGraphConditionalHandle, cudaStream_t);                                \
   template int ilqr_launch_track<R>(int, int, int, int, int, R, const R*, const R*, const R*, const R*,            \
                                     const int32_t*, const R*, R*, R*, R*, R*, uint8_t*, const IlqrState*,          \

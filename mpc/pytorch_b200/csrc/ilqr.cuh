@@ -170,14 +170,15 @@ episode_init_kernel(size_t n_x, size_t n_u, const R* __restrict__ x_init, const 
 // x_init (state) = traj[1]; the next warm start warm[t] = best_u[t+1] for t < T-2, best_u[T-2] at t = T-2, 0 at
 // t = T-1 (cat(u[1:], 0), then w[-2] = w[-3]), with controls past m_ref at 0 as a freshly padded u_init has them;
 // costs[k] = best_costs, info_out[k] = info.  The last block to finish advances ep->step and ends the episode's
-// loop after n_steps control steps: every block has read ep->step by then.
-template <typename R>
-__global__ void __launch_bounds__(256)
-episode_advance_kernel(int B, int T, int N, int M, int m_ref, int n_steps, const R* __restrict__ traj,
-                       const R* __restrict__ best_u, const R* __restrict__ best_costs, const int32_t* __restrict__ info,
-                       R* __restrict__ state, R* __restrict__ warm, R* __restrict__ xs, R* __restrict__ us,
-                       R* __restrict__ costs, int32_t* __restrict__ info_out, EpisodeState* __restrict__ ep,
-                       cudaGraphConditionalHandle handle) {
+// loop after n_steps control steps: every block has read ep->step by then.  DISTURB (mpcb200_episode_plant_*):
+// traj[1] + w[k] instead of traj[1], w [n_steps, B, N] staged at the problem's shape.
+template <typename R, bool DISTURB>
+__device__ __forceinline__ void
+episode_advance_body(int B, int T, int N, int M, int m_ref, int n_steps, const R* __restrict__ traj,
+                     const R* __restrict__ best_u, const R* __restrict__ best_costs, const int32_t* __restrict__ info,
+                     const R* __restrict__ w, R* __restrict__ state, R* __restrict__ warm, R* __restrict__ xs,
+                     R* __restrict__ us, R* __restrict__ costs, int32_t* __restrict__ info_out,
+                     EpisodeState* __restrict__ ep, cudaGraphConditionalHandle handle) {
   const int k = ep->step;
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t BM = (size_t)B * M, BN = (size_t)B * N;
@@ -189,7 +190,7 @@ episode_advance_kernel(int B, int T, int N, int M, int m_ref, int n_steps, const
   }
   for (size_t i = i0; i < BM; i += step) us[(size_t)k * BM + i] = best_u[i];
   for (size_t i = i0; i < BN; i += step) {
-    const R v = traj[BN + i];
+    const R v = DISTURB ? traj[BN + i] + w[(size_t)k * BN + i] : traj[BN + i];
     state[i] = v;
     xs[(size_t)(k + 1) * BN + i] = v;
   }
@@ -208,6 +209,27 @@ episode_advance_kernel(int B, int T, int N, int M, int m_ref, int n_steps, const
     }
   }
 }
+template <typename R>
+__global__ void __launch_bounds__(256)
+episode_advance_kernel(int B, int T, int N, int M, int m_ref, int n_steps, const R* __restrict__ traj,
+                       const R* __restrict__ best_u, const R* __restrict__ best_costs, const int32_t* __restrict__ info,
+                       R* __restrict__ state, R* __restrict__ warm, R* __restrict__ xs, R* __restrict__ us,
+                       R* __restrict__ costs, int32_t* __restrict__ info_out, EpisodeState* __restrict__ ep,
+                       cudaGraphConditionalHandle handle) {
+  episode_advance_body<R, false>(B, T, N, M, m_ref, n_steps, traj, best_u, best_costs, info, nullptr, state, warm, xs,
+                                 us, costs, info_out, ep, handle);
+}
+template <typename R>
+__global__ void __launch_bounds__(256)
+episode_advance_disturbed_kernel(int B, int T, int N, int M, int m_ref, int n_steps, const R* __restrict__ traj,
+                                 const R* __restrict__ best_u, const R* __restrict__ best_costs,
+                                 const int32_t* __restrict__ info, const R* __restrict__ w, R* __restrict__ state,
+                                 R* __restrict__ warm, R* __restrict__ xs, R* __restrict__ us, R* __restrict__ costs,
+                                 int32_t* __restrict__ info_out, EpisodeState* __restrict__ ep,
+                                 cudaGraphConditionalHandle handle) {
+  episode_advance_body<R, true>(B, T, N, M, m_ref, n_steps, traj, best_u, best_costs, info, w, state, warm, xs, us,
+                                costs, info_out, ep, handle);
+}
 
 // Launchers (ilqr.cu), instantiated for float and double; 0 or MPCB200_ERR_LAUNCH.
 template <typename R>
@@ -216,10 +238,11 @@ int ilqr_launch_init(size_t n_u, const R* u_init, R* u, IlqrState* st, int32_t* 
 template <typename R>
 int episode_launch_init(size_t n_x, size_t n_u, const R* x_init, const R* u_init, R* state, R* xs0, R* warm,
                         EpisodeState* ep, cudaGraphConditionalHandle handle, cudaStream_t stream);
+// w NULL: episode_advance_kernel; otherwise its disturbed form
 template <typename R>
 int episode_launch_advance(int B, int T, int N, int M, int m_ref, int n_steps, const R* traj, const R* best_u,
-                           const R* best_costs, const int32_t* info, R* state, R* warm, R* xs, R* us, R* costs,
-                           int32_t* info_out, EpisodeState* ep, cudaGraphConditionalHandle handle,
+                           const R* best_costs, const int32_t* info, const R* w, R* state, R* warm, R* xs, R* us,
+                           R* costs, int32_t* info_out, EpisodeState* ep, cudaGraphConditionalHandle handle,
                            cudaStream_t stream);
 template <typename R>
 int ilqr_launch_track(int B, int T, int N, int M, int m_ref, R best_cost_eps, const R* new_x, const R* new_u,

@@ -255,8 +255,41 @@ class _Pad:
         return F[..., : self.n, self.idx] if self.active and F is not None else F
 
 
-# n_prev: an episode's slew-rate augmentation, the leading states that hold the previous control (0: none)
-_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev", defaults=(0,))
+# n_prev: an episode's slew-rate augmentation, the leading states that hold the previous control (0: none); plant: the
+# _StagedPlant of an episode closed on a plant other than the model (None: the model steps it)
+_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev plant",
+                                  defaults=(0, None))
+# rec: the mpcb200_plant record; F, f: a LinDx plant's slice 0 at the problem's (padded) sizes [B, N, N+M], [B, N]
+# (f None without one); disturbed: the episode added w
+_StagedPlant = collections.namedtuple("_StagedPlant", "rec F f disturbed")
+
+
+def _stage_plant(pad, plant, dtype, B, n, m):
+    """The plant of episode_raw as the kernels take it (_StagedPlant, without w): (DYN_LINEAR, None, F_p, f_p) with
+    F_p [T', B, n, n+m] and f_p [T', B, n] (or None / empty) of which slice 0 steps, widened like the model (_Pad); or
+    (kind, params, None, None) of a known system (its passthrough kind under a slew-rate penalty), whose own (n, m)
+    must be the staged instance's.  Checked on metadata before anything runs."""
+    kind, params, F_p, f_p = plant
+    rec = _lib.Plant(kind=int(kind))
+    if kind != DYN_LINEAR:
+        if DYN_DIMS.get(kind) != (pad.N, pad.M):
+            raise MpcB200Error(f"a plant of dynamics kind {kind} steps (n_state, n_ctrl) = {DYN_DIMS.get(kind)}, "
+                               f"but the episode runs at {(pad.N, pad.M)}")
+        for i, v in enumerate(params):
+            rec.dyn[i] = float(v)
+        return _StagedPlant(rec, None, None, False)
+    for name, t, shape in (("plant F", F_p, (B, n, n + m)), ("plant f", f_p, (B, n))):
+        if name == "plant F" and t is None:
+            raise MpcB200Error("a LinDx plant needs F")
+        if not _is_empty(t) and (t.dim() != len(shape) + 1 or t.shape[0] < 1 or tuple(t.shape[1:]) != shape):
+            raise MpcB200Error(f"{name}: expected shape (T', {', '.join(map(str, shape))}), got {tuple(t.shape)}")
+    F0 = _dense(F_p[:1], dtype)
+    F0 = (pad.mat_np(F0) if pad.active else F0)[0].contiguous()
+    f0 = None
+    if not _is_empty(f_p):
+        f0 = pad.vec_n(_dense(f_p[0], dtype)).contiguous()
+        rec.has_f = 1
+    return _StagedPlant(rec, F0, f0, False)
 
 
 def _problem(n, m, T, B, dtype, dev, C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None,
@@ -412,7 +445,7 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
 
 def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
-                best_cost_eps=1e-4, dyn=None, keep_plans=False, n_prev=0):
+                best_cost_eps=1e-4, dyn=None, keep_plans=False, n_prev=0, plant=None, w=None):
     """A receding-horizon episode of n_steps control steps in ONE library call (mpcb200_episode_*): each step solves
     the problem from the current state as ilqr_raw does (u_init = the warm start), applies the plan's first control,
     steps the model (LinDx: F[0] [x; u] + f[0]; a known system `dyn`: one step of it) and shifts the warm start
@@ -423,7 +456,11 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     mpcb200_episode_plans_*, and the dict also holds "saved", what episode_backward_raw takes: the staged problem and
     the padded xs, us and each solve's best iterate plan_x [n_steps, T, B, N], plan_u [n_steps, T, B, M].
     n_prev > 0: the problem is a slew-rate penalty's augmented one over [u_{k-1}; x_k] and its first n_prev states
-    are the previous control; the staged problem records it, so episode_backward_raw detaches them."""
+    are the previous control; the staged problem records it, so episode_backward_raw detaches them.
+    plant (mpcb200_episode_plant_*): what steps the loop instead of the model, (DYN_LINEAR, None, F_p, f_p) for a
+    LinDx's t = 0 slice or (kind, params, None, None) for a known system (_stage_plant); w [n_steps, B, n]: added to
+    each step, x_{k+1} = plant(x_k, u_k) + w_k (under a slew-rate penalty its first n_prev entries are the caller's
+    zeros).  Either one takes that entry; the staged problem records the plant for episode_backward_raw."""
     n, m = n_state, n_ctrl
     if T < 3 or n_steps < 1:
         raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
@@ -435,6 +472,17 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
                  max_linesearch_iter, dyn)
     pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
     x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
+    sp = w_ = None
+    if plant is not None or w is not None:
+        if plant is None:                 # the model steps, disturbed
+            plant = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
+        sp = _stage_plant(pad, plant, dtype, B, n, m)
+        if w is not None:
+            if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
+                raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
+                                   f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
+            w_ = pad.vec_n(_dense(w, dtype)).contiguous()
+            sp = sp._replace(disturbed=True)
     opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
                          best_cost_eps=float(best_cost_eps))
     nbytes = _lib.lib().mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
@@ -444,15 +492,22 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
     info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
     u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
-    args = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), ptr_view(s.C),
-            ptr_view(s.c), ptr_view(s.F), ptr_view(s.f), ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper),
-            ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info), ptr(u_next)]
+    head = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), ptr_view(s.C),
+            ptr_view(s.c), ptr_view(s.F), ptr_view(s.f)]
+    tail = [ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper), ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs),
+            ptr(info), ptr(u_next)]
     name = "mpcb200_episode"
+    plan_x = plan_u = None
     if keep_plans:
         name = "mpcb200_episode_plans"
         plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
         plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
-        args += [ptr(plan_x), ptr(plan_u)]
+    if sp is not None:
+        name = "mpcb200_episode_plant"
+        args = head[:3] + [ctypes.byref(sp.rec)] + head[3:] + [ptr(sp.F), ptr(sp.f), ptr(w_)] + tail + \
+            [ptr(plan_x), ptr(plan_u)]
+    else:
+        args = head + tail + ([ptr(plan_x), ptr(plan_u)] if keep_plans else [])
     fn = _lib.entry(name, dtype)
     with _on_device(dev):
         rc = fn(*args, ptr(ws), nbytes, stream_handle(dev))
@@ -461,7 +516,7 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     check(rc, name)
     res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
     if keep_plans:
-        res["saved"] = (s._replace(n_prev=int(n_prev)), n_steps, xs, us, plan_x, plan_u)
+        res["saved"] = (s._replace(n_prev=int(n_prev), plant=sp), n_steps, xs, us, plan_x, plan_u)
     return res
 
 
@@ -473,7 +528,10 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
     system dF = df = None and dtheta [B, NP], one row per problem (the caller sums over b, as DynLinearize does).
     A slew-rate episode (the staged problem's n_prev > 0) runs mpcb200_episode_backward_slew_*: every size is the
     augmented problem's, and the first n_prev states of each augmented state get no gradient (dx_init[:, :n_prev] = 0);
-    the caller crops the gradients to the system's own blocks."""
+    the caller crops the gradients to the system's own blocks.
+    An episode closed on a plant (the staged problem's plant) runs mpcb200_episode_backward_plant_* and returns four
+    more: dF_p [B, n, p] and df_p [B, n] (a LinDx plant's slice 0; df_p None without f), dtheta_p [B, NP_plant] (a
+    known plant) and dw [n_steps, B, n] (None when no w was added); dF, df or dtheta are then the solves' part only."""
     s, n_steps, xs, us, plan_x, plan_u = saved
     pad, dims = s.pad, s.dims
     T, B, N, M = dims.T, dims.B, pad.N, pad.M
@@ -493,6 +551,31 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
         from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_NPARAMS
         dtheta = torch.empty(B, DYN_NPARAMS[kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
     L = _lib.lib()
+    sp = s.plant
+    if sp is not None:
+        from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_NPARAMS
+        pk = sp.rec.kind
+        dF_p = torch.empty(B, N, P, dtype=dtype, device=dev) if pk == DYN_LINEAR else None
+        df_p = torch.empty(B, N, dtype=dtype, device=dev) if pk == DYN_LINEAR and sp.rec.has_f else None
+        dth_p = (torch.empty(B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
+                 if pk != DYN_LINEAR else None)
+        dw = torch.empty(n_steps, B, N, dtype=dtype, device=dev) if sp.disturbed else None
+        name = "mpcb200_episode_backward_plant"
+        nbytes = L.mpcb200_episode_backward_plant_workspace_bytes(ctypes.byref(dims), int(s.n_prev),
+                                                                  ctypes.byref(sp.rec), xs.element_size())
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        fn = _lib.entry(name, dtype)
+        with _on_device(dev):
+            rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(sp.rec), int(n_steps), int(s.n_prev),
+                    ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr(sp.F), ptr(s.u_lower), ptr(s.u_upper), ptr(xs),
+                    ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF),
+                    ptr(df), ptr(dtheta), ptr(dF_p), ptr(df_p), ptr(dth_p), ptr(dw), ptr(ws), nbytes,
+                    stream_handle(dev))
+        check(rc, name)
+        if df is not None and s.f.shape[0] == T:
+            df = torch.cat((df, torch.zeros_like(df[:1])), 0)
+        return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta,
+                pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
     if s.n_prev:
         name = "mpcb200_episode_backward_slew"
         nbytes = L.mpcb200_episode_backward_slew_workspace_bytes(ctypes.byref(dims), int(s.n_prev), xs.element_size())

@@ -229,9 +229,36 @@ static int run_episode_backward_slew() {
   return 0;
 }
 
+// the plant entries' argument checks (they run before anything is launched): a pendulum model on a cartpole plant is
+// refused (the plant steps (5, 1)), and the backward sizes its stage buffer by the five-parameter pendulum plant
+static int run_episode_plant() {
+  mpcb200_dims d = {4, 5, 3, 1, 4, 1, 0, 0, 0, 10, 20, 1, MPCB200_DYN_PENDULUM};
+  mpcb200_params prm = {0.0, 0.0, 0.0, 0.2, {10.0, 1.0, 1.0, 2.0, 0.05}};
+  mpcb200_ilqr_opts opts = {5, 5, 1, 0, 1e-7, 1e-4};
+  mpcb200_plant cart = {MPCB200_DYN_CARTPOLE, 0, {9.8, 1.0, 0.1, 0.5, 100.0, 0.05}};
+  mpcb200_plant full = {MPCB200_DYN_PENDULUM_FULL, 0, {10.0, 1.0, 1.0, 0.3, 0.2, 2.0, 0.05}};
+  const size_t need = mpcb200_episode_backward_plant_workspace_bytes(&d, 0, &full, 4);
+  if (need == 0 || mpcb200_episode_backward_plant_workspace_bytes(&d, 0, &cart, 4) != 0)
+    return printf("episode backward plant workspace %zu\n", need), 1;
+  const size_t fw = mpcb200_episode_workspace_bytes(&d, &opts, 4);
+  Dev<float> buf(1024), ws((need > fw ? need : fw) / sizeof(float) + 64);
+  int32_t* info = (int32_t*)buf.p;
+  float* p = buf.p;
+  int rc = mpcb200_episode_plant_f32(&d, &prm, &opts, &cart, 3, p, p, p, p, p, p, p, p, p, p, p, nullptr, p, p, p, info,
+                                     p, nullptr, nullptr, ws.p, fw, nullptr);
+  if (rc != MPCB200_ERR_BAD_DIMS) return printf("episode plant (cartpole plant) rc=%d\n", rc), 1;
+  full.kind |= MPCB200_DYN_CTRL_PASSTHROUGH;      // a passthrough plant without a slew-rate penalty
+  rc = mpcb200_episode_backward_plant_f32(&d, &prm, &full, 3, 0, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p, p,
+                                          p, p, p, p, ws.p, need, nullptr);
+  if (rc != MPCB200_ERR_BAD_DIMS) return printf("episode backward plant (passthrough) rc=%d\n", rc), 1;
+  printf("episode plant: backward workspace %zu bytes, other-shape and passthrough plants refused\n", need);
+  return 0;
+}
+
 int main() {
   int fails = 0;
   fails += run_episode_backward_slew();
+  fails += run_episode_plant();
   fails += run_pnqp_large(3, 100);
   fails += run_dyn(MPCB200_DYN_CARTPOLE, 37, 9);
   fails += run_dyn(MPCB200_DYN_PENDULUM, 20, 7);
