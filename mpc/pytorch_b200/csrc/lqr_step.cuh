@@ -71,7 +71,8 @@ struct StepCfg {
   static constexpr int EA = 16 / (int)sizeof(R);
   static_assert(P <= 32, "one problem must fit a warp");
   // Lane layout.  By default P lanes own one problem, one column each.  (8, 2) in fp32 uses n lanes: lane j
-  // keeps state column j, and lanes 0, 1 also keep control columns 8, 9 in a second slot.  A warp then holds
+  // keeps state column j, and lanes 0, 1 also keep control columns 8, 9 in a second slot (in the Riccati sweep
+  // the control columns are split by rows instead, XS).  A warp then holds
   // 4 problems instead of 3 for about the same broadcast loads of V and F, and shared memory charges for the
   // bytes delivered to lanes, which bound that kernel (DESIGN.md section 7).  fp64 keeps one column per lane:
   // with the second slot it spilled under the 128-register cap of one-warp CTAs (92 B in PLAIN, 184 B in BOX).
@@ -79,6 +80,12 @@ struct StepCfg {
   static constexpr int LP = STATE_LANES ? N : P;    // lanes per problem
   static constexpr int CPL = (P + LP - 1) / LP;     // column slots per lane; slot s of lane j is column j + s*LP
   static constexpr int PPW = 32 / LP;               // problems per warp
+  // Slots whose columns the Riccati sweep computes one per lane.  With STATE_LANES only slot 0 does: the control
+  // columns are split by rows over the problem's lanes instead (lane j: row j of Q_xu, and row n+ua of Q_uu with q_u[ua]
+  // for the control ua of its slot 1), so no lane runs a whole control column and lanes 2..7 no longer compute a dead
+  // one.  Each element keeps the FMA chain, and the chain order, of the column it belongs to.
+  static constexpr int XS = STATE_LANES ? 1 : CPL;
+  static_assert(!STATE_LANES || M == 2, "the row split keeps the two control columns as one pair");
   // slot sl can hold a state column (compile time: the later slots of the (8, 2) layout hold controls only)
   static constexpr bool x_slot(int sl) { return sl * LP < N; }
   // consumer warps per CTA: the smallest count whose per-time-step spans stay 16-byte aligned for every
@@ -582,11 +589,18 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     // owned columns of C_t; c_back = (C_t tau_bar) + c for the owned rows  (lqr_step.py:289-295)
     Vec<R, P> Qc[CPL];
     R qj[CPL];
+    // STATE_LANES: Q[j, n:n+2] (row j of Q_xu) and Q[cc[1], n:n+2] (the row of Q_uu of the control slot)
+    P2<R> Qxu{}, Quq{};
 #pragma unroll
     for (int sl = 0; sl < CPL; ++sl) {
-      Qc[sl].gather(st + oC + cc[sl], P);
+      if constexpr (!K::STATE_LANES) Qc[sl].gather(st + oC + cc[sl], P);
+      else if (sl == 0) Qc[sl].gather(st + oC + cc[sl], P);
       Vec<R, P> Crow;
       Crow.template load<A_ROW>(st + oC + cc[sl] * P);
+      if constexpr (K::STATE_LANES) {
+        if (sl == 0) Qxu = Crow.p[N / 2];
+        else Quq = Crow.p[N / 2];
+      }
       const R Ct = Crow.dot(tb);
       const R cj = st[oc + cc[sl]];
       const R tbj = st[(isx[sl] ? ox : ou - N) + cc[sl]];
@@ -600,16 +614,29 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     if (t < T - 1) {                            // Q = C + F'VF, q = c_back + F'v  (:66-70)
       Vec<R, N> Fcol[CPL], Wc[CPL];
 #pragma unroll
-      for (int sl = 0; sl < CPL; ++sl) Fcol[sl].gather(st + oF + cc[sl], P);
+      for (int sl = 0; sl < K::XS; ++sl) Fcol[sl].gather(st + oF + cc[sl], P);
+      Vec<R, N> Fuc;                              // STATE_LANES: F[:, cc[1]], for F[:, cc[1]]' v
       {
 #pragma unroll
-        for (int sl = 0; sl < CPL; ++sl) Wc[sl].zero();
+        for (int sl = 0; sl < K::XS; ++sl) Wc[sl].zero();
+        P2<R> Wu{R(0), R(0)};                     // STATE_LANES: W[j, n:n+2]
 #pragma unroll
-        for (int k = 0; k < N; ++k) {             // W[:, c] = V F[:, c]; each V column load feeds CPL columns
+        for (int k = 0; k < N; ++k) {             // W[:, c] = V F[:, c]; each V column load feeds XS columns
           Vec<R, N> Vcol;                         // Vs holds V transposed: row k of Vs == column k of V
           Vcol.template load<EA>(Vs + k * VS);
 #pragma unroll
-          for (int sl = 0; sl < CPL; ++sl) Wc[sl].axpy(Vcol, Fcol[sl].get(k));
+          for (int sl = 0; sl < K::XS; ++sl) Wc[sl].axpy(Vcol, Fcol[sl].get(k));
+          if constexpr (K::STATE_LANES) {         // W[j, n+a] += V[j, k] F[k, n+a]
+            Vec<R, M> Fu;
+            Fu.template load<A_ROW>(st + oF + k * P + N);
+            const R vjk = Vs[k * VS + j];
+            Wu = fma2(P2<R>{vjk, vjk}, Fu.p[0], Wu);
+          }
+        }
+        P2<R> Wk[K::STATE_LANES ? N : 1];         // STATE_LANES: W[k, n:n+2] from lane k
+        if constexpr (K::STATE_LANES) {
+#pragma unroll
+          for (int k = 0; k < N; ++k) Wk[k] = P2<R>{shfl(Wu.x, base + k), shfl(Wu.y, base + k)};
         }
         static_for<0, N>([&](auto kc) {           // Q[:, c] += F' W[:, c]; rows of F are contiguous
           constexpr int k = decltype(kc)::value;
@@ -617,22 +644,40 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
           Vec<R, P> Frow;
           Frow.template load<(AK < A_NP ? AK : A_NP)>(st + oF + k * P);
 #pragma unroll
-          for (int sl = 0; sl < CPL; ++sl) Qc[sl].axpy(Frow, Wc[sl].get(k));
+          for (int sl = 0; sl < K::XS; ++sl) Qc[sl].axpy(Frow, Wc[sl].get(k));
+          if constexpr (K::STATE_LANES) {         // Q[r, n+a] += F[k, r] W[k, n+a] for r = j and r = cc[1]
+            const R fx = Fcol[0].get(k);
+            const R fu = ua[1] == 0 ? Frow.get(N) : Frow.get(N + 1);
+            Fuc.set(k, fu);
+            Qxu = fma2(P2<R>{fx, fx}, Wk[k], Qxu);
+            Quq = fma2(P2<R>{fu, fu}, Wk[k], Quq);
+          }
         });
       }
       Vec<R, N> vv;
       vv.template load<EA>(vs);
 #pragma unroll
-      for (int sl = 0; sl < CPL; ++sl) qj[sl] += Fcol[sl].dot(vv);
+      for (int sl = 0; sl < K::XS; ++sl) qj[sl] += Fcol[sl].dot(vv);
+      if constexpr (K::STATE_LANES) qj[1] += Fuc.dot(vv);
     }
-    // replicate Q_uu, q_u on every lane of the problem (column n+b2 lives in lane (n+b2)%LP, slot (n+b2)/LP)
+    // replicate Q_uu, q_u on every lane of the problem (column n+b2 lives in lane (n+b2)%LP, slot (n+b2)/LP;
+    // STATE_LANES: row n+b1 of Q_uu and q_u[b1] live in lane b1)
     R Quu[M][M], qu[M];
+    if constexpr (K::STATE_LANES) {
 #pragma unroll
-    for (int p2 = 0; p2 < M; ++p2) {
-      const int src = base + (N + p2) % LP;
+      for (int p1 = 0; p1 < M; ++p1) {
+        Quu[p1][0] = shfl(Quq.x, base + p1);
+        Quu[p1][1] = shfl(Quq.y, base + p1);
+        qu[p1] = shfl(qj[1], base + p1);
+      }
+    } else {
 #pragma unroll
-      for (int p1 = 0; p1 < M; ++p1) Quu[p1][p2] = shfl(Qc[(N + p2) / LP].get(N + p1), src);
-      qu[p2] = shfl(qj[(N + p2) / LP], src);
+      for (int p2 = 0; p2 < M; ++p2) {
+        const int src = base + (N + p2) % LP;
+#pragma unroll
+        for (int p1 = 0; p1 < M; ++p1) Quu[p1][p2] = shfl(Qc[(N + p2) / LP].get(N + p1), src);
+        qu[p2] = shfl(qj[(N + p2) / LP], src);
+      }
     }
     // This kernel keeps its own copy of box_control_solve and ldl_control_solve: with the shared ones, ptxas contracts
     // the f64 (8, 2) BOX kernel's multiplies and adds differently, so its outputs are no longer bitwise the same, and
@@ -700,7 +745,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     R Kc[CPL][M];
     R* Kt = a.k_in_smem ? kst + (size_t)t * KT : kst;
 #pragma unroll
-    for (int sl = 0; sl < CPL; ++sl) {
+    for (int sl = 0; sl < K::XS; ++sl) {
       R rhs[M], sol[M];
 #pragma unroll
       for (int q = 0; q < M; ++q) rhs[q] = ((fm >> q) & 1u) ? Qc[sl].get(N + q) : R(0);
@@ -719,6 +764,12 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
         }
       }
     }
+    if constexpr (K::STATE_LANES) {       // every lane publishes its row of Q_xu
+      if (wsl[0]) {
+        Qx[j] = Qxu.x;
+        Qx[VS + j] = Qxu.y;
+      }
+    }
     if (j == 0) {
 #pragma unroll
       for (int q = 0; q < M; ++q) Kt[M * VS + q] = kk[q];
@@ -727,7 +778,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
       const size_t tbo = (size_t)t * B + b;
       if (gKs != nullptr) {
 #pragma unroll
-        for (int sl = 0; sl < CPL; ++sl) {
+        for (int sl = 0; sl < K::XS; ++sl) {
           if (wsl[sl] && isx[sl]) {
 #pragma unroll
             for (int q = 0; q < M; ++q) gKs[(tbo * M + q) * N + cc[sl]] = Kc[sl][q];
@@ -751,7 +802,7 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
     Vec<R, N> Vn[CPL];
     R vn[CPL], G[CPL][M];
 #pragma unroll
-    for (int sl = 0; sl < CPL; ++sl) {
+    for (int sl = 0; sl < K::XS; ++sl) {
 #pragma unroll
       for (int p1 = 0; p1 < M; ++p1) {
         R sacc = Qc[sl].get(N + p1);
@@ -773,14 +824,17 @@ MPCB_DEV void step_consumer(const StepArgs& a, unsigned char* stage_base, uint64
 #pragma unroll
       for (int p2 = 0; p2 < M; ++p2) sacc += Quu[q][p2] * kk[p2];
 #pragma unroll
-      for (int sl = 0; sl < CPL; ++sl) {
+      for (int sl = 0; sl < K::XS; ++sl) {
         Vn[sl].axpy(Qrow, Kc[sl][q]);
         Vn[sl].axpy(Krow, G[sl][q]);
-        vn[sl] += Qx[q * VS + fr[sl]] * kk[q] + Kc[sl][q] * sacc;
+        if constexpr (K::STATE_LANES)            // Q[j, n+q]: this lane's own row of Q_xu
+          vn[sl] += (q == 0 ? Qxu.x : Qxu.y) * kk[q] + Kc[sl][q] * sacc;
+        else
+          vn[sl] += Qx[q * VS + fr[sl]] * kk[q] + Kc[sl][q] * sacc;
       }
     }
 #pragma unroll
-    for (int sl = 0; sl < CPL; ++sl) {
+    for (int sl = 0; sl < K::XS; ++sl) {
       if (wsl[sl] && isx[sl]) {
         Vn[sl].template store<EA>(Vs + cc[sl] * VS);        // column c of V, stored as row c (vector stores)
         vs[cc[sl]] = vn[sl];
