@@ -878,11 +878,14 @@ SWITCH_PLANS = {"generic": ("generic_smem", "generic_ks"), "kreduce": ("generic_
 
 
 @functools.lru_cache(maxsize=None)
-def pick_switch(group, dtype):
+def pick_switch(group, dtype, augmentable=False):
     """(n, m, T*, impls) of the instance whose `group` switch of the loop's step plan comes first, None if no
-    instance has it within ORACLE_TMAX.  Below T* the loop runs SWITCH_PLANS[group][0], from T* on [1]."""
+    instance has it within ORACLE_TMAX.  Below T* the loop runs SWITCH_PLANS[group][0], from T* on [1].
+    augmentable: only instances with n > m, the slew-rate augmented shapes of the systems (n - m, m)."""
     cands = []
     for n, m in INSTANCES:
+        if augmentable and n <= m:
+            continue
         sw = switches(n, m, dtype)
         pair = (n, m) in PAIR_SHAPES
         impls = (None, 1, 2) if pair else (None, 1)
@@ -920,13 +923,19 @@ def _owned(poison, *shape, dtype):
 
 def abi_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5,
-                eps=1e-7, best_cost_eps=1e-4, dyn=None, poison=False):
+                eps=1e-7, best_cost_eps=1e-4, dyn=None, poison=False, n_prev=0, plant=None, w=None,
+                nan_outputs=False):
     """The call step.episode_raw(..., keep_plans=True) makes (mpcb200_episode_plans_*, the problem staged by the same
     step._problem), with caller-owned outputs and workspace.  poison: every workspace byte and every output starts at
-    0xFF, so a kernel that reads an element nothing wrote reads NaN (or info -1).  Returns (res, launches, plan): res
-    as episode_raw's dict, "saved" included, launches the library kernels the call recorded, plan
-    mpcb200_last_step_plan() after it (the step plan of the solve)."""
+    0xFF, so a kernel that reads an element nothing wrote reads NaN (or info -1); nan_outputs: the outputs alone start
+    at 0xFF, so an element the call does not write comes back NaN (or -1).  n_prev: a slew-rate penalty's
+    augmented problem, recorded in the staged problem for abi_episode_backward.  plant ("lin", F_p, f_p) of a LinDx
+    plant (f_p None: none) or (kind, params) of a known one, and w [n_steps, B, n]: the call is
+    mpcb200_episode_plant_*, the plant and w staged as step.episode_raw stages them (plant None with w: the model
+    steps, disturbed).  Returns (res, launches, plan): res as episode_raw's dict, "saved" included, launches the
+    library kernels the call recorded, plan mpcb200_last_step_plan() after it (the step plan of the solve)."""
     from mpc.pytorch_b200 import step as S
+    from mpc.pytorch_b200.dynamics import DYN_LINEAR
     L = _L()
     B = x_init.shape[0]
     dtype = C.dtype
@@ -934,65 +943,179 @@ def abi_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_up
                    max_linesearch_iter, dyn)
     pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
     x0_, u0_ = pad.vec_n(S._dense(x_init, dtype)), pad.vec_m(S._dense(u_init, dtype))
+    sp = w_ = None
+    if plant is not None or w is not None:
+        if plant is None:
+            spec = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
+        elif plant[0] == "lin":
+            spec = (DYN_LINEAR, None, plant[1], plant[2])
+        else:
+            spec = (plant[0], plant[1], None, None)
+        sp = S._stage_plant(pad, spec, dtype, B, n, m)
+        if w is not None:
+            w_ = pad.vec_n(S._dense(w, dtype)).contiguous()
+            sp = sp._replace(disturbed=True)
     opts = L.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
                       best_cost_eps=float(best_cost_eps))
     nbytes = L.lib().mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
     ws = _owned(poison, nbytes, dtype=torch.uint8)
-    xs, us = _owned(poison, n_steps + 1, B, N, dtype=dtype), _owned(poison, n_steps, B, M, dtype=dtype)
-    costs, info = _owned(poison, n_steps, B, dtype=dtype), _owned(poison, n_steps, 2, dtype=torch.int32)
-    u_next = _owned(poison, T, B, M, dtype=dtype)
-    plan_x, plan_u = _owned(poison, n_steps, T, B, N, dtype=dtype), _owned(poison, n_steps, T, B, M, dtype=dtype)
+    fill = poison or nan_outputs
+    xs, us = _owned(fill, n_steps + 1, B, N, dtype=dtype), _owned(fill, n_steps, B, M, dtype=dtype)
+    costs, info = _owned(fill, n_steps, B, dtype=dtype), _owned(fill, n_steps, 2, dtype=torch.int32)
+    u_next = _owned(fill, T, B, M, dtype=dtype)
+    plan_x, plan_u = _owned(fill, n_steps, T, B, N, dtype=dtype), _owned(fill, n_steps, T, B, M, dtype=dtype)
+    head = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts)]
+    problem = [int(n_steps), L.ptr_view(s.C), L.ptr_view(s.c), L.ptr_view(s.F), L.ptr_view(s.f)]
+    tail = [L.ptr(x0_), L.ptr(u0_), L.ptr(s.u_lower), L.ptr(s.u_upper), L.ptr(s.u_zero_I), L.ptr(xs), L.ptr(us),
+            L.ptr(costs), L.ptr(info), L.ptr(u_next), L.ptr(plan_x), L.ptr(plan_u), L.ptr(ws), nbytes,
+            L.stream_handle(DEV)]
+    if sp is None:
+        name, args = "mpcb200_episode_plans", head + problem + tail
+    else:
+        name = "mpcb200_episode_plant"
+        args = head + [ctypes.byref(sp.rec)] + problem + [L.ptr(sp.F), L.ptr(sp.f), L.ptr(w_)] + tail
     before = L.launch_count()
     with L._on_device(DEV):
-        rc = L.entry("mpcb200_episode_plans", dtype)(
-            ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), L.ptr_view(s.C),
-            L.ptr_view(s.c), L.ptr_view(s.F), L.ptr_view(s.f), L.ptr(x0_), L.ptr(u0_), L.ptr(s.u_lower),
-            L.ptr(s.u_upper), L.ptr(s.u_zero_I), L.ptr(xs), L.ptr(us), L.ptr(costs), L.ptr(info), L.ptr(u_next),
-            L.ptr(plan_x), L.ptr(plan_u), L.ptr(ws), nbytes, L.stream_handle(DEV))
-    L.check(rc, "mpcb200_episode_plans")
+        rc = L.entry(name, dtype)(*args)
+    L.check(rc, name)
     launches, p = L.launch_count() - before, L.last_step_plan()
     torch.cuda.synchronize()
     res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next),
-           "saved": (s, n_steps, xs, us, plan_x, plan_u)}
+           "saved": (s._replace(n_prev=int(n_prev), plant=sp), n_steps, xs, us, plan_x, plan_u)}
     return res, launches, p
 
 
-def abi_episode_backward(saved, dl_dxs, dl_dus, poison=False):
-    """The call step.episode_backward_raw makes (mpcb200_episode_backward_*), with caller-owned outputs and
-    workspace, poison as in abi_episode.  Returns ((dx_init, dC, dc, dF, df, dtheta) cropped as episode_backward_raw
-    crops them, launches, plan): plan is the nested step's, recorded in the sweep's body."""
+def abi_episode_backward(saved, dl_dxs, dl_dus, poison=False, nan_outputs=False):
+    """The call step.episode_backward_raw makes, with caller-owned outputs and workspace, poison as in abi_episode:
+    mpcb200_episode_backward_plant_* when the staged problem records a plant, mpcb200_episode_backward_slew_* when it
+    records n_prev > 0, else mpcb200_episode_backward_*.  Returns ((dx_init, dC, dc, dF, df, dtheta) cropped as
+    episode_backward_raw crops them, and for a plant four more: dF_p [B, n, p], df_p [B, n] (None without the plant's
+    f), dtheta_p [B, NP_plant] and dw [n_steps, B, n] (None without w); launches, plan): plan is the nested step's,
+    recorded in the sweep's body.  Under a slew-rate penalty every size is the augmented problem's."""
     from mpc.pytorch_b200 import step as S
-    from mpc.pytorch_b200.dynamics import DYN_LINEAR, DYN_NPARAMS
+    from mpc.pytorch_b200.dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, DYN_NPARAMS
     L = _L()
     s, n_steps, xs, us, plan_x, plan_u = saved
-    pad, dims = s.pad, s.dims
+    pad, dims, sp = s.pad, s.dims, s.plant
     T, B, N, M = dims.T, dims.B, pad.N, pad.M
     dtype, P = xs.dtype, pad.N + pad.M
     gx_, gu_ = pad.vec_n(S._dense(dl_dxs, dtype)), pad.vec_m(S._dense(dl_dus, dtype))
-    dx_init, dC, dc = (_owned(poison, B, N, dtype=dtype), _owned(poison, T, B, P, P, dtype=dtype),
-                       _owned(poison, T, B, P, dtype=dtype))
+    fill = poison or nan_outputs
+    dx_init, dC, dc = (_owned(fill, B, N, dtype=dtype), _owned(fill, T, B, P, P, dtype=dtype),
+                       _owned(fill, T, B, P, dtype=dtype))
     dF = df = dtheta = None
     if dims.dynamics_kind == DYN_LINEAR:
-        dF = _owned(poison, s.F.shape[0], B, N, P, dtype=dtype)
-        df = _owned(poison, T - 1, B, N, dtype=dtype) if dims.has_f else None
+        dF = _owned(fill, s.F.shape[0], B, N, P, dtype=dtype)
+        df = _owned(fill, T - 1, B, N, dtype=dtype) if dims.has_f else None
     else:
-        dtheta = _owned(poison, B, DYN_NPARAMS[dims.dynamics_kind], dtype=dtype)
-    nbytes = L.lib().mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), xs.element_size())
+        dtheta = _owned(fill, B, DYN_NPARAMS[dims.dynamics_kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype)
+    ins = [L.ptr(s.u_lower), L.ptr(s.u_upper), L.ptr(xs), L.ptr(us), L.ptr(plan_x), L.ptr(plan_u), L.ptr(gx_),
+           L.ptr(gu_), L.ptr(dx_init), L.ptr(dC), L.ptr(dc), L.ptr(dF), L.ptr(df), L.ptr(dtheta)]
+    model = [L.ptr_view(s.C), L.ptr_view(s.c), L.ptr_view(s.F)]
+    sz = xs.element_size()
+    plant_out = ()
+    if sp is not None:
+        pk = sp.rec.kind
+        plant_out = (_owned(fill, B, N, P, dtype=dtype) if pk == DYN_LINEAR else None,
+                     _owned(fill, B, N, dtype=dtype) if pk == DYN_LINEAR and sp.rec.has_f else None,
+                     _owned(fill, B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype)
+                     if pk != DYN_LINEAR else None,
+                     _owned(fill, n_steps, B, N, dtype=dtype) if sp.disturbed else None)
+        name = "mpcb200_episode_backward_plant"
+        nbytes = L.lib().mpcb200_episode_backward_plant_workspace_bytes(ctypes.byref(dims), int(s.n_prev),
+                                                                        ctypes.byref(sp.rec), sz)
+        head = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(sp.rec), int(n_steps), int(s.n_prev)]
+        args = head + model + [L.ptr(sp.F)] + ins + [L.ptr(t) for t in plant_out]
+    elif s.n_prev:
+        name = "mpcb200_episode_backward_slew"
+        nbytes = L.lib().mpcb200_episode_backward_slew_workspace_bytes(ctypes.byref(dims), int(s.n_prev), sz)
+        args = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), int(s.n_prev)] + model + ins
+    else:
+        name = "mpcb200_episode_backward"
+        nbytes = L.lib().mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), sz)
+        args = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps)] + model + ins
     ws = _owned(poison, nbytes, dtype=torch.uint8)
     before = L.launch_count()
     with L._on_device(DEV):
-        rc = L.entry("mpcb200_episode_backward", dtype)(
-            ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), L.ptr_view(s.C), L.ptr_view(s.c),
-            L.ptr_view(s.F), L.ptr(s.u_lower), L.ptr(s.u_upper), L.ptr(xs), L.ptr(us), L.ptr(plan_x), L.ptr(plan_u),
-            L.ptr(gx_), L.ptr(gu_), L.ptr(dx_init), L.ptr(dC), L.ptr(dc), L.ptr(dF), L.ptr(df), L.ptr(dtheta),
-            L.ptr(ws), nbytes, L.stream_handle(DEV))
-    L.check(rc, "mpcb200_episode_backward")
+        rc = L.entry(name, dtype)(*args, L.ptr(ws), nbytes, L.stream_handle(DEV))
+    L.check(rc, name)
     launches, p = L.launch_count() - before, L.last_step_plan()
     torch.cuda.synchronize()
     if df is not None and s.f.shape[0] == T:
         df = torch.cat((df, torch.zeros_like(df[:1])), 0)
-    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta), \
-        launches, p
+    out = (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)
+    if sp is not None:
+        dF_p, df_p, dth_p, dw = plant_out
+        out += (pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
+    return out, launches, p
+
+
+def _episode_per_problem(a, b):
+    """max |a - b| per problem of [S, B, k] tensors -> [B]."""
+    return (a.double() - b.double()).abs().amax((0, 2))
+
+
+def _episode_on_bounds(u, kw):
+    """[2, S, B, m]: which applied controls u [S, B, m] sit on the lower / upper bound (each solve's bound at t = 0)."""
+    at0 = lambda b: b[0] if torch.is_tensor(b) else b  # noqa: E731
+    return torch.stack([u.double() == torch.as_tensor(at0(kw[k]), dtype=F64) for k in ("u_lower", "u_upper")])
+
+
+def check_episode_forward(tag, r, o64, o32, kw, dtype, several):
+    """x, u, costs, info, u_next and the plans of the device episode against the oracle's, problem by problem, under
+    test_ilqr_oracle_gpu.check_loop's rule.  A problem departs where its x, u, u_next, plan_x or plan_u misses the
+    tolerance, or where its applied controls on a bound differ from the oracle's bit for bit.  The plans' later
+    controls are held to the value tolerance only: they are T times as many pnqp end points, whose landing exactly on
+    a bound or within 1e-8 of it round-off decides often enough that a bitwise rule over every plan left more than
+    one problem in four at (3,2), (6,2) and (8,2) with 5 control steps and tensor bounds.  Only bounded episodes of
+    more than one solve iteration (`several`: lqr_iter > 1, or more than one control step, whose solves start from
+    states and warm starts that carry the earlier solves' round-off) may have departing problems, at most one in
+    four: there pnqp's |dx| >= 1e-4 stop and its Armijo test decide some problems' paths by round-off.  float32
+    problems whose float32 oracle departs from the float64 one are left out.  costs by the `within` policy over the
+    rest.  Returns (largest x / u / u_next / plan error of the problems kept, relative to max(1, max|x|, max|u|),
+    departing problems, compared problems)."""
+    x, u = r["x"].cpu(), r["u"].cpu()
+    B = x.shape[1]
+    bounded = "u_lower" in kw
+    sc = max(1.0, float(o64.x.abs().max()), float(o64.u.abs().max()))
+    s, _, _, _, plan_x, plan_u = r["saved"]
+    got = (x, u, r["u_next"].cpu(), s.pad.crop_n(plan_x).cpu(), s.pad.crop_m(plan_u).cpu())
+
+    def per_problem(a, o):              # x, u, u_next and each solve's best iterate (the sweep's linearisation points)
+        e = [_episode_per_problem(a[i], w) for i, w in enumerate((o.x, o.u, o.u_next))]
+        e += [(a[i].double() - w.double()).abs().amax((0, 1, 3)) for i, w in ((3, o.plan_x), (4, o.plan_u))]
+        return torch.stack(e).amax(0)
+
+    def bounds_differ(a, b):            # [B]: a problem's applied controls on a bound differ
+        return (_episode_on_bounds(a, kw) != _episode_on_bounds(b, kw)).any(3).any(1).any(0)
+    err = per_problem(got, o64)
+    out = torch.zeros(B, dtype=torch.bool)
+    if o32 is None:
+        tol = 1e-9 * sc
+    else:
+        e32 = per_problem((o32.x, o32.u, o32.u_next, o32.plan_x, o32.plan_u), o64)
+        out = e32 > 1e-4 * sc
+        if bounded:
+            out |= bounds_differ(o32.u, o64.u)
+        assert not bool(out.all()), f"{tag}: no comparable problem"
+        tol = 4 * float(e32[~out].max()) + 1e-6 * sc
+    dep = err > tol
+    if bounded:
+        dep |= bounds_differ(u, o64.u)
+    dep &= ~out
+    n_dep, n_cmp = int(dep.sum()), int((~out).sum())
+    allowed = max(1, n_cmp // 4) if bounded and several else 0
+    assert n_dep <= allowed, (f"{tag}: {n_dep} of {n_cmp} problems depart from the oracle (allowed {allowed}), "
+                              f"largest x/u/u_next/plan error {float(err[~out].max()):.3e}, tolerance {tol:.3e}")
+    keep = ~(out | dep)
+    assert bool(keep.any()), f"{tag}: no comparable problem"
+    within(tag, "costs", r["costs"].cpu()[:, keep], o64.costs[:, keep],
+           None if o32 is None else o32.costs[:, keep], dtype)
+    want = o64.iters if o32 is None else o32.iters
+    assert r["info"][:, 0].cpu().tolist() == want, f"{tag}: iterations {r['info'][:, 0].tolist()} vs {want}"
+    if "u_zero_I" in kw:
+        assert bool((u[:, kw["u_zero_I"][0]] == 0).all()), f"{tag}: masked controls"
+    return float(err[keep].max()) / sc, n_dep, n_cmp
 
 
 def episode_linear_inputs(seed, B, T, n, m, dtype, mode, F_T=None, f_T="T-1", time_invariant=()):

@@ -32,7 +32,7 @@ import torch
 
 from oracle import lqr_oracle as orc
 from tests.gpu_harness import (DEV, DT, F32, F64, INSTANCES, PAIR_SHAPES, SWITCH_PLANS, abi_episode,
-                               abi_episode_backward, episode_device_inputs, episode_known_inputs,
+                               abi_episode_backward, check_episode_forward, episode_device_inputs, episode_known_inputs,
                                episode_known_module, episode_known_step, episode_linear_inputs, epgrad_launches,
                                kernel_env, loop_plan, pick_switch, plan_name, plan_str, switches, within)
 from tests.helpers import maxdiff
@@ -75,72 +75,12 @@ def run_device(n, m, T, n_steps, P, kw, opts, dtype, impl, dyn=None, poison=Fals
                            **opts, dyn=dyn, poison=poison)
 
 
-def _per_problem(a, b):
-    """max |a - b| per problem of [S, B, k] tensors -> [B]."""
-    return (a.double() - b.double()).abs().amax((0, 2))
-
-
-def _on_bounds(u, kw):
-    """[2, S, B, m]: which applied controls u [S, B, m] sit on the lower / upper bound (each solve's bound at t = 0)."""
-    at0 = lambda b: b[0] if torch.is_tensor(b) else b  # noqa: E731
-    return torch.stack([u.double() == torch.as_tensor(at0(kw[k]), dtype=F64) for k in ("u_lower", "u_upper")])
-
-
 def check_forward(tag, r, o64, o32, kw, dtype, several):
-    """x, u, costs, info, u_next and the plans of the device episode against the oracle's, problem by problem, under
-    test_ilqr_oracle_gpu.check_loop's rule.  A problem departs where its x, u, u_next, plan_x or plan_u misses the
-    tolerance, or where its applied controls on a bound differ from the oracle's bit for bit.  The plans' later
-    controls are held to the value tolerance only: they are T times as many pnqp end points, whose landing exactly on
-    a bound or within 1e-8 of it round-off decides often enough that a bitwise rule over every plan left more than
-    one problem in four at (3,2), (6,2) and (8,2) with 5 control steps and tensor bounds.  Only bounded episodes of
-    more than one solve iteration (`several`: lqr_iter > 1, or more than one control step, whose solves start from
-    states and warm starts that carry the earlier solves' round-off) may have departing problems, at most one in
-    four: there pnqp's |dx| >= 1e-4 stop and its Armijo test decide some problems' paths by round-off.  float32
-    problems whose float32 oracle departs from the float64 one are left out.  costs by the `within` policy over the
-    rest."""
-    x, u = r["x"].cpu(), r["u"].cpu()
-    B = x.shape[1]
-    bounded = "u_lower" in kw
-    sc = max(1.0, float(o64.x.abs().max()), float(o64.u.abs().max()))
-    s, _, _, _, plan_x, plan_u = r["saved"]
-    got = (x, u, r["u_next"].cpu(), s.pad.crop_n(plan_x).cpu(), s.pad.crop_m(plan_u).cpu())
-
-    def per_problem(a, o):              # x, u, u_next and each solve's best iterate (the sweep's linearisation points)
-        e = [_per_problem(a[i], w) for i, w in enumerate((o.x, o.u, o.u_next))]
-        e += [(a[i].double() - w.double()).abs().amax((0, 1, 3)) for i, w in ((3, o.plan_x), (4, o.plan_u))]
-        return torch.stack(e).amax(0)
-
-    def bounds_differ(a, b):            # [B]: a problem's applied controls on a bound differ
-        return (_on_bounds(a, kw) != _on_bounds(b, kw)).any(3).any(1).any(0)
-    err = per_problem(got, o64)
-    out = torch.zeros(B, dtype=torch.bool)
-    if o32 is None:
-        tol = 1e-9 * sc
-    else:
-        e32 = per_problem((o32.x, o32.u, o32.u_next, o32.plan_x, o32.plan_u), o64)
-        out = e32 > 1e-4 * sc
-        if bounded:
-            out |= bounds_differ(o32.u, o64.u)
-        assert not bool(out.all()), f"{tag}: no comparable problem"
-        tol = 4 * float(e32[~out].max()) + 1e-6 * sc
-    dep = err > tol
-    if bounded:
-        dep |= bounds_differ(u, o64.u)
-    dep &= ~out
-    n_dep, n_cmp = int(dep.sum()), int((~out).sum())
+    """gpu_harness.check_episode_forward: x, u, costs, info, u_next and the plans against the oracle's, problem by
+    problem; its largest error and departures recorded for test_zz_coverage."""
+    err, n_dep, n_cmp = check_episode_forward(tag, r, o64, o32, kw, dtype, several)
     DEPARTED.setdefault(dtype, []).append((n_dep, n_cmp))
-    allowed = max(1, n_cmp // 4) if bounded and several else 0
-    assert n_dep <= allowed, (f"{tag}: {n_dep} of {n_cmp} problems depart from the oracle (allowed {allowed}), "
-                              f"largest x/u/u_next/plan error {float(err[~out].max()):.3e}, tolerance {tol:.3e}")
-    keep = ~(out | dep)
-    assert bool(keep.any()), f"{tag}: no comparable problem"
-    _note(dtype, "forward x/u/u_next/plans", float(err[keep].max()) / sc)
-    within(tag, "costs", r["costs"].cpu()[:, keep], o64.costs[:, keep],
-           None if o32 is None else o32.costs[:, keep], dtype)
-    want = o64.iters if o32 is None else o32.iters
-    assert r["info"][:, 0].cpu().tolist() == want, f"{tag}: iterations {r['info'][:, 0].tolist()} vs {want}"
-    if "u_zero_I" in kw:
-        assert bool((u[:, kw["u_zero_I"][0]] == 0).all()), f"{tag}: masked controls"
+    _note(dtype, "forward x/u/u_next/plans", err)
 
 
 GNAMES = ("dx_init", "dC", "dc", "dF", "df", "dtheta")
