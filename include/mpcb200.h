@@ -532,6 +532,91 @@ int mpcb200_episode_backward_plant_f64(const mpcb200_dims* dims, const mpcb200_p
                                        double* df_plant, double* dtheta_plant, double* dw, void* workspace,
                                        size_t workspace_bytes, void* stream);
 
+/*
+ * Episodes on a time-varying problem: every time-indexed input lies on the EPISODE's time axis of L >= n_steps + T - 1
+ * slices, and solve k plans on the window of slices k .. k+T-1 of it.  At the start of each control step (and of each
+ * step of the reverse sweep) one kernel node copies that window into fixed workspace buffers, which the solve's nodes
+ * were recorded with; the solve kernels are those of mpcb200_episode_*.  Per input, its bit in `on`:
+ *   MPCB200_WIN_COST:   C[L,B,p,p], c[L,B,p]; solve k takes C[k .. k+T-1], c[k .. k+T-1];
+ *   MPCB200_WIN_DYN:    a LinDx model's F[L-T+F_T,B,n,p] and f[L-1 or L,B,n]; solve k takes F[k .. k+F_T-1] and
+ *                       f[k .. k+T-2], and the model steps control step k with F[k], f[k];
+ *   MPCB200_WIN_BOUNDS: tensor bounds u_lower, u_upper [L,B,m] (dims->bounds_kind 2); solve k takes [k .. k+T-1];
+ *   MPCB200_WIN_PLANT:  a LinDx plant's F_plant[L-1 or L,B,n,p] and f_plant[L-1 or L,B,n]; control step k steps
+ *                       with slice k.
+ * An input whose bit is clear is what mpcb200_episode_plant_* takes (the solve's own [T,...] with dims' time strides,
+ * or a plant's slice [B,...]).  MPCB200_WIN_COST is required, MPCB200_WIN_DYN only with a LinDx model,
+ * MPCB200_WIN_BOUNDS only with tensor bounds, MPCB200_WIN_PLANT only with a LinDx plant (else MPCB200_ERR_BAD_DIMS).
+ * The *_tstride fields give the elements between consecutive slices of each windowed input, with dims' convention:
+ * 0 dense, > 0 that many elements (each [B,...] slice contiguous), MPCB200_TIME_INVARIANT one slice for every time.
+ */
+#define MPCB200_WIN_COST 1
+#define MPCB200_WIN_DYN 2
+#define MPCB200_WIN_BOUNDS 4
+#define MPCB200_WIN_PLANT 8
+typedef struct mpcb200_window {
+  int32_t L;              /* slices on the episode's axis; L < n_steps + T - 1 is MPCB200_ERR_BAD_DIMS          */
+  int32_t on;             /* MPCB200_WIN_* bits                                                                 */
+  int64_t C_tstride, c_tstride, F_tstride, f_tstride, lo_tstride, hi_tstride, Fp_tstride, fp_tstride;
+} mpcb200_window;
+
+/*
+ * mpcb200_episode_plant_* on a time-varying problem (mpcb200_window above).  plant may be NULL: the model steps the
+ * loop (its window's F[k], f[k] for a LinDx model), and w (NULL: none) is still added.  plan_x and plan_u may both be
+ * NULL.  Checks, capture contract, launch counting and outputs as for mpcb200_episode_plant_*; every argument error is
+ * reported before anything is captured.  workspace: mpcb200_episode_window_workspace_bytes() bytes (0 for arguments
+ * it does not take), 256-byte aligned.
+ */
+size_t mpcb200_episode_window_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts,
+                                              const mpcb200_window* window, int32_t elem_size);
+int mpcb200_episode_window_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                               const mpcb200_window* window, const mpcb200_plant* plant, int32_t n_steps,
+                               const float* C, const float* c, const float* F, const float* f, const float* F_plant,
+                               const float* f_plant, const float* w, const float* x_init, const float* u_init,
+                               const float* u_lower, const float* u_upper, const uint8_t* u_zero_I, float* xs,
+                               float* us, float* costs, int32_t* info, float* u_next, float* plan_x, float* plan_u,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_window_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                               const mpcb200_window* window, const mpcb200_plant* plant, int32_t n_steps,
+                               const double* C, const double* c, const double* F, const double* f,
+                               const double* F_plant, const double* f_plant, const double* w, const double* x_init,
+                               const double* u_init, const double* u_lower, const double* u_upper,
+                               const uint8_t* u_zero_I, double* xs, double* us, double* costs, int32_t* info,
+                               double* u_next, double* plan_x, double* plan_u, void* workspace, size_t workspace_bytes,
+                               void* stream);
+
+/*
+ * The reverse sweep of an episode of mpcb200_episode_window_* (run with plan_x, plan_u), with the rules of
+ * mpcb200_episode_backward_* (plant NULL, n_prev 0), _slew_* (plant NULL, n_prev > 0) or _plant_* (plant given).  The
+ * inputs are the forward's, on the same window.  Each step's window is staged before its adjoint, and the outputs of
+ * windowed inputs are full length, element t summing, in the order k = n_steps-1 .. 0, every solve whose window holds
+ * t: dC[L,B,p,p] and dc[L,B,p] (MPCB200_WIN_COST); dF[L-T+F_T,B,n,p] and df[L-1,B,n] (MPCB200_WIN_DYN), with the
+ * model step's g_k [x_k; u_k]^T and g_k in slice k; dF_plant[L-1,B,n,p] and df_plant[L-1,B,n] (MPCB200_WIN_PLANT),
+ * the plant step's in slice k.  Outputs of inputs whose bit is clear are those of the entry named above.  Every output
+ * is written in full.  workspace: mpcb200_episode_backward_window_workspace_bytes() bytes (0 for arguments it does
+ * not take), 256-byte aligned.
+ */
+size_t mpcb200_episode_backward_window_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev,
+                                                       const mpcb200_window* window, const mpcb200_plant* plant,
+                                                       int32_t elem_size);
+int mpcb200_episode_backward_window_f32(const mpcb200_dims* dims, const mpcb200_params* params,
+                                        const mpcb200_window* window, const mpcb200_plant* plant, int32_t n_steps,
+                                        int32_t n_prev, const float* C, const float* c, const float* F,
+                                        const float* F_plant, const float* u_lower, const float* u_upper,
+                                        const float* xs, const float* us, const float* plan_x, const float* plan_u,
+                                        const float* dl_dxs, const float* dl_dus, float* dx_init, float* dC, float* dc,
+                                        float* dF, float* df, float* dtheta, float* dF_plant, float* df_plant,
+                                        float* dtheta_plant, float* dw, void* workspace, size_t workspace_bytes,
+                                        void* stream);
+int mpcb200_episode_backward_window_f64(const mpcb200_dims* dims, const mpcb200_params* params,
+                                        const mpcb200_window* window, const mpcb200_plant* plant, int32_t n_steps,
+                                        int32_t n_prev, const double* C, const double* c, const double* F,
+                                        const double* F_plant, const double* u_lower, const double* u_upper,
+                                        const double* xs, const double* us, const double* plan_x,
+                                        const double* plan_u, const double* dl_dxs, const double* dl_dus,
+                                        double* dx_init, double* dC, double* dc, double* dF, double* df,
+                                        double* dtheta, double* dF_plant, double* df_plant, double* dtheta_plant,
+                                        double* dw, void* workspace, size_t workspace_bytes, void* stream);
+
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);
 

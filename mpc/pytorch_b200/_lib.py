@@ -36,6 +36,16 @@ class Plant(ctypes.Structure):
     _fields_ = [("kind", ctypes.c_int32), ("has_f", ctypes.c_int32), ("dyn", ctypes.c_double * 8)]
 
 
+# mpcb200_window.on bits (include/mpcb200.h): which inputs of a time-varying episode lie on its time axis
+WIN_COST, WIN_DYN, WIN_BOUNDS, WIN_PLANT = 1, 2, 4, 8
+
+
+class Window(ctypes.Structure):
+    _fields_ = [("L", ctypes.c_int32), ("on", ctypes.c_int32)] + \
+        [(k, ctypes.c_int64) for k in ("C_tstride", "c_tstride", "F_tstride", "f_tstride", "lo_tstride", "hi_tstride",
+                                       "Fp_tstride", "fp_tstride")]
+
+
 class MpcB200Error(RuntimeError):
     pass
 
@@ -61,7 +71,9 @@ EXPORTED_SYMBOLS = (
     "mpcb200_episode_backward_slew_f32", "mpcb200_episode_backward_slew_f64",
     "mpcb200_episode_backward_slew_workspace_bytes", "mpcb200_episode_plant_f32", "mpcb200_episode_plant_f64",
     "mpcb200_episode_backward_plant_f32", "mpcb200_episode_backward_plant_f64",
-    "mpcb200_episode_backward_plant_workspace_bytes",
+    "mpcb200_episode_backward_plant_workspace_bytes", "mpcb200_episode_window_f32", "mpcb200_episode_window_f64",
+    "mpcb200_episode_window_workspace_bytes", "mpcb200_episode_backward_window_f32",
+    "mpcb200_episode_backward_window_f64", "mpcb200_episode_backward_window_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -163,6 +175,23 @@ def lib():
     L.mpcb200_episode_backward_plant_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32,
                                                                  ctypes.POINTER(Plant), ctypes.c_int32]
     L.mpcb200_episode_backward_plant_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_episode_window_f32", "mpcb200_episode_window_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(IlqrOpts), ctypes.POINTER(Window),
+                       ctypes.POINTER(Plant), ctypes.c_int32] + [vp] * 20 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_episode_window_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(IlqrOpts),
+                                                         ctypes.POINTER(Window), ctypes.c_int32]
+    L.mpcb200_episode_window_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_episode_backward_window_f32", "mpcb200_episode_backward_window_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(Window), ctypes.POINTER(Plant),
+                       ctypes.c_int32, ctypes.c_int32] + [vp] * 23 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_episode_backward_window_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32,
+                                                                  ctypes.POINTER(Window), ctypes.POINTER(Plant),
+                                                                  ctypes.c_int32]
+    L.mpcb200_episode_backward_window_workspace_bytes.restype = ctypes.c_size_t
     L.mpcb200_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_supported.restype = ctypes.c_int
     L.mpcb200_supported_list.argtypes = [ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]

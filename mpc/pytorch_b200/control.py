@@ -26,7 +26,8 @@ from .solver import CtrlPassthroughDynamics, LinDx, QuadCost, _mv
 Episode = namedtuple("Episode", "x u costs info u_next")
 
 
-def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plant=None, disturbance=None):
+def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plant=None, disturbance=None,
+                     time_varying=False):
     """Run `n_steps` control steps of receding-horizon MPC from `x_init` [B, n] with the solver `ctrl` (an ``MPC``,
     which supplies every solver option).  For k = 0 .. n_steps-1:
 
@@ -36,8 +37,7 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plan
       * the applied control: ``u_k = plan_u[0]``;
       * the next state, by the model itself: a known system (``CartpoleDx``, ``PendulumDx``) takes one step of its own
         dynamics, any other Module is called as ``dx(x_k, u_k)``, and ``LinDx`` takes its t = 0 slice,
-        ``x_{k+1} = F_0 [x_k; u_k] + f_0``.  That is exact for a time-invariant system; a time-varying F is not
-        shifted along the episode;
+        ``x_{k+1} = F_0 [x_k; u_k] + f_0`` (with ``time_varying=False``; see below for a time-varying F);
       * the next warm start: ``w_{k+1} = cat(plan_u[1:], 0)``, then ``w_{k+1}[-2] = w_{k+1}[-3]`` (the notebooks'
         rule, which needs T >= 3);
       * with ``ctrl.slew_rate_penalty``: solve k takes ``prev_ctrl = u_{k-1}``; solve 0 takes ``ctrl.prev_ctrl``, or
@@ -81,7 +81,21 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plan
     model and the plant share gets the sum.  The episode runs as one graph when the model's episode would and the
     plant steps at the staged shape (a LinDx plant with F, f on the episode's device and dtype; a known plant whose
     state width is the staged one); otherwise (an opaque Module plant, say) the host path runs, stepping the plant
-    with the kernels the graph uses and adding w_k, so the two agree bit for bit wherever both apply."""
+    with the kernels the graph uses and adding w_k, so the two agree bit for bit wherever both apply.
+
+    ``time_varying=True``: every time-indexed input lies on the episode's time axis of L = n_steps + T - 1 slices,
+    and solve k plans on the window of absolute times k .. k+T-1.  ``cost`` is a QuadCost with C [L, B, p, p] or
+    [L, p, p] (or [p, p], expanded to L) and c [L, B, p] or [L, p] (or [p]); a LinDx model's F and f, and a LinDx
+    plant's, have a leading axis of L - 1 or L; tensor bounds ``ctrl.u_lower`` / ``ctrl.u_upper`` are [L, B, m].
+    ``u_zero_I``, ``delta_u``, a known system's ``params`` and ``disturbance`` are not windowed.  A time-invariant
+    piece is passed as a stride-0 ``expand(L, ...)``.  The loop is
+        for k: _, plan_u, _ = ctrl'(x_k, QuadCost(C[k:k+T], c[k:k+T]), LinDx(F[k:k+F_T], f[k:k+f_T]))
+               x_{k+1} = step_k(x_k, plan_u[0])
+    with F_T = T - (L - len(F)) (and f_T likewise), bounds [k:k+T], and the model's (or a LinDx plant's) step at
+    slice k: x_{k+1} = F[k] [x_k; u_k] + f[k] (+ w_k).  Gradients are autograd's for that loop: dC, dc, dF and df
+    are full length, element t summing every solve whose window holds t and, for F[k], f[k], the step at k.  A
+    later call continues the episode with the axis from n_steps on (C[n_steps : n_steps + n2 + T - 1], ...).
+    Wrong lengths, and a Module cost, raise MpcB200Error before anything runs."""
     T, n, m = ctrl.T, ctrl.n_state, ctrl.n_ctrl
     if T < 3:
         raise MpcB200Error(f"a receding-horizon episode needs a horizon T >= 3 (the warm-start shift), got T={T}")
@@ -91,24 +105,52 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plan
     if plant is dx:
         plant = None
     _check_plant(plant, disturbance, x_init, n, m, n_steps)
+    L = n_steps + T - 1 if time_varying else None
+    if time_varying:
+        _check_axis(ctrl, cost, dx, plant, L, B)
     if plant is None and disturbance is not None:
         plant = dx                        # the model steps the disturbed loop
-    cost = solver._expand_cost(cost, T, ctrl.n_batch if ctrl.n_batch is not None else B, n + m)
+    cost = solver._expand_cost(cost, L or T, ctrl.n_batch if ctrl.n_batch is not None else B, n + m)
     w0 = _first_warm_start(ctrl, x_init)
     from .dynamics import params_scope
     if differentiable and torch.is_grad_enabled() and _requires_grad(x_init, cost, dx, plant, disturbance):
         with params_scope():
             if _takes_device_path(ctrl, x_init, cost, dx, w0, plant):
-                ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+                ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
                 if ep is not None:
                     return ep
-            return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+            return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
     with torch.no_grad(), params_scope():     # a known system's CUDA parameters are read once per episode
         if _takes_device_path(ctrl, x_init, cost, dx, w0, plant):
-            ep = _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+            ep = _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
             if ep is not None:
                 return ep
-        return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+        return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
+
+
+def _check_axis(ctrl, cost, dx, plant, L, B):
+    """The inputs of a time-varying episode against its axis of L slices, before anything runs: a QuadCost whose C
+    and c have L slices (or no time axis: [p, p], [p]); a LinDx model's or plant's F and f with L - 1 or L; tensor
+    bounds [L, B, m]."""
+    n, m = ctrl.n_state, ctrl.n_ctrl
+    if not isinstance(cost, QuadCost):
+        raise MpcB200Error("time_varying=True needs a QuadCost: a Module cost has no time axis")
+    for name, t, flat in (("cost.C", cost.C, 2), ("cost.c", cost.c, 1)):
+        if not isinstance(t, torch.Tensor) or (t.dim() != flat and (t.dim() not in (flat + 1, flat + 2) or
+                                                                    t.shape[0] != L)):
+            raise MpcB200Error(f"{name}: a time-varying episode needs {L} slices (n_steps + T - 1), got shape "
+                               f"{tuple(t.shape) if isinstance(t, torch.Tensor) else t}")
+    for who, d in (("dx", dx), ("plant", plant)):
+        if not isinstance(d, LinDx):
+            continue
+        for name, t in (("F", d.F), ("f", d.f)):
+            if isinstance(t, torch.Tensor) and t.nelement() > 0 and t.shape[0] not in (L - 1, L):
+                raise MpcB200Error(f"{who}: a time-varying episode needs a LinDx {name} of {L - 1} or {L} slices, "
+                                   f"got shape {tuple(t.shape)}")
+    for name, b in (("u_lower", ctrl.u_lower), ("u_upper", ctrl.u_upper)):
+        if isinstance(b, torch.Tensor) and tuple(b.shape) != (L, B, m):
+            raise MpcB200Error(f"{name}: a time-varying episode needs tensor bounds of shape {(L, B, m)}, got "
+                               f"{tuple(b.shape)}")
 
 
 def _check_plant(plant, w, x_init, n, m, n_steps):
@@ -148,7 +190,7 @@ def _requires_grad(x_init, cost, dx, plant=None, w=None):
 def _takes_device_path(ctrl, x_init, cost, dx, w0, plant=None):
     """Whether the episode runs as one graph: exactly when each of its solves would take the device loop (T >= 3 is
     checked before) and the plant, if any, steps at the staged shape (_plant_on_device).  Decided on tensor metadata
-    alone."""
+    alone, which a time-varying episode's full-length inputs share with its windows, so the same rule serves both."""
     return (solver._use_device_loop(ctrl, x_init, cost, dx, w0) or
             solver._use_slew_device_loop(ctrl, x_init, cost, dx, w0)) and \
         (plant is None or _plant_on_device(ctrl, x_init, dx, plant))
@@ -156,9 +198,9 @@ def _takes_device_path(ctrl, x_init, cost, dx, w0, plant=None):
 
 def _plant_on_device(ctrl, x_init, dx, plant):
     """Whether the plant steps inside the episode's graph: a LinDx plant whose F (and f) are tensors of the episode's
-    dtype and device (staged like the model's, _Pad), or a known system whose state width, n or n + m under a
-    slew-rate penalty, is the staged one.  A known model always runs at its own width; a LinDx model where
-    _pick_instance gives the exact shape or the large-shape kernels."""
+    dtype and device (staged like the model's, _Pad; in a time-varying episode whole, its slice k copied per step), or
+    a known system whose state width, n or n + m under a slew-rate penalty, is the staged one.  A known model always
+    runs at its own width; a LinDx model where _pick_instance gives the exact shape or the large-shape kernels."""
     from .dynamics import DYN_LINEAR, known_kind
     from .step import _pick_instance
     n, m = ctrl.n_state, ctrl.n_ctrl
@@ -173,22 +215,23 @@ def _plant_on_device(ctrl, x_init, dx, plant):
     return _pick_instance(n_aug, m, x_init.element_size(), DYN_LINEAR) == (n_aug, m)
 
 
-def _plant_spec(ctrl, x_init, C, plant, F_p, f_p):
+def _plant_spec(ctrl, x_init, C, plant, F_p, f_p, whole=False):
     """The plant as step.episode_raw takes it, on the problem MPC._device_problem stages: (DYN_LINEAR, None, F, f) of
     a LinDx plant (under a slew-rate penalty its slice 0 alone, the one that steps, augmented as MPC._slew_augment
-    augments F, f), or (kind, params, None, None) of a known system (its passthrough kind under a slew-rate
-    penalty)."""
+    augments F, f; with `whole`, a time-varying episode's, every slice), or (kind, params, None, None) of a known
+    system (its passthrough kind under a slew-rate penalty)."""
     from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, known_kind
     slew = ctrl.slew_rate_penalty is not None
     if isinstance(plant, LinDx):
-        if slew:                          # [[0, 0, I], [0, F_p]] and [0; f_p] of the slice that steps
+        if slew:                          # [[0, 0, I], [0, F_p]] and [0; f_p] of the slices that step
             m = ctrl.n_ctrl
-            F0 = F_p[:1]
-            Fu = F0.new_zeros(1, F0.shape[1], m, F0.shape[3] + m)
+            F0 = F_p if whole else F_p[:1]
+            Fu = F0.new_zeros(F0.shape[0], F0.shape[1], m, F0.shape[3] + m)
             Fu[..., F0.shape[3]:] = torch.eye(m, dtype=F0.dtype, device=F0.device)
             F_p = torch.cat((Fu, torch.cat((F0.new_zeros(*F0.shape[:3], m), F0), 3)), 2)
             if f_p is not None and f_p.nelement() > 0:
-                f_p = torch.cat((f_p.new_zeros(1, f_p.shape[1], m), f_p[:1]), 2)
+                f0 = f_p if whole else f_p[:1]
+                f_p = torch.cat((f0.new_zeros(f0.shape[0], f0.shape[1], m), f0), 2)
         return DYN_LINEAR, None, F_p, f_p
     kind, params = known_kind(plant, ctrl.n_state, ctrl.n_ctrl, x_init)
     return (kind | DYN_CTRL_PASSTHROUGH if slew else kind), params, None, None
@@ -219,17 +262,19 @@ def _first_warm_start(ctrl, x_init):
     return u.to(dtype=x_init.dtype, device=x_init.device)
 
 
-def _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
+def _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None, L=None):
     """The episode as one library call (step.episode_raw) on the problem MPC._ilqr_device stages, once; None when the
-    driver refused the graph (nothing ran then)."""
+    driver refused the graph (nothing ran then).  L: a time-varying episode's axis (episode_raw's window)."""
     from . import step as _step
     T, m = ctrl.T, ctrl.n_ctrl
-    n, x0, C, c, F, f, dyn = ctrl._device_problem(x_init, cost, dx)
+    n, x0, C, c, F, f, dyn = ctrl._device_problem(x_init, cost, dx, T=L)
     kw = {}
     if plant is not None:
         F_p, f_p = (plant.F, plant.f) if isinstance(plant, LinDx) else (None, None)
-        kw = dict(plant=_plant_spec(ctrl, x_init, cost.C, plant, F_p, f_p), w=_staged_w(ctrl, w))
-    res = _step.episode_raw(n, m, T, n_steps, x0, C, c, F, f, w0, dyn=dyn, **kw, **ctrl._device_options())
+        kw = dict(plant=_plant_spec(ctrl, x_init, cost.C, plant, F_p, f_p, whole=L is not None),
+                  w=_staged_w(ctrl, w))
+    res = _step.episode_raw(n, m, T, n_steps, x0, C, c, F, f, w0, dyn=dyn, window=L, **kw,
+                            **ctrl._device_options())
     if res is None:
         solver._graph_cond_unavailable = True
         return None
@@ -255,20 +300,22 @@ class EpisodeFn(torch.autograd.Function):
     outputs do not keep themselves alive through ctx; ctx holds only the staged problem's metadata.  First order only:
     the backward is raw kernels.  `o[4]` a plant (receding_horizon's `plant`), or None: F_p, f_p (a LinDx plant's),
     plant_params (a known plant's) and w are then inputs too, the staged plant's F, f go through save_for_backward,
-    and their gradients come from the plant sweep (step.episode_backward_raw), F_p's and f_p's in slice 0."""
+    and their gradients come from the plant sweep (step.episode_backward_raw), F_p's and f_p's in slice 0.  `o[5]`
+    a time-varying episode's axis L, or None: C, c, F, f, bounds and a LinDx plant's F_p, f_p are full length, and so
+    are their gradients."""
 
     @staticmethod
     def forward(ctx, o, x_init, C, c, F, f, params, F_p=None, f_p=None, plant_params=None, w=None):
         from . import step as _step
-        ctrl, dx, n_steps, w0, plant = o
+        ctrl, dx, n_steps, w0, plant, L = o
         T, m = ctrl.T, ctrl.n_ctrl
-        n, x0, C_, c_, F_, f_, dyn = ctrl._device_problem(x_init, QuadCost(C, c), dx)
+        n, x0, C_, c_, F_, f_, dyn = ctrl._device_problem(x_init, QuadCost(C, c), dx, T=L)
         slew = ctrl.slew_rate_penalty is not None
         kw = {}
         if plant is not None:
-            kw = dict(plant=_plant_spec(ctrl, x_init, C, plant, F_p, f_p), w=_staged_w(ctrl, w))
+            kw = dict(plant=_plant_spec(ctrl, x_init, C, plant, F_p, f_p, whole=L is not None), w=_staged_w(ctrl, w))
         res = _step.episode_raw(n, m, T, n_steps, x0, C_, c_, F_, f_, w0, dyn=dyn, keep_plans=True,
-                                n_prev=m if slew else 0, **kw, **ctrl._device_options())
+                                n_prev=m if slew else 0, window=L, **kw, **ctrl._device_options())
         if res is None:
             raise _NoGraph()
         ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
@@ -281,6 +328,7 @@ class EpisodeFn(torch.autograd.Function):
         ctx.p_meta = (params.dtype, params.device) if params is not None else None
         ctx.plant_meta = (F_p.shape if F_p is not None else None, f_p.shape if f_p is not None else None,
                           (plant_params.dtype, plant_params.device) if plant_params is not None else None)
+        ctx.whole = L is not None
         ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
         x = res["x"][:, :, m:] if slew else res["x"]
         return x, res["u"], res["costs"], res["info"], res["u_next"]
@@ -315,12 +363,14 @@ class EpisodeFn(torch.autograd.Function):
         if dtheta is not None and need[6]:
             dparams = dtheta.sum(0).to(dtype=ctx.p_meta[0], device=ctx.p_meta[1])
         F_shape, f_shape, pp_meta = ctx.plant_meta
-        if dF_p is not None and need[7]:          # the plant steps with its slice 0
-            dFp = dF_p.new_zeros(F_shape)
-            dFp[0] = dF_p
+        if dF_p is not None and need[7]:          # the plant steps with its slice 0 (time-varying: slice k)
+            dFp = dF_p if ctx.whole else dF_p.new_zeros(F_shape)
+            if not ctx.whole:
+                dFp[0] = dF_p
         if df_p is not None and need[8]:
-            dfp = df_p.new_zeros(f_shape)
-            dfp[0] = df_p
+            dfp = df_p if ctx.whole else df_p.new_zeros(f_shape)
+            if not ctx.whole:
+                dfp[0] = df_p
         if dth_p is not None and need[9]:
             dpp = dth_p.sum(0).to(dtype=pp_meta[0], device=pp_meta[1])
         return (None, dx_init if need[1] else None, dC if need[2] else None, dc if need[3] else None,
@@ -328,7 +378,7 @@ class EpisodeFn(torch.autograd.Function):
                 dw if dw is not None and need[10] else None)
 
 
-def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
+def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None, L=None):
     """The differentiable episode on the device path (EpisodeFn); None when the driver refused the graph."""
     F, f, params = None, None, None
     if isinstance(dx, LinDx):
@@ -344,30 +394,34 @@ def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None
             p_params = getattr(plant, "params", None)
         extra = (F_p, f_p, p_params, w)
     try:
-        x, u, costs, info, u_next = EpisodeFn.apply((ctrl, dx, n_steps, w0, plant), x_init, cost.C, cost.c, F, f,
-                                                    params, *extra)
+        x, u, costs, info, u_next = EpisodeFn.apply((ctrl, dx, n_steps, w0, plant, L), x_init, cost.C, cost.c, F,
+                                                    f, params, *extra)
     except _NoGraph:
         solver._graph_cond_unavailable = True
         return None
     return Episode(x, u, costs, info, u_next)
 
 
-def _episode_host(ctrl, x_init, cost, dx, n_steps, w, plant=None, dist=None):
+def _episode_host(ctrl, x_init, cost, dx, n_steps, w, plant=None, dist=None, L=None):
     """The episode as a Python loop over MPC.forward, on a shallow copy of ctrl that takes each step's warm start.
     Differentiable where autograd records: the warm starts and prev_ctrl are held constant.  A plant steps the loop
-    in the model's place (_model_step applied to it), and dist[k] is added to its step."""
+    in the model's place (_model_step applied to it), and dist[k] is added to its step.  L: a time-varying episode's
+    axis; step k then solves and steps on its window (_window)."""
     slew = ctrl.slew_rate_penalty is not None
     solve = copy.copy(ctrl)
     solve.exit_unconverged = solve.detach_unconverged = False
     xs, us, costs, infos = [x_init], [], [], []
     x, prev = x_init, ctrl.prev_ctrl
+    cost_k, dx_k, plant_k = cost, dx, plant
     for k in range(n_steps):
         solve.u_init, solve.prev_ctrl = w, prev
-        _, plan_u, plan_costs = solve(x, cost, dx)
-        if plant is None:
-            x = _model_step(solve, x, plan_u, cost, dx)
+        if L is not None:
+            cost_k, dx_k, plant_k = _window(ctrl, solve, cost, dx, plant, k, L)
+        _, plan_u, plan_costs = solve(x, cost_k, dx_k)
+        if plant_k is None:
+            x = _model_step(solve, x, plan_u, cost_k, dx_k)
         else:
-            x = _plant_step(solve, x, plan_u, cost, plant, dist[k] if dist is not None else None)
+            x = _plant_step(solve, x, plan_u, cost_k, plant_k, dist[k] if dist is not None else None)
         w = shift_warm_start(plan_u.detach())
         if slew:
             prev = plan_u[0].detach()
@@ -376,6 +430,29 @@ def _episode_host(ctrl, x_init, cost, dx, n_steps, w, plant=None, dist=None):
         costs.append(plan_costs)
         infos.append(solve._solve_info.to(x_init.device))
     return Episode(torch.stack(xs), torch.stack(us), torch.stack(costs), torch.stack(infos), w)
+
+
+def _window(ctrl, solve, cost, dx, plant, k, L):
+    """Control step k of a time-varying episode on the host path: QuadCost(C[k:k+T], c[k:k+T]), a LinDx model's
+    LinDx(F[k:k+F_T], f[k:k+f_T]) (F_T = T - (L - len(F))), tensor bounds [k:k+T] set on `solve`, and a LinDx
+    plant's slice k (a plant that is the model steps with the model's window)."""
+    T = ctrl.T
+
+    def lin(d, n_keep):
+        f = d.f
+        if isinstance(f, torch.Tensor) and f.nelement() > 0:
+            f = f[k:k + (n_keep - (L - f.shape[0]) if n_keep == T else n_keep)]
+        return LinDx(d.F[k:k + (n_keep - (L - d.F.shape[0]) if n_keep == T else n_keep)], f)
+    for name in ("u_lower", "u_upper"):
+        b = getattr(ctrl, name)
+        if isinstance(b, torch.Tensor):
+            setattr(solve, name, b[k:k + T])
+    dx_k = lin(dx, T) if isinstance(dx, LinDx) else dx
+    if plant is dx:
+        plant_k = dx_k
+    else:
+        plant_k = lin(plant, 1) if isinstance(plant, LinDx) else plant
+    return QuadCost(cost.C[k:k + T], cost.c[k:k + T]), dx_k, plant_k
 
 
 def _plant_step(solve, x, plan_u, cost, plant, w_k):

@@ -837,10 +837,11 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
 }
 
 // Adds the episode's init kernel and its `while` node over control steps (body recorded on `es`) to the graph `os`
-// is capturing.  Body: the iLQR loop (its own `while` node, body on `bs`) -> model step -> [episode_plans_kernel,
-// with plan_x / plan_u] -> episode_advance_kernel.
+// is capturing.  Body: [window_stage_kernel, with wc] -> the iLQR loop (its own `while` node, body on `bs`) -> model
+// step -> [episode_plans_kernel, with plan_x / plan_u] -> episode_advance_kernel.
 template <typename R>
-static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, const EpisodeCall<R>& e, int knob) {
+static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, const EpisodeCall<R>& e, int knob,
+                          const WindowCopy<R>* wc = nullptr) {
   const mpcb200_dims* d = e.d;
   const EpisodeLayout l = episode_layout(d, sizeof(R), knob);
   const IlqrCall<R> q = episode_solve(e, l);
@@ -858,7 +859,8 @@ static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, con
     return MPCB200_ERR_LAUNCH;
   rc = open_while(os, es, handle);
   if (rc) return rc;
-  rc = ilqr_record<R>(es, bs, q, knob);
+  if (wc != nullptr) rc = counted(window_launch_stage<R>(*wc, es));
+  if (rc == 0) rc = ilqr_record<R>(es, bs, q, knob);
   // the model step (the plant's, where the call names one) from the solve's best controls, by the launchers the
   // solve's rollout uses, at T = 2
   const EpisodeStep<R> s = episode_step(e);
@@ -1041,8 +1043,11 @@ static int epgrad_check(const EpGradCall<R>& q, int knob) {
 
 // Adds the init kernel and the `while` node over k = n_steps-1 .. 0 (body recorded on `bs`) to the graph `os` is
 // capturing.  Body: stage -> [linearisation] -> adjoint -> [linearisation VJP] -> accumulate.
+// wc, wn (mpcb200_episode_backward_window_*): window_stage_kernel first in the body, and the window forms of init,
+// stage and accumulate.
 template <typename R>
-static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, int knob) {
+static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, int knob,
+                         const WindowCopy<R>* wc = nullptr, const EpWindow* wn = nullptr) {
   const mpcb200_dims* d = q.d;
   const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
   char* ws = (char*)q.workspace;
@@ -1090,10 +1095,14 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   cudaGraphConditionalHandle handle;
   int rc = while_handle(os, &handle);
   if (rc) return rc;
-  if (counted(epgrad_launch_init<R>(a, q.n_prev, plp, handle, os)) != 0) return MPCB200_ERR_LAUNCH;
+  if (counted(wn != nullptr ? epgrad_launch_init_window<R>(a, q.n_prev, plp, *wn, handle, os)
+                            : epgrad_launch_init<R>(a, q.n_prev, plp, handle, os)) != 0)
+    return MPCB200_ERR_LAUNCH;
   rc = open_while(os, bs, handle);
   if (rc) return rc;
-  rc = counted(epgrad_launch_stage<R>(as, bs));
+  if (wc != nullptr) rc = counted(window_launch_stage<R>(*wc, bs));
+  if (rc == 0)
+    rc = counted(wn != nullptr ? epgrad_launch_stage_window<R>(as, *wn, bs) : epgrad_launch_stage<R>(as, bs));
   const R* F = q.F;
   if (rc == 0 && known) {
     F = (const R*)(ws + l.Fk);
@@ -1112,7 +1121,9 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
     v.x = a.stage_x; v.u = a.stage_u; v.dF = dFk; v.df = dfk; v.first = first; v.second = second;
     rc = counted(epgrad_launch_vjp_passthrough<R>(v, bs));
   }
-  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, q.n_prev, plp, handle, bs));
+  if (rc == 0)
+    rc = counted(wn != nullptr ? epgrad_launch_accum_window<R>(a, q.n_prev, plp, *wn, handle, bs)
+                               : epgrad_launch_accum<R>(a, q.n_prev, plp, handle, bs));
   cudaGraph_t body = nullptr;
   if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
   return rc;
@@ -1127,6 +1138,187 @@ static int epgrad_impl(const EpGradCall<R>& q, void* stream) {
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t bs = ilqr_stream(2);
     return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_record<R>(os, bs, q, knob);
+  });
+}
+
+// ---------------------------------------------------------------------------------------------
+// time-varying episodes (mpcb200_episode_window_*, mpcb200_episode_backward_window_*): each control step's window of
+// the full-length inputs is staged into fixed workspace buffers, which the episode's (or sweep's) nodes read
+// ---------------------------------------------------------------------------------------------
+enum { WIN_C, WIN_c, WIN_F, WIN_f, WIN_LO, WIN_HI, WIN_FP, WIN_FPF };
+struct WindowLayout {                 // byte offsets of the window buffers, after the episode's (sweep's) workspace
+  size_t at[WINDOW_INPUTS], total;
+};
+// d: the solve's dims.  f's buffer holds T slices (the kernels read T-1); a plant's, one
+static WindowLayout window_layout(const mpcb200_dims* d, const mpcb200_window* w, size_t base, size_t sz) {
+  WindowLayout l;
+  const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m;
+  const size_t len[WINDOW_INPUTS] = {T * B * p * p, T * B * p, (size_t)d->F_T * B * n * p, T * B * n,
+                                     T * B * m, T * B * m, B * n * p, B * n};
+  const int bit[WINDOW_INPUTS] = {MPCB200_WIN_COST, MPCB200_WIN_COST, MPCB200_WIN_DYN, MPCB200_WIN_DYN,
+                                  MPCB200_WIN_BOUNDS, MPCB200_WIN_BOUNDS, MPCB200_WIN_PLANT, MPCB200_WIN_PLANT};
+  size_t o = base;
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    l.at[a] = 0;
+    if (w->on & bit[a]) {
+      l.at[a] = o;
+      o += up256(len[a] * sz);
+    }
+  }
+  l.total = o;
+  return l;
+}
+
+// the window record against the caller's dims: MPCB200_WIN_COST set, each other bit only where its input can be
+// windowed, an axis that covers n_steps + T - 1 slices, and time strides of the dims convention
+static int window_check(const mpcb200_dims* d, const mpcb200_window* w, int n_steps, const mpcb200_plant* plant) {
+  if (w == nullptr) return MPCB200_ERR_NULL_POINTER;
+  const int all = MPCB200_WIN_COST | MPCB200_WIN_DYN | MPCB200_WIN_BOUNDS | MPCB200_WIN_PLANT;
+  if (!(w->on & MPCB200_WIN_COST) || (w->on & ~all) != 0) return MPCB200_ERR_BAD_DIMS;
+  if ((w->on & MPCB200_WIN_DYN) && d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  if ((w->on & MPCB200_WIN_BOUNDS) && d->bounds_kind != 2) return MPCB200_ERR_BAD_DIMS;
+  if ((w->on & MPCB200_WIN_PLANT) && (plant == nullptr || plant->kind != DYN_LINEAR)) return MPCB200_ERR_BAD_DIMS;
+  if (n_steps < 1 || (long long)w->L < (long long)n_steps + d->T - 1) return MPCB200_ERR_BAD_DIMS;
+  const int64_t ts[WINDOW_INPUTS] = {w->C_tstride, w->c_tstride, w->F_tstride, w->f_tstride,
+                                     w->lo_tstride, w->hi_tstride, w->Fp_tstride, w->fp_tstride};
+  for (int64_t t : ts)
+    if (t < MPCB200_TIME_INVARIANT) return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+// the solve's dims: the caller's, with the windowed inputs read from dense buffers
+static mpcb200_dims window_solve_dims(const mpcb200_dims* d, const mpcb200_window* w) {
+  mpcb200_dims ds = *d;
+  if (w->on & MPCB200_WIN_COST) ds.C_tstride = ds.c_tstride = 0;
+  if (w->on & MPCB200_WIN_DYN) ds.F_tstride = ds.f_tstride = 0;
+  return ds;
+}
+
+// The copy of each windowed input (src NULL: not windowed or not given), k read from `step`.  Slices: T of C, c and
+// the bounds, F_T of F, T-1 of f, 1 of the plant's F, f.
+template <typename R>
+static WindowCopy<R> window_copy(const mpcb200_dims* d, const mpcb200_window* w, const WindowLayout& l, char* ws,
+                                 const R* const src[WINDOW_INPUTS], const int32_t* step) {
+  WindowCopy<R> c;
+  std::memset(&c, 0, sizeof(c));
+  const long long B = d->B, T = d->T, n = d->n, m = d->m, p = n + m;
+  const long long slice[WINDOW_INPUTS] = {B * p * p, B * p, B * n * p, B * n, B * m, B * m, B * n * p, B * n};
+  const int cnt[WINDOW_INPUTS] = {(int)T, (int)T, d->F_T, (int)T - 1, (int)T, (int)T, 1, 1};
+  const int64_t ts[WINDOW_INPUTS] = {w->C_tstride, w->c_tstride, w->F_tstride, w->f_tstride,
+                                     w->lo_tstride, w->hi_tstride, w->Fp_tstride, w->fp_tstride};
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    if (l.at[a] == 0 || src[a] == nullptr) continue;
+    c.src[a] = src[a];
+    c.dst[a] = (R*)(ws + l.at[a]);
+    c.tstride[a] = ts[a] == 0 ? slice[a] : ts[a];
+    c.slice[a] = slice[a];
+    c.n[a] = cnt[a];
+  }
+  c.k = step;
+  return c;
+}
+
+// e: the call with the full-length pointers.  Every argument error is reported before anything is captured.
+template <typename R>
+static int episode_window_impl(const EpisodeCall<R>& e, const mpcb200_window* w, void* stream) {
+  const int knob = kernel_knob();
+  if (e.d == nullptr) return MPCB200_ERR_NULL_POINTER;
+  int rc = check_dims(e.d);
+  if (rc) return rc;
+  rc = window_check(e.d, w, e.n_steps, e.plant);
+  if (rc) return rc;
+  const bool has_f = e.d->has_f != 0;
+  if (e.C == nullptr || e.c == nullptr || ((w->on & MPCB200_WIN_DYN) && (e.F == nullptr || (has_f && !e.f))) ||
+      ((w->on & MPCB200_WIN_BOUNDS) && (e.u_lower == nullptr || e.u_upper == nullptr)) ||
+      ((w->on & MPCB200_WIN_PLANT) && (e.F_plant == nullptr || (e.plant->has_f && e.f_plant == nullptr))))
+    return MPCB200_ERR_NULL_POINTER;
+  const mpcb200_dims ds = window_solve_dims(e.d, w);
+  const EpisodeLayout el = episode_layout(&ds, sizeof(R), knob);
+  const WindowLayout l = window_layout(&ds, w, el.total, sizeof(R));
+  if (e.workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  char* ws = (char*)e.workspace;
+  const R* src[WINDOW_INPUTS] = {e.C, e.c, e.F, has_f ? e.f : nullptr, e.u_lower, e.u_upper, e.F_plant,
+                                 e.plant != nullptr && e.plant->has_f ? e.f_plant : nullptr};
+  const WindowCopy<R> wc = window_copy<R>(&ds, w, l, ws, src, (const int32_t*)(ws + el.ep));
+  EpisodeCall<R> es = e;              // the episode on the window buffers
+  es.d = &ds;
+  es.workspace_bytes = el.total;
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    if (wc.src[a] == nullptr) continue;
+    const R* buf = wc.dst[a];
+    switch (a) {
+      case WIN_C: es.C = buf; break;
+      case WIN_c: es.c = buf; break;
+      case WIN_F: es.F = buf; break;
+      case WIN_f: es.f = buf; break;
+      case WIN_LO: es.u_lower = buf; break;
+      case WIN_HI: es.u_upper = buf; break;
+      case WIN_FP: es.F_plant = buf; break;
+      default: es.f_plant = buf; break;
+    }
+  }
+  rc = episode_check<R>(es, knob);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t s2 = ilqr_stream(2), s1 = ilqr_stream(1);
+    return s2 == nullptr || s1 == nullptr ? MPCB200_ERR_LAUNCH : episode_record<R>(os, s2, s1, es, knob, &wc);
+  });
+}
+
+// the sweep's layout base: epgrad_layout of the solve's dims, with the plant's kind
+static size_t epgrad_window_base(const mpcb200_dims* ds, const mpcb200_plant* plant, size_t sz, int knob) {
+  return epgrad_layout(ds, sz, knob, plant != nullptr ? plant->kind : -1).total;
+}
+
+template <typename R>
+static int epgrad_window_impl(const EpGradCall<R>& q, const mpcb200_window* w, void* stream) {
+  const int knob = kernel_knob();
+  if (q.d == nullptr) return MPCB200_ERR_NULL_POINTER;
+  int rc = check_dims(q.d);
+  if (rc) return rc;
+  rc = window_check(q.d, w, q.n_steps, q.plant);
+  if (rc) return rc;
+  if (q.C == nullptr || q.c == nullptr || ((w->on & MPCB200_WIN_DYN) && q.F == nullptr) ||
+      ((w->on & MPCB200_WIN_BOUNDS) && (q.u_lower == nullptr || q.u_upper == nullptr)) ||
+      ((w->on & MPCB200_WIN_PLANT) && q.F_plant == nullptr))
+    return MPCB200_ERR_NULL_POINTER;
+  if (q.d->T < 3) return MPCB200_ERR_BAD_DIMS;
+  const mpcb200_dims ds = window_solve_dims(q.d, w);
+  const size_t base = epgrad_window_base(&ds, q.plant, sizeof(R), knob);
+  const WindowLayout l = window_layout(&ds, w, base, sizeof(R));
+  if (q.workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  char* ws = (char*)q.workspace;
+  const EpGradLayout gl = epgrad_layout(&ds, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
+  const R* src[WINDOW_INPUTS] = {q.C, q.c, q.F, nullptr, q.u_lower, q.u_upper, q.F_plant, nullptr};
+  const WindowCopy<R> wc = window_copy<R>(&ds, w, l, ws, src, (const int32_t*)(ws + gl.state));
+  EpGradCall<R> qs = q;               // the sweep on the window buffers
+  qs.d = &ds;
+  qs.workspace_bytes = base;
+  if (wc.src[WIN_C] != nullptr) qs.C = wc.dst[WIN_C];
+  if (wc.src[WIN_c] != nullptr) qs.c = wc.dst[WIN_c];
+  if (wc.src[WIN_F] != nullptr) qs.F = wc.dst[WIN_F];
+  if (wc.src[WIN_LO] != nullptr) qs.u_lower = wc.dst[WIN_LO];
+  if (wc.src[WIN_HI] != nullptr) qs.u_upper = wc.dst[WIN_HI];
+  if (wc.src[WIN_FP] != nullptr) qs.F_plant = wc.dst[WIN_FP];
+  rc = epgrad_check<R>(qs, knob);
+  if (rc) return rc;
+  EpWindow wn;
+  wn.cost = 1;
+  wn.dyn = (w->on & MPCB200_WIN_DYN) != 0;
+  wn.step = q.plant != nullptr ? (w->on & MPCB200_WIN_PLANT) != 0 : wn.dyn;
+  wn.L = w->L;
+  wn.LF = w->L - ds.T + ds.F_T;
+  wn.Lf = w->L - 1;
+  wn.Lp = w->L - 1;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t bs = ilqr_stream(2);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_record<R>(os, bs, qs, knob, &wc, &wn);
   });
 }
 }  // namespace mpcb200
@@ -1396,6 +1588,61 @@ size_t mpcb200_episode_backward_plant_workspace_bytes(const mpcb200_dims* dims, 
 MPCB200_EPISODE_BACKWARD_PLANT(f32, float)
 MPCB200_EPISODE_BACKWARD_PLANT(f64, double)
 #undef MPCB200_EPISODE_BACKWARD_PLANT
+
+size_t mpcb200_episode_window_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts,
+                                              const mpcb200_window* window, int32_t elem_size) {
+  (void)opts;
+  if (dims == nullptr || window == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
+  const mpcb200_dims ds = window_solve_dims(dims, window);
+  const int knob = kernel_knob();
+  return window_layout(&ds, window, episode_layout(&ds, (size_t)elem_size, knob).total, (size_t)elem_size).total;
+}
+#define MPCB200_EPISODE_WINDOW(SUF, R)                                                                             \
+  int mpcb200_episode_window_##SUF(const mpcb200_dims* dims, const mpcb200_params* params,                         \
+                                   const mpcb200_ilqr_opts* opts, const mpcb200_window* window,                    \
+                                   const mpcb200_plant* plant, int32_t n_steps, const R* C, const R* c, const R* F, \
+                                   const R* f, const R* F_plant, const R* f_plant, const R* w, const R* x_init,    \
+                                   const R* u_init, const R* u_lower, const R* u_upper, const uint8_t* u_zero_I,   \
+                                   R* xs, R* us, R* costs, int32_t* info, R* u_next, R* plan_x, R* plan_u,         \
+                                   void* workspace, size_t workspace_bytes, void* stream) {                        \
+    EpisodeCall<R> e = {dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs, us, \
+                        costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u, plant, F_plant, f_plant, w}; \
+    return episode_window_impl<R>(e, window, stream);                                                              \
+  }
+MPCB200_EPISODE_WINDOW(f32, float)
+MPCB200_EPISODE_WINDOW(f64, double)
+#undef MPCB200_EPISODE_WINDOW
+
+size_t mpcb200_episode_backward_window_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev,
+                                                       const mpcb200_window* window, const mpcb200_plant* plant,
+                                                       int32_t elem_size) {
+  if (dims == nullptr || window == nullptr || check_dims(dims) != 0 || dims->T < 3 || n_prev < 0 ||
+      (elem_size != 4 && elem_size != 8))
+    return 0;
+  if (n_prev != 0 ? !slew_dims_ok(dims, n_prev)
+                  : dims->dynamics_kind != DYN_LINEAR && (dyn_nparams(dims->dynamics_kind) == 0 || !known_shape_ok(dims)))
+    return 0;
+  if (plant != nullptr && plant_check(dims, plant) != 0) return 0;
+  const mpcb200_dims ds = window_solve_dims(dims, window);
+  const int knob = kernel_knob();
+  return window_layout(&ds, window, epgrad_window_base(&ds, plant, (size_t)elem_size, knob), (size_t)elem_size).total;
+}
+#define MPCB200_EPISODE_BACKWARD_WINDOW(SUF, R)                                                                    \
+  int mpcb200_episode_backward_window_##SUF(                                                                       \
+      const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_window* window,                         \
+      const mpcb200_plant* plant, int32_t n_steps, int32_t n_prev, const R* C, const R* c, const R* F,             \
+      const R* F_plant, const R* u_lower, const R* u_upper, const R* xs, const R* us, const R* plan_x,             \
+      const R* plan_u, const R* dl_dxs, const R* dl_dus, R* dx_init, R* dC, R* dc, R* dF, R* df, R* dtheta,        \
+      R* dF_plant, R* df_plant, R* dtheta_plant, R* dw, void* workspace, size_t workspace_bytes, void* stream) {    \
+    if (n_prev < 0) return MPCB200_ERR_BAD_DIMS;                                                                   \
+    EpGradCall<R> q = {dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,   \
+                       dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, n_prev > 0, n_prev, plant,     \
+                       F_plant, dF_plant, df_plant, dtheta_plant, dw};                                             \
+    return epgrad_window_impl<R>(q, window, stream);                                                               \
+  }
+MPCB200_EPISODE_BACKWARD_WINDOW(f32, float)
+MPCB200_EPISODE_BACKWARD_WINDOW(f64, double)
+#undef MPCB200_EPISODE_BACKWARD_WINDOW
 
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }
 

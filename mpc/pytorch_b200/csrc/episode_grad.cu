@@ -27,12 +27,32 @@ __global__ void __launch_bounds__(256) fill_zero_kernel(size_t n, R* __restrict_
     p[i] = R(0);
 }
 
+// slices k .. k+n-1 of each windowed input into its fixed buffer (WindowCopy, episode_grad.cuh)
+template <typename R>
+__global__ void __launch_bounds__(256) window_stage_kernel(const WindowCopy<R> w) {
+  const long long k = *w.k;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+#pragma unroll 1
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    if (w.src[a] == nullptr) continue;
+    const size_t slice = (size_t)w.slice[a], len = (size_t)w.n[a] * slice;
+    const long long ts = w.tstride[a];
+    const R* __restrict__ src = w.src[a] + (ts < 0 ? 0 : k * ts);
+    R* __restrict__ dst = w.dst[a];
+    for (size_t i = i0; i < len; i += step) {
+      const size_t t = i / slice, j = i - t * slice;
+      dst[i] = src[ts < 0 ? j : t * (size_t)ts + j];
+    }
+  }
+}
+
 // g = dl_dxs[n_steps]; the accumulators and the adjoint's incoming gradients zeroed; k = n_steps - 1; the loop's
 // handle set to 1.  DETACH (a slew-rate episode): g's first n_prev entries, the previous control, are 0.  PLANT:
 // the plant's accumulators zeroed too, and dw[n_steps-1] = g
-template <typename R, bool DETACH, bool PLANT>
+// WINDOW: the full-length outputs of EpWindow are zeroed over their whole length.
+template <typename R, bool DETACH, bool PLANT, bool WINDOW = false>
 __device__ __forceinline__ void epgrad_init_body(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>& pl,
-                                                 cudaGraphConditionalHandle handle) {
+                                                 cudaGraphConditionalHandle handle, const EpWindow& wn = EpWindow{}) {
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
   for (size_t i = i0; i < B * N; i += step) {
@@ -40,25 +60,50 @@ __device__ __forceinline__ void epgrad_init_body(const EpGradArgs<R>& a, int n_p
     a.g[i] = v;
     if (PLANT && pl.dw != nullptr) pl.dw[(size_t)(a.n_steps - 1) * B * N + i] = v;
   }
-  if (PLANT) {
-    if (pl.kind == DYN_LINEAR) {
-      for (size_t i = i0; i < B * N * P; i += step) pl.dF[i] = R(0);
-      if (pl.has_f)
-        for (size_t i = i0; i < B * N; i += step) pl.df[i] = R(0);
-    } else {
-      for (size_t i = i0; i < B * pl.NP; i += step) pl.dtheta[i] = R(0);
+  if constexpr (WINDOW) {             // the full-length outputs over their whole length
+    const size_t tC = wn.cost ? (size_t)wn.L : T, tp = PLANT && wn.step ? (size_t)wn.Lp : 1;
+    const size_t tF = wn.dyn ? (size_t)wn.LF : (size_t)a.F_T, tf = wn.dyn ? (size_t)wn.Lf : T - 1;
+    if (PLANT) {
+      if (pl.kind == DYN_LINEAR) {
+        for (size_t i = i0; i < tp * B * N * P; i += step) pl.dF[i] = R(0);
+        if (pl.has_f)
+          for (size_t i = i0; i < tp * B * N; i += step) pl.df[i] = R(0);
+      } else {
+        for (size_t i = i0; i < B * pl.NP; i += step) pl.dtheta[i] = R(0);
+      }
     }
-  }
-  for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] = R(0);
-  for (size_t i = i0; i < T * B * P; i += step) a.dc[i] = R(0);
-  for (size_t i = i0; i < T * B * N; i += step) a.dl_dx[i] = R(0);
-  for (size_t i = i0; i < T * B * M; i += step) a.dl_du[i] = R(0);
-  if (a.kind == DYN_LINEAR) {
-    for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) a.dF[i] = R(0);
-    if (a.has_f)
-      for (size_t i = i0; i < (T - 1) * B * N; i += step) a.df[i] = R(0);
+    for (size_t i = i0; i < tC * B * P * P; i += step) a.dC[i] = R(0);
+    for (size_t i = i0; i < tC * B * P; i += step) a.dc[i] = R(0);
+    for (size_t i = i0; i < T * B * N; i += step) a.dl_dx[i] = R(0);
+    for (size_t i = i0; i < T * B * M; i += step) a.dl_du[i] = R(0);
+    if (a.kind == DYN_LINEAR) {
+      for (size_t i = i0; i < tF * B * N * P; i += step) a.dF[i] = R(0);
+      if (a.has_f)
+        for (size_t i = i0; i < tf * B * N; i += step) a.df[i] = R(0);
+    } else {
+      for (size_t i = i0; i < B * a.NP; i += step) a.dtheta[i] = R(0);
+    }
   } else {
-    for (size_t i = i0; i < B * a.NP; i += step) a.dtheta[i] = R(0);
+    if (PLANT) {
+      if (pl.kind == DYN_LINEAR) {
+        for (size_t i = i0; i < B * N * P; i += step) pl.dF[i] = R(0);
+        if (pl.has_f)
+          for (size_t i = i0; i < B * N; i += step) pl.df[i] = R(0);
+      } else {
+        for (size_t i = i0; i < B * pl.NP; i += step) pl.dtheta[i] = R(0);
+      }
+    }
+    for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] = R(0);
+    for (size_t i = i0; i < T * B * P; i += step) a.dc[i] = R(0);
+    for (size_t i = i0; i < T * B * N; i += step) a.dl_dx[i] = R(0);
+    for (size_t i = i0; i < T * B * M; i += step) a.dl_du[i] = R(0);
+    if (a.kind == DYN_LINEAR) {
+      for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) a.dF[i] = R(0);
+      if (a.has_f)
+        for (size_t i = i0; i < (T - 1) * B * N; i += step) a.df[i] = R(0);
+    } else {
+      for (size_t i = i0; i < B * a.NP; i += step) a.dtheta[i] = R(0);
+    }
   }
   if (i0 == 0) {
     a.st->k = a.n_steps - 1; a.st->tickets = 0u; a.st->reserved[0] = a.st->reserved[1] = 0;
@@ -80,6 +125,12 @@ epgrad_init_plant_kernel(const EpGradArgs<R> a, const EpPlantArgs<R> pl, int n_p
                          cudaGraphConditionalHandle handle) {
   epgrad_init_body<R, true, true>(a, n_prev, pl, handle);
 }
+template <typename R, bool PLANT>
+__global__ void __launch_bounds__(256)
+epgrad_init_window_kernel(const EpGradArgs<R> a, const EpPlantArgs<R> pl, const EpWindow wn, int n_prev,
+                          cudaGraphConditionalHandle handle) {
+  epgrad_init_body<R, true, PLANT, true>(a, n_prev, pl, handle, wn);
+}
 
 // the plan of step k into the fixed buffers the body's launchers read
 template <typename R>
@@ -90,20 +141,23 @@ __device__ __forceinline__ void epgrad_stage_plan(const EpGradArgs<R>& a, size_t
 }
 
 // LinDx: x' = F[0] z + f[0] with z = [x_k; u_k].  One thread per (b, column j of F[0]): column j of F[0]^T g goes
-// to gx (j < N) or into dl_du[0] (j >= N), and column j of dF[0] takes g z_j.
-template <typename R>
-__global__ void __launch_bounds__(256) epgrad_stage_linear_kernel(const EpGradArgs<R> a) {
+// to gx (j < N) or into dl_du[0] (j >= N), and column j of dF[0] takes g z_j.  WINDOW: F[0] is the staged window's
+// F[k], and g z^T, g go into slice k of the full-length dF, df.
+template <typename R, bool WINDOW>
+__device__ __forceinline__ void epgrad_stage_linear_body(const EpGradArgs<R>& a) {
   const size_t k = (size_t)a.st->k;
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   epgrad_stage_plan(a, k, i0, step);
   const int N = a.N, M = a.M, P = N + M;
   const size_t B = a.B;
+  R* const dF = WINDOW ? a.dF + k * B * N * P : a.dF;
+  R* const df = WINDOW && a.has_f ? a.df + k * B * N : a.df;
   for (size_t idx = i0; idx < B * P; idx += step) {
     const size_t b = idx / P;
     const int j = (int)(idx % P);
     const R* g = a.g + b * N;
     const R* Fb = a.F + b * N * P;
-    R* dFb = a.dF + b * N * P;
+    R* dFb = dF + b * N * P;
     const R zj = j < N ? a.xs[(k * B + b) * N + j] : a.us[(k * B + b) * M + (j - N)];
     R v = R(0);
     for (int i = 0; i < N; ++i) {
@@ -114,8 +168,16 @@ __global__ void __launch_bounds__(256) epgrad_stage_linear_kernel(const EpGradAr
     if (j < N) a.gx[b * N + j] = v;
     else a.dl_du[b * M + (j - N)] = a.dl_dus[(k * B + b) * M + (j - N)] + v;
     if (a.has_f && j == 0)
-      for (int i = 0; i < N; ++i) a.df[b * N + i] += g[i];
+      for (int i = 0; i < N; ++i) df[b * N + i] += g[i];
   }
+}
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_stage_linear_kernel(const EpGradArgs<R> a) {
+  epgrad_stage_linear_body<R, false>(a);
+}
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_stage_linear_window_kernel(const EpGradArgs<R> a) {
+  epgrad_stage_linear_body<R, true>(a);
 }
 
 // A known system: R, S by the forward-mode duals dyn_linearize_kernel uses, and theta_step = sum_r g_r dx'_r/dtheta
@@ -175,9 +237,10 @@ __global__ void __launch_bounds__(256) epgrad_stage_known_kernel(const EpGradArg
 // theta_step[b] + sum_t (first + second)[t, b] in t order.  The last block to finish counts k down and ends the
 // loop after k = 0: every block has read st->k by then.  DETACH: g's first n_prev entries are 0, as in init.
 // PLANT: theta_step is the plant's and goes into the plant's dtheta, not into the model's; dw[k-1] = g (k > 0).
-template <typename R, bool DETACH, bool PLANT>
+// WINDOW: step k's dC_k, dc_k (wn.cost) and dF_k, df_k (wn.dyn) go into the full-length outputs at offset k.
+template <typename R, bool DETACH, bool PLANT, bool WINDOW = false>
 __device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>& pl,
-                                                  cudaGraphConditionalHandle handle) {
+                                                  cudaGraphConditionalHandle handle, const EpWindow& wn = EpWindow{}) {
   const int k = a.st->k;
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   const size_t B = a.B, T = a.T, N = a.N, M = a.M, P = N + M;
@@ -188,12 +251,30 @@ __device__ __forceinline__ void epgrad_accum_body(const EpGradArgs<R>& a, int n_
   }
   if (PLANT && pl.kind != DYN_LINEAR)
     for (size_t i = i0; i < B * pl.NP; i += step) pl.dtheta[i] += pl.theta_step[i];
-  for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] += a.dC_k[i];
-  for (size_t i = i0; i < T * B * P; i += step) a.dc[i] += a.dc_k[i];
+  if constexpr (WINDOW) {             // at offset k in the full-length outputs
+    const size_t kc = wn.cost ? (size_t)k : 0, kd = wn.dyn ? (size_t)k : 0;
+    R* const dC = a.dC + kc * B * P * P;
+    R* const dc = a.dc + kc * B * P;
+    for (size_t i = i0; i < T * B * P * P; i += step) dC[i] += a.dC_k[i];
+    for (size_t i = i0; i < T * B * P; i += step) dc[i] += a.dc_k[i];
+    if (a.kind == DYN_LINEAR) {
+      R* const dF = a.dF + kd * B * N * P;
+      for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) dF[i] += a.dF_k[i];
+      if (a.has_f) {
+        R* const df = a.df + kd * B * N;
+        for (size_t i = i0; i < (T - 1) * B * N; i += step) df[i] += a.df_k[i];
+      }
+    }
+  } else {
+    for (size_t i = i0; i < T * B * P * P; i += step) a.dC[i] += a.dC_k[i];
+    for (size_t i = i0; i < T * B * P; i += step) a.dc[i] += a.dc_k[i];
+  }
   if (a.kind == DYN_LINEAR) {
-    for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) a.dF[i] += a.dF_k[i];
-    if (a.has_f)
-      for (size_t i = i0; i < (T - 1) * B * N; i += step) a.df[i] += a.df_k[i];
+    if (!WINDOW) {
+      for (size_t i = i0; i < (size_t)a.F_T * B * N * P; i += step) a.dF[i] += a.dF_k[i];
+      if (a.has_f)
+        for (size_t i = i0; i < (T - 1) * B * N; i += step) a.df[i] += a.df_k[i];
+    }
   } else {
     const size_t NP = a.NP;
     for (size_t i = i0; i < B * NP; i += step) {
@@ -228,6 +309,12 @@ epgrad_accum_plant_kernel(const EpGradArgs<R> a, const EpPlantArgs<R> pl, int n_
                           cudaGraphConditionalHandle handle) {
   epgrad_accum_body<R, true, true>(a, n_prev, pl, handle);
 }
+template <typename R, bool PLANT>
+__global__ void __launch_bounds__(256)
+epgrad_accum_window_kernel(const EpGradArgs<R> a, const EpPlantArgs<R> pl, const EpWindow wn, int n_prev,
+                           cudaGraphConditionalHandle handle) {
+  epgrad_accum_body<R, true, PLANT, true>(a, n_prev, pl, handle, wn);
+}
 
 template <typename R>
 int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
@@ -235,6 +322,17 @@ int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* b
   const size_t nx = (size_t)T * B * N, nu = (size_t)T * B * M;
   episode_plans_kernel<R><<<epgrad_grid(nx > nu ? nx : nu), 256, 0, stream>>>(nx, nu, best_x, best_u, plan_x, plan_u,
                                                                               ep);
+  return launched();
+}
+
+template <typename R>
+int window_launch_stage(const WindowCopy<R>& w, cudaStream_t stream) {
+  size_t items = 0;
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    const size_t len = w.src[a] != nullptr ? (size_t)w.n[a] * (size_t)w.slice[a] : 0;
+    if (len > items) items = len;
+  }
+  window_stage_kernel<R><<<epgrad_grid(items), 256, 0, stream>>>(w);
   return launched();
 }
 
@@ -258,6 +356,39 @@ int epgrad_launch_init(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>*
     epgrad_init_plant_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, *pl, n_prev, handle);
   else if (n_prev == 0) epgrad_init_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, handle);
   else epgrad_init_detach_kernel<R><<<epgrad_grid(epgrad_items(a)), 256, 0, stream>>>(a, n_prev, handle);
+  return launched();
+}
+
+// the largest grid-stride range of the window forms of init and accumulate: dC over the axis
+template <typename R>
+static size_t epgrad_window_items(const EpGradArgs<R>& a, const EpWindow& wn) {
+  const size_t P = (size_t)a.N + a.M;
+  return (size_t)(wn.cost ? wn.L : a.T) * a.B * P * P;
+}
+
+template <typename R>
+int epgrad_launch_init_window(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl, const EpWindow& wn,
+                              cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  const unsigned grid = epgrad_grid(epgrad_window_items(a, wn));
+  if (pl != nullptr) epgrad_init_window_kernel<R, true><<<grid, 256, 0, stream>>>(a, *pl, wn, n_prev, handle);
+  else epgrad_init_window_kernel<R, false><<<grid, 256, 0, stream>>>(a, EpPlantArgs<R>{}, wn, n_prev, handle);
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_accum_window(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl, const EpWindow& wn,
+                               cudaGraphConditionalHandle handle, cudaStream_t stream) {
+  const unsigned grid = epgrad_grid(epgrad_items(a));
+  if (pl != nullptr) epgrad_accum_window_kernel<R, true><<<grid, 256, 0, stream>>>(a, *pl, wn, n_prev, handle);
+  else epgrad_accum_window_kernel<R, false><<<grid, 256, 0, stream>>>(a, EpPlantArgs<R>{}, wn, n_prev, handle);
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_stage_window(const EpGradArgs<R>& a, const EpWindow& wn, cudaStream_t stream) {
+  if (a.kind != DYN_LINEAR || !wn.step) return epgrad_launch_stage<R>(a, stream);
+  const size_t items = (size_t)a.T * a.B * (a.N > a.M ? a.N : a.M);
+  epgrad_stage_linear_window_kernel<R><<<epgrad_grid(items), 256, 0, stream>>>(a);
   return launched();
 }
 
@@ -317,7 +448,13 @@ int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream) {
   template int epgrad_launch_stage<R>(const EpGradArgs<R>&, cudaStream_t);                                         \
   template int epgrad_launch_accum<R>(const EpGradArgs<R>&, int, const EpPlantArgs<R>*,                            \
                                       cudaGraphConditionalHandle, cudaStream_t);                                   \
-  template int epgrad_launch_vjp_passthrough<R>(const DynVjpArgs&, cudaStream_t);
+  template int epgrad_launch_vjp_passthrough<R>(const DynVjpArgs&, cudaStream_t);                                  \
+  template int window_launch_stage<R>(const WindowCopy<R>&, cudaStream_t);                                         \
+  template int epgrad_launch_init_window<R>(const EpGradArgs<R>&, int, const EpPlantArgs<R>*, const EpWindow&,     \
+                                            cudaGraphConditionalHandle, cudaStream_t);                             \
+  template int epgrad_launch_accum_window<R>(const EpGradArgs<R>&, int, const EpPlantArgs<R>*, const EpWindow&,    \
+                                             cudaGraphConditionalHandle, cudaStream_t);                            \
+  template int epgrad_launch_stage_window<R>(const EpGradArgs<R>&, const EpWindow&, cudaStream_t);
 MPCB200_EPGRAD_INST(float)
 MPCB200_EPGRAD_INST(double)
 

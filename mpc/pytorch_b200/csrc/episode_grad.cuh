@@ -19,6 +19,8 @@
 // (mpcb200_episode_backward_plant_*): step a. runs on the plant (its kind, dp, F; its dF, df, theta_step), and the
 // *_plant_kernel forms of init and accumulate zero and sum the plant's own accumulators, keep theta_step out of the
 // model's dtheta, and write dw[k] = g.  They apply the detach rule too, with n_prev = 0 meaning none.
+// A time-varying episode (mpcb200_episode_backward_window_*): window_stage_kernel stages step k's window first, and
+// the *_window_kernel forms zero the full-length outputs and add each step's gradients at offset k (EpWindow).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -60,7 +62,43 @@ struct EpPlantArgs {
   R* dw;                  // dL/dw [n_steps, B, N] (dw[k] = dL/dx_{k+1}), or NULL
 };
 
+// A time-varying episode (mpcb200_episode_window_*, mpcb200_episode_backward_window_*): window_stage_kernel, the
+// first node of each control step's body (forward and sweep), copies slices k .. k+n-1 of each windowed input into
+// the fixed buffers the body's nodes were recorded with, k read from the device-resident step counter (EpisodeState
+// step, EpGradState k).  One grid-stride loop per input.  tstride: elements between the source's slices, < 0 for a
+// time-invariant source (every slice reads its one slice).
+constexpr int WINDOW_INPUTS = 8;      // C, c, F, f, u_lower, u_upper, F_plant, f_plant
+template <typename R>
+struct WindowCopy {
+  const R* src[WINDOW_INPUTS];        // NULL: not windowed
+  R* dst[WINDOW_INPUTS];
+  long long tstride[WINDOW_INPUTS];
+  long long slice[WINDOW_INPUTS];     // elements per slice
+  int n[WINDOW_INPUTS];               // slices copied
+  const int32_t* k;
+};
+
+// The sweep's window (the *_window_kernel forms of init, stage and accumulate): which outputs are full length, and
+// their slice counts.  Solve k's dC_k, dc_k (cost) and dF_k, df_k (dyn) go in at offset k; the stage's g z^T and g
+// go into slice k of the stepping LinDx's dF, df (step).
+struct EpWindow {
+  int cost, dyn, step;    // dC, dc on the axis; the model's dF, df; the stepping LinDx's dF, df (plant or model)
+  int L, LF, Lf, Lp;      // slices of dC / dc, of the model's dF, of its df, of the plant's dF / df
+};
+
 // Launchers (episode_grad.cu), instantiated for float and double; 0 or MPCB200_ERR_LAUNCH.
+template <typename R>
+int window_launch_stage(const WindowCopy<R>& w, cudaStream_t stream);
+// the *_window_kernel forms of init and accumulate (the plant forms when pl is non-NULL); n_prev as below
+template <typename R>
+int epgrad_launch_init_window(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl, const EpWindow& wn,
+                              cudaGraphConditionalHandle handle, cudaStream_t stream);
+template <typename R>
+int epgrad_launch_accum_window(const EpGradArgs<R>& a, int n_prev, const EpPlantArgs<R>* pl, const EpWindow& wn,
+                               cudaGraphConditionalHandle handle, cudaStream_t stream);
+// epgrad_launch_stage, with a LinDx step's parameter part added into slice k of its dF, df when wn.step
+template <typename R>
+int epgrad_launch_stage_window(const EpGradArgs<R>& a, const EpWindow& wn, cudaStream_t stream);
 template <typename R>
 int episode_launch_plans(int B, int T, int N, int M, const R* best_x, const R* best_u, R* plan_x, R* plan_u,
                          const EpisodeState* ep, cudaStream_t stream);

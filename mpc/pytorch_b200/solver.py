@@ -286,15 +286,16 @@ class MPC(Module):
         x = res["x"][:, :, m:] if self.slew_rate_penalty is not None else res["x"]
         return {"x": x, "u": res["u"], "costs": res["costs"], "full_du_norm": res["full_du_norm"], "info": res["info"]}
 
-    def _device_problem(self, x_init, cost, dx):
+    def _device_problem(self, x_init, cost, dx, T=None):
         """The problem of the device loop, staged once per solve (or episode): (n, x_init, C, c, F, f, dyn).  With a
         slew-rate penalty, the augmented problem over [u_{t-1}; x] (n = n_state + n_ctrl).  dyn = (kind, params) of a
-        known system, with F = f = None; None for LinDx."""
+        known system, with F = f = None; None for LinDx.  T: the length of C's time axis when it is not the solve's
+        (a time-varying episode's, control.receding_horizon)."""
         n, m = self.n_state, self.n_ctrl
         C, c = cost.C, cost.c
         F, f = (dx.F, dx.f) if isinstance(dx, LinDx) else (None, None)
         if self.slew_rate_penalty is not None:
-            _, C, c, F, f, _, x_init = self._slew_augment(x_init, C, c, F, f)
+            _, C, c, F, f, _, x_init = self._slew_augment(x_init, C, c, F, f, T=T)
             if not isinstance(dx, LinDx):
                 dx = CtrlPassthroughDynamics(dx)
             n = n + m
@@ -422,11 +423,13 @@ class MPC(Module):
         xo, *rest = _lqr(x_init2, C2, c2, F2, f2)
         return [xo[:, :, m:]] + list(rest)
 
-    def _slew_augment(self, x_init, C, c, F, f):
+    def _slew_augment(self, x_init, C, c, F, f, T=None):
         """The slew-rate augmented problem over the state [u_{t-1}; x] (reference :362-445): (slew_C, C2, c2, F2, f2,
         prev_u[1,B,m], x_init2).  F2 = [[0, 0, I], [0, F]] and f2 = [0; f] (empty without f); both None without F
-        (a known system, which the kernels linearise in augmented form).  Differentiable in C, c, F, f and x_init."""
-        n, m, T = self.n_state, self.n_ctrl, self.T
+        (a known system, which the kernels linearise in augmented form).  Differentiable in C, c, F, f and x_init.
+        T: C's time axis when it is not the solve's (a time-varying episode's); each slice is augmented alike."""
+        n, m = self.n_state, self.n_ctrl
+        T = self.T if T is None else T
         B = C.size(1)
         n2, p2 = n + m, n + 2 * m
         kw = dict(dtype=C.dtype, device=C.device)

@@ -257,8 +257,10 @@ class _Pad:
 
 # n_prev: an episode's slew-rate augmentation, the leading states that hold the previous control (0: none); plant: the
 # _StagedPlant of an episode closed on a plant other than the model (None: the model steps it)
-_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev plant",
-                                  defaults=(0, None))
+# window: the mpcb200_window record of a time-varying episode (episode_raw(..., window=L)), whose C, c, F, f and
+# bounds are then the staged full-length inputs (the solve's own where the record does not window them)
+_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev plant window",
+                                  defaults=(0, None, None))
 # rec: the mpcb200_plant record; F, f: a LinDx plant's slice 0 at the problem's (padded) sizes [B, N, N+M], [B, N]
 # (f None without one); disturbed: the episode added w
 _StagedPlant = collections.namedtuple("_StagedPlant", "rec F f disturbed")
@@ -445,7 +447,7 @@ def ilqr_raw(n_state, n_ctrl, T, x_init, C, c, F, f, u_init, u_lower=None, u_upp
 
 def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
-                best_cost_eps=1e-4, dyn=None, keep_plans=False, n_prev=0, plant=None, w=None):
+                best_cost_eps=1e-4, dyn=None, keep_plans=False, n_prev=0, plant=None, w=None, window=None):
     """A receding-horizon episode of n_steps control steps in ONE library call (mpcb200_episode_*): each step solves
     the problem from the current state as ilqr_raw does (u_init = the warm start), applies the plan's first control,
     steps the model (LinDx: F[0] [x; u] + f[0]; a known system `dyn`: one step of it) and shifts the warm start
@@ -460,10 +462,17 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     plant (mpcb200_episode_plant_*): what steps the loop instead of the model, (DYN_LINEAR, None, F_p, f_p) for a
     LinDx's t = 0 slice or (kind, params, None, None) for a known system (_stage_plant); w [n_steps, B, n]: added to
     each step, x_{k+1} = plant(x_k, u_k) + w_k (under a slew-rate penalty its first n_prev entries are the caller's
-    zeros).  Either one takes that entry; the staged problem records the plant for episode_backward_raw."""
+    zeros).  Either one takes that entry; the staged problem records the plant for episode_backward_raw.
+    window = L (mpcb200_episode_window_*): a time-varying episode whose inputs lie on its time axis of
+    L = n_steps + T - 1 slices (_episode_window)."""
     n, m = n_state, n_ctrl
     if T < 3 or n_steps < 1:
         raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
+    if window is not None:
+        return _episode_window(n, m, T, n_steps, window, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I,
+                               delta_u, linesearch_decay, max_linesearch_iter, dyn, keep_plans, n_prev, plant, w,
+                               _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m,
+                                             eps=float(eps), best_cost_eps=float(best_cost_eps)))
     B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
                   F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
                   dyn_kind=dyn[0] if dyn is not None else None, need_F=dyn is None)
@@ -520,6 +529,163 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     return res
 
 
+def _episode_window(n, m, T, n_steps, L, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I, delta_u,
+                    linesearch_decay, max_linesearch_iter, dyn, keep_plans, n_prev, plant, w, opts):
+    """episode_raw on a time-varying problem (mpcb200_episode_window_*).  C [L, B, p, p], c [L, B, p], a LinDx
+    model's F [L-1|L, B, n, p] and f [L-1|L, B, n], tensor bounds [L, B, m] and a LinDx plant's F_p, f_p [L-1|L, ...]
+    lie on the episode's axis, L = n_steps + T - 1; u_init and u_zero_I are the solve's [T, B, m].  Solve k plans on
+    slices k .. k+T-1 (F: k .. k+F_T-1, F_T = T - (L - len(F))), and control step k steps with slice k of a LinDx
+    model or plant.  The per-solve problem is _problem's on the first window (its Dims, _Pad and widened u_zero_I);
+    the full-length inputs are staged once, by the same _Pad widening, and the library copies each window on the
+    device.  Same outputs as episode_raw; "saved" holds the staged full-length inputs and the window record."""
+    if L != n_steps + T - 1:
+        raise MpcB200Error(f"window: a time-varying episode of {n_steps} steps at T={T} has an axis of "
+                           f"{n_steps + T - 1} slices, got {L}")
+    B = _validate(n, m, L, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), F=F, f=f,
+                  bounds=(u_lower, u_upper), dyn_kind=dyn[0] if dyn is not None else None, need_F=dyn is None)
+    dtype, dev = C.dtype, C.device
+    for name, t in (("u_init", u_init), ("u_zero_I", u_zero_I)):
+        if t is not None and tuple(t.shape) != (T, B, m):
+            raise MpcB200Error(f"{name}: expected shape {(T, B, m)}, got {tuple(t.shape)}")
+    F_T = None if _is_empty(F) else T - (L - F.shape[0])
+
+    def first(b):                         # the first window of a tensor bound
+        return b[:T] if isinstance(b, torch.Tensor) else b
+    s = _problem(n, m, T, B, dtype, dev, C[:T], c[:T], F[:F_T] if F_T else None, None if _is_empty(f) else f[:T - 1],
+                 first(u_lower), first(u_upper), u_zero_I, delta_u, linesearch_decay, max_linesearch_iter, dyn)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    rec = _lib.Window(L=int(L), on=_lib.WIN_COST)
+    C_, rec.C_tstride = pad.stage(C, dtype, pad.mat_pp)
+    c_, rec.c_tstride = pad.stage(c, dtype, pad.vec_p)
+    F_, f_ = s.F, s.f
+    if dyn is None:
+        rec.on |= _lib.WIN_DYN
+        F_, rec.F_tstride = pad.stage(F, dtype, pad.mat_np)
+        f_, rec.f_tstride = pad.stage(f, dtype, pad.vec_n)
+    lo_, hi_ = s.u_lower, s.u_upper
+    if isinstance(u_lower, torch.Tensor) or isinstance(u_upper, torch.Tensor):
+        rec.on |= _lib.WIN_BOUNDS
+        _, _, _, lo_t, hi_t = _bounds(u_lower, u_upper, (L, B, m), dtype, dev, pad.active)
+        lo_, hi_ = pad.vec_m(lo_t, -1.0).contiguous(), pad.vec_m(hi_t, 1.0).contiguous()
+    x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
+    sp = w_ = None
+    if plant is not None or w is not None:
+        if plant is None:                 # the model steps, disturbed
+            plant = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
+        sp = _stage_plant_window(pad, plant, dtype, B, n, m, L, rec)
+        if w is not None:
+            if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
+                raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
+                                   f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
+            w_ = pad.vec_n(_dense(w, dtype)).contiguous()
+            sp = sp._replace(disturbed=True)
+    nbytes = _lib.lib().mpcb200_episode_window_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts),
+                                                               ctypes.byref(rec), C.element_size())
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    xs = torch.empty(n_steps + 1, B, N, dtype=dtype, device=dev)
+    us = torch.empty(n_steps, B, M, dtype=dtype, device=dev)
+    costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
+    info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
+    u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
+    plan_x = plan_u = None
+    if keep_plans:
+        plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
+        plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
+    fn = _lib.entry("mpcb200_episode_window", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), ctypes.byref(rec),
+                ctypes.byref(sp.rec) if sp is not None else None, int(n_steps), ptr_view(C_), ptr_view(c_),
+                ptr_view(F_), ptr_view(f_), ptr_view(sp.F) if sp is not None else None,
+                ptr_view(sp.f) if sp is not None else None, ptr(w_), ptr(x0_), ptr(u0_), ptr(lo_), ptr(hi_),
+                ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info), ptr(u_next), ptr(plan_x), ptr(plan_u),
+                ptr(ws), nbytes, stream_handle(dev))
+    if rc == _lib.ERR_NO_GRAPH_COND:
+        return None
+    check(rc, "mpcb200_episode_window")
+    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
+    if keep_plans:
+        res["saved"] = (s._replace(C=C_, c=c_, F=F_, f=f_, u_lower=lo_, u_upper=hi_, n_prev=int(n_prev), plant=sp,
+                                   window=rec), n_steps, xs, us, plan_x, plan_u)
+    return res
+
+
+def _stage_plant_window(pad, plant, dtype, B, n, m, L, rec):
+    """_stage_plant for a time-varying episode: a LinDx plant's F_p, f_p [L-1|L, B, ...] staged whole (its slice k
+    steps control step k; MPCB200_WIN_PLANT set in `rec`); a known plant as _stage_plant stages it."""
+    kind, _, F_p, f_p = plant
+    if kind != DYN_LINEAR:
+        return _stage_plant(pad, plant, dtype, B, n, m)
+    for name, t, shape in (("plant F", F_p, (B, n, n + m)), ("plant f", f_p, (B, n))):
+        if name == "plant F" and t is None:
+            raise MpcB200Error("a LinDx plant needs F")
+        if not _is_empty(t) and (t.dim() != len(shape) + 1 or t.shape[0] not in (L - 1, L) or
+                                 tuple(t.shape[1:]) != shape):
+            raise MpcB200Error(f"{name}: expected shape ({L - 1} or {L}, {', '.join(map(str, shape))}), "
+                               f"got {tuple(t.shape)}")
+    prec = _lib.Plant(kind=int(kind))
+    rec.on |= _lib.WIN_PLANT
+    Fp, rec.Fp_tstride = pad.stage(F_p, dtype, pad.mat_np)
+    fp, rec.fp_tstride = pad.stage(f_p, dtype, pad.vec_n)
+    prec.has_f = int(fp is not None)
+    return _StagedPlant(prec, Fp, fp, False)
+
+
+def _episode_backward_window(s, n_steps, xs, us, plan_x, plan_u, gx_, gu_):
+    """episode_backward_raw of a time-varying episode (mpcb200_episode_backward_window_*): the gradients of the
+    windowed inputs are full length, with zero slices up to their inputs' lengths (slices no step reads)."""
+    pad, dims, rec = s.pad, s.dims, s.window
+    T, B, N, M, L = dims.T, dims.B, pad.N, pad.M, rec.L
+    dtype, dev = xs.dtype, xs.device
+    P = N + M
+    kind = dims.dynamics_kind
+    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
+    dC = torch.empty(L, B, P, P, dtype=dtype, device=dev)
+    dc = torch.empty(L, B, P, dtype=dtype, device=dev)
+    dF = df = dtheta = None
+    from .dynamics import DYN_NPARAMS
+    if kind == DYN_LINEAR:
+        dF = torch.empty(L - T + dims.F_T, B, N, P, dtype=dtype, device=dev)
+        if dims.has_f:
+            df = torch.empty(L - 1, B, N, dtype=dtype, device=dev)
+    else:
+        dtheta = torch.empty(B, DYN_NPARAMS[kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
+    sp = s.plant
+    dF_p = df_p = dth_p = dw = None
+    if sp is not None:
+        pk = sp.rec.kind
+        lead = (L - 1,) if rec.on & _lib.WIN_PLANT else ()
+        dF_p = torch.empty(*lead, B, N, P, dtype=dtype, device=dev) if pk == DYN_LINEAR else None
+        df_p = torch.empty(*lead, B, N, dtype=dtype, device=dev) if pk == DYN_LINEAR and sp.rec.has_f else None
+        dth_p = (torch.empty(B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
+                 if pk != DYN_LINEAR else None)
+        dw = torch.empty(n_steps, B, N, dtype=dtype, device=dev) if sp.disturbed else None
+    prec = ctypes.byref(sp.rec) if sp is not None else None
+    nbytes = _lib.lib().mpcb200_episode_backward_window_workspace_bytes(ctypes.byref(dims), int(s.n_prev),
+                                                                        ctypes.byref(rec), prec, xs.element_size())
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    name = "mpcb200_episode_backward_window"
+    fn = _lib.entry(name, dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(rec), prec, int(n_steps), int(s.n_prev),
+                ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr_view(sp.F) if sp is not None else None,
+                ptr(s.u_lower), ptr(s.u_upper), ptr(xs), ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_),
+                ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(dtheta), ptr(dF_p), ptr(df_p), ptr(dth_p),
+                ptr(dw), ptr(ws), nbytes, stream_handle(dev))
+    check(rc, name)
+
+    def full(g, t):                       # zero slices up to the input's length
+        if g is None or t is None or t.shape[0] == g.shape[0]:
+            return g
+        return torch.cat((g, g.new_zeros(t.shape[0] - g.shape[0], *g.shape[1:])), 0)
+    df = full(df, s.f)
+    if sp is not None and rec.on & _lib.WIN_PLANT:
+        dF_p, df_p = full(dF_p, sp.F), full(df_p, sp.f)
+    out = (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)
+    if sp is None:
+        return out
+    return out + (pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
+
+
 def episode_backward_raw(saved, dl_dxs, dl_dus):
     """The reverse sweep of an episode run by episode_raw(..., keep_plans=True) in ONE library call
     (mpcb200_episode_backward_*): `saved` is that call's res["saved"], dl_dxs [n_steps+1, B, n] and dl_dus
@@ -531,12 +697,16 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
     the caller crops the gradients to the system's own blocks.
     An episode closed on a plant (the staged problem's plant) runs mpcb200_episode_backward_plant_* and returns four
     more: dF_p [B, n, p] and df_p [B, n] (a LinDx plant's slice 0; df_p None without f), dtheta_p [B, NP_plant] (a
-    known plant) and dw [n_steps, B, n] (None when no w was added); dF, df or dtheta are then the solves' part only."""
+    known plant) and dw [n_steps, B, n] (None when no w was added); dF, df or dtheta are then the solves' part only.
+    A time-varying episode (episode_raw(..., window=L)) runs mpcb200_episode_backward_window_*: dC, dc, dF, df and a
+    windowed LinDx plant's dF_p, df_p are full length (_episode_backward_window)."""
     s, n_steps, xs, us, plan_x, plan_u = saved
     pad, dims = s.pad, s.dims
     T, B, N, M = dims.T, dims.B, pad.N, pad.M
     dtype, dev = xs.dtype, xs.device
     gx_, gu_ = pad.vec_n(_dense(dl_dxs, dtype)), pad.vec_m(_dense(dl_dus, dtype))
+    if s.window is not None:
+        return _episode_backward_window(s, n_steps, xs, us, plan_x, plan_u, gx_, gu_)
     kind = dims.dynamics_kind
     P = N + M
     dx_init = torch.empty(B, N, dtype=dtype, device=dev)

@@ -255,10 +255,42 @@ static int run_episode_plant() {
   return 0;
 }
 
+// the window entries' argument checks (they run before anything is captured): an axis one slice short and a window
+// on a known model's F are refused; the workspace is the episode's plus the window buffers
+static int run_episode_window() {
+  mpcb200_dims d = {4, 5, 3, 1, 4, 1, 0, 0, 0, 10, 20, 1, MPCB200_DYN_PENDULUM};
+  mpcb200_params prm = {0.0, 0.0, 0.0, 0.2, {10.0, 1.0, 1.0, 2.0, 0.05}};
+  mpcb200_ilqr_opts opts = {5, 5, 1, 0, 1e-7, 1e-4};
+  mpcb200_window win = {};
+  win.L = 3 + 5 - 1;
+  win.on = MPCB200_WIN_COST;
+  const size_t need = mpcb200_episode_window_workspace_bytes(&d, &opts, &win, 4);
+  const size_t bw = mpcb200_episode_backward_window_workspace_bytes(&d, 0, &win, nullptr, 4);
+  if (need <= mpcb200_episode_workspace_bytes(&d, &opts, 4) || bw == 0)
+    return printf("episode window workspace %zu / %zu\n", need, bw), 1;
+  Dev<float> buf(4096), ws((need > bw ? need : bw) / sizeof(float) + 64);
+  int32_t* info = (int32_t*)buf.p;
+  float* p = buf.p;
+  win.L -= 1;
+  int rc = mpcb200_episode_window_f32(&d, &prm, &opts, &win, nullptr, 3, p, p, nullptr, nullptr, nullptr, nullptr,
+                                      nullptr, p, p, nullptr, nullptr, nullptr, p, p, p, info, p, nullptr, nullptr,
+                                      ws.p, need, nullptr);
+  if (rc != MPCB200_ERR_BAD_DIMS) return printf("episode window (short axis) rc=%d\n", rc), 1;
+  win.L += 1;
+  win.on |= MPCB200_WIN_DYN;
+  rc = mpcb200_episode_backward_window_f32(&d, &prm, &win, nullptr, 3, 0, p, p, p, nullptr, nullptr, nullptr, p, p, p,
+                                           p, p, p, p, p, p, nullptr, nullptr, p, nullptr, nullptr, nullptr, nullptr,
+                                           ws.p, bw, nullptr);
+  if (rc != MPCB200_ERR_BAD_DIMS) return printf("episode backward window (known F) rc=%d\n", rc), 1;
+  printf("episode window: workspace %zu / %zu bytes, short axis and known-model F window refused\n", need, bw);
+  return 0;
+}
+
 int main() {
   int fails = 0;
   fails += run_episode_backward_slew();
   fails += run_episode_plant();
+  fails += run_episode_window();
   fails += run_pnqp_large(3, 100);
   fails += run_dyn(MPCB200_DYN_CARTPOLE, 37, 9);
   fails += run_dyn(MPCB200_DYN_PENDULUM, 20, 7);
