@@ -617,6 +617,93 @@ int mpcb200_episode_backward_window_f64(const mpcb200_dims* dims, const mpcb200_
                                         double* dtheta, double* dF_plant, double* df_plant, double* dtheta_plant,
                                         double* dw, void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * A learned model in the kernels: the network of the reference's NNDynamics (mpc/dynamics.py:15-131),
+ * x' = [x +] MLP([x; u]), with n_layers Linear layers (1..4), an activation after every layer but the last, and the
+ * last layer linear.  width[0] = n_s + m_s (the network's own state and control counts), width[n_layers] = n_s,
+ * every width 1..MPCB200_MLP_MAX_WIDTH.  params: ONE device buffer of the element type holding every layer's weight
+ * W_i [width[i+1], width[i]] (row-major, as nn.Linear stores it) at element offset W_off[i] and bias b_i
+ * [width[i+1]] at b_off[i]; the kernels stage elements [0, max end) of it into shared memory per CTA.
+ * n_prev: 0, or m_s for the slew-rate augmented state [u_{t-1}; x] of CtrlPassthroughDynamics, stepped as
+ * [u; MLP(x, u)].  The calls work on a staged problem of N states and M controls (zero padded as the step is):
+ * the network reads states n_prev .. n_prev+n_s-1 and controls 0 .. m_s-1, N >= n_prev + n_s, M >= m_s and
+ * N + M <= n_prev + width[0] + MPCB200_MLP_PAD_SLACK (else MPCB200_ERR_BAD_DIMS); states past n_prev + n_s are
+ * written as 0.
+ */
+#define MPCB200_MLP_MAX_LAYERS 4
+#define MPCB200_MLP_MAX_WIDTH 256
+#define MPCB200_MLP_PAD_SLACK 16
+enum { MPCB200_ACT_SIGMOID = 0, MPCB200_ACT_RELU = 1, MPCB200_ACT_ELU = 2 };
+typedef struct mpcb200_mlp {
+  int32_t n_layers;
+  int32_t width[MPCB200_MLP_MAX_LAYERS + 1];
+  int32_t activation;     /* MPCB200_ACT_*; ELU with alpha = 1                                              */
+  int32_t passthrough;    /* 1: x' = x + MLP(z)                                                             */
+  int32_t n_prev;
+  int32_t reserved0;
+  const void* params;
+  int64_t W_off[MPCB200_MLP_MAX_LAYERS];
+  int64_t b_off[MPCB200_MLP_MAX_LAYERS];
+} mpcb200_mlp;
+
+/* 1 if the kernels below take the network in elem_size-byte elements: its parameters plus one warp's activation
+ * buffers fit the opt-in shared memory of an H100 (227 KB); 0 otherwise or for a malformed record.  Needs no
+ * device.  A caller keeps its own path for a network that does not fit. */
+int mpcb200_mlp_fits(const mpcb200_mlp* mlp, int32_t elem_size);
+
+/* x[T,B,N]: x[0] = x_init[B,N], x[t+1] = step(x[t], u[t]) for t < T-1 (reference mpc/util.py:102-126). */
+int mpcb200_mlp_rollout_f32(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M,
+                            const float* x_init, const float* u, float* x, void* stream);
+int mpcb200_mlp_rollout_f64(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M,
+                            const double* x_init, const double* u, double* x, void* stream);
+/* The exact linearisation for t < T-1: F[T-1,B,N,N+M] = [R S] and f[T-1,B,N] = x' - R x - S u at (x[t], u[t]) of
+ * x[T,B,N], u[T,B,M], with the Jacobian chain of NNDynamics.grad_input (the activation's slope taken from its
+ * output, relu's 0 at 0) and I added to R with passthrough.  Under n_prev the rows of the previous control are
+ * [0 0 I] and f 0.  Nothing is written or launched for T = 1. */
+int mpcb200_mlp_linearize_f32(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const float* x,
+                              const float* u, float* F, float* f, void* stream);
+int mpcb200_mlp_linearize_f64(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const double* x,
+                              const double* u, double* F, double* f, void* stream);
+/* One LQR step whose true dynamics are the network and whose true cost is QuadCost(C, c): mpcb200_lqr_step_* with
+ * do_rollout = 0 (dims->do_rollout is ignored, dims->dynamics_kind must be 0) writes the gains into the workspace,
+ * then one kernel runs the line search of the reference's lqr_forward (mpc/lqr_step.py:164-261) per problem:
+ * u = K (x - cur_x) + cur_u + alpha k, u_zero_I, then the box (with delta_u) clamped lower bound first, x stepped by
+ * the network, the true cost summed; alpha *= ls_decay while the cost exceeds that of (cur_x, cur_u), for at most
+ * max_ls_iter passes, and alpha /= ls_decay after a last pass that was still worse.  Outputs new_x, new_u, costs[B],
+ * alphas[B] and optional du_first (cur_u - new_u of the first pass), qp_iters, free_mask, status (the step's).
+ * workspace: mpcb200_mlp_step_workspace_bytes() bytes, 256-byte aligned. */
+size_t mpcb200_mlp_step_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size);
+int mpcb200_mlp_step_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp,
+                         const float* C, const float* c, const float* F, const float* f, const float* x_init,
+                         const float* cur_x, const float* cur_u, const float* u_lower, const float* u_upper,
+                         const uint8_t* u_zero_I, float* new_x, float* new_u, float* costs, float* alphas,
+                         float* du_first, int32_t* qp_iters, uint8_t* free_mask, int32_t* status, void* workspace,
+                         size_t workspace_bytes, void* stream);
+int mpcb200_mlp_step_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp,
+                         const double* C, const double* c, const double* F, const double* f, const double* x_init,
+                         const double* cur_x, const double* cur_u, const double* u_lower, const double* u_upper,
+                         const uint8_t* u_zero_I, double* new_x, double* new_u, double* costs, double* alphas,
+                         double* du_first, int32_t* qp_iters, uint8_t* free_mask, int32_t* status, void* workspace,
+                         size_t workspace_bytes, void* stream);
+/* mpcb200_ilqr_* with the network as the dynamics (dims->dynamics_kind 0, no F or f): the loop body is
+ *   mlp rollout -> mlp linearisation (F, f into the workspace) -> step (do_rollout = 0, gains into the workspace)
+ *   -> mlp line search -> track -> stop
+ * with the init, track and stop kernels, outputs, capture contract, launch counting and MPCB200_ERR_NO_GRAPH_COND of
+ * mpcb200_ilqr_*.  Under a slew-rate penalty the caller passes the augmented problem and mlp->n_prev = m.
+ * workspace: mpcb200_ilqr_mlp_workspace_bytes() bytes, 256-byte aligned. */
+size_t mpcb200_ilqr_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size);
+int mpcb200_ilqr_mlp_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                         const mpcb200_mlp* mlp, const float* C, const float* c, const float* x_init,
+                         const float* u_init, const float* u_lower, const float* u_upper, const uint8_t* u_zero_I,
+                         float* best_x, float* best_u, float* best_costs, float* best_full_du_norm, int32_t* info,
+                         void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_ilqr_mlp_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                         const mpcb200_mlp* mlp, const double* C, const double* c, const double* x_init,
+                         const double* u_init, const double* u_lower, const double* u_upper,
+                         const uint8_t* u_zero_I, double* best_x, double* best_u, double* best_costs,
+                         double* best_full_du_norm, int32_t* info, void* workspace, size_t workspace_bytes,
+                         void* stream);
+
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);
 

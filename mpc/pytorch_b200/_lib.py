@@ -46,6 +46,16 @@ class Window(ctypes.Structure):
                                        "Fp_tstride", "fp_tstride")]
 
 
+# mpcb200_mlp.activation (include/mpcb200.h)
+ACT = {"sigmoid": 0, "relu": 1, "elu": 2}
+
+
+class Mlp(ctypes.Structure):
+    _fields_ = [("n_layers", ctypes.c_int32), ("width", ctypes.c_int32 * 5), ("activation", ctypes.c_int32),
+                ("passthrough", ctypes.c_int32), ("n_prev", ctypes.c_int32), ("reserved0", ctypes.c_int32),
+                ("params", ctypes.c_void_p), ("W_off", ctypes.c_int64 * 4), ("b_off", ctypes.c_int64 * 4)]
+
+
 class MpcB200Error(RuntimeError):
     pass
 
@@ -74,6 +84,9 @@ EXPORTED_SYMBOLS = (
     "mpcb200_episode_backward_plant_workspace_bytes", "mpcb200_episode_window_f32", "mpcb200_episode_window_f64",
     "mpcb200_episode_window_workspace_bytes", "mpcb200_episode_backward_window_f32",
     "mpcb200_episode_backward_window_f64", "mpcb200_episode_backward_window_workspace_bytes",
+    "mpcb200_mlp_fits", "mpcb200_mlp_rollout_f32", "mpcb200_mlp_rollout_f64", "mpcb200_mlp_linearize_f32",
+    "mpcb200_mlp_linearize_f64", "mpcb200_mlp_step_f32", "mpcb200_mlp_step_f64", "mpcb200_mlp_step_workspace_bytes",
+    "mpcb200_ilqr_mlp_f32", "mpcb200_ilqr_mlp_f64", "mpcb200_ilqr_mlp_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -192,6 +205,30 @@ def lib():
                                                                   ctypes.POINTER(Window), ctypes.POINTER(Plant),
                                                                   ctypes.c_int32]
     L.mpcb200_episode_backward_window_workspace_bytes.restype = ctypes.c_size_t
+    mlp = ctypes.POINTER(Mlp)
+    L.mpcb200_mlp_fits.argtypes = [mlp, ctypes.c_int32]
+    L.mpcb200_mlp_fits.restype = ctypes.c_int
+    for name in ("mpcb200_mlp_rollout_f32", "mpcb200_mlp_rollout_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [mlp] + [ctypes.c_int32] * 4 + [vp] * 4
+        fn.restype = ctypes.c_int
+    for name in ("mpcb200_mlp_linearize_f32", "mpcb200_mlp_linearize_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [mlp] + [ctypes.c_int32] * 4 + [vp] * 5
+        fn.restype = ctypes.c_int
+    for name in ("mpcb200_mlp_step_f32", "mpcb200_mlp_step_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), mlp] + [vp] * 19 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_mlp_step_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.c_int32]
+    L.mpcb200_mlp_step_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_ilqr_mlp_f32", "mpcb200_ilqr_mlp_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(IlqrOpts), mlp] + [vp] * 13 + \
+            [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_ilqr_mlp_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(IlqrOpts), ctypes.c_int32]
+    L.mpcb200_ilqr_mlp_workspace_bytes.restype = ctypes.c_size_t
     L.mpcb200_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_supported.restype = ctypes.c_int
     L.mpcb200_supported_list.argtypes = [ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]

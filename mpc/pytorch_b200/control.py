@@ -190,7 +190,11 @@ def _requires_grad(x_init, cost, dx, plant=None, w=None):
 def _takes_device_path(ctrl, x_init, cost, dx, w0, plant=None):
     """Whether the episode runs as one graph: exactly when each of its solves would take the device loop (T >= 3 is
     checked before) and the plant, if any, steps at the staged shape (_plant_on_device).  Decided on tensor metadata
-    alone, which a time-varying episode's full-length inputs share with its windows, so the same rule serves both."""
+    alone, which a time-varying episode's full-length inputs share with its windows, so the same rule serves both.
+    A learned model (NNDynamics) as model or plant keeps the host path, whose solves take MPC.forward's device loop."""
+    from .mlp import _net
+    if _net(dx)[0] is not None or _net(plant)[0] is not None:     # the episode's graph cannot step a network
+        return False
     return (solver._use_device_loop(ctrl, x_init, cost, dx, w0) or
             solver._use_slew_device_loop(ctrl, x_init, cost, dx, w0)) and \
         (plant is None or _plant_on_device(ctrl, x_init, dx, plant))

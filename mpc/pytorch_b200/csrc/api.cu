@@ -10,6 +10,7 @@
 #include "ilqr.cuh"
 #include "instance.cuh"
 #include "lqr_large.cuh"
+#include "mlp.cuh"
 #include "pnqp.cuh"
 
 namespace mpcb200 {
@@ -729,6 +730,214 @@ static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t bs = ilqr_stream(1);
     return bs == nullptr ? MPCB200_ERR_LAUNCH : ilqr_record<R>(os, bs, q, knob);
+  });
+}
+
+// ---------------------------------------------------------------------------------------------
+// a learned model's network (mlp.cu): its rollout and linearisation, the split-mode step (the step kernels with
+// do_rollout = 0, then the network's line search), and the iLQR loop of MPC.forward around them
+// ---------------------------------------------------------------------------------------------
+static int mlp_check(const mpcb200_mlp* mlp, int B, int T, int N, int M, MlpShape& s) {
+  if (mlp == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (!mlp_shape(mlp, s)) return MPCB200_ERR_BAD_DIMS;
+  if (B <= 0 || T <= 0 || N < s.n_prev + s.ns || M < s.ms || N + M > s.p_max) return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+template <typename R>
+static int mlp_rollout_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x_init, const R* u, R* x,
+                            void* stream) {
+  MlpShape s;
+  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
+  if (x_init == nullptr || u == nullptr || x == nullptr) return MPCB200_ERR_NULL_POINTER;
+  return counted(mlp_launch_rollout<R>(mlp, B, T, N, M, x_init, u, x, (cudaStream_t)stream));
+}
+
+template <typename R>
+static int mlp_linearize_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x, const R* u, R* F, R* f,
+                              void* stream) {
+  MlpShape s;
+  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
+  if (x == nullptr || u == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (T == 1) return MPCB200_OK;
+  if (F == nullptr || f == nullptr) return MPCB200_ERR_NULL_POINTER;
+  return counted(mlp_launch_linearize<R>(mlp, B, T, N, M, x, u, F, f, (cudaStream_t)stream));
+}
+
+static size_t mlp_step_ws(const mpcb200_dims* d, size_t sz) {
+  const size_t TBM = (size_t)d->T * d->B * d->m;
+  return up256(TBM * d->n * sz) + up256(TBM * sz);
+}
+
+// the arguments of mpcb200_mlp_step_* after dims, params and the record, in the header's order
+template <typename R>
+struct MlpStepCall {
+  const R *C, *c, *F, *f, *x_init, *cur_x, *cur_u, *u_lower, *u_upper;
+  const uint8_t* u_zero_I;
+  R *new_x, *new_u, *costs, *alphas, *du_first;
+  int32_t* qp_iters;
+  uint8_t* free_mask;
+  int32_t* status;
+};
+
+// The line search's arguments; Ks, ks: the gains the step wrote.
+template <typename R>
+static MlpLsArgs<R> mlp_ls_args(const mpcb200_dims* d, const mpcb200_params* p, const MlpStepCall<R>& q, const R* Ks,
+                                const R* ks) {
+  MlpLsArgs<R> a;
+  std::memset(&a, 0, sizeof(a));
+  a.B = d->B; a.T = d->T; a.N = d->n; a.M = d->m;
+  a.bounds_kind = d->bounds_kind; a.has_mask = d->has_zero_mask ? 1 : 0; a.has_delta = d->has_delta_u ? 1 : 0;
+  a.max_ls = d->max_ls_iter;
+  const TimeStrides ts = time_strides(d);
+  a.C_ts = ts.C; a.c_ts = ts.c;
+  a.u_lo = (R)p->u_lo; a.u_hi = (R)p->u_hi; a.delta_u = (R)p->delta_u; a.decay = (R)p->ls_decay;
+  a.C = q.C; a.c = q.c; a.x_init = q.x_init; a.cur_x = q.cur_x; a.cur_u = q.cur_u; a.Ks = Ks; a.ks = ks;
+  a.u_lower = q.u_lower; a.u_upper = q.u_upper; a.zero_mask = q.u_zero_I;
+  a.new_x = q.new_x; a.new_u = q.new_u; a.costs = q.costs; a.alphas = q.alphas; a.du_first = q.du_first;
+  return a;
+}
+
+// the checks of a split-mode step that need no device, before anything is launched
+template <typename R>
+static int mlp_step_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp,
+                          const MlpStepCall<R>& q) {
+  int rc = check_dims(d);
+  if (rc) return rc;
+  MlpShape s;
+  if ((rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s))) return rc;
+  if (p == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr || q.cur_x == nullptr ||
+      q.cur_u == nullptr || q.new_x == nullptr || q.new_u == nullptr || q.costs == nullptr || q.alphas == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (d->T > 1 && q.F == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (d->has_f && q.f == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if ((rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I))) return rc;
+  if (d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
+  return MPCB200_OK;
+}
+
+template <typename R>
+static int mlp_step_impl(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp,
+                         const MlpStepCall<R>& q, void* workspace, size_t workspace_bytes, void* stream) {
+  const int knob = kernel_knob();
+  int rc = mlp_step_check<R>(d, p, mlp, q);
+  if (rc) return rc;
+  if (workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (workspace_bytes < mlp_step_ws(d, sizeof(R)) || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  mpcb200_dims ds = *d;
+  ds.do_rollout = 0;
+  StepCall<R> sc = {};
+  sc.C = q.C; sc.c = q.c; sc.F = q.F; sc.f = q.f; sc.x_init = q.x_init; sc.cur_x = q.cur_x; sc.cur_u = q.cur_u;
+  sc.u_lower = q.u_lower; sc.u_upper = q.u_upper; sc.u_zero_I = q.u_zero_I;
+  sc.qp_iters = q.qp_iters; sc.free_mask = q.free_mask; sc.status = q.status;
+  sc.Ks = (R*)workspace;
+  sc.ks = (R*)((char*)workspace + up256((size_t)d->T * d->B * d->m * d->n * sizeof(R)));
+  if ((rc = step_impl<R>(&ds, p, sc, knob, stream))) return rc;
+  return counted(mlp_launch_linesearch<R>(mlp, mlp_ls_args<R>(d, p, q, sc.Ks, sc.ks), (cudaStream_t)stream));
+}
+
+// the iLQR loop's workspace: ilqr_layout's, plus the linearisation F, f and, where the step would not ask for them,
+// the gains (the split-mode step always writes them)
+static IlqrLayout ilqr_mlp_layout(const mpcb200_dims* d, size_t sz, int knob) {
+  IlqrLayout l = ilqr_layout(d, sz, knob);
+  const size_t TB = (size_t)d->T * d->B, TB1 = (size_t)(d->T - 1) * d->B;
+  const size_t n = d->n, m = d->m;
+  size_t o = l.total;
+  l.F = o; o += up256(TB1 * n * (n + m) * sz);
+  l.f = o; o += up256(TB1 * n * sz);
+  if (!l.gains) {
+    l.Ks = o; o += up256(TB * m * n * sz);
+    l.ks = o; o += up256(TB * m * sz);
+    l.gains = true;
+  }
+  l.total = o;
+  return l;
+}
+
+template <typename R>
+static int ilqr_mlp_check(const IlqrCall<R>& q, const mpcb200_mlp* mlp, int knob) {
+  const mpcb200_dims* d = q.d;
+  int rc = check_dims(d);
+  if (rc) return rc;
+  MlpShape s;
+  if ((rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s))) return rc;
+  if (q.p == nullptr || q.o == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr ||
+      q.best_x == nullptr || q.best_u == nullptr || q.best_costs == nullptr || q.best_fdn == nullptr ||
+      q.info == nullptr || q.workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (q.o->lqr_iter < 1 || q.o->m_ref < 1 || q.o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
+  if (d->T < 2 || d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  if ((rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I))) return rc;
+  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
+  const IlqrLayout l = ilqr_mlp_layout(d, sizeof(R), knob);
+  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+// ilqr_record with the network: rollout -> linearisation -> step (no rollout) -> line search -> track -> stop
+template <typename R>
+static int ilqr_mlp_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, const mpcb200_mlp* mlp, int knob) {
+  const mpcb200_dims* d = q.d;
+  const mpcb200_ilqr_opts* o = q.o;
+  const IlqrLayout l = ilqr_mlp_layout(d, sizeof(R), knob);
+  char* ws = (char*)q.workspace;
+  R* u = (R*)(ws + l.u);
+  R* x = (R*)(ws + l.x);
+  R* F = (R*)(ws + l.F);
+  R* f = (R*)(ws + l.f);
+  R* fdn = (R*)(ws + l.fdn);
+  uint8_t* flags = (uint8_t*)(ws + l.flags);
+  IlqrState* st = (IlqrState*)(ws + l.state);
+  const int B = d->B, T = d->T, N = d->n, M = d->m;
+  cudaGraphConditionalHandle handle;
+  int rc = while_handle(os, &handle);
+  if (rc) return rc;
+  if (counted(ilqr_launch_init<R>((size_t)T * B * M, q.u_init, u, st, q.info, handle, os)) != 0)
+    return MPCB200_ERR_LAUNCH;
+  rc = open_while(os, bs, handle);
+  if (rc) return rc;
+  mpcb200_dims ds = *d;                 // the step reads the workspace F, f
+  ds.F_T = T - 1; ds.has_f = 1; ds.F_tstride = 0; ds.f_tstride = 0;
+  MlpStepCall<R> mc = {};
+  mc.C = q.C; mc.c = q.c; mc.F = F; mc.f = f; mc.x_init = q.x_init; mc.cur_x = x; mc.cur_u = u;
+  mc.u_lower = q.u_lower; mc.u_upper = q.u_upper; mc.u_zero_I = q.u_zero_I;
+  mc.new_x = (R*)(ws + l.new_x); mc.new_u = (R*)(ws + l.new_u); mc.costs = (R*)(ws + l.costs);
+  mc.alphas = (R*)(ws + l.alphas); mc.du_first = (R*)(ws + l.du_first); mc.status = (int32_t*)(ws + l.status);
+  rc = mlp_rollout_impl<R>(mlp, B, T, N, M, q.x_init, u, x, bs);
+  if (rc == 0) rc = mlp_linearize_impl<R>(mlp, B, T, N, M, x, u, F, f, bs);
+  if (rc == 0) {
+    ds.do_rollout = 0;
+    StepCall<R> sc = {};
+    sc.C = q.C; sc.c = q.c; sc.F = F; sc.f = f; sc.x_init = q.x_init; sc.cur_x = x; sc.cur_u = u;
+    sc.u_lower = q.u_lower; sc.u_upper = q.u_upper; sc.u_zero_I = q.u_zero_I; sc.status = mc.status;
+    sc.Ks = (R*)(ws + l.Ks); sc.ks = (R*)(ws + l.ks);
+    rc = step_impl<R>(&ds, q.p, sc, knob, bs);
+    if (rc == 0)
+      rc = counted(mlp_launch_linesearch<R>(mlp, mlp_ls_args<R>(&ds, q.p, mc, sc.Ks, sc.ks), bs));
+  }
+  if (rc == 0)
+    rc = counted(ilqr_launch_track<R>(B, T, N, M, o->m_ref, (R)o->best_cost_eps, mc.new_x, mc.new_u, mc.costs,
+                                      mc.du_first, mc.status, q.best_costs, q.best_x, q.best_u, u, fdn, flags, st, bs));
+  if (rc == 0)
+    rc = counted(ilqr_launch_stop<R>(B, o->lqr_iter, o->not_improved_lim, o->eps, mc.costs, fdn, flags, q.best_costs,
+                                     q.best_fdn, st, q.info, handle, bs));
+  cudaGraph_t body = nullptr;
+  if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+  return rc;
+}
+
+template <typename R>
+static int ilqr_mlp_impl(const IlqrCall<R>& q, const mpcb200_mlp* mlp, void* stream) {
+  const int knob = kernel_knob();
+  int rc = ilqr_mlp_check<R>(q, mlp, knob);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t bs = ilqr_stream(1);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH : ilqr_mlp_record<R>(os, bs, q, mlp, knob);
   });
 }
 
@@ -1643,6 +1852,51 @@ size_t mpcb200_episode_backward_window_workspace_bytes(const mpcb200_dims* dims,
 MPCB200_EPISODE_BACKWARD_WINDOW(f32, float)
 MPCB200_EPISODE_BACKWARD_WINDOW(f64, double)
 #undef MPCB200_EPISODE_BACKWARD_WINDOW
+
+int mpcb200_mlp_fits(const mpcb200_mlp* mlp, int32_t elem_size) {
+  MlpShape s;
+  if ((elem_size != 4 && elem_size != 8) || !mlp_shape(mlp, s)) return 0;
+  return mlp_smem_bytes(s, elem_size, 1) <= (size_t)kOptinAssumed ? 1 : 0;
+}
+size_t mpcb200_mlp_step_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size) {
+  if (check_dims(dims) != MPCB200_OK || (elem_size != 4 && elem_size != 8)) return 0;
+  return mlp_step_ws(dims, (size_t)elem_size);
+}
+size_t mpcb200_ilqr_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
+  if (check_dims(dims) != MPCB200_OK || opts == nullptr || dims->T < 2 || (elem_size != 4 && elem_size != 8))
+    return 0;
+  return ilqr_mlp_layout(dims, (size_t)elem_size, kernel_knob()).total;
+}
+#define MPCB200_MLP_ENTRIES(sfx, R)                                                                                    \
+  int mpcb200_mlp_rollout_##sfx(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const R* x_init,  \
+                                const R* u, R* x, void* stream) {                                                      \
+    return mlp_rollout_impl<R>(mlp, B, T, N, M, x_init, u, x, stream);                                                \
+  }                                                                                                                    \
+  int mpcb200_mlp_linearize_##sfx(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const R* x,     \
+                                  const R* u, R* F, R* f, void* stream) {                                              \
+    return mlp_linearize_impl<R>(mlp, B, T, N, M, x, u, F, f, stream);                                                \
+  }                                                                                                                    \
+  int mpcb200_mlp_step_##sfx(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp,           \
+                             const R* C, const R* c, const R* F, const R* f, const R* x_init, const R* cur_x,          \
+                             const R* cur_u, const R* u_lower, const R* u_upper, const uint8_t* u_zero_I, R* new_x,    \
+                             R* new_u, R* costs, R* alphas, R* du_first, int32_t* qp_iters, uint8_t* free_mask,        \
+                             int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {                 \
+    return mlp_step_impl<R>(dims, params, mlp,                                                                         \
+                            {C, c, F, f, x_init, cur_x, cur_u, u_lower, u_upper, u_zero_I, new_x, new_u, costs,        \
+                             alphas, du_first, qp_iters, free_mask, status},                                           \
+                            workspace, workspace_bytes, stream);                                                       \
+  }                                                                                                                    \
+  int mpcb200_ilqr_mlp_##sfx(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,   \
+                             const mpcb200_mlp* mlp, const R* C, const R* c, const R* x_init, const R* u_init,         \
+                             const R* u_lower, const R* u_upper, const uint8_t* u_zero_I, R* best_x, R* best_u,        \
+                             R* best_costs, R* best_full_du_norm, int32_t* info, void* workspace,                      \
+                             size_t workspace_bytes, void* stream) {                                                   \
+    return ilqr_mlp_impl<R>({dims, params, opts, C, c, nullptr, nullptr, x_init, u_init, u_lower, u_upper, u_zero_I,   \
+                             best_x, best_u, best_costs, best_full_du_norm, info, workspace, workspace_bytes},         \
+                            mlp, stream);                                                                              \
+  }
+MPCB200_MLP_ENTRIES(f32, float)
+MPCB200_MLP_ENTRIES(f64, double)
 
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl) { return find(n_state, n_ctrl) != nullptr; }
 

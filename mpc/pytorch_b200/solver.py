@@ -71,6 +71,9 @@ def get_traj(T, u, x_init, dynamics):
             kind, kparams = known_kind(dynamics, x_init.shape[1], u.shape[2], x_init)
             if kind:                                          # one kernel instead of T-1 Module calls
                 return dyn_rollout_raw(kind, kparams, T, _detach(x_init), _detach(u))
+            from . import mlp
+            if mlp.on_device(dynamics, x_init.shape[1], u.shape[2], x_init):
+                return mlp.rollout_raw(dynamics, T, _detach(x_init), _detach(u))
         xs = [_detach(x_init)]
         if isinstance(dynamics, LinDx):
             F, f = _detach(dynamics.F), _detach(dynamics.f)
@@ -278,7 +281,11 @@ class MPC(Module):
         from . import step as _step
         T, m = self.T, self.n_ctrl
         n, x_init, C, c, F, f, dyn = self._device_problem(x_init, cost, dx)
-        res = _step.ilqr_raw(n, m, T, x_init, C, c, F, f, u, dyn=dyn, **self._device_options())
+        if dyn is not None and dyn[0] == "mlp":         # a learned model: mpcb200_ilqr_mlp_*
+            from .mlp import ilqr_raw
+            res = ilqr_raw(dyn[1], n, m, T, x_init, C, c, u, **self._device_options())
+        else:
+            res = _step.ilqr_raw(n, m, T, x_init, C, c, F, f, u, dyn=dyn, **self._device_options())
         if res is None:
             _graph_cond_unavailable = True
             return None
@@ -289,7 +296,9 @@ class MPC(Module):
     def _device_problem(self, x_init, cost, dx, T=None):
         """The problem of the device loop, staged once per solve (or episode): (n, x_init, C, c, F, f, dyn).  With a
         slew-rate penalty, the augmented problem over [u_{t-1}; x] (n = n_state + n_ctrl).  dyn = (kind, params) of a
-        known system, with F = f = None; None for LinDx.  T: the length of C's time axis when it is not the solve's
+        known system, with F = f = None; ("mlp", Module) for a learned model in the kernels (mlp.on_device; the Module
+        a CtrlPassthroughDynamics under a slew-rate penalty), F = f = None; None for LinDx.  T: the length of C's time
+        axis when it is not the solve's
         (a time-varying episode's, control.receding_horizon)."""
         n, m = self.n_state, self.n_ctrl
         C, c = cost.C, cost.c
@@ -303,8 +312,9 @@ class MPC(Module):
             dyn = None
         else:
             from .dynamics import known_kind
+            from .mlp import on_device
             F = f = None
-            dyn = known_kind(dx, n, m, x_init)
+            dyn = ("mlp", dx) if on_device(dx, n, m, x_init) else known_kind(dx, n, m, x_init)
         return n, x_init, C, c, F, f, dyn
 
     def _device_options(self):
@@ -499,12 +509,21 @@ class MPC(Module):
             return DYN_LINEAR, None
         return kind, kparams
 
+    def _mlp_on_device(self, dynamics, x):
+        """Whether a learned model's network runs in the kernels here (mlp.on_device), under ANALYTIC or AUTO_DIFF."""
+        from .mlp import on_device
+        return self.grad_method in (GradMethods.ANALYTIC, GradMethods.AUTO_DIFF) and \
+            on_device(dynamics, self.n_state, self.n_ctrl, x)
+
     def linearize_dynamics(self, x, u, dynamics, diff):
         """First-order expansion x' ~ F [x;u] + f of Module dynamics (reference :490-601),
         evaluated for all T-1 steps and the whole batch at once."""
         T, n, m = self.T, self.n_state, self.n_ctrl
         B = x.shape[1]
         kind, kparams = self._kernel_linearization(dynamics, x, diff)
+        if not kind and not diff and self._mlp_on_device(dynamics, x):    # a network's exact Jacobians, one kernel
+            from .mlp import linearize_raw
+            return linearize_raw(dynamics, T, x.detach(), u.detach())
         if kind:               # exact Jacobians of a known system by forward-mode duals, one kernel
             from .dynamics import dyn_linearize_raw, linearize_known
             if diff:           # differentiable in the system's parameters through the VJP kernel
@@ -564,8 +583,9 @@ def _use_device_loop(mpc, x_init, cost, dx, u):
     """Whether MPC.forward runs its iLQR iterations as one device-side graph (MPC._ilqr_device) rather than from
     Python (MPC._ilqr_host).  Decided on what the call shows without reading the device: the results are the same
     either way, so there is no user option.  Taken for CUDA float32/float64 tensors of one dtype, a QuadCost, LinDx
-    dynamics or a known system linearised by ANALYTIC / AUTO_DIFF, no slew-rate penalty, verbose <= 0, lqr_iter >= 1,
-    T >= 2 and a shape the step kernels take (an exact or zero-padded instance, or the large-shape kernels for LinDx)."""
+    dynamics, or a known system or a learned model in the kernels (mlp.on_device) linearised by ANALYTIC / AUTO_DIFF,
+    no slew-rate penalty, verbose <= 0, lqr_iter >= 1, T >= 2 and a shape the step kernels take (an exact or
+    zero-padded instance, or the large-shape kernels for LinDx)."""
     return mpc.slew_rate_penalty is None and _device_loop_takes(mpc, x_init, cost, dx, u, slew=False)
 
 
@@ -611,6 +631,8 @@ def _device_loop_takes(mpc, x_init, cost, dx, u, slew):
             return False
         kind = dx.mpcb200_kind | (DYN_CTRL_PASSTHROUGH if slew else 0)
         known = True
+    elif mpc._mlp_on_device(dx, x_init):              # a learned model: the network's kernels around the step
+        known = False
     else:
         return False
     same += [b for b in (mpc.u_lower, mpc.u_upper) if isinstance(b, torch.Tensor)]

@@ -961,6 +961,11 @@ def reference_full_du_norm(du_first):
     return du_first.transpose(1, 2).reshape(B, -1).norm(2, 1)
 
 
+def _mlp_on_device(dx, n, m, x):
+    from .mlp import on_device
+    return isinstance(dx, Module) and on_device(dx, n, m, x)
+
+
 def _same_storage(a, b):
     if a is None or b is None:
         return _is_empty(a) and _is_empty(b)
@@ -1010,6 +1015,14 @@ class LQRStepFn(Function):
                                want_du_first=True, dyn=dyn)
             new_x, new_u = res["new_x"], res["new_u"]
             costs, alphas = res["costs"], res["alphas"]
+            fdn = reference_full_du_norm(res["du_first"])
+        elif quad_same and _mlp_on_device(o.true_dynamics, o.n_state, o.n_ctrl, C):
+            # a learned model: the step's gains, then the network's line search in one kernel (mpcb200_mlp_step_*)
+            from .mlp import step_raw
+            res = step_raw(o.true_dynamics, o.n_state, o.n_ctrl, o.T, x_init, C, c, F, f, o.current_x, o.current_u,
+                           u_lower=o.u_lower, u_upper=o.u_upper, u_zero_I=o.u_zero_I, delta_u=o.delta_u,
+                           linesearch_decay=o.linesearch_decay, max_linesearch_iter=o.max_linesearch_iter)
+            new_x, new_u, costs, alphas = res["new_x"], res["new_u"], res["costs"], res["alphas"]
             fdn = reference_full_du_norm(res["du_first"])
         else:
             assert o.true_cost is not None and o.true_dynamics is not None

@@ -286,8 +286,46 @@ static int run_episode_window() {
   return 0;
 }
 
+// the network entries: a passthrough network with zero weights steps x' = x, so the rollout repeats x_init and the
+// linearisation is F = [I 0], f = 0; a network too large for shared memory is refused by mpcb200_mlp_fits
+static int run_mlp() {
+  const int B = 5, T = 4, n = 3, m = 2, h = 8, p = n + m;
+  mpcb200_mlp net = {};
+  net.n_layers = 2; net.width[0] = p; net.width[1] = h; net.width[2] = n;
+  net.activation = MPCB200_ACT_SIGMOID; net.passthrough = 1;
+  net.W_off[0] = 0; net.b_off[0] = h * p; net.W_off[1] = h * p + h; net.b_off[1] = h * p + h + n * h;
+  Dev<float> prm(h * p + h + n * h + n), x0(B * n), u(T * B * m), x(T * B * n);
+  Dev<float> F((T - 1) * B * n * p), f((T - 1) * B * n);
+  prm.up(std::vector<float>(prm.n, 0.f));
+  std::vector<float> hx(B * n);
+  for (auto& v : hx) v = rnd();
+  x0.up(hx);
+  u.up(std::vector<float>(u.n, 0.5f));
+  net.params = prm.p;
+  if (!mpcb200_mlp_fits(&net, 4)) return printf("mlp: small network does not fit\n"), 1;
+  int rc = mpcb200_mlp_rollout_f32(&net, B, T, n, m, x0.p, u.p, x.p, nullptr);
+  if (rc == 0) rc = mpcb200_mlp_linearize_f32(&net, B, T, n, m, x.p, u.p, F.p, f.p, nullptr);
+  if (rc != 0 || cudaDeviceSynchronize() != cudaSuccess) return printf("mlp rollout / linearize rc=%d\n", rc), 1;
+  int bad = 0;
+  const auto gx = x.down(), gF = F.down(), gf = f.down();
+  for (int i = 0; i < T * B * n; ++i) bad += gx[i] != hx[i % (B * n)];
+  for (int i = 0; i < (T - 1) * B * n * p; ++i) {
+    const int c = i % p, r = (i / p) % n;
+    bad += gF[i] != (c == r ? 1.f : 0.f);
+  }
+  for (float v : gf) bad += v != 0.f;
+  mpcb200_mlp big = net;
+  big.n_layers = 3; big.width[1] = big.width[2] = 256; big.width[3] = n;
+  big.W_off[1] = 256 * p + 256; big.b_off[1] = big.W_off[1] + 256 * 256;
+  big.W_off[2] = big.b_off[1] + 256; big.b_off[2] = big.W_off[2] + 256 * n;
+  if (mpcb200_mlp_fits(&big, 4)) ++bad;
+  printf("mlp: rollout and linearisation of x' = x, %d bad; [256, 256] refused by mpcb200_mlp_fits\n", bad);
+  return bad != 0;
+}
+
 int main() {
   int fails = 0;
+  fails += run_mlp();
   fails += run_episode_backward_slew();
   fails += run_episode_plant();
   fails += run_episode_window();
