@@ -664,6 +664,22 @@ int mpcb200_mlp_linearize_f32(const mpcb200_mlp* mlp, int32_t B, int32_t T, int3
                               const float* u, float* F, float* f, void* stream);
 int mpcb200_mlp_linearize_f64(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const double* x,
                               const double* u, double* F, double* f, void* stream);
+/* The VJP of mpcb200_mlp_linearize_* in the parameters: dtheta[n_params] (the record's packed layout, n_params the
+ * largest end of a W_i or b_i; elements of no layer are 0) = d/dtheta of the sum over t < T-1 and b of
+ * <dF[t,b], F[t,b]> + <df[t,b], f[t,b]>, with x, u, dF[T-1,B,N,N+M] and df[T-1,B,N] at the staged shapes of
+ * mpcb200_mlp_linearize_*.  Only the network's block of dF and df enters (rows n_prev .. n_prev+n_s-1, columns of
+ * its state and control); the passthrough identity, the rows of the previous control and the padding are constants.
+ * The (t, b) items are summed in an order fixed by B, T and the record alone, with no atomics: dtheta is bitwise the
+ * same for every call, stream and graph replay on one card type.  Two kernels; T = 1 writes dtheta = 0.
+ * workspace: mpcb200_mlp_linearize_vjp_workspace_bytes() bytes, 256-byte aligned.  MPCB200_ERR_SMEM for a network
+ * whose VJP does not fit (that function's 0). */
+size_t mpcb200_mlp_linearize_vjp_workspace_bytes(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t elem_size);
+int mpcb200_mlp_linearize_vjp_f32(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const float* x,
+                                  const float* u, const float* dF, const float* df, float* dtheta, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+int mpcb200_mlp_linearize_vjp_f64(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M,
+                                  const double* x, const double* u, const double* dF, const double* df,
+                                  double* dtheta, void* workspace, size_t workspace_bytes, void* stream);
 /* One LQR step whose true dynamics are the network and whose true cost is QuadCost(C, c): mpcb200_lqr_step_* with
  * do_rollout = 0 (dims->do_rollout is ignored, dims->dynamics_kind must be 0) writes the gains into the workspace,
  * then one kernel runs the line search of the reference's lqr_forward (mpc/lqr_step.py:164-261) per problem:

@@ -87,6 +87,7 @@ EXPORTED_SYMBOLS = (
     "mpcb200_mlp_fits", "mpcb200_mlp_rollout_f32", "mpcb200_mlp_rollout_f64", "mpcb200_mlp_linearize_f32",
     "mpcb200_mlp_linearize_f64", "mpcb200_mlp_step_f32", "mpcb200_mlp_step_f64", "mpcb200_mlp_step_workspace_bytes",
     "mpcb200_ilqr_mlp_f32", "mpcb200_ilqr_mlp_f64", "mpcb200_ilqr_mlp_workspace_bytes",
+    "mpcb200_mlp_linearize_vjp_f32", "mpcb200_mlp_linearize_vjp_f64", "mpcb200_mlp_linearize_vjp_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -216,6 +217,12 @@ def lib():
         fn = getattr(L, name)
         fn.argtypes = [mlp] + [ctypes.c_int32] * 4 + [vp] * 5
         fn.restype = ctypes.c_int
+    for name in ("mpcb200_mlp_linearize_vjp_f32", "mpcb200_mlp_linearize_vjp_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [mlp] + [ctypes.c_int32] * 4 + [vp] * 6 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_mlp_linearize_vjp_workspace_bytes.argtypes = [mlp] + [ctypes.c_int32] * 3
+    L.mpcb200_mlp_linearize_vjp_workspace_bytes.restype = ctypes.c_size_t
     for name in ("mpcb200_mlp_step_f32", "mpcb200_mlp_step_f64"):
         fn = getattr(L, name)
         fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), mlp] + [vp] * 19 + [ctypes.c_size_t, vp]

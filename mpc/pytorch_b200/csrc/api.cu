@@ -764,6 +764,27 @@ static int mlp_linearize_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M
   return counted(mlp_launch_linearize<R>(mlp, B, T, N, M, x, u, F, f, (cudaStream_t)stream));
 }
 
+// the linearisation VJP's workspace ([G, n_params] slot rows), 0 where its per-warp slice does not fit
+static size_t mlp_vjp_ws(const MlpShape& s, int B, int T, size_t sz) {
+  if (mlp_smem_bytes(mlp_vjp_shape(s), (int)sz, 1) > (size_t)kOptinAssumed) return 0;
+  return up256((size_t)mlp_vjp_slots((long long)(T - 1) * B, s.n_params) * (size_t)s.n_params * sz);
+}
+
+template <typename R>
+static int mlp_linearize_vjp_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x, const R* u,
+                                  const R* dF, const R* df, R* dtheta, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  MlpShape s;
+  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
+  if (x == nullptr || u == nullptr || dF == nullptr || df == nullptr || dtheta == nullptr || workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  const size_t need = mlp_vjp_ws(s, B, T, sizeof(R));
+  if (need == 0) return MPCB200_ERR_SMEM;
+  if (workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
+  return counted(mlp_launch_linearize_vjp<R>(mlp, B, T, N, M, x, u, dF, df, dtheta, (R*)workspace,
+                                             (cudaStream_t)stream), 2);
+}
+
 static size_t mlp_step_ws(const mpcb200_dims* d, size_t sz) {
   const size_t TBM = (size_t)d->T * d->B * d->m;
   return up256(TBM * d->n * sz) + up256(TBM * sz);
@@ -1858,6 +1879,11 @@ int mpcb200_mlp_fits(const mpcb200_mlp* mlp, int32_t elem_size) {
   if ((elem_size != 4 && elem_size != 8) || !mlp_shape(mlp, s)) return 0;
   return mlp_smem_bytes(s, elem_size, 1) <= (size_t)kOptinAssumed ? 1 : 0;
 }
+size_t mpcb200_mlp_linearize_vjp_workspace_bytes(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t elem_size) {
+  MlpShape s;
+  if ((elem_size != 4 && elem_size != 8) || B <= 0 || T <= 0 || !mlp_shape(mlp, s)) return 0;
+  return mlp_vjp_ws(s, B, T, (size_t)elem_size);
+}
 size_t mpcb200_mlp_step_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size) {
   if (check_dims(dims) != MPCB200_OK || (elem_size != 4 && elem_size != 8)) return 0;
   return mlp_step_ws(dims, (size_t)elem_size);
@@ -1875,6 +1901,11 @@ size_t mpcb200_ilqr_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_
   int mpcb200_mlp_linearize_##sfx(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const R* x,     \
                                   const R* u, R* F, R* f, void* stream) {                                              \
     return mlp_linearize_impl<R>(mlp, B, T, N, M, x, u, F, f, stream);                                                \
+  }                                                                                                                    \
+  int mpcb200_mlp_linearize_vjp_##sfx(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const R* x, \
+                                      const R* u, const R* dF, const R* df, R* dtheta, void* workspace,                \
+                                      size_t workspace_bytes, void* stream) {                                          \
+    return mlp_linearize_vjp_impl<R>(mlp, B, T, N, M, x, u, dF, df, dtheta, workspace, workspace_bytes, stream);      \
   }                                                                                                                    \
   int mpcb200_mlp_step_##sfx(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp,           \
                              const R* C, const R* c, const R* F, const R* f, const R* x_init, const R* cur_x,          \

@@ -71,6 +71,14 @@ MPCB_DEV R act_slope(int act, R a) {
   return a > R(0) ? R(1) : a + R(1);
 }
 
+// d^2 act / d pre-activation^2 from the post-activation value a: the derivative of act_slope through a
+template <typename R>
+MPCB_DEV R act_curv(int act, R a) {
+  if (act == MPCB200_ACT_SIGMOID) return a * (R(1) - a) * (R(1) - R(2) * a);
+  if (act == MPCB200_ACT_RELU) return R(0);
+  return a > R(0) ? R(0) : a + R(1);
+}
+
 template <typename R>
 MPCB_DEV R warp_sum(R v) {
 #pragma unroll
@@ -377,6 +385,147 @@ mlp_linesearch_kernel(const __grid_constant__ MlpShape s, const R* __restrict__ 
   }
 }
 
+// The VJP of mlp_linearize_kernel's (F, f) in the parameters, per item reverse over forward with matrix tangents
+// (mlp.cuh).  Warp w serves the slots w, w + warps, ...; slot g runs the items g, g + G, ... in increasing order and
+// adds each item's gradient into its own workspace row ws[g], every element of it always by the same lane.  s is the
+// shape of mlp_vjp_shape (its per_warp is this kernel's slice).
+template <typename R>
+__global__ void __launch_bounds__(256, 1)
+mlp_linearize_vjp_kernel(const __grid_constant__ MlpShape s, const R* __restrict__ params, int B, int T, int N, int M,
+                         const R* __restrict__ x, const R* __restrict__ u, const R* __restrict__ dF,
+                         const R* __restrict__ df, int G, R* __restrict__ ws) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+  const MlpSmem<R> sm = carve<R>(s, mlp_smem, warp);
+  stage_params(s, params, sm.prm, sm.bar);
+  const int L = s.L, ns = s.ns, p = s.w[0], P = N + M;
+  int hidden = 0;
+  for (int i = 1; i < L; ++i) hidden += s.w[i];
+  // z | hidden outputs h_1 .. h_{L-1} | tangents T_1 .. T_{L-1} [w_i, p] | adjoints X, Y [maxw, p] | hx, hy [maxw]
+  R* z = sm.mine;
+  R* hid = z + p;
+  R* tan = hid + hidden;
+  R* X = tan + (size_t)hidden * p;
+  R* Y = X + (size_t)s.maxw * p;
+  R* hx = Y + (size_t)s.maxw * p;
+  R* hy = hx + s.maxw;
+  const long long items = (long long)(T - 1) * B;
+  for (int g = blockIdx.x * wpb + warp; g < G; g += gridDim.x * wpb) {
+    R* row = ws + (size_t)g * s.n_params;
+    for (long long e = lane; e < s.n_params; e += 32) row[e] = R(0);
+    __syncwarp();
+    for (long long it = g; it < items; it += G) {
+      const int t = (int)(it / B), b = (int)(it - (long long)t * B);
+      const size_t tb = (size_t)t * B + b;
+      mlp_input(s, x + tb * N, u + tb * M, z, lane);
+      // forward: h_{i+1} = act(W_i h_i + b_i), T_{i+1} = diag(act'(h_{i+1})) W_i T_i, T_0 = I (Ti == nullptr)
+      const R* hin = z;
+      const R* Tin = nullptr;
+      R* ho = hid;
+      R* To = tan;
+      for (int i = 0; i + 1 < L; ++i) {
+        const R* W = sm.prm + s.W_off[i];
+        const int wi = s.w[i], wo = s.w[i + 1];
+        mlp_layer(W, sm.prm + s.b_off[i], hin, ho, wi, wo, s.act, lane);
+        for (int e = lane; e < wo * p; e += 32) {
+          const int r = e / p, c = e - r * p;
+          R acc = R(0);
+          if (Tin == nullptr) acc = W[(size_t)r * wi + c];
+          else
+            for (int k = 0; k < wi; ++k) acc = fma(W[(size_t)r * wi + k], Tin[(size_t)k * p + c], acc);
+          To[e] = act_slope(s.act, ho[r]) * acc;
+        }
+        __syncwarp();
+        hin = ho; Tin = To;
+        ho += wo; To += (size_t)wo * p;
+      }
+      // seeds: X = G^ = dJ - df z^T and hx = df, the network's rows and columns of dF and df
+      const R* dFt = dF + tb * N * P;
+      const R* dft = df + tb * N + s.n_prev;
+      for (int e = lane; e < ns * p; e += 32) {
+        const int r = e / p, c = e - r * p;
+        const R* dr = dFt + (size_t)(s.n_prev + r) * P;
+        X[e] = (c < ns ? dr[s.n_prev + c] : dr[N + c - ns]) - dft[r] * z[c];
+      }
+      for (int r = lane; r < ns; r += 32) hx[r] = dft[r];
+      __syncwarp();
+      // reverse: layer i with X = the adjoint of its output tangent, hx = that of its output
+      const R* hout = nullptr;
+      for (int i = L - 1; i >= 0; --i) {
+        const R* W = sm.prm + s.W_off[i];
+        const int wi = s.w[i], wo = s.w[i + 1];
+        if (i + 1 < L) {
+          // a hidden layer: s^bar = rowsum(X .* A_i) with A_i = W_i T_i (Y holds the products),
+          // a^bar = h^bar .* act' + s^bar .* act'' into hx, A^bar = diag(act') X into X
+          if (s.act != MPCB200_ACT_RELU) {
+            for (int e = lane; e < wo * p; e += 32) {
+              const int r = e / p, c = e - r * p;
+              R acc = R(0);
+              if (Tin == nullptr) acc = W[(size_t)r * wi + c];
+              else
+                for (int k = 0; k < wi; ++k) acc = fma(W[(size_t)r * wi + k], Tin[(size_t)k * p + c], acc);
+              Y[e] = X[e] * acc;
+            }
+            __syncwarp();
+          }
+          for (int r = lane; r < wo; r += 32) {
+            R sb = R(0);
+            if (s.act != MPCB200_ACT_RELU)
+              for (int c = 0; c < p; ++c) sb += Y[(size_t)r * p + c];
+            hx[r] = hx[r] * act_slope(s.act, hout[r]) + sb * act_curv(s.act, hout[r]);
+          }
+          for (int e = lane; e < wo * p; e += 32) X[e] *= act_slope(s.act, hout[e / p]);
+          __syncwarp();
+        }
+        // dW_i += X T_i^T + hx h_i^T, db_i += hx
+        R* dW = row + s.W_off[i];
+        for (int e = lane; e < wo * wi; e += 32) {
+          const int r = e / wi, k = e - r * wi;
+          R v = R(0);
+          if (Tin == nullptr) v = X[(size_t)r * p + k];
+          else
+            for (int c = 0; c < p; ++c) v = fma(X[(size_t)r * p + c], Tin[(size_t)k * p + c], v);
+          dW[e] += fma(hx[r], hin[k], v);
+        }
+        R* db = row + s.b_off[i];
+        for (int r = lane; r < wo; r += 32) db[r] += hx[r];
+        if (i > 0) {
+          // the adjoints of layer i's input: Y = W_i^T X, hy = W_i^T hx
+          for (int e = lane; e < wi * p; e += 32) {
+            const int k = e / p, c = e - k * p;
+            R acc = R(0);
+            for (int r = 0; r < wo; ++r) acc = fma(W[(size_t)r * wi + k], X[(size_t)r * p + c], acc);
+            Y[e] = acc;
+          }
+          for (int k = lane; k < wi; k += 32) {
+            R acc = R(0);
+            for (int r = 0; r < wo; ++r) acc = fma(W[(size_t)r * wi + k], hx[r], acc);
+            hy[k] = acc;
+          }
+          __syncwarp();
+          R* t = X; X = Y; Y = t;
+          t = hx; hx = hy; hy = t;
+          hout = hin;
+          hin = i == 1 ? z : hin - s.w[i - 1];
+          Tin = i == 1 ? nullptr : Tin - (size_t)s.w[i - 1] * p;
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// dtheta[e] = sum of ws[g][e] over the slots g = 0 .. G-1, in that order
+template <typename R>
+__global__ void __launch_bounds__(256)
+mlp_vjp_reduce_kernel(const R* __restrict__ ws, int G, long long n_params, R* __restrict__ dtheta) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n_params;
+       e += (long long)gridDim.x * blockDim.x) {
+    R acc = ws[e];
+    for (int g = 1; g < G; ++g) acc += ws[(size_t)g * n_params + e];
+    dtheta[e] = acc;
+  }
+}
+
 // warps per CTA: up to 8, as many as the opt-in shared memory holds, no more than there are items
 int mlp_warps(const MlpShape& s, int elem_size, long long items, int smem_optin) {
   int w = 8;
@@ -437,11 +586,49 @@ int mlp_launch_linesearch(const mpcb200_mlp* rec, const MlpLsArgs<R>& a, cudaStr
   return launched();
 }
 
+MlpShape mlp_vjp_shape(const MlpShape& s) {
+  MlpShape v = s;
+  const int p = s.w[0];
+  int hidden = 0;
+  for (int i = 1; i < s.L; ++i) hidden += s.w[i];
+  v.per_warp = round_up(p + hidden + hidden * p + 2 * s.maxw * p + 2 * s.maxw, 4);
+  return v;
+}
+
+int mlp_vjp_slots(long long items, long long n_params) {
+  long long g = kMlpVjpSlotElems / n_params;
+  if (g < 1) g = 1;
+  if (g > kMlpVjpMaxSlots) g = kMlpVjpMaxSlots;
+  if (g > items) g = items;
+  return g < 1 ? 1 : (int)g;
+}
+
+template <typename R>
+int mlp_launch_linearize_vjp(const mpcb200_mlp* rec, int B, int T, int N, int M, const R* x, const R* u, const R* dF,
+                             const R* df, R* dtheta, R* ws, cudaStream_t stream) {
+  MlpShape s;
+  if (!mlp_shape(rec, s)) return MPCB200_ERR_BAD_DIMS;
+  const MlpShape v = mlp_vjp_shape(s);
+  const int G = mlp_vjp_slots((long long)(T - 1) * B, s.n_params);
+  int warps, grid;
+  size_t smem;
+  if (const int rc = mlp_prepare<mlp_linearize_vjp_kernel<R>>(v, sizeof(R), G, warps, grid, smem)) return rc;
+  if (grid > kMlpVjpMaxCtas) grid = kMlpVjpMaxCtas;
+  mlp_linearize_vjp_kernel<R><<<grid, 32 * warps, smem, stream>>>(v, (const R*)rec->params, B, T, N, M, x, u, dF, df,
+                                                                   G, ws);
+  if (const int rc = launched()) return rc;
+  const long long blocks = (s.n_params + 255) / 256;
+  mlp_vjp_reduce_kernel<R><<<(int)(blocks < 1024 ? blocks : 1024), 256, 0, stream>>>(ws, G, s.n_params, dtheta);
+  return launched();
+}
+
 #define MPCB200_MLP_INSTANTIATE(R)                                                                                    \
   template int mlp_launch_rollout<R>(const mpcb200_mlp*, int, int, int, int, const R*, const R*, R*, cudaStream_t);    \
   template int mlp_launch_linearize<R>(const mpcb200_mlp*, int, int, int, int, const R*, const R*, R*, R*,             \
                                        cudaStream_t);                                                                  \
-  template int mlp_launch_linesearch<R>(const mpcb200_mlp*, const MlpLsArgs<R>&, cudaStream_t);
+  template int mlp_launch_linesearch<R>(const mpcb200_mlp*, const MlpLsArgs<R>&, cudaStream_t);                        \
+  template int mlp_launch_linearize_vjp<R>(const mpcb200_mlp*, int, int, int, int, const R*, const R*, const R*,       \
+                                           const R*, R*, R*, cudaStream_t);
 MPCB200_MLP_INSTANTIATE(float)
 MPCB200_MLP_INSTANTIATE(double)
 

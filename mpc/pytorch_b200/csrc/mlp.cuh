@@ -54,4 +54,22 @@ int mlp_launch_linearize(const mpcb200_mlp* rec, int B, int T, int N, int M, con
 template <typename R>
 int mlp_launch_linesearch(const mpcb200_mlp* rec, const MlpLsArgs<R>& a, cudaStream_t stream);
 
+// The linearisation's VJP in the parameters (mpcb200_mlp_linearize_vjp_*): one warp per item (t, b) computes
+// d/dtheta [<G^, J> + <df, y>], G^ = dJ - df z^T, by reverse over forward with matrix tangents T_i = dh_i/dz.  Its
+// per-warp slice holds z, the hidden outputs, T_1 .. T_{L-1} [w_i, w_0], two adjoint buffers [maxw, w_0] and two
+// [maxw] (mlp_vjp_shape).  The items are dealt to G slots (mlp_vjp_slots, a function of the item and parameter
+// counts alone): slot g sums items g, g + G, ... in increasing order into row g of a [G, n_params] workspace, and a
+// second kernel adds the G rows in slot order into dtheta, so dtheta is bitwise the same for any grid.
+constexpr long long kMlpVjpSlotElems = 1ll << 23;   // G * n_params stays at or below this (or G = 1)
+constexpr int kMlpVjpMaxSlots = 2048;
+constexpr int kMlpVjpMaxCtas = 128;                 // CTAs of the VJP kernel; a warp serves every (warps)-th slot
+// s with per_warp set to the VJP kernel's slice
+MlpShape mlp_vjp_shape(const MlpShape& s);
+// G = max(1, min(items, kMlpVjpMaxSlots, max(1, kMlpVjpSlotElems / n_params)))
+int mlp_vjp_slots(long long items, long long n_params);
+// ws: G * n_params elements
+template <typename R>
+int mlp_launch_linearize_vjp(const mpcb200_mlp* rec, int B, int T, int N, int M, const R* x, const R* u, const R* dF,
+                             const R* df, R* dtheta, R* ws, cudaStream_t stream);
+
 }  // namespace mpcb200

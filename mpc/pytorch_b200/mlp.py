@@ -10,6 +10,8 @@ packed into one buffer once per solve (``dynamics.params_scope``), so an in-plac
 Only the linearisation depends on ``MPC.grad_method`` (ANALYTIC / AUTO_DIFF take ``linearize_raw``; FINITE_DIFF keeps
 its central differences in torch, and with it the host loop).  The rollout (``get_traj``) and the split-mode step's line
 search compute the same function under every grad_method, so they take the kernels whenever ``on_device`` holds.
+MPC's differentiable tail (``linearize_dynamics(diff=True)``) takes ``linearize_diff``: ``MlpLinearize``, whose backward
+is the VJP of the linearisation in the weights (``mpcb200_mlp_linearize_vjp_*``, DESIGN.md section 3.11).
 """
 import ctypes
 
@@ -114,13 +116,15 @@ def rollout_raw(dx, T, x_init, u):
     return x
 
 
-def linearize_raw(dx, T, x, u):
-    """MPC.linearize_dynamics(x, u, dx, diff=False) in one kernel: F [T-1, B, n, n+m], f [T-1, B, n]."""
+def linearize_raw(dx, T, x, u, rec=None, buf=None):
+    """MPC.linearize_dynamics(x, u, dx, diff=False) in one kernel: F [T-1, B, n, n+m], f [T-1, B, n].  rec, buf: the
+    record and packed buffer to run (default: record(dx, x))."""
     from .step import _dense
     _, B, n = x.shape
     m = u.shape[2]
     dtype, dev = x.dtype, x.device
-    rec, buf = record(dx, x)
+    if rec is None:
+        rec, buf = record(dx, x)
     x_, u_ = _dense(x, dtype), _dense(u, dtype)
     F = torch.empty(T - 1, B, n, n + m, dtype=dtype, device=dev)
     f = torch.empty(T - 1, B, n, dtype=dtype, device=dev)
@@ -129,6 +133,112 @@ def linearize_raw(dx, T, x, u):
         rc = fn(ctypes.byref(rec), B, T, n, m, ptr(x_), ptr(u_), ptr(F), ptr(f), stream_handle(dev))
     check(rc, "mpcb200_mlp_linearize")
     return F, f
+
+
+def vjp_workspace_bytes(dx, B, T, elem_size):
+    """Bytes of mpcb200_mlp_linearize_vjp_*'s workspace for the network of `dx`; 0 when its VJP does not fit the
+    kernel's shared memory (mpcb200_mlp_linearize_vjp_workspace_bytes, no device needed)."""
+    net, n_prev = _net(dx)
+    return int(_lib.lib().mpcb200_mlp_linearize_vjp_workspace_bytes(ctypes.byref(_record(net, n_prev, 1)), int(B),
+                                                                     int(T), int(elem_size)))
+
+
+def linearize_vjp_raw(dx, T, x, u, dF, df, rec=None, buf=None):
+    """dtheta [n_params]: the gradient of sum(dF * F) + sum(df * f) for (F, f) = linearize_raw(dx, T, x, u) in the
+    network's parameters, packed W0 b0 W1 b1 ... as _layout orders them; two kernels.  rec, buf: the record and
+    packed buffer to differentiate at (default: record(dx, x))."""
+    from .step import _dense
+    _, B, n = x.shape
+    m = u.shape[2]
+    dtype, dev = x.dtype, x.device
+    for name, t, shape in (("dF", dF, (T - 1, B, n, n + m)), ("df", df, (T - 1, B, n))):
+        if tuple(t.shape) != shape:
+            raise MpcB200Error(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
+    if rec is None:
+        rec, buf = record(dx, x)
+    nbytes = vjp_workspace_bytes(dx, B, T, x.element_size())
+    if nbytes == 0:
+        raise MpcB200Error("mpcb200_mlp_linearize_vjp: the network's VJP does not fit the kernel's shared memory")
+    x_, u_, dF_, df_ = (_dense(t, dtype) for t in (x, u, dF, df))
+    dtheta = torch.empty(buf.numel(), dtype=dtype, device=dev)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    fn = _lib.entry("mpcb200_mlp_linearize_vjp", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(rec), B, T, n, m, ptr(x_), ptr(u_), ptr(dF_), ptr(df_), ptr(dtheta), ptr(ws), nbytes,
+                stream_handle(dev))
+    check(rc, "mpcb200_mlp_linearize_vjp")
+    return dtheta
+
+
+def _torch_linearize(dx, x, u):
+    """(F, f) of linearize_raw by torch ops: the network and NNDynamics.grad_input at every (t, b), as
+    MPC.linearize_dynamics's ANALYTIC tail forms them; differentiable in the weights under enable_grad."""
+    net, n_prev = _net(dx)
+    T, B, N = x.shape
+    m = u.shape[2]
+    xs, us = x[:-1].reshape(-1, N)[:, n_prev:], u[:-1].reshape(-1, m)
+    R, S = net.grad_input(xs, us)
+    f = net(xs, us) - (R @ xs.unsqueeze(2)).squeeze(2) - (S @ us.unsqueeze(2)).squeeze(2)
+    F = torch.cat((R, S), 2)
+    if n_prev:                  # the rows [0 0 I] and f 0 of the previous control, no column for it in the network's
+        eye = torch.eye(n_prev, dtype=x.dtype, device=x.device).expand(xs.shape[0], -1, -1)
+        top = torch.cat((torch.zeros(xs.shape[0], n_prev, N, dtype=x.dtype, device=x.device), eye), 2)
+        F = torch.cat((top, torch.cat((torch.zeros_like(F[:, :, :n_prev]), F), 2)), 1)
+        f = torch.cat((torch.zeros_like(f[:, :n_prev]), f), 1)
+    return F.view(T - 1, B, N, N + m), f.view(T - 1, B, N)
+
+
+class MlpLinearize(torch.autograd.Function):
+    """(F, f) = linearize_raw(dx, T, x, u) along detached (x, u), differentiable in the network's parameter tensors
+    (the inputs after dx, T, x, u, in _layout's order W0 b0 W1 b1 ...): the backward is mpcb200_mlp_linearize_vjp_*
+    on the packed buffer the forward used.  The parameters are saved for backward, so an in-place edit between the
+    two raises autograd's version-counter error.  Under create_graph the backward recomputes the VJP with torch ops
+    (_torch_linearize), so higher-order gradients are those of the torch path.  One module-level Function (DESIGN.md
+    section 3.2)."""
+
+    @staticmethod
+    def forward(ctx, dx, T, x, u, *params):
+        rec, buf = record(dx, x)
+        F, f = linearize_raw(dx, T, x, u, rec, buf)
+        ctx.save_for_backward(*params)
+        ctx.dx, ctx.T, ctx.rec, ctx.buf, ctx.x, ctx.u = dx, T, rec, buf, x, u
+        return F, f
+
+    @staticmethod
+    def backward(ctx, dF, df):
+        params = ctx.saved_tensors              # raises if a parameter was edited in place since the forward
+        want = ctx.needs_input_grad[4:]
+        if torch.is_grad_enabled():             # create_graph: the torch formula, differentiable again
+            net, _ = _net(ctx.dx)
+            live = [t for fc in net.fcs for t in (fc.weight, fc.bias)]
+            wanted = [p for p, w in zip(live, want) if w]
+            F, f = _torch_linearize(ctx.dx, ctx.x, ctx.u)
+            g = iter(torch.autograd.grad((F * dF).sum() + (f * df).sum(), wanted, create_graph=True,
+                                         allow_unused=True))
+            grads = [next(g) if w else None for w in want]
+            grads = [torch.zeros_like(p) if w and gi is None else gi for p, w, gi in zip(params, want, grads)]
+        else:
+            dtheta = linearize_vjp_raw(ctx.dx, ctx.T, ctx.x, ctx.u, dF, df, ctx.rec, ctx.buf)
+            grads, o = [], 0
+            for p, w in zip(params, want):
+                grads.append(dtheta[o:o + p.numel()].view(p.shape) if w else None)
+                o += p.numel()
+        return (None, None, None, None, *grads)
+
+
+def linearize_diff(dx, T, x, u):
+    """(F, f) of linearize_raw as MPC's differentiable tail needs them, or None where the torch tail must form them:
+    through MlpLinearize when autograd records and a parameter of the network requires grad, one linearize_raw
+    launch and no graph when none does; None when its VJP does not fit the kernel (vjp_workspace_bytes 0).  x and u
+    are detached (no gradient reaches the linearisation point)."""
+    net, _ = _net(dx)
+    params = [t for fc in net.fcs for t in (fc.weight, fc.bias)]
+    x, u = x.detach(), u.detach()
+    if not torch.is_grad_enabled() or not any(p.requires_grad for p in params):
+        return linearize_raw(dx, T, x, u)
+    if vjp_workspace_bytes(dx, x.shape[1], T, x.element_size()) == 0:
+        return None
+    return MlpLinearize.apply(dx, T, x, u, *params)
 
 
 def step_raw(dx, n_state, n_ctrl, T, x_init, C, c, F, f, cur_x, cur_u, u_lower=None, u_upper=None, u_zero_I=None,

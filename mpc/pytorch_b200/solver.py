@@ -521,9 +521,13 @@ class MPC(Module):
         T, n, m = self.T, self.n_state, self.n_ctrl
         B = x.shape[1]
         kind, kparams = self._kernel_linearization(dynamics, x, diff)
-        if not kind and not diff and self._mlp_on_device(dynamics, x):    # a network's exact Jacobians, one kernel
-            from .mlp import linearize_raw
-            return linearize_raw(dynamics, T, x.detach(), u.detach())
+        if not kind and self._mlp_on_device(dynamics, x):
+            from .mlp import linearize_diff, linearize_raw
+            if not diff:       # a network's exact Jacobians, one kernel
+                return linearize_raw(dynamics, T, x.detach(), u.detach())
+            Ff = linearize_diff(dynamics, T, x, u)     # differentiable in the weights through the VJP kernel
+            if Ff is not None:
+                return Ff
         if kind:               # exact Jacobians of a known system by forward-mode duals, one kernel
             from .dynamics import dyn_linearize_raw, linearize_known
             if diff:           # differentiable in the system's parameters through the VJP kernel

@@ -314,12 +314,23 @@ static int run_mlp() {
     bad += gF[i] != (c == r ? 1.f : 0.f);
   }
   for (float v : gf) bad += v != 0.f;
+  // the VJP with dF = 0, df = 1: every hidden output is sigmoid(0) = 1/2 and every tangent 0, so only the last layer
+  // has a gradient, db_1 = (T-1) B and dW_1 = (T-1) B / 2
+  const size_t vws = mpcb200_mlp_linearize_vjp_workspace_bytes(&net, B, T, 4);
+  Dev<float> dF((T - 1) * B * n * p), df((T - 1) * B * n), dth(prm.n), vw(vws / sizeof(float) + 64);
+  dF.up(std::vector<float>(dF.n, 0.f));
+  df.up(std::vector<float>(df.n, 1.f));
+  rc = vws == 0 ? -1 : mpcb200_mlp_linearize_vjp_f32(&net, B, T, n, m, x.p, u.p, dF.p, df.p, dth.p, vw.p, vws, nullptr);
+  if (rc != 0 || cudaDeviceSynchronize() != cudaSuccess) return printf("mlp linearize vjp rc=%d\n", rc), 1;
+  const auto gth = dth.down();
+  for (int i = 0; i < (int)prm.n; ++i)
+    bad += gth[i] != (i >= net.b_off[1] ? (T - 1) * B : i >= net.W_off[1] ? 0.5f * (T - 1) * B : 0.f);
   mpcb200_mlp big = net;
   big.n_layers = 3; big.width[1] = big.width[2] = 256; big.width[3] = n;
   big.W_off[1] = 256 * p + 256; big.b_off[1] = big.W_off[1] + 256 * 256;
   big.W_off[2] = big.b_off[1] + 256; big.b_off[2] = big.W_off[2] + 256 * n;
   if (mpcb200_mlp_fits(&big, 4)) ++bad;
-  printf("mlp: rollout and linearisation of x' = x, %d bad; [256, 256] refused by mpcb200_mlp_fits\n", bad);
+  printf("mlp: rollout, linearisation and its VJP of x' = x, %d bad; [256, 256] refused by mpcb200_mlp_fits\n", bad);
   return bad != 0;
 }
 
