@@ -719,6 +719,58 @@ int mpcb200_ilqr_mlp_f64(const mpcb200_dims* dims, const mpcb200_params* params,
                          const uint8_t* u_zero_I, double* best_x, double* best_u, double* best_costs,
                          double* best_full_du_norm, int32_t* info, void* workspace, size_t workspace_bytes,
                          void* stream);
+/* A receding-horizon episode planned with the network (mlp->n_prev 0; no slew-rate penalty): mpcb200_episode_plant_*
+ * with every solve the loop of mpcb200_ilqr_mlp_* (dims->dynamics_kind 0, no F or f).  plant NULL: the network steps
+ * the loop, x_{k+1} = net(x_k, u_k) (+ w_k), by mpcb200_mlp_rollout_* at T = 2 from x_k and the solve's best
+ * controls.  Otherwise the plant steps it as in mpcb200_episode_plant_* (a LinDx or a known system's own kind, not a
+ * passthrough kind).  w, plan_x and plan_u are optional (plan_x and plan_u together).  Checks, capture contract,
+ * launch counting and MPCB200_ERR_NO_GRAPH_COND as for mpcb200_episode_*; every argument error is reported before
+ * anything is captured: MPCB200_ERR_SMEM for a network that does not fit, MPCB200_ERR_BAD_DIMS for T < 3 or
+ * n_steps < 1.  workspace: mpcb200_episode_mlp_workspace_bytes() bytes (0 for arguments it does not take),
+ * 256-byte aligned. */
+size_t mpcb200_episode_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts,
+                                           const mpcb200_mlp* mlp, int32_t elem_size);
+int mpcb200_episode_mlp_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                            const mpcb200_mlp* mlp, const mpcb200_plant* plant, int32_t n_steps, const float* C,
+                            const float* c, const float* F_plant, const float* f_plant, const float* w,
+                            const float* x_init, const float* u_init, const float* u_lower, const float* u_upper,
+                            const uint8_t* u_zero_I, float* xs, float* us, float* costs, int32_t* info, float* u_next,
+                            float* plan_x, float* plan_u, void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_mlp_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
+                            const mpcb200_mlp* mlp, const mpcb200_plant* plant, int32_t n_steps, const double* C,
+                            const double* c, const double* F_plant, const double* f_plant, const double* w,
+                            const double* x_init, const double* u_init, const double* u_lower, const double* u_upper,
+                            const uint8_t* u_zero_I, double* xs, double* us, double* costs, int32_t* info,
+                            double* u_next, double* plan_x, double* plan_u, void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* The reverse sweep of an episode of mpcb200_episode_mlp_* (run with plan_x, plan_u): mpcb200_episode_backward_plant_*
+ * with each solve's part taken through the network's linearisation along its plan, and dtheta[n_params] (the
+ * record's packed layout) the gradient of the network's parameters: the sum over control steps of the VJP of that
+ * linearisation (mpcb200_mlp_linearize_vjp_*) in the solve's adjoint, plus, with plant NULL, the network step's
+ * d<g_k, x_{k+1}>/dtheta.  The plant's outputs (dF_plant, df_plant or dtheta_plant) are those of
+ * mpcb200_episode_backward_plant_*; dw[n_steps,B,n] (NULL: not written) = g_k.  Every sum runs in a fixed order with
+ * no float atomics: dtheta is bitwise the same for every call, stream and graph replay on one card type.  Checks,
+ * capture contract, launch counting and MPCB200_ERR_NO_GRAPH_COND as for mpcb200_episode_backward_*; every argument
+ * error is reported before anything is captured, MPCB200_ERR_SMEM for a network or network VJP that does not fit.
+ * workspace: mpcb200_episode_backward_mlp_workspace_bytes() bytes (0 for arguments it does not take, among them a
+ * network whose VJP does not fit), 256-byte aligned. */
+size_t mpcb200_episode_backward_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_mlp* mlp,
+                                                    const mpcb200_plant* plant, int32_t elem_size);
+int mpcb200_episode_backward_mlp_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp,
+                                     const mpcb200_plant* plant, int32_t n_steps, const float* C, const float* c,
+                                     const float* F_plant, const float* u_lower, const float* u_upper,
+                                     const float* xs, const float* us, const float* plan_x, const float* plan_u,
+                                     const float* dl_dxs, const float* dl_dus, float* dx_init, float* dC, float* dc,
+                                     float* dtheta, float* dF_plant, float* df_plant, float* dtheta_plant, float* dw,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+int mpcb200_episode_backward_mlp_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp,
+                                     const mpcb200_plant* plant, int32_t n_steps, const double* C, const double* c,
+                                     const double* F_plant, const double* u_lower, const double* u_upper,
+                                     const double* xs, const double* us, const double* plan_x, const double* plan_u,
+                                     const double* dl_dxs, const double* dl_dus, double* dx_init, double* dC,
+                                     double* dc, double* dtheta, double* dF_plant, double* df_plant,
+                                     double* dtheta_plant, double* dw, void* workspace, size_t workspace_bytes,
+                                     void* stream);
 
 /* 1 if a kernel instance for (n_state, n_ctrl) is compiled in, else 0. */
 int mpcb200_supported(int32_t n_state, int32_t n_ctrl);

@@ -88,6 +88,9 @@ EXPORTED_SYMBOLS = (
     "mpcb200_mlp_linearize_f64", "mpcb200_mlp_step_f32", "mpcb200_mlp_step_f64", "mpcb200_mlp_step_workspace_bytes",
     "mpcb200_ilqr_mlp_f32", "mpcb200_ilqr_mlp_f64", "mpcb200_ilqr_mlp_workspace_bytes",
     "mpcb200_mlp_linearize_vjp_f32", "mpcb200_mlp_linearize_vjp_f64", "mpcb200_mlp_linearize_vjp_workspace_bytes",
+    "mpcb200_episode_mlp_f32", "mpcb200_episode_mlp_f64", "mpcb200_episode_mlp_workspace_bytes",
+    "mpcb200_episode_backward_mlp_f32", "mpcb200_episode_backward_mlp_f64",
+    "mpcb200_episode_backward_mlp_workspace_bytes",
 )
 
 # mpcb200_last_step_plan() bits (include/mpcb200.h)
@@ -236,6 +239,22 @@ def lib():
         fn.restype = ctypes.c_int
     L.mpcb200_ilqr_mlp_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(IlqrOpts), ctypes.c_int32]
     L.mpcb200_ilqr_mlp_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_episode_mlp_f32", "mpcb200_episode_mlp_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), ctypes.POINTER(IlqrOpts), mlp,
+                       ctypes.POINTER(Plant), ctypes.c_int32] + [vp] * 18 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_episode_mlp_workspace_bytes.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(IlqrOpts), mlp,
+                                                      ctypes.c_int32]
+    L.mpcb200_episode_mlp_workspace_bytes.restype = ctypes.c_size_t
+    for name in ("mpcb200_episode_backward_mlp_f32", "mpcb200_episode_backward_mlp_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(Params), mlp, ctypes.POINTER(Plant), ctypes.c_int32] + \
+            [vp] * 20 + [ctypes.c_size_t, vp]
+        fn.restype = ctypes.c_int
+    L.mpcb200_episode_backward_mlp_workspace_bytes.argtypes = [ctypes.POINTER(Dims), mlp, ctypes.POINTER(Plant),
+                                                               ctypes.c_int32]
+    L.mpcb200_episode_backward_mlp_workspace_bytes.restype = ctypes.c_size_t
     L.mpcb200_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
     L.mpcb200_supported.restype = ctypes.c_int
     L.mpcb200_supported_list.argtypes = [ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]

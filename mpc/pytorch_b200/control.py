@@ -12,6 +12,11 @@ With ``differentiable=True`` the episode's x and u carry gradients.  On the devi
 solve's best iterate (``step.episode_raw(..., keep_plans=True)``) and the backward is one more library call
 (``step.episode_backward_raw``), the closed loop's reverse sweep as one CUDA graph, with or without a slew-rate
 penalty; the host path runs the same loop with autograd recording.
+
+An episode planned with a learned model (``NNDynamics`` on the kernels, ``mlp.episode_on_device``: no slew-rate
+penalty, not time-varying, the network itself, a LinDx or a known system stepping the loop) is one graph of its own in
+both directions (``mlp.episode_raw`` / ``mlp.episode_backward_raw``, NetEpisodeFn); the network's step there is its
+rollout kernel, where the host path calls the Module.
 """
 import copy
 from collections import namedtuple
@@ -113,16 +118,25 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plan
     cost = solver._expand_cost(cost, L or T, ctrl.n_batch if ctrl.n_batch is not None else B, n + m)
     w0 = _first_warm_start(ctrl, x_init)
     from .dynamics import params_scope
+    from .mlp import episode_on_device
     if differentiable and torch.is_grad_enabled() and _requires_grad(x_init, cost, dx, plant, disturbance):
         with params_scope():
             if _takes_device_path(ctrl, x_init, cost, dx, w0, plant):
                 ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
                 if ep is not None:
                     return ep
+            if episode_on_device(ctrl, x_init, cost, dx, w0, plant, time_varying, differentiable=True):
+                ep = _episode_net_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+                if ep is not None:
+                    return ep
             return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
     with torch.no_grad(), params_scope():     # a known system's CUDA parameters are read once per episode
         if _takes_device_path(ctrl, x_init, cost, dx, w0, plant):
             ep = _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
+            if ep is not None:
+                return ep
+        if episode_on_device(ctrl, x_init, cost, dx, w0, plant, time_varying):
+            ep = _episode_net(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
             if ep is not None:
                 return ep
         return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
@@ -191,7 +205,8 @@ def _takes_device_path(ctrl, x_init, cost, dx, w0, plant=None):
     """Whether the episode runs as one graph: exactly when each of its solves would take the device loop (T >= 3 is
     checked before) and the plant, if any, steps at the staged shape (_plant_on_device).  Decided on tensor metadata
     alone, which a time-varying episode's full-length inputs share with its windows, so the same rule serves both.
-    A learned model (NNDynamics) as model or plant keeps the host path, whose solves take MPC.forward's device loop."""
+    A learned model (NNDynamics) as model or plant never runs on this graph: mlp.episode_on_device decides whether an
+    episode planned with one runs on its own (mlp.episode_raw), and otherwise the host path runs it."""
     from .mlp import _net
     if _net(dx)[0] is not None or _net(plant)[0] is not None:     # the episode's graph cannot step a network
         return False
@@ -400,6 +415,117 @@ def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None
     try:
         x, u, costs, info, u_next = EpisodeFn.apply((ctrl, dx, n_steps, w0, plant, L), x_init, cost.C, cost.c, F,
                                                     f, params, *extra)
+    except _NoGraph:
+        solver._graph_cond_unavailable = True
+        return None
+    return Episode(x, u, costs, info, u_next)
+
+
+def _net_plant_spec(ctrl, x_init, C, dx, plant, F_p=None, f_p=None):
+    """The plant of an episode planned with a learned model as mlp.episode_raw takes it: None where the network itself
+    steps the loop (plant None or dx), else _plant_spec's."""
+    if plant is None or plant is dx:
+        return None
+    return _plant_spec(ctrl, x_init, C, plant, F_p, f_p)
+
+
+def _episode_net(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
+    """The episode planned with a learned model as one library call (mlp.episode_raw) on the problem
+    MPC._ilqr_device stages; None when the driver refused the graph (nothing ran then)."""
+    from .mlp import episode_raw
+    T, m = ctrl.T, ctrl.n_ctrl
+    n, x0, C, c, _, _, _ = ctrl._device_problem(x_init, cost, dx)
+    F_p, f_p = (plant.F, plant.f) if isinstance(plant, LinDx) else (None, None)
+    res = episode_raw(dx, n, m, T, n_steps, x0, C, c, w0, plant=_net_plant_spec(ctrl, x_init, C, dx, plant, F_p, f_p),
+                      w=w, **ctrl._device_options())
+    if res is None:
+        solver._graph_cond_unavailable = True
+        return None
+    ctrl._print_pnqp_warnings(res["info"][:, 1].sum())      # the one host read, and only when they are printed
+    return Episode(res["x"], res["u"], res["costs"], res["info"], res["u_next"])
+
+
+class NetEpisodeFn(torch.autograd.Function):
+    """(x, u, costs, info, u_next) of a differentiable episode planned with a learned model: the forward is
+    mlp.episode_raw with keep_plans, the backward one mlp.episode_backward_raw call.  One module-level Function
+    (DESIGN.md section 3.2).  `o` = (ctrl, dx, n_steps, w0, plant).  The inputs after o are x_init, C, c, a LinDx
+    plant's F_p and f_p, a known plant's params, w, and the network's weights and biases in _layout's order W0 b0 W1
+    b1 ...; dtheta of the sweep is split into views shaped like them.  The weights, like every tensor the backward
+    reads (xs, us, the plans, the staged C, c, bounds and plant), go through save_for_backward, so an in-place edit of
+    a weight before the backward raises; ctx holds the staged problem's metadata, the packed weights the forward ran
+    with and the Module.  First order only: the backward is raw kernels.  costs, info and u_next carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, o, x_init, C, c, F_p, f_p, plant_params, w, *weights):
+        from .mlp import episode_raw
+        ctrl, dx, n_steps, w0, plant = o
+        T, m = ctrl.T, ctrl.n_ctrl
+        n, x0, C_, c_, _, _, _ = ctrl._device_problem(x_init, QuadCost(C, c), dx)
+        res = episode_raw(dx, n, m, T, n_steps, x0, C_, c_, w0,
+                          plant=_net_plant_spec(ctrl, x_init, C, dx, plant, F_p, f_p), w=w, keep_plans=True,
+                          **ctrl._device_options())
+        if res is None:
+            raise _NoGraph()
+        ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
+        s, _, xs, us, plan_x, plan_u, _, rec, buf, disturbed = res["saved"]
+        sp = s.plant
+        ctx.save_for_backward(xs, us, plan_x, plan_u, s.C, s.c, s.u_lower, s.u_upper,
+                              sp.F if sp is not None else None, sp.f if sp is not None else None, *weights)
+        ctx.problem = s._replace(C=None, c=None, u_lower=None, u_upper=None, u_zero_I=None,
+                                 plant=sp._replace(F=None, f=None) if sp is not None else None)
+        ctx.net = (n_steps, dx, rec, buf, disturbed)
+        ctx.plant_meta = (F_p.shape if F_p is not None else None, f_p.shape if f_p is not None else None,
+                          (plant_params.dtype, plant_params.device) if plant_params is not None else None)
+        ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
+        return res["x"], res["u"], res["costs"], res["info"], res["u_next"]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dl_dx, dl_du, *_):
+        from .mlp import episode_backward_raw
+        xs, us, plan_x, plan_u, C, c, lo, hi, Fp, fp, *weights = ctx.saved_tensors    # raises after an in-place edit
+        s = ctx.problem._replace(C=C, c=c, u_lower=lo, u_upper=hi)
+        if s.plant is not None:
+            s = s._replace(plant=s.plant._replace(F=Fp, f=fp))
+        n_steps, dx, rec, buf, disturbed = ctx.net
+        B, n, m = s.dims.B, s.pad.n, s.pad.m
+        if dl_dx is None:
+            dl_dx = xs.new_zeros(n_steps + 1, B, n)
+        if dl_du is None:
+            dl_du = us.new_zeros(n_steps, B, m)
+        dx_init, dC, dc, dtheta, dF_p, df_p, dth_p, dw = episode_backward_raw(
+            (s, n_steps, xs, us, plan_x, plan_u, dx, rec, buf, disturbed), dl_dx, dl_du)
+        need = ctx.needs_input_grad
+        F_shape, f_shape, pp_meta = ctx.plant_meta
+        dFp = dfp = dpp = None
+        if dF_p is not None and need[4]:          # the plant steps with its slice 0
+            dFp = dF_p.new_zeros(F_shape)
+            dFp[0] = dF_p
+        if df_p is not None and need[5]:
+            dfp = df_p.new_zeros(f_shape)
+            dfp[0] = df_p
+        if dth_p is not None and need[6]:
+            dpp = dth_p.sum(0).to(dtype=pp_meta[0], device=pp_meta[1])
+        dweights, o = [], 0
+        for p, want in zip(weights, need[8:]):
+            dweights.append(dtheta[o:o + p.numel()].view(p.shape) if want else None)
+            o += p.numel()
+        return (None, dx_init if need[1] else None, dC if need[2] else None, dc if need[3] else None, dFp, dfp, dpp,
+                dw if dw is not None and need[7] else None, *dweights)
+
+
+def _episode_net_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
+    """The differentiable episode planned with a learned model (NetEpisodeFn); None when the driver refused the
+    graph."""
+    F_p = f_p = p_params = None
+    if isinstance(plant, LinDx):
+        F_p, f_p = plant.F, plant.f
+    elif plant is not None and plant is not dx:
+        p_params = getattr(plant, "params", None)
+    weights = [t for fc in dx.fcs for t in (fc.weight, fc.bias)]
+    try:
+        x, u, costs, info, u_next = NetEpisodeFn.apply((ctrl, dx, n_steps, w0, plant), x_init, cost.C, cost.c, F_p,
+                                                       f_p, p_params, w, *weights)
     except _NoGraph:
         solver._graph_cond_unavailable = True
         return None

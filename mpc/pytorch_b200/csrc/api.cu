@@ -969,9 +969,10 @@ struct EpisodeLayout {                // workspace carve-up: the iLQR loop's wor
   IlqrLayout ilqr;
   size_t best_x, best_u, best_costs, best_fdn, info, state, warm, traj, ep, total;
 };
-static EpisodeLayout episode_layout(const mpcb200_dims* d, size_t sz, int knob) {
+// net: the solve is a learned model's (ilqr_mlp_layout)
+static EpisodeLayout episode_layout(const mpcb200_dims* d, size_t sz, int knob, bool net = false) {
   EpisodeLayout l;
-  l.ilqr = ilqr_layout(d, sz, knob);
+  l.ilqr = net ? ilqr_mlp_layout(d, sz, knob) : ilqr_layout(d, sz, knob);
   const size_t TB = (size_t)d->T * d->B, B = d->B;
   const size_t n = d->n, m = d->m;
   size_t o = l.ilqr.total;
@@ -1006,6 +1007,8 @@ struct EpisodeCall {
   // mpcb200_episode_plant_*: the plant that steps the loop and the disturbances; otherwise the model steps it
   const mpcb200_plant* plant;
   const R *F_plant, *f_plant, *w;
+  // mpcb200_episode_mlp_*: the learned model every solve plans with and, without a plant, that steps the loop
+  const mpcb200_mlp* mlp = nullptr;
 };
 
 // the model step's kind, parameters, F, f and has_f: the plant's where the call names one, else the model's
@@ -1053,6 +1056,13 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
       e.u_next == nullptr || e.workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (e.d->T < 3 || e.n_steps < 1) return MPCB200_ERR_BAD_DIMS;     // the warm-start shift reads u[T-3]
+  if (e.mlp != nullptr) {             // a learned model: a network that fits, without the slew-rate state
+    MlpShape s;
+    rc = mlp_check(e.mlp, e.d->B, e.d->T, e.d->n, e.d->m, s);
+    if (rc) return rc;
+    if (s.n_prev != 0) return MPCB200_ERR_BAD_DIMS;
+    if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
+  }
   if ((e.plan_x == nullptr) != (e.plan_u == nullptr)) return MPCB200_ERR_NULL_POINTER;
   if (e.plant != nullptr) {
     rc = plant_check(e.d, e.plant);
@@ -1060,20 +1070,22 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
     if (e.plant->kind == DYN_LINEAR && (e.F_plant == nullptr || (e.plant->has_f && e.f_plant == nullptr)))
       return MPCB200_ERR_NULL_POINTER;
   }
-  const EpisodeLayout l = episode_layout(e.d, sizeof(R), knob);
+  const EpisodeLayout l = episode_layout(e.d, sizeof(R), knob, e.mlp != nullptr);
   if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
-  return ilqr_check<R>(episode_solve(e, l), knob);
+  const IlqrCall<R> q = episode_solve(e, l);
+  return e.mlp != nullptr ? ilqr_mlp_check<R>(q, e.mlp, knob) : ilqr_check<R>(q, knob);
 }
 
 // Adds the episode's init kernel and its `while` node over control steps (body recorded on `es`) to the graph `os`
 // is capturing.  Body: [window_stage_kernel, with wc] -> the iLQR loop (its own `while` node, body on `bs`) -> model
-// step -> [episode_plans_kernel, with plan_x / plan_u] -> episode_advance_kernel.
+// step -> [episode_plans_kernel, with plan_x / plan_u] -> episode_advance_kernel.  With e.mlp the iLQR loop is
+// ilqr_mlp_record's, and without a plant the model step is the network's rollout at T = 2.
 template <typename R>
 static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, const EpisodeCall<R>& e, int knob,
                           const WindowCopy<R>* wc = nullptr) {
   const mpcb200_dims* d = e.d;
-  const EpisodeLayout l = episode_layout(d, sizeof(R), knob);
+  const EpisodeLayout l = episode_layout(d, sizeof(R), knob, e.mlp != nullptr);
   const IlqrCall<R> q = episode_solve(e, l);
   char* ws = (char*)e.workspace;
   R* state = (R*)(ws + l.state);
@@ -1090,11 +1102,13 @@ static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, con
   rc = open_while(os, es, handle);
   if (rc) return rc;
   if (wc != nullptr) rc = counted(window_launch_stage<R>(*wc, es));
-  if (rc == 0) rc = ilqr_record<R>(es, bs, q, knob);
+  if (rc == 0) rc = e.mlp != nullptr ? ilqr_mlp_record<R>(es, bs, q, e.mlp, knob) : ilqr_record<R>(es, bs, q, knob);
   // the model step (the plant's, where the call names one) from the solve's best controls, by the launchers the
   // solve's rollout uses, at T = 2
   const EpisodeStep<R> s = episode_step(e);
-  if (rc == 0 && s.kind == DYN_LINEAR) {
+  if (rc == 0 && e.mlp != nullptr && e.plant == nullptr) {
+    rc = mlp_rollout_impl<R>(e.mlp, B, 2, N, M, state, q.best_u, traj, es);
+  } else if (rc == 0 && s.kind == DYN_LINEAR) {
     mpcb200_dims d2 = *d;
     d2.T = 2;
     d2.F_T = 1;
@@ -1208,6 +1222,8 @@ struct EpGradCall {
   const mpcb200_plant* plant = nullptr;
   const R* F_plant = nullptr;
   R *dF_plant = nullptr, *df_plant = nullptr, *dtheta_plant = nullptr, *dw = nullptr;
+  // mpcb200_episode_backward_mlp_*: the learned model; dtheta is then its packed parameters' gradient [n_params]
+  const mpcb200_mlp* mlp = nullptr;
 };
 
 // the plant entry's own checks: plant_check, a passthrough kind exactly under a slew-rate penalty (n_prev its
@@ -1368,6 +1384,155 @@ static int epgrad_impl(const EpGradCall<R>& q, void* stream) {
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t bs = ilqr_stream(2);
     return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_record<R>(os, bs, q, knob);
+  });
+}
+
+// ---------------------------------------------------------------------------------------------
+// the reverse sweep of an episode planned with a learned model (mpcb200_episode_backward_mlp_*, episode_grad.cuh):
+// per step the network's linearisation along the staged plan, the model step's VJP from its slice 0 (or the plant's
+// stage), the KKT adjoint, and the linearisation's VJP in the weights summed into dtheta
+// ---------------------------------------------------------------------------------------------
+// dims of the network's linearisation, which the adjoint reads: F [T-1, B, n, p] and f [T-1, B, n], dense
+static mpcb200_dims epgrad_net_dims(const mpcb200_dims* d) {
+  mpcb200_dims dn = *d;
+  dn.F_T = d->T - 1; dn.has_f = 1; dn.F_tstride = 0; dn.f_tstride = 0;
+  return dn;
+}
+
+struct EpNetLayout {                  // epgrad_layout's carve-up at epgrad_net_dims, then the network's buffers
+  EpGradLayout g;
+  size_t Fk, fk, dthk, vjp, vjp_bytes, total;
+};
+// step_kind: the plant's kind, -1 when the network steps the loop; vjp_bytes 0 where its VJP does not fit
+static EpNetLayout epgrad_net_layout(const mpcb200_dims* d, const MlpShape& s, size_t sz, int knob, int step_kind) {
+  EpNetLayout l;
+  const mpcb200_dims dn = epgrad_net_dims(d);
+  l.g = epgrad_layout(&dn, sz, knob, step_kind);
+  const size_t T1B = (size_t)(d->T - 1) * d->B, n = d->n, p = (size_t)d->n + d->m;
+  size_t o = l.g.total;
+  l.Fk = o;   o += up256(T1B * n * p * sz);       // the linearisation along the staged plan
+  l.fk = o;   o += up256(T1B * n * sz);
+  l.dthk = o; o += up256((size_t)s.n_params * sz);  // step k's weight gradient
+  l.vjp_bytes = mlp_vjp_ws(s, d->B, d->T, sz);
+  l.vjp = o;  o += l.vjp_bytes;
+  l.total = o;
+  return l;
+}
+
+// argument checks that need no device: every error is reported before anything is captured or launched
+template <typename R>
+static int epgrad_mlp_check(const EpGradCall<R>& q, int knob, MlpShape& s) {
+  const mpcb200_dims* d = q.d;
+  int rc = check_dims(d);
+  if (rc) return rc;
+  if (q.mlp == nullptr || q.p == nullptr || q.C == nullptr || q.c == nullptr || q.xs == nullptr ||
+      q.us == nullptr || q.plan_x == nullptr || q.plan_u == nullptr || q.dl_dxs == nullptr || q.dl_dus == nullptr ||
+      q.dx_init == nullptr || q.dC == nullptr || q.dc == nullptr || q.dtheta == nullptr || q.workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (d->T < 3 || q.n_steps < 1 || d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  rc = mlp_check(q.mlp, d->B, d->T, d->n, d->m, s);
+  if (rc) return rc;
+  if (s.n_prev != 0) return MPCB200_ERR_BAD_DIMS;
+  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100() || mlp_vjp_ws(s, d->B, d->T, sizeof(R)) == 0)
+    return MPCB200_ERR_SMEM;
+  rc = check_bounds(d, q.u_lower, q.u_upper);
+  if (rc) return rc;
+  if (q.plant != nullptr) {
+    rc = epgrad_plant_check(q);
+    if (rc) return rc;
+  }
+  const EpNetLayout l = epgrad_net_layout(d, s, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
+  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+// Adds dtheta's zeroing, the init kernel and the `while` node over k = n_steps-1 .. 0 (body recorded on `bs`) to the
+// graph `os` is capturing.  Body (episode_grad.cuh): plan or the plant's stage -> linearisation -> [stage_net] ->
+// adjoint -> [net_step_param] -> linearisation VJP -> add -> accumulate.
+template <typename R>
+static int epgrad_mlp_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, const MlpShape& s, int knob) {
+  const mpcb200_dims* d = q.d;
+  const EpNetLayout l = epgrad_net_layout(d, s, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
+  const EpGradLayout& lg = l.g;
+  char* ws = (char*)q.workspace;
+  const int B = d->B, T = d->T, N = d->n, M = d->m;
+  R* Fk = (R*)(ws + l.Fk);
+  R* fk = (R*)(ws + l.fk);
+  R* dthk = (R*)(ws + l.dthk);
+  R* dxk = (R*)(ws + lg.dxk);
+  R* dCk = (R*)(ws + lg.dCk);
+  R* dck = (R*)(ws + lg.dck);
+  R* dFk = (R*)(ws + lg.dFk);
+  R* dfk = (R*)(ws + lg.dfk);
+  EpGradArgs<R> a;
+  std::memset(&a, 0, sizeof(a));
+  a.B = B; a.T = T; a.N = N; a.M = M; a.n_steps = q.n_steps; a.F_T = lg.da.F_T; a.has_f = 1;
+  a.kind = EPGRAD_KIND_NET; a.NP = 0;
+  a.xs = q.xs; a.us = q.us; a.plan_x = q.plan_x; a.plan_u = q.plan_u; a.dl_dxs = q.dl_dxs; a.dl_dus = q.dl_dus;
+  a.F = Fk;                           // slice 0: the Jacobian of the model step at (x_k, u_k)
+  a.stage_x = (R*)(ws + lg.stage_x); a.stage_u = (R*)(ws + lg.stage_u);
+  a.dl_dx = (R*)(ws + lg.dl_dx); a.dl_du = (R*)(ws + lg.dl_du);
+  a.gx = (R*)(ws + lg.gx);
+  a.g = q.dx_init;
+  a.dx_k = dxk; a.dC_k = dCk; a.dc_k = dck; a.dF_k = dFk; a.df_k = dfk;
+  a.dC = q.dC; a.dc = q.dc;
+  a.st = (EpGradState*)(ws + lg.state);
+  // a plant's stage: a copy of `a` with its kind, parameters, F and parameter-part outputs (as epgrad_record)
+  EpGradArgs<R> as = a;
+  EpPlantArgs<R> pl;
+  std::memset(&pl, 0, sizeof(pl));
+  if (q.plant != nullptr) {
+    const bool pknown = q.plant->kind != DYN_LINEAR;
+    as.kind = q.plant->kind; as.has_f = q.plant->has_f; as.NP = epgrad_nparams(q.plant->kind);
+    for (int i = 0; i < 8; ++i) as.dp.p[i] = q.plant->dyn[i];
+    as.F = pknown ? nullptr : q.F_plant;
+    as.dF = pknown ? nullptr : q.dF_plant;
+    as.df = pknown || !q.plant->has_f ? nullptr : q.df_plant;
+    as.theta_step = pknown ? (R*)(ws + lg.theta) : nullptr;
+    pl.kind = as.kind; pl.has_f = as.has_f; pl.NP = as.NP; pl.theta_step = as.theta_step;
+    pl.dF = as.dF; pl.df = as.df; pl.dtheta = pknown ? q.dtheta_plant : nullptr; pl.dw = q.dw;
+  } else if (q.dw != nullptr) {       // the network steps a disturbed loop: the plant forms write dw, nothing else
+    pl.kind = EPGRAD_KIND_NET;
+    pl.dw = q.dw;
+  }
+  const EpPlantArgs<R>* plp = q.plant != nullptr || q.dw != nullptr ? &pl : nullptr;
+  cudaGraphConditionalHandle handle;
+  int rc = while_handle(os, &handle);
+  if (rc) return rc;
+  if (counted(launch_fill_zero<R>((size_t)s.n_params, q.dtheta, os)) != 0 ||
+      counted(epgrad_launch_init<R>(a, 0, plp, handle, os)) != 0)
+    return MPCB200_ERR_LAUNCH;
+  rc = open_while(os, bs, handle);
+  if (rc) return rc;
+  rc = counted(q.plant != nullptr ? epgrad_launch_stage<R>(as, bs) : epgrad_launch_plan<R>(a, bs));
+  if (rc == 0) rc = mlp_linearize_impl<R>(q.mlp, B, T, N, M, a.stage_x, a.stage_u, Fk, fk, bs);
+  if (rc == 0 && q.plant == nullptr) rc = counted(epgrad_launch_stage_net<R>(a, bs));
+  if (rc == 0)
+    rc = adjoint_impl<R>(&lg.da, q.p, q.C, q.c, Fk, a.stage_x, a.stage_u, a.dl_dx, a.dl_du, q.u_lower, q.u_upper,
+                         dxk, dCk, dck, dFk, dfk, ws + lg.adj, lg.adj_bytes, knob, bs, true);
+  // the network's own step: with (dJ, df) = (g z^T, g) the VJP's G^ = dJ - df z^T is 0, so it returns d<g, x'>/dtheta
+  if (rc == 0 && q.plant == nullptr) rc = counted(epgrad_launch_net_step_param<R>(a, dFk, dfk, bs));
+  if (rc == 0)
+    rc = mlp_linearize_vjp_impl<R>(q.mlp, B, T, N, M, a.stage_x, a.stage_u, dFk, dfk, dthk, ws + l.vjp, l.vjp_bytes,
+                                   bs);
+  if (rc == 0) rc = counted(epgrad_launch_add<R>((size_t)s.n_params, dthk, q.dtheta, bs));
+  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, 0, plp, handle, bs));
+  cudaGraph_t body = nullptr;
+  if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
+  return rc;
+}
+
+template <typename R>
+static int epgrad_mlp_impl(const EpGradCall<R>& q, void* stream) {
+  const int knob = kernel_knob();
+  MlpShape s;
+  int rc = epgrad_mlp_check<R>(q, knob, s);
+  if (rc) return rc;
+  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
+  return run_graph(stream, [&](cudaStream_t os) {
+    cudaStream_t bs = ilqr_stream(2);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_mlp_record<R>(os, bs, q, s, knob);
   });
 }
 
@@ -1873,6 +2038,62 @@ size_t mpcb200_episode_backward_window_workspace_bytes(const mpcb200_dims* dims,
 MPCB200_EPISODE_BACKWARD_WINDOW(f32, float)
 MPCB200_EPISODE_BACKWARD_WINDOW(f64, double)
 #undef MPCB200_EPISODE_BACKWARD_WINDOW
+
+size_t mpcb200_episode_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts,
+                                           const mpcb200_mlp* mlp, int32_t elem_size) {
+  MlpShape s;
+  if (dims == nullptr || opts == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8))
+    return 0;
+  if (mlp_check(mlp, dims->B, dims->T, dims->n, dims->m, s) != 0 || s.n_prev != 0 ||
+      mlp_smem_bytes(s, elem_size, 1) > (size_t)kOptinAssumed)
+    return 0;
+  return episode_layout(dims, (size_t)elem_size, kernel_knob(), true).total;
+}
+#define MPCB200_EPISODE_MLP(SUF, R)                                                                                \
+  int mpcb200_episode_mlp_##SUF(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts, \
+                                const mpcb200_mlp* mlp, const mpcb200_plant* plant, int32_t n_steps, const R* C,   \
+                                const R* c, const R* F_plant, const R* f_plant, const R* w, const R* x_init,       \
+                                const R* u_init, const R* u_lower, const R* u_upper, const uint8_t* u_zero_I,      \
+                                R* xs, R* us, R* costs, int32_t* info, R* u_next, R* plan_x, R* plan_u,            \
+                                void* workspace, size_t workspace_bytes, void* stream) {                           \
+    if (mlp == nullptr) return MPCB200_ERR_NULL_POINTER;                                                           \
+    EpisodeCall<R> e = {dims, params, opts, n_steps, C, c, nullptr, nullptr, x_init, u_init, u_lower, u_upper,     \
+                        u_zero_I, xs, us, costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u, plant,  \
+                        F_plant, f_plant, w, mlp};                                                                 \
+    return episode_impl<R>(e, stream);                                                                             \
+  }
+MPCB200_EPISODE_MLP(f32, float)
+MPCB200_EPISODE_MLP(f64, double)
+#undef MPCB200_EPISODE_MLP
+
+size_t mpcb200_episode_backward_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_mlp* mlp,
+                                                    const mpcb200_plant* plant, int32_t elem_size) {
+  MlpShape s;
+  if (dims == nullptr || check_dims(dims) != 0 || dims->T < 3 || dims->dynamics_kind != DYN_LINEAR ||
+      (elem_size != 4 && elem_size != 8))
+    return 0;
+  if (mlp_check(mlp, dims->B, dims->T, dims->n, dims->m, s) != 0 || s.n_prev != 0 ||
+      mlp_smem_bytes(s, elem_size, 1) > (size_t)kOptinAssumed)
+    return 0;
+  if (plant != nullptr && (plant_check(dims, plant) != 0 || (plant->kind & DYN_CTRL_PASSTHROUGH) != 0)) return 0;
+  const EpNetLayout l = epgrad_net_layout(dims, s, (size_t)elem_size, kernel_knob(), plant != nullptr ? plant->kind : -1);
+  return l.vjp_bytes == 0 ? 0 : l.total;
+}
+#define MPCB200_EPISODE_BACKWARD_MLP(SUF, R)                                                                       \
+  int mpcb200_episode_backward_mlp_##SUF(                                                                          \
+      const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_mlp* mlp, const mpcb200_plant* plant,  \
+      int32_t n_steps, const R* C, const R* c, const R* F_plant, const R* u_lower, const R* u_upper, const R* xs,  \
+      const R* us, const R* plan_x, const R* plan_u, const R* dl_dxs, const R* dl_dus, R* dx_init, R* dC, R* dc,    \
+      R* dtheta, R* dF_plant, R* df_plant, R* dtheta_plant, R* dw, void* workspace, size_t workspace_bytes,        \
+      void* stream) {                                                                                              \
+    EpGradCall<R> q = {dims, params, n_steps, C, c, nullptr, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,     \
+                       dl_dus, dx_init, dC, dc, nullptr, nullptr, dtheta, workspace, workspace_bytes, false, 0,    \
+                       plant, F_plant, dF_plant, df_plant, dtheta_plant, dw, mlp};                                 \
+    return epgrad_mlp_impl<R>(q, stream);                                                                          \
+  }
+MPCB200_EPISODE_BACKWARD_MLP(f32, float)
+MPCB200_EPISODE_BACKWARD_MLP(f64, double)
+#undef MPCB200_EPISODE_BACKWARD_MLP
 
 int mpcb200_mlp_fits(const mpcb200_mlp* mlp, int32_t elem_size) {
   MlpShape s;

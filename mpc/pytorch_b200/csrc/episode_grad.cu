@@ -439,7 +439,86 @@ int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream) {
   return launched();
 }
 
+// ---- a learned model's sweep (episode_grad.cuh, EPGRAD_KIND_NET) ----
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_plan_kernel(const EpGradArgs<R> a) {
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  epgrad_stage_plan(a, (size_t)a.st->k, i0, step);
+}
+
+// One thread per (b, column j of F[0]), as epgrad_stage_linear_body, without the parameter part
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_stage_net_kernel(const EpGradArgs<R> a) {
+  const size_t k = (size_t)a.st->k;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const int N = a.N, M = a.M, P = N + M;
+  for (size_t idx = i0; idx < (size_t)a.B * P; idx += step) {
+    const size_t b = idx / P;
+    const int j = (int)(idx % P);
+    const R* g = a.g + b * N;
+    const R* Fb = a.F + b * N * P;
+    R v = R(0);
+    for (int i = 0; i < N; ++i) v += Fb[(size_t)i * P + j] * g[i];
+    if (j < N) a.gx[b * N + j] = v;
+    else a.dl_du[b * M + (j - N)] = a.dl_dus[(k * a.B + b) * M + (j - N)] + v;
+  }
+}
+
+// One thread per (b, column j): column j of dF_k[0] += g z_j, and (j = 0) df_k[0] += g
+template <typename R>
+__global__ void __launch_bounds__(256)
+epgrad_net_step_param_kernel(const EpGradArgs<R> a, R* __restrict__ dF_k, R* __restrict__ df_k) {
+  const size_t k = (size_t)a.st->k;
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+  const int N = a.N, M = a.M, P = N + M;
+  for (size_t idx = i0; idx < (size_t)a.B * P; idx += step) {
+    const size_t b = idx / P;
+    const int j = (int)(idx % P);
+    const R* g = a.g + b * N;
+    const R zj = j < N ? a.xs[(k * a.B + b) * N + j] : a.us[(k * a.B + b) * M + (j - N)];
+    R* dFb = dF_k + b * N * P;
+    for (int i = 0; i < N; ++i) dFb[(size_t)i * P + j] += g[i] * zj;
+    if (j == 0)
+      for (int i = 0; i < N; ++i) df_k[b * N + i] += g[i];
+  }
+}
+
+template <typename R>
+__global__ void __launch_bounds__(256) epgrad_add_kernel(size_t n, const R* __restrict__ src, R* __restrict__ dst) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    dst[i] += src[i];
+}
+
+template <typename R>
+int epgrad_launch_plan(const EpGradArgs<R>& a, cudaStream_t stream) {
+  const size_t items = (size_t)a.T * a.B * (a.N > a.M ? a.N : a.M);
+  epgrad_plan_kernel<R><<<epgrad_grid(items), 256, 0, stream>>>(a);
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_stage_net(const EpGradArgs<R>& a, cudaStream_t stream) {
+  epgrad_stage_net_kernel<R><<<epgrad_grid((size_t)a.B * (a.N + a.M)), 256, 0, stream>>>(a);
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_net_step_param(const EpGradArgs<R>& a, R* dF_k, R* df_k, cudaStream_t stream) {
+  epgrad_net_step_param_kernel<R><<<epgrad_grid((size_t)a.B * (a.N + a.M)), 256, 0, stream>>>(a, dF_k, df_k);
+  return launched();
+}
+
+template <typename R>
+int epgrad_launch_add(size_t n, const R* src, R* dst, cudaStream_t stream) {
+  epgrad_add_kernel<R><<<epgrad_grid(n), 256, 0, stream>>>(n, src, dst);
+  return launched();
+}
+
 #define MPCB200_EPGRAD_INST(R)                                                                                     \
+  template int epgrad_launch_plan<R>(const EpGradArgs<R>&, cudaStream_t);                                          \
+  template int epgrad_launch_stage_net<R>(const EpGradArgs<R>&, cudaStream_t);                                     \
+  template int epgrad_launch_net_step_param<R>(const EpGradArgs<R>&, R*, R*, cudaStream_t);                        \
+  template int epgrad_launch_add<R>(size_t, const R*, R*, cudaStream_t);                                           \
   template int episode_launch_plans<R>(int, int, int, int, const R*, const R*, R*, R*, const EpisodeState*,        \
                                        cudaStream_t);                                                              \
   template int launch_fill_zero<R>(size_t, R*, cudaStream_t);                                                      \

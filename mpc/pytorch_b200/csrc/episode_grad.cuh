@@ -117,4 +117,26 @@ int epgrad_launch_vjp_passthrough(const DynVjpArgs& a, cudaStream_t stream);
 template <typename R>
 int launch_fill_zero(size_t n, R* p, cudaStream_t stream);
 
+// An episode planned with a learned model (mpcb200_episode_backward_mlp_*).  Its parameters are the network's packed
+// weights, shared by every problem, so the per-problem parameter part of init and accumulate does not apply: the
+// sweep runs them with kind EPGRAD_KIND_NET and NP = 0 (and a plant record of that kind when the network itself
+// steps a disturbed loop), and they do everything else (g, dC, dc, dw, the plant's accumulators, the loop counter).
+// Body, no plant: plan -> the network's linearisation along the staged plan (Fk) -> stage_net (the model step's VJP
+// in x_k, u_k from slice 0 of Fk) -> adjoint -> net_step_param (g z_0^T, g into the adjoint's dF_k[0], df_k[0]) ->
+// the linearisation VJP into dtheta_k -> add (dtheta += dtheta_k) -> accumulate.  With a plant, the plant's stage
+// replaces plan and stage_net, and net_step_param is not run.
+constexpr int EPGRAD_KIND_NET = -1;
+// stage_x, stage_u = plan_x[k], plan_u[k]
+template <typename R>
+int epgrad_launch_plan(const EpGradArgs<R>& a, cudaStream_t stream);
+// gx = R^T g, dl_du[0] = dl_dus[k] + S^T g with [R S] = a.F, slice 0 of the network's linearisation
+template <typename R>
+int epgrad_launch_stage_net(const EpGradArgs<R>& a, cudaStream_t stream);
+// dF_k[0] += g [x_k; u_k]^T, df_k[0] += g
+template <typename R>
+int epgrad_launch_net_step_param(const EpGradArgs<R>& a, R* dF_k, R* df_k, cudaStream_t stream);
+// dst[i] += src[i], i < n
+template <typename R>
+int epgrad_launch_add(size_t n, const R* src, R* dst, cudaStream_t stream);
+
 }  // namespace mpcb200

@@ -12,6 +12,9 @@ its central differences in torch, and with it the host loop).  The rollout (``ge
 search compute the same function under every grad_method, so they take the kernels whenever ``on_device`` holds.
 MPC's differentiable tail (``linearize_dynamics(diff=True)``) takes ``linearize_diff``: ``MlpLinearize``, whose backward
 is the VJP of the linearisation in the weights (``mpcb200_mlp_linearize_vjp_*``, DESIGN.md section 3.11).
+
+A receding-horizon episode planned with the network runs as one graph in each direction where ``episode_on_device``
+holds (``episode_raw``, ``episode_backward_raw``; ``mpcb200_episode_mlp_*``, DESIGN.md section 3.12).
 """
 import ctypes
 
@@ -315,3 +318,134 @@ def ilqr_raw(dx, n_state, n_ctrl, T, x_init, C, c, u_init, u_lower=None, u_upper
         return None
     check(rc, "mpcb200_ilqr_mlp")
     return {"x": pad.crop_n(best_x), "u": pad.crop_m(best_u), "costs": costs, "full_du_norm": fdn, "info": info}
+
+
+def episode_on_device(ctrl, x_init, cost, dx, w0, plant=None, time_varying=False, differentiable=False):
+    """Whether a receding-horizon episode planned with the learned model `dx` runs as one graph
+    (mpcb200_episode_mlp_*, and with `differentiable` mpcb200_episode_backward_mlp_*): `dx` is exactly NNDynamics and
+    every solve would take MPC.forward's device loop with it (solver._use_device_loop: the network on the kernels,
+    ANALYTIC or AUTO_DIFF, a QuadCost, verbose <= 0, ...); no slew-rate penalty and not time-varying; the plant is None
+    or `dx` itself (the network steps the loop), a LinDx of x_init's dtype and device, or a known system at its own
+    (n_state, n_ctrl) where the episode runs unpadded; and, with `differentiable`, the network's linearisation VJP
+    fits its kernel.  Decided on metadata alone."""
+    from . import solver
+    from .control import _plant_on_device
+    from .dynamics import DYN_LINEAR
+    from .step import _pick_instance
+    if type(dx) is not NNDynamics or ctrl.slew_rate_penalty is not None or time_varying:
+        return False
+    if not solver._use_device_loop(ctrl, x_init, cost, dx, w0):
+        return False
+    if plant is not None and plant is not dx:
+        if isinstance(plant, NNDynamics) or not _plant_on_device(ctrl, x_init, dx, plant):
+            return False
+        if not isinstance(plant, solver.LinDx):       # a known plant steps at its own width: the staged one
+            n, m = ctrl.n_state, ctrl.n_ctrl
+            if _pick_instance(n, m, x_init.element_size(), DYN_LINEAR) != (n, m):
+                return False
+    return not differentiable or vjp_workspace_bytes(dx, x_init.shape[0], ctrl.T, x_init.element_size()) > 0
+
+
+def episode_raw(dx, n_state, n_ctrl, T, n_steps, x_init, C, c, u_init, u_lower=None, u_upper=None, u_zero_I=None,
+                delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5, eps=1e-7,
+                best_cost_eps=1e-4, plant=None, w=None, keep_plans=False):
+    """step.episode_raw with the network of `dx` as the model every solve plans with (mpcb200_episode_mlp_*): each
+    solve is ilqr_raw's graph, and without a plant the network steps the loop by its rollout kernel at T = 2,
+    x_{k+1} = rollout_raw(dx, 2, x_k, plan_u[:2])[1] (+ w_k).  plant: (kind, params, F_p, f_p) as step.episode_raw
+    takes it (a LinDx's slice 0, or a known system), or None; w [n_steps, B, n] or None.  The weights are packed once
+    (record, within the caller's params_scope).  Returns step.episode_raw's dict; keep_plans adds "saved", what
+    episode_backward_raw takes.  None when the driver has no conditional graph nodes (nothing was launched then)."""
+    from .step import _dense, _problem, _stage_plant, _validate
+    n, m = n_state, n_ctrl
+    if T < 3 or n_steps < 1:
+        raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
+    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
+                  bounds=(u_lower, u_upper), u_zero_I=u_zero_I, need_F=False)
+    dtype, dev = C.dtype, C.device
+    s = _problem(n, m, T, B, dtype, dev, C, c, None, None, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+                 max_linesearch_iter)
+    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    rec, buf = record(dx, C)
+    x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
+    sp = _stage_plant(pad, plant, dtype, B, n, m) if plant is not None else None
+    w_ = None
+    if w is not None:
+        if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
+            raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
+                               f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
+        w_ = pad.vec_n(_dense(w, dtype)).contiguous()
+    opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
+                         best_cost_eps=float(best_cost_eps))
+    nbytes = _lib.lib().mpcb200_episode_mlp_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), ctypes.byref(rec),
+                                                            C.element_size())
+    if nbytes == 0:
+        raise MpcB200Error("mpcb200_episode_mlp: the episode has no workspace size (the network does not fit, or bad "
+                           "dimensions)")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    xs = torch.empty(n_steps + 1, B, N, dtype=dtype, device=dev)
+    us = torch.empty(n_steps, B, M, dtype=dtype, device=dev)
+    costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
+    info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
+    u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
+    plan_x = plan_u = None
+    if keep_plans:
+        plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
+        plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
+    fn = _lib.entry("mpcb200_episode_mlp", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), ctypes.byref(rec),
+                ctypes.byref(sp.rec) if sp is not None else None, int(n_steps), ptr_view(s.C), ptr_view(s.c),
+                ptr(sp.F if sp is not None else None), ptr(sp.f if sp is not None else None), ptr(w_), ptr(x0_),
+                ptr(u0_), ptr(s.u_lower), ptr(s.u_upper), ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info),
+                ptr(u_next), ptr(plan_x), ptr(plan_u), ptr(ws), nbytes, stream_handle(dev))
+    if rc == _lib.ERR_NO_GRAPH_COND:
+        return None
+    check(rc, "mpcb200_episode_mlp")
+    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
+    if keep_plans:
+        res["saved"] = (s._replace(plant=sp), n_steps, xs, us, plan_x, plan_u, dx, rec, buf, w is not None)
+    return res
+
+
+def episode_backward_raw(saved, dl_dxs, dl_dus):
+    """The reverse sweep of an episode run by episode_raw(..., keep_plans=True) in ONE library call
+    (mpcb200_episode_backward_mlp_*): `saved` is that call's res["saved"], dl_dxs [n_steps+1, B, n] and dl_dus
+    [n_steps, B, m] the gradients of its x and u.  Returns (dx_init [B, n], dC [T, B, p, p], dc [T, B, p], dtheta
+    [n_params], dF_p [B, n, p], df_p [B, n], dtheta_p [B, NP_plant], dw [n_steps, B, n]): dtheta is the network's
+    packed W0 b0 W1 b1 ... (_layout); the plant's outputs are None where the episode had no such plant (or no f), dw
+    None where it added no w."""
+    from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, DYN_NPARAMS
+    from .step import _dense
+    s, n_steps, xs, us, plan_x, plan_u, dx, rec, buf, disturbed = saved
+    pad, dims = s.pad, s.dims
+    T, B, N, M = dims.T, dims.B, pad.N, pad.M
+    P = N + M
+    dtype, dev = xs.dtype, xs.device
+    gx_, gu_ = pad.vec_n(_dense(dl_dxs, dtype)), pad.vec_m(_dense(dl_dus, dtype))
+    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
+    dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
+    dc = torch.empty(T, B, P, dtype=dtype, device=dev)
+    dtheta = torch.empty(buf.numel(), dtype=dtype, device=dev)
+    sp = s.plant
+    pk = sp.rec.kind if sp is not None else None
+    dF_p = torch.empty(B, N, P, dtype=dtype, device=dev) if pk == DYN_LINEAR else None
+    df_p = torch.empty(B, N, dtype=dtype, device=dev) if pk == DYN_LINEAR and sp.rec.has_f else None
+    dth_p = (torch.empty(B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
+             if sp is not None and pk != DYN_LINEAR else None)
+    dw = torch.empty(n_steps, B, N, dtype=dtype, device=dev) if disturbed else None
+    prec = ctypes.byref(sp.rec) if sp is not None else None
+    nbytes = _lib.lib().mpcb200_episode_backward_mlp_workspace_bytes(ctypes.byref(dims), ctypes.byref(rec), prec,
+                                                                     xs.element_size())
+    if nbytes == 0:
+        raise MpcB200Error("mpcb200_episode_backward_mlp: the episode has no workspace size (the network's VJP does "
+                           "not fit, or bad dimensions)")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    fn = _lib.entry("mpcb200_episode_backward_mlp", dtype)
+    with _on_device(dev):
+        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(rec), prec, int(n_steps), ptr_view(s.C),
+                ptr_view(s.c), ptr(sp.F if sp is not None else None), ptr(s.u_lower), ptr(s.u_upper), ptr(xs),
+                ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dtheta),
+                ptr(dF_p), ptr(df_p), ptr(dth_p), ptr(dw), ptr(ws), nbytes, stream_handle(dev))
+    check(rc, "mpcb200_episode_backward_mlp")
+    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), dtheta, pad.crop_np(dF_p), pad.crop_n(df_p),
+            dth_p, pad.crop_n(dw))

@@ -334,9 +334,70 @@ static int run_mlp() {
   return bad != 0;
 }
 
+// the network episode entries: the zero-weight passthrough network steps x' = x, so with C = I, c = 0 every plan is
+// u = 0 and the episode holds x_init; its reverse sweep with dl_dx = 0, dl_du = 0 gives zero gradients.  T < 3 and a
+// network too large for shared memory are refused before anything is captured.
+static int run_episode_mlp() {
+  const int B = 3, T = 4, n = 3, m = 2, h = 8, p = n + m, steps = 3;
+  mpcb200_mlp net = {};
+  net.n_layers = 2; net.width[0] = p; net.width[1] = h; net.width[2] = n;
+  net.activation = MPCB200_ACT_SIGMOID; net.passthrough = 1;
+  net.W_off[0] = 0; net.b_off[0] = h * p; net.W_off[1] = h * p + h; net.b_off[1] = h * p + h + n * h;
+  const int np = h * p + h + n * h + n;
+  Dev<float> prm(np), C(T * B * p * p), c(T * B * p), x0(B * n), u0(T * B * m), xs((steps + 1) * B * n),
+      us(steps * B * m), costs(steps * B), info(2 * steps), un(T * B * m), px(steps * T * B * n), pu(steps * T * B * m);
+  prm.up(std::vector<float>(np, 0.f));
+  std::vector<float> hC(C.n, 0.f), hx(B * n);
+  for (int i = 0; i < T * B; ++i)
+    for (int j = 0; j < p; ++j) hC[(size_t)i * p * p + j * p + j] = 1.f;
+  for (auto& v : hx) v = rnd();
+  C.up(hC); c.up(std::vector<float>(c.n, 0.f)); x0.up(hx); u0.up(std::vector<float>(u0.n, 0.f));
+  net.params = prm.p;
+  mpcb200_dims d = {B, T, n, m, T - 1, 0, 0, 0, 0, 10, 20, 1, 0};
+  mpcb200_params pr = {0.0, 0.0, 0.0, 0.2, {}};
+  mpcb200_ilqr_opts opts = {5, 5, m, 0, 1e-7, 1e-4};
+  const size_t fw = mpcb200_episode_mlp_workspace_bytes(&d, &opts, &net, 4);
+  const size_t bw = mpcb200_episode_backward_mlp_workspace_bytes(&d, &net, nullptr, 4);
+  if (fw == 0 || bw == 0) return printf("episode mlp workspace %zu / %zu\n", fw, bw), 1;
+  Dev<float> ws((fw > bw ? fw : bw) / sizeof(float) + 64);
+  int rc = mpcb200_episode_mlp_f32(&d, &pr, &opts, &net, nullptr, steps, C.p, c.p, nullptr, nullptr, nullptr, x0.p,
+                                   u0.p, nullptr, nullptr, nullptr, xs.p, us.p, costs.p, (int32_t*)info.p, un.p, px.p,
+                                   pu.p, ws.p, fw, nullptr);
+  if (rc != 0 || cudaDeviceSynchronize() != cudaSuccess) return printf("episode mlp rc=%d\n", rc), 1;
+  int bad = 0;
+  const auto gx = xs.down(), gu = us.down();
+  for (int i = 0; i < (steps + 1) * B * n; ++i) bad += gx[i] != hx[i % (B * n)];
+  for (float v : gu) bad += v != 0.f;
+  Dev<float> gxs((steps + 1) * B * n), gus(steps * B * m), dx(B * n), dC(T * B * p * p), dc(T * B * p), dth(np);
+  gxs.up(std::vector<float>(gxs.n, 0.f)); gus.up(std::vector<float>(gus.n, 0.f));
+  rc = mpcb200_episode_backward_mlp_f32(&d, &pr, &net, nullptr, steps, C.p, c.p, nullptr, nullptr, nullptr, xs.p, us.p,
+                                        px.p, pu.p, gxs.p, gus.p, dx.p, dC.p, dc.p, dth.p, nullptr, nullptr, nullptr,
+                                        nullptr, ws.p, bw, nullptr);
+  if (rc != 0 || cudaDeviceSynchronize() != cudaSuccess) return printf("episode backward mlp rc=%d\n", rc), 1;
+  for (float v : dth.down()) bad += v != 0.f;
+  for (float v : dx.down()) bad += v != 0.f;
+  mpcb200_dims d2 = d;
+  d2.T = 2;
+  rc = mpcb200_episode_mlp_f32(&d2, &pr, &opts, &net, nullptr, steps, C.p, c.p, nullptr, nullptr, nullptr, x0.p, u0.p,
+                               nullptr, nullptr, nullptr, xs.p, us.p, costs.p, (int32_t*)info.p, un.p, nullptr,
+                               nullptr, ws.p, fw, nullptr);
+  bad += rc != MPCB200_ERR_BAD_DIMS;
+  mpcb200_mlp big = net;
+  big.n_layers = 3; big.width[1] = big.width[2] = 256; big.width[3] = n;
+  big.W_off[1] = 256 * p + 256; big.b_off[1] = big.W_off[1] + 256 * 256;
+  big.W_off[2] = big.b_off[1] + 256; big.b_off[2] = big.W_off[2] + 256 * n;
+  rc = mpcb200_episode_backward_mlp_f32(&d, &pr, &big, nullptr, steps, C.p, c.p, nullptr, nullptr, nullptr, xs.p, us.p,
+                                        px.p, pu.p, gxs.p, gus.p, dx.p, dC.p, dc.p, dth.p, nullptr, nullptr, nullptr,
+                                        nullptr, ws.p, bw, nullptr);
+  bad += rc != MPCB200_ERR_SMEM;
+  printf("episode mlp: x' = x held, zero gradients, %d bad; T < 3 and [256, 256] refused\n", bad);
+  return bad != 0;
+}
+
 int main() {
   int fails = 0;
   fails += run_mlp();
+  fails += run_episode_mlp();
   fails += run_episode_backward_slew();
   fails += run_episode_plant();
   fails += run_episode_window();
