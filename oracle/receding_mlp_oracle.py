@@ -5,7 +5,8 @@ episode(): for k: plan = mlp_oracle.ilqr(x_k, u_init = w_k); x_{k+1} = step(x_k,
 network (plant None) or a plant(x, u); w_{k+1} = lqr_oracle.shift_warm_start(plan_u).
 backward(): autograd's gradient of sum(dl_dxs * xs) + sum(dl_dus * us) for that loop, each solve contributing
 MPC.forward's differentiable tail at its plan (the adjoint on the network's linearisation, differentiated in the
-weights), the warm starts held constant: lqr_oracle.receding_horizon_backward's sweep with the network's parts."""
+weights), the warm starts held constant: lqr_oracle.receding_horizon_backward's sweep with the network's parts.
+backward() runs in the dtype of its inputs: float64 for the oracle, float32 for the yardstick of float32 kernels."""
 import torch
 
 from . import lqr_oracle as lo
@@ -46,7 +47,7 @@ def backward(n, m, T, C, c, layers, act, passthrough, xs, us, plan_x, plan_u, dl
     th = theta.detach().clone().requires_grad_(True) if theta is not None else None
     dth = torch.zeros_like(th) if th is not None else None
     dC, dc = torch.zeros_like(C), torch.zeros_like(c)
-    dw = torch.zeros(n_steps, B, n, dtype=torch.float64)
+    dw = torch.zeros(n_steps, B, n, dtype=C.dtype)
     g = dl_dxs[n_steps].clone()
     for k in range(n_steps - 1, -1, -1):
         dw[k] = g
@@ -62,8 +63,8 @@ def backward(n, m, T, C, c, layers, act, passthrough, xs, us, plan_x, plan_u, dl
             if th is not None:
                 dth += gs[2]
         Fk, fk = mo.linearize(layers, act, passthrough, plan_x[k], plan_u[k])
-        dl_dx = torch.zeros(T, B, n, dtype=torch.float64)
-        dl_du = torch.zeros(T, B, m, dtype=torch.float64)
+        dl_dx = torch.zeros(T, B, n, dtype=C.dtype)
+        dl_du = torch.zeros(T, B, m, dtype=C.dtype)
         dl_du[0] = dl_dus[k] + gu
         dxk, dCk, dck, dFk, dfk, _, _ = lo.lqr_step_backward(n, m, T, plan_x[k][0], C, c, Fk, fk, plan_x[k],
                                                              plan_u[k], dl_dx, dl_du, u_lower=u_lower,
