@@ -126,7 +126,7 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plan
                 if ep is not None:
                     return ep
             if episode_on_device(ctrl, x_init, cost, dx, w0, plant, time_varying, differentiable=True):
-                ep = _episode_net_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+                ep = _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
                 if ep is not None:
                     return ep
             return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
@@ -136,7 +136,7 @@ def receding_horizon(ctrl, x_init, cost, dx, n_steps, differentiable=False, plan
             if ep is not None:
                 return ep
         if episode_on_device(ctrl, x_init, cost, dx, w0, plant, time_varying):
-            ep = _episode_net(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
+            ep = _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance)
             if ep is not None:
                 return ep
         return _episode_host(ctrl, x_init, cost, dx, n_steps, w0, plant, disturbance, L)
@@ -281,24 +281,41 @@ def _first_warm_start(ctrl, x_init):
     return u.to(dtype=x_init.dtype, device=x_init.device)
 
 
-def _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None, L=None):
-    """The episode as one library call (step.episode_raw) on the problem MPC._ilqr_device stages, once; None when the
-    driver refused the graph (nothing ran then).  L: a time-varying episode's axis (episode_raw's window)."""
-    from . import step as _step
+def _dyn_inputs(d):
+    """(F, f, params) of a model or plant, the inputs a differentiable episode takes its gradients in: a LinDx's F and
+    f, another Module's ``params`` (None without them); all None for None."""
+    if isinstance(d, LinDx):
+        return d.F, d.f, None
+    return None, None, getattr(d, "params", None)
+
+
+def _run_episode(ctrl, x_init, C, c, dx, n_steps, w0, plant, F_p, f_p, w, L=None, keep_plans=False):
+    """The episode as one library call on the problem MPC._device_problem stages, once: mlp.episode_raw for a learned
+    model, else step.episode_raw; None when the driver refused the graph (nothing ran then).  F_p, f_p: a LinDx
+    plant's; L: a time-varying episode's axis (episode_raw's window)."""
+    from . import mlp, step
     T, m = ctrl.T, ctrl.n_ctrl
-    n, x0, C, c, F, f, dyn = ctrl._device_problem(x_init, cost, dx, T=L)
+    n, x0, C_, c_, F_, f_, dyn = ctrl._device_problem(x_init, QuadCost(C, c), dx, T=L)
+    if dyn is not None and dyn[0] == "mlp":
+        return mlp.episode_raw(dx, n, m, T, n_steps, x0, C_, c_, w0, keep_plans=keep_plans, w=w,
+                               plant=_net_plant_spec(ctrl, x_init, C, dx, plant, F_p, f_p), **ctrl._device_options())
     kw = {}
     if plant is not None:
-        F_p, f_p = (plant.F, plant.f) if isinstance(plant, LinDx) else (None, None)
-        kw = dict(plant=_plant_spec(ctrl, x_init, cost.C, plant, F_p, f_p, whole=L is not None),
-                  w=_staged_w(ctrl, w))
-    res = _step.episode_raw(n, m, T, n_steps, x0, C, c, F, f, w0, dyn=dyn, window=L, **kw,
+        kw = dict(plant=_plant_spec(ctrl, x_init, C, plant, F_p, f_p, whole=L is not None), w=_staged_w(ctrl, w))
+    return step.episode_raw(n, m, T, n_steps, x0, C_, c_, F_, f_, w0, dyn=dyn, keep_plans=keep_plans,
+                            n_prev=m if ctrl.slew_rate_penalty is not None else 0, window=L, **kw,
                             **ctrl._device_options())
+
+
+def _episode_device(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None, L=None):
+    """The episode as one library call (_run_episode); None when the driver refused the graph (nothing ran then)."""
+    F_p, f_p, _ = _dyn_inputs(plant)
+    res = _run_episode(ctrl, x_init, cost.C, cost.c, dx, n_steps, w0, plant, F_p, f_p, w, L)
     if res is None:
         solver._graph_cond_unavailable = True
         return None
     ctrl._print_pnqp_warnings(res["info"][:, 1].sum())      # the one host read, and only when they are printed
-    x = res["x"][:, :, m:] if ctrl.slew_rate_penalty is not None else res["x"]
+    x = res["x"][:, :, ctrl.n_ctrl:] if ctrl.slew_rate_penalty is not None else res["x"]
     return Episode(x, res["u"], res["costs"], res["info"], res["u_next"])
 
 
@@ -306,70 +323,93 @@ class _NoGraph(Exception):
     """The driver refused the episode's graph (nothing ran)."""
 
 
+def _keep_for_backward(ctx, ctrl, res, F_p, f_p, plant_params, whole, *weights):
+    """What a differentiable episode's backward reads, from the forward's res: every tensor (xs, us, the plans, the
+    staged C, c, F, f, bounds and plant, `weights`) through save_for_backward, so an in-place edit before the backward
+    raises and the outputs do not keep themselves alive through ctx; ctx holds only the staged problem's metadata and
+    that of the plant's inputs.  The pnqp warnings are printed here, once."""
+    ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
+    s, ctx.n_steps, xs, us, plan_x, plan_u = res["saved"]
+    sp = s.plant
+    ctx.save_for_backward(xs, us, plan_x, plan_u, s.C, s.c, s.F, s.f, s.u_lower, s.u_upper,
+                          sp.F if sp is not None else None, sp.f if sp is not None else None, *weights)
+    ctx.problem = s._replace(C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None,
+                             plant=sp._replace(F=None, f=None) if sp is not None else None)
+    ctx.plant_meta = (F_p.shape if F_p is not None else None, f_p.shape if f_p is not None else None,
+                      (plant_params.dtype, plant_params.device) if plant_params is not None else None, whole)
+    ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
+
+
+def _saved_for_backward(ctx, dl_dx, dl_du):
+    """(saved as the backward raw call takes it, dl_dx, dl_du, weights) from _keep_for_backward's ctx: a missing
+    gradient is zeros, and under a slew-rate penalty dl_dx gets zeros in front for the previous control's states."""
+    xs, us, plan_x, plan_u, C, c, F, f, lo, hi, Fp, fp, *weights = ctx.saved_tensors    # raises after an in-place edit
+    s = ctx.problem._replace(C=C, c=c, F=F, f=f, u_lower=lo, u_upper=hi)
+    if s.plant is not None:
+        s = s._replace(plant=s.plant._replace(F=Fp, f=fp))
+    n_steps, k = ctx.n_steps, s.n_prev
+    if dl_dx is None:
+        dl_dx = xs.new_zeros(n_steps + 1, s.dims.B, s.pad.n)
+    elif k:                                   # the previous control's states: no gradient of their own
+        dl_dx = torch.cat((dl_dx.new_zeros(n_steps + 1, s.dims.B, k), dl_dx), 2)
+    if dl_du is None:
+        dl_du = us.new_zeros(n_steps, s.dims.B, s.pad.m)
+    return (s, n_steps, xs, us, plan_x, plan_u), dl_dx, dl_du, weights
+
+
+def _plant_grads(ctx, need, dF_p, df_p, dth_p):
+    """The plant's gradients as its inputs take them, where `need` (F_p, f_p, params) asks for them: a LinDx plant's
+    in slice 0 of F_p, f_p (whole in a time-varying episode, where slice k steps control step k), a known plant's
+    params summed over the batch."""
+    F_shape, f_shape, pp_meta, whole = ctx.plant_meta
+
+    def placed(g, shape):
+        if whole:
+            return g
+        out = g.new_zeros(shape)
+        out[0] = g
+        return out
+    dFp = placed(dF_p, F_shape) if dF_p is not None and need[0] else None
+    dfp = placed(df_p, f_shape) if df_p is not None and need[1] else None
+    dpp = dth_p.sum(0).to(dtype=pp_meta[0], device=pp_meta[1]) if dth_p is not None and need[2] else None
+    return dFp, dfp, dpp
+
+
 class EpisodeFn(torch.autograd.Function):
     """(x, u, costs, info, u_next) of a differentiable device episode: the forward is step.episode_raw with
     keep_plans, the backward one step.episode_backward_raw call.  One module-level Function (DESIGN.md section 3.2).
-    `o` = (ctrl, dx, n_steps, w0, plant); the known system's parameter values are the host numbers the forward took
+    `o` = (ctrl, dx, n_steps, w0, plant, L); the known system's parameter values are the host numbers the forward took
     (params_scope) and the backward reuses them.  Under a slew-rate penalty the staged problem is the augmented one
     over [u_{k-1}; x] (MPC._device_problem): x is returned without its first m states, the backward pads dl_dx with
     m zeros in front, the sweep detaches those states (n_prev = m), and the gradients are cropped to the blocks of
-    x_init, C, c, F and f inside the augmented ones (prev_ctrl and the warm starts get none).  Every tensor the
-    backward reads (xs, us, the plans, the staged C, c,
-    F, f and bounds) goes through save_for_backward, so an in-place edit of x or u before the backward raises, and the
-    outputs do not keep themselves alive through ctx; ctx holds only the staged problem's metadata.  First order only:
-    the backward is raw kernels.  `o[4]` a plant (receding_horizon's `plant`), or None: F_p, f_p (a LinDx plant's),
-    plant_params (a known plant's) and w are then inputs too, the staged plant's F, f go through save_for_backward,
-    and their gradients come from the plant sweep (step.episode_backward_raw), F_p's and f_p's in slice 0.  `o[5]`
-    a time-varying episode's axis L, or None: C, c, F, f, bounds and a LinDx plant's F_p, f_p are full length, and so
-    are their gradients."""
+    x_init, C, c, F and f inside the augmented ones (prev_ctrl and the warm starts get none).  The backward reads
+    only what _keep_for_backward kept.  First order only: the backward is raw kernels.  `o[4]` a plant
+    (receding_horizon's `plant`), or None: F_p, f_p (a LinDx plant's), plant_params (a known plant's) and w are then
+    inputs too, and their gradients come from the plant sweep (step.episode_backward_raw), F_p's and f_p's in slice
+    0 (_plant_grads).  `o[5]` a time-varying episode's axis L, or None: C, c, F, f, bounds and a LinDx plant's F_p,
+    f_p are full length, and so are their gradients."""
 
     @staticmethod
     def forward(ctx, o, x_init, C, c, F, f, params, F_p=None, f_p=None, plant_params=None, w=None):
-        from . import step as _step
         ctrl, dx, n_steps, w0, plant, L = o
-        T, m = ctrl.T, ctrl.n_ctrl
-        n, x0, C_, c_, F_, f_, dyn = ctrl._device_problem(x_init, QuadCost(C, c), dx, T=L)
-        slew = ctrl.slew_rate_penalty is not None
-        kw = {}
-        if plant is not None:
-            kw = dict(plant=_plant_spec(ctrl, x_init, C, plant, F_p, f_p, whole=L is not None), w=_staged_w(ctrl, w))
-        res = _step.episode_raw(n, m, T, n_steps, x0, C_, c_, F_, f_, w0, dyn=dyn, keep_plans=True,
-                                n_prev=m if slew else 0, window=L, **kw, **ctrl._device_options())
+        res = _run_episode(ctrl, x_init, C, c, dx, n_steps, w0, plant, F_p, f_p, w, L, keep_plans=True)
         if res is None:
             raise _NoGraph()
-        ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
-        s, ctx.n_steps, xs, us, plan_x, plan_u = res["saved"]
-        sp = s.plant
-        ctx.save_for_backward(xs, us, plan_x, plan_u, s.C, s.c, s.F, s.f, s.u_lower, s.u_upper,
-                              sp.F if sp is not None else None, sp.f if sp is not None else None)
-        ctx.problem = s._replace(C=None, c=None, F=None, f=None, u_lower=None, u_upper=None, u_zero_I=None,
-                                 plant=sp._replace(F=None, f=None) if sp is not None else None)
+        _keep_for_backward(ctx, ctrl, res, F_p, f_p, plant_params, L is not None)
         ctx.p_meta = (params.dtype, params.device) if params is not None else None
-        ctx.plant_meta = (F_p.shape if F_p is not None else None, f_p.shape if f_p is not None else None,
-                          (plant_params.dtype, plant_params.device) if plant_params is not None else None)
-        ctx.whole = L is not None
-        ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
-        x = res["x"][:, :, m:] if slew else res["x"]
+        m = ctrl.n_ctrl
+        x = res["x"][:, :, m:] if ctrl.slew_rate_penalty is not None else res["x"]
         return x, res["u"], res["costs"], res["info"], res["u_next"]
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dl_dx, dl_du, *_):
         from . import step as _step
-        xs, us, plan_x, plan_u, C, c, F, f, lo, hi, Fp, fp = ctx.saved_tensors
-        s = ctx.problem._replace(C=C, c=c, F=F, f=f, u_lower=lo, u_upper=hi)
-        if s.plant is not None:
-            s = s._replace(plant=s.plant._replace(F=Fp, f=fp))
-        n_steps, k = ctx.n_steps, s.n_prev
-        if dl_dx is None:
-            dl_dx = xs.new_zeros(n_steps + 1, s.dims.B, s.pad.n)
-        elif k:                                   # the previous control's states: no gradient of their own
-            dl_dx = torch.cat((dl_dx.new_zeros(n_steps + 1, s.dims.B, k), dl_dx), 2)
-        if dl_du is None:
-            dl_du = us.new_zeros(n_steps, s.dims.B, s.pad.m)
-        out = _step.episode_backward_raw((s, n_steps, xs, us, plan_x, plan_u), dl_dx, dl_du)
+        saved, dl_dx, dl_du, _ = _saved_for_backward(ctx, dl_dx, dl_du)
+        out = _step.episode_backward_raw(saved, dl_dx, dl_du)
         dx_init, dC, dc, dF, df, dtheta = out[:6]
-        dF_p, df_p, dth_p, dw = out[6:] if s.plant is not None else (None, None, None, None)
+        dF_p, df_p, dth_p, dw = out[6:] if len(out) > 6 else (None, None, None, None)
+        k = saved[0].n_prev
         if k:                                     # the blocks of x_init, C, c, F, f inside the augmented problem
             dx_init, dC, dc = dx_init[:, k:], dC[..., k:, k:], dc[..., k:]
             dF = dF[..., k:, k:] if dF is not None else None
@@ -378,47 +418,12 @@ class EpisodeFn(torch.autograd.Function):
             df_p = df_p[..., k:] if df_p is not None else None
             dw = dw[..., k:] if dw is not None else None
         need = ctx.needs_input_grad
-        dparams = dFp = dfp = dpp = None
+        dparams = None
         if dtheta is not None and need[6]:
             dparams = dtheta.sum(0).to(dtype=ctx.p_meta[0], device=ctx.p_meta[1])
-        F_shape, f_shape, pp_meta = ctx.plant_meta
-        if dF_p is not None and need[7]:          # the plant steps with its slice 0 (time-varying: slice k)
-            dFp = dF_p if ctx.whole else dF_p.new_zeros(F_shape)
-            if not ctx.whole:
-                dFp[0] = dF_p
-        if df_p is not None and need[8]:
-            dfp = df_p if ctx.whole else df_p.new_zeros(f_shape)
-            if not ctx.whole:
-                dfp[0] = df_p
-        if dth_p is not None and need[9]:
-            dpp = dth_p.sum(0).to(dtype=pp_meta[0], device=pp_meta[1])
         return (None, dx_init if need[1] else None, dC if need[2] else None, dc if need[3] else None,
-                dF if need[4] else None, df if need[5] else None, dparams if need[6] else None, dFp, dfp, dpp,
-                dw if dw is not None and need[10] else None)
-
-
-def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None, L=None):
-    """The differentiable episode on the device path (EpisodeFn); None when the driver refused the graph."""
-    F, f, params = None, None, None
-    if isinstance(dx, LinDx):
-        F, f = dx.F, dx.f
-    else:
-        params = getattr(dx, "params", None)
-    extra = ()
-    if plant is not None:
-        F_p = f_p = p_params = None
-        if isinstance(plant, LinDx):
-            F_p, f_p = plant.F, plant.f
-        else:
-            p_params = getattr(plant, "params", None)
-        extra = (F_p, f_p, p_params, w)
-    try:
-        x, u, costs, info, u_next = EpisodeFn.apply((ctrl, dx, n_steps, w0, plant, L), x_init, cost.C, cost.c, F,
-                                                    f, params, *extra)
-    except _NoGraph:
-        solver._graph_cond_unavailable = True
-        return None
-    return Episode(x, u, costs, info, u_next)
+                dF if need[4] else None, df if need[5] else None, dparams,
+                *_plant_grads(ctx, need[7:10], dF_p, df_p, dth_p), dw if dw is not None and need[10] else None)
 
 
 def _net_plant_spec(ctrl, x_init, C, dx, plant, F_p=None, f_p=None):
@@ -429,107 +434,57 @@ def _net_plant_spec(ctrl, x_init, C, dx, plant, F_p=None, f_p=None):
     return _plant_spec(ctrl, x_init, C, plant, F_p, f_p)
 
 
-def _episode_net(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
-    """The episode planned with a learned model as one library call (mlp.episode_raw) on the problem
-    MPC._ilqr_device stages; None when the driver refused the graph (nothing ran then)."""
-    from .mlp import episode_raw
-    T, m = ctrl.T, ctrl.n_ctrl
-    n, x0, C, c, _, _, _ = ctrl._device_problem(x_init, cost, dx)
-    F_p, f_p = (plant.F, plant.f) if isinstance(plant, LinDx) else (None, None)
-    res = episode_raw(dx, n, m, T, n_steps, x0, C, c, w0, plant=_net_plant_spec(ctrl, x_init, C, dx, plant, F_p, f_p),
-                      w=w, **ctrl._device_options())
-    if res is None:
-        solver._graph_cond_unavailable = True
-        return None
-    ctrl._print_pnqp_warnings(res["info"][:, 1].sum())      # the one host read, and only when they are printed
-    return Episode(res["x"], res["u"], res["costs"], res["info"], res["u_next"])
-
-
 class NetEpisodeFn(torch.autograd.Function):
     """(x, u, costs, info, u_next) of a differentiable episode planned with a learned model: the forward is
     mlp.episode_raw with keep_plans, the backward one mlp.episode_backward_raw call.  One module-level Function
     (DESIGN.md section 3.2).  `o` = (ctrl, dx, n_steps, w0, plant).  The inputs after o are x_init, C, c, a LinDx
     plant's F_p and f_p, a known plant's params, w, and the network's weights and biases in _layout's order W0 b0 W1
     b1 ...; dtheta of the sweep is split into views shaped like them.  The weights, like every tensor the backward
-    reads (xs, us, the plans, the staged C, c, bounds and plant), go through save_for_backward, so an in-place edit of
-    a weight before the backward raises; ctx holds the staged problem's metadata, the packed weights the forward ran
-    with and the Module.  First order only: the backward is raw kernels.  costs, info and u_next carry no gradient."""
+    reads, go through save_for_backward (_keep_for_backward), so an in-place edit of a weight before the backward
+    raises; the staged problem holds the packed weights the forward ran with.  First order only: the backward is raw
+    kernels.  costs, info and u_next carry no gradient."""
 
     @staticmethod
     def forward(ctx, o, x_init, C, c, F_p, f_p, plant_params, w, *weights):
-        from .mlp import episode_raw
         ctrl, dx, n_steps, w0, plant = o
-        T, m = ctrl.T, ctrl.n_ctrl
-        n, x0, C_, c_, _, _, _ = ctrl._device_problem(x_init, QuadCost(C, c), dx)
-        res = episode_raw(dx, n, m, T, n_steps, x0, C_, c_, w0,
-                          plant=_net_plant_spec(ctrl, x_init, C, dx, plant, F_p, f_p), w=w, keep_plans=True,
-                          **ctrl._device_options())
+        res = _run_episode(ctrl, x_init, C, c, dx, n_steps, w0, plant, F_p, f_p, w, keep_plans=True)
         if res is None:
             raise _NoGraph()
-        ctrl._print_pnqp_warnings(res["info"][:, 1].sum())
-        s, _, xs, us, plan_x, plan_u, _, rec, buf, disturbed = res["saved"]
-        sp = s.plant
-        ctx.save_for_backward(xs, us, plan_x, plan_u, s.C, s.c, s.u_lower, s.u_upper,
-                              sp.F if sp is not None else None, sp.f if sp is not None else None, *weights)
-        ctx.problem = s._replace(C=None, c=None, u_lower=None, u_upper=None, u_zero_I=None,
-                                 plant=sp._replace(F=None, f=None) if sp is not None else None)
-        ctx.net = (n_steps, dx, rec, buf, disturbed)
-        ctx.plant_meta = (F_p.shape if F_p is not None else None, f_p.shape if f_p is not None else None,
-                          (plant_params.dtype, plant_params.device) if plant_params is not None else None)
-        ctx.mark_non_differentiable(res["costs"], res["info"], res["u_next"])
+        _keep_for_backward(ctx, ctrl, res, F_p, f_p, plant_params, False, *weights)
         return res["x"], res["u"], res["costs"], res["info"], res["u_next"]
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dl_dx, dl_du, *_):
         from .mlp import episode_backward_raw
-        xs, us, plan_x, plan_u, C, c, lo, hi, Fp, fp, *weights = ctx.saved_tensors    # raises after an in-place edit
-        s = ctx.problem._replace(C=C, c=c, u_lower=lo, u_upper=hi)
-        if s.plant is not None:
-            s = s._replace(plant=s.plant._replace(F=Fp, f=fp))
-        n_steps, dx, rec, buf, disturbed = ctx.net
-        B, n, m = s.dims.B, s.pad.n, s.pad.m
-        if dl_dx is None:
-            dl_dx = xs.new_zeros(n_steps + 1, B, n)
-        if dl_du is None:
-            dl_du = us.new_zeros(n_steps, B, m)
-        dx_init, dC, dc, dtheta, dF_p, df_p, dth_p, dw = episode_backward_raw(
-            (s, n_steps, xs, us, plan_x, plan_u, dx, rec, buf, disturbed), dl_dx, dl_du)
+        saved, dl_dx, dl_du, weights = _saved_for_backward(ctx, dl_dx, dl_du)
+        dx_init, dC, dc, dtheta, dF_p, df_p, dth_p, dw = episode_backward_raw(saved, dl_dx, dl_du)
         need = ctx.needs_input_grad
-        F_shape, f_shape, pp_meta = ctx.plant_meta
-        dFp = dfp = dpp = None
-        if dF_p is not None and need[4]:          # the plant steps with its slice 0
-            dFp = dF_p.new_zeros(F_shape)
-            dFp[0] = dF_p
-        if df_p is not None and need[5]:
-            dfp = df_p.new_zeros(f_shape)
-            dfp[0] = df_p
-        if dth_p is not None and need[6]:
-            dpp = dth_p.sum(0).to(dtype=pp_meta[0], device=pp_meta[1])
         dweights, o = [], 0
         for p, want in zip(weights, need[8:]):
             dweights.append(dtheta[o:o + p.numel()].view(p.shape) if want else None)
             o += p.numel()
-        return (None, dx_init if need[1] else None, dC if need[2] else None, dc if need[3] else None, dFp, dfp, dpp,
-                dw if dw is not None and need[7] else None, *dweights)
+        return (None, dx_init if need[1] else None, dC if need[2] else None, dc if need[3] else None,
+                *_plant_grads(ctx, need[4:7], dF_p, df_p, dth_p), dw if dw is not None and need[7] else None,
+                *dweights)
 
 
-def _episode_net_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None):
-    """The differentiable episode planned with a learned model (NetEpisodeFn); None when the driver refused the
-    graph."""
-    F_p = f_p = p_params = None
-    if isinstance(plant, LinDx):
-        F_p, f_p = plant.F, plant.f
-    elif plant is not None and plant is not dx:
-        p_params = getattr(plant, "params", None)
-    weights = [t for fc in dx.fcs for t in (fc.weight, fc.bias)]
+def _episode_device_grad(ctrl, x_init, cost, dx, n_steps, w0, plant=None, w=None, L=None):
+    """The differentiable episode on the device (NetEpisodeFn for a learned model, else EpisodeFn); None when the
+    driver refused the graph."""
+    from .models import NNDynamics
+    plant_in = _dyn_inputs(plant) + (w,)
     try:
-        x, u, costs, info, u_next = NetEpisodeFn.apply((ctrl, dx, n_steps, w0, plant), x_init, cost.C, cost.c, F_p,
-                                                       f_p, p_params, w, *weights)
+        if type(dx) is NNDynamics:
+            weights = [t for fc in dx.fcs for t in (fc.weight, fc.bias)]
+            out = NetEpisodeFn.apply((ctrl, dx, n_steps, w0, plant), x_init, cost.C, cost.c, *plant_in, *weights)
+        else:
+            out = EpisodeFn.apply((ctrl, dx, n_steps, w0, plant, L), x_init, cost.C, cost.c, *_dyn_inputs(dx),
+                                  *plant_in)
     except _NoGraph:
         solver._graph_cond_unavailable = True
         return None
-    return Episode(x, u, costs, info, u_next)
+    return Episode(*out)
 
 
 def _episode_host(ctrl, x_init, cost, dx, n_steps, w, plant=None, dist=None, L=None):

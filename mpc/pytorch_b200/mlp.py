@@ -354,57 +354,14 @@ def episode_raw(dx, n_state, n_ctrl, T, n_steps, x_init, C, c, u_init, u_lower=N
     x_{k+1} = rollout_raw(dx, 2, x_k, plan_u[:2])[1] (+ w_k).  plant: (kind, params, F_p, f_p) as step.episode_raw
     takes it (a LinDx's slice 0, or a known system), or None; w [n_steps, B, n] or None.  The weights are packed once
     (record, within the caller's params_scope).  Returns step.episode_raw's dict; keep_plans adds "saved", what
-    episode_backward_raw takes.  None when the driver has no conditional graph nodes (nothing was launched then)."""
-    from .step import _dense, _problem, _stage_plant, _validate
-    n, m = n_state, n_ctrl
-    if T < 3 or n_steps < 1:
-        raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
-    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
-                  bounds=(u_lower, u_upper), u_zero_I=u_zero_I, need_F=False)
-    dtype, dev = C.dtype, C.device
-    s = _problem(n, m, T, B, dtype, dev, C, c, None, None, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
-                 max_linesearch_iter)
-    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
-    rec, buf = record(dx, C)
-    x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
-    sp = _stage_plant(pad, plant, dtype, B, n, m) if plant is not None else None
-    w_ = None
-    if w is not None:
-        if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
-            raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
-                               f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
-        w_ = pad.vec_n(_dense(w, dtype)).contiguous()
-    opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
-                         best_cost_eps=float(best_cost_eps))
-    nbytes = _lib.lib().mpcb200_episode_mlp_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), ctypes.byref(rec),
-                                                            C.element_size())
-    if nbytes == 0:
-        raise MpcB200Error("mpcb200_episode_mlp: the episode has no workspace size (the network does not fit, or bad "
-                           "dimensions)")
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    xs = torch.empty(n_steps + 1, B, N, dtype=dtype, device=dev)
-    us = torch.empty(n_steps, B, M, dtype=dtype, device=dev)
-    costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
-    info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
-    u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
-    plan_x = plan_u = None
-    if keep_plans:
-        plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
-        plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
-    fn = _lib.entry("mpcb200_episode_mlp", dtype)
-    with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), ctypes.byref(rec),
-                ctypes.byref(sp.rec) if sp is not None else None, int(n_steps), ptr_view(s.C), ptr_view(s.c),
-                ptr(sp.F if sp is not None else None), ptr(sp.f if sp is not None else None), ptr(w_), ptr(x0_),
-                ptr(u0_), ptr(s.u_lower), ptr(s.u_upper), ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info),
-                ptr(u_next), ptr(plan_x), ptr(plan_u), ptr(ws), nbytes, stream_handle(dev))
-    if rc == _lib.ERR_NO_GRAPH_COND:
-        return None
-    check(rc, "mpcb200_episode_mlp")
-    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
-    if keep_plans:
-        res["saved"] = (s._replace(plant=sp), n_steps, xs, us, plan_x, plan_u, dx, rec, buf, w is not None)
-    return res
+    episode_backward_raw takes.  None when the driver has no conditional graph nodes (nothing was launched then).
+    step._stage_episode stages the call."""
+    from .step import _call, _episode_result, _stage_episode
+    s, name, args, out = _stage_episode(n_state, n_ctrl, T, n_steps, x_init, C, c, None, None, u_init, u_lower, u_upper,
+                                        u_zero_I, delta_u, linesearch_decay, max_linesearch_iter, lqr_iter,
+                                        not_improved_lim, eps, best_cost_eps, keep_plans=keep_plans, plant=plant, w=w,
+                                        net=dx)
+    return _episode_result(_call(name, C.dtype, C.device, args), name, s, out)
 
 
 def episode_backward_raw(saved, dl_dxs, dl_dus):
@@ -413,39 +370,9 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
     [n_steps, B, m] the gradients of its x and u.  Returns (dx_init [B, n], dC [T, B, p, p], dc [T, B, p], dtheta
     [n_params], dF_p [B, n, p], df_p [B, n], dtheta_p [B, NP_plant], dw [n_steps, B, n]): dtheta is the network's
     packed W0 b0 W1 b1 ... (_layout); the plant's outputs are None where the episode had no such plant (or no f), dw
-    None where it added no w."""
-    from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, DYN_NPARAMS
-    from .step import _dense
-    s, n_steps, xs, us, plan_x, plan_u, dx, rec, buf, disturbed = saved
-    pad, dims = s.pad, s.dims
-    T, B, N, M = dims.T, dims.B, pad.N, pad.M
-    P = N + M
-    dtype, dev = xs.dtype, xs.device
-    gx_, gu_ = pad.vec_n(_dense(dl_dxs, dtype)), pad.vec_m(_dense(dl_dus, dtype))
-    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
-    dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
-    dc = torch.empty(T, B, P, dtype=dtype, device=dev)
-    dtheta = torch.empty(buf.numel(), dtype=dtype, device=dev)
-    sp = s.plant
-    pk = sp.rec.kind if sp is not None else None
-    dF_p = torch.empty(B, N, P, dtype=dtype, device=dev) if pk == DYN_LINEAR else None
-    df_p = torch.empty(B, N, dtype=dtype, device=dev) if pk == DYN_LINEAR and sp.rec.has_f else None
-    dth_p = (torch.empty(B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
-             if sp is not None and pk != DYN_LINEAR else None)
-    dw = torch.empty(n_steps, B, N, dtype=dtype, device=dev) if disturbed else None
-    prec = ctypes.byref(sp.rec) if sp is not None else None
-    nbytes = _lib.lib().mpcb200_episode_backward_mlp_workspace_bytes(ctypes.byref(dims), ctypes.byref(rec), prec,
-                                                                     xs.element_size())
-    if nbytes == 0:
-        raise MpcB200Error("mpcb200_episode_backward_mlp: the episode has no workspace size (the network's VJP does "
-                           "not fit, or bad dimensions)")
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    fn = _lib.entry("mpcb200_episode_backward_mlp", dtype)
-    with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(rec), prec, int(n_steps), ptr_view(s.C),
-                ptr_view(s.c), ptr(sp.F if sp is not None else None), ptr(s.u_lower), ptr(s.u_upper), ptr(xs),
-                ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dtheta),
-                ptr(dF_p), ptr(df_p), ptr(dth_p), ptr(dw), ptr(ws), nbytes, stream_handle(dev))
-    check(rc, "mpcb200_episode_backward_mlp")
-    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), dtheta, pad.crop_np(dF_p), pad.crop_n(df_p),
-            dth_p, pad.crop_n(dw))
+    None where it added no w.  step._stage_episode_backward stages the call."""
+    from .step import _call, _episode_grads, _stage_episode_backward
+    name, args, out = _stage_episode_backward(saved, dl_dxs, dl_dus)
+    check(_call(name, saved[2].dtype, saved[2].device, args), name)
+    g = _episode_grads(saved[0], out)
+    return g[:3] + g[5:]

@@ -16,7 +16,7 @@ from torch.nn import Module
 
 from . import _lib
 from ._lib import Dims, Params, MpcB200Error, _on_device, check, ptr, ptr_view, stream_handle
-from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_DIMS, DYN_LINEAR, DYN_OWN_INSTANCE
+from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_DIMS, DYN_LINEAR, DYN_NPARAMS, DYN_OWN_INSTANCE
 
 PNQP_MAX_ITER = 20  # reference passes n_iter=20 (mpc/lqr_step.py:137)
 
@@ -259,18 +259,22 @@ class _Pad:
 # _StagedPlant of an episode closed on a plant other than the model (None: the model steps it)
 # window: the mpcb200_window record of a time-varying episode (episode_raw(..., window=L)), whose C, c, F, f and
 # bounds are then the staged full-length inputs (the solve's own where the record does not window them)
-_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev plant window",
-                                  defaults=(0, None, None))
+# net: (mpcb200_mlp record, packed weights) of an episode planned with a learned model (mlp.episode_raw); disturbed:
+# w was added to the network's own step (no plant: a staged plant records its own)
+_Problem = collections.namedtuple("_Problem", "pad C c F f u_lower u_upper u_zero_I dims params n_prev plant window "
+                                  "net disturbed", defaults=(0, None, None, None, False))
 # rec: the mpcb200_plant record; F, f: a LinDx plant's slice 0 at the problem's (padded) sizes [B, N, N+M], [B, N]
-# (f None without one); disturbed: the episode added w
+# (f None without one), or in a time-varying episode its whole staged F_p, f_p; disturbed: w was added to its step
 _StagedPlant = collections.namedtuple("_StagedPlant", "rec F f disturbed")
 
 
-def _stage_plant(pad, plant, dtype, B, n, m):
+def _stage_plant(pad, plant, dtype, B, n, m, win=None):
     """The plant of episode_raw as the kernels take it (_StagedPlant, without w): (DYN_LINEAR, None, F_p, f_p) with
     F_p [T', B, n, n+m] and f_p [T', B, n] (or None / empty) of which slice 0 steps, widened like the model (_Pad); or
     (kind, params, None, None) of a known system (its passthrough kind under a slew-rate penalty), whose own (n, m)
-    must be the staged instance's.  Checked on metadata before anything runs."""
+    must be the staged instance's.  `win`: the mpcb200_window record of a time-varying episode, whose LinDx plant has
+    F_p, f_p [L-1|L, B, ...] staged whole (slice k steps control step k; MPCB200_WIN_PLANT set in `win`).  Checked on
+    metadata before anything runs."""
     kind, params, F_p, f_p = plant
     rec = _lib.Plant(kind=int(kind))
     if kind != DYN_LINEAR:
@@ -280,11 +284,19 @@ def _stage_plant(pad, plant, dtype, B, n, m):
         for i, v in enumerate(params):
             rec.dyn[i] = float(v)
         return _StagedPlant(rec, None, None, False)
+    lead = "T'" if win is None else f"{win.L - 1} or {win.L}"
     for name, t, shape in (("plant F", F_p, (B, n, n + m)), ("plant f", f_p, (B, n))):
         if name == "plant F" and t is None:
             raise MpcB200Error("a LinDx plant needs F")
-        if not _is_empty(t) and (t.dim() != len(shape) + 1 or t.shape[0] < 1 or tuple(t.shape[1:]) != shape):
-            raise MpcB200Error(f"{name}: expected shape (T', {', '.join(map(str, shape))}), got {tuple(t.shape)}")
+        if not _is_empty(t) and (t.dim() != len(shape) + 1 or tuple(t.shape[1:]) != shape or
+                                 (t.shape[0] < 1 if win is None else t.shape[0] not in (win.L - 1, win.L))):
+            raise MpcB200Error(f"{name}: expected shape ({lead}, {', '.join(map(str, shape))}), got {tuple(t.shape)}")
+    if win is not None:
+        win.on |= _lib.WIN_PLANT
+        Fp, win.Fp_tstride = pad.stage(F_p, dtype, pad.mat_np)
+        fp, win.fp_tstride = pad.stage(f_p, dtype, pad.vec_n)
+        rec.has_f = int(fp is not None)
+        return _StagedPlant(rec, Fp, fp, False)
     F0 = _dense(F_p[:1], dtype)
     F0 = (pad.mat_np(F0) if pad.active else F0)[0].contiguous()
     f0 = None
@@ -464,80 +476,122 @@ def episode_raw(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower
     each step, x_{k+1} = plant(x_k, u_k) + w_k (under a slew-rate penalty its first n_prev entries are the caller's
     zeros).  Either one takes that entry; the staged problem records the plant for episode_backward_raw.
     window = L (mpcb200_episode_window_*): a time-varying episode whose inputs lie on its time axis of
-    L = n_steps + T - 1 slices (_episode_window)."""
-    n, m = n_state, n_ctrl
+    L = n_steps + T - 1 slices (_window_problem).  _stage_episode stages the call."""
+    s, name, args, out = _stage_episode(n_state, n_ctrl, T, n_steps, x_init, C, c, F, f, u_init, u_lower, u_upper,
+                                        u_zero_I, delta_u, linesearch_decay, max_linesearch_iter, lqr_iter,
+                                        not_improved_lim, eps, best_cost_eps, dyn=dyn, keep_plans=keep_plans,
+                                        n_prev=n_prev, plant=plant, w=w, window=window)
+    return _episode_result(_call(name, C.dtype, C.device, args), name, s, out)
+
+
+def _stage_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
+                   delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5,
+                   eps=1e-7, best_cost_eps=1e-4, dyn=None, keep_plans=False, n_prev=0, plant=None, w=None,
+                   window=None, net=None, alloc=None):
+    """An episode's call as episode_raw (or, with `net`, mlp.episode_raw) makes it, staged but not made: (s, name,
+    args, out).  s: the staged problem, which records n_prev, the plant, the window, the network and whether w was
+    added; name: the entry (mpcb200_episode, _plans with keep_plans, _plant with a plant or w, _window with `window`,
+    _mlp with `net`); args: its arguments in the header's order, a tensor standing for its device pointer (_call);
+    out: (xs, us, costs, info, u_next, plan_x, plan_u), plan_x, plan_u None without keep_plans.  Every buffer, the
+    workspace included, comes from alloc(shape, dtype) (default torch.empty on the inputs' device).
+    net: the NNDynamics (or CtrlPassthroughDynamics) every solve plans with, F = f = dyn = None; without a plant the
+    network steps the loop, and w is added to its step."""
     if T < 3 or n_steps < 1:
         raise MpcB200Error(f"an episode needs T >= 3 and n_steps >= 1, got T={T}, n_steps={n_steps}")
-    if window is not None:
-        return _episode_window(n, m, T, n_steps, window, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I,
-                               delta_u, linesearch_decay, max_linesearch_iter, dyn, keep_plans, n_prev, plant, w,
-                               _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m,
-                                             eps=float(eps), best_cost_eps=float(best_cost_eps)))
-    B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
-                  F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
-                  dyn_kind=dyn[0] if dyn is not None else None, need_F=dyn is None)
+    if window is None:
+        B = _validate(n, m, T, ("C", C, "TBpp"), ("c", c, "TBp"), ("x_init", x_init, "Bn"), ("u_init", u_init, "TBm"),
+                      F=F, f=f, bounds=(u_lower, u_upper), u_zero_I=u_zero_I,
+                      dyn_kind=dyn[0] if dyn is not None else None, need_F=dyn is None and net is None)
+        s = _problem(n, m, T, B, C.dtype, C.device, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+                     max_linesearch_iter, dyn)
+    else:
+        s = _window_problem(n, m, T, n_steps, window, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I, delta_u,
+                            linesearch_decay, max_linesearch_iter, dyn)
+    pad, dims, N, M, B = s.pad, s.dims, s.pad.N, s.pad.M, s.dims.B
     dtype, dev = C.dtype, C.device
-    s = _problem(n, m, T, B, dtype, dev, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
-                 max_linesearch_iter, dyn)
-    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    if net is not None:
+        from .mlp import record
+        net = record(net, C)
     x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
-    sp = w_ = None
-    if plant is not None or w is not None:
-        if plant is None:                 # the model steps, disturbed
-            plant = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
-        sp = _stage_plant(pad, plant, dtype, B, n, m)
-        if w is not None:
-            if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
-                raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
-                                   f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
-            w_ = pad.vec_n(_dense(w, dtype)).contiguous()
+    if plant is None and w is not None and net is None:      # the model steps, disturbed
+        plant = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
+    sp = _stage_plant(pad, plant, dtype, B, n, m, s.window) if plant is not None else None
+    w_ = None
+    if w is not None:
+        if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
+            raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
+                               f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
+        w_ = pad.vec_n(_dense(w, dtype)).contiguous()
+        if sp is not None:
             sp = sp._replace(disturbed=True)
+    s = s._replace(n_prev=int(n_prev), plant=sp, net=net, disturbed=w is not None and sp is None)
     opts = _lib.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
                          best_cost_eps=float(best_cost_eps))
-    nbytes = _lib.lib().mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    xs = torch.empty(n_steps + 1, B, N, dtype=dtype, device=dev)
-    us = torch.empty(n_steps, B, M, dtype=dtype, device=dev)
-    costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
-    info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
-    u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
-    head = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), int(n_steps), ptr_view(s.C),
-            ptr_view(s.c), ptr_view(s.F), ptr_view(s.f)]
-    tail = [ptr(x0_), ptr(u0_), ptr(s.u_lower), ptr(s.u_upper), ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs),
-            ptr(info), ptr(u_next)]
-    name = "mpcb200_episode"
+    lib, esz = _lib.lib(), C.element_size()
+    prec = ctypes.byref(sp.rec) if sp is not None else None
+    if net is not None:
+        name, recs = "mpcb200_episode_mlp", [ctypes.byref(net[0]), prec]
+        nbytes = lib.mpcb200_episode_mlp_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), recs[0], esz)
+        if nbytes == 0:
+            raise MpcB200Error("mpcb200_episode_mlp: the episode has no workspace size (the network does not fit, or "
+                               "bad dimensions)")
+    elif s.window is not None:
+        name, recs = "mpcb200_episode_window", [ctypes.byref(s.window), prec]
+        nbytes = lib.mpcb200_episode_window_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), recs[0], esz)
+    else:
+        name = ("mpcb200_episode_plant" if sp is not None else
+                "mpcb200_episode_plans" if keep_plans else "mpcb200_episode")
+        recs = [prec] if sp is not None else []
+        nbytes = lib.mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), esz)
+    if alloc is None:
+        def alloc(shape, dt):
+            return torch.empty(shape, dtype=dt, device=dev)
+    ws = alloc((nbytes,), torch.uint8)
+    xs, us = alloc((n_steps + 1, B, N), dtype), alloc((n_steps, B, M), dtype)
+    costs, info, u_next = alloc((n_steps, B), dtype), alloc((n_steps, 2), torch.int32), alloc((T, B, M), dtype)
     plan_x = plan_u = None
     if keep_plans:
-        name = "mpcb200_episode_plans"
-        plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
-        plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
-    if sp is not None:
-        name = "mpcb200_episode_plant"
-        args = head[:3] + [ctypes.byref(sp.rec)] + head[3:] + [ptr(sp.F), ptr(sp.f), ptr(w_)] + tail + \
-            [ptr(plan_x), ptr(plan_u)]
-    else:
-        args = head + tail + ([ptr(plan_x), ptr(plan_u)] if keep_plans else [])
+        plan_x, plan_u = alloc((n_steps, T, B, N), dtype), alloc((n_steps, T, B, M), dtype)
+    model = [s.C, s.c] if net is not None else [s.C, s.c, s.F, s.f]
+    plant_in = [] if not recs else [sp.F if sp is not None else None, sp.f if sp is not None else None, w_]
+    plans = [plan_x, plan_u] if name != "mpcb200_episode" else []
+    args = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), *recs, int(n_steps), *model, *plant_in,
+            x0_, u0_, s.u_lower, s.u_upper, s.u_zero_I, xs, us, costs, info, u_next, *plans, ws, nbytes,
+            stream_handle(dev)]
+    return s, name, args, (xs, us, costs, info, u_next, plan_x, plan_u)
+
+
+def _call(name, dtype, dev, args):
+    """The status of the library entry `name` for `dtype` called with `args` on `dev`, each tensor in `args` passed as
+    its device pointer (ptr_view: the staging made it dense, or validated its time stride)."""
     fn = _lib.entry(name, dtype)
     with _on_device(dev):
-        rc = fn(*args, ptr(ws), nbytes, stream_handle(dev))
+        return fn(*[ptr_view(a) if isinstance(a, torch.Tensor) else a for a in args])
+
+
+def _episode_result(rc, name, s, out):
+    """episode_raw's dict from the status of the call _stage_episode staged and its outputs; None when the driver has
+    no conditional graph nodes.  "saved" where the plans were kept."""
     if rc == _lib.ERR_NO_GRAPH_COND:
         return None
     check(rc, name)
+    xs, us, costs, info, u_next, plan_x, plan_u = out
+    pad = s.pad
     res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
-    if keep_plans:
-        res["saved"] = (s._replace(n_prev=int(n_prev), plant=sp), n_steps, xs, us, plan_x, plan_u)
+    if plan_x is not None:
+        res["saved"] = (s, us.shape[0], xs, us, plan_x, plan_u)
     return res
 
 
-def _episode_window(n, m, T, n_steps, L, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I, delta_u,
-                    linesearch_decay, max_linesearch_iter, dyn, keep_plans, n_prev, plant, w, opts):
-    """episode_raw on a time-varying problem (mpcb200_episode_window_*).  C [L, B, p, p], c [L, B, p], a LinDx
-    model's F [L-1|L, B, n, p] and f [L-1|L, B, n], tensor bounds [L, B, m] and a LinDx plant's F_p, f_p [L-1|L, ...]
-    lie on the episode's axis, L = n_steps + T - 1; u_init and u_zero_I are the solve's [T, B, m].  Solve k plans on
-    slices k .. k+T-1 (F: k .. k+F_T-1, F_T = T - (L - len(F))), and control step k steps with slice k of a LinDx
-    model or plant.  The per-solve problem is _problem's on the first window (its Dims, _Pad and widened u_zero_I);
-    the full-length inputs are staged once, by the same _Pad widening, and the library copies each window on the
-    device.  Same outputs as episode_raw; "saved" holds the staged full-length inputs and the window record."""
+def _window_problem(n, m, T, n_steps, L, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I, delta_u,
+                    linesearch_decay, max_linesearch_iter, dyn):
+    """The staged problem of a time-varying episode (episode_raw(..., window=L), mpcb200_episode_window_*).
+    C [L, B, p, p], c [L, B, p], a LinDx model's F [L-1|L, B, n, p] and f [L-1|L, B, n], tensor bounds [L, B, m] and a
+    LinDx plant's F_p, f_p [L-1|L, ...] lie on the episode's axis, L = n_steps + T - 1; u_init and u_zero_I are the
+    solve's [T, B, m].  Solve k plans on slices k .. k+T-1 (F: k .. k+F_T-1, F_T = T - (L - len(F))), and control
+    step k steps with slice k of a LinDx model or plant.  The per-solve problem is _problem's on the first window (its
+    Dims, _Pad and widened u_zero_I); the full-length inputs are staged once, by the same _Pad widening, into its C, c,
+    F, f and bounds, and the library copies each window on the device (the mpcb200_window record `window`)."""
     if L != n_steps + T - 1:
         raise MpcB200Error(f"window: a time-varying episode of {n_steps} steps at T={T} has an axis of "
                            f"{n_steps + T - 1} slices, got {L}")
@@ -553,7 +607,7 @@ def _episode_window(n, m, T, n_steps, L, x_init, C, c, F, f, u_init, u_lower, u_
         return b[:T] if isinstance(b, torch.Tensor) else b
     s = _problem(n, m, T, B, dtype, dev, C[:T], c[:T], F[:F_T] if F_T else None, None if _is_empty(f) else f[:T - 1],
                  first(u_lower), first(u_upper), u_zero_I, delta_u, linesearch_decay, max_linesearch_iter, dyn)
-    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
+    pad = s.pad
     rec = _lib.Window(L=int(L), on=_lib.WIN_COST)
     C_, rec.C_tstride = pad.stage(C, dtype, pad.mat_pp)
     c_, rec.c_tstride = pad.stage(c, dtype, pad.vec_p)
@@ -567,123 +621,7 @@ def _episode_window(n, m, T, n_steps, L, x_init, C, c, F, f, u_init, u_lower, u_
         rec.on |= _lib.WIN_BOUNDS
         _, _, _, lo_t, hi_t = _bounds(u_lower, u_upper, (L, B, m), dtype, dev, pad.active)
         lo_, hi_ = pad.vec_m(lo_t, -1.0).contiguous(), pad.vec_m(hi_t, 1.0).contiguous()
-    x0_, u0_ = pad.vec_n(_dense(x_init, dtype)), pad.vec_m(_dense(u_init, dtype))
-    sp = w_ = None
-    if plant is not None or w is not None:
-        if plant is None:                 # the model steps, disturbed
-            plant = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
-        sp = _stage_plant_window(pad, plant, dtype, B, n, m, L, rec)
-        if w is not None:
-            if tuple(w.shape) != (n_steps, B, n) or w.dtype != dtype or w.device != dev:
-                raise MpcB200Error(f"w: expected a {dtype} tensor of shape {(n_steps, B, n)} on {dev}, got a "
-                                   f"{w.dtype} tensor of shape {tuple(w.shape)} on {w.device}")
-            w_ = pad.vec_n(_dense(w, dtype)).contiguous()
-            sp = sp._replace(disturbed=True)
-    nbytes = _lib.lib().mpcb200_episode_window_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts),
-                                                               ctypes.byref(rec), C.element_size())
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    xs = torch.empty(n_steps + 1, B, N, dtype=dtype, device=dev)
-    us = torch.empty(n_steps, B, M, dtype=dtype, device=dev)
-    costs = torch.empty(n_steps, B, dtype=dtype, device=dev)
-    info = torch.empty(n_steps, 2, dtype=torch.int32, device=dev)
-    u_next = torch.empty(T, B, M, dtype=dtype, device=dev)
-    plan_x = plan_u = None
-    if keep_plans:
-        plan_x = torch.empty(n_steps, T, B, N, dtype=dtype, device=dev)
-        plan_u = torch.empty(n_steps, T, B, M, dtype=dtype, device=dev)
-    fn = _lib.entry("mpcb200_episode_window", dtype)
-    with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts), ctypes.byref(rec),
-                ctypes.byref(sp.rec) if sp is not None else None, int(n_steps), ptr_view(C_), ptr_view(c_),
-                ptr_view(F_), ptr_view(f_), ptr_view(sp.F) if sp is not None else None,
-                ptr_view(sp.f) if sp is not None else None, ptr(w_), ptr(x0_), ptr(u0_), ptr(lo_), ptr(hi_),
-                ptr(s.u_zero_I), ptr(xs), ptr(us), ptr(costs), ptr(info), ptr(u_next), ptr(plan_x), ptr(plan_u),
-                ptr(ws), nbytes, stream_handle(dev))
-    if rc == _lib.ERR_NO_GRAPH_COND:
-        return None
-    check(rc, "mpcb200_episode_window")
-    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next)}
-    if keep_plans:
-        res["saved"] = (s._replace(C=C_, c=c_, F=F_, f=f_, u_lower=lo_, u_upper=hi_, n_prev=int(n_prev), plant=sp,
-                                   window=rec), n_steps, xs, us, plan_x, plan_u)
-    return res
-
-
-def _stage_plant_window(pad, plant, dtype, B, n, m, L, rec):
-    """_stage_plant for a time-varying episode: a LinDx plant's F_p, f_p [L-1|L, B, ...] staged whole (its slice k
-    steps control step k; MPCB200_WIN_PLANT set in `rec`); a known plant as _stage_plant stages it."""
-    kind, _, F_p, f_p = plant
-    if kind != DYN_LINEAR:
-        return _stage_plant(pad, plant, dtype, B, n, m)
-    for name, t, shape in (("plant F", F_p, (B, n, n + m)), ("plant f", f_p, (B, n))):
-        if name == "plant F" and t is None:
-            raise MpcB200Error("a LinDx plant needs F")
-        if not _is_empty(t) and (t.dim() != len(shape) + 1 or t.shape[0] not in (L - 1, L) or
-                                 tuple(t.shape[1:]) != shape):
-            raise MpcB200Error(f"{name}: expected shape ({L - 1} or {L}, {', '.join(map(str, shape))}), "
-                               f"got {tuple(t.shape)}")
-    prec = _lib.Plant(kind=int(kind))
-    rec.on |= _lib.WIN_PLANT
-    Fp, rec.Fp_tstride = pad.stage(F_p, dtype, pad.mat_np)
-    fp, rec.fp_tstride = pad.stage(f_p, dtype, pad.vec_n)
-    prec.has_f = int(fp is not None)
-    return _StagedPlant(prec, Fp, fp, False)
-
-
-def _episode_backward_window(s, n_steps, xs, us, plan_x, plan_u, gx_, gu_):
-    """episode_backward_raw of a time-varying episode (mpcb200_episode_backward_window_*): the gradients of the
-    windowed inputs are full length, with zero slices up to their inputs' lengths (slices no step reads)."""
-    pad, dims, rec = s.pad, s.dims, s.window
-    T, B, N, M, L = dims.T, dims.B, pad.N, pad.M, rec.L
-    dtype, dev = xs.dtype, xs.device
-    P = N + M
-    kind = dims.dynamics_kind
-    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
-    dC = torch.empty(L, B, P, P, dtype=dtype, device=dev)
-    dc = torch.empty(L, B, P, dtype=dtype, device=dev)
-    dF = df = dtheta = None
-    from .dynamics import DYN_NPARAMS
-    if kind == DYN_LINEAR:
-        dF = torch.empty(L - T + dims.F_T, B, N, P, dtype=dtype, device=dev)
-        if dims.has_f:
-            df = torch.empty(L - 1, B, N, dtype=dtype, device=dev)
-    else:
-        dtheta = torch.empty(B, DYN_NPARAMS[kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
-    sp = s.plant
-    dF_p = df_p = dth_p = dw = None
-    if sp is not None:
-        pk = sp.rec.kind
-        lead = (L - 1,) if rec.on & _lib.WIN_PLANT else ()
-        dF_p = torch.empty(*lead, B, N, P, dtype=dtype, device=dev) if pk == DYN_LINEAR else None
-        df_p = torch.empty(*lead, B, N, dtype=dtype, device=dev) if pk == DYN_LINEAR and sp.rec.has_f else None
-        dth_p = (torch.empty(B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
-                 if pk != DYN_LINEAR else None)
-        dw = torch.empty(n_steps, B, N, dtype=dtype, device=dev) if sp.disturbed else None
-    prec = ctypes.byref(sp.rec) if sp is not None else None
-    nbytes = _lib.lib().mpcb200_episode_backward_window_workspace_bytes(ctypes.byref(dims), int(s.n_prev),
-                                                                        ctypes.byref(rec), prec, xs.element_size())
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    name = "mpcb200_episode_backward_window"
-    fn = _lib.entry(name, dtype)
-    with _on_device(dev):
-        rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(rec), prec, int(n_steps), int(s.n_prev),
-                ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr_view(sp.F) if sp is not None else None,
-                ptr(s.u_lower), ptr(s.u_upper), ptr(xs), ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_),
-                ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df), ptr(dtheta), ptr(dF_p), ptr(df_p), ptr(dth_p),
-                ptr(dw), ptr(ws), nbytes, stream_handle(dev))
-    check(rc, name)
-
-    def full(g, t):                       # zero slices up to the input's length
-        if g is None or t is None or t.shape[0] == g.shape[0]:
-            return g
-        return torch.cat((g, g.new_zeros(t.shape[0] - g.shape[0], *g.shape[1:])), 0)
-    df = full(df, s.f)
-    if sp is not None and rec.on & _lib.WIN_PLANT:
-        dF_p, df_p = full(dF_p, sp.F), full(df_p, sp.f)
-    out = (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)
-    if sp is None:
-        return out
-    return out + (pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
+    return s._replace(C=C_, c=c_, F=F_, f=f_, u_lower=lo_, u_upper=hi_, window=rec)
 
 
 def episode_backward_raw(saved, dl_dxs, dl_dus):
@@ -699,71 +637,95 @@ def episode_backward_raw(saved, dl_dxs, dl_dus):
     more: dF_p [B, n, p] and df_p [B, n] (a LinDx plant's slice 0; df_p None without f), dtheta_p [B, NP_plant] (a
     known plant) and dw [n_steps, B, n] (None when no w was added); dF, df or dtheta are then the solves' part only.
     A time-varying episode (episode_raw(..., window=L)) runs mpcb200_episode_backward_window_*: dC, dc, dF, df and a
-    windowed LinDx plant's dF_p, df_p are full length (_episode_backward_window)."""
+    windowed LinDx plant's dF_p, df_p are full length, with zero slices up to their inputs' lengths (slices no step
+    reads).  _stage_episode_backward stages the call."""
+    name, args, out = _stage_episode_backward(saved, dl_dxs, dl_dus)
+    check(_call(name, saved[2].dtype, saved[2].device, args), name)
+    g = _episode_grads(saved[0], out)
+    return g if saved[0].plant is not None else g[:6]
+
+
+def _stage_episode_backward(saved, dl_dxs, dl_dus, alloc=None):
+    """The reverse sweep's call as episode_backward_raw (or mlp.episode_backward_raw) makes it, staged but not made:
+    (name, args, out).  The entry is the network's (mpcb200_episode_backward_mlp) for an episode planned with one,
+    else the window's, the plant's (a plant or w), the slew-rate penalty's (n_prev > 0) or the plain one; args and
+    alloc as _stage_episode's.  out: the padded (dx_init, dC, dc, dF, df, dtheta, dF_p, df_p, dtheta_p, dw), None
+    where the entry writes no such output: dF, df a LinDx model's (df with f, T-1 slices); dtheta a known system's
+    [B, NP] or the network's [n_params]; dF_p, df_p a LinDx plant's, dtheta_p [B, NP_plant] a known plant's; dw where
+    w was added.  dC, dc and df lie on a time-varying episode's axis of L slices, and so do a windowed LinDx plant's
+    dF_p, df_p [L-1, B, ...]."""
     s, n_steps, xs, us, plan_x, plan_u = saved
-    pad, dims = s.pad, s.dims
-    T, B, N, M = dims.T, dims.B, pad.N, pad.M
+    pad, dims, sp, win, net = s.pad, s.dims, s.plant, s.window, s.net
+    B, N, P, k = dims.B, pad.N, pad.N + pad.M, int(s.n_prev)
+    L = win.L if win is not None else dims.T          # the cost's time axis
     dtype, dev = xs.dtype, xs.device
     gx_, gu_ = pad.vec_n(_dense(dl_dxs, dtype)), pad.vec_m(_dense(dl_dus, dtype))
-    if s.window is not None:
-        return _episode_backward_window(s, n_steps, xs, us, plan_x, plan_u, gx_, gu_)
-    kind = dims.dynamics_kind
-    P = N + M
-    dx_init = torch.empty(B, N, dtype=dtype, device=dev)
-    dC = torch.empty(T, B, P, P, dtype=dtype, device=dev)
-    dc = torch.empty(T, B, P, dtype=dtype, device=dev)
+    lib, esz = _lib.lib(), xs.element_size()
+    prec = ctypes.byref(sp.rec) if sp is not None else None
+    if net is not None:
+        name, head = "mpcb200_episode_backward_mlp", [ctypes.byref(net[0]), prec, int(n_steps)]
+        nbytes = lib.mpcb200_episode_backward_mlp_workspace_bytes(ctypes.byref(dims), head[0], prec, esz)
+        if nbytes == 0:
+            raise MpcB200Error("mpcb200_episode_backward_mlp: the episode has no workspace size (the network's VJP "
+                               "does not fit, or bad dimensions)")
+    elif win is not None:
+        name, head = "mpcb200_episode_backward_window", [ctypes.byref(win), prec, int(n_steps), k]
+        nbytes = lib.mpcb200_episode_backward_window_workspace_bytes(ctypes.byref(dims), k, head[0], prec, esz)
+    elif sp is not None:
+        name, head = "mpcb200_episode_backward_plant", [prec, int(n_steps), k]
+        nbytes = lib.mpcb200_episode_backward_plant_workspace_bytes(ctypes.byref(dims), k, prec, esz)
+    elif k:
+        name, head = "mpcb200_episode_backward_slew", [int(n_steps), k]
+        nbytes = lib.mpcb200_episode_backward_slew_workspace_bytes(ctypes.byref(dims), k, esz)
+    else:
+        name, head = "mpcb200_episode_backward", [int(n_steps)]
+        nbytes = lib.mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), esz)
+    if alloc is None:
+        def alloc(shape, dt):
+            return torch.empty(shape, dtype=dt, device=dev)
+
+    def n_params(kind):
+        return DYN_NPARAMS[kind & ~DYN_CTRL_PASSTHROUGH]
+    dx_init, dC, dc = alloc((B, N), dtype), alloc((L, B, P, P), dtype), alloc((L, B, P), dtype)
     dF = df = dtheta = None
-    if kind == DYN_LINEAR:
-        dF = torch.empty(s.F.shape[0], B, N, P, dtype=dtype, device=dev)
-        if dims.has_f:
-            df = torch.empty(T - 1, B, N, dtype=dtype, device=dev)
+    if net is not None:
+        dtheta = alloc((net[1].numel(),), dtype)
+    elif dims.dynamics_kind == DYN_LINEAR:
+        dF = alloc((s.F.shape[0], B, N, P), dtype)
+        df = alloc((L - 1, B, N), dtype) if dims.has_f else None
     else:
-        from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_NPARAMS
-        dtheta = torch.empty(B, DYN_NPARAMS[kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
-    L = _lib.lib()
-    sp = s.plant
-    if sp is not None:
-        from .dynamics import DYN_CTRL_PASSTHROUGH, DYN_NPARAMS
-        pk = sp.rec.kind
-        dF_p = torch.empty(B, N, P, dtype=dtype, device=dev) if pk == DYN_LINEAR else None
-        df_p = torch.empty(B, N, dtype=dtype, device=dev) if pk == DYN_LINEAR and sp.rec.has_f else None
-        dth_p = (torch.empty(B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype, device=dev)
-                 if pk != DYN_LINEAR else None)
-        dw = torch.empty(n_steps, B, N, dtype=dtype, device=dev) if sp.disturbed else None
-        name = "mpcb200_episode_backward_plant"
-        nbytes = L.mpcb200_episode_backward_plant_workspace_bytes(ctypes.byref(dims), int(s.n_prev),
-                                                                  ctypes.byref(sp.rec), xs.element_size())
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        fn = _lib.entry(name, dtype)
-        with _on_device(dev):
-            rc = fn(ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(sp.rec), int(n_steps), int(s.n_prev),
-                    ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr(sp.F), ptr(s.u_lower), ptr(s.u_upper), ptr(xs),
-                    ptr(us), ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF),
-                    ptr(df), ptr(dtheta), ptr(dF_p), ptr(df_p), ptr(dth_p), ptr(dw), ptr(ws), nbytes,
-                    stream_handle(dev))
-        check(rc, name)
-        if df is not None and s.f.shape[0] == T:
-            df = torch.cat((df, torch.zeros_like(df[:1])), 0)
-        return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta,
-                pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
-    if s.n_prev:
-        name = "mpcb200_episode_backward_slew"
-        nbytes = L.mpcb200_episode_backward_slew_workspace_bytes(ctypes.byref(dims), int(s.n_prev), xs.element_size())
-        head = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), int(s.n_prev)]
-    else:
-        name = "mpcb200_episode_backward"
-        nbytes = L.mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), xs.element_size())
-        head = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps)]
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    fn = _lib.entry(name, dtype)
-    with _on_device(dev):
-        rc = fn(*head, ptr_view(s.C), ptr_view(s.c), ptr_view(s.F), ptr(s.u_lower), ptr(s.u_upper), ptr(xs), ptr(us),
-                ptr(plan_x), ptr(plan_u), ptr(gx_), ptr(gu_), ptr(dx_init), ptr(dC), ptr(dc), ptr(dF), ptr(df),
-                ptr(dtheta), ptr(ws), nbytes, stream_handle(dev))
-    check(rc, name)
-    if df is not None and s.f.shape[0] == T:          # a full-length f: its last slice never enters the episode
-        df = torch.cat((df, torch.zeros_like(df[:1])), 0)
-    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)
+        dtheta = alloc((B, n_params(dims.dynamics_kind)), dtype)
+    lin_plant = sp is not None and sp.rec.kind == DYN_LINEAR
+    lead = (L - 1,) if win is not None and win.on & _lib.WIN_PLANT else ()
+    dF_p = alloc((*lead, B, N, P), dtype) if lin_plant else None
+    df_p = alloc((*lead, B, N), dtype) if lin_plant and sp.rec.has_f else None
+    dth_p = alloc((B, n_params(sp.rec.kind)), dtype) if sp is not None and not lin_plant else None
+    dw = alloc((n_steps, B, N), dtype) if s.disturbed or (sp is not None and sp.disturbed) else None
+    ws = alloc((nbytes,), torch.uint8)
+    plant_sweep = net is not None or win is not None or sp is not None
+    args = [ctypes.byref(dims), ctypes.byref(s.params), *head, s.C, s.c, *([] if net is not None else [s.F]),
+            *([sp.F if sp is not None else None] if plant_sweep else []), s.u_lower, s.u_upper, xs, us, plan_x, plan_u,
+            gx_, gu_, dx_init, dC, dc, *([] if net is not None else [dF, df]), dtheta,
+            *([dF_p, df_p, dth_p, dw] if plant_sweep else []), ws, nbytes, stream_handle(dev)]
+    return name, args, (dx_init, dC, dc, dF, df, dtheta, dF_p, df_p, dth_p, dw)
+
+
+def _episode_grads(s, out):
+    """The ten gradients of a reverse sweep's outputs (_stage_episode_backward) as the staged problem's inputs take
+    them: cropped to its own (n, m), and df (and a windowed LinDx plant's dF_p, df_p) zero-extended to the staged
+    input's length, the slices no step reads."""
+    dx_init, dC, dc, dF, df, dtheta, dF_p, df_p, dth_p, dw = out
+    pad, sp = s.pad, s.plant
+
+    def full(g, t):
+        if g is None or t is None or t.shape[0] == g.shape[0]:
+            return g
+        return torch.cat((g, g.new_zeros(t.shape[0] - g.shape[0], *g.shape[1:])), 0)
+    df = full(df, s.f)
+    if s.window is not None and s.window.on & _lib.WIN_PLANT:
+        dF_p, df_p = full(dF_p, sp.F), full(df_p, sp.f)
+    return (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta,
+            pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
 
 
 def lqr_grad_raw(n_state, n_ctrl, T, C, c, F, new_x, new_u, dx, du, dl_dx, want_df, f_T=None):

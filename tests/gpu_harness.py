@@ -911,7 +911,7 @@ def pick_switch(group, dtype, augmentable=False):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# receding-horizon episodes through the C ABI (mpcb200_episode_plans_*, mpcb200_episode_backward_*)
+# receding-horizon episodes through the library's own staging (step._stage_episode, step._stage_episode_backward)
 # ------------------------------------------------------------------------------------------------------------------
 def _owned(poison, *shape, dtype):
     """A caller-owned buffer: every byte 0xFF when `poison` (NaN in float32 and float64, -1 in int32), else empty."""
@@ -921,133 +921,61 @@ def _owned(poison, *shape, dtype):
     return t
 
 
+def _owned_alloc(poison, nan_outputs):
+    """The staging's alloc hook: the workspace (the one byte buffer) _owned when `poison`, every output when `poison`
+    or `nan_outputs`."""
+    return lambda shape, dtype: _owned(poison or (nan_outputs and dtype != torch.uint8), *shape, dtype=dtype)
+
+
 def abi_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5,
                 eps=1e-7, best_cost_eps=1e-4, dyn=None, poison=False, n_prev=0, plant=None, w=None,
                 nan_outputs=False):
-    """The call step.episode_raw(..., keep_plans=True) makes (mpcb200_episode_plans_*, the problem staged by the same
-    step._problem), with caller-owned outputs and workspace.  poison: every workspace byte and every output starts at
-    0xFF, so a kernel that reads an element nothing wrote reads NaN (or info -1); nan_outputs: the outputs alone start
-    at 0xFF, so an element the call does not write comes back NaN (or -1).  n_prev: a slew-rate penalty's
-    augmented problem, recorded in the staged problem for abi_episode_backward.  plant ("lin", F_p, f_p) of a LinDx
-    plant (f_p None: none) or (kind, params) of a known one, and w [n_steps, B, n]: the call is
-    mpcb200_episode_plant_*, the plant and w staged as step.episode_raw stages them (plant None with w: the model
-    steps, disturbed).  Returns (res, launches, plan): res as episode_raw's dict, "saved" included, launches the
-    library kernels the call recorded, plan mpcb200_last_step_plan() after it (the step plan of the solve)."""
+    """step.episode_raw(..., keep_plans=True): the call its staging makes (step._stage_episode: mpcb200_episode_plans_*,
+    or mpcb200_episode_plant_* with a plant or w), with caller-owned outputs and workspace.  poison: every workspace
+    byte and every output starts at 0xFF, so a kernel that reads an element nothing wrote reads NaN (or info -1);
+    nan_outputs: the outputs alone start at 0xFF, so an element the call does not write comes back NaN (or -1).
+    n_prev: a slew-rate penalty's augmented problem, recorded in the staged problem for abi_episode_backward.  plant
+    ("lin", F_p, f_p) of a LinDx plant (f_p None: none) or (kind, params) of a known one, and w [n_steps, B, n] (plant
+    None with w: the model steps, disturbed).  Returns (res, launches, plan): res as episode_raw's dict, "saved"
+    included, launches the library kernels the call recorded, plan mpcb200_last_step_plan() after it (the step plan of
+    the solve)."""
     from mpc.pytorch_b200 import step as S
     from mpc.pytorch_b200.dynamics import DYN_LINEAR
     L = _L()
-    B = x_init.shape[0]
-    dtype = C.dtype
-    s = S._problem(n, m, T, B, dtype, DEV, C, c, F, f, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
-                   max_linesearch_iter, dyn)
-    pad, dims, N, M = s.pad, s.dims, s.pad.N, s.pad.M
-    x0_, u0_ = pad.vec_n(S._dense(x_init, dtype)), pad.vec_m(S._dense(u_init, dtype))
-    sp = w_ = None
-    if plant is not None or w is not None:
-        if plant is None:
-            spec = (DYN_LINEAR, None, F, f) if dyn is None else (dyn[0], dyn[1], None, None)
-        elif plant[0] == "lin":
-            spec = (DYN_LINEAR, None, plant[1], plant[2])
-        else:
-            spec = (plant[0], plant[1], None, None)
-        sp = S._stage_plant(pad, spec, dtype, B, n, m)
-        if w is not None:
-            w_ = pad.vec_n(S._dense(w, dtype)).contiguous()
-            sp = sp._replace(disturbed=True)
-    opts = L.IlqrOpts(lqr_iter=int(lqr_iter), not_improved_lim=int(not_improved_lim), m_ref=m, eps=float(eps),
-                      best_cost_eps=float(best_cost_eps))
-    nbytes = L.lib().mpcb200_episode_workspace_bytes(ctypes.byref(dims), ctypes.byref(opts), C.element_size())
-    ws = _owned(poison, nbytes, dtype=torch.uint8)
-    fill = poison or nan_outputs
-    xs, us = _owned(fill, n_steps + 1, B, N, dtype=dtype), _owned(fill, n_steps, B, M, dtype=dtype)
-    costs, info = _owned(fill, n_steps, B, dtype=dtype), _owned(fill, n_steps, 2, dtype=torch.int32)
-    u_next = _owned(fill, T, B, M, dtype=dtype)
-    plan_x, plan_u = _owned(fill, n_steps, T, B, N, dtype=dtype), _owned(fill, n_steps, T, B, M, dtype=dtype)
-    head = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(opts)]
-    problem = [int(n_steps), L.ptr_view(s.C), L.ptr_view(s.c), L.ptr_view(s.F), L.ptr_view(s.f)]
-    tail = [L.ptr(x0_), L.ptr(u0_), L.ptr(s.u_lower), L.ptr(s.u_upper), L.ptr(s.u_zero_I), L.ptr(xs), L.ptr(us),
-            L.ptr(costs), L.ptr(info), L.ptr(u_next), L.ptr(plan_x), L.ptr(plan_u), L.ptr(ws), nbytes,
-            L.stream_handle(DEV)]
-    if sp is None:
-        name, args = "mpcb200_episode_plans", head + problem + tail
-    else:
-        name = "mpcb200_episode_plant"
-        args = head + [ctypes.byref(sp.rec)] + problem + [L.ptr(sp.F), L.ptr(sp.f), L.ptr(w_)] + tail
+    if plant is not None:
+        plant = (DYN_LINEAR, None, plant[1], plant[2]) if plant[0] == "lin" else (plant[0], plant[1], None, None)
+    s, name, args, out = S._stage_episode(
+        n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
+        max_linesearch_iter, lqr_iter, not_improved_lim, eps, best_cost_eps, dyn=dyn, keep_plans=True, n_prev=n_prev,
+        plant=plant, w=w, alloc=_owned_alloc(poison, nan_outputs))
     before = L.launch_count()
-    with L._on_device(DEV):
-        rc = L.entry(name, dtype)(*args)
-    L.check(rc, name)
+    rc = S._call(name, C.dtype, DEV, args)
     launches, p = L.launch_count() - before, L.last_step_plan()
     torch.cuda.synchronize()
-    res = {"x": pad.crop_n(xs), "u": pad.crop_m(us), "costs": costs, "info": info, "u_next": pad.crop_m(u_next),
-           "saved": (s._replace(n_prev=int(n_prev), plant=sp), n_steps, xs, us, plan_x, plan_u)}
+    res = S._episode_result(rc, name, s, out)
+    assert res is not None, "the driver has no conditional graph nodes"
     return res, launches, p
 
 
 def abi_episode_backward(saved, dl_dxs, dl_dus, poison=False, nan_outputs=False):
-    """The call step.episode_backward_raw makes, with caller-owned outputs and workspace, poison as in abi_episode:
+    """step.episode_backward_raw: the call its staging makes (step._stage_episode_backward:
     mpcb200_episode_backward_plant_* when the staged problem records a plant, mpcb200_episode_backward_slew_* when it
-    records n_prev > 0, else mpcb200_episode_backward_*.  Returns ((dx_init, dC, dc, dF, df, dtheta) cropped as
-    episode_backward_raw crops them, and for a plant four more: dF_p [B, n, p], df_p [B, n] (None without the plant's
-    f), dtheta_p [B, NP_plant] and dw [n_steps, B, n] (None without w); launches, plan): plan is the nested step's,
-    recorded in the sweep's body.  Under a slew-rate penalty every size is the augmented problem's."""
+    records n_prev > 0, else mpcb200_episode_backward_*), with caller-owned outputs and workspace, poison as in
+    abi_episode.  Returns ((dx_init, dC, dc, dF, df, dtheta) as episode_backward_raw returns them, and for a plant
+    four more: dF_p [B, n, p], df_p [B, n] (None without the plant's f), dtheta_p [B, NP_plant] and dw
+    [n_steps, B, n] (None without w); launches, plan): plan is the nested step's, recorded in the sweep's body.  Under
+    a slew-rate penalty every size is the augmented problem's."""
     from mpc.pytorch_b200 import step as S
-    from mpc.pytorch_b200.dynamics import DYN_CTRL_PASSTHROUGH, DYN_LINEAR, DYN_NPARAMS
     L = _L()
-    s, n_steps, xs, us, plan_x, plan_u = saved
-    pad, dims, sp = s.pad, s.dims, s.plant
-    T, B, N, M = dims.T, dims.B, pad.N, pad.M
-    dtype, P = xs.dtype, pad.N + pad.M
-    gx_, gu_ = pad.vec_n(S._dense(dl_dxs, dtype)), pad.vec_m(S._dense(dl_dus, dtype))
-    fill = poison or nan_outputs
-    dx_init, dC, dc = (_owned(fill, B, N, dtype=dtype), _owned(fill, T, B, P, P, dtype=dtype),
-                       _owned(fill, T, B, P, dtype=dtype))
-    dF = df = dtheta = None
-    if dims.dynamics_kind == DYN_LINEAR:
-        dF = _owned(fill, s.F.shape[0], B, N, P, dtype=dtype)
-        df = _owned(fill, T - 1, B, N, dtype=dtype) if dims.has_f else None
-    else:
-        dtheta = _owned(fill, B, DYN_NPARAMS[dims.dynamics_kind & ~DYN_CTRL_PASSTHROUGH], dtype=dtype)
-    ins = [L.ptr(s.u_lower), L.ptr(s.u_upper), L.ptr(xs), L.ptr(us), L.ptr(plan_x), L.ptr(plan_u), L.ptr(gx_),
-           L.ptr(gu_), L.ptr(dx_init), L.ptr(dC), L.ptr(dc), L.ptr(dF), L.ptr(df), L.ptr(dtheta)]
-    model = [L.ptr_view(s.C), L.ptr_view(s.c), L.ptr_view(s.F)]
-    sz = xs.element_size()
-    plant_out = ()
-    if sp is not None:
-        pk = sp.rec.kind
-        plant_out = (_owned(fill, B, N, P, dtype=dtype) if pk == DYN_LINEAR else None,
-                     _owned(fill, B, N, dtype=dtype) if pk == DYN_LINEAR and sp.rec.has_f else None,
-                     _owned(fill, B, DYN_NPARAMS[pk & ~DYN_CTRL_PASSTHROUGH], dtype=dtype)
-                     if pk != DYN_LINEAR else None,
-                     _owned(fill, n_steps, B, N, dtype=dtype) if sp.disturbed else None)
-        name = "mpcb200_episode_backward_plant"
-        nbytes = L.lib().mpcb200_episode_backward_plant_workspace_bytes(ctypes.byref(dims), int(s.n_prev),
-                                                                        ctypes.byref(sp.rec), sz)
-        head = [ctypes.byref(dims), ctypes.byref(s.params), ctypes.byref(sp.rec), int(n_steps), int(s.n_prev)]
-        args = head + model + [L.ptr(sp.F)] + ins + [L.ptr(t) for t in plant_out]
-    elif s.n_prev:
-        name = "mpcb200_episode_backward_slew"
-        nbytes = L.lib().mpcb200_episode_backward_slew_workspace_bytes(ctypes.byref(dims), int(s.n_prev), sz)
-        args = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps), int(s.n_prev)] + model + ins
-    else:
-        name = "mpcb200_episode_backward"
-        nbytes = L.lib().mpcb200_episode_backward_workspace_bytes(ctypes.byref(dims), sz)
-        args = [ctypes.byref(dims), ctypes.byref(s.params), int(n_steps)] + model + ins
-    ws = _owned(poison, nbytes, dtype=torch.uint8)
+    name, args, out = S._stage_episode_backward(saved, dl_dxs, dl_dus, alloc=_owned_alloc(poison, nan_outputs))
     before = L.launch_count()
-    with L._on_device(DEV):
-        rc = L.entry(name, dtype)(*args, L.ptr(ws), nbytes, L.stream_handle(DEV))
+    rc = S._call(name, saved[2].dtype, DEV, args)
     L.check(rc, name)
     launches, p = L.launch_count() - before, L.last_step_plan()
     torch.cuda.synchronize()
-    if df is not None and s.f.shape[0] == T:
-        df = torch.cat((df, torch.zeros_like(df[:1])), 0)
-    out = (pad.crop_n(dx_init), pad.crop_pp(dC), pad.crop_p(dc), pad.crop_np(dF), pad.crop_n(df), dtheta)
-    if sp is not None:
-        dF_p, df_p, dth_p, dw = plant_out
-        out += (pad.crop_np(dF_p), pad.crop_n(df_p), dth_p, pad.crop_n(dw))
-    return out, launches, p
+    g = S._episode_grads(saved[0], out)
+    return (g if saved[0].plant is not None else g[:6]), launches, p
 
 
 def _episode_per_problem(a, b):
