@@ -113,6 +113,11 @@ static int check_dims(const mpcb200_dims* d) {
   if (d->F_T != d->T - 1 && d->F_T != d->T) return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
 }
+// a call whose network or window record is NULL: check_dims's error where there is one, as where the record is checked
+static int null_record(const mpcb200_dims* d) {
+  const int rc = check_dims(d);
+  return rc ? rc : MPCB200_ERR_NULL_POINTER;
+}
 
 // the step's option checks, one order for every entry point: an argument error gets the same code from each
 static int check_bounds(const mpcb200_dims* d, const void* lo, const void* hi) {
@@ -480,13 +485,145 @@ static int dyn_vjp_impl(int kind, const double* dyn, int B, int T, const R* x, c
 }
 
 // ---------------------------------------------------------------------------------------------
-// the iLQR loop of MPC.forward as one CUDA graph (reference mpc/mpc.py:244-301)
+// a learned model's network (mlp.cu): its rollout and linearisation, and the split-mode step (the step kernels with
+// do_rollout = 0, then the network's line search)
 // ---------------------------------------------------------------------------------------------
-// dims of the step inside the loop: the caller's, with the rollout on and, for a known system, the workspace F, f
-static mpcb200_dims ilqr_step_dims(const mpcb200_dims* d) {
+static int mlp_check(const mpcb200_mlp* mlp, int B, int T, int N, int M, MlpShape& s) {
+  if (mlp == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (!mlp_shape(mlp, s)) return MPCB200_ERR_BAD_DIMS;
+  if (B <= 0 || T <= 0 || N < s.n_prev + s.ns || M < s.ms || N + M > s.p_max) return MPCB200_ERR_BAD_DIMS;
+  return MPCB200_OK;
+}
+
+// A network an episode takes: mlp_check's, without the slew-rate state, with kernels that fit `smem` bytes of shared
+// memory (an entry's device, or kOptinAssumed for a workspace size).
+static int episode_net_check(const mpcb200_dims* d, const mpcb200_mlp* mlp, int elem_size, int smem, MlpShape& s) {
+  if (const int rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s)) return rc;
+  if (s.n_prev != 0) return MPCB200_ERR_BAD_DIMS;
+  return mlp_smem_bytes(s, elem_size, 1) > (size_t)smem ? MPCB200_ERR_SMEM : MPCB200_OK;
+}
+
+template <typename R>
+static int mlp_rollout_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x_init, const R* u, R* x,
+                            void* stream) {
+  MlpShape s;
+  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
+  if (x_init == nullptr || u == nullptr || x == nullptr) return MPCB200_ERR_NULL_POINTER;
+  return counted(mlp_launch_rollout<R>(mlp, B, T, N, M, x_init, u, x, (cudaStream_t)stream));
+}
+
+template <typename R>
+static int mlp_linearize_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x, const R* u, R* F, R* f,
+                              void* stream) {
+  MlpShape s;
+  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
+  if (x == nullptr || u == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (T == 1) return MPCB200_OK;
+  if (F == nullptr || f == nullptr) return MPCB200_ERR_NULL_POINTER;
+  return counted(mlp_launch_linearize<R>(mlp, B, T, N, M, x, u, F, f, (cudaStream_t)stream));
+}
+
+// the linearisation VJP's workspace ([G, n_params] slot rows), 0 where its per-warp slice does not fit
+static size_t mlp_vjp_ws(const MlpShape& s, int B, int T, size_t sz) {
+  if (mlp_smem_bytes(mlp_vjp_shape(s), (int)sz, 1) > (size_t)kOptinAssumed) return 0;
+  return up256((size_t)mlp_vjp_slots((long long)(T - 1) * B, s.n_params) * (size_t)s.n_params * sz);
+}
+
+template <typename R>
+static int mlp_linearize_vjp_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x, const R* u,
+                                  const R* dF, const R* df, R* dtheta, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  MlpShape s;
+  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
+  if (x == nullptr || u == nullptr || dF == nullptr || df == nullptr || dtheta == nullptr || workspace == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  const size_t need = mlp_vjp_ws(s, B, T, sizeof(R));
+  if (need == 0) return MPCB200_ERR_SMEM;
+  if (workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
+  return counted(mlp_launch_linearize_vjp<R>(mlp, B, T, N, M, x, u, dF, df, dtheta, (R*)workspace,
+                                             (cudaStream_t)stream), 2);
+}
+
+static size_t mlp_step_ws(const mpcb200_dims* d, size_t sz) {
+  const size_t TBM = (size_t)d->T * d->B * d->m;
+  return up256(TBM * d->n * sz) + up256(TBM * sz);
+}
+
+// The line search's arguments: the gains the step wrote into q.Ks, q.ks, the iterate it writes into q's new_x, new_u,
+// costs, alphas and du_first.
+template <typename R>
+static MlpLsArgs<R> mlp_ls_args(const mpcb200_dims* d, const mpcb200_params* p, const StepCall<R>& q) {
+  MlpLsArgs<R> a;
+  std::memset(&a, 0, sizeof(a));
+  a.B = d->B; a.T = d->T; a.N = d->n; a.M = d->m;
+  a.bounds_kind = d->bounds_kind; a.has_mask = d->has_zero_mask ? 1 : 0; a.has_delta = d->has_delta_u ? 1 : 0;
+  a.max_ls = d->max_ls_iter;
+  const TimeStrides ts = time_strides(d);
+  a.C_ts = ts.C; a.c_ts = ts.c;
+  a.u_lo = (R)p->u_lo; a.u_hi = (R)p->u_hi; a.delta_u = (R)p->delta_u; a.decay = (R)p->ls_decay;
+  a.C = q.C; a.c = q.c; a.x_init = q.x_init; a.cur_x = q.cur_x; a.cur_u = q.cur_u; a.Ks = q.Ks; a.ks = q.ks;
+  a.u_lower = q.u_lower; a.u_upper = q.u_upper; a.zero_mask = q.u_zero_I;
+  a.new_x = q.new_x; a.new_u = q.new_u; a.costs = q.costs; a.alphas = q.alphas; a.du_first = q.du_first;
+  return a;
+}
+
+// the checks of a split-mode step that need no device, before anything is launched
+template <typename R>
+static int mlp_step_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp,
+                          const StepCall<R>& q) {
+  int rc = check_dims(d);
+  if (rc) return rc;
+  MlpShape s;
+  if ((rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s))) return rc;
+  if (p == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr || q.cur_x == nullptr ||
+      q.cur_u == nullptr || q.new_x == nullptr || q.new_u == nullptr || q.costs == nullptr || q.alphas == nullptr)
+    return MPCB200_ERR_NULL_POINTER;
+  if (d->T > 1 && q.F == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (d->has_f && q.f == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if ((rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I))) return rc;
+  if (d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
+  return MPCB200_OK;
+}
+
+// The split-mode step of q: the step kernels with do_rollout = 0 write the gains into q.Ks, q.ks (and qp_iters,
+// free_mask, status), then the network's line search writes the iterate.
+template <typename R>
+static int mlp_split_step(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp, const StepCall<R>& q,
+                          int knob, void* stream) {
+  mpcb200_dims ds = *d;
+  ds.do_rollout = 0;
+  StepCall<R> sc = q;
+  sc.new_x = sc.new_u = sc.costs = sc.full_du_norm = sc.alphas = sc.du_first = nullptr;
+  if (const int rc = step_impl<R>(&ds, p, sc, knob, stream)) return rc;
+  return counted(mlp_launch_linesearch<R>(mlp, mlp_ls_args<R>(d, p, q), (cudaStream_t)stream));
+}
+
+// q: the arguments of mpcb200_mlp_step_* after dims, params and the record (no full_du_norm, Ks or ks)
+template <typename R>
+static int mlp_step_impl(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp, StepCall<R> q,
+                         void* workspace, size_t workspace_bytes, void* stream) {
+  const int knob = kernel_knob();
+  int rc = mlp_step_check<R>(d, p, mlp, q);
+  if (rc) return rc;
+  if (workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (workspace_bytes < mlp_step_ws(d, sizeof(R)) || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0)
+    return MPCB200_ERR_BAD_DIMS;
+  q.Ks = (R*)workspace;
+  q.ks = (R*)((char*)workspace + up256((size_t)d->T * d->B * d->m * d->n * sizeof(R)));
+  return mlp_split_step<R>(d, p, mlp, q, knob, stream);
+}
+
+// ---------------------------------------------------------------------------------------------
+// the iLQR loop of MPC.forward as one CUDA graph (reference mpc/mpc.py:244-301), on LinDx, a known system or a
+// learned model's network (mpcb200_ilqr_mlp_*)
+// ---------------------------------------------------------------------------------------------
+// dims of the step inside the loop: the caller's, with the rollout on and, for a known system or a network (net), the
+// workspace F, f
+static mpcb200_dims ilqr_step_dims(const mpcb200_dims* d, bool net) {
   mpcb200_dims ds = *d;
   ds.do_rollout = 1;
-  if (d->dynamics_kind != DYN_LINEAR) {
+  if (net || d->dynamics_kind != DYN_LINEAR) {
     ds.F_T = d->T - 1; ds.has_f = d->T > 1 ? 1 : 0; ds.F_tstride = 0; ds.f_tstride = 0;
   }
   return ds;
@@ -496,7 +633,8 @@ struct IlqrLayout {                   // workspace carve-up (byte offsets, every
   size_t u, x, new_x, new_u, costs, fdn_step, alphas, du_first, status, fdn, flags, state, F, f, Ks, ks, total;
   bool gains;
 };
-static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz, int knob) {
+// net: the loop of mpcb200_ilqr_mlp_*, whose split-mode step always writes the gains
+static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz, int knob, bool net) {
   IlqrLayout l;
   const size_t TB = (size_t)d->T * d->B, B = d->B;
   const size_t n = d->n, m = d->m;
@@ -513,14 +651,16 @@ static IlqrLayout ilqr_layout(const mpcb200_dims* d, size_t sz, int knob) {
   l.fdn = o;      o += up256(B * sz);
   l.flags = o;    o += up256(B);
   l.state = o;    o += up256(sizeof(IlqrState));
+  // the linearisation of a known system or the network, rewritten every iteration.  The network's entries refuse a
+  // known kind; their workspace sizes for one count both linearisations.
+  const size_t TB1 = (size_t)(d->T > 1 ? d->T - 1 : 0) * B;
   l.F = l.f = 0;
-  if (d->dynamics_kind != DYN_LINEAR) {         // the linearisation of a known system, rewritten every iteration
-    const size_t TB1 = (size_t)(d->T > 1 ? d->T - 1 : 0) * B;
+  for (int k = (d->dynamics_kind != DYN_LINEAR) + (net ? 1 : 0); k > 0; --k) {
     l.F = o;      o += up256(TB1 * n * (n + m) * sz);
     l.f = o;      o += up256(TB1 * n * sz);
   }
-  const mpcb200_dims ds = ilqr_step_dims(d);
-  l.gains = gains_in_workspace(&ds, (int)sz, knob) != 0;
+  const mpcb200_dims ds = ilqr_step_dims(d, net);
+  l.gains = net || gains_in_workspace(&ds, (int)sz, knob) != 0;
   l.Ks = l.ks = 0;
   if (l.gains) {
     l.Ks = o;     o += up256(TB * m * n * sz);
@@ -544,18 +684,23 @@ struct IlqrCall {
   size_t workspace_bytes;
 };
 
-// argument checks that need no device: every error is reported before anything is captured or launched
+// argument checks that need no device: every error is reported before anything is captured or launched.  mlp: the
+// network the loop plans with (non-NULL from mpcb200_ilqr_mlp_*), or NULL.
 template <typename R>
-static int ilqr_check(const IlqrCall<R>& q, int knob) {
+static int ilqr_check(const IlqrCall<R>& q, const mpcb200_mlp* mlp, int knob) {
   const mpcb200_dims* d = q.d;
   int rc = check_dims(d);
   if (rc) return rc;
+  MlpShape s;
+  if (mlp != nullptr && (rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s))) return rc;
   if (q.p == nullptr || q.o == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr ||
       q.best_x == nullptr || q.best_u == nullptr || q.best_costs == nullptr || q.best_fdn == nullptr ||
       q.info == nullptr || q.workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (q.o->lqr_iter < 1 || q.o->m_ref < 1 || q.o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
-  if (d->dynamics_kind != DYN_LINEAR) {
+  if (mlp != nullptr) {
+    if (d->T < 2 || d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  } else if (d->dynamics_kind != DYN_LINEAR) {
     if (!known_shape_ok(d)) return MPCB200_ERR_BAD_DIMS;
   } else {
     if (d->T > 1 && q.F == nullptr) return MPCB200_ERR_NULL_POINTER;
@@ -563,8 +708,12 @@ static int ilqr_check(const IlqrCall<R>& q, int knob) {
   }
   rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I);
   if (rc) return rc;
-  if (d->dynamics_kind != DYN_LINEAR && find_step(d) == nullptr) return MPCB200_ERR_UNSUPPORTED_DIMS;
-  const IlqrLayout l = ilqr_layout(d, sizeof(R), knob);
+  if (mlp != nullptr) {
+    if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
+  } else if (d->dynamics_kind != DYN_LINEAR && find_step(d) == nullptr) {
+    return MPCB200_ERR_UNSUPPORTED_DIMS;
+  }
+  const IlqrLayout l = ilqr_layout(d, sizeof(R), knob, mlp != nullptr);
   if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
@@ -625,12 +774,14 @@ static int open_while(cudaStream_t os, cudaStream_t bs, cudaGraphConditionalHand
   return MPCB200_OK;
 }
 
-// Adds the init kernel and the `while` node (body recorded on `bs`) to the graph `os` is capturing.
+// Adds the init kernel and the `while` node (body recorded on `bs`) to the graph `os` is capturing.  Body: the model
+// part, then track -> stop.  The model part: LinDx: rollout -> step; a known system: rollout -> linearisation -> step;
+// mlp (non-NULL): the network's rollout -> linearisation -> split-mode step (mlp_split_step: step, line search).
 template <typename R>
-static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, int knob) {
+static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, int knob, const mpcb200_mlp* mlp) {
   const mpcb200_dims* d = q.d;
   const mpcb200_ilqr_opts* o = q.o;
-  const IlqrLayout l = ilqr_layout(d, sizeof(R), knob);
+  const IlqrLayout l = ilqr_layout(d, sizeof(R), knob, mlp != nullptr);
   char* ws = (char*)q.workspace;
   R* u = (R*)(ws + l.u);
   R* x = (R*)(ws + l.x);
@@ -646,7 +797,7 @@ static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, i
   // the body: the library's own launchers, recorded on bs (same plan selection as a direct call)
   rc = open_while(os, bs, handle);
   if (rc) return rc;
-  const mpcb200_dims ds = ilqr_step_dims(d);
+  const mpcb200_dims ds = ilqr_step_dims(d, mlp != nullptr);
   StepCall<R> sc = {};
   sc.C = q.C; sc.c = q.c; sc.F = q.F; sc.f = q.f; sc.x_init = q.x_init; sc.cur_x = x; sc.cur_u = u;
   sc.u_lower = q.u_lower; sc.u_upper = q.u_upper; sc.u_zero_I = q.u_zero_I;
@@ -657,16 +808,25 @@ static int ilqr_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, i
     sc.Ks = (R*)(ws + l.Ks);
     sc.ks = (R*)(ws + l.ks);
   }
-  if (d->dynamics_kind == DYN_LINEAR) {
-    rc = rollout_impl<R>(d, q.F, q.f, q.x_init, u, x, knob, bs);
-  } else {                            // a known system: the step reads the workspace F, f, rewritten every iteration
-    sc.F = T > 1 ? (R*)(ws + l.F) : nullptr;
-    sc.f = T > 1 ? (R*)(ws + l.f) : nullptr;
-    rc = dyn_impl<R>(false, d->dynamics_kind, q.p->dyn, B, T, q.x_init, u, x, nullptr, nullptr, bs);
-    if (rc == 0)
-      rc = dyn_impl<R>(true, d->dynamics_kind, q.p->dyn, B, T, x, u, nullptr, (R*)(ws + l.F), (R*)(ws + l.f), bs);
+  R* F = (R*)(ws + l.F);              // a known system's or the network's linearisation: the step reads it
+  R* f = (R*)(ws + l.f);
+  if (mlp != nullptr || d->dynamics_kind != DYN_LINEAR) {
+    sc.F = T > 1 ? F : nullptr;
+    sc.f = T > 1 ? f : nullptr;
   }
-  if (rc == 0) rc = step_impl<R>(&ds, q.p, sc, knob, bs);
+  if (mlp != nullptr) {
+    rc = mlp_rollout_impl<R>(mlp, B, T, N, M, q.x_init, u, x, bs);
+    if (rc == 0) rc = mlp_linearize_impl<R>(mlp, B, T, N, M, x, u, F, f, bs);
+    if (rc == 0) rc = mlp_split_step<R>(&ds, q.p, mlp, sc, knob, bs);
+  } else {
+    if (d->dynamics_kind == DYN_LINEAR) {
+      rc = rollout_impl<R>(d, q.F, q.f, q.x_init, u, x, knob, bs);
+    } else {
+      rc = dyn_impl<R>(false, d->dynamics_kind, q.p->dyn, B, T, q.x_init, u, x, nullptr, nullptr, bs);
+      if (rc == 0) rc = dyn_impl<R>(true, d->dynamics_kind, q.p->dyn, B, T, x, u, nullptr, F, f, bs);
+    }
+    if (rc == 0) rc = step_impl<R>(&ds, q.p, sc, knob, bs);
+  }
   if (rc == 0)
     rc = counted(ilqr_launch_track<R>(B, T, N, M, o->m_ref, (R)o->best_cost_eps, sc.new_x, sc.new_u, sc.costs,
                                       sc.du_first, sc.status, q.best_costs, q.best_x, q.best_u, u, fdn, flags, st, bs));
@@ -722,244 +882,93 @@ static int run_graph(void* stream, Record&& record) {
 }
 
 template <typename R>
-static int ilqr_impl(const IlqrCall<R>& q, void* stream) {
+static int ilqr_impl(const IlqrCall<R>& q, const mpcb200_mlp* mlp, void* stream) {
   const int knob = kernel_knob();
-  int rc = ilqr_check<R>(q, knob);
+  int rc = ilqr_check<R>(q, mlp, knob);
   if (rc) return rc;
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t bs = ilqr_stream(1);
-    return bs == nullptr ? MPCB200_ERR_LAUNCH : ilqr_record<R>(os, bs, q, knob);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH : ilqr_record<R>(os, bs, q, knob, mlp);
   });
 }
 
 // ---------------------------------------------------------------------------------------------
-// a learned model's network (mlp.cu): its rollout and linearisation, the split-mode step (the step kernels with
-// do_rollout = 0, then the network's line search), and the iLQR loop of MPC.forward around them
+// time-varying episodes (mpcb200_episode_window_*, mpcb200_episode_backward_window_*): each control step's window of
+// the full-length inputs is staged into fixed workspace buffers, which the episode's (or sweep's) nodes read
 // ---------------------------------------------------------------------------------------------
-static int mlp_check(const mpcb200_mlp* mlp, int B, int T, int N, int M, MlpShape& s) {
-  if (mlp == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (!mlp_shape(mlp, s)) return MPCB200_ERR_BAD_DIMS;
-  if (B <= 0 || T <= 0 || N < s.n_prev + s.ns || M < s.ms || N + M > s.p_max) return MPCB200_ERR_BAD_DIMS;
-  return MPCB200_OK;
-}
-
-template <typename R>
-static int mlp_rollout_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x_init, const R* u, R* x,
-                            void* stream) {
-  MlpShape s;
-  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
-  if (x_init == nullptr || u == nullptr || x == nullptr) return MPCB200_ERR_NULL_POINTER;
-  return counted(mlp_launch_rollout<R>(mlp, B, T, N, M, x_init, u, x, (cudaStream_t)stream));
-}
-
-template <typename R>
-static int mlp_linearize_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x, const R* u, R* F, R* f,
-                              void* stream) {
-  MlpShape s;
-  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
-  if (x == nullptr || u == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (T == 1) return MPCB200_OK;
-  if (F == nullptr || f == nullptr) return MPCB200_ERR_NULL_POINTER;
-  return counted(mlp_launch_linearize<R>(mlp, B, T, N, M, x, u, F, f, (cudaStream_t)stream));
-}
-
-// the linearisation VJP's workspace ([G, n_params] slot rows), 0 where its per-warp slice does not fit
-static size_t mlp_vjp_ws(const MlpShape& s, int B, int T, size_t sz) {
-  if (mlp_smem_bytes(mlp_vjp_shape(s), (int)sz, 1) > (size_t)kOptinAssumed) return 0;
-  return up256((size_t)mlp_vjp_slots((long long)(T - 1) * B, s.n_params) * (size_t)s.n_params * sz);
-}
-
-template <typename R>
-static int mlp_linearize_vjp_impl(const mpcb200_mlp* mlp, int B, int T, int N, int M, const R* x, const R* u,
-                                  const R* dF, const R* df, R* dtheta, void* workspace, size_t workspace_bytes,
-                                  void* stream) {
-  MlpShape s;
-  if (const int rc = mlp_check(mlp, B, T, N, M, s)) return rc;
-  if (x == nullptr || u == nullptr || dF == nullptr || df == nullptr || dtheta == nullptr || workspace == nullptr)
-    return MPCB200_ERR_NULL_POINTER;
-  const size_t need = mlp_vjp_ws(s, B, T, sizeof(R));
-  if (need == 0) return MPCB200_ERR_SMEM;
-  if (workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return MPCB200_ERR_BAD_DIMS;
-  return counted(mlp_launch_linearize_vjp<R>(mlp, B, T, N, M, x, u, dF, df, dtheta, (R*)workspace,
-                                             (cudaStream_t)stream), 2);
-}
-
-static size_t mlp_step_ws(const mpcb200_dims* d, size_t sz) {
-  const size_t TBM = (size_t)d->T * d->B * d->m;
-  return up256(TBM * d->n * sz) + up256(TBM * sz);
-}
-
-// the arguments of mpcb200_mlp_step_* after dims, params and the record, in the header's order
-template <typename R>
-struct MlpStepCall {
-  const R *C, *c, *F, *f, *x_init, *cur_x, *cur_u, *u_lower, *u_upper;
-  const uint8_t* u_zero_I;
-  R *new_x, *new_u, *costs, *alphas, *du_first;
-  int32_t* qp_iters;
-  uint8_t* free_mask;
-  int32_t* status;
+struct WindowLayout {                 // byte offsets of the window buffers, after the episode's (sweep's) workspace
+  size_t at[WINDOW_INPUTS], total;
 };
-
-// The line search's arguments; Ks, ks: the gains the step wrote.
-template <typename R>
-static MlpLsArgs<R> mlp_ls_args(const mpcb200_dims* d, const mpcb200_params* p, const MlpStepCall<R>& q, const R* Ks,
-                                const R* ks) {
-  MlpLsArgs<R> a;
-  std::memset(&a, 0, sizeof(a));
-  a.B = d->B; a.T = d->T; a.N = d->n; a.M = d->m;
-  a.bounds_kind = d->bounds_kind; a.has_mask = d->has_zero_mask ? 1 : 0; a.has_delta = d->has_delta_u ? 1 : 0;
-  a.max_ls = d->max_ls_iter;
-  const TimeStrides ts = time_strides(d);
-  a.C_ts = ts.C; a.c_ts = ts.c;
-  a.u_lo = (R)p->u_lo; a.u_hi = (R)p->u_hi; a.delta_u = (R)p->delta_u; a.decay = (R)p->ls_decay;
-  a.C = q.C; a.c = q.c; a.x_init = q.x_init; a.cur_x = q.cur_x; a.cur_u = q.cur_u; a.Ks = Ks; a.ks = ks;
-  a.u_lower = q.u_lower; a.u_upper = q.u_upper; a.zero_mask = q.u_zero_I;
-  a.new_x = q.new_x; a.new_u = q.new_u; a.costs = q.costs; a.alphas = q.alphas; a.du_first = q.du_first;
-  return a;
-}
-
-// the checks of a split-mode step that need no device, before anything is launched
-template <typename R>
-static int mlp_step_check(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp,
-                          const MlpStepCall<R>& q) {
-  int rc = check_dims(d);
-  if (rc) return rc;
-  MlpShape s;
-  if ((rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s))) return rc;
-  if (p == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr || q.cur_x == nullptr ||
-      q.cur_u == nullptr || q.new_x == nullptr || q.new_u == nullptr || q.costs == nullptr || q.alphas == nullptr)
-    return MPCB200_ERR_NULL_POINTER;
-  if (d->T > 1 && q.F == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (d->has_f && q.f == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if ((rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I))) return rc;
-  if (d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
-  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
-  return MPCB200_OK;
-}
-
-template <typename R>
-static int mlp_step_impl(const mpcb200_dims* d, const mpcb200_params* p, const mpcb200_mlp* mlp,
-                         const MlpStepCall<R>& q, void* workspace, size_t workspace_bytes, void* stream) {
-  const int knob = kernel_knob();
-  int rc = mlp_step_check<R>(d, p, mlp, q);
-  if (rc) return rc;
-  if (workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (workspace_bytes < mlp_step_ws(d, sizeof(R)) || (reinterpret_cast<uintptr_t>(workspace) & 255u) != 0)
-    return MPCB200_ERR_BAD_DIMS;
-  mpcb200_dims ds = *d;
-  ds.do_rollout = 0;
-  StepCall<R> sc = {};
-  sc.C = q.C; sc.c = q.c; sc.F = q.F; sc.f = q.f; sc.x_init = q.x_init; sc.cur_x = q.cur_x; sc.cur_u = q.cur_u;
-  sc.u_lower = q.u_lower; sc.u_upper = q.u_upper; sc.u_zero_I = q.u_zero_I;
-  sc.qp_iters = q.qp_iters; sc.free_mask = q.free_mask; sc.status = q.status;
-  sc.Ks = (R*)workspace;
-  sc.ks = (R*)((char*)workspace + up256((size_t)d->T * d->B * d->m * d->n * sizeof(R)));
-  if ((rc = step_impl<R>(&ds, p, sc, knob, stream))) return rc;
-  return counted(mlp_launch_linesearch<R>(mlp, mlp_ls_args<R>(d, p, q, sc.Ks, sc.ks), (cudaStream_t)stream));
-}
-
-// the iLQR loop's workspace: ilqr_layout's, plus the linearisation F, f and, where the step would not ask for them,
-// the gains (the split-mode step always writes them)
-static IlqrLayout ilqr_mlp_layout(const mpcb200_dims* d, size_t sz, int knob) {
-  IlqrLayout l = ilqr_layout(d, sz, knob);
-  const size_t TB = (size_t)d->T * d->B, TB1 = (size_t)(d->T - 1) * d->B;
-  const size_t n = d->n, m = d->m;
-  size_t o = l.total;
-  l.F = o; o += up256(TB1 * n * (n + m) * sz);
-  l.f = o; o += up256(TB1 * n * sz);
-  if (!l.gains) {
-    l.Ks = o; o += up256(TB * m * n * sz);
-    l.ks = o; o += up256(TB * m * sz);
-    l.gains = true;
+// d: the solve's dims.  f's buffer holds T slices (the kernels read T-1); a plant's, one
+static WindowLayout window_layout(const mpcb200_dims* d, const mpcb200_window* w, size_t base, size_t sz) {
+  WindowLayout l;
+  const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m;
+  const size_t len[WINDOW_INPUTS] = {T * B * p * p, T * B * p, (size_t)d->F_T * B * n * p, T * B * n,
+                                     T * B * m, T * B * m, B * n * p, B * n};
+  const int bit[WINDOW_INPUTS] = {MPCB200_WIN_COST, MPCB200_WIN_COST, MPCB200_WIN_DYN, MPCB200_WIN_DYN,
+                                  MPCB200_WIN_BOUNDS, MPCB200_WIN_BOUNDS, MPCB200_WIN_PLANT, MPCB200_WIN_PLANT};
+  size_t o = base;
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    l.at[a] = 0;
+    if (w->on & bit[a]) {
+      l.at[a] = o;
+      o += up256(len[a] * sz);
+    }
   }
   l.total = o;
   return l;
 }
 
-template <typename R>
-static int ilqr_mlp_check(const IlqrCall<R>& q, const mpcb200_mlp* mlp, int knob) {
-  const mpcb200_dims* d = q.d;
-  int rc = check_dims(d);
-  if (rc) return rc;
-  MlpShape s;
-  if ((rc = mlp_check(mlp, d->B, d->T, d->n, d->m, s))) return rc;
-  if (q.p == nullptr || q.o == nullptr || q.C == nullptr || q.c == nullptr || q.x_init == nullptr ||
-      q.best_x == nullptr || q.best_u == nullptr || q.best_costs == nullptr || q.best_fdn == nullptr ||
-      q.info == nullptr || q.workspace == nullptr)
-    return MPCB200_ERR_NULL_POINTER;
-  if (q.o->lqr_iter < 1 || q.o->m_ref < 1 || q.o->m_ref > d->m) return MPCB200_ERR_BAD_DIMS;
-  if (d->T < 2 || d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
-  if ((rc = check_step_options(d, q.u_lower, q.u_upper, q.u_zero_I))) return rc;
-  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
-  const IlqrLayout l = ilqr_mlp_layout(d, sizeof(R), knob);
-  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
-    return MPCB200_ERR_BAD_DIMS;
+// the window record against the caller's dims: MPCB200_WIN_COST set, each other bit only where its input can be
+// windowed, an axis that covers n_steps + T - 1 slices, and time strides of the dims convention
+static int window_check(const mpcb200_dims* d, const mpcb200_window* w, int n_steps, const mpcb200_plant* plant) {
+  if (w == nullptr) return MPCB200_ERR_NULL_POINTER;
+  const int all = MPCB200_WIN_COST | MPCB200_WIN_DYN | MPCB200_WIN_BOUNDS | MPCB200_WIN_PLANT;
+  if (!(w->on & MPCB200_WIN_COST) || (w->on & ~all) != 0) return MPCB200_ERR_BAD_DIMS;
+  if ((w->on & MPCB200_WIN_DYN) && d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
+  if ((w->on & MPCB200_WIN_BOUNDS) && d->bounds_kind != 2) return MPCB200_ERR_BAD_DIMS;
+  if ((w->on & MPCB200_WIN_PLANT) && (plant == nullptr || plant->kind != DYN_LINEAR)) return MPCB200_ERR_BAD_DIMS;
+  if (n_steps < 1 || (long long)w->L < (long long)n_steps + d->T - 1) return MPCB200_ERR_BAD_DIMS;
+  const int64_t ts[WINDOW_INPUTS] = {w->C_tstride, w->c_tstride, w->F_tstride, w->f_tstride,
+                                     w->lo_tstride, w->hi_tstride, w->Fp_tstride, w->fp_tstride};
+  for (int64_t t : ts)
+    if (t < MPCB200_TIME_INVARIANT) return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
 }
 
-// ilqr_record with the network: rollout -> linearisation -> step (no rollout) -> line search -> track -> stop
-template <typename R>
-static int ilqr_mlp_record(cudaStream_t os, cudaStream_t bs, const IlqrCall<R>& q, const mpcb200_mlp* mlp, int knob) {
-  const mpcb200_dims* d = q.d;
-  const mpcb200_ilqr_opts* o = q.o;
-  const IlqrLayout l = ilqr_mlp_layout(d, sizeof(R), knob);
-  char* ws = (char*)q.workspace;
-  R* u = (R*)(ws + l.u);
-  R* x = (R*)(ws + l.x);
-  R* F = (R*)(ws + l.F);
-  R* f = (R*)(ws + l.f);
-  R* fdn = (R*)(ws + l.fdn);
-  uint8_t* flags = (uint8_t*)(ws + l.flags);
-  IlqrState* st = (IlqrState*)(ws + l.state);
-  const int B = d->B, T = d->T, N = d->n, M = d->m;
-  cudaGraphConditionalHandle handle;
-  int rc = while_handle(os, &handle);
-  if (rc) return rc;
-  if (counted(ilqr_launch_init<R>((size_t)T * B * M, q.u_init, u, st, q.info, handle, os)) != 0)
-    return MPCB200_ERR_LAUNCH;
-  rc = open_while(os, bs, handle);
-  if (rc) return rc;
-  mpcb200_dims ds = *d;                 // the step reads the workspace F, f
-  ds.F_T = T - 1; ds.has_f = 1; ds.F_tstride = 0; ds.f_tstride = 0;
-  MlpStepCall<R> mc = {};
-  mc.C = q.C; mc.c = q.c; mc.F = F; mc.f = f; mc.x_init = q.x_init; mc.cur_x = x; mc.cur_u = u;
-  mc.u_lower = q.u_lower; mc.u_upper = q.u_upper; mc.u_zero_I = q.u_zero_I;
-  mc.new_x = (R*)(ws + l.new_x); mc.new_u = (R*)(ws + l.new_u); mc.costs = (R*)(ws + l.costs);
-  mc.alphas = (R*)(ws + l.alphas); mc.du_first = (R*)(ws + l.du_first); mc.status = (int32_t*)(ws + l.status);
-  rc = mlp_rollout_impl<R>(mlp, B, T, N, M, q.x_init, u, x, bs);
-  if (rc == 0) rc = mlp_linearize_impl<R>(mlp, B, T, N, M, x, u, F, f, bs);
-  if (rc == 0) {
-    ds.do_rollout = 0;
-    StepCall<R> sc = {};
-    sc.C = q.C; sc.c = q.c; sc.F = F; sc.f = f; sc.x_init = q.x_init; sc.cur_x = x; sc.cur_u = u;
-    sc.u_lower = q.u_lower; sc.u_upper = q.u_upper; sc.u_zero_I = q.u_zero_I; sc.status = mc.status;
-    sc.Ks = (R*)(ws + l.Ks); sc.ks = (R*)(ws + l.ks);
-    rc = step_impl<R>(&ds, q.p, sc, knob, bs);
-    if (rc == 0)
-      rc = counted(mlp_launch_linesearch<R>(mlp, mlp_ls_args<R>(&ds, q.p, mc, sc.Ks, sc.ks), bs));
-  }
-  if (rc == 0)
-    rc = counted(ilqr_launch_track<R>(B, T, N, M, o->m_ref, (R)o->best_cost_eps, mc.new_x, mc.new_u, mc.costs,
-                                      mc.du_first, mc.status, q.best_costs, q.best_x, q.best_u, u, fdn, flags, st, bs));
-  if (rc == 0)
-    rc = counted(ilqr_launch_stop<R>(B, o->lqr_iter, o->not_improved_lim, o->eps, mc.costs, fdn, flags, q.best_costs,
-                                     q.best_fdn, st, q.info, handle, bs));
-  cudaGraph_t body = nullptr;
-  if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
-  return rc;
+// the solve's dims: the caller's, with the windowed inputs read from dense buffers
+static mpcb200_dims window_solve_dims(const mpcb200_dims* d, const mpcb200_window* w) {
+  mpcb200_dims ds = *d;
+  if (w->on & MPCB200_WIN_COST) ds.C_tstride = ds.c_tstride = 0;
+  if (w->on & MPCB200_WIN_DYN) ds.F_tstride = ds.f_tstride = 0;
+  return ds;
 }
 
+// The copy of each windowed input into its staging buffer, k read from `step`.  in[a]: the call's field of input a
+// (NULL, or a NULL field: not windowed or not given), which is pointed at the buffer.  Slices: T of C, c and the
+// bounds, F_T of F, T-1 of f, 1 of the plant's F, f.
 template <typename R>
-static int ilqr_mlp_impl(const IlqrCall<R>& q, const mpcb200_mlp* mlp, void* stream) {
-  const int knob = kernel_knob();
-  int rc = ilqr_mlp_check<R>(q, mlp, knob);
-  if (rc) return rc;
-  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
-  return run_graph(stream, [&](cudaStream_t os) {
-    cudaStream_t bs = ilqr_stream(1);
-    return bs == nullptr ? MPCB200_ERR_LAUNCH : ilqr_mlp_record<R>(os, bs, q, mlp, knob);
-  });
+static WindowCopy<R> window_copy(const mpcb200_dims* d, const mpcb200_window* w, const WindowLayout& l, char* ws,
+                                 const R** const in[WINDOW_INPUTS], const int32_t* step) {
+  WindowCopy<R> c;
+  std::memset(&c, 0, sizeof(c));
+  const long long B = d->B, T = d->T, n = d->n, m = d->m, p = n + m;
+  const long long slice[WINDOW_INPUTS] = {B * p * p, B * p, B * n * p, B * n, B * m, B * m, B * n * p, B * n};
+  const int cnt[WINDOW_INPUTS] = {(int)T, (int)T, d->F_T, (int)T - 1, (int)T, (int)T, 1, 1};
+  const int64_t ts[WINDOW_INPUTS] = {w->C_tstride, w->c_tstride, w->F_tstride, w->f_tstride,
+                                     w->lo_tstride, w->hi_tstride, w->Fp_tstride, w->fp_tstride};
+  for (int a = 0; a < WINDOW_INPUTS; ++a) {
+    if (l.at[a] == 0 || in[a] == nullptr || *in[a] == nullptr) continue;
+    c.src[a] = *in[a];
+    c.dst[a] = (R*)(ws + l.at[a]);
+    c.tstride[a] = ts[a] == 0 ? slice[a] : ts[a];
+    c.slice[a] = slice[a];
+    c.n[a] = cnt[a];
+    *in[a] = c.dst[a];
+  }
+  c.k = step;
+  return c;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -969,10 +978,10 @@ struct EpisodeLayout {                // workspace carve-up: the iLQR loop's wor
   IlqrLayout ilqr;
   size_t best_x, best_u, best_costs, best_fdn, info, state, warm, traj, ep, total;
 };
-// net: the solve is a learned model's (ilqr_mlp_layout)
+// net: the solve is a learned model's
 static EpisodeLayout episode_layout(const mpcb200_dims* d, size_t sz, int knob, bool net = false) {
   EpisodeLayout l;
-  l.ilqr = net ? ilqr_mlp_layout(d, sz, knob) : ilqr_layout(d, sz, knob);
+  l.ilqr = ilqr_layout(d, sz, knob, net);
   const size_t TB = (size_t)d->T * d->B, B = d->B;
   const size_t n = d->n, m = d->m;
   size_t o = l.ilqr.total;
@@ -1056,13 +1065,8 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
       e.u_next == nullptr || e.workspace == nullptr)
     return MPCB200_ERR_NULL_POINTER;
   if (e.d->T < 3 || e.n_steps < 1) return MPCB200_ERR_BAD_DIMS;     // the warm-start shift reads u[T-3]
-  if (e.mlp != nullptr) {             // a learned model: a network that fits, without the slew-rate state
-    MlpShape s;
-    rc = mlp_check(e.mlp, e.d->B, e.d->T, e.d->n, e.d->m, s);
-    if (rc) return rc;
-    if (s.n_prev != 0) return MPCB200_ERR_BAD_DIMS;
-    if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100()) return MPCB200_ERR_SMEM;
-  }
+  MlpShape s;
+  if (e.mlp != nullptr && (rc = episode_net_check(e.d, e.mlp, sizeof(R), smem_optin_or_h100(), s))) return rc;
   if ((e.plan_x == nullptr) != (e.plan_u == nullptr)) return MPCB200_ERR_NULL_POINTER;
   if (e.plant != nullptr) {
     rc = plant_check(e.d, e.plant);
@@ -1074,13 +1078,13 @@ static int episode_check(const EpisodeCall<R>& e, int knob) {
   if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
   const IlqrCall<R> q = episode_solve(e, l);
-  return e.mlp != nullptr ? ilqr_mlp_check<R>(q, e.mlp, knob) : ilqr_check<R>(q, knob);
+  return ilqr_check<R>(q, e.mlp, knob);
 }
 
 // Adds the episode's init kernel and its `while` node over control steps (body recorded on `es`) to the graph `os`
 // is capturing.  Body: [window_stage_kernel, with wc] -> the iLQR loop (its own `while` node, body on `bs`) -> model
-// step -> [episode_plans_kernel, with plan_x / plan_u] -> episode_advance_kernel.  With e.mlp the iLQR loop is
-// ilqr_mlp_record's, and without a plant the model step is the network's rollout at T = 2.
+// step -> [episode_plans_kernel, with plan_x / plan_u] -> episode_advance_kernel.  With e.mlp the iLQR loop plans
+// with the network, and without a plant the model step is the network's rollout at T = 2.
 template <typename R>
 static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, const EpisodeCall<R>& e, int knob,
                           const WindowCopy<R>* wc = nullptr) {
@@ -1102,7 +1106,7 @@ static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, con
   rc = open_while(os, es, handle);
   if (rc) return rc;
   if (wc != nullptr) rc = counted(window_launch_stage<R>(*wc, es));
-  if (rc == 0) rc = e.mlp != nullptr ? ilqr_mlp_record<R>(es, bs, q, e.mlp, knob) : ilqr_record<R>(es, bs, q, knob);
+  if (rc == 0) rc = ilqr_record<R>(es, bs, q, knob, e.mlp);
   // the model step (the plant's, where the call names one) from the solve's best controls, by the launchers the
   // solve's rollout uses, at T = 2
   const EpisodeStep<R> s = episode_step(e);
@@ -1133,21 +1137,50 @@ static int episode_record(cudaStream_t os, cudaStream_t es, cudaStream_t bs, con
   return rc;
 }
 
+// The episode of `e`; w (mpcb200_episode_window_*, non-NULL): each control step's window of e's full-length inputs is
+// staged into workspace buffers that the episode reads.  Every argument error is reported before anything is captured.
 template <typename R>
-static int episode_impl(const EpisodeCall<R>& e, void* stream) {
+static int episode_impl(EpisodeCall<R> e, const mpcb200_window* w, void* stream) {
   const int knob = kernel_knob();
+  mpcb200_dims ds;
+  WindowCopy<R> wc;
+  if (w != nullptr) {
+    int rc = check_dims(e.d);
+    if (rc) return rc;
+    rc = window_check(e.d, w, e.n_steps, e.plant);
+    if (rc) return rc;
+    const bool has_f = e.d->has_f != 0;
+    if (e.C == nullptr || e.c == nullptr || ((w->on & MPCB200_WIN_DYN) && (e.F == nullptr || (has_f && !e.f))) ||
+        ((w->on & MPCB200_WIN_BOUNDS) && (e.u_lower == nullptr || e.u_upper == nullptr)) ||
+        ((w->on & MPCB200_WIN_PLANT) && (e.F_plant == nullptr || (e.plant->has_f && e.f_plant == nullptr))))
+      return MPCB200_ERR_NULL_POINTER;
+    ds = window_solve_dims(e.d, w);
+    const EpisodeLayout el = episode_layout(&ds, sizeof(R), knob);
+    const WindowLayout l = window_layout(&ds, w, el.total, sizeof(R));
+    if (e.workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
+    if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
+      return MPCB200_ERR_BAD_DIMS;
+    char* ws = (char*)e.workspace;
+    const R** in[WINDOW_INPUTS] = {&e.C, &e.c, &e.F, has_f ? &e.f : nullptr, &e.u_lower, &e.u_upper, &e.F_plant,
+                                   e.plant != nullptr && e.plant->has_f ? &e.f_plant : nullptr};
+    wc = window_copy<R>(&ds, w, l, ws, in, (const int32_t*)(ws + el.ep));
+    e.d = &ds;
+    e.workspace_bytes = el.total;
+  }
   int rc = episode_check<R>(e, knob);
   if (rc) return rc;
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t es = ilqr_stream(2), bs = ilqr_stream(1);
-    return es == nullptr || bs == nullptr ? MPCB200_ERR_LAUNCH : episode_record<R>(os, es, bs, e, knob);
+    return es == nullptr || bs == nullptr ? MPCB200_ERR_LAUNCH
+                                          : episode_record<R>(os, es, bs, e, knob, w != nullptr ? &wc : nullptr);
   });
 }
 
 // ---------------------------------------------------------------------------------------------
 // the reverse sweep of an episode (episode_grad.cuh): for k = n_steps-1 .. 0, the model step's VJP, each solve's KKT
-// adjoint at its best iterate (a known system: through its linearisation and that linearisation's VJP), summed
+// adjoint at its best iterate (a known system or a network: through its linearisation and that linearisation's VJP),
+// summed
 // ---------------------------------------------------------------------------------------------
 // learnable parameters of a known system (DynLearnable), 0 for anything else
 static int dyn_nparams(int kind) {
@@ -1157,10 +1190,11 @@ static int dyn_nparams(int kind) {
 }
 // a sweep's parameter count: the system's, for its passthrough kind too
 static int epgrad_nparams(int kind) { return dyn_nparams(kind & ~DYN_CTRL_PASSTHROUGH); }
-// dims of each step's adjoint: the episode's; a known system's F, f are its dense linearisation [T-1, B, ...]
-static mpcb200_dims epgrad_adjoint_dims(const mpcb200_dims* d) {
+// dims of each step's adjoint: the episode's; a known system's or the network's (net) F, f are its dense
+// linearisation [T-1, B, ...]
+static mpcb200_dims epgrad_adjoint_dims(const mpcb200_dims* d, bool net) {
   mpcb200_dims da = *d;
-  if (d->dynamics_kind != DYN_LINEAR) {
+  if (net || d->dynamics_kind != DYN_LINEAR) {
     da.F_T = d->T - 1; da.has_f = 1; da.F_tstride = 0; da.f_tstride = 0;
   }
   da.dynamics_kind = DYN_LINEAR;
@@ -1170,12 +1204,15 @@ static mpcb200_dims epgrad_adjoint_dims(const mpcb200_dims* d) {
 struct EpGradLayout {                 // workspace carve-up (byte offsets, every piece 256-byte aligned)
   mpcb200_dims da;
   size_t adj, adj_bytes, stage_x, stage_u, dl_dx, dl_du, gx, theta, dxk, dCk, dck, dFk, dfk, Fk, fk, first, second,
-      state, total;
+      dthk, vjp, vjp_bytes, state, total;
 };
-// step_kind: the kind of the step whose parameter part the stage writes (the plant's; -1: the model's)
-static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob, int step_kind = -1) {
+// step_kind: the kind of the step whose parameter part the stage writes (the plant's; -1: the model's).  net: the
+// shape of the network the episode planned with (mpcb200_episode_backward_mlp_*), or NULL; vjp_bytes is 0 where its
+// linearisation VJP does not fit.
+static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob, int step_kind = -1,
+                                  const MlpShape* net = nullptr) {
   EpGradLayout l;
-  l.da = epgrad_adjoint_dims(d);
+  l.da = epgrad_adjoint_dims(d, net != nullptr);
   const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m, TB = T * B, T1B = (T - 1) * B;
   const size_t NP = epgrad_nparams(d->dynamics_kind);
   const size_t NP_step = step_kind < 0 ? NP : (size_t)epgrad_nparams(step_kind);
@@ -1194,12 +1231,19 @@ static EpGradLayout epgrad_layout(const mpcb200_dims* d, size_t sz, int knob, in
   l.dck = o;      o += up256(TB * p * sz);
   l.dFk = o;      o += up256((size_t)l.da.F_T * B * n * p * sz);
   l.dfk = o;      o += up256(l.da.has_f ? T1B * n * sz : 0);
-  l.Fk = l.fk = l.first = l.second = 0;
-  if (known) {                        // the linearisation along the staged plan, and its VJP
+  l.Fk = l.fk = l.first = l.second = l.dthk = l.vjp = l.vjp_bytes = 0;
+  if (known || net != nullptr) {      // the linearisation along the staged plan
     l.Fk = o;     o += up256(T1B * n * p * sz);
     l.fk = o;     o += up256(T1B * n * sz);
+  }
+  if (known) {                        // a known system's linearisation VJP
     l.first = o;  o += up256(T1B * NP * sz);
     l.second = o; o += up256(T1B * NP * sz);
+  }
+  if (net != nullptr) {               // step k's weight gradient, and the network's linearisation VJP
+    l.dthk = o;   o += up256((size_t)net->n_params * sz);
+    l.vjp_bytes = mlp_vjp_ws(*net, d->B, d->T, sz);
+    l.vjp = o;    o += l.vjp_bytes;
   }
   l.state = o;    o += up256(sizeof(EpGradState));
   l.total = o;
@@ -1255,33 +1299,48 @@ static bool slew_dims_ok(const mpcb200_dims* d, int n_prev) {
          known_shape_ok(d) && dyn_kind_dims(d->dynamics_kind & ~DYN_CTRL_PASSTHROUGH, n, m) && n_prev == m;
 }
 
-// argument checks that need no device: every error is reported before anything is captured or launched
+// the model a reverse sweep takes: under a slew-rate penalty slew_dims_ok's, otherwise LinDx or a known system with
+// learnable parameters at its own shape (mpcb200_episode_backward_*)
+static bool sweep_model_ok(const mpcb200_dims* d, bool slew, int n_prev) {
+  if (slew) return slew_dims_ok(d, n_prev);
+  return d->dynamics_kind == DYN_LINEAR || (dyn_nparams(d->dynamics_kind) != 0 && known_shape_ok(d));
+}
+
+// argument checks that need no device: every error is reported before anything is captured or launched.  s: the
+// shape of q.mlp, where the call has one.
 template <typename R>
-static int epgrad_check(const EpGradCall<R>& q, int knob) {
+static int epgrad_check(const EpGradCall<R>& q, int knob, MlpShape& s) {
   const mpcb200_dims* d = q.d;
+  const bool net = q.mlp != nullptr;
   int rc = check_dims(d);
   if (rc) return rc;
   if (q.p == nullptr || q.C == nullptr || q.c == nullptr || q.xs == nullptr || q.us == nullptr ||
       q.plan_x == nullptr || q.plan_u == nullptr || q.dl_dxs == nullptr || q.dl_dus == nullptr ||
-      q.dx_init == nullptr || q.dC == nullptr || q.dc == nullptr || q.workspace == nullptr)
+      q.dx_init == nullptr || q.dC == nullptr || q.dc == nullptr || q.workspace == nullptr ||
+      (net && q.dtheta == nullptr))
     return MPCB200_ERR_NULL_POINTER;
-  if (d->T < 3 || q.n_steps < 1) return MPCB200_ERR_BAD_DIMS;
+  if (d->T < 3 || q.n_steps < 1 || (net && d->dynamics_kind != DYN_LINEAR)) return MPCB200_ERR_BAD_DIMS;
+  if (net) {                          // a network that fits, and whose linearisation VJP fits
+    rc = episode_net_check(d, q.mlp, sizeof(R), smem_optin_or_h100(), s);
+    if (rc) return rc;
+    if (mlp_vjp_ws(s, d->B, d->T, sizeof(R)) == 0) return MPCB200_ERR_SMEM;
+  }
   if (q.slew && !slew_dims_ok(d, q.n_prev)) return MPCB200_ERR_BAD_DIMS;
   rc = check_bounds(d, q.u_lower, q.u_upper);
   if (rc) return rc;
-  if (d->dynamics_kind != DYN_LINEAR) {
-    // mpcb200_episode_backward_* takes a known system itself, the slew entry its passthrough kind (slew_dims_ok)
-    if (!q.slew && (dyn_nparams(d->dynamics_kind) == 0 || !known_shape_ok(d))) return MPCB200_ERR_BAD_DIMS;
-    if (q.dtheta == nullptr) return MPCB200_ERR_NULL_POINTER;
-  } else {
-    if (q.F == nullptr || q.dF == nullptr) return MPCB200_ERR_NULL_POINTER;
-    if (d->has_f && q.df == nullptr) return MPCB200_ERR_NULL_POINTER;
+  if (!net) {
+    if (!sweep_model_ok(d, q.slew, q.n_prev)) return MPCB200_ERR_BAD_DIMS;
+    if (d->dynamics_kind != DYN_LINEAR) {
+      if (q.dtheta == nullptr) return MPCB200_ERR_NULL_POINTER;
+    } else if (q.F == nullptr || q.dF == nullptr || (d->has_f && q.df == nullptr)) {
+      return MPCB200_ERR_NULL_POINTER;
+    }
   }
   if (q.plant != nullptr) {
     rc = epgrad_plant_check(q);
     if (rc) return rc;
   }
-  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
+  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1, net ? &s : nullptr);
   if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
     return MPCB200_ERR_BAD_DIMS;
   return MPCB200_OK;
@@ -1291,21 +1350,27 @@ static int epgrad_check(const EpGradCall<R>& q, int knob) {
 // capturing.  Body: stage -> [linearisation] -> adjoint -> [linearisation VJP] -> accumulate.
 // wc, wn (mpcb200_episode_backward_window_*): window_stage_kernel first in the body, and the window forms of init,
 // stage and accumulate.
+// q.mlp, s its shape (episode_grad.cuh): dtheta's zeroing before the init kernel, and the body plan or the plant's
+// stage -> the network's linearisation -> [stage_net] -> adjoint -> [net_step_param] -> linearisation VJP -> add ->
+// accumulate.
 template <typename R>
-static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, int knob,
-                         const WindowCopy<R>* wc = nullptr, const EpWindow* wn = nullptr) {
+static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, const MlpShape& s, int knob,
+                         const WindowCopy<R>* wc, const EpWindow* wn) {
   const mpcb200_dims* d = q.d;
-  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
+  const bool net = q.mlp != nullptr;
+  const EpGradLayout l = epgrad_layout(d, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1, net ? &s : nullptr);
   char* ws = (char*)q.workspace;
   const bool known = d->dynamics_kind != DYN_LINEAR;
-  const int B = d->B, T = d->T;
+  const int B = d->B, T = d->T, N = d->n, M = d->m;
+  R* Fk = (R*)(ws + l.Fk);
+  R* fk = (R*)(ws + l.fk);
   EpGradArgs<R> a;
   std::memset(&a, 0, sizeof(a));
-  a.B = B; a.T = T; a.N = d->n; a.M = d->m; a.n_steps = q.n_steps; a.F_T = l.da.F_T; a.has_f = l.da.has_f;
-  a.kind = d->dynamics_kind; a.NP = epgrad_nparams(d->dynamics_kind);
+  a.B = B; a.T = T; a.N = N; a.M = M; a.n_steps = q.n_steps; a.F_T = l.da.F_T; a.has_f = l.da.has_f;
+  a.kind = net ? EPGRAD_KIND_NET : d->dynamics_kind; a.NP = epgrad_nparams(d->dynamics_kind);
   for (int i = 0; i < 8; ++i) a.dp.p[i] = q.p->dyn[i];
   a.xs = q.xs; a.us = q.us; a.plan_x = q.plan_x; a.plan_u = q.plan_u; a.dl_dxs = q.dl_dxs; a.dl_dus = q.dl_dus;
-  a.F = known ? nullptr : q.F;
+  a.F = net ? Fk : known ? nullptr : q.F;         // the network's: slice 0 is the model step's Jacobian at (x_k, u_k)
   a.stage_x = (R*)(ws + l.stage_x); a.stage_u = (R*)(ws + l.stage_u);
   a.dl_dx = (R*)(ws + l.dl_dx); a.dl_du = (R*)(ws + l.dl_du);
   a.gx = (R*)(ws + l.gx); a.theta_step = known ? (R*)(ws + l.theta) : nullptr;
@@ -1336,11 +1401,15 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
     as.theta_step = pknown ? (R*)(ws + l.theta) : nullptr;
     pl.kind = as.kind; pl.has_f = as.has_f; pl.NP = as.NP; pl.theta_step = as.theta_step;
     pl.dF = as.dF; pl.df = as.df; pl.dtheta = pknown ? q.dtheta_plant : nullptr; pl.dw = q.dw;
+  } else if (net && q.dw != nullptr) {  // the network steps a disturbed loop: the plant forms write dw, nothing else
+    pl.kind = EPGRAD_KIND_NET;
+    pl.dw = q.dw;
   }
-  const EpPlantArgs<R>* plp = q.plant != nullptr ? &pl : nullptr;
+  const EpPlantArgs<R>* plp = q.plant != nullptr || (net && q.dw != nullptr) ? &pl : nullptr;
   cudaGraphConditionalHandle handle;
   int rc = while_handle(os, &handle);
   if (rc) return rc;
+  if (net && counted(launch_fill_zero<R>((size_t)s.n_params, q.dtheta, os)) != 0) return MPCB200_ERR_LAUNCH;
   if (counted(wn != nullptr ? epgrad_launch_init_window<R>(a, q.n_prev, plp, *wn, handle, os)
                             : epgrad_launch_init<R>(a, q.n_prev, plp, handle, os)) != 0)
     return MPCB200_ERR_LAUNCH;
@@ -1348,17 +1417,27 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   if (rc) return rc;
   if (wc != nullptr) rc = counted(window_launch_stage<R>(*wc, bs));
   if (rc == 0)
-    rc = counted(wn != nullptr ? epgrad_launch_stage_window<R>(as, *wn, bs) : epgrad_launch_stage<R>(as, bs));
-  const R* F = q.F;
-  if (rc == 0 && known) {
-    F = (const R*)(ws + l.Fk);
-    rc = dyn_impl<R>(true, d->dynamics_kind, q.p->dyn, B, T, a.stage_x, a.stage_u, nullptr, (R*)(ws + l.Fk),
-                     (R*)(ws + l.fk), bs);
+    rc = counted(net && q.plant == nullptr ? epgrad_launch_plan<R>(a, bs)
+                 : wn != nullptr           ? epgrad_launch_stage_window<R>(as, *wn, bs)
+                                           : epgrad_launch_stage<R>(as, bs));
+  if (rc == 0 && net) {
+    rc = mlp_linearize_impl<R>(q.mlp, B, T, N, M, a.stage_x, a.stage_u, Fk, fk, bs);
+    if (rc == 0 && q.plant == nullptr) rc = counted(epgrad_launch_stage_net<R>(a, bs));
+  } else if (rc == 0 && known) {
+    rc = dyn_impl<R>(true, d->dynamics_kind, q.p->dyn, B, T, a.stage_x, a.stage_u, nullptr, Fk, fk, bs);
   }
   if (rc == 0)
-    rc = adjoint_impl<R>(&l.da, q.p, q.C, q.c, F, a.stage_x, a.stage_u, a.dl_dx, a.dl_du, q.u_lower, q.u_upper, dxk,
-                         dCk, dck, dFk, dfk, ws + l.adj, l.adj_bytes, knob, bs, true);
-  if (rc == 0 && known && !q.slew) {
+    rc = adjoint_impl<R>(&l.da, q.p, q.C, q.c, net || known ? Fk : q.F, a.stage_x, a.stage_u, a.dl_dx, a.dl_du,
+                         q.u_lower, q.u_upper, dxk, dCk, dck, dFk, dfk, ws + l.adj, l.adj_bytes, knob, bs, true);
+  if (rc == 0 && net) {
+    R* dthk = (R*)(ws + l.dthk);
+    // the network's own step: with (dJ, df) = (g z^T, g) the VJP's G^ = dJ - df z^T is 0, so it returns d<g, x'>/dtheta
+    if (q.plant == nullptr) rc = counted(epgrad_launch_net_step_param<R>(a, dFk, dfk, bs));
+    if (rc == 0)
+      rc = mlp_linearize_vjp_impl<R>(q.mlp, B, T, N, M, a.stage_x, a.stage_u, dFk, dfk, dthk, ws + l.vjp, l.vjp_bytes,
+                                     bs);
+    if (rc == 0) rc = counted(epgrad_launch_add<R>((size_t)s.n_params, dthk, q.dtheta, bs));
+  } else if (rc == 0 && known && !q.slew) {
     rc = dyn_vjp_impl<R>(d->dynamics_kind, q.p->dyn, B, T, a.stage_x, a.stage_u, dFk, dfk, first, second, bs);
   } else if (rc == 0 && known) {
     DynVjpArgs v;
@@ -1375,345 +1454,53 @@ static int epgrad_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& 
   return rc;
 }
 
+// The sweep of `q`; w (mpcb200_episode_backward_window_*, non-NULL): each control step's window of q's full-length
+// inputs is staged into workspace buffers that the sweep reads.  Every argument error is reported before anything is
+// captured.
 template <typename R>
-static int epgrad_impl(const EpGradCall<R>& q, void* stream) {
+static int epgrad_impl(EpGradCall<R> q, const mpcb200_window* w, void* stream) {
   const int knob = kernel_knob();
-  int rc = epgrad_check<R>(q, knob);
-  if (rc) return rc;
-  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
-  return run_graph(stream, [&](cudaStream_t os) {
-    cudaStream_t bs = ilqr_stream(2);
-    return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_record<R>(os, bs, q, knob);
-  });
-}
-
-// ---------------------------------------------------------------------------------------------
-// the reverse sweep of an episode planned with a learned model (mpcb200_episode_backward_mlp_*, episode_grad.cuh):
-// per step the network's linearisation along the staged plan, the model step's VJP from its slice 0 (or the plant's
-// stage), the KKT adjoint, and the linearisation's VJP in the weights summed into dtheta
-// ---------------------------------------------------------------------------------------------
-// dims of the network's linearisation, which the adjoint reads: F [T-1, B, n, p] and f [T-1, B, n], dense
-static mpcb200_dims epgrad_net_dims(const mpcb200_dims* d) {
-  mpcb200_dims dn = *d;
-  dn.F_T = d->T - 1; dn.has_f = 1; dn.F_tstride = 0; dn.f_tstride = 0;
-  return dn;
-}
-
-struct EpNetLayout {                  // epgrad_layout's carve-up at epgrad_net_dims, then the network's buffers
-  EpGradLayout g;
-  size_t Fk, fk, dthk, vjp, vjp_bytes, total;
-};
-// step_kind: the plant's kind, -1 when the network steps the loop; vjp_bytes 0 where its VJP does not fit
-static EpNetLayout epgrad_net_layout(const mpcb200_dims* d, const MlpShape& s, size_t sz, int knob, int step_kind) {
-  EpNetLayout l;
-  const mpcb200_dims dn = epgrad_net_dims(d);
-  l.g = epgrad_layout(&dn, sz, knob, step_kind);
-  const size_t T1B = (size_t)(d->T - 1) * d->B, n = d->n, p = (size_t)d->n + d->m;
-  size_t o = l.g.total;
-  l.Fk = o;   o += up256(T1B * n * p * sz);       // the linearisation along the staged plan
-  l.fk = o;   o += up256(T1B * n * sz);
-  l.dthk = o; o += up256((size_t)s.n_params * sz);  // step k's weight gradient
-  l.vjp_bytes = mlp_vjp_ws(s, d->B, d->T, sz);
-  l.vjp = o;  o += l.vjp_bytes;
-  l.total = o;
-  return l;
-}
-
-// argument checks that need no device: every error is reported before anything is captured or launched
-template <typename R>
-static int epgrad_mlp_check(const EpGradCall<R>& q, int knob, MlpShape& s) {
-  const mpcb200_dims* d = q.d;
-  int rc = check_dims(d);
-  if (rc) return rc;
-  if (q.mlp == nullptr || q.p == nullptr || q.C == nullptr || q.c == nullptr || q.xs == nullptr ||
-      q.us == nullptr || q.plan_x == nullptr || q.plan_u == nullptr || q.dl_dxs == nullptr || q.dl_dus == nullptr ||
-      q.dx_init == nullptr || q.dC == nullptr || q.dc == nullptr || q.dtheta == nullptr || q.workspace == nullptr)
-    return MPCB200_ERR_NULL_POINTER;
-  if (d->T < 3 || q.n_steps < 1 || d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
-  rc = mlp_check(q.mlp, d->B, d->T, d->n, d->m, s);
-  if (rc) return rc;
-  if (s.n_prev != 0) return MPCB200_ERR_BAD_DIMS;
-  if (mlp_smem_bytes(s, sizeof(R), 1) > (size_t)smem_optin_or_h100() || mlp_vjp_ws(s, d->B, d->T, sizeof(R)) == 0)
-    return MPCB200_ERR_SMEM;
-  rc = check_bounds(d, q.u_lower, q.u_upper);
-  if (rc) return rc;
-  if (q.plant != nullptr) {
-    rc = epgrad_plant_check(q);
-    if (rc) return rc;
-  }
-  const EpNetLayout l = epgrad_net_layout(d, s, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
-  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
-    return MPCB200_ERR_BAD_DIMS;
-  return MPCB200_OK;
-}
-
-// Adds dtheta's zeroing, the init kernel and the `while` node over k = n_steps-1 .. 0 (body recorded on `bs`) to the
-// graph `os` is capturing.  Body (episode_grad.cuh): plan or the plant's stage -> linearisation -> [stage_net] ->
-// adjoint -> [net_step_param] -> linearisation VJP -> add -> accumulate.
-template <typename R>
-static int epgrad_mlp_record(cudaStream_t os, cudaStream_t bs, const EpGradCall<R>& q, const MlpShape& s, int knob) {
-  const mpcb200_dims* d = q.d;
-  const EpNetLayout l = epgrad_net_layout(d, s, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
-  const EpGradLayout& lg = l.g;
-  char* ws = (char*)q.workspace;
-  const int B = d->B, T = d->T, N = d->n, M = d->m;
-  R* Fk = (R*)(ws + l.Fk);
-  R* fk = (R*)(ws + l.fk);
-  R* dthk = (R*)(ws + l.dthk);
-  R* dxk = (R*)(ws + lg.dxk);
-  R* dCk = (R*)(ws + lg.dCk);
-  R* dck = (R*)(ws + lg.dck);
-  R* dFk = (R*)(ws + lg.dFk);
-  R* dfk = (R*)(ws + lg.dfk);
-  EpGradArgs<R> a;
-  std::memset(&a, 0, sizeof(a));
-  a.B = B; a.T = T; a.N = N; a.M = M; a.n_steps = q.n_steps; a.F_T = lg.da.F_T; a.has_f = 1;
-  a.kind = EPGRAD_KIND_NET; a.NP = 0;
-  a.xs = q.xs; a.us = q.us; a.plan_x = q.plan_x; a.plan_u = q.plan_u; a.dl_dxs = q.dl_dxs; a.dl_dus = q.dl_dus;
-  a.F = Fk;                           // slice 0: the Jacobian of the model step at (x_k, u_k)
-  a.stage_x = (R*)(ws + lg.stage_x); a.stage_u = (R*)(ws + lg.stage_u);
-  a.dl_dx = (R*)(ws + lg.dl_dx); a.dl_du = (R*)(ws + lg.dl_du);
-  a.gx = (R*)(ws + lg.gx);
-  a.g = q.dx_init;
-  a.dx_k = dxk; a.dC_k = dCk; a.dc_k = dck; a.dF_k = dFk; a.df_k = dfk;
-  a.dC = q.dC; a.dc = q.dc;
-  a.st = (EpGradState*)(ws + lg.state);
-  // a plant's stage: a copy of `a` with its kind, parameters, F and parameter-part outputs (as epgrad_record)
-  EpGradArgs<R> as = a;
-  EpPlantArgs<R> pl;
-  std::memset(&pl, 0, sizeof(pl));
-  if (q.plant != nullptr) {
-    const bool pknown = q.plant->kind != DYN_LINEAR;
-    as.kind = q.plant->kind; as.has_f = q.plant->has_f; as.NP = epgrad_nparams(q.plant->kind);
-    for (int i = 0; i < 8; ++i) as.dp.p[i] = q.plant->dyn[i];
-    as.F = pknown ? nullptr : q.F_plant;
-    as.dF = pknown ? nullptr : q.dF_plant;
-    as.df = pknown || !q.plant->has_f ? nullptr : q.df_plant;
-    as.theta_step = pknown ? (R*)(ws + lg.theta) : nullptr;
-    pl.kind = as.kind; pl.has_f = as.has_f; pl.NP = as.NP; pl.theta_step = as.theta_step;
-    pl.dF = as.dF; pl.df = as.df; pl.dtheta = pknown ? q.dtheta_plant : nullptr; pl.dw = q.dw;
-  } else if (q.dw != nullptr) {       // the network steps a disturbed loop: the plant forms write dw, nothing else
-    pl.kind = EPGRAD_KIND_NET;
-    pl.dw = q.dw;
-  }
-  const EpPlantArgs<R>* plp = q.plant != nullptr || q.dw != nullptr ? &pl : nullptr;
-  cudaGraphConditionalHandle handle;
-  int rc = while_handle(os, &handle);
-  if (rc) return rc;
-  if (counted(launch_fill_zero<R>((size_t)s.n_params, q.dtheta, os)) != 0 ||
-      counted(epgrad_launch_init<R>(a, 0, plp, handle, os)) != 0)
-    return MPCB200_ERR_LAUNCH;
-  rc = open_while(os, bs, handle);
-  if (rc) return rc;
-  rc = counted(q.plant != nullptr ? epgrad_launch_stage<R>(as, bs) : epgrad_launch_plan<R>(a, bs));
-  if (rc == 0) rc = mlp_linearize_impl<R>(q.mlp, B, T, N, M, a.stage_x, a.stage_u, Fk, fk, bs);
-  if (rc == 0 && q.plant == nullptr) rc = counted(epgrad_launch_stage_net<R>(a, bs));
-  if (rc == 0)
-    rc = adjoint_impl<R>(&lg.da, q.p, q.C, q.c, Fk, a.stage_x, a.stage_u, a.dl_dx, a.dl_du, q.u_lower, q.u_upper,
-                         dxk, dCk, dck, dFk, dfk, ws + lg.adj, lg.adj_bytes, knob, bs, true);
-  // the network's own step: with (dJ, df) = (g z^T, g) the VJP's G^ = dJ - df z^T is 0, so it returns d<g, x'>/dtheta
-  if (rc == 0 && q.plant == nullptr) rc = counted(epgrad_launch_net_step_param<R>(a, dFk, dfk, bs));
-  if (rc == 0)
-    rc = mlp_linearize_vjp_impl<R>(q.mlp, B, T, N, M, a.stage_x, a.stage_u, dFk, dfk, dthk, ws + l.vjp, l.vjp_bytes,
-                                   bs);
-  if (rc == 0) rc = counted(epgrad_launch_add<R>((size_t)s.n_params, dthk, q.dtheta, bs));
-  if (rc == 0) rc = counted(epgrad_launch_accum<R>(a, 0, plp, handle, bs));
-  cudaGraph_t body = nullptr;
-  if (cudaStreamEndCapture(bs, &body) != cudaSuccess && rc == 0) rc = MPCB200_ERR_LAUNCH;
-  return rc;
-}
-
-template <typename R>
-static int epgrad_mlp_impl(const EpGradCall<R>& q, void* stream) {
-  const int knob = kernel_knob();
-  MlpShape s;
-  int rc = epgrad_mlp_check<R>(q, knob, s);
-  if (rc) return rc;
-  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
-  return run_graph(stream, [&](cudaStream_t os) {
-    cudaStream_t bs = ilqr_stream(2);
-    return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_mlp_record<R>(os, bs, q, s, knob);
-  });
-}
-
-// ---------------------------------------------------------------------------------------------
-// time-varying episodes (mpcb200_episode_window_*, mpcb200_episode_backward_window_*): each control step's window of
-// the full-length inputs is staged into fixed workspace buffers, which the episode's (or sweep's) nodes read
-// ---------------------------------------------------------------------------------------------
-enum { WIN_C, WIN_c, WIN_F, WIN_f, WIN_LO, WIN_HI, WIN_FP, WIN_FPF };
-struct WindowLayout {                 // byte offsets of the window buffers, after the episode's (sweep's) workspace
-  size_t at[WINDOW_INPUTS], total;
-};
-// d: the solve's dims.  f's buffer holds T slices (the kernels read T-1); a plant's, one
-static WindowLayout window_layout(const mpcb200_dims* d, const mpcb200_window* w, size_t base, size_t sz) {
-  WindowLayout l;
-  const size_t B = d->B, T = d->T, n = d->n, m = d->m, p = n + m;
-  const size_t len[WINDOW_INPUTS] = {T * B * p * p, T * B * p, (size_t)d->F_T * B * n * p, T * B * n,
-                                     T * B * m, T * B * m, B * n * p, B * n};
-  const int bit[WINDOW_INPUTS] = {MPCB200_WIN_COST, MPCB200_WIN_COST, MPCB200_WIN_DYN, MPCB200_WIN_DYN,
-                                  MPCB200_WIN_BOUNDS, MPCB200_WIN_BOUNDS, MPCB200_WIN_PLANT, MPCB200_WIN_PLANT};
-  size_t o = base;
-  for (int a = 0; a < WINDOW_INPUTS; ++a) {
-    l.at[a] = 0;
-    if (w->on & bit[a]) {
-      l.at[a] = o;
-      o += up256(len[a] * sz);
-    }
-  }
-  l.total = o;
-  return l;
-}
-
-// the window record against the caller's dims: MPCB200_WIN_COST set, each other bit only where its input can be
-// windowed, an axis that covers n_steps + T - 1 slices, and time strides of the dims convention
-static int window_check(const mpcb200_dims* d, const mpcb200_window* w, int n_steps, const mpcb200_plant* plant) {
-  if (w == nullptr) return MPCB200_ERR_NULL_POINTER;
-  const int all = MPCB200_WIN_COST | MPCB200_WIN_DYN | MPCB200_WIN_BOUNDS | MPCB200_WIN_PLANT;
-  if (!(w->on & MPCB200_WIN_COST) || (w->on & ~all) != 0) return MPCB200_ERR_BAD_DIMS;
-  if ((w->on & MPCB200_WIN_DYN) && d->dynamics_kind != DYN_LINEAR) return MPCB200_ERR_BAD_DIMS;
-  if ((w->on & MPCB200_WIN_BOUNDS) && d->bounds_kind != 2) return MPCB200_ERR_BAD_DIMS;
-  if ((w->on & MPCB200_WIN_PLANT) && (plant == nullptr || plant->kind != DYN_LINEAR)) return MPCB200_ERR_BAD_DIMS;
-  if (n_steps < 1 || (long long)w->L < (long long)n_steps + d->T - 1) return MPCB200_ERR_BAD_DIMS;
-  const int64_t ts[WINDOW_INPUTS] = {w->C_tstride, w->c_tstride, w->F_tstride, w->f_tstride,
-                                     w->lo_tstride, w->hi_tstride, w->Fp_tstride, w->fp_tstride};
-  for (int64_t t : ts)
-    if (t < MPCB200_TIME_INVARIANT) return MPCB200_ERR_BAD_DIMS;
-  return MPCB200_OK;
-}
-
-// the solve's dims: the caller's, with the windowed inputs read from dense buffers
-static mpcb200_dims window_solve_dims(const mpcb200_dims* d, const mpcb200_window* w) {
-  mpcb200_dims ds = *d;
-  if (w->on & MPCB200_WIN_COST) ds.C_tstride = ds.c_tstride = 0;
-  if (w->on & MPCB200_WIN_DYN) ds.F_tstride = ds.f_tstride = 0;
-  return ds;
-}
-
-// The copy of each windowed input (src NULL: not windowed or not given), k read from `step`.  Slices: T of C, c and
-// the bounds, F_T of F, T-1 of f, 1 of the plant's F, f.
-template <typename R>
-static WindowCopy<R> window_copy(const mpcb200_dims* d, const mpcb200_window* w, const WindowLayout& l, char* ws,
-                                 const R* const src[WINDOW_INPUTS], const int32_t* step) {
-  WindowCopy<R> c;
-  std::memset(&c, 0, sizeof(c));
-  const long long B = d->B, T = d->T, n = d->n, m = d->m, p = n + m;
-  const long long slice[WINDOW_INPUTS] = {B * p * p, B * p, B * n * p, B * n, B * m, B * m, B * n * p, B * n};
-  const int cnt[WINDOW_INPUTS] = {(int)T, (int)T, d->F_T, (int)T - 1, (int)T, (int)T, 1, 1};
-  const int64_t ts[WINDOW_INPUTS] = {w->C_tstride, w->c_tstride, w->F_tstride, w->f_tstride,
-                                     w->lo_tstride, w->hi_tstride, w->Fp_tstride, w->fp_tstride};
-  for (int a = 0; a < WINDOW_INPUTS; ++a) {
-    if (l.at[a] == 0 || src[a] == nullptr) continue;
-    c.src[a] = src[a];
-    c.dst[a] = (R*)(ws + l.at[a]);
-    c.tstride[a] = ts[a] == 0 ? slice[a] : ts[a];
-    c.slice[a] = slice[a];
-    c.n[a] = cnt[a];
-  }
-  c.k = step;
-  return c;
-}
-
-// e: the call with the full-length pointers.  Every argument error is reported before anything is captured.
-template <typename R>
-static int episode_window_impl(const EpisodeCall<R>& e, const mpcb200_window* w, void* stream) {
-  const int knob = kernel_knob();
-  if (e.d == nullptr) return MPCB200_ERR_NULL_POINTER;
-  int rc = check_dims(e.d);
-  if (rc) return rc;
-  rc = window_check(e.d, w, e.n_steps, e.plant);
-  if (rc) return rc;
-  const bool has_f = e.d->has_f != 0;
-  if (e.C == nullptr || e.c == nullptr || ((w->on & MPCB200_WIN_DYN) && (e.F == nullptr || (has_f && !e.f))) ||
-      ((w->on & MPCB200_WIN_BOUNDS) && (e.u_lower == nullptr || e.u_upper == nullptr)) ||
-      ((w->on & MPCB200_WIN_PLANT) && (e.F_plant == nullptr || (e.plant->has_f && e.f_plant == nullptr))))
-    return MPCB200_ERR_NULL_POINTER;
-  const mpcb200_dims ds = window_solve_dims(e.d, w);
-  const EpisodeLayout el = episode_layout(&ds, sizeof(R), knob);
-  const WindowLayout l = window_layout(&ds, w, el.total, sizeof(R));
-  if (e.workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (e.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(e.workspace) & 255u) != 0)
-    return MPCB200_ERR_BAD_DIMS;
-  char* ws = (char*)e.workspace;
-  const R* src[WINDOW_INPUTS] = {e.C, e.c, e.F, has_f ? e.f : nullptr, e.u_lower, e.u_upper, e.F_plant,
-                                 e.plant != nullptr && e.plant->has_f ? e.f_plant : nullptr};
-  const WindowCopy<R> wc = window_copy<R>(&ds, w, l, ws, src, (const int32_t*)(ws + el.ep));
-  EpisodeCall<R> es = e;              // the episode on the window buffers
-  es.d = &ds;
-  es.workspace_bytes = el.total;
-  for (int a = 0; a < WINDOW_INPUTS; ++a) {
-    if (wc.src[a] == nullptr) continue;
-    const R* buf = wc.dst[a];
-    switch (a) {
-      case WIN_C: es.C = buf; break;
-      case WIN_c: es.c = buf; break;
-      case WIN_F: es.F = buf; break;
-      case WIN_f: es.f = buf; break;
-      case WIN_LO: es.u_lower = buf; break;
-      case WIN_HI: es.u_upper = buf; break;
-      case WIN_FP: es.F_plant = buf; break;
-      default: es.f_plant = buf; break;
-    }
-  }
-  rc = episode_check<R>(es, knob);
-  if (rc) return rc;
-  if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
-  return run_graph(stream, [&](cudaStream_t os) {
-    cudaStream_t s2 = ilqr_stream(2), s1 = ilqr_stream(1);
-    return s2 == nullptr || s1 == nullptr ? MPCB200_ERR_LAUNCH : episode_record<R>(os, s2, s1, es, knob, &wc);
-  });
-}
-
-// the sweep's layout base: epgrad_layout of the solve's dims, with the plant's kind
-static size_t epgrad_window_base(const mpcb200_dims* ds, const mpcb200_plant* plant, size_t sz, int knob) {
-  return epgrad_layout(ds, sz, knob, plant != nullptr ? plant->kind : -1).total;
-}
-
-template <typename R>
-static int epgrad_window_impl(const EpGradCall<R>& q, const mpcb200_window* w, void* stream) {
-  const int knob = kernel_knob();
-  if (q.d == nullptr) return MPCB200_ERR_NULL_POINTER;
-  int rc = check_dims(q.d);
-  if (rc) return rc;
-  rc = window_check(q.d, w, q.n_steps, q.plant);
-  if (rc) return rc;
-  if (q.C == nullptr || q.c == nullptr || ((w->on & MPCB200_WIN_DYN) && q.F == nullptr) ||
-      ((w->on & MPCB200_WIN_BOUNDS) && (q.u_lower == nullptr || q.u_upper == nullptr)) ||
-      ((w->on & MPCB200_WIN_PLANT) && q.F_plant == nullptr))
-    return MPCB200_ERR_NULL_POINTER;
-  if (q.d->T < 3) return MPCB200_ERR_BAD_DIMS;
-  const mpcb200_dims ds = window_solve_dims(q.d, w);
-  const size_t base = epgrad_window_base(&ds, q.plant, sizeof(R), knob);
-  const WindowLayout l = window_layout(&ds, w, base, sizeof(R));
-  if (q.workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
-  if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
-    return MPCB200_ERR_BAD_DIMS;
-  char* ws = (char*)q.workspace;
-  const EpGradLayout gl = epgrad_layout(&ds, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
-  const R* src[WINDOW_INPUTS] = {q.C, q.c, q.F, nullptr, q.u_lower, q.u_upper, q.F_plant, nullptr};
-  const WindowCopy<R> wc = window_copy<R>(&ds, w, l, ws, src, (const int32_t*)(ws + gl.state));
-  EpGradCall<R> qs = q;               // the sweep on the window buffers
-  qs.d = &ds;
-  qs.workspace_bytes = base;
-  if (wc.src[WIN_C] != nullptr) qs.C = wc.dst[WIN_C];
-  if (wc.src[WIN_c] != nullptr) qs.c = wc.dst[WIN_c];
-  if (wc.src[WIN_F] != nullptr) qs.F = wc.dst[WIN_F];
-  if (wc.src[WIN_LO] != nullptr) qs.u_lower = wc.dst[WIN_LO];
-  if (wc.src[WIN_HI] != nullptr) qs.u_upper = wc.dst[WIN_HI];
-  if (wc.src[WIN_FP] != nullptr) qs.F_plant = wc.dst[WIN_FP];
-  rc = epgrad_check<R>(qs, knob);
-  if (rc) return rc;
+  mpcb200_dims ds;
+  WindowCopy<R> wc;
   EpWindow wn;
-  wn.cost = 1;
-  wn.dyn = (w->on & MPCB200_WIN_DYN) != 0;
-  wn.step = q.plant != nullptr ? (w->on & MPCB200_WIN_PLANT) != 0 : wn.dyn;
-  wn.L = w->L;
-  wn.LF = w->L - ds.T + ds.F_T;
-  wn.Lf = w->L - 1;
-  wn.Lp = w->L - 1;
+  if (w != nullptr) {
+    int rc = check_dims(q.d);
+    if (rc) return rc;
+    rc = window_check(q.d, w, q.n_steps, q.plant);
+    if (rc) return rc;
+    if (q.C == nullptr || q.c == nullptr || ((w->on & MPCB200_WIN_DYN) && q.F == nullptr) ||
+        ((w->on & MPCB200_WIN_BOUNDS) && (q.u_lower == nullptr || q.u_upper == nullptr)) ||
+        ((w->on & MPCB200_WIN_PLANT) && q.F_plant == nullptr))
+      return MPCB200_ERR_NULL_POINTER;
+    if (q.d->T < 3) return MPCB200_ERR_BAD_DIMS;
+    ds = window_solve_dims(q.d, w);
+    const EpGradLayout gl = epgrad_layout(&ds, sizeof(R), knob, q.plant != nullptr ? q.plant->kind : -1);
+    const WindowLayout l = window_layout(&ds, w, gl.total, sizeof(R));
+    if (q.workspace == nullptr) return MPCB200_ERR_NULL_POINTER;
+    if (q.workspace_bytes < l.total || (reinterpret_cast<uintptr_t>(q.workspace) & 255u) != 0)
+      return MPCB200_ERR_BAD_DIMS;
+    char* ws = (char*)q.workspace;
+    const R** in[WINDOW_INPUTS] = {&q.C, &q.c, &q.F, nullptr, &q.u_lower, &q.u_upper, &q.F_plant, nullptr};
+    wc = window_copy<R>(&ds, w, l, ws, in, (const int32_t*)(ws + gl.state));
+    q.d = &ds;
+    q.workspace_bytes = gl.total;
+    wn.cost = 1;
+    wn.dyn = (w->on & MPCB200_WIN_DYN) != 0;
+    wn.step = q.plant != nullptr ? (w->on & MPCB200_WIN_PLANT) != 0 : wn.dyn;
+    wn.L = w->L;
+    wn.LF = w->L - ds.T + ds.F_T;
+    wn.Lf = w->L - 1;
+    wn.Lp = w->L - 1;
+  }
+  MlpShape s;
+  int rc = epgrad_check<R>(q, knob, s);
+  if (rc) return rc;
   if (max_smem_optin() <= 0) return MPCB200_ERR_NO_DEVICE;
   return run_graph(stream, [&](cudaStream_t os) {
     cudaStream_t bs = ilqr_stream(2);
-    return bs == nullptr ? MPCB200_ERR_LAUNCH : epgrad_record<R>(os, bs, qs, knob, &wc, &wn);
+    return bs == nullptr ? MPCB200_ERR_LAUNCH
+                         : epgrad_record<R>(os, bs, q, s, knob, w != nullptr ? &wc : nullptr,
+                                            w != nullptr ? &wn : nullptr);
   });
 }
 }  // namespace mpcb200
@@ -1819,7 +1606,7 @@ int mpcb200_dyn_linearize_vjp_f64(int32_t kind, const double* dyn, int32_t B, in
 size_t mpcb200_ilqr_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
   if (dims == nullptr || opts == nullptr || check_dims(dims) != 0 || (elem_size != 4 && elem_size != 8)) return 0;
   if (dims->dynamics_kind != DYN_LINEAR && !known_shape_ok(dims)) return 0;
-  return ilqr_layout(dims, (size_t)elem_size, kernel_knob()).total;
+  return ilqr_layout(dims, (size_t)elem_size, kernel_knob(), false).total;
 }
 int mpcb200_ilqr_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
                      const float* C, const float* c, const float* F, const float* f, const float* x_init,
@@ -1828,7 +1615,7 @@ int mpcb200_ilqr_f32(const mpcb200_dims* dims, const mpcb200_params* params, con
                      void* workspace, size_t workspace_bytes, void* stream) {
   return ilqr_impl<float>({dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
                            best_costs, best_full_du_norm, info, workspace, workspace_bytes},
-                          stream);
+                          nullptr, stream);
 }
 int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
                      const double* C, const double* c, const double* F, const double* f, const double* x_init,
@@ -1837,7 +1624,7 @@ int mpcb200_ilqr_f64(const mpcb200_dims* dims, const mpcb200_params* params, con
                      void* workspace, size_t workspace_bytes, void* stream) {
   return ilqr_impl<double>({dims, params, opts, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, best_x, best_u,
                             best_costs, best_full_du_norm, info, workspace, workspace_bytes},
-                           stream);
+                           nullptr, stream);
 }
 
 size_t mpcb200_episode_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
@@ -1851,7 +1638,7 @@ int mpcb200_episode_f32(const mpcb200_dims* dims, const mpcb200_params* params, 
                         void* workspace, size_t workspace_bytes, void* stream) {
   return episode_impl<float>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs,
                               us, costs, info, u_next, workspace, workspace_bytes},
-                             stream);
+                             nullptr, stream);
 }
 int mpcb200_episode_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
                         int32_t n_steps, const double* C, const double* c, const double* F, const double* f,
@@ -1860,7 +1647,7 @@ int mpcb200_episode_f64(const mpcb200_dims* dims, const mpcb200_params* params, 
                         void* workspace, size_t workspace_bytes, void* stream) {
   return episode_impl<double>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I,
                                xs, us, costs, info, u_next, workspace, workspace_bytes},
-                              stream);
+                              nullptr, stream);
 }
 
 int mpcb200_episode_plans_f32(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
@@ -1872,7 +1659,7 @@ int mpcb200_episode_plans_f32(const mpcb200_dims* dims, const mpcb200_params* pa
   if (plan_x == nullptr || plan_u == nullptr) return MPCB200_ERR_NULL_POINTER;
   return episode_impl<float>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs,
                               us, costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u},
-                             stream);
+                             nullptr, stream);
 }
 int mpcb200_episode_plans_f64(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,
                               int32_t n_steps, const double* C, const double* c, const double* F, const double* f,
@@ -1883,12 +1670,12 @@ int mpcb200_episode_plans_f64(const mpcb200_dims* dims, const mpcb200_params* pa
   if (plan_x == nullptr || plan_u == nullptr) return MPCB200_ERR_NULL_POINTER;
   return episode_impl<double>({dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I,
                                xs, us, costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u},
-                              stream);
+                              nullptr, stream);
 }
 
 size_t mpcb200_episode_backward_workspace_bytes(const mpcb200_dims* dims, int32_t elem_size) {
   if (dims == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8)) return 0;
-  if (dims->dynamics_kind != DYN_LINEAR && (dyn_nparams(dims->dynamics_kind) == 0 || !known_shape_ok(dims))) return 0;
+  if (!sweep_model_ok(dims, false, 0)) return 0;
   return epgrad_layout(dims, (size_t)elem_size, kernel_knob()).total;
 }
 int mpcb200_episode_backward_f32(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
@@ -1899,7 +1686,7 @@ int mpcb200_episode_backward_f32(const mpcb200_dims* dims, const mpcb200_params*
                                  size_t workspace_bytes, void* stream) {
   return epgrad_impl<float>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,
                              dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes},
-                            stream);
+                            nullptr, stream);
 }
 int mpcb200_episode_backward_f64(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
                                  const double* C, const double* c, const double* F, const double* u_lower,
@@ -1909,12 +1696,12 @@ int mpcb200_episode_backward_f64(const mpcb200_dims* dims, const mpcb200_params*
                                  size_t workspace_bytes, void* stream) {
   return epgrad_impl<double>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,
                               dl_dus, dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes},
-                             stream);
+                             nullptr, stream);
 }
 
 size_t mpcb200_episode_backward_slew_workspace_bytes(const mpcb200_dims* dims, int32_t n_prev, int32_t elem_size) {
   if (dims == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8)) return 0;
-  if (!slew_dims_ok(dims, n_prev)) return 0;
+  if (!sweep_model_ok(dims, true, n_prev)) return 0;
   return epgrad_layout(dims, (size_t)elem_size, kernel_knob()).total;
 }
 int mpcb200_episode_backward_slew_f32(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
@@ -1925,7 +1712,7 @@ int mpcb200_episode_backward_slew_f32(const mpcb200_dims* dims, const mpcb200_pa
                                       float* dtheta, void* workspace, size_t workspace_bytes, void* stream) {
   return epgrad_impl<float>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,
                              dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, true, n_prev},
-                            stream);
+                            nullptr, stream);
 }
 int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_params* params, int32_t n_steps,
                                       int32_t n_prev, const double* C, const double* c, const double* F,
@@ -1936,7 +1723,7 @@ int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_pa
                                       size_t workspace_bytes, void* stream) {
   return epgrad_impl<double>({dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,
                               dl_dus, dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, true, n_prev},
-                             stream);
+                             nullptr, stream);
 }
 
 #define MPCB200_EPISODE_PLANT(SUF, R)                                                                              \
@@ -1950,7 +1737,7 @@ int mpcb200_episode_backward_slew_f64(const mpcb200_dims* dims, const mpcb200_pa
     if (plant == nullptr) return MPCB200_ERR_NULL_POINTER;                                                         \
     EpisodeCall<R> e = {dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs, us, \
                         costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u, plant, F_plant, f_plant, w}; \
-    return episode_impl<R>(e, stream);                                                                             \
+    return episode_impl<R>(e, nullptr, stream);                                                                    \
   }
 MPCB200_EPISODE_PLANT(f32, float)
 MPCB200_EPISODE_PLANT(f64, double)
@@ -1960,9 +1747,7 @@ size_t mpcb200_episode_backward_plant_workspace_bytes(const mpcb200_dims* dims, 
                                                       const mpcb200_plant* plant, int32_t elem_size) {
   if (dims == nullptr || plant == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8))
     return 0;
-  if (n_prev != 0 ? !slew_dims_ok(dims, n_prev)
-                  : dims->dynamics_kind != DYN_LINEAR && (dyn_nparams(dims->dynamics_kind) == 0 || !known_shape_ok(dims)))
-    return 0;
+  if (!sweep_model_ok(dims, n_prev != 0, n_prev)) return 0;
   if (plant_check(dims, plant) != 0) return 0;
   return epgrad_layout(dims, (size_t)elem_size, kernel_knob(), plant->kind).total;
 }
@@ -1978,7 +1763,7 @@ size_t mpcb200_episode_backward_plant_workspace_bytes(const mpcb200_dims* dims, 
     EpGradCall<R> q = {dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,   \
                        dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, n_prev > 0, n_prev, plant,     \
                        F_plant, dF_plant, df_plant, dtheta_plant, dw};                                             \
-    return epgrad_impl<R>(q, stream);                                                                              \
+    return epgrad_impl<R>(q, nullptr, stream);                                                                     \
   }
 MPCB200_EPISODE_BACKWARD_PLANT(f32, float)
 MPCB200_EPISODE_BACKWARD_PLANT(f64, double)
@@ -2002,7 +1787,8 @@ size_t mpcb200_episode_window_workspace_bytes(const mpcb200_dims* dims, const mp
                                    void* workspace, size_t workspace_bytes, void* stream) {                        \
     EpisodeCall<R> e = {dims, params, opts, n_steps, C, c, F, f, x_init, u_init, u_lower, u_upper, u_zero_I, xs, us, \
                         costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u, plant, F_plant, f_plant, w}; \
-    return episode_window_impl<R>(e, window, stream);                                                              \
+    if (window == nullptr) return null_record(dims);                                                               \
+    return episode_impl<R>(e, window, stream);                                                                     \
   }
 MPCB200_EPISODE_WINDOW(f32, float)
 MPCB200_EPISODE_WINDOW(f64, double)
@@ -2014,13 +1800,12 @@ size_t mpcb200_episode_backward_window_workspace_bytes(const mpcb200_dims* dims,
   if (dims == nullptr || window == nullptr || check_dims(dims) != 0 || dims->T < 3 || n_prev < 0 ||
       (elem_size != 4 && elem_size != 8))
     return 0;
-  if (n_prev != 0 ? !slew_dims_ok(dims, n_prev)
-                  : dims->dynamics_kind != DYN_LINEAR && (dyn_nparams(dims->dynamics_kind) == 0 || !known_shape_ok(dims)))
-    return 0;
+  if (!sweep_model_ok(dims, n_prev != 0, n_prev)) return 0;
   if (plant != nullptr && plant_check(dims, plant) != 0) return 0;
   const mpcb200_dims ds = window_solve_dims(dims, window);
   const int knob = kernel_knob();
-  return window_layout(&ds, window, epgrad_window_base(&ds, plant, (size_t)elem_size, knob), (size_t)elem_size).total;
+  const size_t base = epgrad_layout(&ds, (size_t)elem_size, knob, plant != nullptr ? plant->kind : -1).total;
+  return window_layout(&ds, window, base, (size_t)elem_size).total;
 }
 #define MPCB200_EPISODE_BACKWARD_WINDOW(SUF, R)                                                                    \
   int mpcb200_episode_backward_window_##SUF(                                                                       \
@@ -2033,7 +1818,8 @@ size_t mpcb200_episode_backward_window_workspace_bytes(const mpcb200_dims* dims,
     EpGradCall<R> q = {dims, params, n_steps, C, c, F, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs, dl_dus,   \
                        dx_init, dC, dc, dF, df, dtheta, workspace, workspace_bytes, n_prev > 0, n_prev, plant,     \
                        F_plant, dF_plant, df_plant, dtheta_plant, dw};                                             \
-    return epgrad_window_impl<R>(q, window, stream);                                                               \
+    if (window == nullptr) return null_record(dims);                                                               \
+    return epgrad_impl<R>(q, window, stream);                                                                      \
   }
 MPCB200_EPISODE_BACKWARD_WINDOW(f32, float)
 MPCB200_EPISODE_BACKWARD_WINDOW(f64, double)
@@ -2044,9 +1830,7 @@ size_t mpcb200_episode_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb2
   MlpShape s;
   if (dims == nullptr || opts == nullptr || check_dims(dims) != 0 || dims->T < 3 || (elem_size != 4 && elem_size != 8))
     return 0;
-  if (mlp_check(mlp, dims->B, dims->T, dims->n, dims->m, s) != 0 || s.n_prev != 0 ||
-      mlp_smem_bytes(s, elem_size, 1) > (size_t)kOptinAssumed)
-    return 0;
+  if (episode_net_check(dims, mlp, elem_size, kOptinAssumed, s) != 0) return 0;
   return episode_layout(dims, (size_t)elem_size, kernel_knob(), true).total;
 }
 #define MPCB200_EPISODE_MLP(SUF, R)                                                                                \
@@ -2060,7 +1844,7 @@ size_t mpcb200_episode_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb2
     EpisodeCall<R> e = {dims, params, opts, n_steps, C, c, nullptr, nullptr, x_init, u_init, u_lower, u_upper,     \
                         u_zero_I, xs, us, costs, info, u_next, workspace, workspace_bytes, plan_x, plan_u, plant,  \
                         F_plant, f_plant, w, mlp};                                                                 \
-    return episode_impl<R>(e, stream);                                                                             \
+    return episode_impl<R>(e, nullptr, stream);                                                                    \
   }
 MPCB200_EPISODE_MLP(f32, float)
 MPCB200_EPISODE_MLP(f64, double)
@@ -2072,11 +1856,9 @@ size_t mpcb200_episode_backward_mlp_workspace_bytes(const mpcb200_dims* dims, co
   if (dims == nullptr || check_dims(dims) != 0 || dims->T < 3 || dims->dynamics_kind != DYN_LINEAR ||
       (elem_size != 4 && elem_size != 8))
     return 0;
-  if (mlp_check(mlp, dims->B, dims->T, dims->n, dims->m, s) != 0 || s.n_prev != 0 ||
-      mlp_smem_bytes(s, elem_size, 1) > (size_t)kOptinAssumed)
-    return 0;
+  if (episode_net_check(dims, mlp, elem_size, kOptinAssumed, s) != 0) return 0;
   if (plant != nullptr && (plant_check(dims, plant) != 0 || (plant->kind & DYN_CTRL_PASSTHROUGH) != 0)) return 0;
-  const EpNetLayout l = epgrad_net_layout(dims, s, (size_t)elem_size, kernel_knob(), plant != nullptr ? plant->kind : -1);
+  const EpGradLayout l = epgrad_layout(dims, (size_t)elem_size, kernel_knob(), plant != nullptr ? plant->kind : -1, &s);
   return l.vjp_bytes == 0 ? 0 : l.total;
 }
 #define MPCB200_EPISODE_BACKWARD_MLP(SUF, R)                                                                       \
@@ -2086,10 +1868,11 @@ size_t mpcb200_episode_backward_mlp_workspace_bytes(const mpcb200_dims* dims, co
       const R* us, const R* plan_x, const R* plan_u, const R* dl_dxs, const R* dl_dus, R* dx_init, R* dC, R* dc,    \
       R* dtheta, R* dF_plant, R* df_plant, R* dtheta_plant, R* dw, void* workspace, size_t workspace_bytes,        \
       void* stream) {                                                                                              \
+    if (mlp == nullptr) return null_record(dims);                                                                  \
     EpGradCall<R> q = {dims, params, n_steps, C, c, nullptr, u_lower, u_upper, xs, us, plan_x, plan_u, dl_dxs,     \
                        dl_dus, dx_init, dC, dc, nullptr, nullptr, dtheta, workspace, workspace_bytes, false, 0,    \
                        plant, F_plant, dF_plant, df_plant, dtheta_plant, dw, mlp};                                 \
-    return epgrad_mlp_impl<R>(q, stream);                                                                          \
+    return epgrad_impl<R>(q, nullptr, stream);                                                                     \
   }
 MPCB200_EPISODE_BACKWARD_MLP(f32, float)
 MPCB200_EPISODE_BACKWARD_MLP(f64, double)
@@ -2112,7 +1895,7 @@ size_t mpcb200_mlp_step_workspace_bytes(const mpcb200_dims* dims, int32_t elem_s
 size_t mpcb200_ilqr_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_ilqr_opts* opts, int32_t elem_size) {
   if (check_dims(dims) != MPCB200_OK || opts == nullptr || dims->T < 2 || (elem_size != 4 && elem_size != 8))
     return 0;
-  return ilqr_mlp_layout(dims, (size_t)elem_size, kernel_knob()).total;
+  return ilqr_layout(dims, (size_t)elem_size, kernel_knob(), true).total;
 }
 #define MPCB200_MLP_ENTRIES(sfx, R)                                                                                    \
   int mpcb200_mlp_rollout_##sfx(const mpcb200_mlp* mlp, int32_t B, int32_t T, int32_t N, int32_t M, const R* x_init,  \
@@ -2135,7 +1918,7 @@ size_t mpcb200_ilqr_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_
                              int32_t* status, void* workspace, size_t workspace_bytes, void* stream) {                 \
     return mlp_step_impl<R>(dims, params, mlp,                                                                         \
                             {C, c, F, f, x_init, cur_x, cur_u, u_lower, u_upper, u_zero_I, new_x, new_u, costs,        \
-                             alphas, du_first, qp_iters, free_mask, status},                                           \
+                             nullptr, alphas, du_first, qp_iters, free_mask, status},                                  \
                             workspace, workspace_bytes, stream);                                                       \
   }                                                                                                                    \
   int mpcb200_ilqr_mlp_##sfx(const mpcb200_dims* dims, const mpcb200_params* params, const mpcb200_ilqr_opts* opts,   \
@@ -2143,9 +1926,10 @@ size_t mpcb200_ilqr_mlp_workspace_bytes(const mpcb200_dims* dims, const mpcb200_
                              const R* u_lower, const R* u_upper, const uint8_t* u_zero_I, R* best_x, R* best_u,        \
                              R* best_costs, R* best_full_du_norm, int32_t* info, void* workspace,                      \
                              size_t workspace_bytes, void* stream) {                                                   \
-    return ilqr_mlp_impl<R>({dims, params, opts, C, c, nullptr, nullptr, x_init, u_init, u_lower, u_upper, u_zero_I,   \
-                             best_x, best_u, best_costs, best_full_du_norm, info, workspace, workspace_bytes},         \
-                            mlp, stream);                                                                              \
+    if (mlp == nullptr) return null_record(dims);                                                                     \
+    return ilqr_impl<R>({dims, params, opts, C, c, nullptr, nullptr, x_init, u_init, u_lower, u_upper, u_zero_I,       \
+                         best_x, best_u, best_costs, best_full_du_norm, info, workspace, workspace_bytes},             \
+                        mlp, stream);                                                                                  \
   }
 MPCB200_MLP_ENTRIES(f32, float)
 MPCB200_MLP_ENTRIES(f64, double)
