@@ -443,6 +443,38 @@ def mpc_forward_lin(n_state, n_ctrl, T, x_init, C, c, F, f, u_lower=None, u_uppe
     return best["x"], best["u"], best["costs"], best["full_du_norm"]
 
 
+def ilqr_loop(n_state, n_ctrl, T, x_init, C, c, rollout, linearize, dynamics, u_init=None, lqr_iter=10, eps=1e-7,
+              not_improved_lim=5, best_cost_eps=1e-4, **step_kw):
+    """MPC.forward's iterations (mpc/mpc.py:244-301) with QuadCost(C, c) and nonlinear dynamics given as callables:
+    x = rollout(u) [T, B, n] from x_init, (F, f) = linearize(x, u), and x_{t+1} = dynamics(x_t, u_t), the line search's
+    true dynamics in lqr_step_forward.  Best-iterate tracking and the stop test as mpc_forward_lin's.  n_state is the
+    (augmented) state count; step_kw: lqr_step_forward's options.  Returns (x, u, costs, iterations)."""
+    B = x_init.shape[0]
+    u = torch.zeros(T, B, n_ctrl, dtype=torch.float64) if u_init is None else u_init.clone()
+    best, n_not_improved, it = None, 0, 0
+    for it in range(1, lqr_iter + 1):
+        x = rollout(u)
+        F, f = linearize(x, u)
+        o = lqr_step_forward(n_state, n_ctrl, T, x_init, C, c, F, f, x, u, dynamics=dynamics, **step_kw)
+        x, u = o.new_x, o.new_u
+        n_not_improved += 1
+        if best is None:
+            best = {"x": x, "u": u, "costs": o.costs, "fdn": o.full_du_norm}
+            any_better = False
+        else:
+            better = o.costs <= best["costs"] + best_cost_eps
+            sel = better.view(1, -1, 1)
+            best = {"x": torch.where(sel, x, best["x"]), "u": torch.where(sel, u, best["u"]),
+                    "costs": torch.where(better, o.costs, best["costs"]),
+                    "fdn": torch.where(better, o.full_du_norm, best["fdn"])}
+            any_better = bool(better.any())
+        if any_better:
+            n_not_improved = 0
+        if float(o.full_du_norm.max()) < eps or n_not_improved > not_improved_lim:
+            break
+    return best["x"], best["u"], best["costs"], it
+
+
 # ----------------------------------------------------------------------------
 # receding-horizon episodes (the notebooks' loop, examples/*.ipynb) and their reverse sweep
 # ----------------------------------------------------------------------------

@@ -88,32 +88,9 @@ def ilqr(n, m, T, x_init, C, c, layers, act, passthrough, u_init=None, u_lower=N
          eps=1e-7, not_improved_lim=5, best_cost_eps=1e-4, n_prev=0, **step_kw):
     """MPC.forward's iterations (mpc/mpc.py:244-301) with QuadCost(C, c) and the network: rollout, linearisation,
     lqr_step_forward with the network as the line search's dynamics, best-iterate tracking and the stop test.  n is
-    the (augmented) state count.  Returns (x, u, costs, iterations)."""
-    B = x_init.shape[0]
-    u = torch.zeros(T, B, m, dtype=torch.float64) if u_init is None else u_init.clone()
-
-    def dyn(x, uu):
-        return step(layers, act, passthrough, x, uu, n_prev)
-    best, n_not_improved, it = None, 0, 0
-    for it in range(1, lqr_iter + 1):
-        x = rollout(layers, act, passthrough, x_init, u, n_prev)
-        F, f = linearize(layers, act, passthrough, x, u, n_prev)
-        o = lo.lqr_step_forward(n, m, T, x_init, C, c, F, f, x, u, u_lower=u_lower, u_upper=u_upper,
-                                dynamics=dyn, **step_kw)
-        x, u = o.new_x, o.new_u
-        n_not_improved += 1
-        if best is None:
-            best = {"x": x, "u": u, "costs": o.costs, "fdn": o.full_du_norm}
-            any_better = False
-        else:
-            better = o.costs <= best["costs"] + best_cost_eps
-            sel = better.view(1, -1, 1)
-            best = {"x": torch.where(sel, x, best["x"]), "u": torch.where(sel, u, best["u"]),
-                    "costs": torch.where(better, o.costs, best["costs"]),
-                    "fdn": torch.where(better, o.full_du_norm, best["fdn"])}
-            any_better = bool(better.any())
-        if any_better:
-            n_not_improved = 0
-        if float(o.full_du_norm.max()) < eps or n_not_improved > not_improved_lim:
-            break
-    return best["x"], best["u"], best["costs"], it
+    the (augmented) state count.  The loop is lqr_oracle.ilqr_loop.  Returns (x, u, costs, iterations)."""
+    return lo.ilqr_loop(n, m, T, x_init, C, c, lambda uu: rollout(layers, act, passthrough, x_init, uu, n_prev),
+                        lambda x, uu: linearize(layers, act, passthrough, x, uu, n_prev),
+                        lambda x, uu: step(layers, act, passthrough, x, uu, n_prev), u_init=u_init, lqr_iter=lqr_iter,
+                        eps=eps, not_improved_lim=not_improved_lim, best_cost_eps=best_cost_eps, u_lower=u_lower,
+                        u_upper=u_upper, **step_kw)

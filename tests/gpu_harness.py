@@ -629,6 +629,66 @@ def check_clamps(tag, r, o, kw, keep=None):
                            _cols(o.new_u.double() == b.double(), keep)), f"{tag}: {side} clamp mask"
 
 
+def on_bounds(u, kw, sel=lambda t: t):
+    """[2, T, B, m]: which controls u [T, B, m] sit on the lower / upper bound; tensor bounds go through sel (the
+    batch rows u holds)."""
+    lo_, hi = (sel(kw[k]) if torch.is_tensor(kw[k]) else torch.full_like(u.double(), kw[k]) for k in ("u_lower",
+                                                                                                    "u_upper"))
+    return torch.stack((u.double() == lo_.double(), u.double() == hi.double()))
+
+
+def check_loop_departures(tag, r, o64, o32, kw, lqr_iter, sensitive, dtype, idx=None):
+    """x, u and costs of a device iLQR loop per problem against the oracle's loop (x, u, costs, iterations), under
+    test_ilqr_oracle_gpu.check_loop's rule.  A problem departs where its x or u misses the tolerance (float64 1e-9 x
+    scale; float32 4x the float32 oracle's own error plus 1e-6 x scale), or where its controls on a bound differ from
+    the oracle's.  Only bounded loops of more than one iteration may have departing problems, at most one in four:
+    pnqp's |dx| >= 1e-4 stop decides some problems' paths by round-off.  Where more depart, each one beyond that
+    allowance must be a problem whose float64 oracle loop itself moves under a 1e-15 relative change of C
+    (sensitive(tol) -> [B] of the oracle's batch).  float32 problems the float32 oracle itself departs on are left out.
+    Costs of the rest by `within`; under u_zero_I the masked controls exactly 0.  idx: the oracle's batch rows that
+    r holds.  Returns (tag, departing problems, compared problems, largest x / u error of the kept problems relative
+    to the scale)."""
+    sel = (lambda t: t) if idx is None else (lambda t: t[idx] if t.dim() == 1 else t[:, idx])
+    x64, u64, c64 = (sel(t) for t in o64[:3])
+    B = x64.shape[1]
+    bounded = "u_lower" in kw
+    sc = max(1.0, float(x64.abs().max()), float(u64.abs().max()))
+    per = lambda a, b: (a.double() - b.double()).abs().amax((0, 2))  # noqa: E731
+    differ = lambda a, b: (on_bounds(a, kw, sel) != on_bounds(b, kw, sel)).any(3).any(1).any(0)  # noqa: E731
+    err = torch.maximum(per(r["x"], x64), per(r["u"], u64))
+    out = torch.zeros(B, dtype=torch.bool)
+    if o32 is None:
+        tol = tol_for(F64, False)["xu"] * sc
+    else:
+        x32, u32 = sel(o32[0]), sel(o32[1])
+        e32 = torch.maximum(per(x32, x64), per(u32, u64))
+        out = e32 > 1e-4 * sc
+        if bounded:
+            out |= differ(u32, u64)
+        assert not bool(out.all()), f"{tag}: no comparable problem"
+        tol = 4 * float(e32[~out].max()) + 1e-6 * sc
+    dep = err > tol
+    if bounded:
+        dep |= differ(r["u"], u64)
+    dep &= ~out
+    n_dep, n_cmp = int(dep.sum()), int((~out).sum())
+    report = (tag, n_dep, n_cmp)
+    allowed = max(1, n_cmp // 4) if bounded and lqr_iter > 1 else 0
+    unexplained = n_dep
+    if n_dep > allowed and allowed > 0 and o32 is None:
+        unexplained = int((dep & ~sel(sensitive(tol))).sum())
+        report = (tag + f" ({n_dep - unexplained} the oracle's own round-off moves)", n_dep, n_cmp)
+    assert unexplained <= allowed, (f"{tag}: {n_dep} of {n_cmp} depart, {unexplained} of them where the oracle is "
+                                    f"not round-off sensitive (allowed {allowed}), max err {float(err.max()):.3e} "
+                                    f"tolerance {tol:.3e}")
+    keep = ~(out | dep)
+    within(tag, "costs", r["costs"][keep], c64[keep], None if o32 is None else sel(o32[2])[keep].double(), dtype)
+    if "u_zero_I" in kw:
+        mask = kw["u_zero_I"] if idx is None else kw["u_zero_I"][:, idx]
+        assert bool((r["u"][mask] == 0).all()), f"{tag}: masked controls"
+    return report + (float(err[keep].max()) / sc,)
+
+
 @functools.lru_cache(maxsize=16)
 def adjoint_case(seed, B, T, n, m, dtype, bounds, with_f, F_T=None):
     """A solved problem (one oracle step from u = 0, so box bounds leave an active set), upstream gradients,

@@ -35,6 +35,7 @@ from oracle import lqr_oracle as lo
 from oracle import mlp_oracle as mo
 from oracle import receding_mlp_oracle as rmo
 from tests.gpu_harness import (DT, F32, F64, INSTANCES, LS_MARGIN, MAX, MID, ONE, ORACLE_TMAX, PAIR_SHAPES,
+                               check_loop_departures, on_bounds,
                                kernel_env, layout_batches, ls_classes, ls_layout, misaligned, plan,
                                plan_str, pool_size, probe_step, rollout_passes, round_through, staged, switches,
                                tol_for, within)
@@ -798,7 +799,7 @@ def loop_case(seed, B, T, n, m, dtype, mode, lqr_iter=3, n_prev=0, time_invarian
                         **kw, **opts)
             moved |= torch.maximum((o[0] - o64[0]).abs().amax((0, 2)), (o[1] - o64[1]).abs().amax((0, 2))) > tol
             if "u_lower" in kw:
-                moved |= (_on_bounds(o[1], kw, lambda t: t) != _on_bounds(o64[1], kw, lambda t: t)).any(3).any(1).any(0)
+                moved |= (on_bounds(o[1], kw) != on_bounds(o64[1], kw)).any(3).any(1).any(0)
         return moved
     return net, P, kw, opts, o64, o32, sensitive
 
@@ -821,62 +822,13 @@ def run_mlp_loop(net, n, m, T, P, kw, opts, dtype, impl=None, n_prev=0, idx=None
     return {k: v.cpu() for k, v in res.items()}, p
 
 
-def _on_bounds(u, kw, sel):
-    """[B]-indexable [2, T, B, m]: which controls sit on the lower / upper bound."""
-    lo_, hi = (sel(kw[k]) if torch.is_tensor(kw[k]) else torch.full_like(u.double(), kw[k]) for k in ("u_lower",
-                                                                                                    "u_upper"))
-    return torch.stack((u.double() == lo_.double(), u.double() == hi.double()))
-
-
 def check_mlp_loop(tag, r, case, dtype, idx=None):
-    """x, u and costs per problem against the oracle, under test_ilqr_oracle_gpu.check_loop's rule.  A problem
-    departs where its x or u misses the tolerance (float64 1e-9 x scale; float32 4x the float32 oracle's own error
-    plus 1e-6 x scale), or where its controls on a bound differ from the oracle's.  Only bounded loops of more than
-    one iteration may have departing problems, at most one in four: pnqp's |dx| >= 1e-4 stop decides some problems'
-    paths by round-off.  Where more depart, each one beyond that allowance must be a problem whose float64 oracle
-    loop itself moves under a 1e-15 relative change of C (at (16, 4) T = 101 and (18, 5) with tensor bounds that is
-    5 of 8 and 7 of 16 problems, by up to 1e-4).  float32 problems the float32 oracle itself departs on are left out.
-    Costs of the rest by `within`, and the iteration count."""
+    """x, u and costs per problem against the oracle under gpu_harness.check_loop_departures (at (16, 4) T = 101 and
+    (18, 5) with tensor bounds, 5 of 8 and 7 of 16 problems depart where the oracle's own loop moves, by up to 1e-4),
+    and the iteration count."""
     _, P, kw, opts, o64, o32, sensitive = case
-    sel = (lambda t: t) if idx is None else (lambda t: t[idx] if t.dim() == 1 else t[:, idx])
-    x64, u64, c64 = (sel(t) for t in o64[:3])
-    B = x64.shape[1]
-    bounded = "u_lower" in kw
-    sc = max(1.0, float(x64.abs().max()), float(u64.abs().max()))
-    per = lambda a, b: (a.double() - b.double()).abs().amax((0, 2))  # noqa: E731
-    differ = lambda a, b: (_on_bounds(a, kw, sel) != _on_bounds(b, kw, sel)).any(3).any(1).any(0)  # noqa: E731
-    err = torch.maximum(per(r["x"], x64), per(r["u"], u64))
-    out = torch.zeros(B, dtype=torch.bool)
-    if o32 is None:
-        tol = tol_for(F64, False)["xu"] * sc
-    else:
-        x32, u32 = sel(o32[0]), sel(o32[1])
-        e32 = torch.maximum(per(x32, x64), per(u32, u64))
-        out = e32 > 1e-4 * sc
-        if bounded:
-            out |= differ(u32, u64)
-        assert not bool(out.all()), f"{tag}: no comparable problem"
-        tol = 4 * float(e32[~out].max()) + 1e-6 * sc
-    dep = err > tol
-    if bounded:
-        dep |= differ(r["u"], u64)
-    dep &= ~out
-    n_dep, n_cmp = int(dep.sum()), int((~out).sum())
-    LOOP_DEPARTED.append((tag, n_dep, n_cmp))
-    allowed = max(1, n_cmp // 4) if bounded and opts["lqr_iter"] > 1 else 0
-    unexplained = n_dep
-    if n_dep > allowed and allowed > 0 and o32 is None:
-        unexplained = int((dep & ~sel(sensitive(tol))).sum())
-        LOOP_DEPARTED[-1] = (tag + f" ({n_dep - unexplained} the oracle's own round-off moves)", n_dep, n_cmp)
-    assert unexplained <= allowed, (f"{tag}: {n_dep} of {n_cmp} depart, {unexplained} of them where the oracle is "
-                                    f"not round-off sensitive (allowed {allowed}), max err {float(err.max()):.3e} "
-                                    f"tolerance {tol:.3e}")
-    keep = ~(out | dep)
-    within(tag, "costs", r["costs"][keep], c64[keep], None if o32 is None else sel(o32[2])[keep].double(), dtype)
+    LOOP_DEPARTED.append(check_loop_departures(tag, r, o64, o32, kw, opts["lqr_iter"], sensitive, dtype, idx)[:3])
     assert int(r["info"][0]) == opts["lqr_iter"], f"{tag}: {int(r['info'][0])} iterations"
-    if "u_zero_I" in kw:
-        mask = kw["u_zero_I"] if idx is None else kw["u_zero_I"][:, idx]
-        assert bool((r["u"][mask] == 0).all()), f"{tag}: masked controls"
 
 
 @functools.lru_cache(maxsize=None)

@@ -19,8 +19,9 @@ Cases: LinDx at every compiled instance and a padded shape, with batch tails and
 several passes; every step plan of the solve on both sides of its switch horizon (tests/gpu_harness.pick_switch);
 every adjoint route of the sweep's body; the input forms (bounds, u_zero_I, F_T, f, a time-invariant F and a
 time-invariant cost, which reach the library as stride-0 views over time); the known systems, whose sweep is checked
-against the oracle's per-problem parameter gradient and whose forward, for want of a known-system iLQR oracle, only
-for consistency (check_known_forward) and end to end against the reference's fixture; and poisoned workspaces, where
+against the oracle's per-problem parameter gradient and whose forward for consistency (check_known_forward) and end to
+end against the reference's fixture (tests/test_known_oracle_gpu.py compares it with oracle/known_oracle.py's
+episode); and poisoned workspaces, where
 every workspace byte and output starts at 0xFF and the results must be bitwise those of an unpoisoned call.
 test_zz_coverage fails if a plan or route never ran."""
 import functools
@@ -390,9 +391,10 @@ def check_known_forward(tag, r, mod, theta, clamp, dtype):
 @pytest.mark.parametrize("name", KNOWN)
 def test_known_systems(name, B, dtype):
     """The known system's sweep (stage kernel's model-step VJP, linearisation, three-launch adjoint, linearisation
-    VJP) against the oracle's on the device's own plans; dtheta per problem.  Controls reach the clamp.  The oracle
-    has no known-system iLQR loop, so the forward is checked for consistency (check_known_forward) and, for the
-    optimality of its plans, only end to end against the reference (test_known_against_reference_fixture)."""
+    VJP) against the oracle's on the device's own plans; dtheta per problem.  Controls reach the clamp.  The forward
+    is checked here for consistency (check_known_forward: the model step and the plans' rollouts) and end to end
+    against the reference (test_known_against_reference_fixture); tests/test_known_oracle_gpu.py checks its plans
+    against known_oracle's iLQR loop."""
     T, n_steps, seed = 10, 3, 800 + B + KNOWN.index(name)
     mod, n, m, P, kw, dyn, theta = episode_known_inputs(name, B, T, dtype, seed)
     opts = dict(fixed_opts(4), linesearch_decay=mod.linesearch_decay, max_linesearch_iter=mod.max_linesearch_iter)
