@@ -990,9 +990,10 @@ def _owned_alloc(poison, nan_outputs):
 def abi_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_upper=None, u_zero_I=None,
                 delta_u=None, linesearch_decay=0.2, max_linesearch_iter=10, lqr_iter=10, not_improved_lim=5,
                 eps=1e-7, best_cost_eps=1e-4, dyn=None, poison=False, n_prev=0, plant=None, w=None,
-                nan_outputs=False):
+                nan_outputs=False, window=None):
     """step.episode_raw(..., keep_plans=True): the call its staging makes (step._stage_episode: mpcb200_episode_plans_*,
-    or mpcb200_episode_plant_* with a plant or w), with caller-owned outputs and workspace.  poison: every workspace
+    mpcb200_episode_plant_* with a plant or w, mpcb200_episode_window_* with window = L, the time-varying episode
+    whose inputs lie on the axis of L slices), with caller-owned outputs and workspace.  poison: every workspace
     byte and every output starts at 0xFF, so a kernel that reads an element nothing wrote reads NaN (or info -1);
     nan_outputs: the outputs alone start at 0xFF, so an element the call does not write comes back NaN (or -1).
     n_prev: a slew-rate penalty's augmented problem, recorded in the staged problem for abi_episode_backward.  plant
@@ -1008,7 +1009,7 @@ def abi_episode(n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower=None, u_up
     s, name, args, out = S._stage_episode(
         n, m, T, n_steps, x_init, C, c, F, f, u_init, u_lower, u_upper, u_zero_I, delta_u, linesearch_decay,
         max_linesearch_iter, lqr_iter, not_improved_lim, eps, best_cost_eps, dyn=dyn, keep_plans=True, n_prev=n_prev,
-        plant=plant, w=w, alloc=_owned_alloc(poison, nan_outputs))
+        plant=plant, w=w, window=window, alloc=_owned_alloc(poison, nan_outputs))
     before = L.launch_count()
     rc = S._call(name, C.dtype, DEV, args)
     launches, p = L.launch_count() - before, L.last_step_plan()
@@ -1106,13 +1107,16 @@ def check_episode_forward(tag, r, o64, o32, kw, dtype, several):
     return float(err[keep].max()) / sc, n_dep, n_cmp
 
 
-def episode_linear_inputs(seed, B, T, n, m, dtype, mode, F_T=None, f_T="T-1", time_invariant=()):
+def episode_linear_inputs(seed, B, T, n, m, dtype, mode, F_T=None, f_T="T-1", time_invariant=(), L=None):
     """A LinDx episode's inputs, float64 rounded through dtype, and the solver's problem options: (P, kw).
     mode: plain | box (+-0.25) | tensor (tensor box) | boxT (tensor box + delta_u) | mask (u_zero_I).  F_T = T: F has
     T slices; f_T: "none", "T-1" or "T" slices of f.  time_invariant: names among "F", "C", "c" whose slices all
     equal slice 0; P holds them dense (what the oracle takes), and P["time_invariant"] names them, so that
-    episode_device_inputs hands them over as stride-0 views over time made on the device."""
-    C, c, F, f, x0 = gen_problem(seed, B, T, n, m, F64)
+    episode_device_inputs hands them over as stride-0 views over time made on the device.
+    L: a time-varying episode's axis (episode_raw(..., window=L)): C, c and tensor bounds have L slices, F and f L-1
+    (L with F_T = T, f_T = "T"), each slice its own (F too); u_zero_I stays the solve's [T, B, m]."""
+    Ta = T if L is None else L
+    C, c, F, f, x0 = gen_problem(seed, B, Ta, n, m, F64, time_varying=L is not None)
     F = 0.9 * F
     g = torch.Generator().manual_seed(seed + 1)
     if F_T == T:
@@ -1128,8 +1132,8 @@ def episode_linear_inputs(seed, B, T, n, m, dtype, mode, F_T=None, f_T="T-1", ti
     if mode == "box":
         kw = dict(u_lower=-0.25, u_upper=0.25)
     elif mode in ("tensor", "boxT"):
-        kw = dict(u_lower=-0.5 * torch.rand(T, B, m, generator=g, dtype=F64) - 0.05,
-                  u_upper=0.5 * torch.rand(T, B, m, generator=g, dtype=F64) + 0.05)
+        kw = dict(u_lower=-0.5 * torch.rand(Ta, B, m, generator=g, dtype=F64) - 0.05,
+                  u_upper=0.5 * torch.rand(Ta, B, m, generator=g, dtype=F64) + 0.05)
         if mode == "boxT":
             kw["delta_u"] = 0.125
     elif mode == "mask":
@@ -1155,11 +1159,20 @@ def episode_device_inputs(P, dtype):
     return out
 
 
-def epgrad_launches(route, known):
+def epgrad_launches(route, known, window=False):
     """Library kernels an mpcb200_episode_backward_* call records (api.cu epgrad_record): the init, stage and
     accumulate kernels; a known system's linearisation and its VJP; the adjoint: prep + fused column-pair kernel, or
-    prep, fill_zero, masked step and the two gradient kernels on every three-launch route."""
-    return 3 + (2 if known else 0) + (2 if route == "fused" else 5)
+    prep, fill_zero, masked step and the two gradient kernels on every three-launch route.  window
+    (mpcb200_episode_backward_window_*): one more, the body's window_stage_kernel."""
+    return 3 + (2 if known else 0) + (2 if route == "fused" else 5) + (1 if window else 0)
+
+
+def episode_window_bounds(kw, n_steps):
+    """kw for check_episode_forward on a time-varying episode: each solve's t = 0 bound is slice k of a windowed
+    tensor bound [L, B, m], so a tensor bound becomes [1, n_steps, B, m] (its slice 0 holds solve k's at k); scalar
+    bounds and the other options as they are."""
+    return {k: v[:n_steps].unsqueeze(0) if k in ("u_lower", "u_upper") and torch.is_tensor(v) else v
+            for k, v in kw.items()}
 
 
 def episode_known_module(name):
