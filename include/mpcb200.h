@@ -278,6 +278,29 @@ int mpcb200_pnqp_f64(int32_t B, int32_t n, const double* H, const double* q, con
 int32_t mpcb200_pnqp_max_n(int32_t elem_size);
 
 /*
+ * Implicit gradient of a standalone pnqp solution, for a loss L(x).  Inputs: H[B,n,n] and lower,upper[B,n] of the
+ * solved QPs, the solution x[B,n] and free set If[B,n] (uint8, 1 = free) that mpcb200_pnqp_* returned, and
+ * dl_dx[B,n].  With F the free set and A the rest (clamped, x_i exactly at lower_i or upper_i), v solves
+ * (H_FF + 1e-11 I) v = dl_dx_F, the regularised block the forward factors; then
+ *   dq[B,n]:     -v on F, 0 on A;
+ *   dH[B,n,n]:   row i = -v_i x^T for i in F, 0 on the rows of A (unsymmetrised: autograd of g = Hx + q);
+ *   dlower, dupper[B,n]: on i in A, dl_dx_i - sum_{k in F} H_ki v_k goes to dlower_i when x_i == lower_i, else to
+ *                dupper_i; every other entry is 0.
+ * This is the reference's unrolled autograd (mpc/pnqp.py:5-82) on a problem whose last accepted Newton step was a
+ * full step with the final free set; on an unconverged problem it is the same formula at the returned point, not the
+ * derivative of the iterations.  x_init gets no gradient.  status[B] optional: MPCB200_ST_BAD_PIVOT when a pivot of
+ * the free block is <= 0 or not finite, else 0.  H must be symmetric (LDL^T of the lower triangle).  n <= 8 runs one
+ * thread per QP, larger n one thread block per QP; n > mpcb200_pnqp_max_n returns MPCB200_ERR_SMEM before any device
+ * is needed.  Every output element is written, without atomics: the result is the same bits on every call.
+ */
+int mpcb200_pnqp_backward_f32(int32_t B, int32_t n, const float* H, const float* x, const uint8_t* If,
+                              const float* lower, const float* upper, const float* dl_dx, float* dH, float* dq,
+                              float* dlower, float* dupper, int32_t* status, void* stream);
+int mpcb200_pnqp_backward_f64(int32_t B, int32_t n, const double* H, const double* x, const uint8_t* If,
+                              const double* lower, const double* upper, const double* dl_dx, double* dH, double* dq,
+                              double* dlower, double* dupper, int32_t* status, void* stream);
+
+/*
  * Shapes without a compiled instance.  The step, the gradient assembly, the rollout and the adjoint's nested solve
  * of an (n_state, n_ctrl) pair that no instance covers run the large-shape kernels: one thread block per problem,
  * runtime sizes, the per-time-step tiles of one problem in shared memory.  Their step needs Ks/ks (it returns

@@ -69,6 +69,7 @@ _lib = None
 EXPORTED_SYMBOLS = (
     "mpcb200_lqr_step_f32", "mpcb200_lqr_step_f64", "mpcb200_lqr_grad_f32", "mpcb200_lqr_grad_f64",
     "mpcb200_rollout_f32", "mpcb200_rollout_f64", "mpcb200_pnqp_f32", "mpcb200_pnqp_f64", "mpcb200_pnqp_max_n",
+    "mpcb200_pnqp_backward_f32", "mpcb200_pnqp_backward_f64",
     "mpcb200_lqr_adjoint_f32", "mpcb200_lqr_adjoint_f64", "mpcb200_adjoint_workspace_bytes",
     "mpcb200_dyn_rollout_f32", "mpcb200_dyn_rollout_f64", "mpcb200_dyn_linearize_f32", "mpcb200_dyn_linearize_f64",
     "mpcb200_dyn_linearize_vjp_f32", "mpcb200_dyn_linearize_vjp_f64",
@@ -125,6 +126,10 @@ def lib():
     for name in ("mpcb200_pnqp_f32", "mpcb200_pnqp_f64"):
         fn = getattr(L, name)
         fn.argtypes = [ctypes.c_int32, ctypes.c_int32] + [vp] * 5 + [ctypes.c_int32] + [vp] * 6
+        fn.restype = ctypes.c_int
+    for name in ("mpcb200_pnqp_backward_f32", "mpcb200_pnqp_backward_f64"):
+        fn = getattr(L, name)
+        fn.argtypes = [ctypes.c_int32, ctypes.c_int32] + [vp] * 12
         fn.restype = ctypes.c_int
     L.mpcb200_pnqp_max_n.argtypes = [ctypes.c_int32]
     L.mpcb200_pnqp_max_n.restype = ctypes.c_int32

@@ -1,6 +1,8 @@
 // pnqp_cta.cuh - projected-Newton box QP (reference mpc/pnqp.py:5-82) solved by a whole thread block on a QP
 // that is already in shared memory.  Used by the standalone CTA-per-QP kernel (pnqp_large.cu) and by the step
 // kernel for shapes without a compiled instance (lqr_large.cu), so both run the same operations in the same order.
+// The standalone kernel's implicit gradient (pnqp_large.cu) factors the same H_ with the same pack_free_block and
+// ldl_solve.
 // Shared-memory operands of one QP (n = its size):
 //   H    n x LD, LD = n | 1.  Row i of every mat-vec belongs to thread i % NT, so a warp reads a column of H at
 //        a stride of LD elements; an odd LD puts its 32 rows in 32 banks (16 bank pairs in fp64).
@@ -111,6 +113,17 @@ MPCB_DEV bool ldl_solve(R* P, R* v, R* w, R* dinv, int n) {
   return bad;
 }
 
+// P <- the masked matrix H_ (pnqp.py:46-48), lower triangle packed by rows: H on the rows and columns that fr marks
+// free, 0 elsewhere, plus 1e-11 on the diagonal.  Row i of H starts at H + i * ld (shared or global memory).
+template <typename R, int NT>
+MPCB_DEV void pack_free_block(R* P, const R* H, int ld, const int* fr, int n) {
+  for (int i = 0; i < n; ++i) {
+    const bool fi = fr[i] != 0;
+    for (int k = threadIdx.x; k <= i; k += NT)
+      P[tri(i) + k] = ((fi && fr[k]) ? H[i * ld + k] : R(0)) + (k == i ? R(1e-11) : R(0));
+  }
+}
+
 // The projected-Newton iteration (pnqp.py:14-82) on the QP (H, q, lo, hi) in shared memory, from x (read when
 // has_init) or from the clamped -H^{-1} q.  On return x is the solution, fr the free set and P, dinv the LDL^T
 // factor of the H_ of the returning iteration (what the reference returns the LU of); conv / badpiv as in
@@ -151,11 +164,7 @@ MPCB_DEV int pnqp_cta_solve(const R* H, R* P, const R* q, const R* lo, const R* 
       fx += x[i] * (R(0.5) * hx + q[i]);       // objective at x (:11-12) for the Armijo ratio
     }
     __syncthreads();
-    for (int i = 0; i < n; ++i) {              // :46-48  H_ = H on free rows and columns, + 1e-11 I
-      const bool fi = fr[i] != 0;
-      for (int k = t; k <= i; k += NT)
-        P[tri(i) + k] = ((fi && fr[k]) ? H[i * LD + k] : R(0)) + (k == i ? R(1e-11) : R(0));
-    }
+    pack_free_block<R, NT>(P, H, LD, fr, n);   // :46-48
     __syncthreads();
     badpiv = ldl_solve<R, NT>(P, v, w, dinv, n) || badpiv;
     for (int i = t; i < n; i += NT) {          // :53-54  dx = -H_^{-1} g_

@@ -113,6 +113,9 @@ static int run_case(int B, int T, int n, int m, int bounds_kind, int with_mask) 
     dH.up(H); dq.up(q); dl.up(l2); dh.up(h2);
     rc = mpcb200_pnqp_f32(B, m, dH.p, dq.p, dl.p, dh.p, nullptr, 20, ox.p, oH.p, oI.p, oit.p, ost.p, nullptr);
     if (rc) return printf("pnqp rc=%d\n", rc), 1;
+    Dev<float> gH(H.size()), gq(q.size()), gl(q.size()), gh(q.size());   // its gradient for dL/dx = q
+    rc = mpcb200_pnqp_backward_f32(B, m, dH.p, ox.p, oI.p, dl.p, dh.p, dq.p, gH.p, gq.p, gl.p, gh.p, ost.p, nullptr);
+    if (rc) return printf("pnqp backward rc=%d\n", rc), 1;
   }
   if (cudaDeviceSynchronize() != cudaSuccess) return printf("CUDA error: %s\n", cudaGetErrorString(cudaGetLastError())), 1;
   double s = 0;
@@ -202,12 +205,17 @@ static int run_pnqp_large(int B, int n) {
   if (rc) return printf("pnqp n=%d rc=%d (%s)\n", n, rc, mpcb200_strerror(rc)), 1;
   rc = mpcb200_pnqp_f64(B, max_n + 1, dH.p, dq.p, dl.p, dh.p, nullptr, 20, ox.p, oH.p, oI.p, oit.p, ost.p, nullptr);
   if (rc != MPCB200_ERR_SMEM) return printf("pnqp n=max_n+1 rc=%d\n", rc), 1;
+  Dev<double> gH(H.size()), gq(q.size()), gl(q.size()), gh(q.size());   // the gradient for dL/dx = q
+  Dev<int> gst(B);
+  rc = mpcb200_pnqp_backward_f64(B, n, dH.p, ox.p, oI.p, dl.p, dh.p, dq.p, gH.p, gq.p, gl.p, gh.p, gst.p, nullptr);
+  if (rc) return printf("pnqp backward n=%d rc=%d (%s)\n", n, rc, mpcb200_strerror(rc)), 1;
   if (cudaDeviceSynchronize() != cudaSuccess) return printf("CUDA error: %s\n", cudaGetErrorString(cudaGetLastError())), 1;
   double s = 0;
   int bad = 0;
   for (double v : ox.down()) { s += v; bad += !std::isfinite(v); }
-  std::vector<int> st = ost.down();
-  for (int v : st) bad += v != 0;
+  for (double v : gH.down()) { s += v; bad += !std::isfinite(v); }
+  for (int v : ost.down()) bad += v != 0;
+  for (int v : gst.down()) bad += v != 0;
   printf("pnqp B=%d n=%d (max_n f32 %d, f64 %d): checksum %.6f bad %d\n", B, n, mpcb200_pnqp_max_n(4), max_n, s, bad);
   return bad != 0;
 }
